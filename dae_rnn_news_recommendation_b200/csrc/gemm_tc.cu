@@ -7,13 +7,16 @@
 //   D += A_hi.B_hi + A_lo.B_hi + A_hi.B_lo      (three bf16 wgmma per k-step, fp32 accumulation in registers)
 // The dropped lo.lo term is <= 2^-18 relative, so the product is fp32-grade (1e-5 rel. worst case vs the 1e-4 budget).
 //
-// Structure (one CTA per SM, persistent over output tiles; 384 threads = three warpgroups):
+// Structure (one CTA per SM, persistent over output tiles):
+//   store GEMM (dae_gemm_bf16x3, dae_gemm_sym_bf16x3; 384 threads = three warpgroups):
 //   warpgroup 0   : TMA producer -- one lane issues cp.async.bulk.tensor.2d, 128B swizzle, into a STAGES-deep smem ring (hi and lo
 //                   tiles); the other warps only take part in the CTA-wide barriers
 //   warpgroups 1-2: consumers    -- each owns 64 rows of the 128-row tile: wgmma.mma_async m64 x BLOCK_N x k16 from shared-memory
-//                   descriptors, then the fused epilogue.  The accumulators go through a shared-memory staging tile so that the
-//                   epilogue works on whole rows (one thread = one output row, like the decode loss needs); meanwhile the producer
-//                   already fills the ring with the next tile's operands.
+//                   descriptors, then the store epilogue from a shared-memory staging tile; meanwhile the producer already fills the
+//                   ring with the next tile's operands.
+//   fused decode (dae_decode_fused_bf16x3; 640 threads = five warpgroups, see decode_fused_kernel): the same producer, two MMA
+//                   warpgroups that only run the main loop, and two epilogue warpgroups that run the loss epilogue of tile i from
+//                   the staging tile while the MMA warpgroups accumulate tile i + 1.
 // Operands may be K-major (K contiguous) or MN-major (M/N contiguous) -- both straight from row-major arrays (wgmma's transpose
 // bits), so no transposed copies of dZ / E / W are ever made.
 #include <cuda.h>
@@ -125,15 +128,15 @@ __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_grou
 template <int N>
 __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
-// Shared-memory matrix descriptor (sm_90 wgmma), 128-byte swizzle.
-//   K-major : rows of 128 B, 8-row groups 1024 B apart (SBO); LBO unused (1).
+// Shared-memory matrix descriptor (sm_90 wgmma), 128-byte swizzle (layout 1) or, for 32-wide K-major k-blocks, 64-byte swizzle (layout 2).
+//   K-major : rows of 128 B (64 B), 8-row groups 1024 B (512 B) apart (SBO); LBO unused (1).
 //   MN-major: 64-element (128 B) column slabs, 8 k-rows per 1024 B group (SBO), next slab LBO bytes further.
-__device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+__device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes, uint32_t layout = 1) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr >> 4) & 0x3FFF);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 62;  // SWIZZLE_128B
+  d |= (uint64_t)layout << 62;
   return d;
 }
 
@@ -179,12 +182,12 @@ struct GemmParams {
   int a_sym_kb;          // > 0: C = (A + A^T).B -- k-blocks [0, a_sym_kb) read the square A K-major, k-blocks [a_sym_kb, 2 a_sym_kb) read it
                          // MN-major (= A^T) through the second pair of tensor maps, and B's k index wraps (both halves multiply B)
   float alpha;
-  float* C;              // EPI_STORE: fp32 output [M x ldc]
+  float* C;              // store GEMM: fp32 output [M x ldc]
   int64_t ldc;
   int n_store;           // columns < n_store are stored
-  int special_col;       // EPI_STORE: this column (the all-ones column of [E | 1]) goes to special_out[m] instead; -1 = none
+  int special_col;       // store GEMM: this column (the all-ones column of [E | 1]) goes to special_out[m] instead; -1 = none
   float* special_out;
-  // EPI_DECODE (fused decode loss; M = batch rows, N = features)
+  // fused decode loss (M = batch rows, N = features)
   const int64_t* indptr; const int32_t* indices; const float* values; const int32_t* rows;
   const float* bv; const float* weight; const double* stats;
   __nv_bfloat16* dz_hi; __nv_bfloat16* dz_lo; int64_t ld_dz;
@@ -192,9 +195,7 @@ struct GemmParams {
   const int32_t* tile_ptr; // [M x (2 * n_tiles_n + 1)]: first CSR entry of every half tile, relative to the row start
 };
 
-enum { EPI_STORE = 0, EPI_DECODE = 1 };
-
-// Work distribution, walked identically by the TMA producer and the consumer warpgroups of a CTA.
+// Work distribution, walked identically by every warpgroup of a CTA.
 //   classic : work item w = (tile, k split), items blockIdx.x, blockIdx.x + gridDim.x, ...
 //   stream-K: the tiles x k-blocks units are cut into gridDim.x equal contiguous ranges; a CTA's range covers the tail of one
 //             tile, whole tiles, and the head of another -- every segment is one accumulator pass + one (atomic) epilogue.
@@ -203,13 +204,13 @@ struct Sched {
   int tiles_m, tiles, kb_total, kb_per_split, n_work, stream, w, n_cta;
   long long u, u_end;
   // pair != 0: the two CTAs of a cluster walk the SAME list; an m index then names a pair of 128-row tiles
-  __device__ __forceinline__ void init(const GemmParams& p, int block_n, int pair = 0) {
+  __device__ __forceinline__ void init(const GemmParams& p, int block_n, int pair = 0, int block_k = BLOCK_K) {
     const int cta = pair ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;
     n_cta = pair ? (int)(gridDim.x >> 1) : (int)gridDim.x;
     tiles_m = (p.M + BLOCK_M - 1) / BLOCK_M;
     if (pair) tiles_m = (tiles_m + 1) / 2;
     tiles = tiles_m * ((p.N + block_n - 1) / block_n);
-    kb_total = (p.K + BLOCK_K - 1) / BLOCK_K;
+    kb_total = (p.K + block_k - 1) / block_k;
     stream = p.stream_k;
     kb_per_split = (kb_total + p.k_splits - 1) / p.k_splits;
     n_work = tiles * p.k_splits;
@@ -330,16 +331,19 @@ __device__ __forceinline__ bool decode_chunk_sigmoid_ce(const uint32_t (&r)[16],
   return ok;
 }
 
-// One k-block (BLOCK_K = 4 k16 steps) of a warpgroup's 64 x BLOCK_N tile: lo.hi, hi.lo, hi.hi per step, small terms first.
-template <int BLOCK_N, int TA, int TB>
+// One k-block (BK / 16 k16 steps) of a warpgroup's 64 x BLOCK_N tile: lo.hi, hi.lo, hi.hi per step, small terms first.
+// BK = 64: 128-byte swizzle, either majorness; BK = 32: 64-byte swizzle, K-major operands only.
+template <int BLOCK_N, int TA, int TB, int BK = BLOCK_K>
 __device__ __forceinline__ void mma_kblock(float (&acc)[BLOCK_N / 2], uint32_t sa_hi, uint32_t sa_lo, uint32_t sb_hi, uint32_t sb_lo,
                                            bool first) {
+  static_assert(BK == 64 || (BK == 32 && !TA && !TB), "32-wide k-blocks are K-major only");
+  constexpr uint32_t layout = BK == 64 ? 1u : 2u, sbo = BK == 64 ? 1024u : 512u;
   constexpr uint32_t a_lbo = TA ? 8192u : 16u, b_lbo = TB ? 8192u : 16u;
   constexpr uint32_t a_step = TA ? 2048u : 32u, b_step = TB ? 2048u : 32u;  // bytes per WGMMA_K
 #pragma unroll
-  for (int k = 0; k < BLOCK_K / WGMMA_K; ++k) {
-    const uint64_t da_hi = make_desc(sa_hi + k * a_step, a_lbo, 1024), da_lo = make_desc(sa_lo + k * a_step, a_lbo, 1024);
-    const uint64_t db_hi = make_desc(sb_hi + k * b_step, b_lbo, 1024), db_lo = make_desc(sb_lo + k * b_step, b_lbo, 1024);
+  for (int k = 0; k < BK / WGMMA_K; ++k) {
+    const uint64_t da_hi = make_desc(sa_hi + k * a_step, a_lbo, sbo, layout), da_lo = make_desc(sa_lo + k * a_step, a_lbo, sbo, layout);
+    const uint64_t db_hi = make_desc(sb_hi + k * b_step, b_lbo, sbo, layout), db_lo = make_desc(sb_lo + k * b_step, b_lbo, sbo, layout);
     const uint32_t sc = (first && k == 0) ? 0u : 1u;
     if constexpr (BLOCK_N == 128) {
       wgmma_n128<TA, TB>(acc, da_lo, db_hi, sc);
@@ -362,10 +366,117 @@ __device__ __forceinline__ void stage_ld16(const float* src, uint32_t (&r)[16]) 
   }
 }
 
-// PAIR = 1: two-CTA cluster sharing the B tile through TMA multicast (see the PTX wrappers above); needs BLOCK_N = 128.
+// ---- the two halves of the main loop, shared by the store GEMM and the fused decode
+
+// TMA producer (one lane): fills the STAGES-deep ring with the A and B k-blocks (hi and lo) of every work item of `sched`, in order.
+// PAIR = 1: two-CTA cluster sharing the B tile through TMA multicast (see the PTX wrappers above).
+template <int BLOCK_N, int STAGES, int PAIR, int BK = BLOCK_K>
+__device__ __forceinline__ void tma_produce(const GemmParams& p, Sched& sched, uint8_t* smem, uint64_t* full_bar, uint64_t* empty_bar,
+                                            uint32_t crank, const CUtensorMap* tm_a_hi, const CUtensorMap* tm_a_lo,
+                                            const CUtensorMap* tm_b_hi, const CUtensorMap* tm_b_lo, const CUtensorMap* tm_at_hi,
+                                            const CUtensorMap* tm_at_lo) {
+  constexpr int A_TILE = BLOCK_M * BK * 2;        // bytes of one bf16 A tile (16 KB at BK = 64)
+  constexpr int B_TILE = BLOCK_N * BK * 2;
+  constexpr int STAGE_BYTES = 2 * A_TILE + 2 * B_TILE;
+  int stage = 0; uint32_t phase = 0;
+  int mb, nb, kb0, kb1;
+  while (sched.next(mb, nb, kb0, kb1)) {
+    for (int kb = kb0; kb < kb1; ++kb) {
+      if (PAIR) mbar_wait_cluster(&empty_bar[stage], phase ^ 1); else mbar_wait(&empty_bar[stage], phase ^ 1);
+      uint8_t* sa_hi = smem + stage * STAGE_BYTES;
+      uint8_t* sa_lo = sa_hi + A_TILE;
+      uint8_t* sb_hi = sa_lo + A_TILE;
+      uint8_t* sb_lo = sb_hi + B_TILE;
+      const int mt = PAIR ? mb * 2 + (int)crank : mb;            // this CTA's 128-row m tile
+      mbar_expect_tx(&full_bar[stage], STAGE_BYTES);             // PAIR: half of the B bytes come from the peer's multicast
+      if (p.a_sym_kb > 0 && kb >= p.a_sym_kb) {      // second half of (A + A^T).B: the same square array read M-contiguous
+#pragma unroll
+        for (int j = 0; j < BLOCK_M / 64; ++j) {
+          tma_load_2d(tm_at_hi, &full_bar[stage], sa_hi + j * (64 * BK * 2), mt * BLOCK_M + j * 64, (kb - p.a_sym_kb) * BK);
+          tma_load_2d(tm_at_lo, &full_bar[stage], sa_lo + j * (64 * BK * 2), mt * BLOCK_M + j * 64, (kb - p.a_sym_kb) * BK);
+        }
+      } else if (!p.a_mn) {
+        tma_load_2d(tm_a_hi, &full_bar[stage], sa_hi, kb * BK, mt * BLOCK_M);
+        tma_load_2d(tm_a_lo, &full_bar[stage], sa_lo, kb * BK, mt * BLOCK_M);
+      } else {
+#pragma unroll
+        for (int j = 0; j < BLOCK_M / 64; ++j) {
+          tma_load_2d(tm_a_hi, &full_bar[stage], sa_hi + j * (64 * BK * 2), mt * BLOCK_M + j * 64, kb * BK);
+          tma_load_2d(tm_a_lo, &full_bar[stage], sa_lo + j * (64 * BK * 2), mt * BLOCK_M + j * 64, kb * BK);
+        }
+      }
+      const int kbb = (p.a_sym_kb > 0 && kb >= p.a_sym_kb) ? kb - p.a_sym_kb : kb;   // B's k block
+      if (PAIR) {   // this CTA's 64-row half of the B tile, into both CTAs (K-major: rows 64 crank..; MN-major: slab crank)
+        const int off = (int)crank * 8192, n_half = nb * BLOCK_N + (int)crank * 64;
+        if (!p.b_mn) {
+          tma_load_2d_mc(tm_b_hi, &full_bar[stage], sb_hi + off, kbb * BK, n_half, 0x3);
+          tma_load_2d_mc(tm_b_lo, &full_bar[stage], sb_lo + off, kbb * BK, n_half, 0x3);
+        } else {
+          tma_load_2d_mc(tm_b_hi, &full_bar[stage], sb_hi + off, n_half, kbb * BK, 0x3);
+          tma_load_2d_mc(tm_b_lo, &full_bar[stage], sb_lo + off, n_half, kbb * BK, 0x3);
+        }
+      } else if (!p.b_mn) {
+        tma_load_2d(tm_b_hi, &full_bar[stage], sb_hi, kbb * BK, nb * BLOCK_N);
+        tma_load_2d(tm_b_lo, &full_bar[stage], sb_lo, kbb * BK, nb * BLOCK_N);
+      } else {
+#pragma unroll
+        for (int j = 0; j < BLOCK_N / 64; ++j) {
+          tma_load_2d(tm_b_hi, &full_bar[stage], sb_hi + j * (64 * BK * 2), nb * BLOCK_N + j * 64, kbb * BK);
+          tma_load_2d(tm_b_lo, &full_bar[stage], sb_lo + j * (64 * BK * 2), nb * BLOCK_N + j * 64, kbb * BK);
+        }
+      }
+      if (++stage == STAGES) { stage = 0; phase ^= 1; }
+    }
+  }
+}
+
+// The k-blocks [kb0, kb1) of one work item for MMA warpgroup wg (rows [64 wg, 64 wg + 64) of the tile): wgmma into acc, each ring stage
+// released to the producer (of both CTAs of a pair) once its wgmma have retired.  stage / phase carry the ring position across work items.
 // MAJ: bit 0 = A MN-major, bit 1 = B MN-major, bit 2 = (A + A^T).B (A K-major for k-blocks < a_sym_kb, MN-major after).  A
 // compile-time constant, because a runtime choice between wgmma variants inside the k loop makes ptxas serialise the wgmma.
-template <int BLOCK_N, int STAGES, int EPI, int ACT, int LOSS, int PAIR, int MAJ>
+template <int BLOCK_N, int STAGES, int PAIR, int MAJ, int BK = BLOCK_K>
+__device__ __forceinline__ void mma_work_item(float (&acc)[BLOCK_N / 2], const GemmParams& p, uint8_t* smem, uint64_t* full_bar,
+                                              uint64_t* empty_bar, int wg, int lane, uint32_t crank, int& stage, uint32_t& phase,
+                                              int kb0, int kb1) {
+  constexpr int A_TILE = BLOCK_M * BK * 2;
+  constexpr int B_TILE = BLOCK_N * BK * 2;
+  constexpr int STAGE_BYTES = 2 * A_TILE + 2 * B_TILE;
+  auto release = [&](int s) {   // this warp is done reading ring stage s (its wgmma have retired)
+    __syncwarp();
+    if (lane == 0) { mbar_arrive(&empty_bar[s]); if (PAIR) mbar_arrive_cluster(&empty_bar[s], crank ^ 1u); }
+  };
+  int prev = -1;
+  auto run_k = [&](auto ta, auto tb, int kb_begin, int kb_end) {   // k-blocks [kb_begin, kb_end) with fixed majorness
+    for (int kb = kb_begin; kb < kb_end; ++kb) {
+      mbar_wait(&full_bar[stage], phase);
+      const uint32_t sa_hi = smem_u32(smem + stage * STAGE_BYTES) + wg * (64 * BK * 2);   // K-major: 64 rows x 2 BK B; MN-major: slab wg
+      const uint32_t sa_lo = sa_hi + A_TILE;
+      const uint32_t sb_hi = smem_u32(smem + stage * STAGE_BYTES) + 2 * A_TILE, sb_lo = sb_hi + B_TILE;
+      wgmma_fence();
+      mma_kblock<BLOCK_N, decltype(ta)::value, decltype(tb)::value, BK>(acc, sa_hi, sa_lo, sb_hi, sb_lo, kb == kb0);
+      wgmma_commit();
+      wgmma_wait<1>();                     // the previous k-block's wgmma have retired: its stage can be refilled
+      if (prev >= 0) release(prev);
+      prev = stage;
+      if (++stage == STAGES) { stage = 0; phase ^= 1; }
+    }
+  };
+  using K0 = std::integral_constant<int, 0>;
+  using K1 = std::integral_constant<int, 1>;
+  if constexpr ((MAJ & 4) != 0) {
+    run_k(K0{}, K1{}, kb0, min(kb1, p.a_sym_kb));
+    run_k(K1{}, K1{}, max(kb0, p.a_sym_kb), kb1);
+  } else {
+    run_k(std::integral_constant<int, MAJ & 1>{}, std::integral_constant<int, (MAJ >> 1) & 1>{}, kb0, kb1);
+  }
+  wgmma_wait<0>();
+  if (prev >= 0) release(prev);
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// store GEMM: C (+)= alpha A.B, 384 threads = producer + two consumer warpgroups that run the main loop and then the store epilogue
+// ---------------------------------------------------------------------------------------------------------------------
+template <int BLOCK_N, int STAGES, int PAIR, int MAJ>
 __global__ void __launch_bounds__(kThreads, 1) gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap tm_a_hi,
                                                                    const __grid_constant__ CUtensorMap tm_a_lo,
                                                                    const __grid_constant__ CUtensorMap tm_b_hi,
@@ -374,20 +485,14 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_bf16x3_kernel(const __grid_c
                                                                    const __grid_constant__ CUtensorMap tm_at_lo,
                                                                    const GemmParams p) {
   static_assert(!PAIR || BLOCK_N == 128, "CTA pairs split the B tile into two 64-row halves");
-  constexpr int A_TILE = BLOCK_M * BLOCK_K * 2;   // bytes of one bf16 A tile (16 KB)
-  constexpr int B_TILE = BLOCK_N * BLOCK_K * 2;
-  constexpr int STAGE_BYTES = 2 * A_TILE + 2 * B_TILE;
+  constexpr int STAGE_BYTES = 2 * BLOCK_M * BLOCK_K * 2 + 2 * BLOCK_N * BLOCK_K * 2;
   constexpr int SROW = BLOCK_N + 4;               // staging row stride (floats): conflict-free 16-byte row reads
   constexpr int kParts = 2;                       // column parts per tile (one per epilogue warp of a 32-row quarter)
   constexpr int HALF_N = BLOCK_N / kParts;        // columns handled by one epilogue warp
-  constexpr bool kFast = (EPI == EPI_DECODE) && (ACT == DAE_ACT_SIGMOID) && (LOSS == DAE_LOSS_CE);
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   float* stg = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES);   // [BLOCK_M][SROW] accumulator staging
   __shared__ __align__(8) uint64_t full_bar[STAGES], empty_bar[STAGES];
-  __shared__ float s_bias[EPI == EPI_DECODE ? 2 : 1][EPI == EPI_DECODE ? BLOCK_N : 1];   // per consumer warpgroup
-  __shared__ float s_biasc[kFast ? 2 : 1][kFast ? BLOCK_N : 1];   // bv * log2(e) for the sigmoid/CE fast path
-  __shared__ __align__(16) uint8_t s_stage[EPI == EPI_DECODE ? 8 : 1][2][32][48];  // bf16 hi / lo dZ blocks [32 rows x 16 cols], rows padded to 48 B
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   Sched sched;
@@ -406,104 +511,23 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_bf16x3_kernel(const __grid_c
   if (PAIR) cluster_sync_all(); else __syncthreads();   // the peer's barriers must be initialised before anything signals them
 
   if (warp == 0) {
-    // ===================== TMA producer =====================
-    if (lane == 0) {
-      int stage = 0; uint32_t phase = 0;
-      int mb, nb, kb0, kb1;
-      while (sched.next(mb, nb, kb0, kb1)) {
-        for (int kb = kb0; kb < kb1; ++kb) {
-          if (PAIR) mbar_wait_cluster(&empty_bar[stage], phase ^ 1); else mbar_wait(&empty_bar[stage], phase ^ 1);
-          uint8_t* sa_hi = smem + stage * STAGE_BYTES;
-          uint8_t* sa_lo = sa_hi + A_TILE;
-          uint8_t* sb_hi = sa_lo + A_TILE;
-          uint8_t* sb_lo = sb_hi + B_TILE;
-          const int mt = PAIR ? mb * 2 + (int)crank : mb;            // this CTA's 128-row m tile
-          mbar_expect_tx(&full_bar[stage], STAGE_BYTES);             // PAIR: half of the B bytes come from the peer's multicast
-          if (p.a_sym_kb > 0 && kb >= p.a_sym_kb) {      // second half of (A + A^T).B: the same square array read M-contiguous
-#pragma unroll
-            for (int j = 0; j < BLOCK_M / 64; ++j) {
-              tma_load_2d(&tm_at_hi, &full_bar[stage], sa_hi + j * 8192, mt * BLOCK_M + j * 64, (kb - p.a_sym_kb) * BLOCK_K);
-              tma_load_2d(&tm_at_lo, &full_bar[stage], sa_lo + j * 8192, mt * BLOCK_M + j * 64, (kb - p.a_sym_kb) * BLOCK_K);
-            }
-          } else if (!p.a_mn) {
-            tma_load_2d(&tm_a_hi, &full_bar[stage], sa_hi, kb * BLOCK_K, mt * BLOCK_M);
-            tma_load_2d(&tm_a_lo, &full_bar[stage], sa_lo, kb * BLOCK_K, mt * BLOCK_M);
-          } else {
-#pragma unroll
-            for (int j = 0; j < BLOCK_M / 64; ++j) {
-              tma_load_2d(&tm_a_hi, &full_bar[stage], sa_hi + j * 8192, mt * BLOCK_M + j * 64, kb * BLOCK_K);
-              tma_load_2d(&tm_a_lo, &full_bar[stage], sa_lo + j * 8192, mt * BLOCK_M + j * 64, kb * BLOCK_K);
-            }
-          }
-          const int kbb = (p.a_sym_kb > 0 && kb >= p.a_sym_kb) ? kb - p.a_sym_kb : kb;   // B's k block
-          if (PAIR) {   // this CTA's 64-row half of the B tile, into both CTAs (K-major: rows 64 crank..; MN-major: slab crank)
-            const int off = (int)crank * 8192, n_half = nb * BLOCK_N + (int)crank * 64;
-            if (!p.b_mn) {
-              tma_load_2d_mc(&tm_b_hi, &full_bar[stage], sb_hi + off, kbb * BLOCK_K, n_half, 0x3);
-              tma_load_2d_mc(&tm_b_lo, &full_bar[stage], sb_lo + off, kbb * BLOCK_K, n_half, 0x3);
-            } else {
-              tma_load_2d_mc(&tm_b_hi, &full_bar[stage], sb_hi + off, n_half, kbb * BLOCK_K, 0x3);
-              tma_load_2d_mc(&tm_b_lo, &full_bar[stage], sb_lo + off, n_half, kbb * BLOCK_K, 0x3);
-            }
-          } else if (!p.b_mn) {
-            tma_load_2d(&tm_b_hi, &full_bar[stage], sb_hi, kbb * BLOCK_K, nb * BLOCK_N);
-            tma_load_2d(&tm_b_lo, &full_bar[stage], sb_lo, kbb * BLOCK_K, nb * BLOCK_N);
-          } else {
-#pragma unroll
-            for (int j = 0; j < BLOCK_N / 64; ++j) {
-              tma_load_2d(&tm_b_hi, &full_bar[stage], sb_hi + j * 8192, nb * BLOCK_N + j * 64, kbb * BLOCK_K);
-              tma_load_2d(&tm_b_lo, &full_bar[stage], sb_lo + j * 8192, nb * BLOCK_N + j * 64, kbb * BLOCK_K);
-            }
-          }
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
+    if (lane == 0)
+      tma_produce<BLOCK_N, STAGES, PAIR>(p, sched, smem, full_bar, empty_bar, crank, &tm_a_hi, &tm_a_lo, &tm_b_hi, &tm_b_lo, &tm_at_hi,
+                                         &tm_at_lo);
   } else if (warp >= 4) {
-    // ===================== consumers: wgmma main loop, then the epilogue =====================
+    // ===================== consumers: wgmma main loop, then the store epilogue =====================
     const int wg = (warp >> 2) - 1;          // consumer warpgroup: rows [64 wg, 64 wg + 64) of the tile
     const int wi = warp & 3;                 // warp within the warpgroup
     const int quarter = wg * 2 + (wi & 1);   // 32-row quarter of the tile this warp's epilogue handles
     const int half = wi >> 1;                // which column part of the tile
-    const int row_in_tile = quarter * 32 + lane;
-    const int tiles_n = (p.N + BLOCK_N - 1) / BLOCK_N;
     float acc[BLOCK_N / 2];
 #pragma unroll
     for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] = 0.0f;
     int stage = 0; uint32_t phase = 0;
-    auto release = [&](int s) {   // this warp is done reading ring stage s (its wgmma have retired)
-      __syncwarp();
-      if (lane == 0) { mbar_arrive(&empty_bar[s]); if (PAIR) mbar_arrive_cluster(&empty_bar[s], crank ^ 1u); }
-    };
     int mb, nb, kb0, kb1;
     while (sched.next(mb, nb, kb0, kb1)) {
       if (PAIR) mb = mb * 2 + (int)crank;     // this CTA's 128-row m tile of the pair
-      int prev = -1;
-      auto run_k = [&](auto ta, auto tb, int kb_begin, int kb_end) {   // k-blocks [kb_begin, kb_end) with fixed majorness
-        for (int kb = kb_begin; kb < kb_end; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          const uint32_t sa_hi = smem_u32(smem + stage * STAGE_BYTES) + wg * 8192;   // K-major: 64 rows x 128 B; MN-major: slab wg
-          const uint32_t sa_lo = sa_hi + A_TILE;
-          const uint32_t sb_hi = smem_u32(smem + stage * STAGE_BYTES) + 2 * A_TILE, sb_lo = sb_hi + B_TILE;
-          wgmma_fence();
-          mma_kblock<BLOCK_N, decltype(ta)::value, decltype(tb)::value>(acc, sa_hi, sa_lo, sb_hi, sb_lo, kb == kb0);
-          wgmma_commit();
-          wgmma_wait<1>();                     // the previous k-block's wgmma have retired: its stage can be refilled
-          if (prev >= 0) release(prev);
-          prev = stage;
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-      };
-      using K0 = std::integral_constant<int, 0>;
-      using K1 = std::integral_constant<int, 1>;
-      if (MAJ & 4) {
-        run_k(K0{}, K1{}, kb0, min(kb1, p.a_sym_kb));
-        run_k(K1{}, K1{}, max(kb0, p.a_sym_kb), kb1);
-      } else {
-        run_k(std::integral_constant<int, MAJ & 1>{}, std::integral_constant<int, (MAJ >> 1) & 1>{}, kb0, kb1);
-      }
-      wgmma_wait<0>();
-      if (prev >= 0) release(prev);
+      mma_work_item<BLOCK_N, STAGES, PAIR, MAJ>(acc, p, smem, full_bar, empty_bar, wg, lane, crank, stage, phase, kb0, kb1);
 
       // accumulators -> staging rows (the previous tile's epilogue of this warpgroup must be done with them)
       named_bar_sync(1 + wg, 128);
@@ -515,157 +539,261 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_bf16x3_kernel(const __grid_c
           *reinterpret_cast<float2*>(&stg[(r0 + 8) * SROW + 8 * j + c0]) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
         }
       }
-      if (EPI == EPI_DECODE) {  // this tile's visible-bias slice
-        for (int j = threadIdx.x - 128 * (wg + 1); j < BLOCK_N; j += 128) {
-          const float b = (nb * BLOCK_N + j < p.N) ? p.bv[nb * BLOCK_N + j] : 0.0f;
-          s_bias[wg][j] = b;
-          if (kFast) s_biasc[wg][j] = b * kLog2e;
-        }
-      }
       named_bar_sync(1 + wg, 128);
-      const float* srow = stg + row_in_tile * SROW + half * HALF_N;   // this thread's row, this warp's column part
-      const int m = mb * BLOCK_M + row_in_tile;
       const int n0 = nb * BLOCK_N + half * HALF_N;
-
-      if (EPI == EPI_STORE) {
-        const float* tr = stg + (quarter * 32) * SROW + half * HALF_N;   // the warp's 32 rows
-        const int m_base = mb * BLOCK_M + quarter * 32;
-        const bool vec_ok = ((p.ldc & 3) == 0) && ((reinterpret_cast<uintptr_t>(p.C) & 15) == 0);
+      const float* tr = stg + (quarter * 32) * SROW + half * HALF_N;   // the warp's 32 rows
+      const int m_base = mb * BLOCK_M + quarter * 32;
+      const bool vec_ok = ((p.ldc & 3) == 0) && ((reinterpret_cast<uintptr_t>(p.C) & 15) == 0);
 #pragma unroll 1
-        for (int c = 0; c < HALF_N / 16; ++c) {
-          const int nc = n0 + c * 16;   // first column of this 16-wide chunk
-          const bool interior = vec_ok && (m_base + 32 <= p.M) && (nc + 16 <= p.n_store) && (p.special_col < nc || p.special_col >= nc + 16);
-          if (interior) {               // fast path: 8 rows x 64 B per store instruction, 128-bit accesses
-            const int rsub = lane >> 2, c4 = (lane & 3) * 4;
-            float* dst = p.C + (int64_t)(m_base + rsub) * p.ldc + nc + c4;
-            const int64_t step = 8 * p.ldc;
+      for (int c = 0; c < HALF_N / 16; ++c) {
+        const int nc = n0 + c * 16;   // first column of this 16-wide chunk
+        const bool interior = vec_ok && (m_base + 32 <= p.M) && (nc + 16 <= p.n_store) && (p.special_col < nc || p.special_col >= nc + 16);
+        if (interior) {               // fast path: 8 rows x 64 B per store instruction, 128-bit accesses
+          const int rsub = lane >> 2, c4 = (lane & 3) * 4;
+          float* dst = p.C + (int64_t)(m_base + rsub) * p.ldc + nc + c4;
+          const int64_t step = 8 * p.ldc;
 #pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              float4 v = *reinterpret_cast<const float4*>(&tr[(rsub + 8 * i) * SROW + c * 16 + c4]);
-              v.x *= p.alpha; v.y *= p.alpha; v.z *= p.alpha; v.w *= p.alpha;
-              if (p.atomic) atomicAdd(reinterpret_cast<float4*>(dst), v); else *reinterpret_cast<float4*>(dst) = v;
-              dst += step;
-            }
-          } else {                      // edge tiles / the [dW | dbv] column / unaligned C
-            const int rsub = lane >> 4, csub = lane & 15;
-            const int n = nc + csub;
-            for (int i = 0; i < 16; ++i) {
-              const int rr = 2 * i + rsub;
-              const int mm = m_base + rr;
-              const float v = p.alpha * tr[rr * SROW + c * 16 + csub];
-              if (mm < p.M) {
-                if (n == p.special_col) {
-                  if (p.atomic) atomicAdd(p.special_out + mm, v); else p.special_out[mm] = v;
-                } else if (n < p.n_store) {
-                  float* dst = p.C + (int64_t)mm * p.ldc + n;
-                  if (p.atomic) atomicAdd(dst, v); else *dst = v;
-                }
+          for (int i = 0; i < 4; ++i) {
+            float4 v = *reinterpret_cast<const float4*>(&tr[(rsub + 8 * i) * SROW + c * 16 + c4]);
+            v.x *= p.alpha; v.y *= p.alpha; v.z *= p.alpha; v.w *= p.alpha;
+            if (p.atomic) atomicAdd(reinterpret_cast<float4*>(dst), v); else *reinterpret_cast<float4*>(dst) = v;
+            dst += step;
+          }
+        } else {                      // edge tiles / the [dW | dbv] column / unaligned C
+          const int rsub = lane >> 4, csub = lane & 15;
+          const int n = nc + csub;
+          for (int i = 0; i < 16; ++i) {
+            const int rr = 2 * i + rsub;
+            const int mm = m_base + rr;
+            const float v = p.alpha * tr[rr * SROW + c * 16 + csub];
+            if (mm < p.M) {
+              if (n == p.special_col) {
+                if (p.atomic) atomicAdd(p.special_out + mm, v); else p.special_out[mm] = v;
+              } else if (n < p.n_store) {
+                float* dst = p.C + (int64_t)mm * p.ldc + n;
+                if (p.atomic) atomicAdd(dst, v); else *dst = v;
               }
             }
           }
         }
-      } else {
-        // ---- fused decode epilogue: D = g(Z + bv); row loss; dZ -> bf16 hi/lo (autoencoder.py:411, triplet_loss_utils.py:269-275)
-        // 99 % of a bag-of-words target row is zero, so each 16-column chunk is first evaluated branch-free as if x == 0,
-        // stored, and then the row's few stored entries inside the chunk are re-evaluated exactly and patched in place.  The clean
-        // CSR row is walked with a cursor (columns are sorted) that keeps the next THREE entries (c0,v0),(c1,v1),(c2,v2) in
-        // registers, loaded well before they are needed, so the L2 latency of the CSR stream never sits on the column loop.
-        int64_t pc = 0, pe = 0;
-        int c0 = 0x7fffffff, c1 = 0x7fffffff, c2 = 0x7fffffff;
-        float v0 = 0.0f, v1 = 0.0f, v2 = 0.0f;
-        float sc = 0.0f;
-        if (m < p.M) {
-          const int64_t row = p.rows ? (int64_t)p.rows[m] : (int64_t)m;
-          const int64_t rbeg = p.indptr[row];
-          const int32_t* tp = p.tile_ptr + (int64_t)m * (kParts * tiles_n + 1) + nb * kParts + half;
-          pc = rbeg + tp[0]; pe = rbeg + tp[1];     // entries of this row that fall into this half tile
-          if (pc < pe) { c0 = p.indices[pc]; v0 = p.values[pc]; }
-          if (pc + 1 < pe) { c1 = p.indices[pc + 1]; v1 = p.values[pc + 1]; }
-          if (pc + 2 < pe) { c2 = p.indices[pc + 2]; v2 = p.values[pc + 2]; }
-          sc = (p.weight ? p.weight[m] : 1.0f) / ((float)p.stats[DAE_STAT_SUM_W] + kEps);
-        }
-        const float inv_sc = (sc != 0.0f) ? 1.0f / sc : 0.0f;
-        const bool edge = (n0 + HALF_N > p.N);   // only the last column tile has out-of-range columns
-        float lsum = 0.0f;   // CE: accumulated in log2 units, scaled by ln2 at the end
-        // dZ leaves through a per-warp shared-memory transpose: each thread (= batch row) drops the bf16 hi and lo parts of its
-        // 16 values into its two staging rows (patching the row's stored entries there), then the warp writes both 32 x 16
-        // blocks with full 32-byte sectors (16 rows per store instruction).
-        const int ew = warp - 4;
-        uint8_t* stg_hi = reinterpret_cast<uint8_t*>(&s_stage[ew][0][0][0]);
-        uint8_t* stg_lo = reinterpret_cast<uint8_t*>(&s_stage[ew][1][0][0]);
-        const int rsub = lane >> 1, csub = lane & 1;          // write-out mapping: 16 rows x 2 x 16 B per instruction
-        const int m_base = mb * BLOCK_M + quarter * 32;
-        const int n_lim = edge ? p.N : 0x7fffffff;
-#pragma unroll 1
-        for (int c = 0; c < HALF_N / 16; ++c) {
-          uint32_t r[16];
-          stage_ld16(srow + c * 16, r);
-          const int nc = n0 + c * 16;
-          if (m < p.M) {
-            const float* bias = &s_bias[wg][half * HALF_N + c * 16];
-            uint32_t hpk[8], lpk[8];
-            bool fast_ok = false;   // this chunk went through the sigmoid/CE fast path: staged dZ = sc * D exactly
-            if (kFast && !edge) {
-              const float l0 = lsum;
-              fast_ok = decode_chunk_sigmoid_ce(r, &s_biasc[wg][half * HALF_N + c * 16], sc, hpk, lpk, lsum);
-              if (!fast_ok) { lsum = l0; decode_chunk_generic<ACT, LOSS>(r, bias, sc, edge, n_lim, nc, hpk, lpk, lsum); }
-            } else {
-              decode_chunk_generic<ACT, LOSS>(r, bias, sc, edge, n_lim, nc, hpk, lpk, lsum);
-            }
-            uint4* sh = reinterpret_cast<uint4*>(stg_hi + lane * 48);
-            uint4* sl = reinterpret_cast<uint4*>(stg_lo + lane * 48);
-            sh[0] = make_uint4(hpk[0], hpk[1], hpk[2], hpk[3]); sh[1] = make_uint4(hpk[4], hpk[5], hpk[6], hpk[7]);
-            sl[0] = make_uint4(lpk[0], lpk[1], lpk[2], lpk[3]); sl[1] = make_uint4(lpk[4], lpk[5], lpk[6], lpk[7]);
-            // exact re-evaluation of the stored entries of this row inside the group (densified target, :264)
-            while (c0 < nc + 16) {
-              const float x = v0;
-              const int j = c0 - nc;
-              __nv_bfloat16* ph = reinterpret_cast<__nv_bfloat16*>(stg_hi + lane * 48) + j;
-              __nv_bfloat16* pl = reinterpret_cast<__nv_bfloat16*>(stg_lo + lane * 48) + j;
-              float d;
-              if (kFast && fast_ok && sc != 0.0f) d = (__bfloat162float(*ph) + __bfloat162float(*pl)) * inv_sc;   // D back from the staged sc * D
-              else d = act_fast<ACT>(select16(r, j) + bias[j]);
-              const float gp = act_grad_from_y<ACT>(d);
-              float dz;
-              if (LOSS == DAE_LOSS_CE) {
-                const float a = d + kEps, b = (1.0f - d) + kEps;
-                const float la = f_lg2(a), lb = f_lg2(b);
-                lsum += lb - (x * la + (1.0f - x) * lb);      // replace the x == 0 term by the exact one
-                dz = sc * gp * ((1.0f - x) * f_rcp(b) - x * f_rcp(a));
-              } else {
-                const float e2 = x - d;
-                lsum += e2 * e2 - d * d;
-                dz = -2.0f * sc * e2 * gp;
-              }
-              const __nv_bfloat16 hb = __float2bfloat16_rn(dz);
-              *ph = hb;
-              *pl = __float2bfloat16_rn(dz - __bfloat162float(hb));
-              ++pc;
-              c0 = c1; v0 = v1; c1 = c2; v1 = v2;
-              c2 = 0x7fffffff;
-              if (pc + 2 < pe) { c2 = p.indices[pc + 2]; v2 = p.values[pc + 2]; }
-            }
-          }
-          __syncwarp();
-          if (nc < p.ld_dz) {  // ld_dz is a multiple of 32 (launcher), so whole 16-column groups are in range
-#pragma unroll
-            for (int i = 0; i < 2; ++i) {
-              const int rr = rsub + 16 * i;
-              if (m_base + rr < p.M) {
-                const int64_t off = (int64_t)(m_base + rr) * p.ld_dz + nc + csub * 8;
-                *reinterpret_cast<uint4*>(p.dz_hi + off) = *reinterpret_cast<const uint4*>(stg_hi + rr * 48 + csub * 16);
-                *reinterpret_cast<uint4*>(p.dz_lo + off) = *reinterpret_cast<const uint4*>(stg_lo + rr * 48 + csub * 16);
-              }
-            }
-          }
-          __syncwarp();
-        }
-        if (m < p.M) atomicAdd(p.row_loss_part + m, (LOSS == DAE_LOSS_CE) ? lsum * 0.6931471805599453f : lsum);  // 2 * tiles_n partials per row
       }
     }
   }
 
   if (PAIR) cluster_sync_all();   // nobody leaves while the peer may still multicast into this CTA or arrive on its barriers
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// fused decode: D = g(E.W^T + bv), row loss, dZ (bf16 hi / lo), 640 threads = five warpgroups with one role each
+//   warpgroup 0   : TMA producer (one lane), as in the store GEMM
+//   warpgroups 1-2: MMA   -- rows [64 h, 64 h + 64) of the tile (h = warpgroup - 1): the wgmma main loop only; the finished accumulators
+//                   go to their half of the staging tile, and the warpgroup starts on the next tile at once
+//   warpgroups 3-4: epilogue -- the loss epilogue of staging half h = warpgroup - 3, one batch row per thread
+// Each staging half is handed over through an mbarrier pair: staged[h] (4 arrivals: the MMA warps of half h have written it) and
+// drained[h] (4 arrivals: the epilogue warps of half h have read it), with the same phase discipline as the operand ring.  So the
+// epilogue of tile i runs while the tensor cores accumulate tile i + 1, and a tile costs max(MMA, epilogue) instead of their sum.
+// ---------------------------------------------------------------------------------------------------------------------
+constexpr int kDecodeThreads = 640;
+// Operand ring of 32-wide k-blocks (64B swizzle, 32 KB per stage) x 4 stages: the same 128 KB as 2 stages of 64, but three stages
+// (96 KB) in flight behind the one being multiplied instead of one (64 KB).  With K = H = 500 the main loop waits on L2 -> shared
+// memory latency, not on the tensor cores, so the extra bytes in flight shorten it (H100 SXM, C2: 95 -> 76 us per launch).
+constexpr int kDecodeBK = 32;
+constexpr int kDecodeStages = 4;
+// setmaxnreg budgets (the launch gives every thread 65536 / 640 -> 96 registers; the sum may not exceed 640 x 96): the producer
+// needs next to nothing, the MMA warps keep 64 accumulators + descriptors, the epilogue warps take the rest
+constexpr int kRegsProducer = 32, kRegsMma = 104, kRegsEpilogue = 120;
+static_assert(128 * kRegsProducer + 256 * kRegsMma + 256 * kRegsEpilogue <= kDecodeThreads * 96, "register budget");
+
+template <int R> __device__ __forceinline__ void regs_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R> __device__ __forceinline__ void regs_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+
+template <int ACT, int LOSS>
+__global__ void __launch_bounds__(kDecodeThreads, 1) decode_fused_kernel(const __grid_constant__ CUtensorMap tm_a_hi,
+                                                                         const __grid_constant__ CUtensorMap tm_a_lo,
+                                                                         const __grid_constant__ CUtensorMap tm_b_hi,
+                                                                         const __grid_constant__ CUtensorMap tm_b_lo,
+                                                                         const GemmParams p) {
+  constexpr int BLOCK_N = kDecodeN, STAGES = kDecodeStages, BK = kDecodeBK;
+  constexpr int STAGE_BYTES = 2 * BLOCK_M * BK * 2 + 2 * BLOCK_N * BK * 2;
+  constexpr int SROW = BLOCK_N + 4;               // staging row stride (floats): conflict-free 16-byte row reads
+  constexpr int kParts = 2;                       // column parts per tile (one per epilogue warp of a 32-row quarter)
+  constexpr int HALF_N = BLOCK_N / kParts;        // columns handled by one epilogue warp
+  constexpr bool kFast = (ACT == DAE_ACT_SIGMOID) && (LOSS == DAE_LOSS_CE);
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  float* stg = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES);   // [BLOCK_M][SROW] accumulator staging
+  __shared__ __align__(8) uint64_t full_bar[STAGES], empty_bar[STAGES], staged_bar[2], drained_bar[2];
+  __shared__ float s_bias[2][BLOCK_N];            // per epilogue warpgroup
+  __shared__ float s_biasc[kFast ? 2 : 1][kFast ? BLOCK_N : 1];   // bv * log2(e) for the sigmoid/CE fast path
+  __shared__ __align__(16) uint8_t s_stage[8][2][32][48];  // per epilogue warp: bf16 hi / lo dZ blocks [32 rows x 16 cols], rows padded to 48 B
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int role = warp >> 2;                     // warpgroup: 0 producer, 1-2 MMA, 3-4 epilogue
+  Sched sched;                                    // initialised by each role after its register budget is set
+
+  if (warp == 0 && lane == 0) { prefetch_tmap(&tm_a_hi); prefetch_tmap(&tm_a_lo); prefetch_tmap(&tm_b_hi); prefetch_tmap(&tm_b_lo); }
+  if (warp == 1 && lane == 0) {
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 8); }   // empty: one arrival per MMA warp
+    for (int h = 0; h < 2; ++h) { mbar_init(&staged_bar[h], 4); mbar_init(&drained_bar[h], 4); }
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  if (role == 0) {
+    // ===================== TMA producer =====================
+    regs_dec<kRegsProducer>();
+    sched.init(p, BLOCK_N, 0, BK);
+    if (warp == 0 && lane == 0)
+      tma_produce<BLOCK_N, STAGES, 0, BK>(p, sched, smem, full_bar, empty_bar, 0u, &tm_a_hi, &tm_a_lo, &tm_b_hi, &tm_b_lo, &tm_a_hi, &tm_a_lo);
+  } else if (role <= 2) {
+    // ===================== MMA: wgmma main loop -> staging half =====================
+    regs_inc<kRegsMma>();
+    sched.init(p, BLOCK_N, 0, BK);
+    const int h = role - 1;
+    const int wi = warp & 3;
+    float acc[BLOCK_N / 2];
+#pragma unroll
+    for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] = 0.0f;
+    int stage = 0; uint32_t phase = 0, tphase = 0;
+    int mb, nb, kb0, kb1;
+    while (sched.next(mb, nb, kb0, kb1)) {
+      mma_work_item<BLOCK_N, STAGES, 0, 0, BK>(acc, p, smem, full_bar, empty_bar, h, lane, 0u, stage, phase, kb0, kb1);
+      mbar_wait(&drained_bar[h], tphase ^ 1);   // the epilogue is done with the previous tile's rows
+      const int r0 = h * 64 + wi * 16 + (lane >> 2), c0 = 2 * (lane & 3);
+#pragma unroll
+      for (int j = 0; j < BLOCK_N / 8; ++j) {
+        *reinterpret_cast<float2*>(&stg[r0 * SROW + 8 * j + c0]) = make_float2(acc[4 * j], acc[4 * j + 1]);
+        *reinterpret_cast<float2*>(&stg[(r0 + 8) * SROW + 8 * j + c0]) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+      }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&staged_bar[h]);
+      tphase ^= 1;
+    }
+  } else {
+    // ===================== epilogue: D = g(Z + bv); row loss; dZ -> bf16 hi/lo (autoencoder.py:411, triplet_loss_utils.py:269-275)
+    regs_inc<kRegsEpilogue>();
+    sched.init(p, BLOCK_N, 0, BK);
+    const int h = role - 3;                  // staging half: rows [64 h, 64 h + 64)
+    const int ew = warp - 12;                // epilogue warp 0..7 (its dZ transpose buffer)
+    const int wi = warp & 3;
+    const int quarter = h * 2 + (wi & 1);    // 32-row quarter of the tile this warp handles
+    const int half = wi >> 1;                // which column part of the tile
+    const int row_in_tile = quarter * 32 + lane;
+    const int tid = threadIdx.x - 128 * role;
+    const int tiles_n = (p.N + BLOCK_N - 1) / BLOCK_N;
+    uint8_t* stg_hi = reinterpret_cast<uint8_t*>(&s_stage[ew][0][0][0]);
+    uint8_t* stg_lo = reinterpret_cast<uint8_t*>(&s_stage[ew][1][0][0]);
+    const int rsub = lane >> 1, csub = lane & 1;          // write-out mapping: 16 rows x 2 x 16 B per instruction
+    uint32_t tphase = 0;
+    int mb, nb, kb0, kb1;
+    while (sched.next(mb, nb, kb0, kb1)) {
+      const float* srow = stg + row_in_tile * SROW + half * HALF_N;   // this thread's row, this warp's column part
+      const int m = mb * BLOCK_M + row_in_tile;
+      const int n0 = nb * BLOCK_N + half * HALF_N;
+      // 99 % of a bag-of-words target row is zero, so each 16-column chunk is first evaluated branch-free as if x == 0,
+      // stored, and then the row's few stored entries inside the chunk are re-evaluated exactly and patched in place.  The clean
+      // CSR row is walked with a cursor (columns are sorted) that keeps the next THREE entries (c0,v0),(c1,v1),(c2,v2) in
+      // registers.  The cursor, the row scale and the bias slice depend only on the tile's coordinates, so they are loaded
+      // while the MMA warps are still accumulating this tile.
+      int64_t pc = 0, pe = 0;
+      int c0 = 0x7fffffff, c1 = 0x7fffffff, c2 = 0x7fffffff;
+      float v0 = 0.0f, v1 = 0.0f, v2 = 0.0f;
+      float sc = 0.0f;
+      if (m < p.M) {
+        const int64_t row = p.rows ? (int64_t)p.rows[m] : (int64_t)m;
+        const int64_t rbeg = p.indptr[row];
+        const int32_t* tp = p.tile_ptr + (int64_t)m * (kParts * tiles_n + 1) + nb * kParts + half;
+        pc = rbeg + tp[0]; pe = rbeg + tp[1];     // entries of this row that fall into this half tile
+        if (pc < pe) { c0 = p.indices[pc]; v0 = p.values[pc]; }
+        if (pc + 1 < pe) { c1 = p.indices[pc + 1]; v1 = p.values[pc + 1]; }
+        if (pc + 2 < pe) { c2 = p.indices[pc + 2]; v2 = p.values[pc + 2]; }
+        sc = (p.weight ? p.weight[m] : 1.0f) / ((float)p.stats[DAE_STAT_SUM_W] + kEps);
+      }
+      named_bar_sync(1 + h, 128);   // every warp of this warpgroup is done with the previous tile's bias slice
+      {  // this tile's visible-bias slice (BLOCK_N = 128 = one column per thread)
+        const float b = (nb * BLOCK_N + tid < p.N) ? p.bv[nb * BLOCK_N + tid] : 0.0f;
+        s_bias[h][tid] = b;
+        if (kFast) s_biasc[h][tid] = b * kLog2e;
+      }
+      mbar_wait(&staged_bar[h], tphase);
+      named_bar_sync(1 + h, 128);
+      const float inv_sc = (sc != 0.0f) ? 1.0f / sc : 0.0f;
+      const bool edge = (n0 + HALF_N > p.N);   // only the last column tile has out-of-range columns
+      float lsum = 0.0f;   // CE: accumulated in log2 units, scaled by ln2 at the end
+      // dZ leaves through a per-warp shared-memory transpose: each thread (= batch row) drops the bf16 hi and lo parts of its
+      // 16 values into its two staging rows (patching the row's stored entries there), then the warp writes both 32 x 16
+      // blocks with full 32-byte sectors (16 rows per store instruction).
+      const int m_base = mb * BLOCK_M + quarter * 32;
+      const int n_lim = edge ? p.N : 0x7fffffff;
+#pragma unroll 1
+      for (int c = 0; c < HALF_N / 16; ++c) {
+        uint32_t r[16];
+        stage_ld16(srow + c * 16, r);
+        const int nc = n0 + c * 16;
+        if (m < p.M) {
+          const float* bias = &s_bias[h][half * HALF_N + c * 16];
+          uint32_t hpk[8], lpk[8];
+          bool fast_ok = false;   // this chunk went through the sigmoid/CE fast path: staged dZ = sc * D exactly
+          if (kFast && !edge) {
+            const float l0 = lsum;
+            fast_ok = decode_chunk_sigmoid_ce(r, &s_biasc[h][half * HALF_N + c * 16], sc, hpk, lpk, lsum);
+            if (!fast_ok) { lsum = l0; decode_chunk_generic<ACT, LOSS>(r, bias, sc, edge, n_lim, nc, hpk, lpk, lsum); }
+          } else {
+            decode_chunk_generic<ACT, LOSS>(r, bias, sc, edge, n_lim, nc, hpk, lpk, lsum);
+          }
+          uint4* sh = reinterpret_cast<uint4*>(stg_hi + lane * 48);
+          uint4* sl = reinterpret_cast<uint4*>(stg_lo + lane * 48);
+          sh[0] = make_uint4(hpk[0], hpk[1], hpk[2], hpk[3]); sh[1] = make_uint4(hpk[4], hpk[5], hpk[6], hpk[7]);
+          sl[0] = make_uint4(lpk[0], lpk[1], lpk[2], lpk[3]); sl[1] = make_uint4(lpk[4], lpk[5], lpk[6], lpk[7]);
+          // exact re-evaluation of the stored entries of this row inside the group (densified target, :264)
+          while (c0 < nc + 16) {
+            const float x = v0;
+            const int j = c0 - nc;
+            __nv_bfloat16* ph = reinterpret_cast<__nv_bfloat16*>(stg_hi + lane * 48) + j;
+            __nv_bfloat16* pl = reinterpret_cast<__nv_bfloat16*>(stg_lo + lane * 48) + j;
+            float d;
+            if (kFast && fast_ok && sc != 0.0f) d = (__bfloat162float(*ph) + __bfloat162float(*pl)) * inv_sc;   // D back from the staged sc * D
+            else d = act_fast<ACT>(select16(r, j) + bias[j]);
+            const float gp = act_grad_from_y<ACT>(d);
+            float dz;
+            if (LOSS == DAE_LOSS_CE) {
+              const float a = d + kEps, b = (1.0f - d) + kEps;
+              const float la = f_lg2(a), lb = f_lg2(b);
+              lsum += lb - (x * la + (1.0f - x) * lb);      // replace the x == 0 term by the exact one
+              dz = sc * gp * ((1.0f - x) * f_rcp(b) - x * f_rcp(a));
+            } else {
+              const float e2 = x - d;
+              lsum += e2 * e2 - d * d;
+              dz = -2.0f * sc * e2 * gp;
+            }
+            const __nv_bfloat16 hb = __float2bfloat16_rn(dz);
+            *ph = hb;
+            *pl = __float2bfloat16_rn(dz - __bfloat162float(hb));
+            ++pc;
+            c0 = c1; v0 = v1; c1 = c2; v1 = v2;
+            c2 = 0x7fffffff;
+            if (pc + 2 < pe) { c2 = p.indices[pc + 2]; v2 = p.values[pc + 2]; }
+          }
+        }
+        __syncwarp();
+        if (nc < p.ld_dz) {  // ld_dz is a multiple of 32 (launcher), so whole 16-column groups are in range
+#pragma unroll
+          for (int i = 0; i < 2; ++i) {
+            const int rr = rsub + 16 * i;
+            if (m_base + rr < p.M) {
+              const int64_t off = (int64_t)(m_base + rr) * p.ld_dz + nc + csub * 8;
+              *reinterpret_cast<uint4*>(p.dz_hi + off) = *reinterpret_cast<const uint4*>(stg_hi + rr * 48 + csub * 16);
+              *reinterpret_cast<uint4*>(p.dz_lo + off) = *reinterpret_cast<const uint4*>(stg_lo + rr * 48 + csub * 16);
+            }
+          }
+        }
+        __syncwarp();
+      }
+      if (lane == 0) mbar_arrive(&drained_bar[h]);   // this warp's staging rows may be overwritten (the loop ends in __syncwarp)
+      tphase ^= 1;
+      if (m < p.M) atomicAdd(p.row_loss_part + m, (LOSS == DAE_LOSS_CE) ? lsum * 0.6931471805599453f : lsum);  // 2 * tiles_n partials per row
+    }
+  }
 }
 
 // tile_ptr[m][t] = number of stored entries of batch row m with column < t * half_n (t = 0 .. n_half_tiles): where each
@@ -740,16 +868,19 @@ static PFN_encodeTiled get_encode() {
   return fn;
 }
 
-// 2-D bf16 tensor [outer x inner] (inner contiguous), row stride ld elements; box = {64, box_outer}, 128B swizzle.
-static int make_map(CUtensorMap* m, const void* base, uint64_t inner, uint64_t outer, uint64_t ld, uint32_t box_outer) {
+// 2-D bf16 tensor [outer x inner] (inner contiguous), row stride ld elements; box = {box_inner, box_outer}: 64 inner elements with the
+// 128B swizzle, 32 with the 64B swizzle.
+static int make_map(CUtensorMap* m, const void* base, uint64_t inner, uint64_t outer, uint64_t ld, uint32_t box_outer,
+                    uint32_t box_inner = 64) {
   PFN_encodeTiled enc = get_encode();
   if (!enc) { set_error("cuTensorMapEncodeTiled entry point not found"); return DAE_ERR_CUDA; }
   cuuint64_t dims[2] = {inner, outer};
   cuuint64_t strides[1] = {ld * 2};
-  cuuint32_t box[2] = {64, box_outer};
+  cuuint32_t box[2] = {box_inner, box_outer};
   cuuint32_t estr[2] = {1, 1};
   CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                   CU_TENSOR_MAP_INTERLEAVE_NONE, box_inner == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
+                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled failed (%d): inner=%llu outer=%llu ld=%llu", (int)r,
                                      (unsigned long long)inner, (unsigned long long)outer, (unsigned long long)ld); return DAE_ERR_CUDA; }
@@ -774,7 +905,7 @@ static int ensure_smem_attr(Kern kern, int smem, bool (&done)[64]) {
 static int g_pair_mode = -1;   // -1 (default) and 0: never; 1: whenever the shape allows (dae_gemm_config)
 static int g_lean = 0;         // 1: 128 x 64 tiles with 2-stage rings for dae_gemm_bf16x3 (~130 KB of shared memory instead of ~195 KB)
 
-template <int BLOCK_N, int STAGES, int EPI, int ACT, int LOSS, int PAIR, int MAJ>
+template <int BLOCK_N, int STAGES, int PAIR, int MAJ>
 static int launch_gemm_maj(const Operand& A, const Operand& B, GemmParams p, cudaStream_t st) {
   CUtensorMap ta_hi, ta_lo, tb_hi, tb_lo;
   int rc;
@@ -809,7 +940,7 @@ static int launch_gemm_maj(const Operand& A, const Operand& B, GemmParams p, cud
   if (PAIR) tiles_m = (tiles_m + 1) / 2;
   const int tiles_n = (p.N + BLOCK_N - 1) / BLOCK_N;
   const int kblocks = (p.K + BLOCK_K - 1) / BLOCK_K;
-  auto kern = gemm_bf16x3_kernel<BLOCK_N, STAGES, EPI, ACT, LOSS, PAIR, MAJ>;
+  auto kern = gemm_bf16x3_kernel<BLOCK_N, STAGES, PAIR, MAJ>;
   static bool attr_done[64] = {false};
   if ((rc = ensure_smem_attr(kern, smem, attr_done))) return rc;
   const int slots = PAIR ? sm_count() / 2 : sm_count();   // CTAs, or CTA pairs, resident at once
@@ -837,16 +968,33 @@ static int launch_gemm_maj(const Operand& A, const Operand& B, GemmParams p, cud
   return DAE_OK;
 }
 
-// the fused decode reads E and W K-major; the plain GEMMs take any majorness; (A + A^T).B goes through launch_gemm_maj directly
-template <int BLOCK_N, int STAGES, int EPI, int ACT, int LOSS, int PAIR>
+// the plain GEMMs take any majorness; (A + A^T).B goes through launch_gemm_maj directly
+template <int BLOCK_N, int STAGES, int PAIR>
 static int launch_gemm(const Operand& A, const Operand& B, GemmParams p, cudaStream_t st) {
-  if (EPI == EPI_DECODE || (!A.mn_major && !B.mn_major)) return launch_gemm_maj<BLOCK_N, STAGES, EPI, ACT, LOSS, PAIR, 0>(A, B, p, st);
-  if constexpr (EPI == EPI_STORE) {
-    if (A.mn_major && !B.mn_major) return launch_gemm_maj<BLOCK_N, STAGES, EPI, ACT, LOSS, PAIR, 1>(A, B, p, st);
-    if (!A.mn_major) return launch_gemm_maj<BLOCK_N, STAGES, EPI, ACT, LOSS, PAIR, 2>(A, B, p, st);
-    return launch_gemm_maj<BLOCK_N, STAGES, EPI, ACT, LOSS, PAIR, 3>(A, B, p, st);
-  }
-  return DAE_ERR_UNSUPPORTED;
+  if (!A.mn_major && !B.mn_major) return launch_gemm_maj<BLOCK_N, STAGES, PAIR, 0>(A, B, p, st);
+  if (A.mn_major && !B.mn_major) return launch_gemm_maj<BLOCK_N, STAGES, PAIR, 1>(A, B, p, st);
+  if (!A.mn_major) return launch_gemm_maj<BLOCK_N, STAGES, PAIR, 2>(A, B, p, st);
+  return launch_gemm_maj<BLOCK_N, STAGES, PAIR, 3>(A, B, p, st);
+}
+
+// the fused decode: E [M x K] and W [N x K], both K-major; one persistent CTA per SM over the 128 x 128 output tiles
+template <int ACT, int LOSS>
+static int launch_decode(const Operand& A, const Operand& B, const GemmParams& p, cudaStream_t st) {
+  CUtensorMap ta_hi, ta_lo, tb_hi, tb_lo;
+  int rc;
+  if ((rc = make_map(&ta_hi, A.hi, p.K, p.M, A.ld, BLOCK_M, kDecodeBK))) return rc;
+  if ((rc = make_map(&ta_lo, A.lo, p.K, p.M, A.ld, BLOCK_M, kDecodeBK))) return rc;
+  if ((rc = make_map(&tb_hi, B.hi, p.K, p.N, B.ld, kDecodeN, kDecodeBK))) return rc;
+  if ((rc = make_map(&tb_lo, B.lo, p.K, p.N, B.ld, kDecodeN, kDecodeBK))) return rc;
+  // operand ring + accumulator staging tile + alignment slack (the dZ transpose blocks are static)
+  constexpr int smem = kDecodeStages * (2 * BLOCK_M * kDecodeBK * 2 + 2 * kDecodeN * kDecodeBK * 2) + BLOCK_M * (kDecodeN + 4) * 4 + 1024;
+  auto kern = decode_fused_kernel<ACT, LOSS>;
+  static bool attr_done[64] = {false};
+  if ((rc = ensure_smem_attr(kern, smem, attr_done))) return rc;
+  const int tiles = ((p.M + BLOCK_M - 1) / BLOCK_M) * ((p.N + kDecodeN - 1) / kDecodeN);
+  const int n = tiles < sm_count() ? tiles : sm_count();
+  kern<<<n, kDecodeThreads, smem, st>>>(ta_hi, ta_lo, tb_hi, tb_lo, p);
+  return DAE_OK;
 }
 
 // CTA pairs cut the L2 -> SM traffic of the B operand by a quarter, but the multicast ties the two CTAs' pipelines together: measured
@@ -877,7 +1025,8 @@ extern "C" int dae_sym_split_bf16(const float* G, int32_t B, int64_t ldg, float 
   return DAE_OK;
 }
 
-// test hook: pair_mode 1 = CTA pairs (two-CTA clusters sharing the B tile) wherever the shape allows, otherwise never
+// test hook: pair_mode 1 = CTA pairs (two-CTA clusters sharing the B tile) for dae_gemm_bf16x3 wherever the shape allows, otherwise
+// never; lean = 1: 128 x 64 tiles with 2-stage rings for dae_gemm_bf16x3.  The fused decode has one configuration.
 extern "C" int dae_gemm_config(int32_t pair_mode, int32_t lean) {
   dae::g_pair_mode = pair_mode < 0 ? -1 : (pair_mode ? 1 : 0);
   dae::g_lean = lean ? 1 : 0;
@@ -923,10 +1072,10 @@ extern "C" int dae_gemm_bf16x3(int32_t M, int32_t N, int32_t K, float alpha, con
   int rc;
   const int tiles128 = tm * tn128 * k_splits, tiles64 = tm * tn64 * k_splits;
   const float cost128 = 2.0f * (float)((tiles128 + sms - 1) / sms), cost64 = 1.1f * (float)((tiles64 + sms - 1) / sms);
-  if (g_lean) rc = launch_gemm<64, 2, EPI_STORE, 0, 0, 0>(A, B, p, st);
-  else if (use_pair()) rc = launch_gemm<128, 2, EPI_STORE, 0, 0, 1>(A, B, p, st);
-  else if (!stream_k && cost64 < cost128) rc = launch_gemm<64, 3, EPI_STORE, 0, 0, 0>(A, B, p, st);
-  else rc = launch_gemm<128, 2, EPI_STORE, 0, 0, 0>(A, B, p, st);
+  if (g_lean) rc = launch_gemm<64, 2, 0>(A, B, p, st);
+  else if (use_pair()) rc = launch_gemm<128, 2, 1>(A, B, p, st);
+  else if (!stream_k && cost64 < cost128) rc = launch_gemm<64, 3, 0>(A, B, p, st);
+  else rc = launch_gemm<128, 2, 0>(A, B, p, st);
   if (rc) return rc;
   DAE_CHECK_LAUNCH("dae_gemm_bf16x3");
   return DAE_OK;
@@ -947,7 +1096,7 @@ extern "C" int dae_gemm_sym_bf16x3(int32_t M, int32_t N, float alpha, const void
   p.C = C; p.ldc = ldc; p.n_store = N; p.special_col = -1; p.special_out = nullptr; p.a_sym_kb = kb_half;
   if (!accumulate) DAE_CUDA(cudaMemset2DAsync(C, ldc * sizeof(float), 0, (size_t)N * sizeof(float), M, (cudaStream_t)stream));
   Operand A{g_hi, g_lo, ldg, 0}, B{b_hi, b_lo, ldb, 1};
-  int rc = launch_gemm_maj<128, 2, EPI_STORE, 0, 0, 0, 6>(A, B, p, (cudaStream_t)stream);
+  int rc = launch_gemm_maj<128, 2, 0, 6>(A, B, p, (cudaStream_t)stream);
   if (rc) return rc;
   DAE_CHECK_LAUNCH("dae_gemm_sym_bf16x3");
   return DAE_OK;
@@ -986,10 +1135,7 @@ extern "C" int dae_decode_fused_bf16x3(int32_t Brows, int32_t F, int32_t K, cons
   }
   Operand A{e_hi, e_lo, lde, 0}, B{w_hi, w_lo, ldw, 0};
   int rc = 0;
-  // the fused epilogue, not operand traffic, bounds this kernel (K = H is short): CTA pairs only when forced (tests)
-  const bool pair = (g_pair_mode == 1);
-#define DAE_DEC(ACT, LOSS) rc = pair ? launch_gemm<kDecodeN, 2, EPI_DECODE, ACT, LOSS, 1>(A, B, p, st) \
-                              : launch_gemm<kDecodeN, 2, EPI_DECODE, ACT, LOSS, 0>(A, B, p, st)
+#define DAE_DEC(ACT, LOSS) rc = launch_decode<ACT, LOSS>(A, B, p, st)
   if (loss_func == DAE_LOSS_CE) {
     if (dec_act == DAE_ACT_SIGMOID) DAE_DEC(DAE_ACT_SIGMOID, DAE_LOSS_CE);
     else if (dec_act == DAE_ACT_TANH) DAE_DEC(DAE_ACT_TANH, DAE_LOSS_CE);

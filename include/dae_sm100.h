@@ -195,8 +195,8 @@ int dae_gemm_bf16x3(int32_t M, int32_t N, int32_t K, float alpha, const void* a_
 int dae_gemm_sym_bf16x3(int32_t M, int32_t N, float alpha, const void* g_hi, const void* g_lo, int64_t ldg,
                         const void* b_hi, const void* b_lo, int64_t ldb, float* C, int64_t ldc, int32_t accumulate,
                         void* stream);
-/* Tile engine selection of the two entry points above (test hook).  pair_mode: 1 = CTA pairs (a two-CTA cluster works on two
- * adjacent 128-row tiles and each CTA multicasts half of the shared B tile into both) whenever possible (fused decode included);
+/* Tile engine selection of dae_gemm_bf16x3 (test hook).  pair_mode: 1 = CTA pairs (a two-CTA cluster works on two
+ * adjacent 128-row tiles and each CTA multicasts half of the shared B tile into both) whenever possible (not the fused decode);
  * -1 (default) or 0 = never (slower on the H100 at the BASELINE shapes).  lean: 0 (default) = 128x128 / 128x64 tiles chosen by shape;
  * 1 = dae_gemm_bf16x3 on 128x64 tiles with 2-stage rings (~130 KB of shared memory per CTA). */
 int dae_gemm_config(int32_t pair_mode, int32_t lean);
