@@ -17,6 +17,8 @@
 //   fused decode (dae_decode_fused_bf16x3; 640 threads = five warpgroups, see decode_fused_kernel): the same producer, two MMA
 //                   warpgroups that only run the main loop, and two epilogue warpgroups that run the loss epilogue of tile i from
 //                   the staging tile while the MMA warpgroups accumulate tile i + 1.
+//   similarity top-k (dae_similarity_topk_bf16x3; see topk_kernel): the fused decode's five warpgroups with a k-best selection
+//                   epilogue instead of the loss, so the similarity matrix never leaves the SM.
 // Operands may be K-major (K contiguous) or MN-major (M/N contiguous) -- both straight from row-major arrays (wgmma's transpose
 // bits), so no transposed copies of dZ / E / W are ever made.
 #include <cuda.h>
@@ -370,8 +372,9 @@ __device__ __forceinline__ void stage_ld16(const float* src, uint32_t (&r)[16]) 
 
 // TMA producer (one lane): fills the STAGES-deep ring with the A and B k-blocks (hi and lo) of every work item of `sched`, in order.
 // PAIR = 1: two-CTA cluster sharing the B tile through TMA multicast (see the PTX wrappers above).
-template <int BLOCK_N, int STAGES, int PAIR, int BK = BLOCK_K>
-__device__ __forceinline__ void tma_produce(const GemmParams& p, Sched& sched, uint8_t* smem, uint64_t* full_bar, uint64_t* empty_bar,
+// SchedT: Sched, or any walker with the same next(mb, nb, kb0, kb1) (TopkSched).
+template <int BLOCK_N, int STAGES, int PAIR, int BK = BLOCK_K, class SchedT>
+__device__ __forceinline__ void tma_produce(const GemmParams& p, SchedT& sched, uint8_t* smem, uint64_t* full_bar, uint64_t* empty_bar,
                                             uint32_t crank, const CUtensorMap* tm_a_hi, const CUtensorMap* tm_a_lo,
                                             const CUtensorMap* tm_b_hi, const CUtensorMap* tm_b_lo, const CUtensorMap* tm_at_hi,
                                             const CUtensorMap* tm_at_lo) {
@@ -796,6 +799,238 @@ __global__ void __launch_bounds__(kDecodeThreads, 1) decode_fused_kernel(const _
   }
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// fused similarity + k-best selection (dae_similarity_topk_bf16x3): for every query row i the k largest S[i, j] = Q_i . C_j and their
+// corpus indices, without writing S.  The five warpgroups, register split and staged / drained hand-off of the fused decode; the
+// schedule, the epilogue and the shape of the operand ring differ.
+//   work item: (128-row block of Q, contiguous range of column tiles) -- split s of `splits`.  A CTA sweeps its range left to right
+//              and its epilogue threads keep their running lists over the whole sweep.
+//   epilogue : thread = (row, 64-column half of every tile), as in the decode.  A list of KMAX (score, index) pairs sorted by
+//              (score desc, index asc) lives in registers, every index into it unrolled.  Four staged values cost one compare
+//              against the current k-th score; only a value that beats it is inserted.  Columns arrive in increasing order and an
+//              equal score never displaces an entry, so among equal scores the lower index stays first.  At the end of the item
+//              the first k entries go to the workspace (2 * splits lists per row) and topk_merge_kernel merges them.
+// ---------------------------------------------------------------------------------------------------------------------
+constexpr int kTopkMaxK = 32;
+constexpr int kTopkMaxSplits = 32;   // 2 * splits lists per row: at most two per lane of the merging warp
+constexpr int kTopkMinTiles = 4;     // automatic splits sweep at least this many column tiles (amortises the list flush)
+// Operand ring: 2 stages of 64-wide k-blocks (128B swizzle, 64 KB each), as the store GEMM, not the decode's 4 x 32.  Measured on an
+// H100 SXM (700 W) at Nq = Nc = 100 000, H = 500, k = 10: 81 ms per call with 2 x 64, 92 ms with 3 x 32, 113 ms with 4 x 32.
+constexpr int kTopkBK = 64;
+constexpr int kTopkStages = 2;
+
+struct TopkParams {
+  GemmParams g;                      // M = queries, N = corpus rows, K = dim
+  int k, splits;
+  int exclude;                       // != 0: column i + diag_offset is not a candidate of row i
+  int64_t diag_offset;
+  float* ws_val; int32_t* ws_idx;    // [M x 2 splits x k] partial lists
+};
+
+// (row block, column-tile range) work items, items blockIdx.x, blockIdx.x + gridDim.x, ...; next() returns one column tile at a time,
+// with `first` / `last` marking the ends of an item.  Every range is non-empty (the launcher keeps splits <= column tiles).
+struct TopkSched {
+  int tiles_n, splits, kb_total, n_work, n_cta, w;
+  int mb, split, t, t_end;
+  bool first, last;
+  __device__ __forceinline__ void init(const TopkParams& tp, int block_n, int block_k) {
+    const int tiles_m = (tp.g.M + BLOCK_M - 1) / BLOCK_M;
+    tiles_n = (tp.g.N + block_n - 1) / block_n;
+    splits = tp.splits;
+    kb_total = (tp.g.K + block_k - 1) / block_k;
+    n_work = tiles_m * splits;
+    n_cta = (int)gridDim.x;
+    w = (int)blockIdx.x - n_cta;
+    mb = split = t = t_end = 0;
+    first = last = false;
+  }
+  __device__ __forceinline__ bool next(int& mb_, int& nb, int& kb0, int& kb1) {
+    first = false;
+    if (t >= t_end) {
+      w += n_cta;
+      if (w >= n_work) return false;
+      mb = w / splits;
+      split = w - mb * splits;
+      t = split * tiles_n / splits;                 // 32-bit: splits <= 32 and tiles_n < 2^24
+      t_end = (split + 1) * tiles_n / splits;
+      first = true;
+    }
+    mb_ = mb; nb = t; kb0 = 0; kb1 = kb_total;
+    last = (++t == t_end);
+    return true;
+  }
+};
+
+__device__ __forceinline__ float neg_inf() { return __int_as_float(0xff800000); }
+
+// offer (v, col) to a sorted list whose k-th score is thr: inserted if it beats thr and is a candidate
+template <int KMAX>
+__device__ __forceinline__ void topk_offer(float (&sv)[KMAX], int (&si)[KMAX], float& thr, int k, float v, int col, int n_lim,
+                                           int excl) {
+  if (!(v > thr) || col >= n_lim || col == excl) return;
+#pragma unroll
+  for (int j = KMAX - 1; j >= 0; --j) {   // downwards: sv[j - 1] still holds its old value when entry j is rewritten
+    const bool up = (j > 0) && (v > sv[j > 0 ? j - 1 : 0]);
+    const bool here = v > sv[j];
+    si[j] = up ? si[j > 0 ? j - 1 : 0] : (here ? col : si[j]);
+    sv[j] = up ? sv[j > 0 ? j - 1 : 0] : (here ? v : sv[j]);
+  }
+  // thr = sv[k - 1].  The select is PTX so that the compiler cannot fold the unrolled chain back into a dynamic index, which
+  // would move sv to local memory.
+  float t = sv[0];
+#pragma unroll
+  for (int j = 1; j < KMAX; ++j)
+    asm("{\n.reg .pred q;\nsetp.eq.s32 q, %1, %2;\nselp.f32 %0, %3, %0, q;\n}\n" : "+f"(t) : "r"(j), "r"(k - 1), "f"(sv[j]));
+  thr = t;
+}
+
+template <int KMAX>
+__global__ void __launch_bounds__(kDecodeThreads, 1) topk_kernel(const __grid_constant__ CUtensorMap tm_a_hi,
+                                                                 const __grid_constant__ CUtensorMap tm_a_lo,
+                                                                 const __grid_constant__ CUtensorMap tm_b_hi,
+                                                                 const __grid_constant__ CUtensorMap tm_b_lo,
+                                                                 const TopkParams tp) {
+  constexpr int BLOCK_N = kDecodeN, STAGES = kTopkStages, BK = kTopkBK;
+  constexpr int STAGE_BYTES = 2 * BLOCK_M * BK * 2 + 2 * BLOCK_N * BK * 2;
+  constexpr int SROW = BLOCK_N + 4;               // staging row stride (floats): conflict-free 16-byte row reads
+  constexpr int HALF_N = BLOCK_N / 2;             // columns handled by one epilogue thread per tile
+  const GemmParams& p = tp.g;
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  float* stg = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES);   // [BLOCK_M][SROW] accumulator staging
+  __shared__ __align__(8) uint64_t full_bar[STAGES], empty_bar[STAGES], staged_bar[2], drained_bar[2];
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int role = warp >> 2;                     // warpgroup: 0 producer, 1-2 MMA, 3-4 epilogue
+  TopkSched sched;
+
+  if (warp == 0 && lane == 0) { prefetch_tmap(&tm_a_hi); prefetch_tmap(&tm_a_lo); prefetch_tmap(&tm_b_hi); prefetch_tmap(&tm_b_lo); }
+  if (warp == 1 && lane == 0) {
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 8); }
+    for (int h = 0; h < 2; ++h) { mbar_init(&staged_bar[h], 4); mbar_init(&drained_bar[h], 4); }
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  if (role == 0) {
+    // ===================== TMA producer =====================
+    regs_dec<kRegsProducer>();
+    sched.init(tp, BLOCK_N, BK);
+    if (warp == 0 && lane == 0)
+      tma_produce<BLOCK_N, STAGES, 0, BK>(p, sched, smem, full_bar, empty_bar, 0u, &tm_a_hi, &tm_a_lo, &tm_b_hi, &tm_b_lo, &tm_a_hi, &tm_a_lo);
+  } else if (role <= 2) {
+    // ===================== MMA: wgmma main loop -> staging half =====================
+    regs_inc<kRegsMma>();
+    sched.init(tp, BLOCK_N, BK);
+    const int h = role - 1;
+    const int wi = warp & 3;
+    float acc[BLOCK_N / 2];
+#pragma unroll
+    for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] = 0.0f;
+    int stage = 0; uint32_t phase = 0, tphase = 0;
+    int mb, nb, kb0, kb1;
+    while (sched.next(mb, nb, kb0, kb1)) {
+      mma_work_item<BLOCK_N, STAGES, 0, 0, BK>(acc, p, smem, full_bar, empty_bar, h, lane, 0u, stage, phase, kb0, kb1);
+      mbar_wait(&drained_bar[h], tphase ^ 1);   // the epilogue is done with the previous tile's rows
+      const int r0 = h * 64 + wi * 16 + (lane >> 2), c0 = 2 * (lane & 3);
+#pragma unroll
+      for (int j = 0; j < BLOCK_N / 8; ++j) {
+        *reinterpret_cast<float2*>(&stg[r0 * SROW + 8 * j + c0]) = make_float2(acc[4 * j], acc[4 * j + 1]);
+        *reinterpret_cast<float2*>(&stg[(r0 + 8) * SROW + 8 * j + c0]) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+      }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&staged_bar[h]);
+      tphase ^= 1;
+    }
+  } else {
+    // ===================== epilogue: running k-best list of one (row, column half) =====================
+    regs_inc<kRegsEpilogue>();
+    sched.init(tp, BLOCK_N, BK);
+    const int h = role - 3;                  // staging half: rows [64 h, 64 h + 64)
+    const int wi = warp & 3;
+    const int quarter = h * 2 + (wi & 1);    // 32-row quarter of the tile this warp handles
+    const int half = wi >> 1;                // which column half of the tile
+    const int row_in_tile = quarter * 32 + lane;
+    const int k = tp.k;
+    const float* srow = stg + row_in_tile * SROW + half * HALF_N;
+    float sv[KMAX];
+    int si[KMAX];
+    float thr = neg_inf();
+    int m = 0, excl = -1;
+    uint32_t tphase = 0;
+    int mb, nb, kb0, kb1;
+    while (sched.next(mb, nb, kb0, kb1)) {
+      if (sched.first) {
+#pragma unroll
+        for (int j = 0; j < KMAX; ++j) { sv[j] = neg_inf(); si[j] = -1; }
+        thr = neg_inf();
+        m = mb * BLOCK_M + row_in_tile;
+        const int64_t e = (int64_t)m + tp.diag_offset;
+        excl = (tp.exclude && e >= 0 && e < p.N) ? (int)e : -1;
+      }
+      const int n0 = nb * BLOCK_N + half * HALF_N;
+      mbar_wait(&staged_bar[h], tphase);
+      if (m < p.M) {
+#pragma unroll 1
+        for (int c = 0; c < HALF_N; c += 4) {
+          const float4 v = *reinterpret_cast<const float4*>(srow + c);
+          if (fmaxf(fmaxf(v.x, v.y), fmaxf(v.z, v.w)) > thr) {   // rare once the list has filled
+            topk_offer<KMAX>(sv, si, thr, k, v.x, n0 + c, p.N, excl);
+            topk_offer<KMAX>(sv, si, thr, k, v.y, n0 + c + 1, p.N, excl);
+            topk_offer<KMAX>(sv, si, thr, k, v.z, n0 + c + 2, p.N, excl);
+            topk_offer<KMAX>(sv, si, thr, k, v.w, n0 + c + 3, p.N, excl);
+          }
+        }
+      }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&drained_bar[h]);   // this warp's staging rows may be overwritten
+      tphase ^= 1;
+      if (sched.last && m < p.M) {
+        const int64_t base = ((int64_t)m * (2 * sched.splits) + 2 * sched.split + half) * k;
+#pragma unroll
+        for (int j = 0; j < KMAX; ++j)
+          if (j < k) { tp.ws_val[base + j] = sv[j]; tp.ws_idx[base + j] = si[j]; }
+      }
+    }
+  }
+}
+
+// (v1, i1) ranks before (v2, i2): higher score first, lower index among equal scores; index -1 (no entry) ranks last
+__device__ __forceinline__ bool topk_before(float v1, int i1, float v2, int i2) {
+  return i1 >= 0 && (i2 < 0 || v1 > v2 || (v1 == v2 && i1 < i2));
+}
+
+// one warp per query row: n_lists sorted partial lists of k (lane l owns lists l and l + 32) -> the row's k best, padded with -1 / -inf
+__global__ void __launch_bounds__(256) topk_merge_kernel(const float* __restrict__ ws_val, const int32_t* __restrict__ ws_idx, int rows,
+                                                         int n_lists, int k, int32_t* __restrict__ idx_out, float* __restrict__ val_out) {
+  const int lane = threadIdx.x & 31;
+  const int r = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (r >= rows) return;
+  const int64_t base = (int64_t)r * n_lists * k;
+  const int la = lane, lb = lane + 32;
+  int ha = 0, hb = 0;                          // heads of the two lists
+  for (int j = 0; j < k; ++j) {
+    float va = neg_inf(), vb = neg_inf();
+    int ia = -1, ib = -1;
+    if (la < n_lists && ha < k) { va = ws_val[base + (int64_t)la * k + ha]; ia = ws_idx[base + (int64_t)la * k + ha]; }
+    if (lb < n_lists && hb < k) { vb = ws_val[base + (int64_t)lb * k + hb]; ib = ws_idx[base + (int64_t)lb * k + hb]; }
+    float bv = va;
+    int bi = ia;
+    if (topk_before(vb, ib, bv, bi)) { bv = vb; bi = ib; }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
+      const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+      if (topk_before(ov, oi, bv, bi)) { bv = ov; bi = oi; }
+    }
+    if (bi >= 0) {                             // corpus indices are unique across the lists: exactly one head moves
+      if (ia == bi) ++ha;
+      else if (ib == bi) ++hb;
+    }
+    if (lane == 0) { idx_out[(int64_t)r * k + j] = bi; val_out[(int64_t)r * k + j] = (bi >= 0) ? bv : neg_inf(); }
+  }
+}
+
 // tile_ptr[m][t] = number of stored entries of batch row m with column < t * half_n (t = 0 .. n_half_tiles): where each
 // half tile of the fused decode epilogue starts in the (sorted) clean CSR row.  One thread per (row, t).
 __global__ void decode_tile_ptr_kernel(const int64_t* __restrict__ indptr, const int32_t* __restrict__ indices,
@@ -997,6 +1232,46 @@ static int launch_decode(const Operand& A, const Operand& B, const GemmParams& p
   return DAE_OK;
 }
 
+// fused similarity + k-best: Q [M x K] and C [N x K], both K-major; one persistent CTA per SM over the (row block, split) work items
+template <int KMAX>
+static int launch_topk(const Operand& A, const Operand& B, const TopkParams& tp, cudaStream_t st) {
+  CUtensorMap ta_hi, ta_lo, tb_hi, tb_lo;
+  int rc;
+  const GemmParams& p = tp.g;
+  if ((rc = make_map(&ta_hi, A.hi, p.K, p.M, A.ld, BLOCK_M, kTopkBK))) return rc;
+  if ((rc = make_map(&ta_lo, A.lo, p.K, p.M, A.ld, BLOCK_M, kTopkBK))) return rc;
+  if ((rc = make_map(&tb_hi, B.hi, p.K, p.N, B.ld, kDecodeN, kTopkBK))) return rc;
+  if ((rc = make_map(&tb_lo, B.lo, p.K, p.N, B.ld, kDecodeN, kTopkBK))) return rc;
+  // operand ring + accumulator staging tile + alignment slack
+  constexpr int smem = kTopkStages * (2 * BLOCK_M * kTopkBK * 2 + 2 * kDecodeN * kTopkBK * 2) + BLOCK_M * (kDecodeN + 4) * 4 + 1024;
+  auto kern = topk_kernel<KMAX>;
+  static bool attr_done[64] = {false};
+  if ((rc = ensure_smem_attr(kern, smem, attr_done))) return rc;
+  const int items = ((p.M + BLOCK_M - 1) / BLOCK_M) * tp.splits;
+  const int n = items < sm_count() ? items : sm_count();
+  kern<<<n, kDecodeThreads, smem, st>>>(ta_hi, ta_lo, tb_hi, tb_lo, tp);
+  return DAE_OK;
+}
+
+// column splits of dae_similarity_topk_bf16x3: `requested` (> 0), or the fewest that give every SM a work item while each split
+// still sweeps kTopkMinTiles column tiles; always within [1, min(column tiles, kTopkMaxSplits)]
+static int topk_splits(int n_query, int n_corpus, int requested) {
+  const int tiles_m = (n_query + BLOCK_M - 1) / BLOCK_M, tiles_n = (n_corpus + kDecodeN - 1) / kDecodeN;
+  int s = requested;
+  if (s <= 0) {
+    s = (sm_count() + tiles_m - 1) / tiles_m;
+    const int by_len = tiles_n / kTopkMinTiles;
+    if (s > by_len) s = by_len;
+  }
+  if (s > tiles_n) s = tiles_n;
+  if (s > kTopkMaxSplits) s = kTopkMaxSplits;
+  return s < 1 ? 1 : s;
+}
+
+static int64_t topk_workspace_bytes(int n_query, int k, int splits) {
+  return (int64_t)n_query * 2 * splits * k * (int64_t)(sizeof(float) + sizeof(int32_t));
+}
+
 // CTA pairs cut the L2 -> SM traffic of the B operand by a quarter, but the multicast ties the two CTAs' pipelines together: measured
 // on an H100 SXM (700 W) at C2, a training step takes 0.384 ms without pairs and 0.476 ms with them, so they run only when forced
 static bool use_pair() { return g_pair_mode == 1 && !g_lean; }
@@ -1148,5 +1423,42 @@ extern "C" int dae_decode_fused_bf16x3(int32_t Brows, int32_t F, int32_t K, cons
 #undef DAE_DEC
   if (rc) return rc;
   DAE_CHECK_LAUNCH("dae_decode_fused_bf16x3");
+  return DAE_OK;
+}
+
+extern "C" int dae_similarity_topk_workspace(int32_t n_query, int32_t n_corpus, int32_t k, int32_t splits, int64_t* bytes) {
+  DAE_REQUIRE(bytes && n_query > 0 && n_corpus > 0, "dae_similarity_topk_workspace: bad arguments");
+  DAE_REQUIRE(k >= 1 && k <= kTopkMaxK, "dae_similarity_topk_workspace: k = %d is outside the supported range 1 <= k <= %d", k, kTopkMaxK);
+  *bytes = topk_workspace_bytes(n_query, k, topk_splits(n_query, n_corpus, splits));
+  return DAE_OK;
+}
+
+extern "C" int dae_similarity_topk_bf16x3(int32_t n_query, int32_t n_corpus, int32_t dim, const void* q_hi, const void* q_lo, int64_t ldq,
+                                          const void* c_hi, const void* c_lo, int64_t ldc, int32_t k, int64_t diag_offset, int32_t exclude,
+                                          int32_t splits, void* workspace, int64_t workspace_bytes, int32_t* idx_out, float* val_out,
+                                          void* stream) {
+  DAE_REQUIRE(q_hi && q_lo && c_hi && c_lo && workspace && idx_out && val_out, "dae_similarity_topk_bf16x3: null pointer");
+  DAE_REQUIRE(n_query > 0 && n_corpus > 0 && dim > 0, "dae_similarity_topk_bf16x3: bad sizes");
+  DAE_REQUIRE(k >= 1 && k <= kTopkMaxK, "dae_similarity_topk_bf16x3: k = %d is outside the supported range 1 <= k <= %d", k, kTopkMaxK);
+  DAE_REQUIRE(ldq >= dim && ldc >= dim && ldq % 8 == 0 && ldc % 8 == 0,
+              "dae_similarity_topk_bf16x3: leading dimensions must cover dim and be multiples of 8 (TMA 16-byte strides)");
+  DAE_REQUIRE(((uintptr_t)q_hi | (uintptr_t)q_lo | (uintptr_t)c_hi | (uintptr_t)c_lo | (uintptr_t)workspace) % 16 == 0,
+              "dae_similarity_topk_bf16x3: operands and workspace must be 16-byte aligned");
+  const int s = topk_splits(n_query, n_corpus, splits);
+  const int64_t need = topk_workspace_bytes(n_query, k, s);
+  DAE_REQUIRE(workspace_bytes >= need, "dae_similarity_topk_bf16x3: workspace of %lld bytes, %lld needed (dae_similarity_topk_workspace)",
+              (long long)workspace_bytes, (long long)need);
+  cudaStream_t st = (cudaStream_t)stream;
+  TopkParams tp{};
+  tp.g.M = n_query; tp.g.N = n_corpus; tp.g.K = dim; tp.g.k_splits = 1; tp.g.alpha = 1.0f; tp.g.special_col = -1;
+  tp.k = k; tp.splits = s; tp.exclude = exclude ? 1 : 0; tp.diag_offset = diag_offset;
+  tp.ws_val = reinterpret_cast<float*>(workspace);
+  tp.ws_idx = reinterpret_cast<int32_t*>(reinterpret_cast<float*>(workspace) + (int64_t)n_query * 2 * s * k);
+  Operand A{q_hi, q_lo, ldq, 0}, B{c_hi, c_lo, ldc, 0};
+  int rc = (k <= 16) ? launch_topk<16>(A, B, tp, st) : launch_topk<32>(A, B, tp, st);
+  if (rc) return rc;
+  DAE_CHECK_LAUNCH("dae_similarity_topk_bf16x3");
+  topk_merge_kernel<<<(n_query + 7) / 8, 256, 0, st>>>(tp.ws_val, tp.ws_idx, n_query, 2 * s, k, idx_out, val_out);
+  DAE_CHECK_LAUNCH("dae_similarity_topk_bf16x3 (merge)");
   return DAE_OK;
 }

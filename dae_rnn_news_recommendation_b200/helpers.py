@@ -3,11 +3,15 @@ nearest-article lookup of main_autoencoder.py:307-318,352-359) -- SURVEY section
 
     pairwise_similarity(in_df, norm='', metric='cosine', set_diagonal_zero=True) -> ndarray [N, N]     (reference signature)
     nearest_neighbors(embeddings, metric='cosine', chunk=8192) -> (index[N], score[N])                (no N x N matrix on the host)
+    top_k_similar(embeddings, k=10, corpus=None, metric='cosine') -> (index[Nq, k], score[Nq, k])    (no similarity matrix at all)
+    label_precision_at_k(index, query_labels, corpus_labels) -> float                                 (share of same-label neighbours)
     visualize_pairwise_similarity(labels, pairwise_similarity_metrics, ...) -> dict                   (rank 2: AUROC + box statistics)
 
 Dense inputs (embeddings) go through the wgmma bf16x3 GEMM on row-normalised operands; sparse inputs (count / tf-idf
 matrices) through the CSR encode kernel against the dense transpose.  No CPU path.
 """
+import ctypes
+
 import numpy as np
 import scipy.sparse as sp
 import torch
@@ -115,6 +119,71 @@ def nearest_neighbors(embeddings, metric='cosine', chunk=8192, device='cuda:0'):
         call('dae_row_argmax', buf.data_ptr(), r1 - r0, n, buf.stride(0), r0, 0, idx[r0:r1].data_ptr(), val[r0:r1].data_ptr(), _stream())
     torch.cuda.synchronize()
     return idx.cpu().numpy(), val.cpu().numpy()
+
+
+def _similarity_topk(q, c, n_q, n_c, h, k, diag_offset=0, exclude=False, splits=0):
+    """k best corpus rows per query row of the bf16 hi / lo operand pairs q and c (dae_similarity_topk_bf16x3): device tensors
+    (index int32 [n_q, k], score float32 [n_q, k]); with `exclude`, column i + diag_offset is not a candidate of row i."""
+    dev = q[0].device
+    need = (ctypes.c_int64 * 1)()
+    call('dae_similarity_topk_workspace', n_q, n_c, k, splits, ctypes.addressof(need))
+    ws = torch.empty(max(int(need[0]), 16), dtype=torch.uint8, device=dev)
+    idx = torch.empty(n_q, k, dtype=torch.int32, device=dev)
+    val = torch.empty(n_q, k, dtype=torch.float32, device=dev)
+    call('dae_similarity_topk_bf16x3', n_q, n_c, h, q[0].data_ptr(), q[1].data_ptr(), q[0].stride(0), c[0].data_ptr(), c[1].data_ptr(),
+         c[0].stride(0), k, diag_offset, 1 if exclude else 0, splits, ws.data_ptr(), ws.numel(), idx.data_ptr(), val.data_ptr(), _stream())
+    return idx, val
+
+
+def _as_device_dense(x, device):
+    if isinstance(x, torch.Tensor):
+        return x.to(device=device, dtype=torch.float32).contiguous()
+    return _to_device_dense(x, device)
+
+
+def top_k_similar(embeddings, k=10, corpus=None, metric='cosine', device='cuda:0', to_host=True, splits=0):
+    """For every row of `embeddings` the k most similar rows of `corpus` and their scores, best first (among equal scores the
+    lower index first), computed on the tensor cores without forming the similarity matrix.  corpus=None ranks the set
+    against itself and leaves each row's self match out.  Rows with fewer than k candidates are padded with index -1 and
+    score -inf.  metric: 'cosine' or 'linear kernel', as in pairwise_similarity; dense inputs (arrays or torch tensors).
+    Returns (index int32 [Nq, k], score float32 [Nq, k]) as ndarrays, or device tensors with to_host=False.  `splits`
+    (> 0) fixes the number of column ranges the work is cut into; it does not change the result."""
+    assert metric in ['cosine', 'linear kernel']
+    if not 1 <= k <= 32:
+        raise _cabi.DaeError('top_k_similar: k = %d is outside the supported range 1 <= k <= 32' % k)
+    norm_kind = 2 if metric == 'cosine' else 0
+    x = _as_device_dense(embeddings, device)
+    n_q, h = x.shape
+    q = _normalised_operands(x, norm_kind)[:2]
+    if corpus is None:
+        c, n_c = q, n_q
+    else:
+        xc = _as_device_dense(corpus, device)
+        if xc.shape[1] != h:
+            raise ValueError('top_k_similar: corpus rows have %d columns, queries %d' % (xc.shape[1], h))
+        n_c = xc.shape[0]
+        c = _normalised_operands(xc, norm_kind)[:2]
+    idx, val = _similarity_topk(q, c, n_q, n_c, h, k, exclude=corpus is None, splits=splits)
+    if to_host:
+        return idx.cpu().numpy(), val.cpu().numpy()
+    return idx, val
+
+
+def label_precision_at_k(index, query_labels, corpus_labels):
+    """Mean over the queries of the fraction of returned neighbours (index [Nq, k] from top_k_similar) whose corpus label equals
+    the query's label.  Padding (index -1) is not a neighbour; queries labelled -1, or without any neighbour, are skipped.
+    NaN when no query counts."""
+    index = np.asarray(index.cpu() if isinstance(index, torch.Tensor) else index)
+    ql = np.asarray(query_labels.values if hasattr(query_labels, 'values') else query_labels).reshape(-1)
+    cl = np.asarray(corpus_labels.values if hasattr(corpus_labels, 'values') else corpus_labels).reshape(-1)
+    assert index.ndim == 2 and index.shape[0] == ql.shape[0]
+    valid = index >= 0
+    hit = valid & (cl[np.where(valid, index, 0)] == ql[:, None])
+    n = valid.sum(1)
+    use = (ql != -1) & (n > 0)
+    if not use.any():
+        return float('nan')
+    return float((hit.sum(1)[use] / n[use]).mean())
 
 
 def _group_sizes(labels):

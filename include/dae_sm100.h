@@ -288,6 +288,24 @@ int dae_rownorm_split_bf16(const float* X, int32_t rows, int32_t cols, int64_t l
 int dae_row_argmax(float* S, int32_t rows, int32_t cols, int64_t ld, int64_t diag_offset, int32_t zero_diag,
                    int32_t* idx_out, float* val_out, void* stream);
 
+/* ---- k most similar articles without the similarity matrix ---------------------------------------------------------
+ * dae_similarity_topk_bf16x3: S = Q.C^T (Q [n_query x dim], C [n_corpus x dim], both as bf16 hi/lo pairs with row strides ldq /
+ *   ldc, e.g. from dae_rownorm_split_bf16) on the tensor cores, bf16x3 as dae_gemm_bf16x3, with a k-best selection fused into the
+ *   epilogue: S never leaves the SM.  Row i of idx_out / val_out [n_query x k] (int32 / fp32, row stride k) lists the k corpus
+ *   rows of highest score in strictly decreasing (score, -index) order -- among equal scores the lower index first, the rule of
+ *   dae_row_argmax -- padded with -1 / -inf when a row has fewer than k candidates.  exclude != 0: column i + diag_offset is not
+ *   a candidate of row i (the self match when Q is C or a row window of it).  1 <= k <= 32; ldq, ldc >= dim and multiples of 8;
+ *   operands 16-byte aligned.  Each CTA sweeps a contiguous range of column tiles of a 128-row block; `splits` (> 0) sets the
+ *   number of ranges, 0 picks the fewest that fill the SMs.  The scores do not depend on it (no split over dim), so neither
+ *   does the output.  workspace: at least dae_similarity_topk_workspace bytes (same n_query, n_corpus, k, splits), 16-byte aligned.
+ * dae_similarity_topk_workspace: *bytes = the workspace size of that call (2 * splits partial lists of k per query row).
+ */
+int dae_similarity_topk_bf16x3(int32_t n_query, int32_t n_corpus, int32_t dim, const void* q_hi, const void* q_lo,
+                               int64_t ldq, const void* c_hi, const void* c_lo, int64_t ldc, int32_t k,
+                               int64_t diag_offset, int32_t exclude, int32_t splits, void* workspace,
+                               int64_t workspace_bytes, int32_t* idx_out, float* val_out, void* stream);
+int dae_similarity_topk_workspace(int32_t n_query, int32_t n_corpus, int32_t k, int32_t splits, int64_t* bytes);
+
 /* ---- "next" row (SURVEY 8f rank 2): related-vs-unrelated AUROC of a pairwise similarity matrix ---------------------
  * Replaces the numeric part of helpers.visualize_pairwise_similarity (helpers.py:88-100).
  * dae_pair_partition: for every pair i > j of the strict lower triangle with labels[i] >= 0 and labels[j] >= 0

@@ -63,6 +63,9 @@ def build_parser():
     ap.add_argument('--synthetic', type=int, default=0, help='train on N synthetic articles instead of reading --data_path')
     ap.add_argument('--rng_mode', default='device', choices=['numpy', 'device'],
                     help="'device': Philox masking + device permutation (default); 'numpy': the reference's host NumPy RNG stream")
+    ap.add_argument('--top_k', type=int, default=0,
+                    help='K > 0: after transform, save the K most similar training articles of every training and every validation '
+                         'article (K <= 32) and report the share that shares the label; 0 = off')
     return ap
 
 
@@ -107,6 +110,7 @@ def check_flags(F):
     assert F.triplet_strategy in ['batch_all', 'batch_hard', 'none']
     assert F.input_format in ['binary', 'tfidf']
     assert F.label in ['category_publish_name', 'story']
+    assert 0 <= F.top_k <= 32
     if F.input_format == 'tfidf':
         assert F.loss_func in ['mean_squared', 'cosine_proximity']
     if F.main_dir == '':
@@ -244,6 +248,27 @@ def evaluate(F, model, trX, vlX, trL, vlL, enc, enc_v, max_rows=20000):
     return out
 
 
+def recommend_top_k(F, model, enc, enc_v, trL, vlL):
+    """--top_k K: the K most similar training articles of every training article (itself left out) and of every validation
+    article (recommendations for new articles), by cosine similarity of the embeddings, at any number of rows.  Both lists
+    are saved under data_dir as article_top_k_{index,score}[_validate].npy; the label precision of each is returned."""
+    from dae_rnn_news_recommendation_b200 import helpers
+    out = {}
+    print('calculate top %d similar articles' % F.top_k)
+    for split, E, lab in (('', enc, trL), ('_validate', enc_v, vlL)):
+        if E is None or E.shape[0] == 0:
+            continue
+        idx, score = helpers.top_k_similar(E, k=F.top_k, corpus=None if split == '' else enc, metric='cosine')
+        np.save(model.data_dir + 'article_top_k_index' + split, idx)
+        np.save(model.data_dir + 'article_top_k_score' + split, score)
+        out['top_k' + split] = (idx, score)
+        out['top_k_precision' + split] = helpers.label_precision_at_k(idx, lab, trL)
+        print('top %d%s: label precision %.4f' % (F.top_k, split, out['top_k_precision' + split]))
+        for i in range(min(3, len(idx))):
+            print('article %d%s: most similar %s' % (i, split, ', '.join('%d (%.4f)' % (j, s) for j, s in zip(idx[i], score[i]) if j >= 0)))
+    return out
+
+
 def main(argv=None):
     F = check_flags(apply_env_overrides(build_parser().parse_args(argv)))
     print(__file__ + ': Start')
@@ -275,6 +300,8 @@ def main(argv=None):
     if F.save_tsv:
         save_tsv(model, data, enc, enc_v)
     model.evaluation = evaluate(F, model, trX, vlX, trL, vlL, enc, enc_v)
+    if F.top_k > 0:
+        model.evaluation.update(recommend_top_k(F, model, enc, enc_v, trL, vlL))
     print(__file__ + ': End')
     return model
 
