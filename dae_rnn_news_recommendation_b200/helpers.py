@@ -3,12 +3,14 @@ nearest-article lookup of main_autoencoder.py:307-318,352-359) -- SURVEY section
 
     pairwise_similarity(in_df, norm='', metric='cosine', set_diagonal_zero=True) -> ndarray [N, N]     (reference signature)
     nearest_neighbors(embeddings, metric='cosine', chunk=8192) -> (index[N], score[N])                (no N x N matrix on the host)
-    top_k_similar(embeddings, k=10, corpus=None, metric='cosine') -> (index[Nq, k], score[Nq, k])    (no similarity matrix at all)
+    top_k_similar(embeddings, k=10, corpus=None, metric='cosine') -> (index[Nq, k], score[Nq, k])    (no similarity matrix at all;
+                                                                                                        dense or scipy sparse inputs)
     label_precision_at_k(index, query_labels, corpus_labels) -> float                                 (share of same-label neighbours)
     visualize_pairwise_similarity(labels, pairwise_similarity_metrics, ...) -> dict                   (rank 2: AUROC + box statistics)
 
 Dense inputs (embeddings) go through the wgmma bf16x3 GEMM on row-normalised operands; sparse inputs (count / tf-idf
-matrices) through the CSR encode kernel against the dense transpose.  No CPU path.
+matrices) through the CSR encode kernel against the dense transpose, except in top_k_similar, where they go through the
+sparse CSR x CSR top-k kernel (dae_csr_similarity_topk).  No CPU path.
 """
 import ctypes
 
@@ -18,7 +20,7 @@ import torch
 
 from . import _cabi
 from ._cabi import call
-from .engine import DeviceCSR
+from .engine import DeviceCSR, canonical_csr
 from .io_formats import save_file, read_file  # noqa: F401  (reference helpers.py:138-264; SURVEY 8f rank 3)
 
 _NORM = {'': 0, 'l1': 1, 'l2': 2, 'max': 3}
@@ -141,16 +143,60 @@ def _as_device_dense(x, device):
     return _to_device_dense(x, device)
 
 
+def _csr_operand(x, metric):
+    """The CSR matrix the sparse top-k ranks: canonical (sorted, no duplicates), fp32, rows L2-normalised for 'cosine' with
+    all-zero rows left zero (sklearn.preprocessing.normalize, as _pairwise_sparse)."""
+    m = canonical_csr(x).astype(np.float32)
+    if metric == 'cosine':
+        from sklearn.preprocessing import normalize   # host-side row scaling of the CSR values only (data prep)
+        m = canonical_csr(normalize(m, norm='l2')).astype(np.float32)
+    return m
+
+
+def _csr_similarity_topk(q, c, k, diag_offset=0, exclude=False, splits=0):
+    """k best corpus rows per query row of the DeviceCSR matrices q and c by S = Q.C^T (dae_csr_similarity_topk): device tensors
+    (index int32 [n_q, k], score float32 [n_q, k]); with `exclude`, column i + diag_offset is not a candidate of row i."""
+    dev = q.indptr.device
+    n_q, n_c = q.shape[0], c.shape[0]
+    need = (ctypes.c_int64 * 1)()
+    call('dae_csr_similarity_topk_workspace', n_q, n_c, c.nnz, c.shape[1], k, splits, ctypes.addressof(need))
+    ws = torch.empty(max(int(need[0]), 16), dtype=torch.uint8, device=dev)
+    idx = torch.empty(n_q, k, dtype=torch.int32, device=dev)
+    val = torch.empty(n_q, k, dtype=torch.float32, device=dev)
+    call('dae_csr_similarity_topk', q.indptr.data_ptr(), q.indices.data_ptr(), q.values.data_ptr(), n_q, q.nnz, q.shape[1],
+         c.indptr.data_ptr(), c.indices.data_ptr(), c.values.data_ptr(), n_c, c.nnz, c.shape[1], k, diag_offset, 1 if exclude else 0,
+         splits, ws.data_ptr(), ws.numel(), idx.data_ptr(), val.data_ptr(), _stream())
+    return idx, val
+
+
+def _top_k_similar_sparse(embeddings, k, corpus, metric, device, splits):
+    if corpus is not None and corpus.shape[1] != embeddings.shape[1]:
+        raise ValueError('top_k_similar: corpus rows have %d columns, queries %d' % (corpus.shape[1], embeddings.shape[1]))
+    q = DeviceCSR(_csr_operand(embeddings, metric), device)
+    c = q if corpus is None else DeviceCSR(_csr_operand(corpus, metric), device)
+    return _csr_similarity_topk(q, c, k, exclude=corpus is None, splits=splits)
+
+
 def top_k_similar(embeddings, k=10, corpus=None, metric='cosine', device='cuda:0', to_host=True, splits=0):
     """For every row of `embeddings` the k most similar rows of `corpus` and their scores, best first (among equal scores the
-    lower index first), computed on the tensor cores without forming the similarity matrix.  corpus=None ranks the set
-    against itself and leaves each row's self match out.  Rows with fewer than k candidates are padded with index -1 and
-    score -inf.  metric: 'cosine' or 'linear kernel', as in pairwise_similarity; dense inputs (arrays or torch tensors).
+    lower index first), without forming the similarity matrix.  corpus=None ranks the set against itself and leaves each row's
+    self match out.  Rows with fewer than k candidates are padded with index -1 and score -inf.  metric: 'cosine' or
+    'linear kernel', as in pairwise_similarity.
+    Dense inputs (arrays or torch tensors) run on the tensor cores (bf16x3).  Sparse inputs (scipy sparse matrices: the binary /
+    tf-idf bag of words) run through dae_csr_similarity_topk, which only spends work on the columns two rows share; every score
+    is the fp32 sum of the rounded products in increasing column order.  Queries and corpus must be both dense or both sparse.
     Returns (index int32 [Nq, k], score float32 [Nq, k]) as ndarrays, or device tensors with to_host=False.  `splits`
-    (> 0) fixes the number of column ranges the work is cut into; it does not change the result."""
+    (> 0) fixes the number of corpus parts the work is cut into; it does not change the result."""
     assert metric in ['cosine', 'linear kernel']
     if not 1 <= k <= 32:
         raise _cabi.DaeError('top_k_similar: k = %d is outside the supported range 1 <= k <= 32' % k)
+    if corpus is not None and sp.issparse(embeddings) != sp.issparse(corpus):
+        raise ValueError('top_k_similar: queries and corpus must be both sparse or both dense')
+    if sp.issparse(embeddings):
+        idx, val = _top_k_similar_sparse(embeddings, k, corpus, metric, device, splits)
+        if to_host:
+            return idx.cpu().numpy(), val.cpu().numpy()
+        return idx, val
     norm_kind = 2 if metric == 'cosine' else 0
     x = _as_device_dense(embeddings, device)
     n_q, h = x.shape

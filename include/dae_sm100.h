@@ -306,6 +306,26 @@ int dae_similarity_topk_bf16x3(int32_t n_query, int32_t n_corpus, int32_t dim, c
                                int64_t workspace_bytes, int32_t* idx_out, float* val_out, void* stream);
 int dae_similarity_topk_workspace(int32_t n_query, int32_t n_corpus, int32_t k, int32_t splits, int64_t* bytes);
 
+/* ---- k most similar articles of sparse (bag-of-words) vectors ------------------------------------------------------
+ * dae_csr_similarity_topk: the same selection as dae_similarity_topk_bf16x3 for S[q, c] = sum_f Q[q, f] C[c, f] of two CSR
+ *   matrices (indptr int64, indices int32 sorted inside a row, values fp32; q_features == c_features), on the CUDA cores and
+ *   without forming S.  Every corpus row is a candidate, a row sharing no column with q included (score 0), except column
+ *   q + diag_offset when `exclude` is set; order (score desc, index asc); padding -1 / -inf.  Each score accumulates in fp32 from
+ *   0, one term per shared column in increasing column order, each term the product rounded to fp32 and then added (no FMA), so
+ *   the output does not depend on `splits` (> 0: the number of corpus parts, 0: automatic) and a float32 host loop over the
+ *   columns reproduces it exactly.  1 <= k <= 32; corpus nnz < 2^31; workspace 16-byte aligned, at least
+ *   dae_csr_similarity_topk_workspace bytes for the same n_query, n_corpus, c_nnz, features, k and splits.
+ * dae_csr_similarity_topk_workspace: *bytes = that workspace: the corpus postings (8 B per entry), their bucket offsets
+ *   ((n_corpus / 2048 + 1) x features int32) and, when the corpus is split, the partial lists (8 B per entry).
+ */
+int dae_csr_similarity_topk(const int64_t* q_indptr, const int32_t* q_indices, const float* q_values, int32_t n_query,
+                            int64_t q_nnz, int32_t q_features, const int64_t* c_indptr, const int32_t* c_indices,
+                            const float* c_values, int32_t n_corpus, int64_t c_nnz, int32_t c_features, int32_t k,
+                            int64_t diag_offset, int32_t exclude, int32_t splits, void* workspace, int64_t workspace_bytes,
+                            int32_t* idx_out, float* val_out, void* stream);
+int dae_csr_similarity_topk_workspace(int32_t n_query, int32_t n_corpus, int64_t corpus_nnz, int32_t n_features, int32_t k,
+                                      int32_t splits, int64_t* bytes);
+
 /* ---- "next" row (SURVEY 8f rank 2): related-vs-unrelated AUROC of a pairwise similarity matrix ---------------------
  * Replaces the numeric part of helpers.visualize_pairwise_similarity (helpers.py:88-100).
  * dae_pair_partition: for every pair i > j of the strict lower triangle with labels[i] >= 0 and labels[j] >= 0

@@ -66,6 +66,9 @@ def build_parser():
     ap.add_argument('--top_k', type=int, default=0,
                     help='K > 0: after transform, save the K most similar training articles of every training and every validation '
                          'article (K <= 32) and report the share that shares the label; 0 = off')
+    ap.add_argument('--top_k_input', action='store_true', default=False,
+                    help='with --top_k K: also rank by the input vectors (cosine for binary, linear kernel for tf-idf), save '
+                         'article_top_k_input_{index,score}[_validate].npy and report their label precision next to the embedding\'s')
     return ap
 
 
@@ -111,6 +114,7 @@ def check_flags(F):
     assert F.input_format in ['binary', 'tfidf']
     assert F.label in ['category_publish_name', 'story']
     assert 0 <= F.top_k <= 32
+    assert not F.top_k_input or F.top_k > 0, '--top_k_input needs --top_k K > 0'
     if F.input_format == 'tfidf':
         assert F.loss_func in ['mean_squared', 'cosine_proximity']
     if F.main_dir == '':
@@ -269,6 +273,27 @@ def recommend_top_k(F, model, enc, enc_v, trL, vlL):
     return out
 
 
+def recommend_top_k_input(F, model, trX, vlX, trL, vlL, emb_out):
+    """--top_k_input: the same K-best lists ranked by the input vectors instead of the embeddings -- the bag-of-words baseline the
+    embedding is meant to beat -- with the metric evaluate() uses for them (cosine for binary, linear kernel for tf-idf), on the
+    sparse top-k kernel.  Saved as article_top_k_input_{index,score}[_validate].npy; both precisions are printed side by side."""
+    from dae_rnn_news_recommendation_b200 import helpers
+    out = {}
+    in_metric = 'cosine' if F.input_format == 'binary' else 'linear kernel'
+    print('calculate top %d similar articles by input vectors (%s)' % (F.top_k, in_metric))
+    for split, X, lab in (('', trX, trL), ('_validate', vlX, vlL)):
+        if X is None or X.shape[0] == 0:
+            continue
+        idx, score = helpers.top_k_similar(X, k=F.top_k, corpus=None if split == '' else trX, metric=in_metric)
+        np.save(model.data_dir + 'article_top_k_input_index' + split, idx)
+        np.save(model.data_dir + 'article_top_k_input_score' + split, score)
+        out['top_k_input' + split] = (idx, score)
+        out['top_k_input_precision' + split] = helpers.label_precision_at_k(idx, lab, trL)
+        print('top %d%s label precision: embedding %.4f  input vectors %.4f' % (
+            F.top_k, split, emb_out.get('top_k_precision' + split, float('nan')), out['top_k_input_precision' + split]))
+    return out
+
+
 def main(argv=None):
     F = check_flags(apply_env_overrides(build_parser().parse_args(argv)))
     print(__file__ + ': Start')
@@ -302,6 +327,8 @@ def main(argv=None):
     model.evaluation = evaluate(F, model, trX, vlX, trL, vlL, enc, enc_v)
     if F.top_k > 0:
         model.evaluation.update(recommend_top_k(F, model, enc, enc_v, trL, vlL))
+        if F.top_k_input:
+            model.evaluation.update(recommend_top_k_input(F, model, trX, vlX, trL, vlL, model.evaluation))
     print(__file__ + ': End')
     return model
 
