@@ -335,18 +335,21 @@ __device__ __forceinline__ bool decode_chunk_sigmoid_ce(const uint32_t (&r)[16],
 }
 
 // One k-block (BK / 16 k16 steps) of a warpgroup's 64 x BLOCK_N tile: lo.hi, hi.lo, hi.hi per step, small terms first.
-// BK = 64: 128-byte swizzle, either majorness; BK = 32: 64-byte swizzle, K-major operands only.
+// K-major: 128-byte swizzle at BK = 64, 64-byte swizzle at BK = 32 (rows of BK bf16, 8-row groups SBO apart).
+// MN-major: 128-byte swizzle at either BK, 64-element column slabs of BK k-rows (LBO = slab stride 64 BK 2 bytes).
 template <int BLOCK_N, int TA, int TB, int BK = BLOCK_K>
 __device__ __forceinline__ void mma_kblock(float (&acc)[BLOCK_N / 2], uint32_t sa_hi, uint32_t sa_lo, uint32_t sb_hi, uint32_t sb_lo,
                                            bool first) {
-  static_assert(BK == 64 || (BK == 32 && !TA && !TB), "32-wide k-blocks are K-major only");
-  constexpr uint32_t layout = BK == 64 ? 1u : 2u, sbo = BK == 64 ? 1024u : 512u;
-  constexpr uint32_t a_lbo = TA ? 8192u : 16u, b_lbo = TB ? 8192u : 16u;
+  static_assert(BK == 64 || BK == 32, "k-blocks are 32 or 64 wide");
+  constexpr uint32_t kmaj_layout = BK == 64 ? 1u : 2u, kmaj_sbo = BK == 64 ? 1024u : 512u, mn_lbo = 64u * BK * 2u;
+  constexpr uint32_t a_layout = TA ? 1u : kmaj_layout, b_layout = TB ? 1u : kmaj_layout;
+  constexpr uint32_t a_sbo = TA ? 1024u : kmaj_sbo, b_sbo = TB ? 1024u : kmaj_sbo;
+  constexpr uint32_t a_lbo = TA ? mn_lbo : 16u, b_lbo = TB ? mn_lbo : 16u;
   constexpr uint32_t a_step = TA ? 2048u : 32u, b_step = TB ? 2048u : 32u;  // bytes per WGMMA_K
 #pragma unroll
   for (int k = 0; k < BK / WGMMA_K; ++k) {
-    const uint64_t da_hi = make_desc(sa_hi + k * a_step, a_lbo, sbo, layout), da_lo = make_desc(sa_lo + k * a_step, a_lbo, sbo, layout);
-    const uint64_t db_hi = make_desc(sb_hi + k * b_step, b_lbo, sbo, layout), db_lo = make_desc(sb_lo + k * b_step, b_lbo, sbo, layout);
+    const uint64_t da_hi = make_desc(sa_hi + k * a_step, a_lbo, a_sbo, a_layout), da_lo = make_desc(sa_lo + k * a_step, a_lbo, a_sbo, a_layout);
+    const uint64_t db_hi = make_desc(sb_hi + k * b_step, b_lbo, b_sbo, b_layout), db_lo = make_desc(sb_lo + k * b_step, b_lbo, b_sbo, b_layout);
     const uint32_t sc = (first && k == 0) ? 0u : 1u;
     if constexpr (BLOCK_N == 128) {
       wgmma_n128<TA, TB>(acc, da_lo, db_hi, sc);
@@ -480,7 +483,7 @@ __device__ __forceinline__ void mma_work_item(float (&acc)[BLOCK_N / 2], const G
 // ---------------------------------------------------------------------------------------------------------------------
 // store GEMM: C (+)= alpha A.B, 384 threads = producer + two consumer warpgroups that run the main loop and then the store epilogue
 // ---------------------------------------------------------------------------------------------------------------------
-template <int BLOCK_N, int STAGES, int PAIR, int MAJ>
+template <int BLOCK_N, int STAGES, int PAIR, int MAJ, int BK = BLOCK_K>
 __global__ void __launch_bounds__(kThreads, 1) gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap tm_a_hi,
                                                                    const __grid_constant__ CUtensorMap tm_a_lo,
                                                                    const __grid_constant__ CUtensorMap tm_b_hi,
@@ -489,7 +492,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_bf16x3_kernel(const __grid_c
                                                                    const __grid_constant__ CUtensorMap tm_at_lo,
                                                                    const GemmParams p) {
   static_assert(!PAIR || BLOCK_N == 128, "CTA pairs split the B tile into two 64-row halves");
-  constexpr int STAGE_BYTES = 2 * BLOCK_M * BLOCK_K * 2 + 2 * BLOCK_N * BLOCK_K * 2;
+  constexpr int STAGE_BYTES = 2 * BLOCK_M * BK * 2 + 2 * BLOCK_N * BK * 2;
   constexpr int SROW = BLOCK_N + 4;               // staging row stride (floats): conflict-free 16-byte row reads
   constexpr int kParts = 2;                       // column parts per tile (one per epilogue warp of a 32-row quarter)
   constexpr int HALF_N = BLOCK_N / kParts;        // columns handled by one epilogue warp
@@ -500,7 +503,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_bf16x3_kernel(const __grid_c
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   Sched sched;
-  sched.init(p, BLOCK_N, PAIR);
+  sched.init(p, BLOCK_N, PAIR, BK);
   const uint32_t crank = PAIR ? cluster_ctarank() : 0u;
 
   if (warp == 0 && lane == 0) {
@@ -516,7 +519,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_bf16x3_kernel(const __grid_c
 
   if (warp == 0) {
     if (lane == 0)
-      tma_produce<BLOCK_N, STAGES, PAIR>(p, sched, smem, full_bar, empty_bar, crank, &tm_a_hi, &tm_a_lo, &tm_b_hi, &tm_b_lo, &tm_at_hi,
+      tma_produce<BLOCK_N, STAGES, PAIR, BK>(p, sched, smem, full_bar, empty_bar, crank, &tm_a_hi, &tm_a_lo, &tm_b_hi, &tm_b_lo, &tm_at_hi,
                                          &tm_at_lo);
   } else if (warp >= 4) {
     // ===================== consumers: wgmma main loop, then the store epilogue =====================
@@ -531,7 +534,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_bf16x3_kernel(const __grid_c
     int mb, nb, kb0, kb1;
     while (sched.next(mb, nb, kb0, kb1)) {
       if (PAIR) mb = mb * 2 + (int)crank;     // this CTA's 128-row m tile of the pair
-      mma_work_item<BLOCK_N, STAGES, PAIR, MAJ>(acc, p, smem, full_bar, empty_bar, wg, lane, crank, stage, phase, kb0, kb1);
+      mma_work_item<BLOCK_N, STAGES, PAIR, MAJ, BK>(acc, p, smem, full_bar, empty_bar, wg, lane, crank, stage, phase, kb0, kb1);
 
       // accumulators -> staging rows (the previous tile's epilogue of this warpgroup must be done with them)
       named_bar_sync(1 + wg, 128);
@@ -1103,27 +1106,27 @@ static int ensure_smem_attr(Kern kern, int smem, bool (&done)[64]) {
 static int g_pair_mode = -1;   // -1 (default) and 0: never; 1: whenever the shape allows (dae_gemm_config)
 static int g_lean = 0;         // 1: 128 x 64 tiles with 2-stage rings for dae_gemm_bf16x3 (~130 KB of shared memory instead of ~195 KB)
 
-template <int BLOCK_N, int STAGES, int PAIR, int MAJ>
+template <int BLOCK_N, int STAGES, int PAIR, int MAJ, int BK = BLOCK_K>
 static int launch_gemm_maj(const Operand& A, const Operand& B, GemmParams p, cudaStream_t st) {
   CUtensorMap ta_hi, ta_lo, tb_hi, tb_lo;
   int rc;
   constexpr int B_ROWS = PAIR ? BLOCK_N / 2 : BLOCK_N;   // n rows of the B tile one CTA loads
-  // K-major: tensor [rows=MN x cols=K], box {64 k, tile rows};  MN-major: tensor [rows=K x cols=MN], box {64 mn, 64 k}
+  // K-major: tensor [rows=MN x cols=K], box {BK k, tile rows};  MN-major: tensor [rows=K x cols=MN], box {64 mn, BK k}
   if (!A.mn_major) {
     const uint64_t a_cols = p.a_sym_kb > 0 ? (uint64_t)p.M : (uint64_t)p.K;   // (A + A^T).B: A is M x M, K = 2 x (padded M)
-    if ((rc = make_map(&ta_hi, A.hi, a_cols, p.M, A.ld, BLOCK_M))) return rc;
-    if ((rc = make_map(&ta_lo, A.lo, a_cols, p.M, A.ld, BLOCK_M))) return rc;
+    if ((rc = make_map(&ta_hi, A.hi, a_cols, p.M, A.ld, BLOCK_M, BK))) return rc;
+    if ((rc = make_map(&ta_lo, A.lo, a_cols, p.M, A.ld, BLOCK_M, BK))) return rc;
   } else {
-    if ((rc = make_map(&ta_hi, A.hi, p.M, p.K, A.ld, 64))) return rc;
-    if ((rc = make_map(&ta_lo, A.lo, p.M, p.K, A.ld, 64))) return rc;
+    if ((rc = make_map(&ta_hi, A.hi, p.M, p.K, A.ld, BK))) return rc;
+    if ((rc = make_map(&ta_lo, A.lo, p.M, p.K, A.ld, BK))) return rc;
   }
   if (!B.mn_major) {
-    if ((rc = make_map(&tb_hi, B.hi, p.K, p.N, B.ld, B_ROWS))) return rc;
-    if ((rc = make_map(&tb_lo, B.lo, p.K, p.N, B.ld, B_ROWS))) return rc;
+    if ((rc = make_map(&tb_hi, B.hi, p.K, p.N, B.ld, B_ROWS, BK))) return rc;
+    if ((rc = make_map(&tb_lo, B.lo, p.K, p.N, B.ld, B_ROWS, BK))) return rc;
   } else {
     const uint64_t b_rows = p.a_sym_kb > 0 ? (uint64_t)p.M : (uint64_t)p.K;
-    if ((rc = make_map(&tb_hi, B.hi, p.N, b_rows, B.ld, 64))) return rc;
-    if ((rc = make_map(&tb_lo, B.lo, p.N, b_rows, B.ld, 64))) return rc;
+    if ((rc = make_map(&tb_hi, B.hi, p.N, b_rows, B.ld, BK))) return rc;
+    if ((rc = make_map(&tb_lo, B.lo, p.N, b_rows, B.ld, BK))) return rc;
   }
   p.a_mn = A.mn_major; p.b_mn = B.mn_major;
   CUtensorMap tat_hi = ta_hi, tat_lo = ta_lo;
@@ -1133,19 +1136,19 @@ static int launch_gemm_maj(const Operand& A, const Operand& B, GemmParams p, cud
     if ((rc = make_map(&tat_lo, A.lo, p.M, p.M, A.ld, 64))) return rc;
   }
   // operand ring + accumulator staging tile + alignment slack
-  constexpr int smem = STAGES * (2 * BLOCK_M * BLOCK_K * 2 + 2 * BLOCK_N * BLOCK_K * 2) + BLOCK_M * (BLOCK_N + 4) * 4 + 1024;
+  constexpr int smem = STAGES * (2 * BLOCK_M * BK * 2 + 2 * BLOCK_N * BK * 2) + BLOCK_M * (BLOCK_N + 4) * 4 + 1024;
   int tiles_m = (p.M + BLOCK_M - 1) / BLOCK_M;
   if (PAIR) tiles_m = (tiles_m + 1) / 2;
   const int tiles_n = (p.N + BLOCK_N - 1) / BLOCK_N;
-  const int kblocks = (p.K + BLOCK_K - 1) / BLOCK_K;
-  auto kern = gemm_bf16x3_kernel<BLOCK_N, STAGES, PAIR, MAJ>;
+  const int kblocks = (p.K + BK - 1) / BK;
+  auto kern = gemm_bf16x3_kernel<BLOCK_N, STAGES, PAIR, MAJ, BK>;
   static bool attr_done[64] = {false};
   if ((rc = ensure_smem_attr(kern, smem, attr_done))) return rc;
   const int slots = PAIR ? sm_count() / 2 : sm_count();   // CTAs, or CTA pairs, resident at once
   int n;
-  if (p.stream_k) {   // segments of at least ~6 k-blocks: a shorter main loop does not amortise its (atomic) epilogue
+  if (p.stream_k) {   // segments of at least 6 k-blocks of 64 (12 of 32): a shorter main loop does not amortise its (atomic) epilogue
     const long long units = (long long)tiles_m * tiles_n * kblocks;
-    long long g = units / 6;
+    long long g = units / (6 * BLOCK_K / BK);
     if (g < 1) g = 1;
     n = (int)(g < slots ? g : slots);
   } else {
@@ -1167,12 +1170,12 @@ static int launch_gemm_maj(const Operand& A, const Operand& B, GemmParams p, cud
 }
 
 // the plain GEMMs take any majorness; (A + A^T).B goes through launch_gemm_maj directly
-template <int BLOCK_N, int STAGES, int PAIR>
+template <int BLOCK_N, int STAGES, int PAIR, int BK = BLOCK_K>
 static int launch_gemm(const Operand& A, const Operand& B, GemmParams p, cudaStream_t st) {
-  if (!A.mn_major && !B.mn_major) return launch_gemm_maj<BLOCK_N, STAGES, PAIR, 0>(A, B, p, st);
-  if (A.mn_major && !B.mn_major) return launch_gemm_maj<BLOCK_N, STAGES, PAIR, 1>(A, B, p, st);
-  if (!A.mn_major) return launch_gemm_maj<BLOCK_N, STAGES, PAIR, 2>(A, B, p, st);
-  return launch_gemm_maj<BLOCK_N, STAGES, PAIR, 3>(A, B, p, st);
+  if (!A.mn_major && !B.mn_major) return launch_gemm_maj<BLOCK_N, STAGES, PAIR, 0, BK>(A, B, p, st);
+  if (A.mn_major && !B.mn_major) return launch_gemm_maj<BLOCK_N, STAGES, PAIR, 1, BK>(A, B, p, st);
+  if (!A.mn_major) return launch_gemm_maj<BLOCK_N, STAGES, PAIR, 2, BK>(A, B, p, st);
+  return launch_gemm_maj<BLOCK_N, STAGES, PAIR, 3, BK>(A, B, p, st);
 }
 
 // the fused decode: E [M x K] and W [N x K], both K-major; one persistent CTA per SM over the 128 x 128 output tiles
@@ -1306,12 +1309,16 @@ extern "C" int dae_gemm_bf16x3(int32_t M, int32_t N, int32_t K, float alpha, con
   p.special_col = (special_out ? special_col : -1); p.special_out = special_out;
   Operand A{a_hi, a_lo, lda, a_mn_major}, B{b_hi, b_lo, ldb, b_mn_major};
   // 128 x 128 tiles move fewer operand bytes per output, 128 x 64 tiles quantise better onto the SMs: pick the variant with the
-  // smaller (waves x relative tile cost).  Stream-K balances by construction, so it always takes the 128 x 128 tiles.
+  // smaller (waves x relative tile cost).  Stream-K balances by construction, so it always takes the 128 x 128 tiles, with a ring of
+  // 4 stages of 32-wide k-blocks: the same 128 KB as 2 x 64, but three stages (96 KB) in flight behind the one being multiplied
+  // instead of one (64 KB), which the L2 -> shared-memory latency of dE / dW needs (see DESIGN 4.1).  The lean and pair test
+  // configurations keep the 2 x 64 rings.
   int rc;
   const int tiles128 = tm * tn128 * k_splits, tiles64 = tm * tn64 * k_splits;
   const float cost128 = 2.0f * (float)((tiles128 + sms - 1) / sms), cost64 = 1.1f * (float)((tiles64 + sms - 1) / sms);
   if (g_lean) rc = launch_gemm<64, 2, 0>(A, B, p, st);
   else if (use_pair()) rc = launch_gemm<128, 2, 1>(A, B, p, st);
+  else if (stream_k) rc = launch_gemm<128, 4, 0, 32>(A, B, p, st);
   else if (!stream_k && cost64 < cost128) rc = launch_gemm<64, 3, 0>(A, B, p, st);
   else rc = launch_gemm<128, 2, 0>(A, B, p, st);
   if (rc) return rc;
