@@ -19,12 +19,15 @@
 //                   the staging tile while the MMA warpgroups accumulate tile i + 1.
 //   similarity top-k (dae_similarity_topk_bf16x3; see topk_kernel): the fused decode's five warpgroups with a k-best selection
 //                   epilogue instead of the loss, so the similarity matrix never leaves the SM.
+//   pair histogram (dae_similarity_pair_hist_bf16x3; see pair_hist_kernel): the same five warpgroups over the lower-triangle tiles
+//                   of X.X^T, binning related / unrelated pair scores into uint64 histograms for the AUROC.
 // Operands may be K-major (K contiguous) or MN-major (M/N contiguous) -- both straight from row-major arrays (wgmma's transpose
 // bits), so no transposed copies of dZ / E / W are ever made.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <type_traits>
 #include "common.cuh"
+#include "pair_hist.cuh"
 #include "topk.cuh"
 
 namespace dae {
@@ -997,6 +1000,167 @@ __global__ void __launch_bounds__(kDecodeThreads, 1) topk_kernel(const __grid_co
   }
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// related / unrelated pair histogram (dae_similarity_pair_hist_bf16x3): for every pair i > j of rows of X with labels >= 0 the
+// bf16x3 score S[i, j] = X_i . X_j is binned into hist[related ? 0 : 1][bin], without writing S.  topk_kernel's five warpgroups,
+// operand ring and staged / drained hand-off; a different schedule and epilogue.
+//   work item: one 128 x 128 tile with nb <= mb (the lower triangle and the diagonal: half of the tiles of S), dealt round-robin.
+//   epilogue : thread = (row, 64-column half), as in top-k.  Each warp copies the labels of its 64 columns to shared memory, then
+//              walks its row's columns in order, skips j >= i and label -1, and adds runs of equal (group, bin) to hist with one
+//              red.global.add.u64 each.  The fp64 score sums of the two groups stay in registers and are flushed once per tile.
+// ---------------------------------------------------------------------------------------------------------------------
+struct PairHistParams {
+  GemmParams g;                      // M = N = rows of X, K = dim
+  const int32_t* labels;             // [N], -1 = no label
+  float range, scale;                // M of the grid and bins / (2M)
+  uint32_t bins;
+  unsigned long long* hist;          // [2 x bins]
+  double* sums;                      // [2]
+};
+
+// tiles t = mb (mb + 1) / 2 + nb, nb <= mb, items blockIdx.x, blockIdx.x + gridDim.x, ...
+struct PairHistSched {
+  long long t, n_tiles;
+  int n_cta, kb_total;
+  __device__ __forceinline__ void init(const PairHistParams& hp, int block_k) {
+    const long long tm = (hp.g.M + BLOCK_M - 1) / BLOCK_M;
+    n_tiles = tm * (tm + 1) / 2;
+    kb_total = (hp.g.K + block_k - 1) / block_k;
+    n_cta = (int)gridDim.x;
+    t = blockIdx.x;
+  }
+  __device__ __forceinline__ bool next(int& mb, int& nb, int& kb0, int& kb1) {
+    if (t >= n_tiles) return false;
+    long long r = (long long)((sqrt(8.0 * (double)t + 1.0) - 1.0) * 0.5);
+    while (r * (r + 1) / 2 > t) --r;
+    while ((r + 1) * (r + 2) / 2 <= t) ++r;
+    mb = (int)r;
+    nb = (int)(t - r * (r + 1) / 2);
+    kb0 = 0; kb1 = kb_total;
+    t += n_cta;
+    return true;
+  }
+};
+
+__global__ void __launch_bounds__(kDecodeThreads, 1) pair_hist_kernel(const __grid_constant__ CUtensorMap tm_a_hi,
+                                                                      const __grid_constant__ CUtensorMap tm_a_lo,
+                                                                      const __grid_constant__ CUtensorMap tm_b_hi,
+                                                                      const __grid_constant__ CUtensorMap tm_b_lo,
+                                                                      const PairHistParams hp) {
+  constexpr int BLOCK_N = kDecodeN, STAGES = kTopkStages, BK = kTopkBK;
+  constexpr int STAGE_BYTES = 2 * BLOCK_M * BK * 2 + 2 * BLOCK_N * BK * 2;
+  constexpr int SROW = BLOCK_N + 4;
+  constexpr int HALF_N = BLOCK_N / 2;
+  const GemmParams& p = hp.g;
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  float* stg = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES);   // [BLOCK_M][SROW] accumulator staging
+  __shared__ __align__(8) uint64_t full_bar[STAGES], empty_bar[STAGES], staged_bar[2], drained_bar[2];
+  __shared__ __align__(16) int32_t s_lab[8][HALF_N];   // per epilogue warp: the labels of its 64 columns of the current tile
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int role = warp >> 2;                     // warpgroup: 0 producer, 1-2 MMA, 3-4 epilogue
+  PairHistSched sched;
+
+  if (warp == 0 && lane == 0) { prefetch_tmap(&tm_a_hi); prefetch_tmap(&tm_a_lo); prefetch_tmap(&tm_b_hi); prefetch_tmap(&tm_b_lo); }
+  if (warp == 1 && lane == 0) {
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 8); }
+    for (int h = 0; h < 2; ++h) { mbar_init(&staged_bar[h], 4); mbar_init(&drained_bar[h], 4); }
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  if (role == 0) {
+    // ===================== TMA producer =====================
+    regs_dec<kRegsProducer>();
+    sched.init(hp, BK);
+    if (warp == 0 && lane == 0)
+      tma_produce<BLOCK_N, STAGES, 0, BK>(p, sched, smem, full_bar, empty_bar, 0u, &tm_a_hi, &tm_a_lo, &tm_b_hi, &tm_b_lo, &tm_a_hi, &tm_a_lo);
+  } else if (role <= 2) {
+    // ===================== MMA: wgmma main loop -> staging half =====================
+    regs_inc<kRegsMma>();
+    sched.init(hp, BK);
+    const int h = role - 1;
+    const int wi = warp & 3;
+    float acc[BLOCK_N / 2];
+#pragma unroll
+    for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] = 0.0f;
+    int stage = 0; uint32_t phase = 0, tphase = 0;
+    int mb, nb, kb0, kb1;
+    while (sched.next(mb, nb, kb0, kb1)) {
+      mma_work_item<BLOCK_N, STAGES, 0, 0, BK>(acc, p, smem, full_bar, empty_bar, h, lane, 0u, stage, phase, kb0, kb1);
+      mbar_wait(&drained_bar[h], tphase ^ 1);   // the epilogue is done with the previous tile's rows
+      const int r0 = h * 64 + wi * 16 + (lane >> 2), c0 = 2 * (lane & 3);
+#pragma unroll
+      for (int j = 0; j < BLOCK_N / 8; ++j) {
+        *reinterpret_cast<float2*>(&stg[r0 * SROW + 8 * j + c0]) = make_float2(acc[4 * j], acc[4 * j + 1]);
+        *reinterpret_cast<float2*>(&stg[(r0 + 8) * SROW + 8 * j + c0]) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+      }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&staged_bar[h]);
+      tphase ^= 1;
+    }
+  } else {
+    // ===================== epilogue: bin the lower-triangle pairs of one (row, column half) =====================
+    regs_inc<kRegsEpilogue>();
+    sched.init(hp, BK);
+    const int h = role - 3;                  // staging half: rows [64 h, 64 h + 64)
+    const int ew = warp - 12;                // epilogue warp 0..7 (its label buffer)
+    const int wi = warp & 3;
+    const int quarter = h * 2 + (wi & 1);    // 32-row quarter of the tile this warp handles
+    const int half = wi >> 1;                // which column half of the tile
+    const int row_in_tile = quarter * 32 + lane;
+    const float* srow = stg + row_in_tile * SROW + half * HALF_N;
+    const float range = hp.range, scale = hp.scale;
+    const uint32_t bins = hp.bins;
+    uint32_t tphase = 0;
+    int mb, nb, kb0, kb1;
+    while (sched.next(mb, nb, kb0, kb1)) {
+      const int i = mb * BLOCK_M + row_in_tile;
+      const int n0 = nb * BLOCK_N + half * HALF_N;
+      {
+        const int j0 = n0 + lane, j1 = n0 + 32 + lane;
+        s_lab[ew][lane] = j0 < p.N ? hp.labels[j0] : -1;
+        s_lab[ew][lane + 32] = j1 < p.N ? hp.labels[j1] : -1;
+      }
+      const int li = i < p.N ? hp.labels[i] : -1;
+      const int c_end = li < 0 ? 0 : min(HALF_N, i - n0);   // columns j < i only (j < i < N)
+      __syncwarp();
+      double sum_rel = 0.0, sum_unrel = 0.0;
+      uint32_t run_key = 0, run_n = 0;
+      auto offer = [&](float s, int lj, bool in) {
+        if (!in || lj < 0) return;
+        const bool rel = (lj == li);
+        const uint32_t key = (rel ? 0u : bins) + pair_bin(s, range, scale, bins);
+        if (rel) sum_rel += (double)s; else sum_unrel += (double)s;
+        if (key != run_key && run_n) { red_add_u64(hp.hist + run_key, run_n); run_n = 0; }
+        run_key = key;
+        ++run_n;
+      };
+      mbar_wait(&staged_bar[h], tphase);
+#pragma unroll 1
+      for (int c = 0; c < c_end; c += 4) {   // 16-byte row reads: conflict-free with the SROW padding
+        const float4 v = *reinterpret_cast<const float4*>(srow + c);
+        const int4 l = *reinterpret_cast<const int4*>(&s_lab[ew][c]);
+        offer(v.x, l.x, true);
+        offer(v.y, l.y, c + 1 < c_end);
+        offer(v.z, l.z, c + 2 < c_end);
+        offer(v.w, l.w, c + 3 < c_end);
+      }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&drained_bar[h]);   // this warp's staging rows (and its label buffer) may be overwritten
+      tphase ^= 1;
+      if (run_n) red_add_u64(hp.hist + run_key, run_n);
+      sum_rel = warp_sum(sum_rel);
+      sum_unrel = warp_sum(sum_unrel);
+      if (lane == 0) {
+        if (sum_rel != 0.0) atomicAdd(hp.sums, sum_rel);
+        if (sum_unrel != 0.0) atomicAdd(hp.sums + 1, sum_unrel);
+      }
+    }
+  }
+}
+
 // tile_ptr[m][t] = number of stored entries of batch row m with column < t * half_n (t = 0 .. n_half_tiles): where each
 // half tile of the fused decode epilogue starts in the (sorted) clean CSR row.  One thread per (row, t).
 __global__ void decode_tile_ptr_kernel(const int64_t* __restrict__ indptr, const int32_t* __restrict__ indices,
@@ -1219,6 +1383,24 @@ static int launch_topk(const Operand& A, const Operand& B, const TopkParams& tp,
   return DAE_OK;
 }
 
+// related / unrelated pair histogram: X [N x K] K-major as both operands; one persistent CTA per SM over the lower-triangle tiles
+static int launch_pair_hist(const Operand& X, const PairHistParams& hp, cudaStream_t st) {
+  CUtensorMap ta_hi, ta_lo, tb_hi, tb_lo;
+  int rc;
+  const GemmParams& p = hp.g;
+  if ((rc = make_map(&ta_hi, X.hi, p.K, p.M, X.ld, BLOCK_M, kTopkBK))) return rc;
+  if ((rc = make_map(&ta_lo, X.lo, p.K, p.M, X.ld, BLOCK_M, kTopkBK))) return rc;
+  if ((rc = make_map(&tb_hi, X.hi, p.K, p.N, X.ld, kDecodeN, kTopkBK))) return rc;
+  if ((rc = make_map(&tb_lo, X.lo, p.K, p.N, X.ld, kDecodeN, kTopkBK))) return rc;
+  constexpr int smem = kTopkStages * (2 * BLOCK_M * kTopkBK * 2 + 2 * kDecodeN * kTopkBK * 2) + BLOCK_M * (kDecodeN + 4) * 4 + 1024;
+  static bool attr_done[64] = {false};
+  if ((rc = ensure_smem_attr(pair_hist_kernel, smem, attr_done))) return rc;
+  const long long tm = (p.M + BLOCK_M - 1) / BLOCK_M, tiles = tm * (tm + 1) / 2;
+  const int n = tiles < sm_count() ? (int)tiles : sm_count();
+  pair_hist_kernel<<<n, kDecodeThreads, smem, st>>>(ta_hi, ta_lo, tb_hi, tb_lo, hp);
+  return DAE_OK;
+}
+
 // column splits of dae_similarity_topk_bf16x3: `requested` (> 0), or the fewest that give every SM a work item while each split
 // still sweeps kTopkMinTiles column tiles; always within [1, min(column tiles, kTopkMaxSplits)]
 static int topk_splits(int n_query, int n_corpus, int requested) {
@@ -1430,5 +1612,28 @@ extern "C" int dae_similarity_topk_bf16x3(int32_t n_query, int32_t n_corpus, int
   DAE_CHECK_LAUNCH("dae_similarity_topk_bf16x3");
   topk_merge_kernel<<<(n_query + 7) / 8, 256, 0, st>>>(tp.ws_val, tp.ws_idx, n_query, 2 * s, k, idx_out, val_out);
   DAE_CHECK_LAUNCH("dae_similarity_topk_bf16x3 (merge)");
+  return DAE_OK;
+}
+
+extern "C" int dae_similarity_pair_hist_bf16x3(int32_t n, int32_t dim, const void* x_hi, const void* x_lo, int64_t ldx,
+                                               const int32_t* labels, float range, int32_t bins, uint64_t* hist, double* sums,
+                                               void* stream) {
+  DAE_REQUIRE(x_hi && x_lo && labels && hist && sums, "dae_similarity_pair_hist_bf16x3: null pointer");
+  DAE_REQUIRE(n >= 2 && dim > 0, "dae_similarity_pair_hist_bf16x3: bad sizes (n = %d >= 2 rows and dim = %d > 0 needed)", n, dim);
+  DAE_REQUIRE(hist_bins_ok(bins), "dae_similarity_pair_hist_bf16x3: bins = %d is not a power of two in [2^%d, 2^%d]", bins,
+              kHistMinLog2Bins, kHistMaxLog2Bins);
+  DAE_REQUIRE(hist_range_ok(range), "dae_similarity_pair_hist_bf16x3: range M = %g is not a power of two in [2^-64, 2^64]", (double)range);
+  DAE_REQUIRE(ldx >= dim && ldx % 8 == 0,
+              "dae_similarity_pair_hist_bf16x3: the leading dimension must cover dim and be a multiple of 8 (TMA 16-byte strides)");
+  DAE_REQUIRE(((uintptr_t)x_hi | (uintptr_t)x_lo) % 16 == 0 && ((uintptr_t)hist | (uintptr_t)sums) % 8 == 0 && (uintptr_t)labels % 4 == 0,
+              "dae_similarity_pair_hist_bf16x3: operands must be 16-byte, hist and sums 8-byte, labels 4-byte aligned");
+  PairHistParams hp{};
+  hp.g.M = n; hp.g.N = n; hp.g.K = dim; hp.g.k_splits = 1; hp.g.alpha = 1.0f; hp.g.special_col = -1;
+  hp.labels = labels; hp.range = range; hp.scale = (float)bins / (2.0f * range); hp.bins = (uint32_t)bins;
+  hp.hist = reinterpret_cast<unsigned long long*>(hist); hp.sums = sums;
+  Operand X{x_hi, x_lo, ldx, 0};
+  int rc = launch_pair_hist(X, hp, (cudaStream_t)stream);
+  if (rc) return rc;
+  DAE_CHECK_LAUNCH("dae_similarity_pair_hist_bf16x3");
   return DAE_OK;
 }

@@ -15,7 +15,10 @@
 //   splits   : with too few queries to fill the SMs the ranges are cut into `splits` groups, one warp each, and topk_merge_kernel
 //              merges the partial lists.  The extra memory is the buckets ((Nc / kSpW + 1) F int32), the postings (8 B per corpus
 //              entry) and, with splits > 1, the partial lists (8 B per entry): never Nq x Nc or Nq x F.
+//   histogram: sp_topk_kernel<true> (dae_csr_similarity_pair_hist) bins the same scores of the strict lower triangle of Q.Q^T into
+//              related / unrelated histograms instead of k-best lists.
 #include "common.cuh"
+#include "pair_hist.cuh"
 #include "topk.cuh"
 
 namespace dae {
@@ -144,6 +147,12 @@ struct SpParams {
   int64_t diag_offset;
   int32_t* idx_out; float* val_out;   // splits == 1: the result
   float* ws_val; int32_t* ws_idx;     // splits > 1: [n_query x splits x k] partial lists
+  // histogram mode (Q = C): labels [n_corpus] (-1 = none), grid M / bins / (2M) / bins, hist [2 x bins], sums [2]
+  const int32_t* labels;
+  float range, scale;
+  uint32_t bins;
+  unsigned long long* hist;
+  double* sums;
 };
 
 // offer (v, col) to the warp's list (lane j < k holds entry j); warp-uniform arguments
@@ -157,6 +166,12 @@ __device__ __forceinline__ void sp_offer(float v, int col, int n_corpus, int exc
   thr = __shfl_sync(kFull, lv, k - 1);
 }
 
+// HIST = false: k-best lists (dae_csr_similarity_topk).  HIST = true: the related / unrelated pair histogram of Q against itself
+// (dae_csr_similarity_pair_hist): the same postings, accumulation and scores, but only the ranges that start below q are
+// accumulated and only slots c < q are counted -- the strict lower triangle.  The scan bins every non-zero slot (runs of equal
+// (group, bin) in one red.global.add.u64); the zero slots, most of them, are only counted per group in registers and added with
+// one atomic per group when the warp is done.
+template <bool HIST>
 __global__ void __launch_bounds__(kSpWarps * 32, 3) sp_topk_kernel(const SpParams p) {
   extern __shared__ float4 sp_smem4[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -165,7 +180,16 @@ __global__ void __launch_bounds__(kSpWarps * 32, 3) sp_topk_kernel(const SpParam
   float4* slab4 = sp_smem4 + warp * (kSpW / 4);
   float* slab = reinterpret_cast<float*>(slab4);
   const int q = (int)(item / p.splits), split = (int)(item - (int64_t)q * p.splits);
-  const int r0 = (int)((int64_t)split * p.ranges / p.splits), r1 = (int)((int64_t)(split + 1) * p.ranges / p.splits);
+  const int r0 = (int)((int64_t)split * p.ranges / p.splits);
+  int r1 = (int)((int64_t)(split + 1) * p.ranges / p.splits);
+  int lq = 0;
+  if constexpr (HIST) {
+    lq = p.labels[q];
+    if (lq < 0) return;                                 // warp-uniform: a row without a label has no pairs
+    r1 = min(r1, (q + kSpW - 1) / kSpW);                // ranges that start below q
+  }
+  double sum_rel = 0.0, sum_unrel = 0.0;
+  uint32_t zero_rel = 0, zero_unrel = 0, run_key = 0, run_n = 0;
   const int64_t qb = p.q_indptr[q], qe = p.q_indptr[q + 1];
   const int64_t e = (int64_t)q + p.diag_offset;
   const int excl = (p.exclude && e >= 0 && e < p.n_corpus) ? (int)e : -1;
@@ -197,26 +221,63 @@ __global__ void __launch_bounds__(kSpWarps * 32, 3) sp_topk_kernel(const SpParam
         __syncwarp();                     // a slot's next term (next column) may come from another lane
       }
     }
-    // scan the slab in increasing corpus index (lane-major float4s), offer what beats the k-th score, zero it for the next range
     const int base = r * kSpW;
     const int width = p.n_corpus - base < kSpW ? p.n_corpus - base : kSpW;
-    for (int j0 = 0; j0 < width; j0 += 128) {
-      const float4 x = slab4[j0 / 4 + lane];
-      slab4[j0 / 4 + lane] = make_float4(0.f, 0.f, 0.f, 0.f);
-      unsigned mask = __ballot_sync(kFull, fmaxf(fmaxf(x.x, x.y), fmaxf(x.z, x.w)) > thr);
-      while (mask) {
-        const int l = __ffs(mask) - 1;
-        mask &= mask - 1;
-        const float y0 = __shfl_sync(kFull, x.x, l), y1 = __shfl_sync(kFull, x.y, l);
-        const float y2 = __shfl_sync(kFull, x.z, l), y3 = __shfl_sync(kFull, x.w, l);
-        const int c = base + j0 + 4 * l;
-        sp_offer(y0, c, p.n_corpus, excl, k, lane, lv, li, thr);
-        sp_offer(y1, c + 1, p.n_corpus, excl, k, lane, lv, li, thr);
-        sp_offer(y2, c + 2, p.n_corpus, excl, k, lane, lv, li, thr);
-        sp_offer(y3, c + 3, p.n_corpus, excl, k, lane, lv, li, thr);
+    if constexpr (HIST) {
+      // bin the slots c < q, zero the whole slab for the next range
+      auto count = [&](float s, int c) {
+        if (c >= q) return;
+        const int lc = p.labels[c];
+        if (lc < 0) return;
+        const bool rel = (lc == lq);
+        if (s == 0.0f) { zero_rel += rel; zero_unrel += !rel; return; }
+        const uint32_t key = (rel ? 0u : p.bins) + pair_bin(s, p.range, p.scale, p.bins);
+        if (rel) sum_rel += (double)s; else sum_unrel += (double)s;
+        if (key != run_key && run_n) { red_add_u64(p.hist + run_key, run_n); run_n = 0; }
+        run_key = key;
+        ++run_n;
+      };
+      for (int j0 = 0; j0 < width; j0 += 128) {
+        const float4 x = slab4[j0 / 4 + lane];
+        slab4[j0 / 4 + lane] = make_float4(0.f, 0.f, 0.f, 0.f);
+        const int c = base + j0 + 4 * lane;
+        count(x.x, c); count(x.y, c + 1); count(x.z, c + 2); count(x.w, c + 3);
+      }
+    } else {
+      // scan the slab in increasing corpus index (lane-major float4s), offer what beats the k-th score, zero it for the next range
+      for (int j0 = 0; j0 < width; j0 += 128) {
+        const float4 x = slab4[j0 / 4 + lane];
+        slab4[j0 / 4 + lane] = make_float4(0.f, 0.f, 0.f, 0.f);
+        unsigned mask = __ballot_sync(kFull, fmaxf(fmaxf(x.x, x.y), fmaxf(x.z, x.w)) > thr);
+        while (mask) {
+          const int l = __ffs(mask) - 1;
+          mask &= mask - 1;
+          const float y0 = __shfl_sync(kFull, x.x, l), y1 = __shfl_sync(kFull, x.y, l);
+          const float y2 = __shfl_sync(kFull, x.z, l), y3 = __shfl_sync(kFull, x.w, l);
+          const int c = base + j0 + 4 * l;
+          sp_offer(y0, c, p.n_corpus, excl, k, lane, lv, li, thr);
+          sp_offer(y1, c + 1, p.n_corpus, excl, k, lane, lv, li, thr);
+          sp_offer(y2, c + 2, p.n_corpus, excl, k, lane, lv, li, thr);
+          sp_offer(y3, c + 3, p.n_corpus, excl, k, lane, lv, li, thr);
+        }
       }
     }
     __syncwarp();
+  }
+  if constexpr (HIST) {
+    if (run_n) red_add_u64(p.hist + run_key, run_n);
+    zero_rel = __reduce_add_sync(kFull, zero_rel);
+    zero_unrel = __reduce_add_sync(kFull, zero_unrel);
+    sum_rel = warp_sum(sum_rel);
+    sum_unrel = warp_sum(sum_unrel);
+    if (lane == 0) {
+      const uint32_t zb = pair_bin(0.0f, p.range, p.scale, p.bins);
+      if (zero_rel) red_add_u64(p.hist + zb, zero_rel);
+      if (zero_unrel) red_add_u64(p.hist + p.bins + zb, zero_unrel);
+      if (sum_rel != 0.0) atomicAdd(p.sums, sum_rel);
+      if (sum_unrel != 0.0) atomicAdd(p.sums + 1, sum_unrel);
+    }
+    return;
   }
   if (lane < k) {
     if (p.splits == 1) {
@@ -231,6 +292,43 @@ __global__ void __launch_bounds__(kSpWarps * 32, 3) sp_topk_kernel(const SpParam
 }
 
 }  // namespace
+
+// corpus postings bucketed by (range, column) into the workspace (layout L)
+static int sp_postings(const SpLayout& L, const int64_t* c_indptr, const int32_t* c_indices, const float* c_values, int n_corpus,
+                       int F, uint8_t* ws, cudaStream_t st) {
+  int32_t* bucket = reinterpret_cast<int32_t*>(ws);
+  int32_t* tiles = reinterpret_cast<int32_t*>(ws + L.off_tiles);
+  int2* post = reinterpret_cast<int2*>(ws + L.off_post);
+  DAE_CUDA(cudaMemsetAsync(bucket, 0, (size_t)L.n_bucket * 4, st));
+  const int row_blocks = (int)((n_corpus + 7) / 8 < sm_count() * 16 ? (n_corpus + 7) / 8 : sm_count() * 16);
+  sp_count_kernel<<<row_blocks, 256, 0, st>>>(c_indptr, c_indices, n_corpus, F, bucket);
+  sp_scan_tiles_kernel<<<(unsigned)L.n_tiles, kScanThreads, 0, st>>>(bucket, L.n_bucket, kScanTile, tiles);
+  if (L.n_tiles > 1) {
+    sp_scan_tiles_kernel<<<1, kScanThreads, 0, st>>>(tiles, L.n_tiles, L.n_tiles, nullptr);
+    const int64_t rest = L.n_bucket - kScanTile;
+    const int blocks = (int)((rest + 255) / 256 < sm_count() * 16 ? (rest + 255) / 256 : sm_count() * 16);
+    sp_add_tile_offsets_kernel<<<blocks, 256, 0, st>>>(bucket, L.n_bucket, kScanTile, tiles);
+  }
+  sp_scatter_kernel<<<row_blocks, 256, 0, st>>>(c_indptr, c_indices, c_values, n_corpus, F, bucket, post);
+  DAE_CHECK_LAUNCH("sparse similarity (postings)");
+  return DAE_OK;
+}
+
+template <bool HIST>
+static int sp_launch(const SpParams& sp, cudaStream_t st) {
+  constexpr int smem = kSpWarps * kSpW * 4;
+  static bool attr_done[64] = {false};
+  int dev = 0;
+  DAE_CUDA(cudaGetDevice(&dev));
+  if (dev >= 0 && dev < 64 && !attr_done[dev]) {
+    DAE_CUDA(cudaFuncSetAttribute(sp_topk_kernel<HIST>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    attr_done[dev] = true;
+  }
+  const int64_t warps = (int64_t)sp.n_query * sp.splits;
+  sp_topk_kernel<HIST><<<(unsigned)((warps + kSpWarps - 1) / kSpWarps), kSpWarps * 32, smem, st>>>(sp);
+  return DAE_OK;
+}
+
 }  // namespace dae
 
 using namespace dae;
@@ -262,23 +360,10 @@ extern "C" int dae_csr_similarity_topk(const int64_t* q_indptr, const int32_t* q
   cudaStream_t st = (cudaStream_t)stream;
   uint8_t* ws = reinterpret_cast<uint8_t*>(workspace);
   int32_t* bucket = reinterpret_cast<int32_t*>(ws);
-  int32_t* tiles = reinterpret_cast<int32_t*>(ws + L.off_tiles);
   int2* post = reinterpret_cast<int2*>(ws + L.off_post);
   const int F = c_features;
-
-  // corpus postings bucketed by (range, column)
-  DAE_CUDA(cudaMemsetAsync(bucket, 0, (size_t)L.n_bucket * 4, st));
-  const int row_blocks = (int)((n_corpus + 7) / 8 < sm_count() * 16 ? (n_corpus + 7) / 8 : sm_count() * 16);
-  sp_count_kernel<<<row_blocks, 256, 0, st>>>(c_indptr, c_indices, n_corpus, F, bucket);
-  sp_scan_tiles_kernel<<<(unsigned)L.n_tiles, kScanThreads, 0, st>>>(bucket, L.n_bucket, kScanTile, tiles);
-  if (L.n_tiles > 1) {
-    sp_scan_tiles_kernel<<<1, kScanThreads, 0, st>>>(tiles, L.n_tiles, L.n_tiles, nullptr);
-    const int64_t rest = L.n_bucket - kScanTile;
-    const int blocks = (int)((rest + 255) / 256 < sm_count() * 16 ? (rest + 255) / 256 : sm_count() * 16);
-    sp_add_tile_offsets_kernel<<<blocks, 256, 0, st>>>(bucket, L.n_bucket, kScanTile, tiles);
-  }
-  sp_scatter_kernel<<<row_blocks, 256, 0, st>>>(c_indptr, c_indices, c_values, n_corpus, F, bucket, post);
-  DAE_CHECK_LAUNCH("dae_csr_similarity_topk (postings)");
+  int rc = sp_postings(L, c_indptr, c_indices, c_values, n_corpus, F, ws, st);
+  if (rc) return rc;
 
   SpParams sp{};
   sp.q_indptr = q_indptr; sp.q_indices = q_indices; sp.q_values = q_values; sp.bucket = bucket; sp.post = post;
@@ -287,20 +372,48 @@ extern "C" int dae_csr_similarity_topk(const int64_t* q_indptr, const int32_t* q
   sp.idx_out = idx_out; sp.val_out = val_out;
   sp.ws_val = reinterpret_cast<float*>(ws + L.off_val);
   sp.ws_idx = reinterpret_cast<int32_t*>(ws + L.off_idx);
-  constexpr int smem = kSpWarps * kSpW * 4;
-  static bool attr_done[64] = {false};
-  int dev = 0;
-  DAE_CUDA(cudaGetDevice(&dev));
-  if (dev >= 0 && dev < 64 && !attr_done[dev]) {
-    DAE_CUDA(cudaFuncSetAttribute(sp_topk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    attr_done[dev] = true;
-  }
-  const int64_t warps = (int64_t)n_query * L.splits;
-  sp_topk_kernel<<<(unsigned)((warps + kSpWarps - 1) / kSpWarps), kSpWarps * 32, smem, st>>>(sp);
+  if ((rc = sp_launch<false>(sp, st))) return rc;
   DAE_CHECK_LAUNCH("dae_csr_similarity_topk");
   if (L.splits > 1) {
     topk_merge_kernel<<<(n_query + 7) / 8, 256, 0, st>>>(sp.ws_val, sp.ws_idx, n_query, L.splits, k, idx_out, val_out);
     DAE_CHECK_LAUNCH("dae_csr_similarity_topk (merge)");
   }
+  return DAE_OK;
+}
+
+extern "C" int dae_csr_similarity_pair_hist_workspace(int32_t n, int64_t nnz, int32_t n_features, int64_t* bytes) {
+  DAE_REQUIRE(bytes && n >= 2 && n_features > 0 && nnz >= 0 && nnz < INT32_MAX, "dae_csr_similarity_pair_hist_workspace: bad arguments");
+  *bytes = sp_layout(n, n, nnz, n_features, 0, 0).total;
+  return DAE_OK;
+}
+
+extern "C" int dae_csr_similarity_pair_hist(const int64_t* indptr, const int32_t* indices, const float* values, int32_t n, int64_t nnz,
+                                            int32_t n_features, const int32_t* labels, float range, int32_t bins, void* workspace,
+                                            int64_t workspace_bytes, uint64_t* hist, double* sums, void* stream) {
+  DAE_REQUIRE(indptr && labels && workspace && hist && sums && (nnz == 0 || (indices && values)),
+              "dae_csr_similarity_pair_hist: null pointer");
+  DAE_REQUIRE(n >= 2 && n_features > 0 && nnz >= 0 && nnz < INT32_MAX,
+              "dae_csr_similarity_pair_hist: bad sizes (n = %d >= 2 rows, features > 0 and 0 <= nnz < 2^31 needed)", n);
+  DAE_REQUIRE(hist_bins_ok(bins), "dae_csr_similarity_pair_hist: bins = %d is not a power of two in [2^%d, 2^%d]", bins,
+              kHistMinLog2Bins, kHistMaxLog2Bins);
+  DAE_REQUIRE(hist_range_ok(range), "dae_csr_similarity_pair_hist: range M = %g is not a power of two in [2^-64, 2^64]", (double)range);
+  DAE_REQUIRE((uintptr_t)workspace % 16 == 0 && ((uintptr_t)hist | (uintptr_t)sums) % 8 == 0,
+              "dae_csr_similarity_pair_hist: workspace must be 16-byte, hist and sums 8-byte aligned");
+  const SpLayout L = sp_layout(n, n, nnz, n_features, 0, 0);
+  DAE_REQUIRE(workspace_bytes >= L.total,
+              "dae_csr_similarity_pair_hist: workspace of %lld bytes, %lld needed (dae_csr_similarity_pair_hist_workspace)",
+              (long long)workspace_bytes, (long long)L.total);
+  cudaStream_t st = (cudaStream_t)stream;
+  uint8_t* ws = reinterpret_cast<uint8_t*>(workspace);
+  int rc = sp_postings(L, indptr, indices, values, n, n_features, ws, st);
+  if (rc) return rc;
+  SpParams sp{};
+  sp.q_indptr = indptr; sp.q_indices = indices; sp.q_values = values;
+  sp.bucket = reinterpret_cast<int32_t*>(ws); sp.post = reinterpret_cast<int2*>(ws + L.off_post);
+  sp.n_query = n; sp.n_corpus = n; sp.F = n_features; sp.k = 1; sp.splits = L.splits; sp.ranges = L.ranges; sp.exclude = 0;
+  sp.labels = labels; sp.range = range; sp.scale = (float)bins / (2.0f * range); sp.bins = (uint32_t)bins;
+  sp.hist = reinterpret_cast<unsigned long long*>(hist); sp.sums = sums;
+  if ((rc = sp_launch<true>(sp, st))) return rc;
+  DAE_CHECK_LAUNCH("dae_csr_similarity_pair_hist");
   return DAE_OK;
 }

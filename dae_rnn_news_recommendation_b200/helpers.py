@@ -7,12 +7,16 @@ nearest-article lookup of main_autoencoder.py:307-318,352-359) -- SURVEY section
                                                                                                         dense or scipy sparse inputs)
     label_precision_at_k(index, query_labels, corpus_labels) -> float                                 (share of same-label neighbours)
     visualize_pairwise_similarity(labels, pairwise_similarity_metrics, ...) -> dict                   (rank 2: AUROC + box statistics)
+    similarity_auroc(data, labels, metric='cosine', bins=1 << 21) -> dict                              (the same numbers on a score
+                                                                                                        grid, without the matrix)
+    auroc_from_histograms(hist, sums, M, bins) -> dict                                                 (its host half, pure NumPy)
 
 Dense inputs (embeddings) go through the wgmma bf16x3 GEMM on row-normalised operands; sparse inputs (count / tf-idf
 matrices) through the CSR encode kernel against the dense transpose, except in top_k_similar, where they go through the
 sparse CSR x CSR top-k kernel (dae_csr_similarity_topk).  No CPU path.
 """
 import ctypes
+import math
 
 import numpy as np
 import scipy.sparse as sp
@@ -321,3 +325,142 @@ def visualize_pairwise_similarity(labels, pairwise_similarity_metrics, plot='box
         with open(os.path.splitext(save_path)[0] + '.json', 'w') as f:
             json.dump(out, f, indent=1)
     return out
+
+
+HIST_MIN_BINS, HIST_MAX_BINS = 1 << 10, 1 << 24
+
+
+def _check_bins(bins):
+    if not isinstance(bins, (int, np.integer)) or not HIST_MIN_BINS <= bins <= HIST_MAX_BINS or bins & (bins - 1):
+        raise ValueError('bins = %r is not a power of two in [2^10, 2^24]' % (bins,))
+
+
+def grid_range(max_sq_norm, metric):
+    """M of the score grid [-M, M]: 1 for cosine; for the linear kernel the smallest power of two >= (1 - 1e-6) max_i ||x_i||^2,
+    which bounds |x_i . x_j| (l2-normalised tf-idf rows get M = 1; 1 as well when every row is zero)."""
+    if metric == 'cosine':
+        return 1.0
+    v = (1.0 - 1e-6) * float(max_sq_norm)
+    if not v > 0.0:
+        return 1.0
+    m, e = math.frexp(v)
+    return math.ldexp(1.0, e - 1 if m == 0.5 else e)
+
+
+def score_bins(scores, M, bins):
+    """The bin of every float32 score, as the pair-histogram kernels compute it: clamp(floor(fl32(s + M) * bins / (2M)), 0, bins - 1).
+    bins / (2M) is a power of two, so the product is exact and the float32 add is the only rounding; NaN goes to bin 0."""
+    with np.errstate(over='ignore', invalid='ignore'):   # +-inf scores clamp into the end bins
+        u = (np.asarray(scores, dtype=np.float32) + np.float32(M)) * np.float32(bins / (2.0 * M))
+    return np.clip(np.floor(np.where(np.isnan(u), np.float32(0), u)), 0, bins - 1).astype(np.int64)
+
+
+def _hist_box_stats(counts, total, centres):
+    """_box_stats of a group known only by its bin counts: every datum is taken as the centre of its bin."""
+    n = int(counts.sum())
+    if n == 0:
+        return {'n': 0}
+    cum = np.cumsum(counts)
+
+    def at(k):
+        return float(centres[int(np.searchsorted(cum, k, side='right'))])
+
+    def pct(q):
+        pos = q * (n - 1)
+        i0 = int(np.floor(pos))
+        i1 = min(i0 + 1, n - 1)
+        a, b = at(i0), at(i1)
+        return a + (b - a) * (pos - i0)
+    q1, med, q3 = pct(0.25), pct(0.5), pct(0.75)
+    iqr = q3 - q1
+    occupied = centres[counts > 0]
+    lo = occupied[occupied >= q1 - 1.5 * iqr]
+    hi = occupied[occupied <= q3 + 1.5 * iqr]
+    return {'q1': q1, 'median': med, 'q3': q3, 'whisker_lo': float(lo.min()) if len(lo) else q1,
+            'whisker_hi': float(hi.max()) if len(hi) else q3, 'mean': float(total) / n, 'n': n}
+
+
+def auroc_from_histograms(hist, sums, M, bins):
+    """Host half of similarity_auroc: the related-vs-unrelated AUROC and box statistics from the pair histograms hist [2, bins]
+    (row 0 related, row 1 unrelated) and the fp64 score sums [2] of the grid [-M, M].
+      twice_u = sum_b n_r[b] (2 sum_{b' < b} n_u[b'] + n_u[b])  -- exact, in Python integers; auroc = twice_u / (2 R U)
+      auroc_error_bound = sum_b n_r[b] n_u[b] / (2 R U): the exact AUROC of the same scores lies within it (the bin map is monotone,
+      so only pairs that share a bin can be ordered differently, and the grid counts each of those as one half).
+    Order statistics are the centres of their bins (quartiles interpolated as np.percentile does, Tukey whiskers on those values),
+    the mean comes from the sums.  No related or no unrelated pair: auroc and the bound are NaN, as in the sort path."""
+    _check_bins(bins)
+    if not M > 0:
+        raise ValueError('M = %r must be positive' % (M,))
+    hist = np.asarray(hist).astype(np.int64)
+    if hist.shape != (2, bins):
+        raise ValueError('hist has shape %s, (2, %d) expected' % (hist.shape, bins))
+    sums = np.asarray(sums, dtype=np.float64).reshape(2)
+    w = 2.0 * M / bins
+    centres = -M + (np.arange(bins, dtype=np.float64) + 0.5) * w
+    nr, nu = hist[0], hist[1]
+    r, u = int(nr.sum()), int(nu.sum())
+    if r == 0 or u == 0:
+        auroc, twice, bound = float('nan'), 0, float('nan')
+    else:
+        occ = np.nonzero(nr)[0]
+        below = (np.cumsum(nu) - nu)[occ]
+        a = nr[occ].astype(object)
+        twice = int((a * (2 * below + nu[occ]).astype(object)).sum())   # products reach ~1e23 at 10^6 rows: Python integers
+        ties = int((a * nu[occ].astype(object)).sum())
+        auroc, bound = twice / (2.0 * r * u), ties / (2.0 * r * u)
+    return {'auroc': auroc, 'twice_u': twice, 'auroc_error_bound': bound, 'bin_width': w,
+            'related': _hist_box_stats(nr, sums[0], centres), 'unrelated': _hist_box_stats(nu, sums[1], centres)}
+
+
+def _max_sq_norm_dense(x, chunk=1 << 16):
+    return max(float(x[i:i + chunk].double().pow(2).sum(1).max()) for i in range(0, x.shape[0], chunk))
+
+
+def similarity_auroc(data, labels, metric='cosine', bins=1 << 21, title=None, save_path=None, device='cuda:0'):
+    """The numbers of visualize_pairwise_similarity (related-vs-unrelated AUROC and box statistics of the strict lower triangle,
+    rows labelled -1 dropped) at any number of rows, without the similarity matrix: the scores are counted into `bins` bins over
+    [-M, M] (grid_range) on the GPU and evaluated by auroc_from_histograms.  Dense arrays or tensors run on the tensor cores
+    (dae_similarity_pair_hist_bf16x3, bf16x3 scores as top_k_similar); scipy sparse matrices through dae_csr_similarity_pair_hist
+    (the fp32 scores of the sparse top_k_similar).  metric: 'cosine' or 'linear kernel'.  Memory beyond the inputs is O(bins) plus
+    the operands (dense) or the postings (sparse), never N x N.
+    Returns {title, auroc, twice_u, auroc_error_bound, bin_width, related, unrelated}; the exact AUROC of the same scores (the
+    sort path) lies within auroc_error_bound of auroc.  Written as JSON next to `save_path` when one is given."""
+    hist, sums, M = _pair_histograms(data, labels, metric, bins, device)
+    out = {'title': title, **auroc_from_histograms(hist.cpu().numpy(), sums.cpu().numpy(), M, bins)}
+    if save_path is not None:
+        import json
+        import os
+        with open(os.path.splitext(save_path)[0] + '.json', 'w') as f:
+            json.dump(out, f, indent=1)
+    return out
+
+
+def _pair_histograms(data, labels, metric, bins, device='cuda:0'):
+    """Device half of similarity_auroc: (hist int64 [2, bins], sums float64 [2]) device tensors and the grid's M."""
+    if metric not in ('cosine', 'linear kernel'):
+        raise ValueError("metric = %r: 'cosine' or 'linear kernel'" % (metric,))
+    _check_bins(bins)
+    labels = np.asarray(labels.values if hasattr(labels, 'values') else labels).reshape(-1)
+    n = data.shape[0]
+    if labels.shape[0] != n:
+        raise ValueError('similarity_auroc: %d labels for %d rows' % (labels.shape[0], n))
+    lab_i = np.where(labels >= 0, np.unique(labels, return_inverse=True)[1].reshape(-1), -1).astype(np.int32)
+    lab_dev = torch.from_numpy(lab_i).to(device)
+    hist = torch.zeros(2, bins, dtype=torch.int64, device=device)      # uint64 counts in the kernels
+    sums = torch.zeros(2, dtype=torch.float64, device=device)
+    if sp.issparse(data):
+        m = _csr_operand(data, metric)
+        M = grid_range(float(np.asarray(m.multiply(m).sum(1), dtype=np.float64).max()) if metric != 'cosine' else 1.0, metric)
+        d = DeviceCSR(m, device)
+        need = (ctypes.c_int64 * 1)()
+        call('dae_csr_similarity_pair_hist_workspace', n, d.nnz, m.shape[1], ctypes.addressof(need))
+        ws = torch.empty(max(int(need[0]), 16), dtype=torch.uint8, device=device)
+        call('dae_csr_similarity_pair_hist', d.indptr.data_ptr(), d.indices.data_ptr(), d.values.data_ptr(), n, d.nnz, m.shape[1],
+             lab_dev.data_ptr(), M, bins, ws.data_ptr(), ws.numel(), hist.data_ptr(), sums.data_ptr(), _stream())
+    else:
+        x = _as_device_dense(data, device)
+        M = grid_range(_max_sq_norm_dense(x) if metric != 'cosine' else 1.0, metric)
+        hi, lo, ld = _normalised_operands(x, 2 if metric == 'cosine' else 0)
+        call('dae_similarity_pair_hist_bf16x3', n, x.shape[1], hi.data_ptr(), lo.data_ptr(), ld, lab_dev.data_ptr(), M, bins,
+             hist.data_ptr(), sums.data_ptr(), _stream())
+    return hist, sums, M

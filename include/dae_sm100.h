@@ -341,6 +341,33 @@ int dae_pair_partition(const float* S, int64_t lds, int32_t n, const int32_t* la
 int dae_auroc_count(const float* queries, int64_t n_queries, const float* sorted_targets, int64_t n_targets,
                     int32_t query_is_positive, uint64_t* twice_u, void* stream);
 
+/* ---- related-vs-unrelated AUROC without the similarity matrix: pair histograms ------------------------------------
+ * The same pairs as dae_pair_partition -- S[i, j] with i > j (i the row / first operand), both labels >= 0; related when the
+ * labels are equal -- of a set against itself, counted on a grid instead of sorted, so that memory stays O(bins) at any n.
+ * Grid: `bins` bins (a power of two, 2^10 .. 2^24) over [-M, M] (`range` = M, a power of two in [2^-64, 2^64]; 1 for cosine, for
+ *   the linear kernel the smallest power of two >= (1 - 1e-6) max_i ||x_i||^2).  A score s goes to bin
+ *   b = clamp(floor(fl32(s + M) * bins / (2M)), 0, bins - 1): bins / (2M) is a power of two, so the only rounding is the fp32
+ *   add and a float32 host expression gives the same bin.  The map is monotone in s; scores outside [-M, M] land in the end bins.
+ * Output, ACCUMULATED into caller-zeroed buffers: hist uint64 [2 x bins] (row 0 related, row 1 unrelated: exact counts, so
+ *   independent of atomic order and launch shape) and sums fp64 [2] (the fp32 scores of each group summed in fp64, for the mean).
+ *   The AUROC on the grid, twice_u = sum_b n_r[b] (2 sum_{b' < b} n_u[b'] + n_u[b]), differs from the exact AUROC of the same
+ *   fp32 scores by at most sum_b n_r[b] n_u[b] / (2 R U); helpers.auroc_from_histograms computes both on the host.
+ * Every argument is checked before any CUDA call; n >= 2.
+ * dae_similarity_pair_hist_bf16x3: S = X.X^T of dense rows (bf16 hi / lo pair [n x ldx], ldx >= dim and a multiple of 8, 16-byte
+ *   aligned, e.g. from dae_rownorm_split_bf16) on the tensor cores, bf16x3 as dae_similarity_topk_bf16x3; only the tiles on and
+ *   below the diagonal are computed and S never leaves the SM.
+ * dae_csr_similarity_pair_hist: S of one CSR matrix (the layout of dae_csr_similarity_topk, nnz < 2^31) with the scores of
+ *   dae_csr_similarity_topk, bit for bit: fp32 from 0, one rounded product per shared column in increasing column order, no FMA.
+ *   workspace: 16-byte aligned, at least dae_csr_similarity_pair_hist_workspace bytes (the postings and their bucket offsets).
+ */
+int dae_similarity_pair_hist_bf16x3(int32_t n, int32_t dim, const void* x_hi, const void* x_lo, int64_t ldx,
+                                    const int32_t* labels, float range, int32_t bins, uint64_t* hist, double* sums,
+                                    void* stream);
+int dae_csr_similarity_pair_hist(const int64_t* indptr, const int32_t* indices, const float* values, int32_t n, int64_t nnz,
+                                 int32_t n_features, const int32_t* labels, float range, int32_t bins, void* workspace,
+                                 int64_t workspace_bytes, uint64_t* hist, double* sums, void* stream);
+int dae_csr_similarity_pair_hist_workspace(int32_t n, int64_t nnz, int32_t n_features, int64_t* bytes);
+
 /* ---- data-parallel exchange step (SURVEY 8e): in-switch all-reduce of the flat gradient buffer -------------------
  * The reference is single-process; row-sharded training adds ONE sum over ranks of [dW | dbh | dbv] between the
  * gradient kernels and dae_optimizer_step.  Default transport: ncclAllReduce.  dae_allreduce_multimem is the

@@ -69,6 +69,9 @@ def build_parser():
     ap.add_argument('--top_k_input', action='store_true', default=False,
                     help='with --top_k K: also rank by the input vectors (cosine for binary, linear kernel for tf-idf), save '
                          'article_top_k_input_{index,score}[_validate].npy and report their label precision next to the embedding\'s')
+    ap.add_argument('--eval_all_rows', action='store_true', default=False,
+                    help='evaluate sets above 20 000 rows instead of skipping them: AUROC and box statistics from score histograms '
+                         '(helpers.similarity_auroc, reported with their error bound) and the nearest article through top_k_similar')
     return ap
 
 
@@ -226,25 +229,38 @@ def prepare_synthetic(F):
 def evaluate(F, model, trX, vlX, trL, vlL, enc, enc_v, max_rows=20000):
     """Reference main_autoencoder.py:307-360: cosine similarity of the input space and of the embeddings, the related / unrelated
     comparison for the label in use, and the nearest article of the first rows.  N x N lives on the GPU only; sets larger than
-    `max_rows` (the reference runs 8000 / 2000 rows) are skipped."""
+    `max_rows` (the reference runs 8000 / 2000 rows) are skipped -- or, with --eval_all_rows, evaluated without the N x N matrix:
+    the same keys and JSON files from helpers.similarity_auroc (AUROC on a score grid, with its error bound) and the nearest
+    article from top_k_similar(k=1)."""
     from dae_rnn_news_recommendation_b200 import helpers
     out = {}
     print('calculate similarity')
     in_metric = 'cosine' if F.input_format == 'binary' else 'linear kernel'   # tf-idf rows are already l2-normalised (:314)
     in_name = 'binary_count' if F.input_format == 'binary' else 'tfidf'
     suffix = '(Category)' if F.label == 'category_publish_name' else '(Story)'
+    all_rows = getattr(F, 'eval_all_rows', False)
     for split, X, E, lab in (('', trX, enc, trL), ('_validate', vlX, enc_v, vlL)):
-        if X is None or X.shape[0] < 2 or X.shape[0] > max_rows:
+        if X is None or X.shape[0] < 2 or (X.shape[0] > max_rows and not all_rows):
             print('similarity%s skipped: %s rows' % (split, None if X is None else X.shape[0]))
             continue
+        large = X.shape[0] > max_rows
         for name, data, metric in ((in_name, X, in_metric), ('encoded', E, 'cosine')):
-            sim = helpers.pairwise_similarity(data, metric=metric, to_host=False)
             key = 'similarity_boxplot_%s%s%s' % (name, split, suffix)
+            if large:
+                out[key] = helpers.similarity_auroc(data, lab, metric=metric, title=key, save_path=model.plot_dir + key + '.png')
+                print('%s: AUROC %.4f (±%.1e)  related median %.4f  unrelated median %.4f' % (
+                    key, out[key]['auroc'], out[key]['auroc_error_bound'], out[key]['related'].get('median', float('nan')),
+                    out[key]['unrelated'].get('median', float('nan'))))
+                continue
+            sim = helpers.pairwise_similarity(data, metric=metric, to_host=False)
             out[key] = helpers.visualize_pairwise_similarity(lab, sim, plot='boxplot', title=key, save_path=model.plot_dir + key + '.png')
             print('%s: AUROC %.4f  related median %.4f  unrelated median %.4f' % (
                 key, out[key]['auroc'], out[key]['related'].get('median', float('nan')), out[key]['unrelated'].get('median', float('nan'))))
             del sim
-        idx, score = helpers.nearest_neighbors(E, metric='cosine')
+        if large:   # nearest_neighbors' 8192 x N block would be 32 GB at 10^6 rows
+            idx, score = (a[:, 0] for a in helpers.top_k_similar(E, k=1, metric='cosine'))
+        else:
+            idx, score = helpers.nearest_neighbors(E, metric='cosine')
         out['nearest' + split] = (idx, score)
         for i in range(min(3, len(idx))):
             print('article %d%s: most similar %d (cosine %.4f)' % (i, split, idx[i], score[i]))
