@@ -17,6 +17,7 @@ OPT = {'gradient_descent': 0, 'ada_grad': 1, 'momentum': 2, 'adam': 3}
 STAT = {'cost': 0, 'ae_loss': 1, 'triplet_loss': 2, 'fraction': 3, 'num': 4, 'sum_w': 5, 'n_valid': 6, 'sum_lw': 7,
         'triplet_sum': 8, 'n_active': 9}
 STAT_SLOTS = 16
+MAX_TRIPLET_BATCH = 32768   # DAE_MAX_TRIPLET_BATCH: largest batch_all / batch_hard batch (S, G and G's bf16 copy: ~13 GB)
 
 
 def act_code(name):
@@ -50,6 +51,7 @@ _SIGNATURES = {
     'dae_decode_loss_bwd': (C.c_int, [p, p, p, p, i32, i32, p, i32, i32, p, p, p, i64, p, p]),
     'dae_colsum': (C.c_int, [p, i32, i32, i64, p, p]),
     'dae_triplet_batch_all': (C.c_int, [p, i64, i32, p, p, p, i64, p, i32, p, p, i64, p]),
+    'dae_triplet_config': (C.c_int, [i32]),
     'dae_gemm_sym_bf16x3': (C.c_int, [i32, i32, f32, p, p, i64, p, p, i64, p, i64, i32, p]),
     'dae_triplet_batch_hard': (C.c_int, [p, i64, i32, p, p, i64, p, p, p]),
     'dae_triplet_explicit': (C.c_int, [p, p, p, i32, i32, i64, f32, p, p, p, p, p]),

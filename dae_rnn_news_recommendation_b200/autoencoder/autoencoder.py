@@ -22,7 +22,7 @@ import torch
 from . import utils
 from .. import _cabi
 from ..engine import TrainEngine, DeviceCSR, canonical_csr
-from .._cabi import STAT, STAT_SLOTS
+from .._cabi import STAT, STAT_SLOTS, MAX_TRIPLET_BATCH
 
 
 class DenoisingAutoencoder(object):
@@ -231,10 +231,13 @@ class DenoisingAutoencoder(object):
         tail = [s0 for s0 in starts if s0 + bs > n]
         use_graph = (os.environ.get('DAE_CUDA_GRAPH', '1') == '1' and self.corr_type != 'salt_and_pepper' and len(full) >= 2)
         perm_buf = torch.zeros(n, dtype=torch.int32, device=eng.device)
-        if self.triplet_strategy != 'none':   # dae_batch_prepare / the mining kernels hold one batch in shared memory
-            assert bs <= 4096, 'triplet strategies need batch_size <= 4096 rows (got %d)' % bs
-            assert validation_set is None or validation_set.shape[0] <= 4096, \
-                'the validation set is fed as ONE batch (autoencoder.py:300-309): at most 4096 rows with a triplet strategy'
+        if self.triplet_strategy != 'none':   # the mining branch keeps S, G and G's bf16 copy: B x B x 12 bytes
+            cap = MAX_TRIPLET_BATCH
+            assert bs <= cap, ('triplet strategies need batch_size <= %d rows (got %d: the B x B similarity / gradient buffers would '
+                               'take %.1f GB)' % (cap, bs, 12.0 * bs * bs / 1e9))
+            nv = 0 if validation_set is None else validation_set.shape[0]
+            assert nv <= cap, ('the validation set is fed as ONE batch (autoencoder.py:300-309): at most %d rows with a triplet '
+                               'strategy (got %d: its B x B buffers would take %.1f GB)' % (cap, nv, 12.0 * nv * nv / 1e9))
         if validation_set is not None:        # size the workspaces once: a larger validation batch must not force a re-capture
             eng._ensure_ws(max(bs, validation_set.shape[0]))
         prefetch = self._host_rng_prefetch(host_csr, n)

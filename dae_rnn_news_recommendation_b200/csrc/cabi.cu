@@ -139,6 +139,116 @@ __global__ void __launch_bounds__(1024) batch_prepare_kernel(
   }
 }
 
+// B > kMaxB (up to DAE_MAX_TRIPLET_BATCH): the same outputs from one CTA that sorts inside the caller's buffers -- labels_out holds
+// the keys, rows_out the row ids.  The network is the bitonic sort whose every compare-exchange puts the smaller (label, row) pair at
+// the lower index (the first step of each merge compares mirrored positions), so the power-of-two padding needs no storage: a
+// virtual +inf at an index >= B never moves.  Partner distances below kMaxB run on aligned kMaxB-element blocks staged in shared
+// memory; only the longer ones (6 stages at B = 32768) go through global memory.  Rows end in ascending (label, row id) order, the
+// order batch_prepare_kernel produces.
+__device__ __forceinline__ bool pair_greater(float ka, int va, float kb, int vb) { return (ka > kb) || (ka == kb && va > vb); }
+
+// one global compare-exchange stage: pair t's lower index a (bit log2(j) clear), partner a + j, or its mirror a ^ (2j - 1) (flip)
+__device__ void prepare_global_stage(float* keys, int32_t* vals, int B, int P, int j, bool flip) {
+  for (int t = threadIdx.x; t < P / 2; t += blockDim.x) {
+    const int a = 2 * t - (t & (j - 1));
+    const int b = flip ? (a ^ (2 * j - 1)) : a + j;
+    if (b < B) {
+      const float ka = keys[a], kb = keys[b];
+      const int va = vals[a], vb = vals[b];
+      if (pair_greater(ka, va, kb, vb)) { keys[a] = kb; keys[b] = ka; vals[a] = vb; vals[b] = va; }
+    }
+  }
+  __syncthreads();
+}
+
+// the stages of merge size k with partner distances j < kMaxB, on each aligned kMaxB block in shared memory (k <= kMaxB: the whole
+// merge, flip step included)
+__device__ void prepare_local_stages(float* keys, int32_t* vals, int B, int k, float* sk, int* sv) {
+  for (int b0 = 0; b0 < B; b0 += kMaxB) {
+    for (int t = threadIdx.x; t < kMaxB; t += blockDim.x) {
+      const bool ok = b0 + t < B;
+      sk[t] = ok ? keys[b0 + t] : __int_as_float(0x7f800000);
+      sv[t] = ok ? vals[b0 + t] : 0x7fffffff;
+    }
+    __syncthreads();
+    // k <= kMaxB: the whole merges of sizes 2 .. k; k > kMaxB: the steps j = kMaxB/2 .. 1 of merge k
+    for (int kk = (k <= kMaxB) ? 2 : k; kk <= k; kk <<= 1) {
+      for (int j = (kk <= kMaxB) ? kk >> 1 : kMaxB >> 1; j > 0; j >>= 1) {
+        const bool flip = (kk <= kMaxB) && j == (kk >> 1);
+        for (int t = threadIdx.x; t < kMaxB / 2; t += blockDim.x) {
+          const int a = 2 * t - (t & (j - 1));
+          const int b = flip ? (a ^ (2 * j - 1)) : a + j;
+          const float ka = sk[a], kb = sk[b];
+          const int va = sv[a], vb = sv[b];
+          if (pair_greater(ka, va, kb, vb)) { sk[a] = kb; sk[b] = ka; sv[a] = vb; sv[b] = va; }
+        }
+        __syncthreads();
+      }
+    }
+    for (int t = threadIdx.x; t < kMaxB && b0 + t < B; t += blockDim.x) { keys[b0 + t] = sk[t]; vals[b0 + t] = sv[t]; }
+    __syncthreads();
+  }
+}
+
+__global__ void __launch_bounds__(1024) batch_prepare_large_kernel(
+    const int32_t* __restrict__ perm, int64_t offset, const int64_t* __restrict__ ctl, int B, const float* __restrict__ labels_all,
+    int strategy, int32_t* rows_out, float* labels_out, int32_t* seg_lo, int32_t* seg_hi, float* __restrict__ weight_out,
+    double* __restrict__ stats, int64_t n_perm) {
+  if (ctl) offset += ctl[0];
+  if (n_perm > 0 && offset + B > n_perm) return;
+  __shared__ float sk[kMaxB];
+  __shared__ int sv[kMaxB];
+  __shared__ double red[32];
+  const int tid = threadIdx.x, nt = blockDim.x;
+  float* keys = labels_out;
+  int32_t* vals = rows_out;
+  for (int i = tid; i < B; i += nt) {
+    const int r = perm ? perm[offset + i] : (int)(offset + i);
+    vals[i] = r;
+    keys[i] = labels_all[r];
+  }
+  __syncthreads();
+  int P = 1;
+  while (P < B) P <<= 1;
+  prepare_local_stages(keys, vals, B, kMaxB, sk, sv);            // every aligned kMaxB block sorted
+  for (int k = 2 * kMaxB; k <= P; k <<= 1) {
+    prepare_global_stage(keys, vals, B, P, k >> 1, true);
+    for (int j = k >> 2; j >= kMaxB; j >>= 1) prepare_global_stage(keys, vals, B, P, j, false);
+    prepare_local_stages(keys, vals, B, k, sk, sv);
+  }
+  // class segments: binary searches in the sorted labels (as batch_prepare_kernel)
+  for (int i = tid; i < B; i += nt) {
+    const float k = keys[i];
+    int a = 0, b = i;
+    while (a < b) { const int m = (a + b) >> 1; if (keys[m] < k) a = m + 1; else b = m; }
+    seg_lo[i] = a;
+    a = i + 1; b = B;
+    while (a < b) { const int m = (a + b) >> 1; if (keys[m] <= k) a = m + 1; else b = m; }
+    seg_hi[i] = a;
+  }
+  __syncthreads();
+  double t_part = 0.0, nv_part = 0.0;
+  for (int i = tid; i < B; i += nt) {
+    const double n = (double)(seg_hi[i] - seg_lo[i]);
+    t_part += n - 1.0;
+    nv_part += (n - 1.0) * ((double)B - n);
+  }
+  const double T = block_sum(t_part, red);
+  const double NV = block_sum(nv_part, red);
+  if (weight_out) {
+    for (int i = tid; i < B; i += nt) {
+      const double n = (double)(seg_hi[i] - seg_lo[i]);
+      weight_out[i] = (strategy == DAE_TRIPLET_BATCH_ALL) ? (float)(2.0 * (n - 1.0) * ((double)B - n) + T - n * (n - 1.0)) : 0.0f;
+    }
+  }
+  if (tid < DAE_STAT_SLOTS) {
+    double v = 0.0;
+    if (tid == DAE_STAT_SUM_W) v = (strategy == DAE_TRIPLET_BATCH_ALL) ? 3.0 * NV : 0.0;
+    if (tid == DAE_STAT_N_VALID) v = (strategy == DAE_TRIPLET_BATCH_ALL) ? NV : 0.0;
+    stats[tid] = v;
+  }
+}
+
 // strategy none: keep the permutation order, w = 1, one segment; any B.
 __global__ void batch_rows_kernel(const int32_t* __restrict__ perm, int64_t offset, const int64_t* __restrict__ ctl, int B,
                                   int32_t* __restrict__ rows_out, float* __restrict__ labels_out, int32_t* __restrict__ seg_lo,
@@ -206,11 +316,18 @@ extern "C" int dae_batch_prepare(const int32_t* perm, int64_t offset, const int6
     DAE_CHECK_LAUNCH("dae_batch_prepare(none)");
     return DAE_OK;
   }
-  DAE_REQUIRE(B <= dae::kMaxB, "dae_batch_prepare: triplet strategies need B <= %d (got %d)", dae::kMaxB, B);
+  DAE_REQUIRE(B <= DAE_MAX_TRIPLET_BATCH, "dae_batch_prepare: triplet strategies need B <= %d rows, the cap of the B x B mining "
+              "buffers (got %d)", DAE_MAX_TRIPLET_BATCH, B);
   DAE_REQUIRE(seg_lo && seg_hi, "dae_batch_prepare: null segment outputs");
   DAE_REQUIRE(strategy == DAE_TRIPLET_NONE || labels_all, "dae_batch_prepare: labels required for triplet strategies");
-  dae::batch_prepare_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(perm, offset, ctl, B, labels_all, strategy, rows_out,
-                                                                 labels_out, seg_lo, seg_hi, weight_out, stats, 0);
+  if (B > dae::kMaxB) {
+    DAE_REQUIRE(labels_out, "dae_batch_prepare: B > %d needs labels_out (the batch is sorted inside it)", dae::kMaxB);
+    dae::batch_prepare_large_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(perm, offset, ctl, B, labels_all, strategy, rows_out,
+                                                                         labels_out, seg_lo, seg_hi, weight_out, stats, 0);
+  } else {
+    dae::batch_prepare_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(perm, offset, ctl, B, labels_all, strategy, rows_out,
+                                                                   labels_out, seg_lo, seg_hi, weight_out, stats, 0);
+  }
   DAE_CHECK_LAUNCH("dae_batch_prepare");
   return DAE_OK;
 }
@@ -218,11 +335,19 @@ extern "C" int dae_batch_prepare(const int32_t* perm, int64_t offset, const int6
 extern "C" int dae_batch_prepare_next(const int32_t* perm, int64_t n_perm, int64_t stride, const int64_t* ctl, int32_t B,
                                       const float* labels_all, int32_t strategy, int32_t* rows_s, float* labels_s, int32_t* seg_lo_s,
                                       int32_t* seg_hi_s, float* weight_s, double* stats_s, void* stream) {
-  DAE_REQUIRE(ctl && n_perm > 0 && B >= 1 && B <= dae::kMaxB && rows_s && seg_lo_s && seg_hi_s && stats_s && labels_all,
+  DAE_REQUIRE(ctl && n_perm > 0 && B >= 1 && rows_s && seg_lo_s && seg_hi_s && stats_s && labels_all,
               "dae_batch_prepare_next: bad arguments");
+  DAE_REQUIRE(B <= DAE_MAX_TRIPLET_BATCH, "dae_batch_prepare_next: triplet strategies need B <= %d rows, the cap of the B x B mining "
+              "buffers (got %d)", DAE_MAX_TRIPLET_BATCH, B);
   DAE_REQUIRE(strategy == DAE_TRIPLET_BATCH_ALL || strategy == DAE_TRIPLET_BATCH_HARD, "dae_batch_prepare_next: triplet strategies only");
-  dae::batch_prepare_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(perm, stride, ctl, B, labels_all, strategy, rows_s, labels_s, seg_lo_s,
-                                                                 seg_hi_s, weight_s, stats_s, n_perm);
+  if (B > dae::kMaxB) {
+    DAE_REQUIRE(labels_s, "dae_batch_prepare_next: B > %d needs labels_s (the batch is sorted inside it)", dae::kMaxB);
+    dae::batch_prepare_large_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(perm, stride, ctl, B, labels_all, strategy, rows_s, labels_s,
+                                                                         seg_lo_s, seg_hi_s, weight_s, stats_s, n_perm);
+  } else {
+    dae::batch_prepare_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(perm, stride, ctl, B, labels_all, strategy, rows_s, labels_s, seg_lo_s,
+                                                                   seg_hi_s, weight_s, stats_s, n_perm);
+  }
   DAE_CHECK_LAUNCH("dae_batch_prepare_next");
   return DAE_OK;
 }

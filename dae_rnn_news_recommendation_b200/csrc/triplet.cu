@@ -277,6 +277,138 @@ __global__ void __launch_bounds__(kTripThreads) triplet_batch_all_kernel(const f
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
+// batch_all above 4096 rows: the same per-anchor sweep with shared memory that does not grow with B.  The anchor's negatives stream
+// through chunks of kChunkK (s, v and the per-warp column-sum slabs), its positives through chunks of kChunkJ (s, u, row sums).  For
+// each negative chunk every positive chunk is swept; the chunk's column sums are then complete and leave as their G entries.  The
+// positives' row sums carry across negative chunks in the CTA's own row of G (one thread per entry, chunks in order: deterministic).
+// The chunk sizes are multiples of the register tiles, so the column sums are accumulated in the same order as in
+// triplet_batch_all_kernel (bit-identical negative entries of G); row sums and the loss differ by fp32 rounding of the chunk partials.
+// The per-thread log accumulator is flushed into fp64 after every (positive, negative) chunk pair.
+// ---------------------------------------------------------------------------------------------------------------------
+constexpr int kChunkJ = 512;    // positives per chunk (16 j-tiles)
+constexpr int kChunkK = 1024;   // negatives per chunk (8 k-tiles)
+static_assert(kChunkJ % kJTile == 0 && kChunkK % kKTile == 0, "chunks must hold whole register tiles");
+
+__global__ void __launch_bounds__(kTripThreads) triplet_batch_all_tiled_kernel(const float* __restrict__ S, int64_t lds, int B,
+                                                                               const int32_t* __restrict__ seg_lo,
+                                                                               const int32_t* __restrict__ seg_hi, float* G, int64_t ldg,
+                                                                               double* __restrict__ stats, int pos_only,
+                                                                               __nv_bfloat16* __restrict__ g_hi,
+                                                                               __nv_bfloat16* __restrict__ g_lo, int64_t ld_split) {
+  __shared__ __align__(16) float sj[kChunkJ];
+  __shared__ __align__(16) float uj[kChunkJ];
+  __shared__ __align__(16) float gj[kChunkJ];
+  __shared__ __align__(16) float sk[kChunkK];
+  __shared__ __align__(16) float vk[kChunkK];
+  __shared__ __align__(16) float gk[kTY * kChunkK];
+  __shared__ float red_f[32];
+  __shared__ double red_d[32];
+  const int i = blockIdx.x;
+  const int tid = threadIdx.x, tx = tid & 31, ty = tid >> 5;
+  const int lo = seg_lo[i], hi = seg_hi[i];
+  const int nj = hi - lo;
+  const int nk = B - nj;
+  const float* srow = S + (int64_t)i * lds;
+  float* grow = G + (int64_t)i * ldg;
+
+  if (nj <= 1 || nk == 0) {
+    for (int c = tid; c < B; c += kTripThreads) {
+      grow[c] = 0.0f;
+      if (g_hi) { g_hi[(int64_t)i * ld_split + c] = __float2bfloat16_rn(0.0f); g_lo[(int64_t)i * ld_split + c] = __float2bfloat16_rn(0.0f); }
+    }
+    return;
+  }
+  // the tier is chosen from the whole row's range
+  float mx = -3.0e38f, mn = 3.0e38f;
+  for (int c = tid; c < B; c += kTripThreads) { const float s = srow[c]; mx = fmaxf(mx, s); mn = fminf(mn, s); }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) { mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o)); mn = fminf(mn, __shfl_xor_sync(0xffffffffu, mn, o)); }
+  if (tx == 0) { red_f[ty] = mx; red_f[8 + ty] = mn; }
+  __syncthreads();
+  mx = red_f[0]; mn = red_f[8];
+#pragma unroll
+  for (int w = 1; w < kTY; ++w) { mx = fmaxf(mx, red_f[w]); mn = fminf(mn, red_f[8 + w]); }
+  const float range = mx - mn;
+  const int tier = pos_only ? 3 : ((range < 10.0f) ? 0 : ((range < 80.0f) ? 1 : 2));
+  const float mid = 0.5f * (mx + mn);
+  const float inv = pos_only ? 1.0f : (float)(1.0 / (stats[DAE_STAT_N_VALID] + 1e-16));
+
+  double lsum = 0.0;   // sum of log2(1 + e^x), fp64 across chunks
+  int npos = 0;
+  for (int k0 = 0; k0 < nk; k0 += kChunkK) {
+    const int ck = min(kChunkK, nk - k0);
+    const int Pk = (ck + kKTile - 1) / kKTile * kKTile;
+    __syncthreads();   // the previous chunk's readers of sk / vk / gk are done
+    for (int q = tid; q < Pk; q += kTripThreads) {
+      const int qq = k0 + q;
+      const int c = (qq < lo) ? qq : qq + nj;
+      const bool ok = q < ck;
+      const float s = ok ? srow[c] : -3.0e38f;
+      sk[q] = s;
+      vk[q] = ok ? fast_ex2((s - mid) * kLog2e) : 0.0f;
+    }
+    for (int e = tid; e < kTY * Pk; e += kTripThreads) gk[(e / Pk) * kChunkK + (e % Pk)] = 0.0f;
+    for (int j0 = 0; j0 < nj; j0 += kChunkJ) {
+      const int cj = min(kChunkJ, nj - j0);
+      const int Pj = (cj + kJTile - 1) / kJTile * kJTile;
+      __syncthreads();   // sj / uj / gj of the previous positive chunk are consumed
+      for (int p = tid; p < Pj; p += kTripThreads) {
+        const int c = lo + j0 + p;
+        const bool ok = (p < cj) && (c != i);
+        const float s = ok ? srow[c] : 3.0e38f;
+        sj[p] = ok ? s + 1e-16f : s;
+        uj[p] = ok ? fast_ex2((mid - s) * kLog2e) : 0.0f;
+        gj[p] = 0.0f;
+      }
+      __syncthreads();
+      float lacc = 0.0f;
+      if (tier == 0) triplet_sweep<0>(sj, uj, gj, sk, vk, gk, Pj, Pk, kChunkK, tx, ty, lacc, npos);
+      else if (tier == 1) triplet_sweep<1>(sj, uj, gj, sk, vk, gk, Pj, Pk, kChunkK, tx, ty, lacc, npos);
+      else if (tier == 2) triplet_sweep<2>(sj, uj, gj, sk, vk, gk, Pj, Pk, kChunkK, tx, ty, lacc, npos);
+      else triplet_sweep<3>(sj, uj, gj, sk, vk, gk, Pj, Pk, kChunkK, tx, ty, lacc, npos);
+      lsum += (double)lacc;
+      __syncthreads();
+      // raw row sums of this chunk pair, carried in G; entry lo + j0 + p is always owned by thread p % kTripThreads
+      for (int p = tid; p < cj; p += kTripThreads) {
+        float* g = grow + lo + j0 + p;
+        *g = (k0 == 0 ? 0.0f : *g) + gj[p];
+      }
+    }
+    __syncthreads();   // the column-sum slabs of this negative chunk are complete
+    for (int q = tid; q < ck; q += kTripThreads) {
+      const int qq = k0 + q;
+      const int c = (qq < lo) ? qq : qq + nj;
+      float t = 0.0f;
+#pragma unroll
+      for (int w = 0; w < kTY; ++w) t += gk[w * kChunkK + q];
+      const float g = t * inv;    // +sum_j sigma(S_ik - S_ij)
+      grow[c] = g;
+      if (g_hi) {
+        const __nv_bfloat16 h = __float2bfloat16_rn(g);
+        g_hi[(int64_t)i * ld_split + c] = h;
+        g_lo[(int64_t)i * ld_split + c] = __float2bfloat16_rn(g - __bfloat162float(h));
+      }
+    }
+  }
+  for (int p = tid; p < nj; p += kTripThreads) {   // same owner thread as the carries above
+    const int c = lo + p;
+    const float g = -grow[c] * inv;    // -sum_k sigma(S_ik - S_ij); the anchor's own slot has u = 0 -> 0
+    grow[c] = g;
+    if (g_hi) {
+      const __nv_bfloat16 h = __float2bfloat16_rn(g);
+      g_hi[(int64_t)i * ld_split + c] = h;
+      g_lo[(int64_t)i * ld_split + c] = __float2bfloat16_rn(g - __bfloat162float(h));
+    }
+  }
+  const double ls = block_sum(lsum * (double)kLn2, red_d);
+  const double ps = block_sum((double)npos, red_d);
+  if (tid == 0) {
+    atomicAdd(stats + DAE_STAT_TRIPLET_SUM, ls);
+    atomicAdd(stats + DAE_STAT_NUM, ps);
+  }
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
 // batch_hard: one CTA per anchor row.
 // ---------------------------------------------------------------------------------------------------------------------
 constexpr int kHardThreads = 256;
@@ -406,14 +538,30 @@ __global__ void triplet_explicit_kernel(const float* __restrict__ E, const float
   if (r == 0 && lane == 0) stats[DAE_STAT_N_ACTIVE] = (double)B;
 }
 
+constexpr int kSmemSweepMaxB = 4096;   // triplet_batch_all_kernel serves B up to here, triplet_batch_all_tiled_kernel above
+static int g_force_tiled = 0;           // test hook (dae_triplet_config): the tiled sweep at every B
+
 }  // namespace dae
+
+extern "C" int dae_triplet_config(int32_t force_tiled) {
+  dae::g_force_tiled = force_tiled ? 1 : 0;
+  return DAE_OK;
+}
 
 extern "C" int dae_triplet_batch_all(const float* S, int64_t lds, int32_t B, const int32_t* seg_lo, const int32_t* seg_hi, float* G,
                                      int64_t ldg, double* stats, int32_t pos_only, void* g_hi, void* g_lo, int64_t ld_split, void* stream) {
   using namespace dae;
-  DAE_REQUIRE(S && seg_lo && seg_hi && G && stats && B >= 1 && B <= 4096 && lds >= B && ldg >= B, "dae_triplet_batch_all: bad arguments");
+  DAE_REQUIRE(S && seg_lo && seg_hi && G && stats && B >= 1 && lds >= B && ldg >= B, "dae_triplet_batch_all: bad arguments");
+  DAE_REQUIRE(B <= DAE_MAX_TRIPLET_BATCH, "dae_triplet_batch_all: B <= %d rows, the cap of the B x B mining buffers (got %d)",
+              DAE_MAX_TRIPLET_BATCH, B);
   DAE_REQUIRE(!g_hi || (g_lo && ld_split >= B), "dae_triplet_batch_all: bad split outputs");
   cudaStream_t st = (cudaStream_t)stream;
+  if (B > kSmemSweepMaxB || g_force_tiled) {
+    triplet_batch_all_tiled_kernel<<<B, kTripThreads, 0, st>>>(S, lds, B, seg_lo, seg_hi, G, ldg, stats, pos_only, (__nv_bfloat16*)g_hi,
+                                                               (__nv_bfloat16*)g_lo, ld_split);
+    DAE_CHECK_LAUNCH("dae_triplet_batch_all(tiled)");
+    return DAE_OK;
+  }
   const int Pj = (B + kJTile - 1) / kJTile * kJTile;
   const int Pk = (B + kKTile - 1) / kKTile * kKTile;
   const size_t smem = sizeof(float) * ((size_t)3 * Pj + (size_t)2 * Pk + (size_t)kTY * Pk);

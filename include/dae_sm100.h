@@ -46,6 +46,8 @@ extern "C" {
 #define DAE_TRIPLET_NONE 0
 #define DAE_TRIPLET_BATCH_ALL 1
 #define DAE_TRIPLET_BATCH_HARD 2
+/* largest batch of the batch_all / batch_hard strategies: S, G and G's bf16 hi/lo copy take ~13 GB at 32768 rows */
+#define DAE_MAX_TRIPLET_BATCH 32768
 
 #define DAE_OPT_SGD 0
 #define DAE_OPT_ADAGRAD 1
@@ -76,7 +78,9 @@ int dae_last_error(char* buf, size_t len);
  * permutation, orders them by label (the loss is invariant to the order of rows in a batch),
  * and emits for each batch row its dataset row id, label, class segment [seg_lo, seg_hi) and -
  * for batch_all - the closed-form data weight w_i and N_valid.  strategy none: order kept, w = 1.
- * One CTA; B <= 4096.  stats: float64[DAE_STAT_SLOTS], zeroed here, SUM_W / N_VALID filled.
+ * One CTA.  Triplet strategies: B <= DAE_MAX_TRIPLET_BATCH; up to 4096 rows the batch is sorted in shared memory, above that
+ * inside labels_out / rows_out (labels_out must then be non-NULL).  The order is ascending (label, row id) either way.
+ * stats: float64[DAE_STAT_SLOTS], zeroed here, SUM_W / N_VALID filled.
  * ctl (optional, device int64[4]): per-step cursors kept in device memory so that a captured CUDA graph of the
  * step can be replayed without host-side argument changes -- ctl[0] is added to `offset`, ctl[1] is the row of the
  * stats log dae_step_finalize writes, ctl[2] the 1-based optimizer step; dae_step_advance moves all three.
@@ -235,11 +239,16 @@ int dae_colsum(const float* M, int32_t n_rows, int32_t n_cols, int64_t ld, float
  *   pos_only != 0 (pos_triplets_only=True, :118-120; never used by the model): the loss sum covers positive triplets
  *   only and G receives raw COUNTS of positive triplets (G[i,j] = -#k, G[i,k] = +#j) from which the caller derives the weights.
  *   g_hi / g_lo (optional, bf16 [B x ld_split]): G also leaves as the hi / lo operand pair dae_gemm_sym_bf16x3 reads.
+ *   B <= DAE_MAX_TRIPLET_BATCH.  Up to 4096 rows one CTA per anchor keeps the whole row in shared memory (~52 B bytes); above,
+ *   a tiled sweep streams the anchor's positives / negatives through fixed-size chunks (47 KB of shared memory at any B).
  * batch_hard (triplet_loss_utils.py:202-259): also writes the data weight (w) and sum_w.
  */
 int dae_triplet_batch_all(const float* S, int64_t lds, int32_t B, const int32_t* seg_lo, const int32_t* seg_hi,
                           float* G, int64_t ldg, double* stats, int32_t pos_only, void* g_hi, void* g_lo,
                           int64_t ld_split, void* stream);
+/* Sweep selection of dae_triplet_batch_all (test hook): force_tiled != 0 runs the tiled sweep at every B; 0 (default) only above
+ * 4096 rows. */
+int dae_triplet_config(int32_t force_tiled);
 int dae_triplet_batch_hard(const float* S, int64_t lds, int32_t B, const float* labels, float* G, int64_t ldg,
                            float* weight, double* stats, void* stream);
 /* explicit triplets (autoencoder_triplet.py:308-311): loss = mean softplus(e.en - e.ep); ACCUMULATES alpha * dloss
