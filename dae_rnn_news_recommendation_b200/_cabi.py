@@ -18,6 +18,7 @@ STAT = {'cost': 0, 'ae_loss': 1, 'triplet_loss': 2, 'fraction': 3, 'num': 4, 'su
         'triplet_sum': 8, 'n_active': 9}
 STAT_SLOTS = 16
 MAX_TRIPLET_BATCH = 32768   # DAE_MAX_TRIPLET_BATCH: largest batch_all / batch_hard batch (S, G and G's bf16 copy: ~13 GB)
+MAX_BLOCKED_BATCH = 262144  # DAE_MAX_BLOCKED_BATCH: largest batch of a block-mined engine (TrainEngine(mining_block_rows=R))
 
 
 def act_code(name):
@@ -32,6 +33,8 @@ _SIGNATURES = {
     'dae_last_error': (C.c_int, [C.c_char_p, sz]),
     'dae_batch_prepare': (C.c_int, [p, i64, p, i32, p, i32, p, p, p, p, p, p, p]),
     'dae_batch_prepare_next': (C.c_int, [p, i64, i64, p, i32, p, i32, p, p, p, p, p, p, p]),
+    'dae_batch_prepare_blocked': (C.c_int, [p, i64, p, i32, p, i32, p, p, p, p, p, p, p]),
+    'dae_batch_prepare_next_blocked': (C.c_int, [p, i64, i64, p, i32, p, i32, p, p, p, p, p, p, p]),
     'dae_batch_commit': (C.c_int, [i32, p, p, p, p, p, p, p, p, p, p, p, p, p]),
     'dae_batch_prepare_explicit': (C.c_int, [p, i64, p, i32, i64, p, p, p]),
     'dae_step_advance': (C.c_int, [p, i64, p]),
@@ -54,6 +57,9 @@ _SIGNATURES = {
     'dae_triplet_config': (C.c_int, [i32]),
     'dae_gemm_sym_bf16x3': (C.c_int, [i32, i32, f32, p, p, i64, p, p, i64, p, i64, i32, p]),
     'dae_triplet_batch_hard': (C.c_int, [p, i64, i32, p, p, i64, p, p, p]),
+    'dae_triplet_batch_all_rows': (C.c_int, [p, i64, i32, i32, i32, p, p, p, i64, p, i32, p, p, i64, p]),
+    'dae_triplet_batch_hard_rows': (C.c_int, [p, i64, i32, i32, i32, p, p, i64, p, p, p]),
+    'dae_triplet_batch_hard_finish': (C.c_int, [p, i32, p, p, i32, i64, p]),
     'dae_triplet_explicit': (C.c_int, [p, p, p, i32, i32, i64, f32, p, p, p, p, p]),
     'dae_step_finalize': (C.c_int, [p, p, i32, p, i32, i32, f32, p, p, p, p]),
     'dae_optimizer_step': (C.c_int, [p, p, p, p, i64, i32, f32, f32, f32, i32, p, p, p, i32, i32, i64, p]),

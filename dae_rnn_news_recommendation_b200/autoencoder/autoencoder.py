@@ -21,8 +21,8 @@ import torch
 
 from . import utils
 from .. import _cabi
-from ..engine import TrainEngine, DeviceCSR, canonical_csr
-from .._cabi import STAT, STAT_SLOTS, MAX_TRIPLET_BATCH
+from ..engine import TrainEngine, DeviceCSR, canonical_csr, check_mining_block_rows
+from .._cabi import STAT, STAT_SLOTS, MAX_TRIPLET_BATCH, MAX_BLOCKED_BATCH
 
 
 class DenoisingAutoencoder(object):
@@ -31,12 +31,14 @@ class DenoisingAutoencoder(object):
                  dec_act_func='none', loss_func='mean_squared', num_epochs=10, batch_size=10,
                  xavier_init=1, opt='gradient_descent', learning_rate=0.01, momentum=0.5, corr_type='none',
                  corr_frac=0., verbose=True, verbose_step=5, seed=-1, alpha=1, triplet_strategy='batch_all',
-                 device=None, rng_mode='device', W_init=None):
+                 device=None, rng_mode='device', W_init=None, mining_block_rows=None):
         """Arguments as in the reference (autoencoder.py:20-45).  Extensions: device ('cuda:N'; default: LOCAL_RANK or 0),
         rng_mode ('device' = Philox mask + device permutation, the default: an epoch of the UCI config is 3 ms of GPU time, the host
         RNG alone would take 6 ms; 'numpy' = the reference's host NumPy RNG stream for corruption and shuffling, drawn one epoch
         ahead on a worker thread -- bit-identical masks and batch order to a seeded reference run), W_init (ndarray F x H
-        overriding the Xavier draw)."""
+        overriding the Xavier draw), mining_block_rows (None: batch_all / batch_hard hold the B x B similarity matrix, batches up to
+        MAX_TRIPLET_BATCH rows; R, a multiple of 128 up to 32768: they mine it R anchor rows at a time in 12 R B bytes, batches up to
+        MAX_BLOCKED_BATCH rows)."""
         self.algo_name = algo_name
         self.model_name = model_name
         self.compress_factor = compress_factor
@@ -82,6 +84,7 @@ class DenoisingAutoencoder(object):
         self.device = device
         self.rng_mode = rng_mode
         self.W_init = W_init
+        self.mining_block_rows = check_mining_block_rows(mining_block_rows)   # not in parameter.txt: its layout is the reference's
         self.engine = None
 
     # ------------------------------------------------------------------------------------------------------------------
@@ -103,7 +106,7 @@ class DenoisingAutoencoder(object):
         eng = TrainEngine(n_features, int(self.n_components), enc_act_func=self.enc_act_func,
                           dec_act_func=self.dec_act_func, loss_func=self.loss_func, opt=self.opt,
                           learning_rate=self.learning_rate, momentum=self.momentum, alpha=self.alpha,
-                          triplet_strategy=self._strategy_name(), device=self.device)
+                          triplet_strategy=self._strategy_name(), device=self.device, mining_block_rows=self.mining_block_rows)
         return eng
 
     def _init_parameters(self, n_features, restore_previous_model):
@@ -231,13 +234,25 @@ class DenoisingAutoencoder(object):
         tail = [s0 for s0 in starts if s0 + bs > n]
         use_graph = (os.environ.get('DAE_CUDA_GRAPH', '1') == '1' and self.corr_type != 'salt_and_pepper' and len(full) >= 2)
         perm_buf = torch.zeros(n, dtype=torch.int32, device=eng.device)
-        if self.triplet_strategy != 'none':   # the mining branch keeps S, G and G's bf16 copy: B x B x 12 bytes
+        R = self.mining_block_rows
+        nv = 0 if validation_set is None else validation_set.shape[0]
+        if self.triplet_strategy != 'none' and R is None:   # the mining branch keeps S, G and G's bf16 copy: B x B x 12 bytes
             cap = MAX_TRIPLET_BATCH
+            hint = ' Set mining_block_rows (e.g. 4096) to mine the similarity matrix in blocks of rows, up to %d rows.' % MAX_BLOCKED_BATCH
             assert bs <= cap, ('triplet strategies need batch_size <= %d rows (got %d: the B x B similarity / gradient buffers would '
-                               'take %.1f GB)' % (cap, bs, 12.0 * bs * bs / 1e9))
-            nv = 0 if validation_set is None else validation_set.shape[0]
+                               'take %.1f GB).' % (cap, bs, 12.0 * bs * bs / 1e9) + hint)
             assert nv <= cap, ('the validation set is fed as ONE batch (autoencoder.py:300-309): at most %d rows with a triplet '
-                               'strategy (got %d: its B x B buffers would take %.1f GB)' % (cap, nv, 12.0 * nv * nv / 1e9))
+                               'strategy (got %d: its B x B buffers would take %.1f GB).' % (cap, nv, 12.0 * nv * nv / 1e9) + hint)
+        elif self.triplet_strategy != 'none':   # block mining: R x B rows of S, G and G's bf16 copy, plus dZ's bf16 hi / lo pair
+            cap = MAX_BLOCKED_BATCH
+            Fp = (host_csr.shape[1] + 31) // 32 * 32
+
+            def gb(b):
+                return (12.0 * min(R, b) * b + 4.0 * b * Fp) / 1e9
+            assert bs <= cap, ('triplet strategies with mining_block_rows need batch_size <= %d rows (got %d: its mining blocks and '
+                               'dZ would take %.1f GB)' % (cap, bs, gb(bs)))
+            assert nv <= cap, ('the validation set is fed as ONE batch (autoencoder.py:300-309): at most %d rows with mining_block_rows '
+                               '(got %d: its mining blocks and dZ would take %.1f GB)' % (cap, nv, gb(nv)))
         if validation_set is not None:        # size the workspaces once: a larger validation batch must not force a re-capture
             eng._ensure_ws(max(bs, validation_set.shape[0]))
         prefetch = self._host_rng_prefetch(host_csr, n)

@@ -306,50 +306,83 @@ extern "C" int dae_step_advance(int64_t* ctl, int64_t row_stride, void* stream) 
   return DAE_OK;
 }
 
-extern "C" int dae_batch_prepare(const int32_t* perm, int64_t offset, const int64_t* ctl, int32_t B, const float* labels_all,
-                                 int32_t strategy, int32_t* rows_out, float* labels_out, int32_t* seg_lo,
-                                 int32_t* seg_hi, float* weight_out, double* stats, void* stream) {
-  DAE_REQUIRE(B >= 1 && rows_out && stats, "dae_batch_prepare: bad B or null output");
+namespace dae {
+// dae_batch_prepare(_blocked) / dae_batch_prepare_next(_blocked): the same kernels under two batch caps, DAE_MAX_TRIPLET_BATCH for the
+// engines that hold B x B mining buffers and DAE_MAX_BLOCKED_BATCH for the block-mined ones.
+static const char* const kCapWhy[2] = {"the cap of the B x B mining buffers", "the cap of block-mined batches"};
+
+static int batch_prepare(const char* fn, int blocked, const int32_t* perm, int64_t offset, const int64_t* ctl, int32_t B,
+                         const float* labels_all, int32_t strategy, int32_t* rows_out, float* labels_out, int32_t* seg_lo,
+                         int32_t* seg_hi, float* weight_out, double* stats, void* stream) {
+  DAE_REQUIRE(B >= 1 && rows_out && stats, "%s: bad B or null output", fn);
   if (strategy == DAE_TRIPLET_NONE) {
-    dae::batch_rows_kernel<<<(B + 255) / 256, 256, 0, (cudaStream_t)stream>>>(perm, offset, ctl, B, rows_out, labels_out, seg_lo,
-                                                                            seg_hi, weight_out, stats);
+    batch_rows_kernel<<<(B + 255) / 256, 256, 0, (cudaStream_t)stream>>>(perm, offset, ctl, B, rows_out, labels_out, seg_lo, seg_hi,
+                                                                         weight_out, stats);
     DAE_CHECK_LAUNCH("dae_batch_prepare(none)");
     return DAE_OK;
   }
-  DAE_REQUIRE(B <= DAE_MAX_TRIPLET_BATCH, "dae_batch_prepare: triplet strategies need B <= %d rows, the cap of the B x B mining "
-              "buffers (got %d)", DAE_MAX_TRIPLET_BATCH, B);
-  DAE_REQUIRE(seg_lo && seg_hi, "dae_batch_prepare: null segment outputs");
-  DAE_REQUIRE(strategy == DAE_TRIPLET_NONE || labels_all, "dae_batch_prepare: labels required for triplet strategies");
-  if (B > dae::kMaxB) {
-    DAE_REQUIRE(labels_out, "dae_batch_prepare: B > %d needs labels_out (the batch is sorted inside it)", dae::kMaxB);
-    dae::batch_prepare_large_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(perm, offset, ctl, B, labels_all, strategy, rows_out,
-                                                                         labels_out, seg_lo, seg_hi, weight_out, stats, 0);
+  const int cap = blocked ? DAE_MAX_BLOCKED_BATCH : DAE_MAX_TRIPLET_BATCH;
+  DAE_REQUIRE(B <= cap, "%s: triplet strategies need B <= %d rows, %s (got %d)", fn, cap, kCapWhy[blocked], B);
+  DAE_REQUIRE(seg_lo && seg_hi, "%s: null segment outputs", fn);
+  DAE_REQUIRE(strategy == DAE_TRIPLET_NONE || labels_all, "%s: labels required for triplet strategies", fn);
+  if (B > kMaxB) {
+    DAE_REQUIRE(labels_out, "%s: B > %d needs labels_out (the batch is sorted inside it)", fn, kMaxB);
+    batch_prepare_large_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(perm, offset, ctl, B, labels_all, strategy, rows_out, labels_out,
+                                                                     seg_lo, seg_hi, weight_out, stats, 0);
   } else {
-    dae::batch_prepare_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(perm, offset, ctl, B, labels_all, strategy, rows_out,
-                                                                   labels_out, seg_lo, seg_hi, weight_out, stats, 0);
+    batch_prepare_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(perm, offset, ctl, B, labels_all, strategy, rows_out, labels_out, seg_lo,
+                                                               seg_hi, weight_out, stats, 0);
   }
-  DAE_CHECK_LAUNCH("dae_batch_prepare");
+  DAE_CHECK_LAUNCH(fn);
   return DAE_OK;
+}
+
+static int batch_prepare_next(const char* fn, int blocked, const int32_t* perm, int64_t n_perm, int64_t stride, const int64_t* ctl,
+                              int32_t B, const float* labels_all, int32_t strategy, int32_t* rows_s, float* labels_s, int32_t* seg_lo_s,
+                              int32_t* seg_hi_s, float* weight_s, double* stats_s, void* stream) {
+  DAE_REQUIRE(ctl && n_perm > 0 && B >= 1 && rows_s && seg_lo_s && seg_hi_s && stats_s && labels_all, "%s: bad arguments", fn);
+  const int cap = blocked ? DAE_MAX_BLOCKED_BATCH : DAE_MAX_TRIPLET_BATCH;
+  DAE_REQUIRE(B <= cap, "%s: triplet strategies need B <= %d rows, %s (got %d)", fn, cap, kCapWhy[blocked], B);
+  DAE_REQUIRE(strategy == DAE_TRIPLET_BATCH_ALL || strategy == DAE_TRIPLET_BATCH_HARD, "%s: triplet strategies only", fn);
+  if (B > kMaxB) {
+    DAE_REQUIRE(labels_s, "%s: B > %d needs labels_s (the batch is sorted inside it)", fn, kMaxB);
+    batch_prepare_large_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(perm, stride, ctl, B, labels_all, strategy, rows_s, labels_s,
+                                                                     seg_lo_s, seg_hi_s, weight_s, stats_s, n_perm);
+  } else {
+    batch_prepare_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(perm, stride, ctl, B, labels_all, strategy, rows_s, labels_s, seg_lo_s,
+                                                               seg_hi_s, weight_s, stats_s, n_perm);
+  }
+  DAE_CHECK_LAUNCH(fn);
+  return DAE_OK;
+}
+}  // namespace dae
+
+extern "C" int dae_batch_prepare(const int32_t* perm, int64_t offset, const int64_t* ctl, int32_t B, const float* labels_all,
+                                 int32_t strategy, int32_t* rows_out, float* labels_out, int32_t* seg_lo,
+                                 int32_t* seg_hi, float* weight_out, double* stats, void* stream) {
+  return dae::batch_prepare("dae_batch_prepare", 0, perm, offset, ctl, B, labels_all, strategy, rows_out, labels_out, seg_lo, seg_hi,
+                            weight_out, stats, stream);
+}
+
+extern "C" int dae_batch_prepare_blocked(const int32_t* perm, int64_t offset, const int64_t* ctl, int32_t B, const float* labels_all,
+                                         int32_t strategy, int32_t* rows_out, float* labels_out, int32_t* seg_lo,
+                                         int32_t* seg_hi, float* weight_out, double* stats, void* stream) {
+  return dae::batch_prepare("dae_batch_prepare_blocked", 1, perm, offset, ctl, B, labels_all, strategy, rows_out, labels_out, seg_lo,
+                            seg_hi, weight_out, stats, stream);
 }
 
 extern "C" int dae_batch_prepare_next(const int32_t* perm, int64_t n_perm, int64_t stride, const int64_t* ctl, int32_t B,
                                       const float* labels_all, int32_t strategy, int32_t* rows_s, float* labels_s, int32_t* seg_lo_s,
                                       int32_t* seg_hi_s, float* weight_s, double* stats_s, void* stream) {
-  DAE_REQUIRE(ctl && n_perm > 0 && B >= 1 && rows_s && seg_lo_s && seg_hi_s && stats_s && labels_all,
-              "dae_batch_prepare_next: bad arguments");
-  DAE_REQUIRE(B <= DAE_MAX_TRIPLET_BATCH, "dae_batch_prepare_next: triplet strategies need B <= %d rows, the cap of the B x B mining "
-              "buffers (got %d)", DAE_MAX_TRIPLET_BATCH, B);
-  DAE_REQUIRE(strategy == DAE_TRIPLET_BATCH_ALL || strategy == DAE_TRIPLET_BATCH_HARD, "dae_batch_prepare_next: triplet strategies only");
-  if (B > dae::kMaxB) {
-    DAE_REQUIRE(labels_s, "dae_batch_prepare_next: B > %d needs labels_s (the batch is sorted inside it)", dae::kMaxB);
-    dae::batch_prepare_large_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(perm, stride, ctl, B, labels_all, strategy, rows_s, labels_s,
-                                                                         seg_lo_s, seg_hi_s, weight_s, stats_s, n_perm);
-  } else {
-    dae::batch_prepare_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(perm, stride, ctl, B, labels_all, strategy, rows_s, labels_s, seg_lo_s,
-                                                                   seg_hi_s, weight_s, stats_s, n_perm);
-  }
-  DAE_CHECK_LAUNCH("dae_batch_prepare_next");
-  return DAE_OK;
+  return dae::batch_prepare_next("dae_batch_prepare_next", 0, perm, n_perm, stride, ctl, B, labels_all, strategy, rows_s, labels_s,
+                                 seg_lo_s, seg_hi_s, weight_s, stats_s, stream);
+}
+
+extern "C" int dae_batch_prepare_next_blocked(const int32_t* perm, int64_t n_perm, int64_t stride, const int64_t* ctl, int32_t B,
+                                              const float* labels_all, int32_t strategy, int32_t* rows_s, float* labels_s,
+                                              int32_t* seg_lo_s, int32_t* seg_hi_s, float* weight_s, double* stats_s, void* stream) {
+  return dae::batch_prepare_next("dae_batch_prepare_next_blocked", 1, perm, n_perm, stride, ctl, B, labels_all, strategy, rows_s,
+                                 labels_s, seg_lo_s, seg_hi_s, weight_s, stats_s, stream);
 }
 
 extern "C" int dae_batch_commit(int32_t B, const int32_t* rows_s, const float* labels_s, const int32_t* seg_lo_s, const int32_t* seg_hi_s,

@@ -1167,14 +1167,15 @@ __global__ void decode_tile_ptr_kernel(const int64_t* __restrict__ indptr, const
                                        const int32_t* __restrict__ rows, int M, int n_half_tiles, int half_n,
                                        int32_t* __restrict__ tile_ptr) {
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
-  const int m = blockIdx.y;
-  if (t > n_half_tiles || m >= M) return;
-  const int64_t row = rows ? (int64_t)rows[m] : (int64_t)m;
-  const int64_t b = indptr[row], e = indptr[row + 1];
-  const int target = t * half_n;
-  int64_t lo = b, hi = e;
-  while (lo < hi) { const int64_t mid = (lo + hi) >> 1; if (indices[mid] < target) lo = mid + 1; else hi = mid; }
-  tile_ptr[(int64_t)m * (n_half_tiles + 1) + t] = (int32_t)(lo - b);
+  if (t > n_half_tiles) return;
+  for (int m = blockIdx.y; m < M; m += gridDim.y) {   // grid.y <= 65 535: batches above that loop over their rows
+    const int64_t row = rows ? (int64_t)rows[m] : (int64_t)m;
+    const int64_t b = indptr[row], e = indptr[row + 1];
+    const int target = t * half_n;
+    int64_t lo = b, hi = e;
+    while (lo < hi) { const int64_t mid = (lo + hi) >> 1; if (indices[mid] < target) lo = mid + 1; else hi = mid; }
+    tile_ptr[(int64_t)m * (n_half_tiles + 1) + t] = (int32_t)(lo - b);
+  }
 }
 
 // fp32 -> (bf16 hi, bf16 lo) split, row by row, zero padding up to ld_dst columns; optional 1.0 in column `ones_col`.
@@ -1535,7 +1536,7 @@ extern "C" int dae_decode_prepare(int32_t Brows, int32_t F, const int64_t* indpt
   cudaStream_t st = (cudaStream_t)stream;
   DAE_CUDA(cudaMemsetAsync(row_loss_part, 0, sizeof(float) * Brows, st));
   const int n_half = 2 * ((F + kDecodeN - 1) / kDecodeN);            // two column parts per tile of the fused decode kernel
-  dim3 grid((n_half + 1 + 127) / 128, Brows);
+  dim3 grid((n_half + 1 + 127) / 128, Brows < 65535 ? Brows : 65535);
   decode_tile_ptr_kernel<<<grid, 128, 0, st>>>(indptr, indices, rows, Brows, n_half, kDecodeN / 2, tile_ptr);
   DAE_CHECK_LAUNCH("dae_decode_prepare");
   return DAE_OK;

@@ -289,7 +289,9 @@ constexpr int kChunkJ = 512;    // positives per chunk (16 j-tiles)
 constexpr int kChunkK = 1024;   // negatives per chunk (8 k-tiles)
 static_assert(kChunkJ % kJTile == 0 && kChunkK % kKTile == 0, "chunks must hold whole register tiles");
 
-__global__ void __launch_bounds__(kTripThreads) triplet_batch_all_tiled_kernel(const float* __restrict__ S, int64_t lds, int B,
+// Anchor i = row0 + blockIdx.x lives in row blockIdx.x of S / G / g_hi / g_lo (row0 = 0: the whole B x B matrices; row0 > 0: an
+// anchor-row block of them, see dae_triplet_batch_all_rows); segments are indexed by the anchor.
+__global__ void __launch_bounds__(kTripThreads) triplet_batch_all_tiled_kernel(const float* __restrict__ S, int64_t lds, int row0, int B,
                                                                                const int32_t* __restrict__ seg_lo,
                                                                                const int32_t* __restrict__ seg_hi, float* G, int64_t ldg,
                                                                                double* __restrict__ stats, int pos_only,
@@ -303,18 +305,18 @@ __global__ void __launch_bounds__(kTripThreads) triplet_batch_all_tiled_kernel(c
   __shared__ __align__(16) float gk[kTY * kChunkK];
   __shared__ float red_f[32];
   __shared__ double red_d[32];
-  const int i = blockIdx.x;
+  const int r = blockIdx.x, i = row0 + r;
   const int tid = threadIdx.x, tx = tid & 31, ty = tid >> 5;
   const int lo = seg_lo[i], hi = seg_hi[i];
   const int nj = hi - lo;
   const int nk = B - nj;
-  const float* srow = S + (int64_t)i * lds;
-  float* grow = G + (int64_t)i * ldg;
+  const float* srow = S + (int64_t)r * lds;
+  float* grow = G + (int64_t)r * ldg;
 
   if (nj <= 1 || nk == 0) {
     for (int c = tid; c < B; c += kTripThreads) {
       grow[c] = 0.0f;
-      if (g_hi) { g_hi[(int64_t)i * ld_split + c] = __float2bfloat16_rn(0.0f); g_lo[(int64_t)i * ld_split + c] = __float2bfloat16_rn(0.0f); }
+      if (g_hi) { g_hi[(int64_t)r * ld_split + c] = __float2bfloat16_rn(0.0f); g_lo[(int64_t)r * ld_split + c] = __float2bfloat16_rn(0.0f); }
     }
     return;
   }
@@ -385,8 +387,8 @@ __global__ void __launch_bounds__(kTripThreads) triplet_batch_all_tiled_kernel(c
       grow[c] = g;
       if (g_hi) {
         const __nv_bfloat16 h = __float2bfloat16_rn(g);
-        g_hi[(int64_t)i * ld_split + c] = h;
-        g_lo[(int64_t)i * ld_split + c] = __float2bfloat16_rn(g - __bfloat162float(h));
+        g_hi[(int64_t)r * ld_split + c] = h;
+        g_lo[(int64_t)r * ld_split + c] = __float2bfloat16_rn(g - __bfloat162float(h));
       }
     }
   }
@@ -396,8 +398,8 @@ __global__ void __launch_bounds__(kTripThreads) triplet_batch_all_tiled_kernel(c
     grow[c] = g;
     if (g_hi) {
       const __nv_bfloat16 h = __float2bfloat16_rn(g);
-      g_hi[(int64_t)i * ld_split + c] = h;
-      g_lo[(int64_t)i * ld_split + c] = __float2bfloat16_rn(g - __bfloat162float(h));
+      g_hi[(int64_t)r * ld_split + c] = h;
+      g_lo[(int64_t)r * ld_split + c] = __float2bfloat16_rn(g - __bfloat162float(h));
     }
   }
   const double ls = block_sum(lsum * (double)kLn2, red_d);
@@ -425,15 +427,16 @@ __device__ __forceinline__ float block_max(float v, float* red) {
   return r;
 }
 
-__global__ void __launch_bounds__(kHardThreads) triplet_batch_hard_kernel(const float* __restrict__ S, int64_t lds, int B,
+// Anchor a = row0 + blockIdx.x lives in row blockIdx.x of S / G (row0 = 0: the whole matrices; see dae_triplet_batch_hard_rows).
+__global__ void __launch_bounds__(kHardThreads) triplet_batch_hard_kernel(const float* __restrict__ S, int64_t lds, int row0, int B,
                                                                           const float* __restrict__ labels, float* __restrict__ G,
                                                                           int64_t ldg, float* __restrict__ weight,
                                                                           double* __restrict__ stats) {
   __shared__ float red[32];
   __shared__ float redi[32];
-  const int a = blockIdx.x, tid = threadIdx.x;
-  const float* srow = S + (int64_t)a * lds;
-  float* grow = G + (int64_t)a * ldg;
+  const int a = row0 + (int)blockIdx.x, tid = threadIdx.x;
+  const float* srow = S + (int64_t)blockIdx.x * lds;
+  float* grow = G + (int64_t)blockIdx.x * ldg;
   const float la = labels[a];
   // m = row max (triplet_loss_utils.py:227); hn = max(an * S) (:240-243)
   float m = -3.0e38f, hn = -3.0e38f;
@@ -511,6 +514,26 @@ __global__ void triplet_hard_scale_kernel(float* __restrict__ G, int64_t ldg, in
   }
 }
 
+// block-mined batch_hard, after the last anchor block: sum_w (block 0, the summation order of triplet_hard_scale_kernel) and
+// dE2 *= 1/(sum c + eps) -- the blocks' dE2 GEMMs ran on the unscaled G.
+__global__ void triplet_hard_finish_kernel(const float* __restrict__ weight, int B, double* __restrict__ stats, float* __restrict__ dE2,
+                                           int H, int64_t ld) {
+  if (blockIdx.x == 0) {
+    __shared__ double red[32];
+    double s = 0.0;
+    for (int i = threadIdx.x; i < B; i += blockDim.x) s += (double)weight[i];
+    s = block_sum(s, red);
+    if (threadIdx.x == 0) stats[DAE_STAT_SUM_W] = s;
+  }
+  if (!dE2) return;
+  const float inv = (float)(1.0 / (stats[DAE_STAT_N_ACTIVE] + 1e-16));
+  const int64_t total = (int64_t)B * H;
+  for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t r = e / H;
+    dE2[r * ld + (e - r * H)] *= inv;
+  }
+}
+
 // explicit triplets: one warp per row
 __global__ void triplet_explicit_kernel(const float* __restrict__ E, const float* __restrict__ Ep, const float* __restrict__ En,
                                         int B, int H, int64_t ld, float alpha, float* __restrict__ dE, float* __restrict__ dEp,
@@ -557,7 +580,7 @@ extern "C" int dae_triplet_batch_all(const float* S, int64_t lds, int32_t B, con
   DAE_REQUIRE(!g_hi || (g_lo && ld_split >= B), "dae_triplet_batch_all: bad split outputs");
   cudaStream_t st = (cudaStream_t)stream;
   if (B > kSmemSweepMaxB || g_force_tiled) {
-    triplet_batch_all_tiled_kernel<<<B, kTripThreads, 0, st>>>(S, lds, B, seg_lo, seg_hi, G, ldg, stats, pos_only, (__nv_bfloat16*)g_hi,
+    triplet_batch_all_tiled_kernel<<<B, kTripThreads, 0, st>>>(S, lds, 0, B, seg_lo, seg_hi, G, ldg, stats, pos_only, (__nv_bfloat16*)g_hi,
                                                                (__nv_bfloat16*)g_lo, ld_split);
     DAE_CHECK_LAUNCH("dae_triplet_batch_all(tiled)");
     return DAE_OK;
@@ -587,10 +610,53 @@ extern "C" int dae_triplet_batch_hard(const float* S, int64_t lds, int32_t B, co
   DAE_REQUIRE(S && labels && G && weight && stats && B >= 1 && lds >= B && ldg >= B, "dae_triplet_batch_hard: bad arguments");
   cudaStream_t st = (cudaStream_t)stream;
   DAE_CUDA(cudaMemsetAsync(weight, 0, sizeof(float) * B, st));
-  triplet_batch_hard_kernel<<<B, kHardThreads, 0, st>>>(S, lds, B, labels, G, ldg, weight, stats);
+  triplet_batch_hard_kernel<<<B, kHardThreads, 0, st>>>(S, lds, 0, B, labels, G, ldg, weight, stats);
   dim3 grid((B + 255) / 256, B);
   triplet_hard_scale_kernel<<<grid, 256, 0, st>>>(G, ldg, B, weight, stats);
   DAE_CHECK_LAUNCH("dae_triplet_batch_hard");
+  return DAE_OK;
+}
+
+extern "C" int dae_triplet_batch_all_rows(const float* S_blk, int64_t lds, int32_t row0, int32_t n_rows, int32_t B, const int32_t* seg_lo,
+                                          const int32_t* seg_hi, float* G_blk, int64_t ldg, double* stats, int32_t pos_only, void* g_hi,
+                                          void* g_lo, int64_t ld_split, void* stream) {
+  using namespace dae;
+  DAE_REQUIRE(S_blk && seg_lo && seg_hi && G_blk && stats && B >= 1 && lds >= B && ldg >= B,
+              "dae_triplet_batch_all_rows: bad arguments");
+  DAE_REQUIRE(B <= DAE_MAX_BLOCKED_BATCH, "dae_triplet_batch_all_rows: B <= %d rows (got %d)", DAE_MAX_BLOCKED_BATCH, B);
+  DAE_REQUIRE(row0 >= 0 && n_rows >= 1 && (int64_t)row0 + n_rows <= B,
+              "dae_triplet_batch_all_rows: anchor rows [%d, %lld) outside the batch of %d", row0, (long long)row0 + n_rows, B);
+  DAE_REQUIRE(!g_hi || (g_lo && ld_split >= B), "dae_triplet_batch_all_rows: bad split outputs");
+  triplet_batch_all_tiled_kernel<<<n_rows, kTripThreads, 0, (cudaStream_t)stream>>>(S_blk, lds, row0, B, seg_lo, seg_hi, G_blk, ldg, stats,
+                                                                                    pos_only, (__nv_bfloat16*)g_hi, (__nv_bfloat16*)g_lo,
+                                                                                    ld_split);
+  DAE_CHECK_LAUNCH("dae_triplet_batch_all_rows");
+  return DAE_OK;
+}
+
+extern "C" int dae_triplet_batch_hard_rows(const float* S_blk, int64_t lds, int32_t row0, int32_t n_rows, int32_t B, const float* labels,
+                                           float* G_blk, int64_t ldg, float* weight, double* stats, void* stream) {
+  using namespace dae;
+  DAE_REQUIRE(S_blk && labels && G_blk && weight && stats && B >= 1 && lds >= B && ldg >= B, "dae_triplet_batch_hard_rows: bad arguments");
+  DAE_REQUIRE(B <= DAE_MAX_BLOCKED_BATCH, "dae_triplet_batch_hard_rows: B <= %d rows (got %d)", DAE_MAX_BLOCKED_BATCH, B);
+  DAE_REQUIRE(row0 >= 0 && n_rows >= 1 && (int64_t)row0 + n_rows <= B,
+              "dae_triplet_batch_hard_rows: anchor rows [%d, %lld) outside the batch of %d", row0, (long long)row0 + n_rows, B);
+  triplet_batch_hard_kernel<<<n_rows, kHardThreads, 0, (cudaStream_t)stream>>>(S_blk, lds, row0, B, labels, G_blk, ldg, weight, stats);
+  DAE_CHECK_LAUNCH("dae_triplet_batch_hard_rows");
+  return DAE_OK;
+}
+
+extern "C" int dae_triplet_batch_hard_finish(const float* weight, int32_t B, double* stats, float* dE2, int32_t H, int64_t ld, void* stream) {
+  using namespace dae;
+  DAE_REQUIRE(weight && stats && B >= 1 && B <= DAE_MAX_BLOCKED_BATCH, "dae_triplet_batch_hard_finish: bad arguments");
+  DAE_REQUIRE(!dE2 || (H >= 1 && ld >= H), "dae_triplet_batch_hard_finish: bad dE2 shape");
+  int blocks = 1;
+  if (dE2) {
+    const int64_t want = ((int64_t)B * H + 255) / 256;
+    blocks = (int)(want < 4096 ? want : 4096);
+  }
+  triplet_hard_finish_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(weight, B, stats, dE2, H, ld);
+  DAE_CHECK_LAUNCH("dae_triplet_batch_hard_finish");
   return DAE_OK;
 }
 

@@ -96,12 +96,27 @@ class _CSRView:
         self.max_row_nnz = None
 
 
+def check_mining_block_rows(R):
+    """mining_block_rows: None (the B x B mining buffers, batches up to MAX_TRIPLET_BATCH rows) or the anchor rows R of S held at once
+    (batches up to MAX_BLOCKED_BATCH rows): a multiple of 128 (the Gram block's TMA base and tiles stay aligned) in [128, 32768]."""
+    if R is None:
+        return None
+    if isinstance(R, bool) or int(R) != R or not (128 <= int(R) <= 32768 and int(R) % 128 == 0):
+        raise ValueError('mining_block_rows must be None or a multiple of 128 in [128, 32768] (got %r)' % (R,))
+    return int(R)
+
+
 class TrainEngine:
     """Flat parameters + per-batch workspaces + the kernel sequence of one step."""
 
     def __init__(self, n_features, n_components, enc_act_func='sigmoid', dec_act_func='sigmoid',
                  loss_func='cross_entropy', opt='gradient_descent', learning_rate=0.1, momentum=0.5, alpha=1.0,
-                 triplet_strategy='batch_all', device='cuda:0', process_group=None, gemm=None, allreduce=None):
+                 triplet_strategy='batch_all', device='cuda:0', process_group=None, gemm=None, allreduce=None,
+                 mining_block_rows=None):
+        """mining_block_rows: None = batch_all / batch_hard mine the whole B x B similarity matrix at once (12 B^2 bytes, batches up to
+        MAX_TRIPLET_BATCH rows); R = they mine it R anchor rows at a time (12 R B bytes, batches up to MAX_BLOCKED_BATCH rows;
+        tensor-core path only)."""
+        self.block_rows = check_mining_block_rows(mining_block_rows)
         _cabi.lib()  # fail loudly if the CUDA library is missing
         if not torch.cuda.is_available():
             raise _cabi.DaeError('no CUDA device: the DAE hot path has no CPU fallback')
@@ -136,6 +151,11 @@ class TrainEngine:
         # cores: the fp32 CUDA-core kernel would co-reside with the persistent tensor-core CTAs (17 KB of shared memory) but is several
         # times slower on these shapes
         self.small_gemm = self.gemm_mode
+        if self.block_rows is not None:
+            assert self.gemm_mode == self.small_gemm == 'tc', 'mining_block_rows needs the tensor-core path (gemm="tc")'
+        # the batch preparation exports of this engine: the block-mined one accepts batches above MAX_TRIPLET_BATCH
+        self._prepare = 'dae_batch_prepare' if self.block_rows is None else 'dae_batch_prepare_blocked'
+        self._prepare_next = 'dae_batch_prepare_next' if self.block_rows is None else 'dae_batch_prepare_next_blocked'
         # encode backward: 'gather' = column-bucketed, atomic-free dW accumulation; 'atomic' = red.global.add per entry
         self.enc_bwd_mode = 'gather'
         if self.H > (1024 if self.H % 4 == 0 else (512 if self.H % 2 == 0 else 256)):
@@ -388,7 +408,8 @@ class TrainEngine:
         self.E = torch.empty(B, self.H, **f32)
         self.dE = torch.empty(B, self.H, **f32)
         self.dE2 = torch.empty(B, self.H, **f32)   # triplet part of dL/dE, alpha (G + G^T) E (written on the mining branch)
-        self.Z = torch.empty(B, self.F, **f32)
+        if self.loss == 2 or self.gemm_mode != 'tc':   # Z = E.W^T is only materialised by the cosine loss and the CUDA-core path
+            self.Z = torch.empty(B, self.F, **f32)
         self.row_loss = torch.empty(B, **f32)
         self.weight = torch.empty(B, **f32)
         self.rows = torch.empty(B, **i32)
@@ -398,9 +419,11 @@ class TrainEngine:
         # staged copy of the per-batch buffers (rows, labels, seg_lo, seg_hi, weight, stats): the NEXT batch of a replayed step
         self._stage = (torch.zeros(B, **i32), torch.zeros(B, **f32), torch.zeros(B, **i32), torch.zeros(B, **i32), torch.zeros(B, **f32),
                        torch.zeros(STAT_SLOTS, dtype=torch.float64, device=self.device))
+        # the mining's S / G (and their bf16 hi / lo pair below): B x B, or R anchor rows x B when mined in blocks
+        mine_rows = B if self.block_rows is None else min(self.block_rows, B)
         if self.strategy in (1, 2):
-            self.S = torch.empty(B, B, **f32)
-            self.G = torch.empty(B, B, **f32)
+            self.S = torch.empty(mine_rows, B, **f32)
+            self.G = torch.empty(mine_rows, B, **f32)
         if self.gemm_mode == 'tc':
             bf = dict(dtype=torch.bfloat16, device=self.device)
             self.Bp = (B + 7) // 8 * 8
@@ -414,8 +437,8 @@ class TrainEngine:
                 self.W_hi = torch.empty(self.F, self.Hp, **bf)
                 self.W_lo = torch.empty(self.F, self.Hp, **bf)
             if self.strategy in (1, 2):
-                self.GG_hi = torch.empty(B, self.Bp, **bf)
-                self.GG_lo = torch.empty(B, self.Bp, **bf)
+                self.GG_hi = torch.empty(mine_rows, self.Bp, **bf)
+                self.GG_lo = torch.empty(mine_rows, self.Bp, **bf)
         self._ws_B = B
 
     def _ensure_bucket_scratch(self, B):
@@ -510,7 +533,7 @@ class TrainEngine:
             self._k('dae_batch_commit', B, *[ptr(t) for t in self._stage], ptr(self.rows), ptr(self.labels_b), ptr(self.seg_lo),
                     ptr(self.seg_hi), ptr(self.weight), ptr(self.stats), st)
         else:
-            self._k('dae_batch_prepare', ptr(perm), int(offset), ptr(ctl), B, ptr(self.labels), strat, ptr(self.rows), ptr(self.labels_b),
+            self._k(self._prepare, ptr(perm), int(offset), ptr(ctl), B, ptr(self.labels), strat, ptr(self.rows), ptr(self.labels_b),
                     ptr(self.seg_lo), ptr(self.seg_hi), ptr(self.weight), ptr(self.stats), st)
         self._branch_b_prologue(B, train)
         self._encode_forward(B, train)
@@ -520,14 +543,14 @@ class TrainEngine:
     def _stage_next_batch(self, perm, staged, B, stream):
         n_perm, stride = staged
         labels = self.labels if self._labels_next is None else self._labels_next    # (run_feeds: the NEXT feed's labels)
-        self._k('dae_batch_prepare_next', ptr(perm), int(n_perm), int(stride), ptr(self._ctl), B, ptr(labels), self.strategy,
+        self._k(self._prepare_next, ptr(perm), int(n_perm), int(stride), ptr(self._ctl), B, ptr(labels), self.strategy,
                 *[ptr(t) for t in self._stage], stream.cuda_stream)
 
     def stage_batch(self, perm, offset, B):
         """Host-side staging of the batch at `offset` (the first replay after a cursor jump, e.g. an epoch start)."""
         self._ensure_ws(B)
         s = self._stage
-        self._k('dae_batch_prepare', ptr(perm), int(offset), None, B, ptr(self.labels), self.strategy, ptr(s[0]), ptr(s[1]), ptr(s[2]),
+        self._k(self._prepare, ptr(perm), int(offset), None, B, ptr(self.labels), self.strategy, ptr(s[0]), ptr(s[1]), ptr(s[2]),
                 ptr(s[3]), ptr(s[4]), ptr(s[5]), _stream())
 
     def _branch_b_prologue(self, B, train):
@@ -594,13 +617,15 @@ class TrainEngine:
             used_a = True
             self._fork(main, sideA)
             with torch.cuda.stream(sideA):
-                self._mining(B, strat, tc)
+                self._mining(B, strat, tc, train)
                 self._dE_triplet(B, sideA)
                 ev_mined = torch.cuda.Event()
                 ev_mined.record(sideA)
         elif strat in (1, 2):
-            self._mining(B, strat, tc)            # in line: batch_hard's data weights come out of the mining kernel
-            if tc and train and par:              # ... but its dE contribution can still run next to the decode chain
+            self._mining(B, strat, tc, train)     # in line: batch_hard's data weights come out of the mining kernel
+            if self.block_rows is not None:       # (mined in blocks: each block's dE contribution is already in dE2)
+                pass
+            elif tc and train and par:            # ... but its dE contribution can still run next to the decode chain
                 used_a = True
                 self._fork(main, sideA)
                 self._dE_triplet(B, sideA)
@@ -684,6 +709,8 @@ class TrainEngine:
 
     def _dE_triplet(self, B, stream):
         """dE2 = alpha (G + G^T) E, the triplet part of dL/dE; the encode backward adds it to the decode part (dE_add)."""
+        if self.block_rows is not None:    # the block loop of _mining_blocked accumulated it block by block
+            return
         with torch.cuda.stream(stream):
             if self.small_gemm == 'tc' and self.strategy == 1:
                 # batch_all: the sweep wrote G as bf16 hi / lo; ONE GEMM walks G's columns and then its rows: alpha (G + G^T) E
@@ -708,8 +735,11 @@ class TrainEngine:
                       n_store=self.H, special_col=self.H, special_out=self._gbv(), k_splits=-1, accumulate=accumulate,
                       tag='gemm_decode_dW')
 
-    def _mining(self, B, strat, tc):
+    def _mining(self, B, strat, tc, train=True):
         """S = E.E^T and the triplet kernel (loss, statistics, G = dL/dS; batch_hard: also the data weights)."""
+        if self.block_rows is not None:
+            self._mining_blocked(B, strat, train)
+            return
         H, st = self.H, _stream()
         if tc and self.small_gemm == 'tc':
             Ehl = (self.E_hi, self.E_lo)
@@ -724,6 +754,41 @@ class TrainEngine:
         else:
             self._k('dae_triplet_batch_hard', ptr(self.S), B, B, ptr(self.labels_b), ptr(self.G), B, ptr(self.weight),
                     ptr(self.stats), st, n_launch=2)
+
+    def _mining_blocked(self, B, strat, train):
+        """The mining one block of R anchor rows at a time, for r0 = 0, R, 2R, ... (the last block is short):
+            S_blk = E[r0:r0+n].E^T;  the strategy's rows kernel -> G_blk (batch_all: scaled, with its bf16 hi / lo pair; batch_hard:
+            unscaled, split to hi / lo times alpha here);  training: dE2[r0:r0+n] += a G_blk.E  and  dE2 += a G_blk^T.E[r0:r0+n].
+        Both strategies are row-local in S, and dE2 = alpha (G + G^T) E splits over row blocks, so this equals _mining + _dE_triplet
+        on the whole matrix.  batch_hard's 1/(number of active anchors) is known after the last block: dae_triplet_batch_hard_finish
+        applies it to dE2 (and fills SUM_W)."""
+        R, H, st = self.block_rows, self.H, _stream()
+        Ehl = (self.E_hi, self.E_lo)
+        Ghl = (self.GG_hi, self.GG_lo)
+        lds, ldg, ldgg = self.S.stride(0), self.G.stride(0), self.GG_hi.stride(0)
+        if strat == 2:
+            self.weight.zero_()          # the rows kernels accumulate the data weights
+        if train:
+            self.dE2.zero_()
+        a = self.alpha if strat == 1 else 1.0   # batch_hard's hi / lo already carry alpha
+        for r0 in range(0, B, R):
+            n = min(R, B - r0)
+            Eblk = (self.E_hi[r0:], self.E_lo[r0:])
+            self._tc_gemm(n, B, H, 1.0, Eblk, 0, Ehl, 0, self.S, lds, tag='gemm_gram')
+            if strat == 1:
+                self._k('dae_triplet_batch_all_rows', ptr(self.S), lds, r0, n, B, ptr(self.seg_lo), ptr(self.seg_hi), ptr(self.G), ldg,
+                        ptr(self.stats), 0, ptr(self.GG_hi) if train else None, ptr(self.GG_lo) if train else None, ldgg if train else 0,
+                        st)
+            else:
+                self._k('dae_triplet_batch_hard_rows', ptr(self.S), lds, r0, n, B, ptr(self.labels_b), ptr(self.G), ldg, ptr(self.weight),
+                        ptr(self.stats), st)
+                if train:
+                    self._tc_split(self.G, n, B, ldg, self.GG_hi, self.GG_lo, scale=self.alpha)
+            if train:
+                self._tc_gemm(n, H, B, a, Ghl, 0, Ehl, 1, self.dE2[r0:], H, accumulate=1, tag='gemm_dE_tri')
+                self._tc_gemm(B, H, n, a, Ghl, 1, Eblk, 1, self.dE2, H, accumulate=1, tag='gemm_dE_tri')
+        if strat == 2:
+            self._k('dae_triplet_batch_hard_finish', ptr(self.weight), B, ptr(self.stats), ptr(self.dE2) if train else None, H, H, st)
 
     def evaluate(self, csr, labels, B=None):
         """Forward-only cost of the whole set fed as ONE batch with x_corr = x, like the reference's validation pass

@@ -48,6 +48,9 @@ extern "C" {
 #define DAE_TRIPLET_BATCH_HARD 2
 /* largest batch of the batch_all / batch_hard strategies: S, G and G's bf16 hi/lo copy take ~13 GB at 32768 rows */
 #define DAE_MAX_TRIPLET_BATCH 32768
+/* Largest batch of a block-mined engine (dae_batch_prepare_blocked, dae_triplet_*_rows): the one-CTA sort and dZ's B x Fp x 4 bytes
+ * bound it, not S -- the mining holds R anchor rows of S / G at a time. */
+#define DAE_MAX_BLOCKED_BATCH 262144
 
 #define DAE_OPT_SGD 0
 #define DAE_OPT_ADAGRAD 1
@@ -95,6 +98,14 @@ int dae_batch_prepare(const int32_t* perm, int64_t offset, const int64_t* ctl, i
 int dae_batch_prepare_next(const int32_t* perm, int64_t n_perm, int64_t stride, const int64_t* ctl, int32_t B,
                            const float* labels_all, int32_t strategy, int32_t* rows_s, float* labels_s,
                            int32_t* seg_lo_s, int32_t* seg_hi_s, float* weight_s, double* stats_s, void* stream);
+/* dae_batch_prepare / dae_batch_prepare_next with the cap DAE_MAX_BLOCKED_BATCH instead of DAE_MAX_TRIPLET_BATCH: same kernels, same
+ * outputs.  For the engines that mine one block of anchor rows at a time (dae_triplet_batch_all_rows / _hard_rows). */
+int dae_batch_prepare_blocked(const int32_t* perm, int64_t offset, const int64_t* ctl, int32_t B, const float* labels_all,
+                              int32_t strategy, int32_t* rows_out, float* labels_out, int32_t* seg_lo,
+                              int32_t* seg_hi, float* weight_out, double* stats, void* stream);
+int dae_batch_prepare_next_blocked(const int32_t* perm, int64_t n_perm, int64_t stride, const int64_t* ctl, int32_t B,
+                                   const float* labels_all, int32_t strategy, int32_t* rows_s, float* labels_s,
+                                   int32_t* seg_lo_s, int32_t* seg_hi_s, float* weight_s, double* stats_s, void* stream);
 int dae_batch_commit(int32_t B, const int32_t* rows_s, const float* labels_s, const int32_t* seg_lo_s,
                      const int32_t* seg_hi_s, const float* weight_s, const double* stats_s, int32_t* rows,
                      float* labels_b, int32_t* seg_lo, int32_t* seg_hi, float* weight, double* stats, void* stream);
@@ -251,6 +262,20 @@ int dae_triplet_batch_all(const float* S, int64_t lds, int32_t B, const int32_t*
 int dae_triplet_config(int32_t force_tiled);
 int dae_triplet_batch_hard(const float* S, int64_t lds, int32_t B, const float* labels, float* G, int64_t ldg,
                            float* weight, double* stats, void* stream);
+/* Block mining (batches up to DAE_MAX_BLOCKED_BATCH without any B x B buffer): the anchors row0 .. row0 + n_rows - 1 of a batch of B
+ * rows.  Row r of S_blk / G_blk (and of g_hi / g_lo) belongs to anchor row0 + r; segments and labels are indexed by the anchor.
+ * dae_triplet_batch_all_rows: the tiled sweep of dae_triplet_batch_all on those anchors (same chunks, order and fp64 flushes, so
+ *   the same G rows bit for bit as the tiled sweep on the whole matrix).
+ * dae_triplet_batch_hard_rows: the per-row batch_hard of dae_triplet_batch_hard on those anchors.  G_blk is written UNSCALED (the
+ *   1/(sum c + eps) factor is known only after the last block) and `weight` is accumulated, not cleared: zero it once per batch.
+ * dae_triplet_batch_hard_finish, after the last block: stats[SUM_W] = sum of weight, and dE2 [B x H, ld] *= 1/(N_ACTIVE + eps)
+ *   (dE2 == NULL: forward only). */
+int dae_triplet_batch_all_rows(const float* S_blk, int64_t lds, int32_t row0, int32_t n_rows, int32_t B, const int32_t* seg_lo,
+                               const int32_t* seg_hi, float* G_blk, int64_t ldg, double* stats, int32_t pos_only, void* g_hi,
+                               void* g_lo, int64_t ld_split, void* stream);
+int dae_triplet_batch_hard_rows(const float* S_blk, int64_t lds, int32_t row0, int32_t n_rows, int32_t B, const float* labels,
+                                float* G_blk, int64_t ldg, float* weight, double* stats, void* stream);
+int dae_triplet_batch_hard_finish(const float* weight, int32_t B, double* stats, float* dE2, int32_t H, int64_t ld, void* stream);
 /* explicit triplets (autoencoder_triplet.py:308-311): loss = mean softplus(e.en - e.ep); ACCUMULATES alpha * dloss
  * into dE/dEp/dEn (on top of the reconstruction gradient) and the loss sum into stats[DAE_STAT_TRIPLET_SUM]. */
 int dae_triplet_explicit(const float* E, const float* Ep, const float* En, int32_t B, int32_t H, int64_t ld,

@@ -1,7 +1,7 @@
 """Training steps with large triplet batches on the C2 data (100 000 synthetic tf-idf rows, F = 10 000, H = 500), one JSON line.
 
     python tools/bench_large_batch.py [--batch-sizes 800,4096,9800,16384,32768] [--strategies batch_all,batch_hard]
-                                      [--steps 3] [--warmup 1] [--ab-rounds 5]
+                                      [--steps 3] [--warmup 1] [--ab-rounds 5] [--mining-block-rows R] [--classes 4]
 
 For each strategy and batch size B:
   * step_ms: a replayed CUDA graph of the whole step (the path `fit` takes), median of --steps CUDA-event timings, the same batch
@@ -9,6 +9,9 @@ For each strategy and batch size B:
   * kernels_ms: one eager step on a single stream with each launch bracketed by CUDA events -- batch preparation, Gram GEMM,
     mining sweep, (G + G^T).E GEMM and the fused decode (median of two steps);
   * peak_gb: torch's peak allocated device memory over the configuration.
+With --mining-block-rows R the engines mine S in blocks of R anchor rows (batches up to 262 144 rows), and kernels_ms holds each
+phase's total over one eager step (after a warm-up step): preparation, Gram blocks, rows kernels, G's hi / lo split (batch_hard),
+dE2 GEMMs, batch_hard's finish and the fused decode.
 For batch_all at B <= 4096 the in-shared-memory sweep and the tiled sweep (the kernel used above 4096, forced through
 dae_triplet_config) are also timed alternately, kernel alone and as the replayed step.
 The card name and its power limit go into the JSON line.  Nothing is written to the source tree.
@@ -25,6 +28,8 @@ import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 KERNELS = ('dae_batch_prepare', 'gemm_gram', 'dae_triplet_batch_all', 'dae_triplet_batch_hard', 'gemm_dE_tri', 'gemm_decode_fwd')
+PHASES_BLOCKED = ('dae_batch_prepare_blocked', 'gemm_gram', 'dae_triplet_batch_all_rows', 'dae_triplet_batch_hard_rows', 'dae_split_bf16',
+                  'gemm_dE_tri', 'dae_triplet_batch_hard_finish', 'gemm_decode_fwd')
 
 
 def _power_limit_w():
@@ -56,7 +61,10 @@ def main():
     ap.add_argument('--steps', type=int, default=3)
     ap.add_argument('--warmup', type=int, default=1)
     ap.add_argument('--ab-rounds', type=int, default=5)
+    ap.add_argument('--mining-block-rows', type=int, default=0, help='R > 0: block mining (TrainEngine(mining_block_rows=R))')
+    ap.add_argument('--classes', type=int, default=4)
     a = ap.parse_args()
+    R = a.mining_block_rows or None
     from dae_rnn_news_recommendation_b200 import _cabi
     from dae_rnn_news_recommendation_b200._cabi import call, ptr
     from dae_rnn_news_recommendation_b200.engine import TrainEngine, DeviceCSR
@@ -64,27 +72,35 @@ def main():
     F, H = 10000, 500
     dev = torch.device('cuda:0')
     x = make_sparse(a.rows, F, 100, 'tfidf', seed=0)
-    labels = make_labels(a.rows, 4, seed=0)
+    labels = make_labels(a.rows, a.classes, seed=0)
     W0 = np.random.default_rng(1).uniform(-1, 1, (F, H)).astype(np.float32) * np.sqrt(6.0 / (F + H))
     csr = DeviceCSR(x, dev)
     lab_d = torch.from_numpy(labels).to(dev)
-    out = {'workload': 'C2 data: %d synthetic tf-idf rows, F=%d, H=%d, 4 classes, masking 0.3, SGD' % (a.rows, F, H),
-           'device': torch.cuda.get_device_name(dev), 'power_limit_w': _power_limit_w(), 'results': [], 'sweep_ab': []}
+    out = {'workload': 'C2 data: %d synthetic tf-idf rows, F=%d, H=%d, %d classes, masking 0.3, SGD' % (a.rows, F, H, a.classes),
+           'mining_block_rows': R, 'device': torch.cuda.get_device_name(dev), 'power_limit_w': _power_limit_w(), 'results': [],
+           'sweep_ab': []}
     for strategy in a.strategies.split(','):
         for B in [int(b) for b in a.batch_sizes.split(',')]:
             torch.cuda.empty_cache()
             torch.cuda.reset_peak_memory_stats(dev)
-            eng = TrainEngine(F, H, device=dev, triplet_strategy=strategy, opt='gradient_descent', learning_rate=0.1)
+            eng = TrainEngine(F, H, device=dev, triplet_strategy=strategy, opt='gradient_descent', learning_rate=0.1,
+                              mining_block_rows=R)
             eng.set_parameters(W0)
             eng.set_data(csr, None, lab_d)
             eng.corrupt_masking(0.3, seed=1234)
             perm = torch.randperm(a.rows, device=dev, dtype=torch.int32)
             # per-kernel times: eager steps on one stream
             eng.fork_branches = False
-            eng.time_kernels(KERNELS)
-            for _ in range(2):
+            if R is None:
+                eng.time_kernels(KERNELS)
+                for _ in range(2):
+                    eng.step(perm, 0, B)
+                kt = {k: float(np.median(v)) for k, v in eng.kernel_times_ms().items() if v}
+            else:   # one block loop launches each phase's kernels many times: their total over the second eager step
                 eng.step(perm, 0, B)
-            kt = {k: float(np.median(v)) for k, v in eng.kernel_times_ms().items() if v}
+                eng.time_kernels(PHASES_BLOCKED)
+                eng.step(perm, 0, B)
+                kt = {k: float(np.sum(v)) for k, v in eng.kernel_times_ms().items() if v}
             eng.time_kernels(None)
             eng.fork_branches = True
             g = eng.capture_step_graph(perm, B, None, row_stride=0)
@@ -96,7 +112,7 @@ def main():
             stats = eng.read_stats()
             row = {'strategy': strategy, 'B': B, 'step_ms': ms, 'articles_per_s': B / ms * 1e3, 'kernels_ms': kt,
                    'peak_gb': torch.cuda.max_memory_allocated(dev) / 1e9, 'cost': stats['cost'], 'triplet_loss': stats['triplet_loss']}
-            if strategy == 'batch_all' and B <= 4096:
+            if strategy == 'batch_all' and B <= 4096 and R is None:
                 g_tiled = None
                 try:
                     call('dae_triplet_config', 1)
