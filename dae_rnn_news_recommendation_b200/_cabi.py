@@ -76,7 +76,30 @@ _SIGNATURES = {
     'dae_csr_similarity_pair_hist_workspace': (C.c_int, [i32, i64, i32, p]),
     'dae_allreduce_multimem': (C.c_int, [p, p, p, i32, i32, i64, i32, p]),
     'dae_mask_values': (C.c_int, [p, p, i64, f32, u64, u64, p, p]),
+    # deterministic training step
+    'dae_gemm_det_workspace': (C.c_int, [p]),
+    'dae_gemm_bf16x3_det': (C.c_int, [i32, i32, i32, f32, p, p, i64, i32, p, p, i64, i32, p, i64, i32, i32, p, i32, i32, p, i64, p]),
+    'dae_gemm_sym_bf16x3_det': (C.c_int, [i32, i32, f32, p, p, i64, p, p, i64, p, i64, i32, p, i64, p]),
+    'dae_decode_loss_parts': (C.c_int, [i32, p]),
+    'dae_decode_fused_bf16x3_det': (C.c_int, [i32, i32, i32, p, p, i64, p, p, i64, p, p, p, p, p, i32, i32, p, p, p, p, i64, p, p, i32,
+                                              p]),
+    'dae_encode_csr_bwd_det_workspace': (C.c_int, [i32, i32, i32, i64, p]),
+    'dae_encode_csr_bwd_det': (C.c_int, [p, p, p, p, i32, i32, i32, f32, p, p, i32, p, p, i64, p, p, i64, p, i64, p]),
+    'dae_encode_sparse_dw_add': (C.c_int, [i32, i32, i32, i64, p, i64, p, p]),
+    'dae_triplet_batch_all_det': (C.c_int, [p, i64, i32, p, p, p, i64, p, i32, p, p, i64, p, p]),
+    'dae_triplet_batch_hard_det': (C.c_int, [p, i64, i32, p, p, i64, p, p, p, p]),
+    'dae_triplet_batch_all_rows_det': (C.c_int, [p, i64, i32, i32, i32, p, p, p, i64, p, i32, p, p, i64, p, p]),
+    'dae_triplet_batch_hard_rows_det': (C.c_int, [p, i64, i32, i32, i32, p, p, i64, p, p, p, p]),
+    'dae_triplet_explicit_det': (C.c_int, [p, p, p, i32, i32, i64, f32, p, p, p, p, p, p]),
+    'dae_triplet_loss_sum': (C.c_int, [p, i32, p, p]),
 }
+
+
+def query(name, *args, ctype=C.c_int64):
+    """Call a size query export whose last argument is an output scalar; returns that scalar."""
+    out = ctype(0)
+    call(name, *args, ctypes.addressof(out))
+    return int(out.value)
 
 _lib = None
 

@@ -21,7 +21,7 @@ import torch
 
 from . import utils
 from .. import _cabi
-from ..engine import TrainEngine, DeviceCSR, canonical_csr, check_mining_block_rows
+from ..engine import TrainEngine, DeviceCSR, canonical_csr, check_mining_block_rows, resolve_deterministic
 from .._cabi import STAT, STAT_SLOTS, MAX_TRIPLET_BATCH, MAX_BLOCKED_BATCH
 
 
@@ -31,14 +31,16 @@ class DenoisingAutoencoder(object):
                  dec_act_func='none', loss_func='mean_squared', num_epochs=10, batch_size=10,
                  xavier_init=1, opt='gradient_descent', learning_rate=0.01, momentum=0.5, corr_type='none',
                  corr_frac=0., verbose=True, verbose_step=5, seed=-1, alpha=1, triplet_strategy='batch_all',
-                 device=None, rng_mode='device', W_init=None, mining_block_rows=None):
+                 device=None, rng_mode='device', W_init=None, mining_block_rows=None, deterministic=False):
         """Arguments as in the reference (autoencoder.py:20-45).  Extensions: device ('cuda:N'; default: LOCAL_RANK or 0),
         rng_mode ('device' = Philox mask + device permutation, the default: an epoch of the UCI config is 3 ms of GPU time, the host
         RNG alone would take 6 ms; 'numpy' = the reference's host NumPy RNG stream for corruption and shuffling, drawn one epoch
         ahead on a worker thread -- bit-identical masks and batch order to a seeded reference run), W_init (ndarray F x H
         overriding the Xavier draw), mining_block_rows (None: batch_all / batch_hard hold the B x B similarity matrix, batches up to
         MAX_TRIPLET_BATCH rows; R, a multiple of 128 up to 32768: they mine it R anchor rows at a time in 12 R B bytes, batches up to
-        MAX_BLOCKED_BATCH rows)."""
+        MAX_BLOCKED_BATCH rows), deterministic (True: every sum of the training step runs in a fixed order, so a run with the same seed
+        >= 0, rng_mode, data, build and GPU model reproduces its parameters, losses and transform output bit for bit; slower, one
+        process, tensor-core path only; None: the environment variable DAE_DETERMINISTIC)."""
         self.algo_name = algo_name
         self.model_name = model_name
         self.compress_factor = compress_factor
@@ -85,6 +87,7 @@ class DenoisingAutoencoder(object):
         self.rng_mode = rng_mode
         self.W_init = W_init
         self.mining_block_rows = check_mining_block_rows(mining_block_rows)   # not in parameter.txt: its layout is the reference's
+        self.deterministic = resolve_deterministic(deterministic)              # (nor this)
         self.engine = None
 
     # ------------------------------------------------------------------------------------------------------------------
@@ -106,7 +109,8 @@ class DenoisingAutoencoder(object):
         eng = TrainEngine(n_features, int(self.n_components), enc_act_func=self.enc_act_func,
                           dec_act_func=self.dec_act_func, loss_func=self.loss_func, opt=self.opt,
                           learning_rate=self.learning_rate, momentum=self.momentum, alpha=self.alpha,
-                          triplet_strategy=self._strategy_name(), device=self.device, mining_block_rows=self.mining_block_rows)
+                          triplet_strategy=self._strategy_name(), device=self.device, mining_block_rows=self.mining_block_rows,
+                          deterministic=self.deterministic)
         return eng
 
     def _init_parameters(self, n_features, restore_previous_model):

@@ -75,6 +75,10 @@ class DenoisingAutoencoderTriplet(DenoisingAutoencoder):
         tail = [s0 for s0 in starts if s0 + bs > n]
         use_graph = (os.environ.get('DAE_CUDA_GRAPH', '1') == '1' and self.corr_type != 'salt_and_pepper' and len(full) >= 2)
         perm_buf = torch.zeros(n, dtype=torch.int32, device=eng.device)
+        # DenoisingAutoencoder's condition (rng_mode 'numpy' draws from np.random, seeded in __init__), here only in the deterministic
+        # mode: the default mode's explicit-triplet runs keep the device permutations they always drew
+        if self.deterministic and self.rng_mode == 'device' and self.seed >= 0:
+            torch.manual_seed(self.seed)
         i = -1
         for i in range(self.num_epochs):
             torch.cuda.synchronize(eng.device)

@@ -7,6 +7,7 @@
 // chunks of 128 with masked (zero) entries compacted away, then every thread gathers its 128-bit slice of W[col,:]
 // with read-only vector loads, several rows of W in flight per thread.  W (20 MB at F=10k,H=500) is L2 resident,
 // so the gather runs at L2 bandwidth; HBM only sees the CSR stream, W once, and the E write.
+#include <algorithm>
 #include <cstdlib>
 #include <cuda_bf16.h>
 #include "common.cuh"
@@ -351,7 +352,9 @@ __global__ void __launch_bounds__(1024) col_scan_kernel(const int32_t* __restric
 // addresses of dbh are otherwise hit by every row of the batch), while the rows still progress in parallel.
 constexpr int kRowsPerCta = 4;
 
-template <int ACT>
+// DET (the deterministic mode): the CTA's dbh sum goes to its own row dbh[blockIdx.x * H + h] of a partial buffer instead of an atomic,
+// and the entries are bucketed by det_place_kernel instead.
+template <int ACT, bool DET = false>
 __global__ void __launch_bounds__(32 * kRowsPerCta) encode_bwd_rows_kernel(
     const int64_t* __restrict__ indptr, const int32_t* __restrict__ indices, const float* __restrict__ values,
     const int32_t* __restrict__ rows, int n_rows, int H, float in_scale, const float* __restrict__ E, const float* __restrict__ bh,
@@ -378,8 +381,10 @@ __global__ void __launch_bounds__(32 * kRowsPerCta) encode_bwd_rows_kernel(
     float t = 0.0f;
 #pragma unroll
     for (int w = 0; w < kRowsPerCta; ++w) t += s_part[(int64_t)w * H + h];
-    atomicAdd(dbh + h, t);
+    if constexpr (DET) dbh[(int64_t)blockIdx.x * H + h] = t;
+    else atomicAdd(dbh + h, t);
   }
+  if constexpr (DET) return;
   if (r < n_rows) {
     const int64_t row = rows ? (int64_t)rows[r] : (int64_t)r;
     const int64_t p0 = indptr[row], p1 = indptr[row + 1];
@@ -478,6 +483,178 @@ __global__ void __launch_bounds__(kEncThreads) encode_bwd_gather_kernel(const in
         else if constexpr (VW == 2) atomicAdd(reinterpret_cast<float2*>(wrow + hcol[c]), make_float2(acc[c][0], acc[c][1]));
         else atomicAdd(wrow + hcol[c], acc[c][0]);
       }
+    }
+  }
+}
+
+// ---- deterministic encode backward (DESIGN 4.7) -------------------------------------------------------------------------------------
+// Stable bucketing: the batch rows are cut into T tiles of RT consecutive rows.  (1) every tile counts its entries per column
+// (integer atomics: exact); (2) one thread per column turns its T counts into the tile's first slot in the column's bucket
+// (col_start[c] + the counts of the earlier tiles); (3) one warp per tile walks its rows IN ORDER and hands each entry the next slot of
+// its column.  A canonical CSR row holds a column at most once, so the lanes of one row never share a column.  Each bucket then lists
+// its entries in batch-row order, whatever the timing.
+constexpr int kDbhGroup = 32;
+
+struct DetLayout {
+  int T, RT, CH;          // row tiles, rows per tile, entries per gather chunk
+  int64_t n_chunks, n_cta, n_groups;   // dbh: n_cta row sums of 4-row CTAs, added in groups of kDbhGroup, then the groups
+  int64_t off_start, off_cursor, off_col, off_row, off_val, off_tile, off_dbh, off_colsum, off_parts, off_dbh2, bytes;
+};
+
+static DetLayout det_layout(int n_rows, int F, int H, int64_t cap) {
+  DetLayout L{};
+  const int64_t max_tiles = std::max<int64_t>(1, ((int64_t)1 << 24) / F);      // the tile table stays under 64 MB
+  L.T = (int)std::min<int64_t>((n_rows + 7) / 8, max_tiles);
+  if (L.T < 1) L.T = 1;
+  L.RT = (n_rows + L.T - 1) / L.T;
+  if (L.RT < 1) L.RT = 1;
+  L.T = (n_rows + L.RT - 1) / L.RT;
+  if (L.T < 1) L.T = 1;
+  L.CH = 64;                                                                   // the chunk partials stay under 256 MB
+  while (((cap + L.CH - 1) / L.CH) * 2 * (int64_t)H * 4 > ((int64_t)256 << 20)) L.CH *= 2;
+  L.n_chunks = std::max<int64_t>(1, (cap + L.CH - 1) / L.CH);
+  L.n_cta = (n_rows + kRowsPerCta - 1) / kRowsPerCta;
+  L.n_groups = (L.n_cta + kDbhGroup - 1) / kDbhGroup;
+  auto al = [](int64_t b) { return (b + 255) / 256 * 256; };
+  int64_t o = 0;
+  L.off_start = o; o += al(4 * ((int64_t)F + 1));
+  L.off_cursor = o; o += al(4 * (int64_t)F);
+  L.off_col = o; o += al(4 * cap);
+  L.off_row = o; o += al(4 * cap);
+  L.off_val = o; o += al(4 * cap);
+  L.off_tile = o; o += al(4 * (int64_t)L.T * F);
+  L.off_dbh = o; o += al(4 * std::max<int64_t>(1, L.n_cta) * H);
+  L.off_colsum = o; o += al(4 * (int64_t)F * H);
+  L.off_parts = o; o += al(4 * L.n_chunks * 2 * H);
+  L.off_dbh2 = o; o += al(4 * std::max<int64_t>(1, L.n_groups) * H);
+  L.bytes = o;
+  return L;
+}
+
+// first level of the fixed-order dbh sum: out[g][h] = parts[32 g][h] + parts[32 g + 1][h] + ... (in order); dae_reduce_parts then adds
+// the groups in order.  Two levels keep the serial chain short at large batches (100 000 rows: 782 + 32 adds instead of 25 000).
+__global__ void det_group_sum_kernel(const float* __restrict__ parts, int n_parts, int H, float* __restrict__ out) {
+  const int h = blockIdx.x * blockDim.x + threadIdx.x, g = blockIdx.y;
+  if (h >= H) return;
+  const int p0 = g * kDbhGroup, p1 = min(n_parts, p0 + kDbhGroup);
+  float s = parts[(int64_t)p0 * H + h];
+  for (int p = p0 + 1; p < p1; ++p) s = __fadd_rn(s, parts[(int64_t)p * H + h]);
+  out[(int64_t)g * H + h] = s;
+}
+
+__global__ void det_tile_count_kernel(const int64_t* __restrict__ indptr, const int32_t* __restrict__ indices,
+                                      const float* __restrict__ values, const int32_t* __restrict__ rows, int n_rows, int F, int RT,
+                                      float in_scale, int32_t* __restrict__ tile_cnt) {
+  const int r = (int)((blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5), lane = threadIdx.x & 31;
+  if (r >= n_rows) return;
+  const int64_t row = rows ? (int64_t)rows[r] : (int64_t)r;
+  int32_t* cnt = tile_cnt + (int64_t)(r / RT) * F;
+  for (int64_t p = indptr[row] + lane; p < indptr[row + 1]; p += 32)
+    if (__ldg(values + p) * in_scale != 0.0f) atomicAdd(cnt + __ldg(indices + p), 1);
+}
+
+__global__ void det_tile_scan_kernel(int32_t* __restrict__ tile, int T, int F, const int32_t* __restrict__ col_start) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= F) return;
+  int run = col_start[c];
+  for (int t = 0; t < T; ++t) { const int x = tile[(int64_t)t * F + c]; tile[(int64_t)t * F + c] = run; run += x; }
+}
+
+__global__ void det_place_kernel(const int64_t* __restrict__ indptr, const int32_t* __restrict__ indices, const float* __restrict__ values,
+                                 const int32_t* __restrict__ rows, int n_rows, int F, int RT, int T, float in_scale,
+                                 int32_t* __restrict__ tile, int32_t* __restrict__ ent_col, int32_t* __restrict__ ent_row,
+                                 float* __restrict__ ent_val) {
+  const int t = (int)((blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5), lane = threadIdx.x & 31;
+  if (t >= T) return;
+  int32_t* cur = tile + (int64_t)t * F;
+  const int r1 = min(n_rows, (t + 1) * RT);
+  for (int r = t * RT; r < r1; ++r) {
+    const int64_t row = rows ? (int64_t)rows[r] : (int64_t)r;
+    for (int64_t p = indptr[row] + lane; p < indptr[row + 1]; p += 32) {
+      const float v = __ldg(values + p) * in_scale;
+      if (v != 0.0f) {
+        const int col = __ldg(indices + p);
+        const int slot = cur[col];
+        cur[col] = slot + 1;
+        ent_col[slot] = col; ent_row[slot] = r; ent_val[slot] = v;
+      }
+    }
+    __syncwarp();   // the next row's lanes read the cursors this row advanced
+  }
+}
+
+// Sparse dW in fixed order: chunks of CH consecutive bucketed entries (fixed positions).  Inside a chunk a run of one column is summed
+// in entry (= batch-row) order with separately rounded multiplies and adds.  A run that is its column's whole bucket is stored to
+// colsum[col]; a run cut by a chunk boundary is the chunk's first run (slot 0) or its last (slot 1) and goes to parts[chunk][slot].
+// Every thread walks the same entry list for its own VW columns of H, so any H works and no thread waits for another.
+template <int VW>
+__global__ void __launch_bounds__(kEncThreads) encode_bwd_gather_det_kernel(const int32_t* __restrict__ col_start, int F,
+                                                                            const int32_t* __restrict__ ent_col,
+                                                                            const int32_t* __restrict__ ent_row,
+                                                                            const float* __restrict__ ent_val, int H,
+                                                                            const float* __restrict__ dA, int64_t ldE, int CH,
+                                                                            float* __restrict__ colsum, float* __restrict__ parts) {
+  const int total = col_start[F];
+  for (int64_t chunk = blockIdx.x; chunk * CH < total; chunk += gridDim.x) {
+    const int base = (int)(chunk * CH), end = min(base + CH, total);
+    for (int h0 = threadIdx.x * VW; h0 < H; h0 += kEncThreads * VW) {
+      float acc[VW];
+#pragma unroll
+      for (int k = 0; k < VW; ++k) acc[k] = 0.0f;
+      int cur = __ldg(ent_col + base), a = base;
+      auto flush = [&](int b) {
+        const bool whole = (a == __ldg(col_start + cur)) && (b == __ldg(col_start + cur + 1));
+        float* dst = whole ? colsum + (int64_t)cur * H : parts + (chunk * 2 + (a == base ? 0 : 1)) * H;
+#pragma unroll
+        for (int k = 0; k < VW; ++k) dst[h0 + k] = acc[k];
+      };
+      for (int q0 = base; q0 < end; q0 += 8) {
+        float x[8][VW];
+        float v[8];
+        int cc[8];
+#pragma unroll
+        for (int u = 0; u < 8; ++u) {   // eight rows of dA in flight per thread
+          const int q = min(q0 + u, end - 1);
+          v[u] = __ldg(ent_val + q);
+          cc[u] = __ldg(ent_col + q);
+          ldg_vec<VW>(dA + (int64_t)__ldg(ent_row + q) * ldE + h0, x[u]);
+        }
+#pragma unroll
+        for (int u = 0; u < 8; ++u) {
+          if (q0 + u < end) {
+            if (cc[u] != cur) {
+              flush(q0 + u);
+#pragma unroll
+              for (int k = 0; k < VW; ++k) acc[k] = 0.0f;
+              cur = cc[u];
+              a = q0 + u;
+            }
+#pragma unroll
+            for (int k = 0; k < VW; ++k) acc[k] = __fadd_rn(acc[k], __fmul_rn(v[u], x[u][k]));
+          }
+        }
+      }
+      flush(end);
+    }
+  }
+}
+
+// After the dense dW is in place: dW[c, :] += the column's sparse sum -- colsum[c], or its chunk partials added in chunk order.
+__global__ void encode_sparse_dw_add_kernel(const int32_t* __restrict__ col_start, int F, int H, int CH, const float* __restrict__ colsum,
+                                            const float* __restrict__ parts, float* __restrict__ dW) {
+  for (int c = blockIdx.x; c < F; c += gridDim.x) {
+    const int s = col_start[c], e = col_start[c + 1];
+    if (s == e) continue;
+    const int k0 = s / CH, k1 = (e - 1) / CH;
+    for (int h = threadIdx.x; h < H; h += blockDim.x) {
+      float v;
+      if (k0 == k1) {
+        v = colsum[(int64_t)c * H + h];
+      } else {
+        v = parts[((int64_t)k0 * 2 + (s == k0 * CH ? 0 : 1)) * H + h];
+        for (int k = k0 + 1; k <= k1; ++k) v = __fadd_rn(v, parts[(int64_t)k * 2 * H + h]);
+      }
+      dW[(int64_t)c * H + h] = __fadd_rn(dW[(int64_t)c * H + h], v);
     }
   }
 }
@@ -658,5 +835,74 @@ extern "C" int dae_encode_csr_fwd_hot(const int64_t* indptr, const int32_t* indi
   });
 #undef DAE_HOT
   DAE_CHECK_LAUNCH("dae_encode_csr_fwd_hot");
+  return DAE_OK;
+}
+
+extern "C" int dae_encode_csr_bwd_det_workspace(int32_t n_rows, int32_t F, int32_t H, int64_t cap_nnz, int64_t* bytes) {
+  using namespace dae;
+  DAE_REQUIRE(bytes && n_rows >= 1 && F > 0 && H > 0 && cap_nnz >= 0, "dae_encode_csr_bwd_det_workspace: bad arguments");
+  *bytes = det_layout(n_rows, F, H, cap_nnz).bytes;
+  return DAE_OK;
+}
+
+extern "C" int dae_encode_csr_bwd_det(const int64_t* indptr, const int32_t* indices, const float* values, const int32_t* rows,
+                                      int32_t n_rows, int32_t F, int32_t H, float in_scale, const float* E, const float* bh,
+                                      int32_t enc_act, float* dE, const float* dE_add, int64_t ldE, float* dbh, const int32_t* col_count,
+                                      int64_t cap_nnz, void* workspace, int64_t workspace_bytes, void* stream) {
+  using namespace dae;
+  DAE_REQUIRE(indptr && indices && values && E && bh && dE && dbh && col_count && workspace, "dae_encode_csr_bwd_det: null pointer");
+  DAE_REQUIRE(n_rows >= 1 && F > 0 && H > 0 && ldE >= H && cap_nnz >= 0, "dae_encode_csr_bwd_det: bad shape");
+  const DetLayout L = det_layout(n_rows, F, H, cap_nnz);
+  DAE_REQUIRE(workspace_bytes >= L.bytes, "dae_encode_csr_bwd_det: workspace of %lld bytes, need %lld", (long long)workspace_bytes,
+              (long long)L.bytes);
+  const size_t smem = sizeof(float) * kRowsPerCta * H;
+  DAE_REQUIRE(smem <= 200 * 1024, "dae_encode_csr_bwd_det: H=%d too large", H);
+  cudaStream_t st = (cudaStream_t)stream;
+  uint8_t* w = (uint8_t*)workspace;
+  int32_t* col_start = (int32_t*)(w + L.off_start);
+  int32_t* tile = (int32_t*)(w + L.off_tile);
+  int32_t* ent_col = (int32_t*)(w + L.off_col);
+  int32_t* ent_row = (int32_t*)(w + L.off_row);
+  float* ent_val = (float*)(w + L.off_val);
+  float* dbh_part = (float*)(w + L.off_dbh);
+  col_scan_kernel<<<1, 1024, 0, st>>>(col_count, F, col_start, (int32_t*)(w + L.off_cursor));
+  DAE_CUDA(cudaMemsetAsync(tile, 0, sizeof(int32_t) * (size_t)L.T * F, st));
+  det_tile_count_kernel<<<(n_rows + 7) / 8, 256, 0, st>>>(indptr, indices, values, rows, n_rows, F, L.RT, in_scale, tile);
+  det_tile_scan_kernel<<<(F + 255) / 256, 256, 0, st>>>(tile, L.T, F, col_start);
+  det_place_kernel<<<(L.T + 3) / 4, 128, 0, st>>>(indptr, indices, values, rows, n_rows, F, L.RT, L.T, in_scale, tile, ent_col, ent_row, ent_val);
+  DAE_DISPATCH_ACT(enc_act, ACT, {
+    auto kern = encode_bwd_rows_kernel<ACT, true>;
+    if (smem > 48 * 1024) DAE_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    kern<<<(unsigned)L.n_cta, 32 * kRowsPerCta, smem, st>>>(indptr, indices, values, rows, n_rows, H, in_scale, E, bh, dE, dE_add, ldE,
+                                                            dbh_part, nullptr, nullptr, nullptr, nullptr);
+  });
+  float* dbh_group = (float*)(w + L.off_dbh2);   // dbh = the CTAs' sums in groups of kDbhGroup, then the groups, each level in order
+  det_group_sum_kernel<<<dim3((H + 127) / 128, (unsigned)L.n_groups), 128, 0, st>>>(dbh_part, (int)L.n_cta, H, dbh_group);
+  int rc = dae_reduce_parts(dbh_group, (int32_t)L.n_groups, H, dbh, stream);
+  if (rc) return rc;
+  const int vw = (H % 4 == 0 && ldE % 4 == 0 && ((uintptr_t)dE & 15) == 0) ? 4 : ((H % 2 == 0 && ldE % 2 == 0 && ((uintptr_t)dE & 7) == 0) ? 2 : 1);
+  const int64_t want = L.n_chunks;
+  const int grid = (int)std::min<int64_t>(want, (int64_t)sm_count() * 16);
+  float* colsum = (float*)(w + L.off_colsum);
+  float* parts = (float*)(w + L.off_parts);
+  if (vw == 4) encode_bwd_gather_det_kernel<4><<<grid, kEncThreads, 0, st>>>(col_start, F, ent_col, ent_row, ent_val, H, dE, ldE, L.CH, colsum, parts);
+  else if (vw == 2) encode_bwd_gather_det_kernel<2><<<grid, kEncThreads, 0, st>>>(col_start, F, ent_col, ent_row, ent_val, H, dE, ldE, L.CH, colsum, parts);
+  else encode_bwd_gather_det_kernel<1><<<grid, kEncThreads, 0, st>>>(col_start, F, ent_col, ent_row, ent_val, H, dE, ldE, L.CH, colsum, parts);
+  DAE_CHECK_LAUNCH("dae_encode_csr_bwd_det");
+  return DAE_OK;
+}
+
+extern "C" int dae_encode_sparse_dw_add(int32_t n_rows, int32_t F, int32_t H, int64_t cap_nnz, const void* workspace, int64_t workspace_bytes,
+                                        float* dW, void* stream) {
+  using namespace dae;
+  DAE_REQUIRE(workspace && dW && n_rows >= 1 && F > 0 && H > 0 && cap_nnz >= 0, "dae_encode_sparse_dw_add: bad arguments");
+  const DetLayout L = det_layout(n_rows, F, H, cap_nnz);
+  DAE_REQUIRE(workspace_bytes >= L.bytes, "dae_encode_sparse_dw_add: workspace of %lld bytes, need %lld", (long long)workspace_bytes,
+              (long long)L.bytes);
+  const uint8_t* w = (const uint8_t*)workspace;
+  encode_sparse_dw_add_kernel<<<std::min(F, 65535), 128, 0, (cudaStream_t)stream>>>((const int32_t*)(w + L.off_start), F, H, L.CH,
+                                                                                   (const float*)(w + L.off_colsum),
+                                                                                   (const float*)(w + L.off_parts), dW);
+  DAE_CHECK_LAUNCH("dae_encode_sparse_dw_add");
   return DAE_OK;
 }

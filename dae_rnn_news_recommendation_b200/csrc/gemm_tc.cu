@@ -199,6 +199,10 @@ struct GemmParams {
   __nv_bfloat16* dz_hi; __nv_bfloat16* dz_lo; int64_t ld_dz;
   float* row_loss_part;  // [M] row losses, accumulated with fp32 atomics (zeroed by the launcher)
   const int32_t* tile_ptr; // [M x (2 * n_tiles_n + 1)]: first CSR entry of every half tile, relative to the row start
+  // deterministic mode (see DESIGN 4.7)
+  float* sk_ws;          // stream-K: a segment that covers part of a tile stores it to slot [cta][first ? 0 : 1] of this
+                         // [n_cta][2][BLOCK_M][BLOCK_N] workspace instead of adding it to C; sk_fixup_kernel sums the slots in k order
+  int loss_parts;        // fused decode: row_loss_part is [2 * n_tiles_n][M], one store per (half tile, row) instead of an atomic
 };
 
 // Work distribution, walked identically by every warpgroup of a CTA.
@@ -535,9 +539,14 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_bf16x3_kernel(const __grid_c
     for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] = 0.0f;
     int stage = 0; uint32_t phase = 0;
     int mb, nb, kb0, kb1;
+    int seg = 0;                             // segments of this CTA so far (deterministic stream-K: slot of a partial tile)
     while (sched.next(mb, nb, kb0, kb1)) {
       if (PAIR) mb = mb * 2 + (int)crank;     // this CTA's 128-row m tile of the pair
       mma_work_item<BLOCK_N, STAGES, PAIR, MAJ, BK>(acc, p, smem, full_bar, empty_bar, wg, lane, crank, stage, phase, kb0, kb1);
+      float* ws_tile = nullptr;              // partial tile of the deterministic mode: goes to the CTA's workspace slot
+      if (p.sk_ws != nullptr && !(kb0 == 0 && kb1 == sched.kb_total))
+        ws_tile = p.sk_ws + ((int64_t)blockIdx.x * 2 + (seg == 0 ? 0 : 1)) * (BLOCK_M * BLOCK_N);
+      ++seg;
 
       // accumulators -> staging rows (the previous tile's epilogue of this warpgroup must be done with them)
       named_bar_sync(1 + wg, 128);
@@ -557,6 +566,16 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_bf16x3_kernel(const __grid_c
 #pragma unroll 1
       for (int c = 0; c < HALF_N / 16; ++c) {
         const int nc = n0 + c * 16;   // first column of this 16-wide chunk
+        if (ws_tile != nullptr) {     // deterministic stream-K: the whole 32 x 16 block, scaled, into the slot (rows of 64 B)
+          const int rsub = lane >> 4, csub = lane & 15;
+          float* dst = ws_tile + (int64_t)(quarter * 32) * BLOCK_N + half * HALF_N + c * 16 + csub;
+#pragma unroll 4
+          for (int i = 0; i < 16; ++i) {
+            const int rr = 2 * i + rsub;
+            dst[(int64_t)rr * BLOCK_N] = p.alpha * tr[rr * SROW + c * 16 + csub];
+          }
+          continue;
+        }
         const bool interior = vec_ok && (m_base + 32 <= p.M) && (nc + 16 <= p.n_store) && (p.special_col < nc || p.special_col >= nc + 16);
         if (interior) {               // fast path: 8 rows x 64 B per store instruction, 128-bit accesses
           const int rsub = lane >> 2, c4 = (lane & 3) * 4;
@@ -801,7 +820,11 @@ __global__ void __launch_bounds__(kDecodeThreads, 1) decode_fused_kernel(const _
       }
       if (lane == 0) mbar_arrive(&drained_bar[h]);   // this warp's staging rows may be overwritten (the loop ends in __syncwarp)
       tphase ^= 1;
-      if (m < p.M) atomicAdd(p.row_loss_part + m, (LOSS == DAE_LOSS_CE) ? lsum * 0.6931471805599453f : lsum);  // 2 * tiles_n partials per row
+      if (m < p.M) {   // 2 * tiles_n partials per row
+        const float l = (LOSS == DAE_LOSS_CE) ? lsum * 0.6931471805599453f : lsum;
+        if (p.loss_parts) p.row_loss_part[(int64_t)(nb * kParts + half) * p.M + m] = l;
+        else atomicAdd(p.row_loss_part + m, l);
+      }
     }
   }
 }
@@ -1272,7 +1295,7 @@ static int g_pair_mode = -1;   // -1 (default) and 0: never; 1: whenever the sha
 static int g_lean = 0;         // 1: 128 x 64 tiles with 2-stage rings for dae_gemm_bf16x3 (~130 KB of shared memory instead of ~195 KB)
 
 template <int BLOCK_N, int STAGES, int PAIR, int MAJ, int BK = BLOCK_K>
-static int launch_gemm_maj(const Operand& A, const Operand& B, GemmParams p, cudaStream_t st) {
+static int launch_gemm_maj(const Operand& A, const Operand& B, GemmParams p, cudaStream_t st, int* grid_out = nullptr) {
   CUtensorMap ta_hi, ta_lo, tb_hi, tb_lo;
   int rc;
   constexpr int B_ROWS = PAIR ? BLOCK_N / 2 : BLOCK_N;   // n rows of the B tile one CTA loads
@@ -1320,6 +1343,7 @@ static int launch_gemm_maj(const Operand& A, const Operand& B, GemmParams p, cud
     const int items = tiles_m * tiles_n * p.k_splits;
     n = items < slots ? items : slots;
   }
+  if (grid_out) *grid_out = n;
   if (!PAIR) {
     kern<<<n, kThreads, smem, st>>>(ta_hi, ta_lo, tb_hi, tb_lo, tat_hi, tat_lo, p);
   } else {
@@ -1336,12 +1360,57 @@ static int launch_gemm_maj(const Operand& A, const Operand& B, GemmParams p, cud
 
 // the plain GEMMs take any majorness; (A + A^T).B goes through launch_gemm_maj directly
 template <int BLOCK_N, int STAGES, int PAIR, int BK = BLOCK_K>
-static int launch_gemm(const Operand& A, const Operand& B, GemmParams p, cudaStream_t st) {
-  if (!A.mn_major && !B.mn_major) return launch_gemm_maj<BLOCK_N, STAGES, PAIR, 0, BK>(A, B, p, st);
-  if (A.mn_major && !B.mn_major) return launch_gemm_maj<BLOCK_N, STAGES, PAIR, 1, BK>(A, B, p, st);
-  if (!A.mn_major) return launch_gemm_maj<BLOCK_N, STAGES, PAIR, 2, BK>(A, B, p, st);
-  return launch_gemm_maj<BLOCK_N, STAGES, PAIR, 3, BK>(A, B, p, st);
+static int launch_gemm(const Operand& A, const Operand& B, GemmParams p, cudaStream_t st, int* grid_out = nullptr) {
+  if (!A.mn_major && !B.mn_major) return launch_gemm_maj<BLOCK_N, STAGES, PAIR, 0, BK>(A, B, p, st, grid_out);
+  if (A.mn_major && !B.mn_major) return launch_gemm_maj<BLOCK_N, STAGES, PAIR, 1, BK>(A, B, p, st, grid_out);
+  if (!A.mn_major) return launch_gemm_maj<BLOCK_N, STAGES, PAIR, 2, BK>(A, B, p, st, grid_out);
+  return launch_gemm_maj<BLOCK_N, STAGES, PAIR, 3, BK>(A, B, p, st, grid_out);
 }
+
+// Deterministic stream-K, after the GEMM: kFixupSlices CTAs per output tile, each over a slice of its rows.  A tile that one CTA
+// covered was stored by that CTA; a tile cut between CTAs c0 < c1 < ... is the sum of their workspace slots in that (= k) order,
+// stored (or added, C += ...) once.  The CTA
+// ranges are recomputed exactly as Sched::init cuts them (u_c = c U / n_cta); CTA c's segment in the tile is its first one (slot 0)
+// iff its range starts inside the tile.
+constexpr int kMaxFixupCtas = 1024;   // CTAs of one stream-K launch (at most one per SM) the fixup can list for a tile
+constexpr int kFixupSlices = 16;      // CTAs per tile: the slot reads of a split tile spread over the SMs (latency, not bandwidth)
+
+template <int BLOCK_N>
+__global__ void __launch_bounds__(256) sk_fixup_kernel(const GemmParams p, int tiles_m, int tiles, int kb_total, int n_cta) {
+  __shared__ int s_slot[kMaxFixupCtas];   // workspace slots of the CTAs that cover this tile, in k order
+  __shared__ int s_n;
+  const int t = blockIdx.x;
+  if (threadIdx.x == 0) {   // the CTA ranges are found once per tile, not per element (64-bit divisions)
+    const long long U = (long long)tiles * kb_total, T0 = (long long)t * kb_total, T1 = T0 + kb_total;
+    auto u_of = [&](int c) { return (long long)c * U / n_cta; };
+    int c0 = (int)(T0 * n_cta / U);
+    while (c0 + 1 < n_cta && u_of(c0 + 1) <= T0) ++c0;
+    while (c0 > 0 && u_of(c0) > T0) --c0;
+    int n = 0;
+    if (u_of(c0 + 1) < T1) {   // otherwise one CTA covered the whole tile and stored it
+      for (int c = c0; c < n_cta && u_of(c) < T1; ++c) {
+        if (u_of(c + 1) == u_of(c)) continue;   // an empty range has no segment
+        s_slot[n++] = 2 * c + (u_of(c) >= T0 ? 0 : 1);
+      }
+    }
+    s_n = n;
+  }
+  __syncthreads();
+  const int n = s_n;
+  if (n == 0) return;
+  const int mb = t % tiles_m, nb = t / tiles_m;
+  constexpr int kPer = BLOCK_M * BLOCK_N / kFixupSlices;   // blockIdx.y: one slice of 128 / kFixupSlices rows of the tile
+  for (int e = blockIdx.y * kPer + threadIdx.x; e < (blockIdx.y + 1) * kPer; e += blockDim.x) {
+    const int m = mb * BLOCK_M + e / BLOCK_N, col = nb * BLOCK_N + e % BLOCK_N;
+    if (m >= p.M || (col != p.special_col && col >= p.n_store)) continue;
+    float s = p.sk_ws[(int64_t)s_slot[0] * (BLOCK_M * BLOCK_N) + e];
+    for (int i = 1; i < n; ++i) s = s + p.sk_ws[(int64_t)s_slot[i] * (BLOCK_M * BLOCK_N) + e];
+    float* dst = (col == p.special_col) ? p.special_out + m : p.C + (int64_t)m * p.ldc + col;
+    *dst = p.atomic ? *dst + s : s;   // (atomic = accumulate here: this is the only writer of the element)
+  }
+}
+
+static int64_t sk_workspace_bytes() { return (int64_t)2 * sm_count() * BLOCK_M * 128 * (int64_t)sizeof(float); }
 
 // the fused decode: E [M x K] and W [N x K], both K-major; one persistent CTA per SM over the 128 x 128 output tiles
 template <int ACT, int LOSS>
@@ -1530,6 +1599,74 @@ extern "C" int dae_gemm_sym_bf16x3(int32_t M, int32_t N, float alpha, const void
   return DAE_OK;
 }
 
+// ---- deterministic variants: the same schedules and main loops; partial stream-K tiles go through the workspace and sk_fixup_kernel
+extern "C" int dae_gemm_det_workspace(int64_t* bytes) {
+  DAE_REQUIRE(bytes, "dae_gemm_det_workspace: null pointer");
+  *bytes = sk_workspace_bytes();
+  return DAE_OK;
+}
+
+extern "C" int dae_gemm_bf16x3_det(int32_t M, int32_t N, int32_t K, float alpha, const void* a_hi, const void* a_lo, int64_t lda,
+                                   int32_t a_mn_major, const void* b_hi, const void* b_lo, int64_t ldb, int32_t b_mn_major, float* C,
+                                   int64_t ldc, int32_t n_store, int32_t special_col, float* special_out, int32_t k_splits,
+                                   int32_t accumulate, void* workspace, int64_t workspace_bytes, void* stream) {
+  DAE_REQUIRE(a_hi && a_lo && b_hi && b_lo && C && M > 0 && N > 0 && K > 0, "dae_gemm_bf16x3_det: bad arguments");
+  DAE_REQUIRE(lda % 8 == 0 && ldb % 8 == 0, "dae_gemm_bf16x3_det: operand leading dimensions must be multiples of 8 (TMA 16-byte strides)");
+  DAE_REQUIRE(((uintptr_t)a_hi | (uintptr_t)a_lo | (uintptr_t)b_hi | (uintptr_t)b_lo) % 16 == 0, "dae_gemm_bf16x3_det: operands must be 16-byte aligned");
+  DAE_REQUIRE(k_splits == 1 || k_splits == -1, "dae_gemm_bf16x3_det: k_splits must be 1 or -1 (stream-K), got %d", k_splits);
+  DAE_REQUIRE(workspace && workspace_bytes >= sk_workspace_bytes(), "dae_gemm_bf16x3_det: workspace of %lld bytes, need %lld",
+              (long long)workspace_bytes, (long long)sk_workspace_bytes());
+  cudaStream_t st = (cudaStream_t)stream;
+  if (n_store <= 0 || n_store > N) n_store = N;
+  const int tm = (M + 127) / 128, tn = (N + 127) / 128;
+  const int stream_k = (k_splits < 0 && (tm * tn) % sm_count() != 0) ? 1 : 0;   // the choice of dae_gemm_bf16x3
+  GemmParams p{};
+  p.M = M; p.N = N; p.K = K; p.k_splits = 1; p.stream_k = stream_k; p.atomic = accumulate ? 1 : 0; p.alpha = alpha;
+  p.C = C; p.ldc = ldc; p.n_store = n_store;
+  p.special_col = (special_out ? special_col : -1); p.special_out = special_out;
+  Operand A{a_hi, a_lo, lda, a_mn_major}, B{b_hi, b_lo, ldb, b_mn_major};
+  int rc;
+  if (stream_k) {
+    p.sk_ws = (float*)workspace;
+    int n = 0;
+    if ((rc = launch_gemm<128, 4, 0, 32>(A, B, p, st, &n))) return rc;
+    DAE_REQUIRE(n <= kMaxFixupCtas, "dae_gemm_bf16x3_det: %d stream-K CTAs exceed the fixup's %d", n, kMaxFixupCtas);
+    sk_fixup_kernel<128><<<dim3(tm * tn, kFixupSlices), 256, 0, st>>>(p, tm, tm * tn, (K + 31) / 32, n);
+  } else {   // whole tiles: every element has one writer
+    const int sms = sm_count(), tn64 = (N + 63) / 64;
+    const float cost128 = 2.0f * (float)((tm * tn + sms - 1) / sms), cost64 = 1.1f * (float)((tm * tn64 + sms - 1) / sms);
+    rc = (cost64 < cost128) ? launch_gemm<64, 3, 0>(A, B, p, st) : launch_gemm<128, 2, 0>(A, B, p, st);
+    if (rc) return rc;
+  }
+  DAE_CHECK_LAUNCH("dae_gemm_bf16x3_det");
+  return DAE_OK;
+}
+
+extern "C" int dae_gemm_sym_bf16x3_det(int32_t M, int32_t N, float alpha, const void* g_hi, const void* g_lo, int64_t ldg, const void* b_hi,
+                                       const void* b_lo, int64_t ldb, float* C, int64_t ldc, int32_t accumulate, void* workspace,
+                                       int64_t workspace_bytes, void* stream) {
+  DAE_REQUIRE(g_hi && g_lo && b_hi && b_lo && C && M > 0 && N > 0, "dae_gemm_sym_bf16x3_det: bad arguments");
+  DAE_REQUIRE(ldg % 8 == 0 && ldb % 8 == 0 && ldg >= M && ldb >= N, "dae_gemm_sym_bf16x3_det: leading dimensions must be multiples of 8 and cover the matrices");
+  DAE_REQUIRE(((uintptr_t)g_hi | (uintptr_t)g_lo | (uintptr_t)b_hi | (uintptr_t)b_lo) % 16 == 0, "dae_gemm_sym_bf16x3_det: operands must be 16-byte aligned");
+  DAE_REQUIRE(workspace && workspace_bytes >= sk_workspace_bytes(), "dae_gemm_sym_bf16x3_det: workspace of %lld bytes, need %lld",
+              (long long)workspace_bytes, (long long)sk_workspace_bytes());
+  cudaStream_t st = (cudaStream_t)stream;
+  GemmParams p{};
+  const int kb_half = (M + BLOCK_K - 1) / BLOCK_K;
+  p.M = M; p.N = N; p.K = 2 * kb_half * BLOCK_K; p.k_splits = 1; p.stream_k = 1; p.atomic = accumulate ? 1 : 0; p.alpha = alpha;
+  p.C = C; p.ldc = ldc; p.n_store = N; p.special_col = -1; p.special_out = nullptr; p.a_sym_kb = kb_half;
+  p.sk_ws = (float*)workspace;
+  Operand A{g_hi, g_lo, ldg, 0}, B{b_hi, b_lo, ldb, 1};
+  int n = 0;
+  int rc = launch_gemm_maj<128, 2, 0, 6>(A, B, p, st, &n);
+  if (rc) return rc;
+  DAE_REQUIRE(n <= kMaxFixupCtas, "dae_gemm_sym_bf16x3_det: %d stream-K CTAs exceed the fixup's %d", n, kMaxFixupCtas);
+  const int tm = (M + 127) / 128, tn = (N + 127) / 128;
+  sk_fixup_kernel<128><<<dim3(tm * tn, kFixupSlices), 256, 0, st>>>(p, tm, tm * tn, 2 * kb_half, n);
+  DAE_CHECK_LAUNCH("dae_gemm_sym_bf16x3_det");
+  return DAE_OK;
+}
+
 extern "C" int dae_decode_prepare(int32_t Brows, int32_t F, const int64_t* indptr, const int32_t* indices, const int32_t* rows,
                                   float* row_loss_part, int32_t* tile_ptr, void* stream) {
   DAE_REQUIRE(Brows > 0 && F > 0 && indptr && indices && row_loss_part && tile_ptr, "dae_decode_prepare: bad arguments");
@@ -1576,6 +1713,49 @@ extern "C" int dae_decode_fused_bf16x3(int32_t Brows, int32_t F, int32_t K, cons
 #undef DAE_DEC
   if (rc) return rc;
   DAE_CHECK_LAUNCH("dae_decode_fused_bf16x3");
+  return DAE_OK;
+}
+
+extern "C" int dae_decode_loss_parts(int32_t F, int32_t* n_parts) {
+  DAE_REQUIRE(F > 0 && n_parts, "dae_decode_loss_parts: bad arguments");
+  *n_parts = 2 * ((F + kDecodeN - 1) / kDecodeN);
+  return DAE_OK;
+}
+
+extern "C" int dae_decode_fused_bf16x3_det(int32_t Brows, int32_t F, int32_t K, const void* e_hi, const void* e_lo, int64_t lde,
+                                           const void* w_hi, const void* w_lo, int64_t ldw, const int64_t* indptr, const int32_t* indices,
+                                           const float* values, const int32_t* rows, const float* bv, int32_t dec_act, int32_t loss_func,
+                                           const float* weight, const double* stats, void* dz_hi, void* dz_lo, int64_t ld_dz,
+                                           float* row_loss_parts, int32_t* tile_ptr, int32_t prepared, void* stream) {
+  DAE_REQUIRE(e_hi && e_lo && w_hi && w_lo && indptr && indices && values && bv && stats && dz_hi && dz_lo && row_loss_parts && tile_ptr,
+              "dae_decode_fused_bf16x3_det: null pointer");
+  DAE_REQUIRE(loss_func == DAE_LOSS_CE || loss_func == DAE_LOSS_MSE, "dae_decode_fused_bf16x3_det: cosine loss uses the unfused path");
+  DAE_REQUIRE(lde % 8 == 0 && ldw % 8 == 0 && ld_dz % 32 == 0 && ld_dz >= F, "dae_decode_fused_bf16x3_det: bad leading dimensions");
+  cudaStream_t st = (cudaStream_t)stream;
+  GemmParams p{};
+  p.M = Brows; p.N = F; p.K = K; p.k_splits = 1; p.alpha = 1.0f; p.special_col = -1;
+  p.indptr = indptr; p.indices = indices; p.values = values; p.rows = rows; p.bv = bv; p.weight = weight; p.stats = stats;
+  p.dz_hi = (__nv_bfloat16*)dz_hi; p.dz_lo = (__nv_bfloat16*)dz_lo; p.ld_dz = ld_dz; p.row_loss_part = row_loss_parts;
+  p.tile_ptr = tile_ptr; p.loss_parts = 1;
+  if (!prepared) {   // (its zeroing of the first Brows floats is harmless: every part is stored)
+    int rc0 = dae_decode_prepare(Brows, F, indptr, indices, rows, row_loss_parts, tile_ptr, stream);
+    if (rc0) return rc0;
+  }
+  Operand A{e_hi, e_lo, lde, 0}, B{w_hi, w_lo, ldw, 0};
+  int rc = 0;
+#define DAE_DEC(ACT, LOSS) rc = launch_decode<ACT, LOSS>(A, B, p, st)
+  if (loss_func == DAE_LOSS_CE) {
+    if (dec_act == DAE_ACT_SIGMOID) DAE_DEC(DAE_ACT_SIGMOID, DAE_LOSS_CE);
+    else if (dec_act == DAE_ACT_TANH) DAE_DEC(DAE_ACT_TANH, DAE_LOSS_CE);
+    else DAE_DEC(DAE_ACT_NONE, DAE_LOSS_CE);
+  } else {
+    if (dec_act == DAE_ACT_SIGMOID) DAE_DEC(DAE_ACT_SIGMOID, DAE_LOSS_MSE);
+    else if (dec_act == DAE_ACT_TANH) DAE_DEC(DAE_ACT_TANH, DAE_LOSS_MSE);
+    else DAE_DEC(DAE_ACT_NONE, DAE_LOSS_MSE);
+  }
+#undef DAE_DEC
+  if (rc) return rc;
+  DAE_CHECK_LAUNCH("dae_decode_fused_bf16x3_det");
   return DAE_OK;
 }
 

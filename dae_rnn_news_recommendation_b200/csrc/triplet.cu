@@ -182,7 +182,8 @@ __global__ void __launch_bounds__(kTripThreads) triplet_batch_all_kernel(const f
                                                                          const int32_t* __restrict__ seg_hi, float* __restrict__ G,
                                                                          int64_t ldg, double* __restrict__ stats, int Pj_max, int Pk_max,
                                                                          int pos_only, __nv_bfloat16* __restrict__ g_hi,
-                                                                         __nv_bfloat16* __restrict__ g_lo, int64_t ld_split) {
+                                                                         __nv_bfloat16* __restrict__ g_lo, int64_t ld_split,
+                                                                         double* __restrict__ loss_slots) {
   extern __shared__ __align__(16) float smem[];
   __shared__ float red_f[32];
   __shared__ double red_d[32];
@@ -195,6 +196,7 @@ __global__ void __launch_bounds__(kTripThreads) triplet_batch_all_kernel(const f
   float* grow = G + (int64_t)i * ldg;
 
   if (nj <= 1 || nk == 0) {  // no valid triplet with this anchor
+    if (loss_slots && tid == 0) loss_slots[i] = 0.0;   // (deterministic mode: its slot adds 0, as the atomic path does)
     for (int c = tid; c < B; c += kTripThreads) {
       grow[c] = 0.0f;
       if (g_hi) { g_hi[(int64_t)i * ld_split + c] = __float2bfloat16_rn(0.0f); g_lo[(int64_t)i * ld_split + c] = __float2bfloat16_rn(0.0f); }
@@ -270,9 +272,9 @@ __global__ void __launch_bounds__(kTripThreads) triplet_batch_all_kernel(const f
   }
   const double lsum = block_sum((double)lacc * (double)kLn2, red_d);
   const double psum = block_sum((double)npos, red_d);
-  if (tid == 0) {
-    atomicAdd(stats + DAE_STAT_TRIPLET_SUM, lsum);
-    atomicAdd(stats + DAE_STAT_NUM, psum);
+  if (tid == 0) {   // loss_slots (deterministic mode): the anchor's loss goes to its own slot, summed in anchor order later
+    if (loss_slots) loss_slots[blockIdx.x] = lsum; else atomicAdd(stats + DAE_STAT_TRIPLET_SUM, lsum);
+    atomicAdd(stats + DAE_STAT_NUM, psum);   // an integer count: exact in any order
   }
 }
 
@@ -296,7 +298,8 @@ __global__ void __launch_bounds__(kTripThreads) triplet_batch_all_tiled_kernel(c
                                                                                const int32_t* __restrict__ seg_hi, float* G, int64_t ldg,
                                                                                double* __restrict__ stats, int pos_only,
                                                                                __nv_bfloat16* __restrict__ g_hi,
-                                                                               __nv_bfloat16* __restrict__ g_lo, int64_t ld_split) {
+                                                                               __nv_bfloat16* __restrict__ g_lo, int64_t ld_split,
+                                                                               double* __restrict__ loss_slots) {
   __shared__ __align__(16) float sj[kChunkJ];
   __shared__ __align__(16) float uj[kChunkJ];
   __shared__ __align__(16) float gj[kChunkJ];
@@ -314,6 +317,7 @@ __global__ void __launch_bounds__(kTripThreads) triplet_batch_all_tiled_kernel(c
   float* grow = G + (int64_t)r * ldg;
 
   if (nj <= 1 || nk == 0) {
+    if (loss_slots && tid == 0) loss_slots[i] = 0.0;   // (deterministic mode: its slot adds 0, as the atomic path does)
     for (int c = tid; c < B; c += kTripThreads) {
       grow[c] = 0.0f;
       if (g_hi) { g_hi[(int64_t)r * ld_split + c] = __float2bfloat16_rn(0.0f); g_lo[(int64_t)r * ld_split + c] = __float2bfloat16_rn(0.0f); }
@@ -404,9 +408,9 @@ __global__ void __launch_bounds__(kTripThreads) triplet_batch_all_tiled_kernel(c
   }
   const double ls = block_sum(lsum * (double)kLn2, red_d);
   const double ps = block_sum((double)npos, red_d);
-  if (tid == 0) {
-    atomicAdd(stats + DAE_STAT_TRIPLET_SUM, ls);
-    atomicAdd(stats + DAE_STAT_NUM, ps);
+  if (tid == 0) {   // loss_slots (deterministic mode): the anchor's loss goes to its own slot, summed in anchor order later
+    if (loss_slots) loss_slots[row0 + (int64_t)blockIdx.x] = ls; else atomicAdd(stats + DAE_STAT_TRIPLET_SUM, ls);
+    atomicAdd(stats + DAE_STAT_NUM, ps);     // an integer count: exact in any order
   }
 }
 
@@ -431,7 +435,7 @@ __device__ __forceinline__ float block_max(float v, float* red) {
 __global__ void __launch_bounds__(kHardThreads) triplet_batch_hard_kernel(const float* __restrict__ S, int64_t lds, int row0, int B,
                                                                           const float* __restrict__ labels, float* __restrict__ G,
                                                                           int64_t ldg, float* __restrict__ weight,
-                                                                          double* __restrict__ stats) {
+                                                                          double* __restrict__ stats, double* __restrict__ loss_slots) {
   __shared__ float red[32];
   __shared__ float redi[32];
   const int a = row0 + (int)blockIdx.x, tid = threadIdx.x;
@@ -492,8 +496,9 @@ __global__ void __launch_bounds__(kHardThreads) triplet_batch_hard_kernel(const 
     }
     grow[c] = g;
   }
+  if (tid == 0 && loss_slots) loss_slots[a] = active ? (double)(fmaxf(td, 0.0f) + log1pf(expf(-td))) : 0.0;
   if (tid == 0 && active) {
-    atomicAdd(stats + DAE_STAT_TRIPLET_SUM, (double)(fmaxf(td, 0.0f) + log1pf(expf(-td))));  // softplus(td), td > 0
+    if (!loss_slots) atomicAdd(stats + DAE_STAT_TRIPLET_SUM, (double)(fmaxf(td, 0.0f) + log1pf(expf(-td))));  // softplus(td), td > 0
     atomicAdd(stats + DAE_STAT_N_ACTIVE, 1.0);
   }
 }
@@ -537,7 +542,7 @@ __global__ void triplet_hard_finish_kernel(const float* __restrict__ weight, int
 // explicit triplets: one warp per row
 __global__ void triplet_explicit_kernel(const float* __restrict__ E, const float* __restrict__ Ep, const float* __restrict__ En,
                                         int B, int H, int64_t ld, float alpha, float* __restrict__ dE, float* __restrict__ dEp,
-                                        float* __restrict__ dEn, double* __restrict__ stats) {
+                                        float* __restrict__ dEn, double* __restrict__ stats, double* __restrict__ loss_slots) {
   const int lane = threadIdx.x & 31;
   const int r = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (r >= B) return;
@@ -557,7 +562,7 @@ __global__ void triplet_explicit_kernel(const float* __restrict__ E, const float
     dEp[(int64_t)r * ld + h] += -c * ev;
     dEn[(int64_t)r * ld + h] += c * ev;
   }
-  if (lane == 0) atomicAdd(stats + DAE_STAT_TRIPLET_SUM, (double)sp);
+  if (lane == 0) { if (loss_slots) loss_slots[r] = (double)sp; else atomicAdd(stats + DAE_STAT_TRIPLET_SUM, (double)sp); }
   if (r == 0 && lane == 0) stats[DAE_STAT_N_ACTIVE] = (double)B;
 }
 
@@ -571,8 +576,8 @@ extern "C" int dae_triplet_config(int32_t force_tiled) {
   return DAE_OK;
 }
 
-extern "C" int dae_triplet_batch_all(const float* S, int64_t lds, int32_t B, const int32_t* seg_lo, const int32_t* seg_hi, float* G,
-                                     int64_t ldg, double* stats, int32_t pos_only, void* g_hi, void* g_lo, int64_t ld_split, void* stream) {
+static int dae_triplet_batch_all_impl(const float* S, int64_t lds, int32_t B, const int32_t* seg_lo, const int32_t* seg_hi, float* G,
+                                     int64_t ldg, double* stats, int32_t pos_only, void* g_hi, void* g_lo, int64_t ld_split, void* stream, double* loss_slots) {
   using namespace dae;
   DAE_REQUIRE(S && seg_lo && seg_hi && G && stats && B >= 1 && lds >= B && ldg >= B, "dae_triplet_batch_all: bad arguments");
   DAE_REQUIRE(B <= DAE_MAX_TRIPLET_BATCH, "dae_triplet_batch_all: B <= %d rows, the cap of the B x B mining buffers (got %d)",
@@ -581,7 +586,7 @@ extern "C" int dae_triplet_batch_all(const float* S, int64_t lds, int32_t B, con
   cudaStream_t st = (cudaStream_t)stream;
   if (B > kSmemSweepMaxB || g_force_tiled) {
     triplet_batch_all_tiled_kernel<<<B, kTripThreads, 0, st>>>(S, lds, 0, B, seg_lo, seg_hi, G, ldg, stats, pos_only, (__nv_bfloat16*)g_hi,
-                                                               (__nv_bfloat16*)g_lo, ld_split);
+                                                               (__nv_bfloat16*)g_lo, ld_split, loss_slots);
     DAE_CHECK_LAUNCH("dae_triplet_batch_all(tiled)");
     return DAE_OK;
   }
@@ -599,27 +604,27 @@ extern "C" int dae_triplet_batch_all(const float* S, int64_t lds, int32_t B, con
     }
   }
   triplet_batch_all_kernel<<<B, kTripThreads, smem, st>>>(S, lds, B, seg_lo, seg_hi, G, ldg, stats, Pj, Pk, pos_only, (__nv_bfloat16*)g_hi,
-                                                          (__nv_bfloat16*)g_lo, ld_split);
+                                                          (__nv_bfloat16*)g_lo, ld_split, loss_slots);
   DAE_CHECK_LAUNCH("dae_triplet_batch_all");
   return DAE_OK;
 }
 
-extern "C" int dae_triplet_batch_hard(const float* S, int64_t lds, int32_t B, const float* labels, float* G, int64_t ldg,
-                                      float* weight, double* stats, void* stream) {
+static int dae_triplet_batch_hard_impl(const float* S, int64_t lds, int32_t B, const float* labels, float* G, int64_t ldg,
+                                      float* weight, double* stats, void* stream, double* loss_slots) {
   using namespace dae;
   DAE_REQUIRE(S && labels && G && weight && stats && B >= 1 && lds >= B && ldg >= B, "dae_triplet_batch_hard: bad arguments");
   cudaStream_t st = (cudaStream_t)stream;
   DAE_CUDA(cudaMemsetAsync(weight, 0, sizeof(float) * B, st));
-  triplet_batch_hard_kernel<<<B, kHardThreads, 0, st>>>(S, lds, 0, B, labels, G, ldg, weight, stats);
+  triplet_batch_hard_kernel<<<B, kHardThreads, 0, st>>>(S, lds, 0, B, labels, G, ldg, weight, stats, loss_slots);
   dim3 grid((B + 255) / 256, B);
   triplet_hard_scale_kernel<<<grid, 256, 0, st>>>(G, ldg, B, weight, stats);
   DAE_CHECK_LAUNCH("dae_triplet_batch_hard");
   return DAE_OK;
 }
 
-extern "C" int dae_triplet_batch_all_rows(const float* S_blk, int64_t lds, int32_t row0, int32_t n_rows, int32_t B, const int32_t* seg_lo,
+static int dae_triplet_batch_all_rows_impl(const float* S_blk, int64_t lds, int32_t row0, int32_t n_rows, int32_t B, const int32_t* seg_lo,
                                           const int32_t* seg_hi, float* G_blk, int64_t ldg, double* stats, int32_t pos_only, void* g_hi,
-                                          void* g_lo, int64_t ld_split, void* stream) {
+                                          void* g_lo, int64_t ld_split, void* stream, double* loss_slots) {
   using namespace dae;
   DAE_REQUIRE(S_blk && seg_lo && seg_hi && G_blk && stats && B >= 1 && lds >= B && ldg >= B,
               "dae_triplet_batch_all_rows: bad arguments");
@@ -629,19 +634,19 @@ extern "C" int dae_triplet_batch_all_rows(const float* S_blk, int64_t lds, int32
   DAE_REQUIRE(!g_hi || (g_lo && ld_split >= B), "dae_triplet_batch_all_rows: bad split outputs");
   triplet_batch_all_tiled_kernel<<<n_rows, kTripThreads, 0, (cudaStream_t)stream>>>(S_blk, lds, row0, B, seg_lo, seg_hi, G_blk, ldg, stats,
                                                                                     pos_only, (__nv_bfloat16*)g_hi, (__nv_bfloat16*)g_lo,
-                                                                                    ld_split);
+                                                                                    ld_split, loss_slots);
   DAE_CHECK_LAUNCH("dae_triplet_batch_all_rows");
   return DAE_OK;
 }
 
-extern "C" int dae_triplet_batch_hard_rows(const float* S_blk, int64_t lds, int32_t row0, int32_t n_rows, int32_t B, const float* labels,
-                                           float* G_blk, int64_t ldg, float* weight, double* stats, void* stream) {
+static int dae_triplet_batch_hard_rows_impl(const float* S_blk, int64_t lds, int32_t row0, int32_t n_rows, int32_t B, const float* labels,
+                                           float* G_blk, int64_t ldg, float* weight, double* stats, void* stream, double* loss_slots) {
   using namespace dae;
   DAE_REQUIRE(S_blk && labels && G_blk && weight && stats && B >= 1 && lds >= B && ldg >= B, "dae_triplet_batch_hard_rows: bad arguments");
   DAE_REQUIRE(B <= DAE_MAX_BLOCKED_BATCH, "dae_triplet_batch_hard_rows: B <= %d rows (got %d)", DAE_MAX_BLOCKED_BATCH, B);
   DAE_REQUIRE(row0 >= 0 && n_rows >= 1 && (int64_t)row0 + n_rows <= B,
               "dae_triplet_batch_hard_rows: anchor rows [%d, %lld) outside the batch of %d", row0, (long long)row0 + n_rows, B);
-  triplet_batch_hard_kernel<<<n_rows, kHardThreads, 0, (cudaStream_t)stream>>>(S_blk, lds, row0, B, labels, G_blk, ldg, weight, stats);
+  triplet_batch_hard_kernel<<<n_rows, kHardThreads, 0, (cudaStream_t)stream>>>(S_blk, lds, row0, B, labels, G_blk, ldg, weight, stats, loss_slots);
   DAE_CHECK_LAUNCH("dae_triplet_batch_hard_rows");
   return DAE_OK;
 }
@@ -660,11 +665,83 @@ extern "C" int dae_triplet_batch_hard_finish(const float* weight, int32_t B, dou
   return DAE_OK;
 }
 
-extern "C" int dae_triplet_explicit(const float* E, const float* Ep, const float* En, int32_t B, int32_t H, int64_t ld, float alpha,
-                                    float* dE, float* dEp, float* dEn, double* stats, void* stream) {
+static int dae_triplet_explicit_impl(const float* E, const float* Ep, const float* En, int32_t B, int32_t H, int64_t ld, float alpha,
+                                    float* dE, float* dEp, float* dEn, double* stats, void* stream, double* loss_slots) {
   using namespace dae;
   DAE_REQUIRE(E && Ep && En && dE && dEp && dEn && stats && B >= 1 && H >= 1 && ld >= H, "dae_triplet_explicit: bad arguments");
-  triplet_explicit_kernel<<<(B + 7) / 8, 256, 0, (cudaStream_t)stream>>>(E, Ep, En, B, H, ld, alpha, dE, dEp, dEn, stats);
+  triplet_explicit_kernel<<<(B + 7) / 8, 256, 0, (cudaStream_t)stream>>>(E, Ep, En, B, H, ld, alpha, dE, dEp, dEn, stats, loss_slots);
   DAE_CHECK_LAUNCH("dae_triplet_explicit");
+  return DAE_OK;
+}
+
+extern "C" int dae_triplet_batch_all(const float* S, int64_t lds, int32_t B, const int32_t* seg_lo, const int32_t* seg_hi, float* G,
+                                     int64_t ldg, double* stats, int32_t pos_only, void* g_hi, void* g_lo, int64_t ld_split, void* stream) {
+  return dae_triplet_batch_all_impl(S, lds, B, seg_lo, seg_hi, G, ldg, stats, pos_only, g_hi, g_lo, ld_split, stream, nullptr);
+}
+extern "C" int dae_triplet_batch_all_det(const float* S, int64_t lds, int32_t B, const int32_t* seg_lo, const int32_t* seg_hi, float* G,
+                                     int64_t ldg, double* stats, int32_t pos_only, void* g_hi, void* g_lo, int64_t ld_split, double* loss_slots, void* stream) {
+  DAE_REQUIRE(loss_slots, "dae_triplet_batch_all_det: null loss_slots");
+  return dae_triplet_batch_all_impl(S, lds, B, seg_lo, seg_hi, G, ldg, stats, pos_only, g_hi, g_lo, ld_split, stream, loss_slots);
+}
+
+extern "C" int dae_triplet_batch_hard(const float* S, int64_t lds, int32_t B, const float* labels, float* G, int64_t ldg,
+                                      float* weight, double* stats, void* stream) {
+  return dae_triplet_batch_hard_impl(S, lds, B, labels, G, ldg, weight, stats, stream, nullptr);
+}
+extern "C" int dae_triplet_batch_hard_det(const float* S, int64_t lds, int32_t B, const float* labels, float* G, int64_t ldg,
+                                      float* weight, double* stats, double* loss_slots, void* stream) {
+  DAE_REQUIRE(loss_slots, "dae_triplet_batch_hard_det: null loss_slots");
+  return dae_triplet_batch_hard_impl(S, lds, B, labels, G, ldg, weight, stats, stream, loss_slots);
+}
+
+extern "C" int dae_triplet_batch_all_rows(const float* S_blk, int64_t lds, int32_t row0, int32_t n_rows, int32_t B, const int32_t* seg_lo,
+                                          const int32_t* seg_hi, float* G_blk, int64_t ldg, double* stats, int32_t pos_only, void* g_hi,
+                                          void* g_lo, int64_t ld_split, void* stream) {
+  return dae_triplet_batch_all_rows_impl(S_blk, lds, row0, n_rows, B, seg_lo, seg_hi, G_blk, ldg, stats, pos_only, g_hi, g_lo, ld_split, stream, nullptr);
+}
+extern "C" int dae_triplet_batch_all_rows_det(const float* S_blk, int64_t lds, int32_t row0, int32_t n_rows, int32_t B, const int32_t* seg_lo,
+                                          const int32_t* seg_hi, float* G_blk, int64_t ldg, double* stats, int32_t pos_only, void* g_hi,
+                                          void* g_lo, int64_t ld_split, double* loss_slots, void* stream) {
+  DAE_REQUIRE(loss_slots, "dae_triplet_batch_all_rows_det: null loss_slots");
+  return dae_triplet_batch_all_rows_impl(S_blk, lds, row0, n_rows, B, seg_lo, seg_hi, G_blk, ldg, stats, pos_only, g_hi, g_lo, ld_split, stream, loss_slots);
+}
+
+extern "C" int dae_triplet_batch_hard_rows(const float* S_blk, int64_t lds, int32_t row0, int32_t n_rows, int32_t B, const float* labels,
+                                           float* G_blk, int64_t ldg, float* weight, double* stats, void* stream) {
+  return dae_triplet_batch_hard_rows_impl(S_blk, lds, row0, n_rows, B, labels, G_blk, ldg, weight, stats, stream, nullptr);
+}
+extern "C" int dae_triplet_batch_hard_rows_det(const float* S_blk, int64_t lds, int32_t row0, int32_t n_rows, int32_t B, const float* labels,
+                                           float* G_blk, int64_t ldg, float* weight, double* stats, double* loss_slots, void* stream) {
+  DAE_REQUIRE(loss_slots, "dae_triplet_batch_hard_rows_det: null loss_slots");
+  return dae_triplet_batch_hard_rows_impl(S_blk, lds, row0, n_rows, B, labels, G_blk, ldg, weight, stats, stream, loss_slots);
+}
+
+extern "C" int dae_triplet_explicit(const float* E, const float* Ep, const float* En, int32_t B, int32_t H, int64_t ld, float alpha,
+                                    float* dE, float* dEp, float* dEn, double* stats, void* stream) {
+  return dae_triplet_explicit_impl(E, Ep, En, B, H, ld, alpha, dE, dEp, dEn, stats, stream, nullptr);
+}
+extern "C" int dae_triplet_explicit_det(const float* E, const float* Ep, const float* En, int32_t B, int32_t H, int64_t ld, float alpha,
+                                    float* dE, float* dEp, float* dEn, double* stats, double* loss_slots, void* stream) {
+  DAE_REQUIRE(loss_slots, "dae_triplet_explicit_det: null loss_slots");
+  return dae_triplet_explicit_impl(E, Ep, En, B, H, ld, alpha, dE, dEp, dEn, stats, stream, loss_slots);
+}
+
+namespace dae {
+// deterministic mode: stats[TRIPLET_SUM] += the per-anchor (per-row) losses in a fixed order -- each thread its strided slots in index
+// order, then block_sum's fixed tree
+__global__ void __launch_bounds__(1024) triplet_loss_sum_kernel(const double* __restrict__ slots, int n, double* __restrict__ stats) {
+  __shared__ double red[32];
+  double s = 0.0;
+  for (int i = threadIdx.x; i < n; i += blockDim.x) s += slots[i];
+  s = block_sum(s, red);
+  if (threadIdx.x == 0) stats[DAE_STAT_TRIPLET_SUM] += s;
+}
+}  // namespace dae
+
+extern "C" int dae_triplet_loss_sum(const double* loss_slots, int32_t n, double* stats, void* stream) {
+  using namespace dae;
+  DAE_REQUIRE(loss_slots && stats && n >= 1, "dae_triplet_loss_sum: bad arguments");
+  triplet_loss_sum_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(loss_slots, n, stats);
+  DAE_CHECK_LAUNCH("dae_triplet_loss_sum");
   return DAE_OK;
 }

@@ -5,6 +5,7 @@ reference autoencoder/autoencoder.py:233,241) and for `transform` (:494-497).
 PyTorch is plumbing here (device memory, streams, torch.distributed); every arithmetic op of the hot path is a
 kernel from the library.  There is no CPU path.
 """
+import ctypes
 import os
 
 import numpy as np
@@ -96,6 +97,27 @@ class _CSRView:
         self.max_row_nnz = None
 
 
+def resolve_deterministic(deterministic):
+    """deterministic: True / False, or None = the environment variable DAE_DETERMINISTIC ('1' turns the mode on)."""
+    if deterministic is None:
+        return os.environ.get('DAE_DETERMINISTIC', '0') == '1'
+    return bool(deterministic)
+
+
+def check_deterministic_supported(gemm=None, process_group=None):
+    """The deterministic mode covers the tensor-core path of one process; anything else is refused before any buffer exists."""
+    mode = gemm or os.environ.get('DAE_GEMM', 'tc')
+    if mode != 'tc':
+        raise ValueError("deterministic=True needs the tensor-core path (gemm='tc', got %r): the fp32 CUDA-core validation kernels "
+                         "add split-K partials and column sums with atomics" % (mode,))
+    world = 1
+    if process_group is not None or (torch.distributed.is_available() and torch.distributed.is_initialized()):
+        world = torch.distributed.get_world_size(process_group)
+    if world > 1:
+        raise ValueError('deterministic=True runs in one process only (world size %d): the gradient exchange across ranks has no '
+                         'fixed summation order' % world)
+
+
 def check_mining_block_rows(R):
     """mining_block_rows: None (the B x B mining buffers, batches up to MAX_TRIPLET_BATCH rows) or the anchor rows R of S held at once
     (batches up to MAX_BLOCKED_BATCH rows): a multiple of 128 (the Gram block's TMA base and tiles stay aligned) in [128, 32768]."""
@@ -112,11 +134,18 @@ class TrainEngine:
     def __init__(self, n_features, n_components, enc_act_func='sigmoid', dec_act_func='sigmoid',
                  loss_func='cross_entropy', opt='gradient_descent', learning_rate=0.1, momentum=0.5, alpha=1.0,
                  triplet_strategy='batch_all', device='cuda:0', process_group=None, gemm=None, allreduce=None,
-                 mining_block_rows=None):
+                 mining_block_rows=None, deterministic=None):
         """mining_block_rows: None = batch_all / batch_hard mine the whole B x B similarity matrix at once (12 B^2 bytes, batches up to
         MAX_TRIPLET_BATCH rows); R = they mine it R anchor rows at a time (12 R B bytes, batches up to MAX_BLOCKED_BATCH rows;
-        tensor-core path only)."""
+        tensor-core path only).
+        deterministic: True = every floating-point sum of the step runs in a fixed order, so the same seed, inputs, build and GPU model
+        give bit-identical parameters, optimizer slots, per-step scalars and transform output on every run (DESIGN 4.7); False = the
+        atomic kernels (faster); None (default) = the environment variable DAE_DETERMINISTIC ('1' = on).  Tensor-core path and one
+        process only."""
         self.block_rows = check_mining_block_rows(mining_block_rows)
+        self.deterministic = resolve_deterministic(deterministic)
+        if self.deterministic:
+            check_deterministic_supported(gemm, process_group)
         _cabi.lib()  # fail loudly if the CUDA library is missing
         if not torch.cuda.is_available():
             raise _cabi.DaeError('no CUDA device: the DAE hot path has no CPU fallback')
@@ -160,6 +189,8 @@ class TrainEngine:
         self.enc_bwd_mode = 'gather'
         if self.H > (1024 if self.H % 4 == 0 else (512 if self.H % 2 == 0 else 256)):
             self.enc_bwd_mode = 'atomic'
+        if self.deterministic:   # stable column buckets, fixed-order sums (any H)
+            self.enc_bwd_mode = 'det'
         self._ent_cap = 0
         self.fork_branches = True   # parallel branches of the step (False: one stream, what the per-kernel timing pass uses)
         self._sides = [None, None]
@@ -439,6 +470,14 @@ class TrainEngine:
             if self.strategy in (1, 2):
                 self.GG_hi = torch.empty(mine_rows, self.Bp, **bf)
                 self.GG_lo = torch.empty(mine_rows, self.Bp, **bf)
+        if self.deterministic:
+            # stream-K slots of the three GEMMs that can run at once (dE on the main branch, dW on branch B, batch_all's dE2 on branch
+            # A), the fused decode's per-(half tile, row) loss partials and one fp64 triplet-loss slot per anchor
+            nb = _cabi.query('dae_gemm_det_workspace')
+            self.gemm_ws = [torch.empty(nb, dtype=torch.uint8, device=self.device) for _ in range(3)]
+            self.n_loss_parts = _cabi.query('dae_decode_loss_parts', self.F, ctype=ctypes.c_int32)
+            self.loss_parts = torch.empty(self.n_loss_parts, B, **f32)
+            self.loss_slots = torch.empty(B, dtype=torch.float64, device=self.device)
         self._ws_B = B
 
     def _ensure_bucket_scratch(self, B):
@@ -458,6 +497,12 @@ class TrainEngine:
             self.ent_row = torch.empty(cap, dtype=torch.int32, device=self.device)
             self.ent_val = torch.empty(cap, dtype=torch.float32, device=self.device)
             self._ent_cap = cap
+        if self.enc_bwd_mode == 'det':
+            need = _cabi.query('dae_encode_csr_bwd_det_workspace', B, self.F, self.H, self._ent_cap)
+            if getattr(self, 'enc_det_ws', None) is None or self.enc_det_ws.numel() < need:   # (laid out per call from B and the cap)
+                self._graph = None
+                self._feed_graph = None
+                self.enc_det_ws = torch.empty(need, dtype=torch.uint8, device=self.device)
 
     # ---- data ----------------------------------------------------------------------------------------------------
     def set_data(self, csr, values_corrupt=None, labels=None, csr_corrupt=None):
@@ -488,11 +533,26 @@ class TrainEngine:
 
     # ---- tensor-core path helpers -------------------------------------------------------------------------------------------
     def _tc_gemm(self, M, N, K, alpha, A, a_mn, Bm, b_mn, C, ldc, n_store=0, special_col=-1, special_out=None, k_splits=1,
-                 accumulate=0, tag='gemm'):
+                 accumulate=0, tag='gemm', ws=None):
+        """ws: a deterministic-mode GEMM workspace (stream-K partial tiles are summed in k order by a fixup kernel), or None."""
         (a_hi, a_lo), (b_hi, b_lo) = A, Bm
+        if ws is not None:
+            # kernels launched (the engine's launch count): the GEMM, plus the fixup where the export runs stream-K -- k_splits = -1 and
+            # 128 x 128 tiles that do not fill the SMs in whole waves (its test, reproduced here)
+            tiles = ((M + 127) // 128) * ((N + 127) // 128)
+            n_launch = 2 if (k_splits < 0 and tiles % self._sm_count() != 0) else 1
+            self._k('dae_gemm_bf16x3_det', M, N, K, float(alpha), ptr(a_hi), ptr(a_lo), a_hi.stride(0), a_mn, ptr(b_hi), ptr(b_lo),
+                    b_hi.stride(0), b_mn, ptr(C), ldc, n_store, special_col, ptr(special_out), k_splits, accumulate, ptr(ws), ws.numel(),
+                    _stream(), n_launch=n_launch, tag=tag)
+            return
         self._k('dae_gemm_bf16x3', M, N, K, float(alpha), ptr(a_hi), ptr(a_lo), a_hi.stride(0), a_mn, ptr(b_hi), ptr(b_lo),
                 b_hi.stride(0), b_mn, ptr(C), ldc, n_store, special_col, ptr(special_out), k_splits, accumulate, _stream(),
                 tag=tag)
+
+    def _sm_count(self):
+        if getattr(self, '_sms', None) is None:
+            self._sms = torch.cuda.get_device_properties(self.device).multi_processor_count
+        return self._sms
 
     def _ensure_w_split(self):
         """W as a bf16 hi/lo pair; refreshed by the optimizer kernel after every update, so only (re)built here after
@@ -579,7 +639,7 @@ class TrainEngine:
         """K1 on the batch rows; also emits E as the bf16 hi/lo pair (plus the all-ones column kept in E_hi) the tensor-core GEMMs
         consume and, for training, the per-column entry counts of the backward gather."""
         cc = self.csr_c
-        gather = train and self.enc_bwd_mode == 'gather'
+        gather = train and self.enc_bwd_mode in ('gather', 'det')
         if gather:
             self._ensure_bucket_scratch(B)
         tc = self.gemm_mode == 'tc'
@@ -655,9 +715,7 @@ class TrainEngine:
             self._decode_tc(B, rows, weight, train, prepared=dec_prepared)
         if not train:
             if explicit_B:   # forward only: the kernel's loss statistics are what is wanted, its dE contribution lands in scratch
-                E, d, Bx = self.E, self.dE, explicit_B
-                self._k('dae_triplet_explicit', ptr(E[0:Bx]), ptr(E[Bx:2 * Bx]), ptr(E[2 * Bx:3 * Bx]), Bx, H, H, self.alpha, ptr(d[0:Bx]),
-                        ptr(d[Bx:2 * Bx]), ptr(d[2 * Bx:3 * Bx]), ptr(self.stats), main.cuda_stream)
+                self._triplet_explicit(explicit_B, main)
             self._finalize(B, strat, weight, stats_log_row, main)
             return
         if fork:
@@ -672,11 +730,11 @@ class TrainEngine:
                 self._dW_gemm(B, accumulate=0)
             # k_splits = -1: stream-K (the 28 tiles of dE / 316 tiles of dW do not fill the 132 SMs in whole waves); with branch B
             # the output was zeroed there, so the GEMM accumulates and needs no memset node of its own
-            self._tc_gemm(B, H, F, 1.0, dZhl, 0, Whl, 1, self.dE, H, k_splits=-1, accumulate=1 if par else 0, tag='gemm_decode_dE')
+            det = self.deterministic   # (deterministic: stored, the zeroing on branch B notwithstanding)
+            self._tc_gemm(B, H, F, 1.0, dZhl, 0, Whl, 1, self.dE, H, k_splits=-1, accumulate=1 if (par and not det) else 0,
+                          tag='gemm_decode_dE', ws=self.gemm_ws[0] if det else None)
         if explicit_B:   # explicit (org, pos, neg) triplets: row-wise softplus(e.e- - e.e+), adds its dE (autoencoder_triplet.py:303-314)
-            E, d, Bx = self.E, self.dE, explicit_B
-            self._k('dae_triplet_explicit', ptr(E[0:Bx]), ptr(E[Bx:2 * Bx]), ptr(E[2 * Bx:3 * Bx]), Bx, H, H, self.alpha, ptr(d[0:Bx]),
-                    ptr(d[Bx:2 * Bx]), ptr(d[2 * Bx:3 * Bx]), ptr(self.stats), main.cuda_stream)
+            self._triplet_explicit(explicit_B, main)
         if par:
             self._fork(main, sideB)           # branch B: after the zeroing (already on sideB) and once dE owns the SMs; it needs
             with torch.cuda.stream(sideB):    # nothing from the mining branch, so it does not wait for it
@@ -697,6 +755,9 @@ class TrainEngine:
                 self._stage_next_batch(stage_next[0], stage_next[1], B, sideA)
         if par:
             self._fork(sideB, main)           # the dense dW / dbv are in the gradient buffer
+        if self.enc_bwd_mode == 'det':        # deterministic: the sparse dW joins the stored dense dW in one fixed-order add
+            self._k('dae_encode_sparse_dw_add', B, F, H, self._ent_cap, ptr(self.enc_det_ws), self.enc_det_ws.numel(), ptr(self._gW()),
+                    main.cuda_stream)
         if getattr(self, '_defer_update', False):
             if used_a:
                 self._fork(sideA, main)
@@ -707,12 +768,27 @@ class TrainEngine:
         if used_a:
             self._fork(sideA, main)
 
+    def _triplet_explicit(self, Bx, stream):
+        E, d, H = self.E, self.dE, self.H
+        args = (ptr(E[0:Bx]), ptr(E[Bx:2 * Bx]), ptr(E[2 * Bx:3 * Bx]), Bx, H, H, self.alpha, ptr(d[0:Bx]), ptr(d[Bx:2 * Bx]),
+                ptr(d[2 * Bx:3 * Bx]), ptr(self.stats))
+        if self.deterministic:
+            self._k('dae_triplet_explicit_det', *args, ptr(self.loss_slots), stream.cuda_stream)
+            self._k('dae_triplet_loss_sum', ptr(self.loss_slots), Bx, ptr(self.stats), stream.cuda_stream)
+        else:
+            self._k('dae_triplet_explicit', *args, stream.cuda_stream)
+
     def _dE_triplet(self, B, stream):
         """dE2 = alpha (G + G^T) E, the triplet part of dL/dE; the encode backward adds it to the decode part (dE_add)."""
         if self.block_rows is not None:    # the block loop of _mining_blocked accumulated it block by block
             return
         with torch.cuda.stream(stream):
-            if self.small_gemm == 'tc' and self.strategy == 1:
+            if self.small_gemm == 'tc' and self.strategy == 1 and self.deterministic:
+                ws = self.gemm_ws[2]
+                self._k('dae_gemm_sym_bf16x3_det', B, self.H, float(self.alpha), ptr(self.GG_hi), ptr(self.GG_lo), self.GG_hi.stride(0),
+                        ptr(self.E_hi), ptr(self.E_lo), self.E_hi.stride(0), ptr(self.dE2), self.H, 0, ptr(ws), ws.numel(),
+                        stream.cuda_stream, n_launch=2, tag='gemm_dE_tri')
+            elif self.small_gemm == 'tc' and self.strategy == 1:
                 # batch_all: the sweep wrote G as bf16 hi / lo; ONE GEMM walks G's columns and then its rows: alpha (G + G^T) E
                 self._k('dae_gemm_sym_bf16x3', B, self.H, float(self.alpha), ptr(self.GG_hi), ptr(self.GG_lo), self.GG_hi.stride(0),
                         ptr(self.E_hi), ptr(self.E_lo), self.E_hi.stride(0), ptr(self.dE2), self.H, 0, stream.cuda_stream, tag='gemm_dE_tri')
@@ -726,14 +802,19 @@ class TrainEngine:
                 self._gemm(B, H, B, self.alpha, self.G, 1, B, self.E, 1, H, 1.0, self.dE2, H, tag='gemm_dE_tri')
 
     def _finalize(self, B, strat, weight, stats_log_row, stream):
+        if self.deterministic and self.loss != 2:
+            # the fused decode's per-(half tile, row) partials, summed in part order by one thread per row (the finalize's parts path does
+            # the same sums on ONE CTA: 4-5x slower at B = 800)
+            self._k('dae_reduce_parts', ptr(self.loss_parts), self.n_loss_parts, B, ptr(self.row_loss), stream.cuda_stream)
         self._k('dae_step_finalize', ptr(self.row_loss), None, 0, ptr(weight), B, strat, self.alpha, ptr(self.stats),
                 ptr(stats_log_row), ptr(getattr(self, '_ctl', None)), stream.cuda_stream)
 
     def _dW_gemm(self, B, accumulate):
         """[dW_dec | dbv] = dZ^T . [E | 1]  (F x (H+1): the all-ones column of E_hl delivers dbv)."""
+        det = self.deterministic   # (deterministic: the dense part is stored; the sparse part is added after the join)
         self._tc_gemm(self.F, self.H + 1, B, 1.0, (self.dZ_hi, self.dZ_lo), 1, (self.E_hi, self.E_lo), 1, self._gW(), self.H,
-                      n_store=self.H, special_col=self.H, special_out=self._gbv(), k_splits=-1, accumulate=accumulate,
-                      tag='gemm_decode_dW')
+                      n_store=self.H, special_col=self.H, special_out=self._gbv(), k_splits=-1, accumulate=0 if det else accumulate,
+                      tag='gemm_decode_dW', ws=self.gemm_ws[1] if det else None)
 
     def _mining(self, B, strat, tc, train=True):
         """S = E.E^T and the triplet kernel (loss, statistics, G = dL/dS; batch_hard: also the data weights)."""
@@ -746,14 +827,18 @@ class TrainEngine:
             self._tc_gemm(B, B, H, 1.0, Ehl, 0, Ehl, 0, self.S, B, tag='gemm_gram')
         else:
             self._gemm(B, B, H, 1.0, self.E, H, 1, self.E, H, 1, 0.0, self.S, B, tag='gemm_gram')  # S = E.E^T
+        det = self.deterministic
+        slots = (ptr(self.loss_slots),) if det else ()   # deterministic: one loss slot per anchor, summed in anchor order below
         if strat == 1:
             # G also leaves as the bf16 hi / lo pair the (G + G^T).E GEMM reads
-            self._k('dae_triplet_batch_all', ptr(self.S), B, B, ptr(self.seg_lo), ptr(self.seg_hi), ptr(self.G), B,
-                    ptr(self.stats), 0, ptr(self.GG_hi) if tc else None, ptr(self.GG_lo) if tc else None,
-                    self.GG_hi.stride(0) if tc else 0, st)
+            self._k('dae_triplet_batch_all_det' if det else 'dae_triplet_batch_all', ptr(self.S), B, B, ptr(self.seg_lo), ptr(self.seg_hi),
+                    ptr(self.G), B, ptr(self.stats), 0, ptr(self.GG_hi) if tc else None, ptr(self.GG_lo) if tc else None,
+                    self.GG_hi.stride(0) if tc else 0, *slots, st)
         else:
-            self._k('dae_triplet_batch_hard', ptr(self.S), B, B, ptr(self.labels_b), ptr(self.G), B, ptr(self.weight),
-                    ptr(self.stats), st, n_launch=2)
+            self._k('dae_triplet_batch_hard_det' if det else 'dae_triplet_batch_hard', ptr(self.S), B, B, ptr(self.labels_b), ptr(self.G),
+                    B, ptr(self.weight), ptr(self.stats), *slots, st, n_launch=2)
+        if det:
+            self._k('dae_triplet_loss_sum', ptr(self.loss_slots), B, ptr(self.stats), st)
 
     def _mining_blocked(self, B, strat, train):
         """The mining one block of R anchor rows at a time, for r0 = 0, R, 2R, ... (the last block is short):
@@ -775,18 +860,22 @@ class TrainEngine:
             n = min(R, B - r0)
             Eblk = (self.E_hi[r0:], self.E_lo[r0:])
             self._tc_gemm(n, B, H, 1.0, Eblk, 0, Ehl, 0, self.S, lds, tag='gemm_gram')
+            det = self.deterministic
+            slots = (ptr(self.loss_slots),) if det else ()
             if strat == 1:
-                self._k('dae_triplet_batch_all_rows', ptr(self.S), lds, r0, n, B, ptr(self.seg_lo), ptr(self.seg_hi), ptr(self.G), ldg,
-                        ptr(self.stats), 0, ptr(self.GG_hi) if train else None, ptr(self.GG_lo) if train else None, ldgg if train else 0,
-                        st)
+                self._k('dae_triplet_batch_all_rows_det' if det else 'dae_triplet_batch_all_rows', ptr(self.S), lds, r0, n, B,
+                        ptr(self.seg_lo), ptr(self.seg_hi), ptr(self.G), ldg, ptr(self.stats), 0, ptr(self.GG_hi) if train else None,
+                        ptr(self.GG_lo) if train else None, ldgg if train else 0, *slots, st)
             else:
-                self._k('dae_triplet_batch_hard_rows', ptr(self.S), lds, r0, n, B, ptr(self.labels_b), ptr(self.G), ldg, ptr(self.weight),
-                        ptr(self.stats), st)
+                self._k('dae_triplet_batch_hard_rows_det' if det else 'dae_triplet_batch_hard_rows', ptr(self.S), lds, r0, n, B,
+                        ptr(self.labels_b), ptr(self.G), ldg, ptr(self.weight), ptr(self.stats), *slots, st)
                 if train:
                     self._tc_split(self.G, n, B, ldg, self.GG_hi, self.GG_lo, scale=self.alpha)
             if train:
                 self._tc_gemm(n, H, B, a, Ghl, 0, Ehl, 1, self.dE2[r0:], H, accumulate=1, tag='gemm_dE_tri')
                 self._tc_gemm(B, H, n, a, Ghl, 1, Eblk, 1, self.dE2, H, accumulate=1, tag='gemm_dE_tri')
+        if self.deterministic:
+            self._k('dae_triplet_loss_sum', ptr(self.loss_slots), B, ptr(self.stats), st)
         if strat == 2:
             self._k('dae_triplet_batch_hard_finish', ptr(self.weight), B, ptr(self.stats), ptr(self.dE2) if train else None, H, H, st)
 
@@ -840,10 +929,11 @@ class TrainEngine:
         c = self.csr
         Ehl, Whl = (self.E_hi, self.E_lo), (self.W_hi, self.W_lo)
         if self.loss != 2:
-            self._k('dae_decode_fused_bf16x3', B, F, H, ptr(self.E_hi), ptr(self.E_lo), self.Hp, ptr(self.W_hi), ptr(self.W_lo),
+            det = self.deterministic   # deterministic: the row-loss partials are stored to [n_parts x B], not added
+            self._k('dae_decode_fused_bf16x3_det' if det else 'dae_decode_fused_bf16x3', B, F, H, ptr(self.E_hi), ptr(self.E_lo), self.Hp, ptr(self.W_hi), ptr(self.W_lo),
                     self.Hp, ptr(c.indptr), ptr(c.indices), ptr(c.values), ptr(rows), ptr(self.bv), self.dec_act, self.loss,
-                    ptr(weight), ptr(self.stats), ptr(self.dZ_hi), ptr(self.dZ_lo), self.Fp, ptr(self.row_loss), ptr(self.tile_ptr),
-                    int(prepared), st, n_launch=1 if prepared else 2, tag='gemm_decode_fwd')
+                    ptr(weight), ptr(self.stats), ptr(self.dZ_hi), ptr(self.dZ_lo), self.Fp, ptr(self.loss_parts if det else self.row_loss),
+                    ptr(self.tile_ptr), int(prepared), st, n_launch=1 if prepared else 2, tag='gemm_decode_fwd')
         else:  # cosine proximity needs whole-row norms before dZ: GEMM -> Z, elementwise loss, split
             self._tc_gemm(B, F, H, 1.0, Ehl, 0, Whl, 0, self.Z, F, tag='gemm_decode_fwd')
             self._k('dae_decode_loss_bwd', ptr(c.indptr), ptr(c.indices), ptr(c.values), ptr(rows), B, F, ptr(self.bv),
@@ -855,7 +945,12 @@ class TrainEngine:
         """K5: dA = dE * f'(A), dbh, and the sparse part of dW (X_c^T . dA) accumulated into the gradient buffer."""
         F, H, st = self.F, self.H, _stream()
         c = self.csr_c
-        if self.enc_bwd_mode == 'gather':
+        if self.enc_bwd_mode == 'det':   # dA, dbh stored; the sparse dW waits in the workspace for dae_encode_sparse_dw_add
+            self._k('dae_encode_csr_bwd_det', ptr(c.indptr), ptr(c.indices), ptr(self.values_c), ptr(rows), B, F, H, self.in_scale,
+                    ptr(self.E), ptr(self.bh), self.enc_act, ptr(self.dE), ptr(dE_add), H, ptr(self._gbh()), ptr(self.col_count),
+                    self._ent_cap, ptr(self.enc_det_ws), self.enc_det_ws.numel(), st, tag='dae_encode_csr_bwd',
+                    n_launch=8)   # column scan, tile count, tile scan, placement, rows (dA), two dbh levels, gather
+        elif self.enc_bwd_mode == 'gather':
             scan_done = getattr(self, '_scan_done', False)
             self._scan_done = False
             self._k('dae_encode_csr_bwd_gather', ptr(c.indptr), ptr(c.indices), ptr(self.values_c), ptr(rows), B, F, H, self.in_scale,

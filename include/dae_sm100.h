@@ -402,6 +402,66 @@ int dae_csr_similarity_pair_hist(const int64_t* indptr, const int32_t* indices, 
                                  int64_t workspace_bytes, uint64_t* hist, double* sums, void* stream);
 int dae_csr_similarity_pair_hist_workspace(int32_t n, int64_t nnz, int32_t n_features, int64_t* bytes);
 
+/* ---- deterministic training step (DESIGN 4.7) ----------------------------------------------------------------------------
+ * Variants of the step's kernels in which no floating-point sum depends on timing: with the same inputs, build and GPU model they
+ * give the same bits on every run.  Each takes caller-owned workspace; the *_workspace / *_parts queries size it.
+ *
+ * dae_gemm_bf16x3_det / dae_gemm_sym_bf16x3_det: dae_gemm_bf16x3 / dae_gemm_sym_bf16x3 with the same schedule and main loop.  A
+ *   stream-K segment that covers a whole tile stores it (adds it when accumulate != 0: it is the element's only writer); a segment
+ *   that covers part of a tile stores it to its CTA's workspace slot, and a fixup kernel adds each split tile's slots in k order and
+ *   stores (adds) the sum once.  k_splits: 1 or -1 (stream-K where dae_gemm_bf16x3 would use it).  workspace: at least
+ *   dae_gemm_det_workspace bytes (2 slots of 128 x 128 fp32 per SM).  Concurrent calls need separate workspaces.
+ * dae_decode_fused_bf16x3_det: dae_decode_fused_bf16x3, but row_loss_parts is [n_parts x Brows] (n_parts from
+ *   dae_decode_loss_parts: two per 128-column tile) and every (half tile, row) partial is stored, not added; dae_step_finalize
+ *   (parts, n_parts) or dae_reduce_parts sums them in part order.
+ * dae_encode_csr_bwd_det: dA = dE * f'(A) in place of dE (dE_add added first, as in dae_encode_csr_bwd_gather) and dbh STORED (the
+ *   sums of 4-row CTAs, added in order in groups of 32, then the groups in order).  The sparse dW = X_c^T . dA stays in the workspace: the batch's kept entries are
+ *   bucketed by column in batch-row order (a stable counting sort), summed per column in that order in chunks of fixed entry
+ *   positions, and dae_encode_sparse_dw_add later adds them onto dW (F x H, e.g. the dense dW stored by dae_gemm_bf16x3_det).
+ *   col_count: the per-column counts dae_encode_csr_fwd wrote for this batch.  cap_nnz: at least the batch's stored entries; the
+ *   same value goes to the workspace query and to dae_encode_sparse_dw_add.  Rows must be canonical (no repeated column).  Any H up
+ *   to 12800.
+ * dae_triplet_*_det: the mining kernels with the triplet loss of anchor (explicit: row) a stored to loss_slots[a] (fp64, one per
+ *   anchor of the batch; batch_hard stores 0 for inactive anchors) instead of added to stats; dae_triplet_loss_sum then adds the n
+ *   slots to stats[DAE_STAT_TRIPLET_SUM] in a fixed order.  The integer-valued statistics (NUM, N_ACTIVE, batch_hard's weights)
+ *   keep their atomics: their sums are exact in any order.
+ */
+int dae_gemm_det_workspace(int64_t* bytes);
+int dae_gemm_bf16x3_det(int32_t M, int32_t N, int32_t K, float alpha, const void* a_hi, const void* a_lo, int64_t lda,
+                        int32_t a_mn_major, const void* b_hi, const void* b_lo, int64_t ldb, int32_t b_mn_major, float* C,
+                        int64_t ldc, int32_t n_store, int32_t special_col, float* special_out, int32_t k_splits,
+                        int32_t accumulate, void* workspace, int64_t workspace_bytes, void* stream);
+int dae_gemm_sym_bf16x3_det(int32_t M, int32_t N, float alpha, const void* g_hi, const void* g_lo, int64_t ldg, const void* b_hi,
+                            const void* b_lo, int64_t ldb, float* C, int64_t ldc, int32_t accumulate, void* workspace,
+                            int64_t workspace_bytes, void* stream);
+int dae_decode_loss_parts(int32_t F, int32_t* n_parts);
+int dae_decode_fused_bf16x3_det(int32_t Brows, int32_t F, int32_t K, const void* e_hi, const void* e_lo,
+                                int64_t lde, const void* w_hi, const void* w_lo, int64_t ldw,
+                                const int64_t* indptr, const int32_t* indices, const float* values,
+                                const int32_t* rows, const float* bv, int32_t dec_act, int32_t loss_func,
+                                const float* weight, const double* stats, void* dz_hi, void* dz_lo,
+                                int64_t ld_dz, float* row_loss_parts, int32_t* tile_ptr, int32_t prepared, void* stream);
+int dae_encode_csr_bwd_det_workspace(int32_t n_rows, int32_t F, int32_t H, int64_t cap_nnz, int64_t* bytes);
+int dae_encode_csr_bwd_det(const int64_t* indptr, const int32_t* indices, const float* values, const int32_t* rows,
+                           int32_t n_rows, int32_t F, int32_t H, float in_scale, const float* E, const float* bh,
+                           int32_t enc_act, float* dE, const float* dE_add, int64_t ldE, float* dbh, const int32_t* col_count,
+                           int64_t cap_nnz, void* workspace, int64_t workspace_bytes, void* stream);
+int dae_encode_sparse_dw_add(int32_t n_rows, int32_t F, int32_t H, int64_t cap_nnz, const void* workspace, int64_t workspace_bytes,
+                             float* dW, void* stream);
+int dae_triplet_batch_all_det(const float* S, int64_t lds, int32_t B, const int32_t* seg_lo, const int32_t* seg_hi,
+                              float* G, int64_t ldg, double* stats, int32_t pos_only, void* g_hi, void* g_lo,
+                              int64_t ld_split, double* loss_slots, void* stream);
+int dae_triplet_batch_hard_det(const float* S, int64_t lds, int32_t B, const float* labels, float* G, int64_t ldg,
+                               float* weight, double* stats, double* loss_slots, void* stream);
+int dae_triplet_batch_all_rows_det(const float* S_blk, int64_t lds, int32_t row0, int32_t n_rows, int32_t B, const int32_t* seg_lo,
+                                   const int32_t* seg_hi, float* G_blk, int64_t ldg, double* stats, int32_t pos_only, void* g_hi,
+                                   void* g_lo, int64_t ld_split, double* loss_slots, void* stream);
+int dae_triplet_batch_hard_rows_det(const float* S_blk, int64_t lds, int32_t row0, int32_t n_rows, int32_t B, const float* labels,
+                                    float* G_blk, int64_t ldg, float* weight, double* stats, double* loss_slots, void* stream);
+int dae_triplet_explicit_det(const float* E, const float* Ep, const float* En, int32_t B, int32_t H, int64_t ld,
+                             float alpha, float* dE, float* dEp, float* dEn, double* stats, double* loss_slots, void* stream);
+int dae_triplet_loss_sum(const double* loss_slots, int32_t n, double* stats, void* stream);
+
 /* ---- data-parallel exchange step (SURVEY 8e): in-switch all-reduce of the flat gradient buffer -------------------
  * The reference is single-process; row-sharded training adds ONE sum over ranks of [dW | dbh | dbv] between the
  * gradient kernels and dae_optimizer_step.  Default transport: ncclAllReduce.  dae_allreduce_multimem is the

@@ -75,6 +75,10 @@ def build_parser():
     ap.add_argument('--mining_block_rows', type=int, default=0,
                     help='R > 0 (a multiple of 128 up to 32768): batch_all / batch_hard mine the similarity matrix R rows at a time '
                          '(12 R B bytes instead of 12 B^2), which trains batches above 32 768 rows; 0 = off')
+    ap.add_argument('--deterministic', action='store_true', default=False,
+                    help='add every floating-point sum of the training step in a fixed order, so that a rerun with the same --seed (>= 0) '
+                         'and data gives bit-identical parameters, losses and embeddings on the same GPU model (slower; default: off, '
+                         'or the environment variable DAE_DETERMINISTIC=1)')
     return ap
 
 
@@ -322,7 +326,8 @@ def main(argv=None):
         dec_act_func=F.dec_act_func, xavier_init=F.xavier_init, corr_type=F.corr_type, corr_frac=F.corr_frac,
         loss_func=F.loss_func, main_dir=F.main_dir, opt=F.opt, learning_rate=F.learning_rate, momentum=F.momentum,
         verbose=F.verbose, verbose_step=F.verbose_step, num_epochs=F.num_epochs, batch_size=F.batch_size, alpha=F.alpha,
-        triplet_strategy=F.triplet_strategy, rng_mode=F.rng_mode, mining_block_rows=F.mining_block_rows or None)
+        triplet_strategy=F.triplet_strategy, rng_mode=F.rng_mode, mining_block_rows=F.mining_block_rows or None,
+        deterministic=True if F.deterministic else None)
     data = None
     if F.synthetic:
         trX, vlX, trL, vlL = prepare_synthetic(F)

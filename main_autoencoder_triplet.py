@@ -158,7 +158,7 @@ def main(argv=None):
         dec_act_func=F.dec_act_func, xavier_init=F.xavier_init, corr_type=F.corr_type, corr_frac=F.corr_frac,
         loss_func=F.loss_func, main_dir=F.main_dir, opt=F.opt, learning_rate=F.learning_rate, momentum=F.momentum,
         verbose=F.verbose, verbose_step=F.verbose_step, num_epochs=F.num_epochs, batch_size=F.batch_size, alpha=F.alpha,
-        rng_mode=F.rng_mode)
+        rng_mode=F.rng_mode, deterministic=True if F.deterministic else None)
     data = None
     if F.synthetic:
         trX, vlX = prepare_synthetic_triplets(F)
