@@ -74,6 +74,11 @@ _SIGNATURES = {
     'dae_similarity_pair_hist_bf16x3': (C.c_int, [i32, i32, p, p, i64, p, f32, i32, p, p, p]),
     'dae_csr_similarity_pair_hist': (C.c_int, [p, p, p, i32, i64, i32, p, f32, i32, p, i64, p, p, p]),
     'dae_csr_similarity_pair_hist_workspace': (C.c_int, [i32, i64, i32, p]),
+    'dae_similarity_pairs_bf16x3': (C.c_int, [i32, i32, i32, p, p, i64, p, p, i64, i32, f32, p, i64, p, p, p, p]),
+    'dae_csr_similarity_pairs': (C.c_int, [p, p, p, i32, i64, i32, p, p, p, i32, i64, i32, i32, f32, p, i64, p, i64, p, p, p, p]),
+    'dae_csr_similarity_pairs_workspace': (C.c_int, [i32, i32, i64, i32, p]),
+    'dae_pairs_sort': (C.c_int, [i64, i32, i32, p, p, p, p, p, i64, p, p]),
+    'dae_pairs_sort_workspace': (C.c_int, [i64, i32, p]),
     'dae_allreduce_multimem': (C.c_int, [p, p, p, i32, i32, i64, i32, p]),
     'dae_mask_values': (C.c_int, [p, p, i64, f32, u64, u64, p, p]),
     # deterministic training step

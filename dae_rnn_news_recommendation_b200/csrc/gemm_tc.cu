@@ -21,6 +21,8 @@
 //                   epilogue instead of the loss, so the similarity matrix never leaves the SM.
 //   pair histogram (dae_similarity_pair_hist_bf16x3; see pair_hist_kernel): the same five warpgroups over the lower-triangle tiles
 //                   of X.X^T, binning related / unrelated pair scores into uint64 histograms for the AUROC.
+//   thresholded pairs (dae_similarity_pairs_bf16x3; see pairs_kernel): the same five warpgroups, emitting every pair with a score
+//                   at or above a threshold (near-duplicates) into caller-sized arrays through a warp-aggregated 64-bit counter.
 // Operands may be K-major (K contiguous) or MN-major (M/N contiguous) -- both straight from row-major arrays (wgmma's transpose
 // bits), so no transposed copies of dZ / E / W are ever made.
 #include <cuda.h>
@@ -28,6 +30,7 @@
 #include <type_traits>
 #include "common.cuh"
 #include "pair_hist.cuh"
+#include "pairs.cuh"
 #include "topk.cuh"
 
 namespace dae {
@@ -1184,6 +1187,157 @@ __global__ void __launch_bounds__(kDecodeThreads, 1) pair_hist_kernel(const __gr
   }
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// thresholded pairs (dae_similarity_pairs_bf16x3): every (i, j) with S[i, j] = Q_i . C_j >= tau as an (i, j, s) triple, without
+// writing S.  topk_kernel's five warpgroups, operand ring, tile shape and k16 order, so every score has the bits
+// dae_similarity_topk_bf16x3 computes for the same (i, j); a different schedule and epilogue.
+//   work item: one 128 x 128 tile, dealt round-robin: self mode (Q is C) the tiles with nb <= mb, as pair_hist_kernel; corpus mode
+//              all of them.
+//   epilogue : thread = (row, 64-column half), as in top-k.  Pass 1 counts the row's qualifying columns (j < i in self mode, j < N
+//              in corpus mode): per float4 one max and compare against tau, the common case.  A warp with any hit reserves its
+//              slots with one atomicAdd on the 64-bit counter (pair_slots) and pass 2 writes the triples to the slots below capacity.
+// ---------------------------------------------------------------------------------------------------------------------
+struct PairsParams {
+  GemmParams g;                      // M = queries, N = corpus rows, K = dim
+  int self;                          // != 0: Q is C; tiles nb <= mb, columns j < i
+  float tau;
+  unsigned long long* count;         // caller-zeroed, accumulated: the number of qualifying pairs
+  unsigned long long capacity;       // slots of i_out / j_out / s_out
+  int32_t* i_out; int32_t* j_out; float* s_out;
+};
+
+// self: tiles t = mb (mb + 1) / 2 + nb, nb <= mb (PairHistSched's order); corpus: t = mb * tiles_n + nb.  Items blockIdx.x,
+// blockIdx.x + gridDim.x, ...
+struct PairsSched {
+  long long t, n_tiles;
+  int tiles_n, self, n_cta, kb_total;
+  __device__ __forceinline__ void init(const PairsParams& pp, int block_n, int block_k) {
+    const long long tm = (pp.g.M + BLOCK_M - 1) / BLOCK_M;
+    tiles_n = (pp.g.N + block_n - 1) / block_n;
+    self = pp.self;
+    n_tiles = self ? tm * (tm + 1) / 2 : tm * tiles_n;
+    kb_total = (pp.g.K + block_k - 1) / block_k;
+    n_cta = (int)gridDim.x;
+    t = blockIdx.x;
+  }
+  __device__ __forceinline__ bool next(int& mb, int& nb, int& kb0, int& kb1) {
+    if (t >= n_tiles) return false;
+    if (self) {
+      long long r = (long long)((sqrt(8.0 * (double)t + 1.0) - 1.0) * 0.5);
+      while (r * (r + 1) / 2 > t) --r;
+      while ((r + 1) * (r + 2) / 2 <= t) ++r;
+      mb = (int)r;
+      nb = (int)(t - r * (r + 1) / 2);
+    } else {
+      mb = (int)(t / tiles_n);
+      nb = (int)(t - (long long)mb * tiles_n);
+    }
+    kb0 = 0; kb1 = kb_total;
+    t += n_cta;
+    return true;
+  }
+};
+
+__global__ void __launch_bounds__(kDecodeThreads, 1) pairs_kernel(const __grid_constant__ CUtensorMap tm_a_hi,
+                                                                  const __grid_constant__ CUtensorMap tm_a_lo,
+                                                                  const __grid_constant__ CUtensorMap tm_b_hi,
+                                                                  const __grid_constant__ CUtensorMap tm_b_lo,
+                                                                  const PairsParams pp) {
+  constexpr int BLOCK_N = kDecodeN, STAGES = kTopkStages, BK = kTopkBK;
+  constexpr int STAGE_BYTES = 2 * BLOCK_M * BK * 2 + 2 * BLOCK_N * BK * 2;
+  constexpr int SROW = BLOCK_N + 4;
+  constexpr int HALF_N = BLOCK_N / 2;
+  const GemmParams& p = pp.g;
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  float* stg = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES);   // [BLOCK_M][SROW] accumulator staging
+  __shared__ __align__(8) uint64_t full_bar[STAGES], empty_bar[STAGES], staged_bar[2], drained_bar[2];
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int role = warp >> 2;                     // warpgroup: 0 producer, 1-2 MMA, 3-4 epilogue
+  PairsSched sched;
+
+  if (warp == 0 && lane == 0) { prefetch_tmap(&tm_a_hi); prefetch_tmap(&tm_a_lo); prefetch_tmap(&tm_b_hi); prefetch_tmap(&tm_b_lo); }
+  if (warp == 1 && lane == 0) {
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 8); }
+    for (int h = 0; h < 2; ++h) { mbar_init(&staged_bar[h], 4); mbar_init(&drained_bar[h], 4); }
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  if (role == 0) {
+    // ===================== TMA producer =====================
+    regs_dec<kRegsProducer>();
+    sched.init(pp, BLOCK_N, BK);
+    if (warp == 0 && lane == 0)
+      tma_produce<BLOCK_N, STAGES, 0, BK>(p, sched, smem, full_bar, empty_bar, 0u, &tm_a_hi, &tm_a_lo, &tm_b_hi, &tm_b_lo, &tm_a_hi, &tm_a_lo);
+  } else if (role <= 2) {
+    // ===================== MMA: wgmma main loop -> staging half =====================
+    regs_inc<kRegsMma>();
+    sched.init(pp, BLOCK_N, BK);
+    const int h = role - 1;
+    const int wi = warp & 3;
+    float acc[BLOCK_N / 2];
+#pragma unroll
+    for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] = 0.0f;
+    int stage = 0; uint32_t phase = 0, tphase = 0;
+    int mb, nb, kb0, kb1;
+    while (sched.next(mb, nb, kb0, kb1)) {
+      mma_work_item<BLOCK_N, STAGES, 0, 0, BK>(acc, p, smem, full_bar, empty_bar, h, lane, 0u, stage, phase, kb0, kb1);
+      mbar_wait(&drained_bar[h], tphase ^ 1);   // the epilogue is done with the previous tile's rows
+      const int r0 = h * 64 + wi * 16 + (lane >> 2), c0 = 2 * (lane & 3);
+#pragma unroll
+      for (int j = 0; j < BLOCK_N / 8; ++j) {
+        *reinterpret_cast<float2*>(&stg[r0 * SROW + 8 * j + c0]) = make_float2(acc[4 * j], acc[4 * j + 1]);
+        *reinterpret_cast<float2*>(&stg[(r0 + 8) * SROW + 8 * j + c0]) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+      }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&staged_bar[h]);
+      tphase ^= 1;
+    }
+  } else {
+    // ===================== epilogue: emit the qualifying pairs of one (row, column half) =====================
+    regs_inc<kRegsEpilogue>();
+    sched.init(pp, BLOCK_N, BK);
+    const int h = role - 3;                  // staging half: rows [64 h, 64 h + 64)
+    const int wi = warp & 3;
+    const int quarter = h * 2 + (wi & 1);    // 32-row quarter of the tile this warp handles
+    const int half = wi >> 1;                // which column half of the tile
+    const int row_in_tile = quarter * 32 + lane;
+    const float* srow = stg + row_in_tile * SROW + half * HALF_N;
+    const float tau = pp.tau;
+    uint32_t tphase = 0;
+    int mb, nb, kb0, kb1;
+    while (sched.next(mb, nb, kb0, kb1)) {
+      const int i = mb * BLOCK_M + row_in_tile;
+      const int n0 = nb * BLOCK_N + half * HALF_N;
+      const int lim = pp.self ? i : p.N;                          // columns j < lim (self: i < M = N)
+      const int c_end = i < p.M ? max(0, min(HALF_N, lim - n0)) : 0;
+      mbar_wait(&staged_bar[h], tphase);
+      int hits = 0;
+#pragma unroll 1
+      for (int c = 0; c < c_end; c += 4) {   // NaN never qualifies: fmaxf drops it and every compare with it is false
+        const float4 v = *reinterpret_cast<const float4*>(srow + c);
+        if (fmaxf(fmaxf(v.x, v.y), fmaxf(v.z, v.w)) >= tau)   // rare at a near-duplicate threshold
+          hits += (v.x >= tau) + (c + 1 < c_end && v.y >= tau) + (c + 2 < c_end && v.z >= tau) + (c + 3 < c_end && v.w >= tau);
+      }
+      if (__any_sync(0xffffffffu, hits != 0)) {
+        unsigned long long slot = pair_slots(pp.count, hits);
+        if (hits) {
+#pragma unroll 1
+          for (int c = 0; c < c_end; ++c) {
+            const float s = srow[c];
+            if (s >= tau) pair_put(slot++, pp.capacity, i, n0 + c, s, pp.i_out, pp.j_out, pp.s_out);
+          }
+        }
+      }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&drained_bar[h]);   // this warp's staging rows may be overwritten
+      tphase ^= 1;
+    }
+  }
+}
+
 // tile_ptr[m][t] = number of stored entries of batch row m with column < t * half_n (t = 0 .. n_half_tiles): where each
 // half tile of the fused decode epilogue starts in the (sorted) clean CSR row.  One thread per (row, t).
 __global__ void decode_tile_ptr_kernel(const int64_t* __restrict__ indptr, const int32_t* __restrict__ indices,
@@ -1468,6 +1622,25 @@ static int launch_pair_hist(const Operand& X, const PairHistParams& hp, cudaStre
   const long long tm = (p.M + BLOCK_M - 1) / BLOCK_M, tiles = tm * (tm + 1) / 2;
   const int n = tiles < sm_count() ? (int)tiles : sm_count();
   pair_hist_kernel<<<n, kDecodeThreads, smem, st>>>(ta_hi, ta_lo, tb_hi, tb_lo, hp);
+  return DAE_OK;
+}
+
+// thresholded pairs: Q [M x K] and C [N x K], both K-major; one persistent CTA per SM over the tiles (self: the lower triangle)
+static int launch_pairs(const Operand& A, const Operand& B, const PairsParams& pp, cudaStream_t st) {
+  CUtensorMap ta_hi, ta_lo, tb_hi, tb_lo;
+  int rc;
+  const GemmParams& p = pp.g;
+  if ((rc = make_map(&ta_hi, A.hi, p.K, p.M, A.ld, BLOCK_M, kTopkBK))) return rc;
+  if ((rc = make_map(&ta_lo, A.lo, p.K, p.M, A.ld, BLOCK_M, kTopkBK))) return rc;
+  if ((rc = make_map(&tb_hi, B.hi, p.K, p.N, B.ld, kDecodeN, kTopkBK))) return rc;
+  if ((rc = make_map(&tb_lo, B.lo, p.K, p.N, B.ld, kDecodeN, kTopkBK))) return rc;
+  constexpr int smem = kTopkStages * (2 * BLOCK_M * kTopkBK * 2 + 2 * kDecodeN * kTopkBK * 2) + BLOCK_M * (kDecodeN + 4) * 4 + 1024;
+  static bool attr_done[64] = {false};
+  if ((rc = ensure_smem_attr(pairs_kernel, smem, attr_done))) return rc;
+  const long long tm = (p.M + BLOCK_M - 1) / BLOCK_M, tn = (p.N + kDecodeN - 1) / kDecodeN;
+  const long long tiles = pp.self ? tm * (tm + 1) / 2 : tm * tn;
+  const int n = tiles < sm_count() ? (int)tiles : sm_count();
+  pairs_kernel<<<n, kDecodeThreads, smem, st>>>(ta_hi, ta_lo, tb_hi, tb_lo, pp);
   return DAE_OK;
 }
 
@@ -1816,5 +1989,33 @@ extern "C" int dae_similarity_pair_hist_bf16x3(int32_t n, int32_t dim, const voi
   int rc = launch_pair_hist(X, hp, (cudaStream_t)stream);
   if (rc) return rc;
   DAE_CHECK_LAUNCH("dae_similarity_pair_hist_bf16x3");
+  return DAE_OK;
+}
+
+extern "C" int dae_similarity_pairs_bf16x3(int32_t n_query, int32_t n_corpus, int32_t dim, const void* q_hi, const void* q_lo, int64_t ldq,
+                                           const void* c_hi, const void* c_lo, int64_t ldc, int32_t self, float threshold, uint64_t* count,
+                                           int64_t capacity, int32_t* i_out, int32_t* j_out, float* s_out, void* stream) {
+  DAE_REQUIRE(q_hi && q_lo && c_hi && c_lo && count, "dae_similarity_pairs_bf16x3: null pointer");
+  DAE_REQUIRE(capacity >= 0, "dae_similarity_pairs_bf16x3: capacity = %lld < 0", (long long)capacity);
+  DAE_REQUIRE(capacity == 0 || (i_out && j_out && s_out), "dae_similarity_pairs_bf16x3: null output with capacity %lld > 0",
+              (long long)capacity);
+  DAE_REQUIRE(n_query > 0 && n_corpus > 0 && dim > 0, "dae_similarity_pairs_bf16x3: bad sizes");
+  DAE_REQUIRE(!self || (n_query == n_corpus && q_hi == c_hi && q_lo == c_lo && ldq == ldc),
+              "dae_similarity_pairs_bf16x3: self mode needs the corpus operands to be the query operands");
+  DAE_REQUIRE(pair_threshold_ok(threshold), "dae_similarity_pairs_bf16x3: threshold %g is not finite", (double)threshold);
+  DAE_REQUIRE(ldq >= dim && ldc >= dim && ldq % 8 == 0 && ldc % 8 == 0,
+              "dae_similarity_pairs_bf16x3: leading dimensions must cover dim and be multiples of 8 (TMA 16-byte strides)");
+  DAE_REQUIRE(((uintptr_t)q_hi | (uintptr_t)q_lo | (uintptr_t)c_hi | (uintptr_t)c_lo) % 16 == 0 && (uintptr_t)count % 8 == 0 &&
+                  ((uintptr_t)i_out | (uintptr_t)j_out | (uintptr_t)s_out) % 4 == 0,
+              "dae_similarity_pairs_bf16x3: operands must be 16-byte, the counter 8-byte and the outputs 4-byte aligned");
+  PairsParams pp{};
+  pp.g.M = n_query; pp.g.N = n_corpus; pp.g.K = dim; pp.g.k_splits = 1; pp.g.alpha = 1.0f; pp.g.special_col = -1;
+  pp.self = self ? 1 : 0; pp.tau = threshold;
+  pp.count = reinterpret_cast<unsigned long long*>(count); pp.capacity = (unsigned long long)capacity;
+  pp.i_out = i_out; pp.j_out = j_out; pp.s_out = s_out;
+  Operand A{q_hi, q_lo, ldq, 0}, B{c_hi, c_lo, ldc, 0};
+  int rc = launch_pairs(A, B, pp, (cudaStream_t)stream);
+  if (rc) return rc;
+  DAE_CHECK_LAUNCH("dae_similarity_pairs_bf16x3");
   return DAE_OK;
 }

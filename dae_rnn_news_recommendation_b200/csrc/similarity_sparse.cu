@@ -15,10 +15,13 @@
 //   splits   : with too few queries to fill the SMs the ranges are cut into `splits` groups, one warp each, and topk_merge_kernel
 //              merges the partial lists.  The extra memory is the buckets ((Nc / kSpW + 1) F int32), the postings (8 B per corpus
 //              entry) and, with splits > 1, the partial lists (8 B per entry): never Nq x Nc or Nq x F.
-//   histogram: sp_topk_kernel<true> (dae_csr_similarity_pair_hist) bins the same scores of the strict lower triangle of Q.Q^T into
-//              related / unrelated histograms instead of k-best lists.
+//   histogram: sp_topk_kernel<kSpHist> (dae_csr_similarity_pair_hist) bins the same scores of the strict lower triangle of Q.Q^T
+//              into related / unrelated histograms instead of k-best lists.
+//   pairs    : sp_topk_kernel<kSpPairs> (dae_csr_similarity_pairs) emits every slot with a score >= tau as an (i, j, s) triple, of
+//              Q.C^T or of the strict lower triangle of Q.Q^T.
 #include "common.cuh"
 #include "pair_hist.cuh"
+#include "pairs.cuh"
 #include "topk.cuh"
 
 namespace dae {
@@ -153,7 +156,15 @@ struct SpParams {
   uint32_t bins;
   unsigned long long* hist;
   double* sums;
+  // pairs mode: self (Q = C: ranges below q, slots c < q), threshold, caller-zeroed counter, output slots
+  int self;
+  float tau;
+  unsigned long long* count;
+  unsigned long long capacity;
+  int32_t* pair_i; int32_t* pair_j; float* pair_s;
 };
+
+enum SpMode { kSpTopk, kSpHist, kSpPairs };
 
 // offer (v, col) to the warp's list (lane j < k holds entry j); warp-uniform arguments
 __device__ __forceinline__ void sp_offer(float v, int col, int n_corpus, int excl, int k, int lane, float& lv, int& li, float& thr) {
@@ -166,13 +177,15 @@ __device__ __forceinline__ void sp_offer(float v, int col, int n_corpus, int exc
   thr = __shfl_sync(kFull, lv, k - 1);
 }
 
-// HIST = false: k-best lists (dae_csr_similarity_topk).  HIST = true: the related / unrelated pair histogram of Q against itself
+// kSpTopk: k-best lists (dae_csr_similarity_topk).  kSpHist: the related / unrelated pair histogram of Q against itself
 // (dae_csr_similarity_pair_hist): the same postings, accumulation and scores, but only the ranges that start below q are
 // accumulated and only slots c < q are counted -- the strict lower triangle.  The scan bins every non-zero slot (runs of equal
 // (group, bin) in one red.global.add.u64); the zero slots, most of them, are only counted per group in registers and added with
-// one atomic per group when the warp is done.
-template <bool HIST>
+// one atomic per group when the warp is done.  kSpPairs: the scan emits the slots with s >= tau (c < q in self mode, whose ranges
+// stop below q as in kSpHist); a warp with any hit in a 128-slot chunk reserves its slots with one atomicAdd (pair_slots).
+template <SpMode MODE>
 __global__ void __launch_bounds__(kSpWarps * 32, 3) sp_topk_kernel(const SpParams p) {
+  constexpr bool HIST = MODE == kSpHist;
   extern __shared__ float4 sp_smem4[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int64_t item = (int64_t)blockIdx.x * kSpWarps + warp;
@@ -187,6 +200,9 @@ __global__ void __launch_bounds__(kSpWarps * 32, 3) sp_topk_kernel(const SpParam
     lq = p.labels[q];
     if (lq < 0) return;                                 // warp-uniform: a row without a label has no pairs
     r1 = min(r1, (q + kSpW - 1) / kSpW);                // ranges that start below q
+  }
+  if constexpr (MODE == kSpPairs) {
+    if (p.self) r1 = min(r1, (q + kSpW - 1) / kSpW);
   }
   double sum_rel = 0.0, sum_unrel = 0.0;
   uint32_t zero_rel = 0, zero_unrel = 0, run_key = 0, run_n = 0;
@@ -243,6 +259,25 @@ __global__ void __launch_bounds__(kSpWarps * 32, 3) sp_topk_kernel(const SpParam
         const int c = base + j0 + 4 * lane;
         count(x.x, c); count(x.y, c + 1); count(x.z, c + 2); count(x.w, c + 3);
       }
+    } else if constexpr (MODE == kSpPairs) {
+      // emit the slots c < lim with s >= tau (tau > 0: the slots past width, never written, stay 0), zero the slab
+      const int lim = p.self ? q : p.n_corpus;
+      const float tau = p.tau;
+      for (int j0 = 0; j0 < width; j0 += 128) {
+        const float4 x = slab4[j0 / 4 + lane];
+        slab4[j0 / 4 + lane] = make_float4(0.f, 0.f, 0.f, 0.f);
+        const int c = base + j0 + 4 * lane;
+        const bool h0 = x.x >= tau && c < lim, h1 = x.y >= tau && c + 1 < lim;
+        const bool h2 = x.z >= tau && c + 2 < lim, h3 = x.w >= tau && c + 3 < lim;
+        const int hits = h0 + h1 + h2 + h3;
+        if (__any_sync(kFull, hits != 0)) {
+          unsigned long long slot = pair_slots(p.count, hits);
+          if (h0) pair_put(slot++, p.capacity, q, c, x.x, p.pair_i, p.pair_j, p.pair_s);
+          if (h1) pair_put(slot++, p.capacity, q, c + 1, x.y, p.pair_i, p.pair_j, p.pair_s);
+          if (h2) pair_put(slot++, p.capacity, q, c + 2, x.z, p.pair_i, p.pair_j, p.pair_s);
+          if (h3) pair_put(slot, p.capacity, q, c + 3, x.w, p.pair_i, p.pair_j, p.pair_s);
+        }
+      }
     } else {
       // scan the slab in increasing corpus index (lane-major float4s), offer what beats the k-th score, zero it for the next range
       for (int j0 = 0; j0 < width; j0 += 128) {
@@ -279,6 +314,7 @@ __global__ void __launch_bounds__(kSpWarps * 32, 3) sp_topk_kernel(const SpParam
     }
     return;
   }
+  if constexpr (MODE == kSpPairs) return;
   if (lane < k) {
     if (p.splits == 1) {
       p.idx_out[(int64_t)q * k + lane] = li;
@@ -314,18 +350,18 @@ static int sp_postings(const SpLayout& L, const int64_t* c_indptr, const int32_t
   return DAE_OK;
 }
 
-template <bool HIST>
+template <SpMode MODE>
 static int sp_launch(const SpParams& sp, cudaStream_t st) {
   constexpr int smem = kSpWarps * kSpW * 4;
   static bool attr_done[64] = {false};
   int dev = 0;
   DAE_CUDA(cudaGetDevice(&dev));
   if (dev >= 0 && dev < 64 && !attr_done[dev]) {
-    DAE_CUDA(cudaFuncSetAttribute(sp_topk_kernel<HIST>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    DAE_CUDA(cudaFuncSetAttribute(sp_topk_kernel<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     attr_done[dev] = true;
   }
   const int64_t warps = (int64_t)sp.n_query * sp.splits;
-  sp_topk_kernel<HIST><<<(unsigned)((warps + kSpWarps - 1) / kSpWarps), kSpWarps * 32, smem, st>>>(sp);
+  sp_topk_kernel<MODE><<<(unsigned)((warps + kSpWarps - 1) / kSpWarps), kSpWarps * 32, smem, st>>>(sp);
   return DAE_OK;
 }
 
@@ -372,7 +408,7 @@ extern "C" int dae_csr_similarity_topk(const int64_t* q_indptr, const int32_t* q
   sp.idx_out = idx_out; sp.val_out = val_out;
   sp.ws_val = reinterpret_cast<float*>(ws + L.off_val);
   sp.ws_idx = reinterpret_cast<int32_t*>(ws + L.off_idx);
-  if ((rc = sp_launch<false>(sp, st))) return rc;
+  if ((rc = sp_launch<kSpTopk>(sp, st))) return rc;
   DAE_CHECK_LAUNCH("dae_csr_similarity_topk");
   if (L.splits > 1) {
     topk_merge_kernel<<<(n_query + 7) / 8, 256, 0, st>>>(sp.ws_val, sp.ws_idx, n_query, L.splits, k, idx_out, val_out);
@@ -413,7 +449,52 @@ extern "C" int dae_csr_similarity_pair_hist(const int64_t* indptr, const int32_t
   sp.n_query = n; sp.n_corpus = n; sp.F = n_features; sp.k = 1; sp.splits = L.splits; sp.ranges = L.ranges; sp.exclude = 0;
   sp.labels = labels; sp.range = range; sp.scale = (float)bins / (2.0f * range); sp.bins = (uint32_t)bins;
   sp.hist = reinterpret_cast<unsigned long long*>(hist); sp.sums = sums;
-  if ((rc = sp_launch<true>(sp, st))) return rc;
+  if ((rc = sp_launch<kSpHist>(sp, st))) return rc;
   DAE_CHECK_LAUNCH("dae_csr_similarity_pair_hist");
+  return DAE_OK;
+}
+
+extern "C" int dae_csr_similarity_pairs_workspace(int32_t n_query, int32_t n_corpus, int64_t corpus_nnz, int32_t n_features, int64_t* bytes) {
+  DAE_REQUIRE(bytes && n_query > 0 && n_corpus > 0 && n_features > 0 && corpus_nnz >= 0 && corpus_nnz < INT32_MAX,
+              "dae_csr_similarity_pairs_workspace: bad arguments");
+  *bytes = sp_layout(n_query, n_corpus, corpus_nnz, n_features, 0, 0).total;
+  return DAE_OK;
+}
+
+extern "C" int dae_csr_similarity_pairs(const int64_t* q_indptr, const int32_t* q_indices, const float* q_values, int32_t n_query,
+                                        int64_t q_nnz, int32_t q_features, const int64_t* c_indptr, const int32_t* c_indices,
+                                        const float* c_values, int32_t n_corpus, int64_t c_nnz, int32_t c_features, int32_t self,
+                                        float threshold, void* workspace, int64_t workspace_bytes, uint64_t* count, int64_t capacity,
+                                        int32_t* i_out, int32_t* j_out, float* s_out, void* stream) {
+  DAE_REQUIRE(q_indptr && c_indptr && workspace && count && (q_nnz == 0 || (q_indices && q_values)) &&
+              (c_nnz == 0 || (c_indices && c_values)), "dae_csr_similarity_pairs: null pointer");
+  DAE_REQUIRE(capacity >= 0, "dae_csr_similarity_pairs: capacity = %lld < 0", (long long)capacity);
+  DAE_REQUIRE(capacity == 0 || (i_out && j_out && s_out), "dae_csr_similarity_pairs: null output with capacity %lld > 0",
+              (long long)capacity);
+  DAE_REQUIRE(n_query > 0 && n_corpus > 0 && q_features > 0 && c_features > 0 && q_nnz >= 0 && c_nnz >= 0 && c_nnz < INT32_MAX,
+              "dae_csr_similarity_pairs: bad sizes");
+  DAE_REQUIRE(q_features == c_features, "dae_csr_similarity_pairs: queries have %d features, the corpus %d", q_features, c_features);
+  DAE_REQUIRE(!self || (n_query == n_corpus && q_nnz == c_nnz && q_indptr == c_indptr && q_indices == c_indices && q_values == c_values),
+              "dae_csr_similarity_pairs: self mode needs the corpus matrix to be the query matrix");
+  DAE_REQUIRE(threshold > 0.0f && pair_threshold_ok(threshold),
+              "dae_csr_similarity_pairs: threshold %g must be finite and > 0 (a pair sharing no column scores 0)", (double)threshold);
+  DAE_REQUIRE((uintptr_t)workspace % 16 == 0 && (uintptr_t)count % 8 == 0 && ((uintptr_t)i_out | (uintptr_t)j_out | (uintptr_t)s_out) % 4 == 0,
+              "dae_csr_similarity_pairs: workspace must be 16-byte, the counter 8-byte and the outputs 4-byte aligned");
+  const SpLayout L = sp_layout(n_query, n_corpus, c_nnz, c_features, 0, 0);
+  DAE_REQUIRE(workspace_bytes >= L.total, "dae_csr_similarity_pairs: workspace of %lld bytes, %lld needed (dae_csr_similarity_pairs_workspace)",
+              (long long)workspace_bytes, (long long)L.total);
+  cudaStream_t st = (cudaStream_t)stream;
+  uint8_t* ws = reinterpret_cast<uint8_t*>(workspace);
+  int rc = sp_postings(L, c_indptr, c_indices, c_values, n_corpus, c_features, ws, st);
+  if (rc) return rc;
+  SpParams sp{};
+  sp.q_indptr = q_indptr; sp.q_indices = q_indices; sp.q_values = q_values;
+  sp.bucket = reinterpret_cast<int32_t*>(ws); sp.post = reinterpret_cast<int2*>(ws + L.off_post);
+  sp.n_query = n_query; sp.n_corpus = n_corpus; sp.F = c_features; sp.k = 1; sp.splits = L.splits; sp.ranges = L.ranges; sp.exclude = 0;
+  sp.self = self ? 1 : 0; sp.tau = threshold;
+  sp.count = reinterpret_cast<unsigned long long*>(count); sp.capacity = (unsigned long long)capacity;
+  sp.pair_i = i_out; sp.pair_j = j_out; sp.pair_s = s_out;
+  if ((rc = sp_launch<kSpPairs>(sp, st))) return rc;
+  DAE_CHECK_LAUNCH("dae_csr_similarity_pairs");
   return DAE_OK;
 }

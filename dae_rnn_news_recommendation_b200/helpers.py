@@ -6,6 +6,10 @@ nearest-article lookup of main_autoencoder.py:307-318,352-359) -- SURVEY section
     top_k_similar(embeddings, k=10, corpus=None, metric='cosine') -> (index[Nq, k], score[Nq, k])    (no similarity matrix at all;
                                                                                                         dense or scipy sparse inputs)
     label_precision_at_k(index, query_labels, corpus_labels) -> float                                 (share of same-label neighbours)
+    similar_pairs(data, threshold, corpus=None, metric='cosine') -> (i[P], j[P], score[P])            (every pair with score >= threshold,
+                                                                                                        near-duplicates; no matrix)
+    duplicate_groups(i, j, n) -> group[n]                                                             (connected components of the pairs)
+    pair_label_agreement(i, j, labels, corpus_labels=None) -> dict                                    (precision / recall against labels)
     visualize_pairwise_similarity(labels, pairwise_similarity_metrics, ...) -> dict                   (rank 2: AUROC + box statistics)
     similarity_auroc(data, labels, metric='cosine', bins=1 << 21) -> dict                              (the same numbers on a score
                                                                                                         grid, without the matrix)
@@ -234,6 +238,186 @@ def label_precision_at_k(index, query_labels, corpus_labels):
     if not use.any():
         return float('nan')
     return float((hit.sum(1)[use] / n[use]).mean())
+
+
+SIMILAR_PAIRS_FIRST_CAPACITY = 1 << 20   # least slots of similar_pairs' first kernel call (12 MB)
+SIMILAR_PAIRS_SLOTS_PER_ROW = 16         # and per query row (192 B): a larger result takes a second call
+
+
+def _pairs_call(run, n_q, n_c, max_pairs, threshold, device):
+    """Two-call protocol of the thresholded-pair kernels: run(count, capacity, i, j, s) accumulates the exact count into the zeroed
+    device counter and fills the first `capacity` slots.  The first call gets max(SIMILAR_PAIRS_FIRST_CAPACITY,
+    SIMILAR_PAIRS_SLOTS_PER_ROW * n_q) slots (at most max_pairs); only a larger count reallocates exactly `count` slots and runs once
+    more.  Returns device tensors (i, j, s) sorted by (i, j)."""
+    count = torch.zeros(1, dtype=torch.int64, device=device)   # uint64 in the kernels
+    cap = min(max(SIMILAR_PAIRS_FIRST_CAPACITY, SIMILAR_PAIRS_SLOTS_PER_ROW * n_q), max_pairs)
+
+    def alloc(n):
+        return (torch.empty(max(n, 1), dtype=torch.int32, device=device), torch.empty(max(n, 1), dtype=torch.int32, device=device),
+                torch.empty(max(n, 1), dtype=torch.float32, device=device))
+    i, j, s = alloc(cap)
+    run(count, cap, i, j, s)
+    n = int(count.item())
+    if n > max_pairs:
+        raise ValueError('similar_pairs: %d pairs reach the threshold %r, more than max_pairs = %d; the output alone would take %d bytes '
+                         '(12 B per pair). Raise the threshold or max_pairs.' % (n, threshold, max_pairs, 12 * n))
+    if n > cap:
+        del i, j, s
+        i, j, s = alloc(n)
+        count.zero_()
+        run(count, n, i, j, s)
+        got = int(count.item())
+        if got != n:
+            raise RuntimeError('similar_pairs: the second call counted %d pairs, the first %d' % (got, n))
+    # canonical order: the unique int64 keys i * Nc + j radix-sorted with the scores as payload (dae_pairs_sort), which writes the
+    # decoded (i, j) into the key buffer it leaves free.  The first call's unused slots are released first, so from here on the
+    # peak is 24 B per pair (two key and two score buffers) plus the sort's fixed scratch (DESIGN 4.8).
+    if n == 0:
+        return i[:0], j[:0], s[:0]
+    keys = i[:n].to(torch.int64)
+    keys.mul_(n_c).add_(j[:n])
+    s = s[:n].clone() if n < s.shape[0] else s
+    del i, j
+    bits = max(1, (n_q * n_c - 1).bit_length())
+    need = (ctypes.c_int64 * 1)()
+    call('dae_pairs_sort_workspace', n, bits, ctypes.addressof(need))
+    ws = torch.empty(max(int(need[0]), 16), dtype=torch.uint8, device=device)
+    keys_alt = torch.empty_like(keys)
+    s_alt = torch.empty_like(s)
+    which = (ctypes.c_int32 * 1)()
+    call('dae_pairs_sort', n, n_c, bits, keys.data_ptr(), keys_alt.data_ptr(), s.data_ptr(), s_alt.data_ptr(), ws.data_ptr(), ws.numel(),
+         ctypes.addressof(which), _stream())
+    del ws
+    ij = (keys if which[0] else keys_alt).view(torch.int32)   # i in the first n int32s, j in the next n
+    s = s_alt if which[0] else s
+    del keys, keys_alt, s_alt
+    return ij[:n], ij[n:2 * n], s
+
+
+def _csr_similarity_pairs(q, c, self_mode, tau, max_pairs, threshold):
+    """similar_pairs of the DeviceCSR matrices q and c (c is q in self mode) through dae_csr_similarity_pairs: device tensors
+    (i, j, s) sorted by (i, j).  tau: the float32 threshold as a Python float (> 0)."""
+    dev = q.indptr.device
+    n_q, n_c = q.shape[0], c.shape[0]
+    need = (ctypes.c_int64 * 1)()
+    call('dae_csr_similarity_pairs_workspace', n_q, n_c, c.nnz, c.shape[1], ctypes.addressof(need))
+    ws = torch.empty(max(int(need[0]), 16), dtype=torch.uint8, device=dev)
+
+    def run(count, cap, i, j, s):
+        call('dae_csr_similarity_pairs', q.indptr.data_ptr(), q.indices.data_ptr(), q.values.data_ptr(), n_q, q.nnz, q.shape[1],
+             c.indptr.data_ptr(), c.indices.data_ptr(), c.values.data_ptr(), n_c, c.nnz, c.shape[1], 1 if self_mode else 0, tau,
+             ws.data_ptr(), ws.numel(), count.data_ptr(), cap, i.data_ptr(), j.data_ptr(), s.data_ptr(), _stream())
+    return _pairs_call(run, n_q, n_c, max_pairs, threshold, dev)
+
+
+def similar_pairs(data, threshold, corpus=None, metric='cosine', device='cuda:0', to_host=True, max_pairs=1 << 28):
+    """Every pair of rows whose similarity reaches `threshold` (near-duplicate articles), without forming the similarity matrix.
+    corpus=None: the pairs (i, j) with i > j of `data` against itself, scored S[i, j] with row i as the query.  With a corpus: every
+    (i, j) of a query row i and a corpus row j.  A pair qualifies when its fp32 score s >= float32(threshold); NaN never does.
+    metric: 'cosine' or 'linear kernel', as in top_k_similar, and the scores are those of top_k_similar bit for bit: dense arrays or
+    tensors run on the tensor cores (dae_similarity_pairs_bf16x3, bf16x3), scipy sparse matrices through dae_csr_similarity_pairs
+    (fp32 sums over the shared columns), where the threshold must be > 0.  Queries and corpus must be both dense or both sparse.
+    Memory beyond the inputs: the operands (dense) or the corpus postings (sparse), the output and the sort of its keys.  The first
+    kernel call counts the pairs into max(2^20, 16 Nq) slots (12 B each); more than `max_pairs` qualifying pairs then raise
+    ValueError before the full output is allocated, and more than the first capacity take exactly one more call.
+    Returns (i int32, j int32, score float32), sorted by (i, j), as ndarrays (device tensors with to_host=False)."""
+    if metric not in ('cosine', 'linear kernel'):
+        raise ValueError("similar_pairs: metric = %r: 'cosine' or 'linear kernel'" % (metric,))
+    if corpus is not None and sp.issparse(data) != sp.issparse(corpus):
+        raise ValueError('similar_pairs: queries and corpus must be both sparse or both dense')
+    try:
+        with np.errstate(over='ignore'):   # out of float32 range: inf, refused below
+            tau = np.float32(threshold)
+    except (TypeError, ValueError):
+        raise ValueError('similar_pairs: threshold %r is not a number' % (threshold,))
+    if not np.isfinite(tau):
+        raise ValueError('similar_pairs: threshold %r is not finite (as float32)' % (threshold,))
+    sparse = sp.issparse(data)
+    if sparse and not tau > 0:
+        raise ValueError('similar_pairs: threshold %r must be > 0 on sparse input: a pair that shares no column scores exactly 0, so '
+                         'almost every pair would qualify' % (threshold,))
+    if not isinstance(max_pairs, (int, np.integer)) or max_pairs < 0:
+        raise ValueError('similar_pairs: max_pairs = %r must be a non-negative integer' % (max_pairs,))
+    max_pairs = int(max_pairs)
+    tau = float(tau)
+    if sparse:
+        if corpus is not None and corpus.shape[1] != data.shape[1]:
+            raise ValueError('similar_pairs: corpus rows have %d columns, queries %d' % (corpus.shape[1], data.shape[1]))
+        q = DeviceCSR(_csr_operand(data, metric), device)
+        c = q if corpus is None else DeviceCSR(_csr_operand(corpus, metric), device)
+        i, j, s = _csr_similarity_pairs(q, c, corpus is None, tau, max_pairs, threshold)
+    else:
+        norm_kind = 2 if metric == 'cosine' else 0
+        x = _as_device_dense(data, device)
+        n_q, h = x.shape
+        q = _normalised_operands(x, norm_kind)[:2]
+        if corpus is None:
+            c, n_c = q, n_q
+        else:
+            xc = _as_device_dense(corpus, device)
+            if xc.shape[1] != h:
+                raise ValueError('similar_pairs: corpus rows have %d columns, queries %d' % (xc.shape[1], h))
+            n_c = xc.shape[0]
+            c = _normalised_operands(xc, norm_kind)[:2]
+
+        def run(count, cap, i, j, s):
+            call('dae_similarity_pairs_bf16x3', n_q, n_c, h, q[0].data_ptr(), q[1].data_ptr(), q[0].stride(0), c[0].data_ptr(),
+                 c[1].data_ptr(), c[0].stride(0), 1 if corpus is None else 0, tau, count.data_ptr(), cap, i.data_ptr(), j.data_ptr(),
+                 s.data_ptr(), _stream())
+        i, j, s = _pairs_call(run, n_q, n_c, max_pairs, threshold, device)
+    if to_host:
+        return i.cpu().numpy(), j.cpu().numpy(), s.cpu().numpy()
+    return i, j, s
+
+
+def _host_ints(a):
+    return np.asarray(a.cpu() if isinstance(a, torch.Tensor) else a).reshape(-1)
+
+
+def duplicate_groups(i, j, n):
+    """Connected components of the graph on n rows whose edges are the pairs (i[t], j[t]) (similar_pairs' output): int32 [n], each
+    row labelled by the smallest row index of its component, so a row without any pair is its own group.  Runs on the host
+    (scipy.sparse.csgraph)."""
+    from scipy.sparse.csgraph import connected_components
+    i, j = _host_ints(i).astype(np.int64), _host_ints(j).astype(np.int64)
+    n = int(n)
+    if n < 0 or i.shape != j.shape:
+        raise ValueError('duplicate_groups: %d row and %d column indices for n = %d' % (i.size, j.size, n))
+    if i.size and (min(i.min(), j.min()) < 0 or max(i.max(), j.max()) >= n):
+        raise ValueError('duplicate_groups: pair indices outside [0, %d)' % n)
+    if n == 0:
+        return np.zeros(0, dtype=np.int32)
+    g = sp.coo_matrix((np.ones(i.size, dtype=np.int8), (i, j)), shape=(n, n)).tocsr()
+    _, comp = connected_components(g, directed=False)
+    first = np.unique(comp, return_index=True)[1]   # the first (smallest) row of each component, components in label order
+    return first[comp].astype(np.int32)
+
+
+def pair_label_agreement(i, j, labels, corpus_labels=None):
+    """How well thresholded pairs (similar_pairs' i, j) agree with known groups such as the UCI `story` labels.
+    Pairs with a row labelled -1 on either side are skipped.  Returns {'pairs': the pairs counted, 'precision': the share of them
+    whose two labels are equal, 'recall': those same-label pairs over all same-label pairs -- sum_l n_l (n_l - 1) / 2 against itself
+    (corpus_labels None: i and j index `labels`), sum_l n_q(l) n_c(l) against a corpus}.  NaN where a denominator is 0."""
+    i, j = _host_ints(i).astype(np.int64), _host_ints(j).astype(np.int64)
+    ql = _host_ints(labels.values if hasattr(labels, 'values') else labels)
+    cl = ql if corpus_labels is None else _host_ints(corpus_labels.values if hasattr(corpus_labels, 'values') else corpus_labels)
+    if i.shape != j.shape:
+        raise ValueError('pair_label_agreement: %d row and %d column indices' % (i.size, j.size))
+    li, lj = ql[i], cl[j]
+    use = (li != -1) & (lj != -1)
+    n_pairs = int(use.sum())
+    same = int((use & (li == lj)).sum())
+    qv = ql[ql != -1]
+    if corpus_labels is None:
+        counts = np.unique(qv, return_counts=True)[1].astype(np.int64)
+        total = int((counts * (counts - 1) // 2).sum())
+    else:
+        cv = cl[cl != -1]
+        uq, nq = np.unique(qv, return_counts=True)
+        uc, nc = np.unique(cv, return_counts=True)
+        _, a, b = np.intersect1d(uq, uc, return_indices=True)
+        total = int((nq[a].astype(np.int64) * nc[b].astype(np.int64)).sum())
+    return {'pairs': n_pairs, 'precision': same / n_pairs if n_pairs else float('nan'), 'recall': same / total if total else float('nan')}
 
 
 def _group_sizes(labels):

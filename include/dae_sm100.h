@@ -402,6 +402,44 @@ int dae_csr_similarity_pair_hist(const int64_t* indptr, const int32_t* indices, 
                                  int64_t workspace_bytes, uint64_t* hist, double* sums, void* stream);
 int dae_csr_similarity_pair_hist_workspace(int32_t n, int64_t nnz, int32_t n_features, int64_t* bytes);
 
+/* ---- near-duplicate articles: every pair at or above a similarity threshold, without the similarity matrix --------
+ * Pairs: self mode (self != 0, the corpus arguments are the query arguments: same pointers and sizes) lists the pairs (i, j) with
+ *   i > j and S[i, j] >= threshold, where S[i, j] is computed with i as the query (first operand) row -- the convention of
+ *   dae_similarity_pair_hist_bf16x3; S[j, i] is not evaluated and need not have the same bits.  Corpus mode (self = 0) lists every
+ *   (i, j), i < n_query, j < n_corpus, with S[i, j] >= threshold.
+ * Threshold: compared as s >= threshold in fp32 (the caller converts it to float once); a NaN score never qualifies.
+ * Output: *count, a uint64 the caller zeroes, is ACCUMULATED by the exact number of qualifying pairs.  The first `capacity` of them
+ *   (in unspecified order: atomic slot reservation) are written as i_out[s], j_out[s] (int32) and s_out[s] (fp32, the score) for
+ *   s < capacity; nothing is written at or past capacity, so a count above capacity means the call must be repeated with at
+ *   least count slots (and a zeroed counter).  capacity = 0 only counts (the outputs may then be null).
+ * Every argument is checked before any CUDA call.
+ * dae_similarity_pairs_bf16x3: dense rows as bf16 hi / lo pairs (as dae_similarity_topk_bf16x3: ldq, ldc >= dim and multiples of
+ *   8, operands 16-byte aligned); the tiles, operand ring and k16 order of dae_similarity_topk_bf16x3, so each score has the bits
+ *   top-k reports for the same (i, j).  Self mode computes only the tiles on and below the diagonal.  threshold finite.
+ * dae_csr_similarity_pairs: CSR rows (the layout of dae_csr_similarity_topk, corpus nnz < 2^31) with its scores, bit for bit:
+ *   fp32 from 0, one rounded product per shared column in increasing column order, no FMA.  threshold finite and > 0: a pair
+ *   sharing no column scores exactly 0 and is never listed.  workspace: 16-byte aligned, at least
+ *   dae_csr_similarity_pairs_workspace bytes (the corpus postings and their bucket offsets).
+ */
+int dae_similarity_pairs_bf16x3(int32_t n_query, int32_t n_corpus, int32_t dim, const void* q_hi, const void* q_lo, int64_t ldq,
+                                const void* c_hi, const void* c_lo, int64_t ldc, int32_t self, float threshold, uint64_t* count,
+                                int64_t capacity, int32_t* i_out, int32_t* j_out, float* s_out, void* stream);
+int dae_csr_similarity_pairs(const int64_t* q_indptr, const int32_t* q_indices, const float* q_values, int32_t n_query,
+                             int64_t q_nnz, int32_t q_features, const int64_t* c_indptr, const int32_t* c_indices,
+                             const float* c_values, int32_t n_corpus, int64_t c_nnz, int32_t c_features, int32_t self,
+                             float threshold, void* workspace, int64_t workspace_bytes, uint64_t* count, int64_t capacity,
+                             int32_t* i_out, int32_t* j_out, float* s_out, void* stream);
+int dae_csr_similarity_pairs_workspace(int32_t n_query, int32_t n_corpus, int64_t corpus_nnz, int32_t n_features, int64_t* bytes);
+/* dae_pairs_sort: the canonical order of n pairs.  keys[t] = i * n_corpus + j (unique, below 2^key_bits) are sorted ascending with
+ *   s[t] as the payload on a double-buffered radix sort: keys_alt and s_alt (n entries each, distinct from keys and s) are the
+ *   alternate buffers, and the workspace (at least dae_pairs_sort_workspace bytes) does not grow with n beyond the sort's tile
+ *   bookkeeping.  On return *which (host int32) = 0 when the sorted keys and scores are in keys / s, 1 when in keys_alt / s_alt; the
+ *   other key buffer holds the decoded pairs as int32: i in its first n entries, j in the next n.  n < 2^31.
+ */
+int dae_pairs_sort(int64_t n, int32_t n_corpus, int32_t key_bits, uint64_t* keys, uint64_t* keys_alt, float* s, float* s_alt,
+                   void* workspace, int64_t workspace_bytes, int32_t* which, void* stream);
+int dae_pairs_sort_workspace(int64_t n, int32_t key_bits, int64_t* bytes);
+
 /* ---- deterministic training step (DESIGN 4.7) ----------------------------------------------------------------------------
  * Variants of the step's kernels in which no floating-point sum depends on timing: with the same inputs, build and GPU model they
  * give the same bits on every run.  Each takes caller-owned workspace; the *_workspace / *_parts queries size it.

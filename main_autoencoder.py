@@ -69,6 +69,14 @@ def build_parser():
     ap.add_argument('--top_k_input', action='store_true', default=False,
                     help='with --top_k K: also rank by the input vectors (cosine for binary, linear kernel for tf-idf), save '
                          'article_top_k_input_{index,score}[_validate].npy and report their label precision next to the embedding\'s')
+    ap.add_argument('--dedup_threshold', type=float, default=0.0,
+                    help='T > 0: after transform, list every pair of training articles whose embedding cosine similarity is >= T '
+                         '(near-duplicates) and every (validation, training) pair, save them with their duplicate groups as '
+                         'article_duplicates[_validate].npz (i, j, score, group) and report the pair and group counts and the '
+                         'precision / recall against --label; 0 = off')
+    ap.add_argument('--dedup_input', action='store_true', default=False,
+                    help='with --dedup_threshold T: the same on the input vectors (cosine for binary, linear kernel for tf-idf), saved '
+                         'as article_duplicates_input[_validate].npz and reported next to the embedding\'s numbers')
     ap.add_argument('--eval_all_rows', action='store_true', default=False,
                     help='evaluate sets above 20 000 rows instead of skipping them: AUROC and box statistics from score histograms '
                          '(helpers.similarity_auroc, reported with their error bound) and the nearest article through top_k_similar')
@@ -125,6 +133,8 @@ def check_flags(F):
     assert F.label in ['category_publish_name', 'story']
     assert 0 <= F.top_k <= 32
     assert not F.top_k_input or F.top_k > 0, '--top_k_input needs --top_k K > 0'
+    assert F.dedup_threshold >= 0.0
+    assert not F.dedup_input or F.dedup_threshold > 0, '--dedup_input needs --dedup_threshold T > 0'
     if F.input_format == 'tfidf':
         assert F.loss_func in ['mean_squared', 'cosine_proximity']
     if F.main_dir == '':
@@ -317,6 +327,38 @@ def recommend_top_k_input(F, model, trX, vlX, trL, vlL, emb_out):
     return out
 
 
+def find_duplicates(F, model, X, X_v, trL, vlL, metric, name, emb_out=None):
+    """--dedup_threshold T: every pair of training rows of X with similarity >= T (self) and every (validation, training) pair
+    (corpus), through helpers.similar_pairs, without the similarity matrix.  Saved under data_dir as <name>[_validate].npz with
+    i, j, score and group (helpers.duplicate_groups of the query rows; for the validation set the components link validation rows
+    through the training rows they match, and carry the smallest validation row index); the pair count, the groups of two or more
+    articles and the precision / recall against the labels are returned and printed (next to emb_out's when given)."""
+    from dae_rnn_news_recommendation_b200 import helpers
+    out = {}
+    key = name[len('article_'):]
+    print('find near-duplicate articles (%s, %s >= %g)' % (key, metric, F.dedup_threshold))
+    for split, Q, lab in (('', X, trL), ('_validate', X_v, vlL)):
+        if Q is None or Q.shape[0] == 0:
+            continue
+        i, j, score = helpers.similar_pairs(Q, F.dedup_threshold, corpus=None if split == '' else X, metric=metric)
+        # validation: components of the graph on validation rows 0 .. Nv-1 and training rows Nv .. Nv+Nt-1
+        off = 0 if split == '' else Q.shape[0]
+        g_all = helpers.duplicate_groups(i, j + off, Q.shape[0] + (0 if split == '' else X.shape[0]))
+        group = g_all[:Q.shape[0]]
+        np.savez(model.data_dir + name + split + '.npz', i=i, j=j, score=score, group=group)
+        agree = helpers.pair_label_agreement(i, j, lab, None if split == '' else trL)
+        stats = {'pairs': int(i.shape[0]), 'groups': int((np.bincount(g_all) >= 2).sum()), 'precision': agree['precision'],
+                 'recall': agree['recall']}
+        out[key + split] = stats
+        line = '%s%s: %d pairs, %d groups of >= 2 articles, label precision %.4f recall %.4f' % (
+            key, split, stats['pairs'], stats['groups'], stats['precision'], stats['recall'])
+        if emb_out is not None and ('duplicates' + split) in emb_out:
+            e = emb_out['duplicates' + split]
+            line += '  (embedding: %d pairs, %d groups, precision %.4f recall %.4f)' % (e['pairs'], e['groups'], e['precision'], e['recall'])
+        print(line)
+    return out
+
+
 def main(argv=None):
     F = check_flags(apply_env_overrides(build_parser().parse_args(argv)))
     print(__file__ + ': Start')
@@ -353,6 +395,11 @@ def main(argv=None):
         model.evaluation.update(recommend_top_k(F, model, enc, enc_v, trL, vlL))
         if F.top_k_input:
             model.evaluation.update(recommend_top_k_input(F, model, trX, vlX, trL, vlL, model.evaluation))
+    if F.dedup_threshold > 0:
+        model.evaluation.update(find_duplicates(F, model, enc, enc_v, trL, vlL, 'cosine', 'article_duplicates'))
+        if F.dedup_input:
+            in_metric = 'cosine' if F.input_format == 'binary' else 'linear kernel'
+            model.evaluation.update(find_duplicates(F, model, trX, vlX, trL, vlL, in_metric, 'article_duplicates_input', model.evaluation))
     print(__file__ + ': End')
     return model
 
