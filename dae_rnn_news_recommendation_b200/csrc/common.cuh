@@ -1,6 +1,7 @@
 // Shared helpers for libdae_sm100.so (built for sm_90a).
 #pragma once
 #include <cuda_runtime.h>
+#include <climits>
 #include <cstdint>
 #include <cstdio>
 #include <cstring>

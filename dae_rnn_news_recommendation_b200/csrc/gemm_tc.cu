@@ -858,6 +858,9 @@ struct TopkParams {
   int exclude;                       // != 0: column i + diag_offset is not a candidate of row i
   int64_t diag_offset;
   float* ws_val; int32_t* ws_idx;    // [M x 2 splits x k] partial lists
+  // topk_kernel<KMAX, true>: per-row exclusion lists (CSR structure, rows sorted, no duplicates, indices in [0, N)).  Last, so the
+  // fields above keep their parameter offsets in the plain instantiations.
+  const int64_t* ex_indptr; const int32_t* ex_indices;
 };
 
 // (row block, column-tile range) work items, items blockIdx.x, blockIdx.x + gridDim.x, ...; next() returns one column tile at a time,
@@ -915,7 +918,11 @@ __device__ __forceinline__ void topk_offer(float (&sv)[KMAX], int (&si)[KMAX], f
   thr = t;
 }
 
-template <int KMAX>
+// EXCL: the columns in row m's exclusion list are never candidates.  Before scanning a tile, the epilogue thread writes -inf over
+// the listed columns of its own (row, 64-column half) staging run -- its alone until it arrives on `drained` -- and -inf never beats
+// thr.  A cursor into the sorted list, placed by binary search at the item's first column, only moves forward during the item; the
+// next listed column waits in a register, so a tile without a listed column costs one compare.
+template <int KMAX, bool EXCL = false>
 __global__ void __launch_bounds__(kDecodeThreads, 1) topk_kernel(const __grid_constant__ CUtensorMap tm_a_hi,
                                                                  const __grid_constant__ CUtensorMap tm_a_lo,
                                                                  const __grid_constant__ CUtensorMap tm_b_hi,
@@ -988,6 +995,8 @@ __global__ void __launch_bounds__(kDecodeThreads, 1) topk_kernel(const __grid_co
     int si[KMAX];
     float thr = neg_inf();
     int m = 0, excl = -1;
+    [[maybe_unused]] int64_t ex_cur = 0, ex_end = 0;   // EXCL: cursor into row m's list and its end
+    [[maybe_unused]] int ex_next = INT_MAX;            // EXCL: the list entry at the cursor (INT_MAX past the end)
     uint32_t tphase = 0;
     int mb, nb, kb0, kb1;
     while (sched.next(mb, nb, kb0, kb1)) {
@@ -998,10 +1007,31 @@ __global__ void __launch_bounds__(kDecodeThreads, 1) topk_kernel(const __grid_co
         m = mb * BLOCK_M + row_in_tile;
         const int64_t e = (int64_t)m + tp.diag_offset;
         excl = (tp.exclude && e >= 0 && e < p.N) ? (int)e : -1;
+        if constexpr (EXCL) {
+          ex_next = INT_MAX;
+          if (m < p.M) {
+            const int c_first = nb * BLOCK_N + half * HALF_N;   // the first column this thread sees in the item
+            int64_t lo = tp.ex_indptr[m], hi = tp.ex_indptr[m + 1];
+            ex_end = hi;
+            while (lo < hi) {
+              const int64_t mid = lo + ((hi - lo) >> 1);
+              if (tp.ex_indices[mid] < c_first) lo = mid + 1; else hi = mid;
+            }
+            ex_cur = lo;
+            if (ex_cur < ex_end) ex_next = tp.ex_indices[ex_cur];
+          }
+        }
       }
       const int n0 = nb * BLOCK_N + half * HALF_N;
       mbar_wait(&staged_bar[h], tphase);
       if (m < p.M) {
+        if constexpr (EXCL) {
+          float* wrow = stg + row_in_tile * SROW + half * HALF_N;
+          while (ex_next < n0 + HALF_N) {   // listed columns of the other half (ex_next < n0) are skipped
+            if (ex_next >= n0) wrow[ex_next - n0] = neg_inf();
+            ex_next = (++ex_cur < ex_end) ? tp.ex_indices[ex_cur] : INT_MAX;
+          }
+        }
 #pragma unroll 1
         for (int c = 0; c < HALF_N; c += 4) {
           const float4 v = *reinterpret_cast<const float4*>(srow + c);
@@ -1587,7 +1617,7 @@ static int launch_decode(const Operand& A, const Operand& B, const GemmParams& p
 }
 
 // fused similarity + k-best: Q [M x K] and C [N x K], both K-major; one persistent CTA per SM over the (row block, split) work items
-template <int KMAX>
+template <int KMAX, bool EXCL>
 static int launch_topk(const Operand& A, const Operand& B, const TopkParams& tp, cudaStream_t st) {
   CUtensorMap ta_hi, ta_lo, tb_hi, tb_lo;
   int rc;
@@ -1598,7 +1628,7 @@ static int launch_topk(const Operand& A, const Operand& B, const TopkParams& tp,
   if ((rc = make_map(&tb_lo, B.lo, p.K, p.N, B.ld, kDecodeN, kTopkBK))) return rc;
   // operand ring + accumulator staging tile + alignment slack
   constexpr int smem = kTopkStages * (2 * BLOCK_M * kTopkBK * 2 + 2 * kDecodeN * kTopkBK * 2) + BLOCK_M * (kDecodeN + 4) * 4 + 1024;
-  auto kern = topk_kernel<KMAX>;
+  auto kern = topk_kernel<KMAX, EXCL>;
   static bool attr_done[64] = {false};
   if ((rc = ensure_smem_attr(kern, smem, attr_done))) return rc;
   const int items = ((p.M + BLOCK_M - 1) / BLOCK_M) * tp.splits;
@@ -1961,11 +1991,47 @@ extern "C" int dae_similarity_topk_bf16x3(int32_t n_query, int32_t n_corpus, int
   tp.ws_val = reinterpret_cast<float*>(workspace);
   tp.ws_idx = reinterpret_cast<int32_t*>(reinterpret_cast<float*>(workspace) + (int64_t)n_query * 2 * s * k);
   Operand A{q_hi, q_lo, ldq, 0}, B{c_hi, c_lo, ldc, 0};
-  int rc = (k <= 16) ? launch_topk<16>(A, B, tp, st) : launch_topk<32>(A, B, tp, st);
+  int rc = (k <= 16) ? launch_topk<16, false>(A, B, tp, st) : launch_topk<32, false>(A, B, tp, st);
   if (rc) return rc;
   DAE_CHECK_LAUNCH("dae_similarity_topk_bf16x3");
   topk_merge_kernel<<<(n_query + 7) / 8, 256, 0, st>>>(tp.ws_val, tp.ws_idx, n_query, 2 * s, k, idx_out, val_out);
   DAE_CHECK_LAUNCH("dae_similarity_topk_bf16x3 (merge)");
+  return DAE_OK;
+}
+
+extern "C" int dae_similarity_topk_excl_bf16x3(int32_t n_query, int32_t n_corpus, int32_t dim, const void* q_hi, const void* q_lo,
+                                               int64_t ldq, const void* c_hi, const void* c_lo, int64_t ldc, int32_t k,
+                                               int64_t diag_offset, int32_t exclude, int32_t splits, void* workspace,
+                                               int64_t workspace_bytes, int32_t* idx_out, float* val_out, const int64_t* ex_indptr,
+                                               const int32_t* ex_indices, int64_t ex_nnz, void* stream) {
+  DAE_REQUIRE(q_hi && q_lo && c_hi && c_lo && workspace && idx_out && val_out && ex_indptr && (ex_nnz == 0 || ex_indices),
+              "dae_similarity_topk_excl_bf16x3: null pointer");
+  DAE_REQUIRE(n_query > 0 && n_corpus > 0 && dim > 0 && ex_nnz >= 0, "dae_similarity_topk_excl_bf16x3: bad sizes");
+  DAE_REQUIRE(k >= 1 && k <= kTopkMaxK, "dae_similarity_topk_excl_bf16x3: k = %d is outside the supported range 1 <= k <= %d", k,
+              kTopkMaxK);
+  DAE_REQUIRE(ldq >= dim && ldc >= dim && ldq % 8 == 0 && ldc % 8 == 0,
+              "dae_similarity_topk_excl_bf16x3: leading dimensions must cover dim and be multiples of 8 (TMA 16-byte strides)");
+  DAE_REQUIRE(((uintptr_t)q_hi | (uintptr_t)q_lo | (uintptr_t)c_hi | (uintptr_t)c_lo | (uintptr_t)workspace) % 16 == 0 &&
+                  (uintptr_t)ex_indptr % 8 == 0 && (uintptr_t)ex_indices % 4 == 0,
+              "dae_similarity_topk_excl_bf16x3: operands and workspace must be 16-byte, ex_indptr 8-byte, ex_indices 4-byte aligned");
+  const int s = topk_splits(n_query, n_corpus, splits);
+  const int64_t need = topk_workspace_bytes(n_query, k, s);
+  DAE_REQUIRE(workspace_bytes >= need,
+              "dae_similarity_topk_excl_bf16x3: workspace of %lld bytes, %lld needed (dae_similarity_topk_workspace)",
+              (long long)workspace_bytes, (long long)need);
+  cudaStream_t st = (cudaStream_t)stream;
+  TopkParams tp{};
+  tp.g.M = n_query; tp.g.N = n_corpus; tp.g.K = dim; tp.g.k_splits = 1; tp.g.alpha = 1.0f; tp.g.special_col = -1;
+  tp.k = k; tp.splits = s; tp.exclude = exclude ? 1 : 0; tp.diag_offset = diag_offset;
+  tp.ws_val = reinterpret_cast<float*>(workspace);
+  tp.ws_idx = reinterpret_cast<int32_t*>(reinterpret_cast<float*>(workspace) + (int64_t)n_query * 2 * s * k);
+  tp.ex_indptr = ex_indptr; tp.ex_indices = ex_indices;
+  Operand A{q_hi, q_lo, ldq, 0}, B{c_hi, c_lo, ldc, 0};
+  int rc = (k <= 16) ? launch_topk<16, true>(A, B, tp, st) : launch_topk<32, true>(A, B, tp, st);
+  if (rc) return rc;
+  DAE_CHECK_LAUNCH("dae_similarity_topk_excl_bf16x3");
+  topk_merge_kernel<<<(n_query + 7) / 8, 256, 0, st>>>(tp.ws_val, tp.ws_idx, n_query, 2 * s, k, idx_out, val_out);
+  DAE_CHECK_LAUNCH("dae_similarity_topk_excl_bf16x3 (merge)");
   return DAE_OK;
 }
 

@@ -162,9 +162,12 @@ struct SpParams {
   unsigned long long* count;
   unsigned long long capacity;
   int32_t* pair_i; int32_t* pair_j; float* pair_s;
+  // kSpTopkExcl: per-query exclusion lists (CSR structure, rows sorted, no duplicates, indices in [0, n_corpus)).  Last, so the
+  // fields above keep their parameter offsets in the other modes.
+  const int64_t* ex_indptr; const int32_t* ex_indices;
 };
 
-enum SpMode { kSpTopk, kSpHist, kSpPairs };
+enum SpMode { kSpTopk, kSpHist, kSpPairs, kSpTopkExcl };
 
 // offer (v, col) to the warp's list (lane j < k holds entry j); warp-uniform arguments
 __device__ __forceinline__ void sp_offer(float v, int col, int n_corpus, int excl, int k, int lane, float& lv, int& li, float& thr) {
@@ -183,6 +186,9 @@ __device__ __forceinline__ void sp_offer(float v, int col, int n_corpus, int exc
 // (group, bin) in one red.global.add.u64); the zero slots, most of them, are only counted per group in registers and added with
 // one atomic per group when the warp is done.  kSpPairs: the scan emits the slots with s >= tau (c < q in self mode, whose ranges
 // stop below q as in kSpHist); a warp with any hit in a 128-slot chunk reserves its slots with one atomicAdd (pair_slots).
+// kSpTopkExcl: kSpTopk, but the corpus rows in q's exclusion list are never candidates.  Before each slab scan the warp writes -inf
+// into the listed slots of the range, 32 list entries per load from a cursor that only moves forward (placed by binary search at
+// the split's first row); -inf never beats thr, and the scan zeroes those slots as it does the others.
 template <SpMode MODE>
 __global__ void __launch_bounds__(kSpWarps * 32, 3) sp_topk_kernel(const SpParams p) {
   constexpr bool HIST = MODE == kSpHist;
@@ -213,6 +219,17 @@ __global__ void __launch_bounds__(kSpWarps * 32, 3) sp_topk_kernel(const SpParam
   for (int j = lane; j < kSpW / 4; j += 32) slab4[j] = make_float4(0.f, 0.f, 0.f, 0.f);
   float lv = neg_inf(), thr = neg_inf();
   int li = -1;
+  [[maybe_unused]] int64_t ex_cur = 0, ex_end = 0;   // kSpTopkExcl: cursor into q's list and its end (warp-uniform)
+  if constexpr (MODE == kSpTopkExcl) {
+    int64_t lo = p.ex_indptr[q], hi = p.ex_indptr[q + 1];
+    ex_end = hi;
+    const int c_first = r0 * kSpW;
+    while (lo < hi) {
+      const int64_t mid = lo + ((hi - lo) >> 1);
+      if (p.ex_indices[mid] < c_first) lo = mid + 1; else hi = mid;
+    }
+    ex_cur = lo;
+  }
   __syncwarp();
   for (int r = r0; r < r1; ++r) {
     const int32_t* brow = p.bucket + (int64_t)r * p.F;
@@ -279,6 +296,18 @@ __global__ void __launch_bounds__(kSpWarps * 32, 3) sp_topk_kernel(const SpParam
         }
       }
     } else {
+      if constexpr (MODE == kSpTopkExcl) {
+        // -inf into the listed slots of this range; the list is sorted, so the lanes below the range's end form a prefix
+        while (ex_cur < ex_end) {
+          const int c = (ex_cur + lane < ex_end) ? p.ex_indices[ex_cur + lane] : INT_MAX;
+          const bool in = c < base + kSpW;
+          if (in) slab[c - base] = neg_inf();
+          const int n_in = __popc(__ballot_sync(kFull, in));
+          ex_cur += n_in;
+          if (n_in < 32) break;
+        }
+        __syncwarp();
+      }
       // scan the slab in increasing corpus index (lane-major float4s), offer what beats the k-th score, zero it for the next range
       for (int j0 = 0; j0 < width; j0 += 128) {
         const float4 x = slab4[j0 / 4 + lane];
@@ -378,20 +407,23 @@ extern "C" int dae_csr_similarity_topk_workspace(int32_t n_query, int32_t n_corp
   return DAE_OK;
 }
 
-extern "C" int dae_csr_similarity_topk(const int64_t* q_indptr, const int32_t* q_indices, const float* q_values, int32_t n_query,
-                                       int64_t q_nnz, int32_t q_features, const int64_t* c_indptr, const int32_t* c_indices,
-                                       const float* c_values, int32_t n_corpus, int64_t c_nnz, int32_t c_features, int32_t k,
-                                       int64_t diag_offset, int32_t exclude, int32_t splits, void* workspace, int64_t workspace_bytes,
-                                       int32_t* idx_out, float* val_out, void* stream) {
+// dae_csr_similarity_topk (excl false) and dae_csr_similarity_topk_excl (excl true, the lists ex_indptr / ex_indices)
+static int csr_topk(const char* fn, const int64_t* q_indptr, const int32_t* q_indices, const float* q_values, int32_t n_query,
+                    int64_t q_nnz, int32_t q_features, const int64_t* c_indptr, const int32_t* c_indices, const float* c_values,
+                    int32_t n_corpus, int64_t c_nnz, int32_t c_features, int32_t k, int64_t diag_offset, int32_t exclude,
+                    int32_t splits, void* workspace, int64_t workspace_bytes, int32_t* idx_out, float* val_out, bool excl,
+                    const int64_t* ex_indptr, const int32_t* ex_indices, int64_t ex_nnz, void* stream) {
   DAE_REQUIRE(q_indptr && c_indptr && workspace && idx_out && val_out && (q_nnz == 0 || (q_indices && q_values)) &&
-              (c_nnz == 0 || (c_indices && c_values)), "dae_csr_similarity_topk: null pointer");
-  DAE_REQUIRE(n_query > 0 && n_corpus > 0 && q_features > 0 && c_features > 0 && q_nnz >= 0 && c_nnz >= 0 && c_nnz < INT32_MAX,
-              "dae_csr_similarity_topk: bad sizes");
-  DAE_REQUIRE(k >= 1 && k <= kSpMaxK, "dae_csr_similarity_topk: k = %d is outside the supported range 1 <= k <= %d", k, kSpMaxK);
-  DAE_REQUIRE(q_features == c_features, "dae_csr_similarity_topk: queries have %d features, the corpus %d", q_features, c_features);
-  DAE_REQUIRE((uintptr_t)workspace % 16 == 0, "dae_csr_similarity_topk: workspace must be 16-byte aligned");
+              (c_nnz == 0 || (c_indices && c_values)) && (!excl || (ex_indptr && (ex_nnz == 0 || ex_indices))), "%s: null pointer", fn);
+  DAE_REQUIRE(n_query > 0 && n_corpus > 0 && q_features > 0 && c_features > 0 && q_nnz >= 0 && c_nnz >= 0 && c_nnz < INT32_MAX &&
+              (!excl || ex_nnz >= 0), "%s: bad sizes", fn);
+  DAE_REQUIRE(k >= 1 && k <= kSpMaxK, "%s: k = %d is outside the supported range 1 <= k <= %d", fn, k, kSpMaxK);
+  DAE_REQUIRE(q_features == c_features, "%s: queries have %d features, the corpus %d", fn, q_features, c_features);
+  DAE_REQUIRE((uintptr_t)workspace % 16 == 0, "%s: workspace must be 16-byte aligned", fn);
+  DAE_REQUIRE(!excl || ((uintptr_t)ex_indptr % 8 == 0 && (uintptr_t)ex_indices % 4 == 0),
+              "%s: ex_indptr must be 8-byte, ex_indices 4-byte aligned", fn);
   const SpLayout L = sp_layout(n_query, n_corpus, c_nnz, c_features, k, splits);
-  DAE_REQUIRE(workspace_bytes >= L.total, "dae_csr_similarity_topk: workspace of %lld bytes, %lld needed (dae_csr_similarity_topk_workspace)",
+  DAE_REQUIRE(workspace_bytes >= L.total, "%s: workspace of %lld bytes, %lld needed (dae_csr_similarity_topk_workspace)", fn,
               (long long)workspace_bytes, (long long)L.total);
   cudaStream_t st = (cudaStream_t)stream;
   uint8_t* ws = reinterpret_cast<uint8_t*>(workspace);
@@ -408,13 +440,35 @@ extern "C" int dae_csr_similarity_topk(const int64_t* q_indptr, const int32_t* q
   sp.idx_out = idx_out; sp.val_out = val_out;
   sp.ws_val = reinterpret_cast<float*>(ws + L.off_val);
   sp.ws_idx = reinterpret_cast<int32_t*>(ws + L.off_idx);
-  if ((rc = sp_launch<kSpTopk>(sp, st))) return rc;
-  DAE_CHECK_LAUNCH("dae_csr_similarity_topk");
+  sp.ex_indptr = ex_indptr; sp.ex_indices = ex_indices;
+  if ((rc = excl ? sp_launch<kSpTopkExcl>(sp, st) : sp_launch<kSpTopk>(sp, st))) return rc;
+  DAE_CHECK_LAUNCH(fn);
   if (L.splits > 1) {
     topk_merge_kernel<<<(n_query + 7) / 8, 256, 0, st>>>(sp.ws_val, sp.ws_idx, n_query, L.splits, k, idx_out, val_out);
-    DAE_CHECK_LAUNCH("dae_csr_similarity_topk (merge)");
+    DAE_CHECK_LAUNCH("sparse similarity top-k (merge)");
   }
   return DAE_OK;
+}
+
+extern "C" int dae_csr_similarity_topk(const int64_t* q_indptr, const int32_t* q_indices, const float* q_values, int32_t n_query,
+                                       int64_t q_nnz, int32_t q_features, const int64_t* c_indptr, const int32_t* c_indices,
+                                       const float* c_values, int32_t n_corpus, int64_t c_nnz, int32_t c_features, int32_t k,
+                                       int64_t diag_offset, int32_t exclude, int32_t splits, void* workspace, int64_t workspace_bytes,
+                                       int32_t* idx_out, float* val_out, void* stream) {
+  return csr_topk("dae_csr_similarity_topk", q_indptr, q_indices, q_values, n_query, q_nnz, q_features, c_indptr, c_indices, c_values,
+                  n_corpus, c_nnz, c_features, k, diag_offset, exclude, splits, workspace, workspace_bytes, idx_out, val_out, false,
+                  nullptr, nullptr, 0, stream);
+}
+
+extern "C" int dae_csr_similarity_topk_excl(const int64_t* q_indptr, const int32_t* q_indices, const float* q_values, int32_t n_query,
+                                            int64_t q_nnz, int32_t q_features, const int64_t* c_indptr, const int32_t* c_indices,
+                                            const float* c_values, int32_t n_corpus, int64_t c_nnz, int32_t c_features, int32_t k,
+                                            int64_t diag_offset, int32_t exclude, int32_t splits, void* workspace,
+                                            int64_t workspace_bytes, int32_t* idx_out, float* val_out, const int64_t* ex_indptr,
+                                            const int32_t* ex_indices, int64_t ex_nnz, void* stream) {
+  return csr_topk("dae_csr_similarity_topk_excl", q_indptr, q_indices, q_values, n_query, q_nnz, q_features, c_indptr, c_indices,
+                  c_values, n_corpus, c_nnz, c_features, k, diag_offset, exclude, splits, workspace, workspace_bytes, idx_out, val_out,
+                  true, ex_indptr, ex_indices, ex_nnz, stream);
 }
 
 extern "C" int dae_csr_similarity_pair_hist_workspace(int32_t n, int64_t nnz, int32_t n_features, int64_t* bytes) {

@@ -3,9 +3,15 @@ nearest-article lookup of main_autoencoder.py:307-318,352-359) -- SURVEY section
 
     pairwise_similarity(in_df, norm='', metric='cosine', set_diagonal_zero=True) -> ndarray [N, N]     (reference signature)
     nearest_neighbors(embeddings, metric='cosine', chunk=8192) -> (index[N], score[N])                (no N x N matrix on the host)
-    top_k_similar(embeddings, k=10, corpus=None, metric='cosine') -> (index[Nq, k], score[Nq, k])    (no similarity matrix at all;
-                                                                                                        dense or scipy sparse inputs)
+    top_k_similar(embeddings, k=10, corpus=None, metric='cosine', exclude=None) -> (index[Nq, k], score[Nq, k])
+                                                                                                      (no similarity matrix at all;
+                                                                                                        dense or scipy sparse inputs;
+                                                                                                        per-query exclusion lists)
     label_precision_at_k(index, query_labels, corpus_labels) -> float                                 (share of same-label neighbours)
+    user_profiles(histories, embeddings) -> [U, H]                                                    (weighted mean of the read articles)
+    recommend(histories, embeddings, k=10, candidates=None, exclude_read=True) -> (index[U, k], score[U, k])
+                                                                                                      (k best unread articles per user)
+    recommendation_recall(index, targets) -> dict                                                     (hit rate / recall of held-out reads)
     similar_pairs(data, threshold, corpus=None, metric='cosine') -> (i[P], j[P], score[P])            (every pair with score >= threshold,
                                                                                                         near-duplicates; no matrix)
     duplicate_groups(i, j, n) -> group[n]                                                             (connected components of the pairs)
@@ -131,18 +137,60 @@ def nearest_neighbors(embeddings, metric='cosine', chunk=8192, device='cuda:0'):
     return idx.cpu().numpy(), val.cpu().numpy()
 
 
-def _similarity_topk(q, c, n_q, n_c, h, k, diag_offset=0, exclude=False, splits=0):
+def _similarity_topk(q, c, n_q, n_c, h, k, diag_offset=0, exclude=False, splits=0, lists=None):
     """k best corpus rows per query row of the bf16 hi / lo operand pairs q and c (dae_similarity_topk_bf16x3): device tensors
-    (index int32 [n_q, k], score float32 [n_q, k]); with `exclude`, column i + diag_offset is not a candidate of row i."""
+    (index int32 [n_q, k], score float32 [n_q, k]); with `exclude`, column i + diag_offset is not a candidate of row i.  lists:
+    per-row exclusion lists (_DeviceLists) through dae_similarity_topk_excl_bf16x3."""
     dev = q[0].device
     need = (ctypes.c_int64 * 1)()
     call('dae_similarity_topk_workspace', n_q, n_c, k, splits, ctypes.addressof(need))
     ws = torch.empty(max(int(need[0]), 16), dtype=torch.uint8, device=dev)
     idx = torch.empty(n_q, k, dtype=torch.int32, device=dev)
     val = torch.empty(n_q, k, dtype=torch.float32, device=dev)
-    call('dae_similarity_topk_bf16x3', n_q, n_c, h, q[0].data_ptr(), q[1].data_ptr(), q[0].stride(0), c[0].data_ptr(), c[1].data_ptr(),
-         c[0].stride(0), k, diag_offset, 1 if exclude else 0, splits, ws.data_ptr(), ws.numel(), idx.data_ptr(), val.data_ptr(), _stream())
+    args = (n_q, n_c, h, q[0].data_ptr(), q[1].data_ptr(), q[0].stride(0), c[0].data_ptr(), c[1].data_ptr(), c[0].stride(0), k, diag_offset,
+            1 if exclude else 0, splits, ws.data_ptr(), ws.numel(), idx.data_ptr(), val.data_ptr())
+    if lists is None:
+        call('dae_similarity_topk_bf16x3', *args, _stream())
+    else:
+        call('dae_similarity_topk_excl_bf16x3', *args, lists.indptr.data_ptr(), lists.indices.data_ptr(), lists.nnz, _stream())
     return idx, val
+
+
+class _DeviceLists:
+    """Per-query exclusion lists on the device: the CSR structure indptr int64 [n + 1], indices int32 [nnz], rows sorted and
+    without duplicates (the layout dae_*_topk_excl* read)."""
+
+    def __init__(self, indptr, indices, nnz):
+        self.indptr, self.indices, self.nnz = indptr, indices, int(nnz)
+
+    @staticmethod
+    def from_host(indptr, indices, device):
+        return _DeviceLists(torch.from_numpy(np.ascontiguousarray(indptr, dtype=np.int64)).to(device),
+                            torch.from_numpy(np.ascontiguousarray(indices, dtype=np.int32)).to(device), len(indices))
+
+
+def _stored_positions(m, shape, what, fn):
+    """The stored positions of the scipy sparse matrix m (values ignored, explicit zeros included) as a canonical CSR structure:
+    (indptr int64 [rows + 1], indices int32, data float64 summed over repeated positions).  ValueError when m is not scipy sparse,
+    has another shape (a None entry of `shape` accepts any size) or holds an index outside it."""
+    if not sp.issparse(m):
+        raise ValueError('%s: %s must be a scipy sparse matrix, not %s' % (fn, what, type(m).__name__))
+    if len(m.shape) != 2 or any(want is not None and got != want for got, want in zip(m.shape, shape)):
+        raise ValueError('%s: %s has shape %s, (%s) expected' % (fn, what, tuple(m.shape),
+                                                                 ', '.join('any' if s is None else str(s) for s in shape)))
+    n_r, n_c = m.shape
+    try:
+        coo = m.tocoo()
+    except (ValueError, IndexError) as e:
+        raise ValueError('%s: %s is malformed or holds an index outside its shape %s (%s)' % (fn, what, (n_r, n_c), e))
+    r, c = np.asarray(coo.row, dtype=np.int64), np.asarray(coo.col, dtype=np.int64)
+    if r.size and (r.min() < 0 or r.max() >= n_r or c.min() < 0 or c.max() >= n_c):
+        raise ValueError('%s: %s holds an index outside its shape %s' % (fn, what, (n_r, n_c)))
+    data = np.asarray(coo.data, dtype=np.float64) if coo.data.dtype != object else np.ones(r.size)
+    out = sp.csr_matrix((data, (r, c)), shape=(n_r, n_c))   # sums repeated positions, keeps explicit zeros
+    out.sum_duplicates()
+    out.sort_indices()
+    return out.indptr.astype(np.int64), out.indices.astype(np.int32), out.data
 
 
 def _as_device_dense(x, device):
@@ -161,9 +209,10 @@ def _csr_operand(x, metric):
     return m
 
 
-def _csr_similarity_topk(q, c, k, diag_offset=0, exclude=False, splits=0):
+def _csr_similarity_topk(q, c, k, diag_offset=0, exclude=False, splits=0, lists=None):
     """k best corpus rows per query row of the DeviceCSR matrices q and c by S = Q.C^T (dae_csr_similarity_topk): device tensors
-    (index int32 [n_q, k], score float32 [n_q, k]); with `exclude`, column i + diag_offset is not a candidate of row i."""
+    (index int32 [n_q, k], score float32 [n_q, k]); with `exclude`, column i + diag_offset is not a candidate of row i.  lists:
+    per-row exclusion lists (_DeviceLists) through dae_csr_similarity_topk_excl."""
     dev = q.indptr.device
     n_q, n_c = q.shape[0], c.shape[0]
     need = (ctypes.c_int64 * 1)()
@@ -171,21 +220,25 @@ def _csr_similarity_topk(q, c, k, diag_offset=0, exclude=False, splits=0):
     ws = torch.empty(max(int(need[0]), 16), dtype=torch.uint8, device=dev)
     idx = torch.empty(n_q, k, dtype=torch.int32, device=dev)
     val = torch.empty(n_q, k, dtype=torch.float32, device=dev)
-    call('dae_csr_similarity_topk', q.indptr.data_ptr(), q.indices.data_ptr(), q.values.data_ptr(), n_q, q.nnz, q.shape[1],
-         c.indptr.data_ptr(), c.indices.data_ptr(), c.values.data_ptr(), n_c, c.nnz, c.shape[1], k, diag_offset, 1 if exclude else 0,
-         splits, ws.data_ptr(), ws.numel(), idx.data_ptr(), val.data_ptr(), _stream())
+    args = (q.indptr.data_ptr(), q.indices.data_ptr(), q.values.data_ptr(), n_q, q.nnz, q.shape[1], c.indptr.data_ptr(),
+            c.indices.data_ptr(), c.values.data_ptr(), n_c, c.nnz, c.shape[1], k, diag_offset, 1 if exclude else 0, splits, ws.data_ptr(),
+            ws.numel(), idx.data_ptr(), val.data_ptr())
+    if lists is None:
+        call('dae_csr_similarity_topk', *args, _stream())
+    else:
+        call('dae_csr_similarity_topk_excl', *args, lists.indptr.data_ptr(), lists.indices.data_ptr(), lists.nnz, _stream())
     return idx, val
 
 
-def _top_k_similar_sparse(embeddings, k, corpus, metric, device, splits):
+def _top_k_similar_sparse(embeddings, k, corpus, metric, device, splits, lists=None):
     if corpus is not None and corpus.shape[1] != embeddings.shape[1]:
         raise ValueError('top_k_similar: corpus rows have %d columns, queries %d' % (corpus.shape[1], embeddings.shape[1]))
     q = DeviceCSR(_csr_operand(embeddings, metric), device)
     c = q if corpus is None else DeviceCSR(_csr_operand(corpus, metric), device)
-    return _csr_similarity_topk(q, c, k, exclude=corpus is None, splits=splits)
+    return _csr_similarity_topk(q, c, k, exclude=corpus is None, splits=splits, lists=lists)
 
 
-def top_k_similar(embeddings, k=10, corpus=None, metric='cosine', device='cuda:0', to_host=True, splits=0):
+def top_k_similar(embeddings, k=10, corpus=None, metric='cosine', device='cuda:0', to_host=True, splits=0, exclude=None):
     """For every row of `embeddings` the k most similar rows of `corpus` and their scores, best first (among equal scores the
     lower index first), without forming the similarity matrix.  corpus=None ranks the set against itself and leaves each row's
     self match out.  Rows with fewer than k candidates are padded with index -1 and score -inf.  metric: 'cosine' or
@@ -193,6 +246,9 @@ def top_k_similar(embeddings, k=10, corpus=None, metric='cosine', device='cuda:0
     Dense inputs (arrays or torch tensors) run on the tensor cores (bf16x3).  Sparse inputs (scipy sparse matrices: the binary /
     tf-idf bag of words) run through dae_csr_similarity_topk, which only spends work on the columns two rows share; every score
     is the fp32 sum of the rounded products in increasing column order.  Queries and corpus must be both dense or both sparse.
+    exclude: a scipy sparse matrix [Nq, Nc] whose stored positions (i, j) are never returned for query i (values ignored,
+    explicit zeros count), e.g. the articles a user has read; the kernels skip them in their epilogues (dae_*_topk_excl*), and
+    the self match stays out with corpus=None.  A wrong shape or an index outside it raises ValueError before any device work.
     Returns (index int32 [Nq, k], score float32 [Nq, k]) as ndarrays, or device tensors with to_host=False.  `splits`
     (> 0) fixes the number of corpus parts the work is cut into; it does not change the result."""
     assert metric in ['cosine', 'linear kernel']
@@ -200,8 +256,14 @@ def top_k_similar(embeddings, k=10, corpus=None, metric='cosine', device='cuda:0
         raise _cabi.DaeError('top_k_similar: k = %d is outside the supported range 1 <= k <= 32' % k)
     if corpus is not None and sp.issparse(embeddings) != sp.issparse(corpus):
         raise ValueError('top_k_similar: queries and corpus must be both sparse or both dense')
+    lists = None
+    if exclude is not None:
+        n_q = embeddings.shape[0]
+        n_c = n_q if corpus is None else corpus.shape[0]
+        indptr, indices, _ = _stored_positions(exclude, (n_q, n_c), 'exclude', 'top_k_similar')
+        lists = _DeviceLists.from_host(indptr, indices, device)
     if sp.issparse(embeddings):
-        idx, val = _top_k_similar_sparse(embeddings, k, corpus, metric, device, splits)
+        idx, val = _top_k_similar_sparse(embeddings, k, corpus, metric, device, splits, lists)
         if to_host:
             return idx.cpu().numpy(), val.cpu().numpy()
         return idx, val
@@ -217,10 +279,158 @@ def top_k_similar(embeddings, k=10, corpus=None, metric='cosine', device='cuda:0
             raise ValueError('top_k_similar: corpus rows have %d columns, queries %d' % (xc.shape[1], h))
         n_c = xc.shape[0]
         c = _normalised_operands(xc, norm_kind)[:2]
-    idx, val = _similarity_topk(q, c, n_q, n_c, h, k, exclude=corpus is None, splits=splits)
+    idx, val = _similarity_topk(q, c, n_q, n_c, h, k, exclude=corpus is None, splits=splits, lists=lists)
     if to_host:
         return idx.cpu().numpy(), val.cpu().numpy()
     return idx, val
+
+
+def _history_weights(histories, n_articles, fn):
+    """Host side of user_profiles / recommend: the canonical history CSR (U x N, float32) with every row's weights divided by their
+    sum (the weighted mean), rows whose weights sum to 0 left at 0, and the boolean mask of those rows (no reads or zero weight)."""
+    indptr, indices, w = _stored_positions(histories, (None, n_articles), 'histories', fn)
+    if not np.isfinite(w).all():
+        raise ValueError('%s: histories hold a weight that is not finite' % fn)
+    n_u = len(indptr) - 1
+    rows = np.repeat(np.arange(n_u), np.diff(indptr))
+    tot = np.bincount(rows, weights=w, minlength=n_u)
+    empty = tot == 0
+    w = np.where(empty[rows], 0.0, w / np.where(empty, 1.0, tot)[rows]).astype(np.float32)
+    m = sp.csr_matrix((w, indices, indptr), shape=(n_u, n_articles))
+    m.has_sorted_indices = True
+    return m, empty
+
+
+def _dense_embeddings(embeddings, device, fn):
+    if sp.issparse(embeddings):
+        raise ValueError('%s: embeddings must be dense (an array or a tensor [N, H]); sparse bag-of-words profiles are not supported' % fn)
+    x = _as_device_dense(embeddings, device)
+    if x.dim() != 2 or x.shape[0] == 0 or x.shape[1] == 0:
+        raise ValueError('%s: embeddings have shape %s, [N, H] with N, H > 0 expected' % (fn, tuple(x.shape)))
+    return x
+
+
+def _profiles(hist, emb):
+    """Profiles [U, H] fp32 on the device: hist (DeviceCSR of the normalised weights, U x N) times emb [N, H] through the CSR encode
+    kernel with activation none and a zero bias, i.e. exactly X.W."""
+    n_u, h = hist.shape[0], emb.shape[1]
+    out = torch.empty(n_u, h, dtype=torch.float32, device=emb.device)
+    zero_b = torch.zeros(h, dtype=torch.float32, device=emb.device)
+    call('dae_encode_csr_fwd', hist.indptr.data_ptr(), hist.indices.data_ptr(), hist.values.data_ptr(), None, n_u, emb.shape[0], h, 1.0,
+         emb.data_ptr(), zero_b.data_ptr(), _cabi.ACT['none'], out.data_ptr(), h, None, None, None, 0, _stream())
+    return out
+
+
+def user_profiles(histories, embeddings, device='cuda:0', to_host=True):
+    """User profiles from reading histories: row u is the weighted mean of the embeddings of the articles user u read.
+    histories: scipy sparse [U, N]; the stored values are the weights (1 for a plain mean, or e.g. decaying with the age of the
+    read), repeated positions add up.  embeddings: [N, H] array or tensor (transform()'s output).  The weights are normalised per
+    user on the host; a user whose weights sum to 0 (no reads, or zero weights) gets a zero row.  The product runs through the CSR
+    encode kernel (dae_encode_csr_fwd, activation none, zero bias).  Returns fp32 [U, H] (ndarray, or a device tensor with
+    to_host=False)."""
+    if sp.issparse(embeddings):
+        _dense_embeddings(embeddings, device, 'user_profiles')
+    w, _ = _history_weights(histories, embeddings.shape[0], 'user_profiles')
+    emb = _dense_embeddings(embeddings, device, 'user_profiles')
+    out = _profiles(DeviceCSR(w, device), emb)
+    return out.cpu().numpy() if to_host else out
+
+
+def _candidate_rows(candidates, n, fn):
+    c = np.asarray(candidates.cpu() if isinstance(candidates, torch.Tensor) else candidates)
+    if c.ndim != 1 or c.size == 0 or not np.issubdtype(c.dtype, np.integer):
+        raise ValueError('%s: candidates must be a non-empty 1-D integer array' % fn)
+    c = c.astype(np.int64)
+    if c.min() < 0 or c.max() >= n:
+        raise ValueError('%s: candidates hold a row outside [0, %d)' % (fn, n))
+    if c.size > 1 and not (np.diff(c) > 0).all():
+        raise ValueError('%s: candidates must be sorted and without duplicates' % fn)
+    return c
+
+
+def _remap_lists(indptr, indices, cand):
+    """Exclusion lists over article rows -> lists over candidate positions: entries that are not candidates drop out, the others
+    become their position in the sorted `cand` (so each row stays sorted)."""
+    pos = np.searchsorted(cand, indices)
+    keep = pos < cand.size
+    keep[keep] = cand[pos[keep]] == indices[keep]
+    rows = np.repeat(np.arange(len(indptr) - 1), np.diff(indptr))
+    new_ptr = np.zeros(len(indptr), dtype=np.int64)
+    np.cumsum(np.bincount(rows[keep], minlength=len(indptr) - 1), out=new_ptr[1:])
+    return new_ptr, pos[keep].astype(np.int32)
+
+
+def recommend(histories, embeddings, k=10, candidates=None, metric='cosine', exclude_read=True, device='cuda:0', to_host=True,
+              splits=0):
+    """For every user the k best articles by `metric` between the user's profile (user_profiles: the weighted mean of the read
+    articles' embeddings) and the articles: 'cosine', or 'linear kernel' (the plain inner product).  Order, ties and padding as in
+    top_k_similar.  exclude_read: no article of the user's history is returned -- the history goes to the top-k kernel as the
+    user's exclusion list, so a long history costs nothing extra on the host.  candidates: an optional sorted int array of rows of
+    `embeddings` that may be recommended (e.g. today's articles); the indices returned are rows of `embeddings` either way.
+    A user without reads, or whose weights sum to 0, gets a padding row (-1 / -inf).  Embeddings only: dense [N, H].
+    Returns (index int32 [U, k], score float32 [U, k]) as ndarrays (device tensors with to_host=False)."""
+    if metric not in ('cosine', 'linear kernel'):
+        raise ValueError("recommend: metric = %r: 'cosine' or 'linear kernel'" % (metric,))
+    if not 1 <= k <= 32:
+        raise _cabi.DaeError('recommend: k = %d is outside the supported range 1 <= k <= 32' % k)
+    n_art = embeddings.shape[0]
+    if sp.issparse(embeddings):
+        _dense_embeddings(embeddings, device, 'recommend')
+    w, empty = _history_weights(histories, n_art, 'recommend')
+    cand = None if candidates is None else _candidate_rows(candidates, n_art, 'recommend')
+    lists_host = None
+    if exclude_read and cand is not None:
+        lists_host = _remap_lists(w.indptr, w.indices, cand)
+    emb = _dense_embeddings(embeddings, device, 'recommend')
+    hist = DeviceCSR(w, device)
+    prof = _profiles(hist, emb)
+    lists = None
+    if exclude_read:
+        lists = _DeviceLists(hist.indptr, hist.indices, hist.nnz) if cand is None else _DeviceLists.from_host(*lists_host, device)
+    cand_dev = None if cand is None else torch.from_numpy(cand).to(device)
+    corpus = emb if cand is None else emb.index_select(0, cand_dev)
+    idx, val = _recommend_topk(prof, corpus, k, metric, lists, splits)
+    if empty.any():
+        e = torch.from_numpy(empty).to(device)
+        idx[e] = -1
+        val[e] = float('-inf')
+    if cand_dev is not None:
+        idx = torch.where(idx >= 0, cand_dev[idx.clamp(min=0).long()].int(), idx)
+    if to_host:
+        return idx.cpu().numpy(), val.cpu().numpy()
+    return idx, val
+
+
+def _recommend_topk(prof, corpus, k, metric, lists, splits=0):
+    """The ranking half of recommend: profiles [U, H] against corpus [Nc, H] on the tensor cores, with the exclusion lists."""
+    norm_kind = 2 if metric == 'cosine' else 0
+    q = _normalised_operands(prof, norm_kind)[:2]
+    c = _normalised_operands(corpus, norm_kind)[:2]
+    return _similarity_topk(q, c, prof.shape[0], corpus.shape[0], prof.shape[1], k, splits=splits, lists=lists)
+
+
+def recommendation_recall(index, targets):
+    """How many held-out reads (e.g. each user's last click) the recommendations find, on the host.  index [U, k] (recommend's
+    output, -1 = padding, never a hit); targets: scipy sparse [U, N] whose stored positions are the held-out articles.  Users
+    without a target are skipped.  Returns {'users': users counted, 'hit_rate': share of them with at least one target among
+    their k, 'recall': mean over them of (targets found) / (their targets)}; NaN when no user counts."""
+    index = np.asarray(index.cpu() if isinstance(index, torch.Tensor) else index)
+    if index.ndim != 2:
+        raise ValueError('recommendation_recall: index has shape %s, [U, k] expected' % (index.shape,))
+    indptr, indices, _ = _stored_positions(targets, (index.shape[0], None), 'targets', 'recommendation_recall')
+    n_u, n = index.shape[0], targets.shape[1]
+    if index.size and index.max() >= n:
+        raise ValueError('recommendation_recall: index holds article %d, targets have %d columns' % (index.max(), n))
+    n_t = np.diff(indptr)
+    use = n_t > 0
+    users = int(use.sum())
+    if users == 0:
+        return {'users': 0, 'hit_rate': float('nan'), 'recall': float('nan')}
+    t_keys = np.repeat(np.arange(n_u, dtype=np.int64), n_t) * n + indices   # sorted: canonical CSR
+    keys = np.arange(n_u, dtype=np.int64)[:, None] * n + index.astype(np.int64)
+    pos = np.minimum(np.searchsorted(t_keys, keys), t_keys.size - 1)
+    hits = ((index >= 0) & (t_keys[pos] == keys)).sum(1)
+    return {'users': users, 'hit_rate': float((hits[use] > 0).mean()), 'recall': float((hits[use] / n_t[use]).mean())}
 
 
 def label_precision_at_k(index, query_labels, corpus_labels):

@@ -57,6 +57,48 @@ def make_sparse(n_rows, n_features, mean_nnz=100, kind='binary', seed=0, zipf_s=
     return m
 
 
+def make_histories(n_users, labels, mean_len=20, seed=0, max_len=2000, holdout=True, second_class=0.5, primary_share=0.7):
+    """Synthetic reading histories over articles labelled `labels` (class ids >= 0; -1 articles are never read).
+    Each user prefers one class, or with probability `second_class` two (a share `primary_share` of the reads from the first);
+    inside a class, article popularity follows a Zipf law (rank r drawn log-uniformly, P ~ 1 / r, over a random order of the
+    class); history lengths are geometric with mean `mean_len`, at least 1 and capped at `max_len`.  A repeated draw counts once.
+    holdout: one more read per user drawn the same way is held out as the target (and removed from the history if already there).
+    Returns (histories, targets): scipy CSR float32 [n_users, N] with weight 1 per read; targets is None without holdout."""
+    rng = np.random.default_rng(seed)
+    labels = np.asarray(labels).reshape(-1)
+    n = labels.shape[0]
+    valid = np.flatnonzero(labels >= 0)
+    classes, inv = np.unique(labels[valid], return_inverse=True)
+    if classes.size == 0:
+        raise ValueError('make_histories: no labelled article')
+    order = valid[np.lexsort((rng.random(valid.size), inv))]   # articles grouped by class, random popularity order inside
+    size = np.bincount(inv, minlength=classes.size)
+    start = np.concatenate([[0], np.cumsum(size)[:-1]])
+    c1 = rng.integers(0, classes.size, n_users)
+    two = rng.random(n_users) < second_class
+    c2 = np.where(two, rng.integers(0, classes.size, n_users), c1)
+    lens = np.minimum(rng.geometric(1.0 / max(mean_len, 1.0), n_users), max_len)
+    draws = lens + (1 if holdout else 0)
+    user = np.repeat(np.arange(n_users), draws)
+    cls = np.where(rng.random(user.size) < primary_share, c1[user], c2[user])
+    rank = np.minimum(np.floor(np.exp(rng.random(user.size) * np.log(size[cls] + 1.0))).astype(np.int64) - 1, size[cls] - 1)
+    art = order[start[cls] + rank]
+    ends = np.cumsum(draws)
+    is_target = np.zeros(user.size, dtype=bool)
+    if holdout:
+        is_target[ends - 1] = True
+    hist = sp.csr_matrix((np.ones(int((~is_target).sum()), np.float32), (user[~is_target], art[~is_target])), shape=(n_users, n))
+    hist.sum_duplicates()
+    hist.data[:] = 1.0
+    targets = None
+    if holdout:
+        targets = sp.csr_matrix((np.ones(n_users, np.float32), (user[is_target], art[is_target])), shape=(n_users, n))
+        hist = (hist - hist.multiply(targets)).tocsr()   # a held-out read is not in the history
+        hist.eliminate_zeros()
+        hist.sort_indices()
+    return hist.astype(np.float32), targets
+
+
 def make_labels(n_rows, n_classes=4, seed=0):
     return np.random.default_rng(seed + 7919).integers(0, n_classes, n_rows).astype(np.float32)
 

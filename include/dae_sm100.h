@@ -360,6 +360,28 @@ int dae_csr_similarity_topk(const int64_t* q_indptr, const int32_t* q_indices, c
 int dae_csr_similarity_topk_workspace(int32_t n_query, int32_t n_corpus, int64_t corpus_nnz, int32_t n_features, int32_t k,
                                       int32_t splits, int64_t* bytes);
 
+/* ---- k best unread articles: top-k with per-query exclusion lists ---------------------------------------------------
+ * dae_similarity_topk_excl_bf16x3 / dae_csr_similarity_topk_excl: dae_similarity_topk_bf16x3 / dae_csr_similarity_topk with the
+ *   same arguments, workspace (the same size queries) and contract, plus an exclusion list per query row: the device CSR structure
+ *   ex_indptr int64 [n_query + 1], ex_indices int32 [ex_nnz] (no values).  Row i lists the corpus rows that are never candidates of
+ *   query i (e.g. the articles a user has read).  The caller guarantees ex_indptr[0] = 0, ex_indptr[n_query] = ex_nnz, and every
+ *   row sorted, without duplicates, inside [0, n_corpus): the kernels do not check the list contents.  `exclude` / diag_offset
+ *   still leave out column i + diag_offset as well.  Order (score desc, index asc), padding -1 / -inf when fewer than k
+ *   candidates remain, independent of `splits`; with every list empty the output equals the plain call's bit for bit.
+ *   ex_indptr 8-byte and ex_indices 4-byte aligned; ex_indices may be NULL when ex_nnz = 0.
+ */
+int dae_similarity_topk_excl_bf16x3(int32_t n_query, int32_t n_corpus, int32_t dim, const void* q_hi, const void* q_lo,
+                                    int64_t ldq, const void* c_hi, const void* c_lo, int64_t ldc, int32_t k,
+                                    int64_t diag_offset, int32_t exclude, int32_t splits, void* workspace,
+                                    int64_t workspace_bytes, int32_t* idx_out, float* val_out, const int64_t* ex_indptr,
+                                    const int32_t* ex_indices, int64_t ex_nnz, void* stream);
+int dae_csr_similarity_topk_excl(const int64_t* q_indptr, const int32_t* q_indices, const float* q_values, int32_t n_query,
+                                 int64_t q_nnz, int32_t q_features, const int64_t* c_indptr, const int32_t* c_indices,
+                                 const float* c_values, int32_t n_corpus, int64_t c_nnz, int32_t c_features, int32_t k,
+                                 int64_t diag_offset, int32_t exclude, int32_t splits, void* workspace, int64_t workspace_bytes,
+                                 int32_t* idx_out, float* val_out, const int64_t* ex_indptr, const int32_t* ex_indices,
+                                 int64_t ex_nnz, void* stream);
+
 /* ---- "next" row (SURVEY 8f rank 2): related-vs-unrelated AUROC of a pairwise similarity matrix ---------------------
  * Replaces the numeric part of helpers.visualize_pairwise_similarity (helpers.py:88-100).
  * dae_pair_partition: for every pair i > j of the strict lower triangle with labels[i] >= 0 and labels[j] >= 0

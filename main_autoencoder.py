@@ -87,6 +87,13 @@ def build_parser():
                     help='add every floating-point sum of the training step in a fixed order, so that a rerun with the same --seed (>= 0) '
                          'and data gives bit-identical parameters, losses and embeddings on the same GPU model (slower; default: off, '
                          'or the environment variable DAE_DETERMINISTIC=1)')
+    ap.add_argument('--user_histories', default='',
+                    help='with --top_k K: a scipy.sparse.save_npz matrix [users x training articles] of reading histories (values: '
+                         'weights); after transform, recommend the K best unread training articles to every user (helpers.recommend) '
+                         'and save user_top_k_{index,score}.npy')
+    ap.add_argument('--user_targets', default='',
+                    help='with --user_histories: a save_npz matrix of the same shape holding held-out reads; report the hit rate '
+                         'and recall of the recommendations against them (user_hit_rate, user_recall)')
     return ap
 
 
@@ -135,6 +142,10 @@ def check_flags(F):
     assert not F.top_k_input or F.top_k > 0, '--top_k_input needs --top_k K > 0'
     assert F.dedup_threshold >= 0.0
     assert not F.dedup_input or F.dedup_threshold > 0, '--dedup_input needs --dedup_threshold T > 0'
+    assert not F.user_histories or F.top_k > 0, '--user_histories needs --top_k K > 0'
+    assert not F.user_histories or os.path.isfile(F.user_histories), '--user_histories %s: no such file' % F.user_histories
+    assert not F.user_targets or F.user_histories, '--user_targets needs --user_histories'
+    assert not F.user_targets or os.path.isfile(F.user_targets), '--user_targets %s: no such file' % F.user_targets
     if F.input_format == 'tfidf':
         assert F.loss_func in ['mean_squared', 'cosine_proximity']
     if F.main_dir == '':
@@ -359,6 +370,40 @@ def find_duplicates(F, model, X, X_v, trL, vlL, metric, name, emb_out=None):
     return out
 
 
+def load_user_files(F, n_train):
+    """--user_histories / --user_targets: the save_npz matrices, checked against the training set's row count before training."""
+    import scipy.sparse as sp
+    out = []
+    for flag, path in (('--user_histories', F.user_histories), ('--user_targets', F.user_targets)):
+        if not path:
+            out.append(None)
+            continue
+        m = sp.load_npz(path)
+        if m.ndim != 2 or m.shape[1] != n_train:
+            raise ValueError('%s %s: shape %s, [users x %d training articles] expected' % (flag, path, m.shape, n_train))
+        out.append(m)
+    if out[1] is not None and out[1].shape[0] != out[0].shape[0]:
+        raise ValueError('--user_targets has %d users, --user_histories %d' % (out[1].shape[0], out[0].shape[0]))
+    return out
+
+
+def recommend_users(F, model, enc, histories, targets):
+    """--user_histories: the --top_k best unread training articles of every user from the profile of the embeddings of the
+    articles the user read (helpers.recommend), saved under data_dir as user_top_k_{index,score}.npy; with --user_targets the hit
+    rate and recall of the held-out reads are returned and printed."""
+    from dae_rnn_news_recommendation_b200 import helpers
+    print('recommend %d unread articles to %d users' % (F.top_k, histories.shape[0]))
+    idx, score = helpers.recommend(histories, enc, k=F.top_k)
+    np.save(model.data_dir + 'user_top_k_index', idx)
+    np.save(model.data_dir + 'user_top_k_score', score)
+    out = {}
+    if targets is not None:
+        r = helpers.recommendation_recall(idx, targets)
+        out = {'user_hit_rate': r['hit_rate'], 'user_recall': r['recall']}
+        print('users: hit rate@%d %.4f recall@%d %.4f (%d users with targets)' % (F.top_k, r['hit_rate'], F.top_k, r['recall'], r['users']))
+    return out
+
+
 def main(argv=None):
     F = check_flags(apply_env_overrides(build_parser().parse_args(argv)))
     print(__file__ + ': Start')
@@ -377,6 +422,7 @@ def main(argv=None):
         data = restore_uci(model) if F.restore_previous_data else prepare_uci(F, model)
         (trX, vlX), (trL, vlL) = data[F.input_format], data['label_' + F.label]
         trX, vlX, trL, vlL = trX.astype(np.float32), vlX.astype(np.float32), np.asarray(trL), np.asarray(vlL)
+    histories, targets = load_user_files(F, trX.shape[0]) if F.user_histories else (None, None)
     print('fit')
     model.fit(train_set=trX, validation_set=vlX if F.validation else None, train_set_label=trL,
               validation_set_label=vlL if F.validation else None, restore_previous_model=F.restore_previous_model)
@@ -395,6 +441,8 @@ def main(argv=None):
         model.evaluation.update(recommend_top_k(F, model, enc, enc_v, trL, vlL))
         if F.top_k_input:
             model.evaluation.update(recommend_top_k_input(F, model, trX, vlX, trL, vlL, model.evaluation))
+        if histories is not None:
+            model.evaluation.update(recommend_users(F, model, enc, histories, targets))
     if F.dedup_threshold > 0:
         model.evaluation.update(find_duplicates(F, model, enc, enc_v, trL, vlL, 'cosine', 'article_duplicates'))
         if F.dedup_input:
