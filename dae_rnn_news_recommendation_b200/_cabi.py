@@ -84,6 +84,12 @@ _SIGNATURES = {
     'dae_pairs_sort_workspace': (C.c_int, [i64, i32, p]),
     'dae_allreduce_multimem': (C.c_int, [p, p, p, i32, i32, i64, i32, p]),
     'dae_mask_values': (C.c_int, [p, p, i64, f32, u64, u64, p, p]),
+    # GRU user encoder
+    'dae_gather_split_bf16': (C.c_int, [p, i64, p, i32, i32, p, p, i64, i32, p]),
+    'dae_gru_cell_fwd': (C.c_int, [i32, i32, p, i64, p, i64, p, i64, p, i64, i32, p, p, i64, p, i64, p]),
+    'dae_gru_cell_bwd': (C.c_int, [i32, i32, p, i64, p, i64, p, i64, p, i64, p, p, p, p, i64, p]),
+    'dae_seq_negatives': (C.c_int, [p, i64, i32, u64, u64, u64, p, p]),
+    'dae_seq_rank_loss': (C.c_int, [p, i64, p, i64, i32, p, p, i64, f32, p, i64, p, p]),
     # deterministic training step
     'dae_gemm_det_workspace': (C.c_int, [p]),
     'dae_gemm_bf16x3_det': (C.c_int, [i32, i32, i32, f32, p, p, i64, i32, p, p, i64, i32, p, i64, i32, i32, p, i32, i32, p, i64, p]),

@@ -95,6 +95,16 @@ __device__ __forceinline__ T block_sum(T v, T* smem32) {
   return smem32[0];
 }
 
+// Philox4x32-10 (Salmon et al. 2011)
+__device__ __forceinline__ void philox_round(uint32_t (&c)[4], uint32_t (&k)[2]) {
+  const uint32_t M0 = 0xD2511F53u, M1 = 0xCD9E8D57u;
+  const uint32_t hi0 = __umulhi(M0, c[0]), lo0 = M0 * c[0];
+  const uint32_t hi1 = __umulhi(M1, c[2]), lo1 = M1 * c[2];
+  const uint32_t n0 = hi1 ^ c[1] ^ k[0], n1 = lo1, n2 = hi0 ^ c[3] ^ k[1], n3 = lo0;
+  c[0] = n0; c[1] = n1; c[2] = n2; c[3] = n3;
+  k[0] += 0x9E3779B9u; k[1] += 0xBB67AE85u;
+}
+
 #define DAE_DISPATCH_ACT(act, ACT, ...)                      \
   switch (act) {                                             \
     case DAE_ACT_SIGMOID: { constexpr int ACT = DAE_ACT_SIGMOID; __VA_ARGS__; } break; \

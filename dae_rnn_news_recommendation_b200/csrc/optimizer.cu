@@ -78,16 +78,6 @@ __global__ void __launch_bounds__(256) optimizer_kernel(float* __restrict__ thet
   }
 }
 
-// Philox4x32-10 (Salmon et al. 2011)
-__device__ __forceinline__ void philox_round(uint32_t (&c)[4], uint32_t (&k)[2]) {
-  const uint32_t M0 = 0xD2511F53u, M1 = 0xCD9E8D57u;
-  const uint32_t hi0 = __umulhi(M0, c[0]), lo0 = M0 * c[0];
-  const uint32_t hi1 = __umulhi(M1, c[2]), lo1 = M1 * c[2];
-  const uint32_t n0 = hi1 ^ c[1] ^ k[0], n1 = lo1, n2 = hi0 ^ c[3] ^ k[1], n3 = lo0;
-  c[0] = n0; c[1] = n1; c[2] = n2; c[3] = n3;
-  k[0] += 0x9E3779B9u; k[1] += 0xBB67AE85u;
-}
-
 __global__ void __launch_bounds__(256) mask_values_kernel(const float* __restrict__ values, const uint8_t* __restrict__ keep,
                                                           int64_t nnz, float corr_frac, uint64_t seed, uint64_t epoch,
                                                           float* __restrict__ out) {

@@ -9,8 +9,10 @@ nearest-article lookup of main_autoencoder.py:307-318,352-359) -- SURVEY section
                                                                                                         per-query exclusion lists)
     label_precision_at_k(index, query_labels, corpus_labels) -> float                                 (share of same-label neighbours)
     user_profiles(histories, embeddings) -> [U, H]                                                    (weighted mean of the read articles)
-    recommend(histories, embeddings, k=10, candidates=None, exclude_read=True) -> (index[U, k], score[U, k])
-                                                                                                      (k best unread articles per user)
+    recommend(histories, embeddings, k=10, candidates=None, exclude_read=True, profiles=None) -> (index[U, k], score[U, k])
+                                                                                                      (k best unread articles per user;
+                                                                                                        mean or given profiles)
+    sequences_from_csr(m) -> (indptr[U + 1], items)                                                   (reads ordered by stored time)
     recommendation_recall(index, targets) -> dict                                                     (hit rate / recall of held-out reads)
     similar_pairs(data, threshold, corpus=None, metric='cosine') -> (i[P], j[P], score[P])            (every pair with score >= threshold,
                                                                                                         near-duplicates; no matrix)
@@ -360,14 +362,30 @@ def _remap_lists(indptr, indices, cand):
     return new_ptr, pos[keep].astype(np.int32)
 
 
+def sequences_from_csr(m):
+    """Reading sequences from a scipy sparse [U, N] matrix whose stored values are read times or positions: user u's articles are
+    the stored columns of row u ordered by value (ties by column).  Explicit zeros count as reads (time 0).  Returns
+    (indptr int64 [U + 1], items int32 [nnz]), the input of user_model.UserGRU."""
+    if not sp.issparse(m):
+        raise ValueError('sequences_from_csr: a scipy sparse matrix is expected, not %s' % type(m).__name__)
+    coo = m.tocoo()
+    r, c, v = np.asarray(coo.row, np.int64), np.asarray(coo.col, np.int64), np.asarray(coo.data, np.float64)
+    order = np.lexsort((c, v, r))
+    indptr = np.zeros(m.shape[0] + 1, dtype=np.int64)
+    np.cumsum(np.bincount(r, minlength=m.shape[0]), out=indptr[1:])
+    return indptr, c[order].astype(np.int32)
+
+
 def recommend(histories, embeddings, k=10, candidates=None, metric='cosine', exclude_read=True, device='cuda:0', to_host=True,
-              splits=0):
+              splits=0, profiles=None):
     """For every user the k best articles by `metric` between the user's profile (user_profiles: the weighted mean of the read
     articles' embeddings) and the articles: 'cosine', or 'linear kernel' (the plain inner product).  Order, ties and padding as in
     top_k_similar.  exclude_read: no article of the user's history is returned -- the history goes to the top-k kernel as the
     user's exclusion list, so a long history costs nothing extra on the host.  candidates: an optional sorted int array of rows of
     `embeddings` that may be recommended (e.g. today's articles); the indices returned are rows of `embeddings` either way.
     A user without reads, or whose weights sum to 0, gets a padding row (-1 / -inf).  Embeddings only: dense [N, H].
+    profiles: an optional [U, H] array or tensor ranked in place of the mean profiles (e.g. UserGRU.transform's user vectors); the
+    histories still give the exclusion lists and the padding rows.
     Returns (index int32 [U, k], score float32 [U, k]) as ndarrays (device tensors with to_host=False)."""
     if metric not in ('cosine', 'linear kernel'):
         raise ValueError("recommend: metric = %r: 'cosine' or 'linear kernel'" % (metric,))
@@ -381,9 +399,13 @@ def recommend(histories, embeddings, k=10, candidates=None, metric='cosine', exc
     lists_host = None
     if exclude_read and cand is not None:
         lists_host = _remap_lists(w.indptr, w.indices, cand)
+    if profiles is not None:
+        if sp.issparse(profiles) or tuple(profiles.shape) != (w.shape[0], embeddings.shape[1]):
+            raise ValueError('recommend: profiles have shape %s, [%d, %d] (users x embedding width) expected'
+                             % (tuple(profiles.shape), w.shape[0], embeddings.shape[1]))
     emb = _dense_embeddings(embeddings, device, 'recommend')
     hist = DeviceCSR(w, device)
-    prof = _profiles(hist, emb)
+    prof = _profiles(hist, emb) if profiles is None else _as_device_dense(profiles, emb.device)
     lists = None
     if exclude_read:
         lists = _DeviceLists(hist.indptr, hist.indices, hist.nnz) if cand is None else _DeviceLists.from_host(*lists_host, device)

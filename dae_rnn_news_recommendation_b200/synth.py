@@ -99,6 +99,57 @@ def make_histories(n_users, labels, mean_len=20, seed=0, max_len=2000, holdout=T
     return hist.astype(np.float32), targets
 
 
+def make_sequences(n_users, labels, mean_len=20, session_len=5, seed=0, max_len=2000, holdout=True, tries=20):
+    """Synthetic ordered reading sequences over articles labelled `labels` (class ids >= 0; -1 articles are never read).
+    Each user prefers 2 or 3 classes.  Reads come in sessions (geometric lengths, mean `session_len`); each session picks one of the
+    user's classes uniformly and reads Zipf-popular articles of it (as make_histories).  Sequence lengths are geometric with mean
+    `mean_len`, at least 1 and capped at `max_len`.  So the next read follows the current session's class, which the order of the
+    reads shows and their mean does not.
+    holdout: the target is the user's next read, drawn in the last session, redrawn up to `tries` times while it is an article the
+    user already read (-1 when every draw was).
+    Returns (indptr int64 [U + 1], items int32, targets int64 [U] or None)."""
+    rng = np.random.default_rng(seed)
+    labels = np.asarray(labels).reshape(-1)
+    valid = np.flatnonzero(labels >= 0)
+    classes, inv = np.unique(labels[valid], return_inverse=True)
+    if classes.size == 0:
+        raise ValueError('make_sequences: no labelled article')
+    nc = classes.size
+    order = valid[np.lexsort((rng.random(valid.size), inv))]
+    size = np.bincount(inv, minlength=nc)
+    start = np.concatenate([[0], np.cumsum(size)[:-1]])
+    prefs = np.argsort(rng.random((n_users, nc)), axis=1)[:, :3]
+    n_pref = np.minimum(rng.integers(2, 4, n_users), nc)
+    lens = np.minimum(rng.geometric(1.0 / max(mean_len, 1.0), n_users), max_len)
+    user = np.repeat(np.arange(n_users), lens)
+    first = np.zeros(user.size, dtype=bool)
+    first[np.cumsum(lens) - lens] = True
+    new = first | (rng.random(user.size) < 1.0 / max(session_len, 1.0))
+    sess = np.cumsum(new) - 1
+    sess_cls = prefs[user[new], (rng.random(int(new.sum())) * n_pref[user[new]]).astype(np.int64)]
+
+    def draw(cls):
+        rank = np.minimum(np.floor(np.exp(rng.random(cls.size) * np.log(size[cls] + 1.0))).astype(np.int64) - 1, size[cls] - 1)
+        return order[start[cls] + rank]
+
+    items = draw(sess_cls[sess]).astype(np.int32)
+    indptr = np.concatenate([[0], np.cumsum(lens)]).astype(np.int64)
+    targets = None
+    if holdout:
+        last_cls = sess_cls[sess[indptr[1:] - 1]]
+        targets = np.full(n_users, -1, np.int64)
+        read = sp.csr_matrix((np.ones(items.size), (user, items)), shape=(n_users, labels.shape[0]))
+        todo = np.arange(n_users)
+        for _ in range(tries):
+            t = draw(last_cls[todo])
+            ok = np.asarray(read[todo, t]).ravel() == 0
+            targets[todo[ok]] = t[ok]
+            todo = todo[~ok]
+            if todo.size == 0:
+                break
+    return indptr, items, targets
+
+
 def make_labels(n_rows, n_classes=4, seed=0):
     return np.random.default_rng(seed + 7919).integers(0, n_classes, n_rows).astype(np.float32)
 

@@ -522,6 +522,37 @@ int dae_triplet_explicit_det(const float* E, const float* Ep, const float* En, i
                              float alpha, float* dE, float* dEp, float* dEn, double* stats, double* loss_slots, void* stream);
 int dae_triplet_loss_sum(const double* loss_slots, int32_t n, double* stats, void* stream);
 
+/* ---- GRU user encoder over reading sequences (DESIGN 4.10) -----------------------------------------------------------------
+ * A batch of users is ordered by length, descending (PackedSequence layout): at step t the users still reading are rows [0, n_t)
+ * and their positions are rows off_t + i of every packed [positions x ...] buffer.  Gates follow torch.nn.GRU (order r, z, n):
+ * r = s(xr + hr), z = s(xz + hz), n = tanh(xn + r hn), h = (1 - z) n + z h_prev, with XP = [X | 1].[W_ih | b_ih]^T and
+ * HP = [h_prev | 1].[W_hh | b_hh]^T computed by dae_gemm_bf16x3.
+ * dae_gather_split_bf16: hi / lo [n_rows x ld_dst] <- rows rows[r] of src (columns [0, cols)), column ones_col (if >= 0) = 1,
+ *   the other columns 0: the packed [X | 1] operand of a batch.
+ * dae_gru_cell_fwd: one step for rows [0, n) from XP (ld_xp >= 3H) and HP (ld_hp >= 3H).  h_prev NULL: h_prev = 0; h_out may equal
+ *   h_prev.  Rows i < n_split of h also go to h_hi / h_lo [.. x ld_split] (the next step's GEMM operand) when h_hi is non-NULL;
+ *   gates (optional, ld_gates >= 4H) <- [r | z | n | hn], what dae_gru_cell_bwd needs.
+ * dae_gru_cell_bwd: one step backward for rows [0, n): dh = carry + dh_in (dh_in optional).  Writes dXP = [dr^, dz^, dn^] and
+ *   dHP = [dr^, dz^, r dn^] as bf16 hi / lo rows (ld_g >= 3H) and carry <- dh z, onto which the caller accumulates dHP . W_hh.
+ * dae_seq_negatives: neg[p] = (pos[p] + 1 + floor(u (n_items - 1))) mod n_items, u = c / 2^32 where c is the first word of
+ *   Philox4x32-10 with key seed and counter (p, batch, epoch lo, epoch hi): uniform over the other articles, never pos[p].
+ *   pos[p] < 0: neg[p] = -1.
+ * dae_seq_rank_loss: one warp per position p with pos[p] >= 0: x = h_p . e(neg[p]) - h_p . e(pos[p]); *loss_sum += softplus(x)
+ *   (fp64 atomics); dh_p = scale s(x) (e(neg) - e(pos)).  Positions with pos[p] < 0 get dh_p = 0.
+ */
+int dae_gather_split_bf16(const float* src, int64_t ld_src, const int32_t* rows, int32_t n_rows, int32_t cols, void* hi, void* lo,
+                          int64_t ld_dst, int32_t ones_col, void* stream);
+int dae_gru_cell_fwd(int32_t n, int32_t H, const float* xp, int64_t ld_xp, const float* hp, int64_t ld_hp, const float* h_prev,
+                     int64_t ld_hprev, float* h_out, int64_t ld_h, int32_t n_split, void* h_hi, void* h_lo, int64_t ld_split,
+                     float* gates, int64_t ld_gates, void* stream);
+int dae_gru_cell_bwd(int32_t n, int32_t H, const float* dh_in, int64_t ld_dh_in, float* carry, int64_t ld_carry, const float* gates,
+                     int64_t ld_gates, const float* h_prev, int64_t ld_hprev, void* dxp_hi, void* dxp_lo, void* dhp_hi, void* dhp_lo,
+                     int64_t ld_g, void* stream);
+int dae_seq_negatives(const int32_t* pos, int64_t n_pos, int32_t n_items, uint64_t seed, uint64_t epoch, uint64_t batch, int32_t* neg,
+                      void* stream);
+int dae_seq_rank_loss(const float* h, int64_t ld_h, const float* emb, int64_t ld_emb, int32_t H, const int32_t* pos, const int32_t* neg,
+                      int64_t n_pos, float scale, float* dh, int64_t ld_dh, double* loss_sum, void* stream);
+
 /* ---- data-parallel exchange step (SURVEY 8e): in-switch all-reduce of the flat gradient buffer -------------------
  * The reference is single-process; row-sharded training adds ONE sum over ranks of [dW | dbh | dbv] between the
  * gradient kernels and dae_optimizer_step.  Default transport: ncclAllReduce.  dae_allreduce_multimem is the

@@ -91,6 +91,12 @@ def build_parser():
                     help='with --top_k K: a scipy.sparse.save_npz matrix [users x training articles] of reading histories (values: '
                          'weights); after transform, recommend the K best unread training articles to every user (helpers.recommend) '
                          'and save user_top_k_{index,score}.npy')
+    ap.add_argument('--user_sequences', default='',
+                    help='with --top_k K: an .npz with indptr [users + 1] and items (training article rows in reading order), '
+                         'optionally targets [users] (the next read, -1 = none); train a GRU user encoder (user_model.UserGRU) on '
+                         'the training embeddings, save user_gru.npz and user_gru_top_k_{index,score}.npy; with targets report '
+                         'user_gru_hit_rate / user_gru_recall next to the mean profile\'s for the same reads')
+    ap.add_argument('--user_epochs', type=int, default=5, help='with --user_sequences: training epochs of the GRU user encoder')
     ap.add_argument('--user_targets', default='',
                     help='with --user_histories: a save_npz matrix of the same shape holding held-out reads; report the hit rate '
                          'and recall of the recommendations against them (user_hit_rate, user_recall)')
@@ -144,6 +150,9 @@ def check_flags(F):
     assert not F.dedup_input or F.dedup_threshold > 0, '--dedup_input needs --dedup_threshold T > 0'
     assert not F.user_histories or F.top_k > 0, '--user_histories needs --top_k K > 0'
     assert not F.user_histories or os.path.isfile(F.user_histories), '--user_histories %s: no such file' % F.user_histories
+    assert not F.user_sequences or F.top_k > 0, '--user_sequences needs --top_k K > 0'
+    assert not F.user_sequences or os.path.isfile(F.user_sequences), '--user_sequences %s: no such file' % F.user_sequences
+    assert F.user_epochs >= 0, '--user_epochs must be >= 0'
     assert not F.user_targets or F.user_histories, '--user_targets needs --user_histories'
     assert not F.user_targets or os.path.isfile(F.user_targets), '--user_targets %s: no such file' % F.user_targets
     if F.input_format == 'tfidf':
@@ -404,6 +413,49 @@ def recommend_users(F, model, enc, histories, targets):
     return out
 
 
+def load_user_sequences(F, n_train):
+    """--user_sequences: (indptr, items, targets or None), checked against the training set's row count before training."""
+    from dae_rnn_news_recommendation_b200.user_model import check_sequences
+    z = np.load(F.user_sequences)
+    indptr, items = check_sequences((z['indptr'], z['items']), n_train, '--user_sequences %s' % F.user_sequences)
+    targets = None
+    if 'targets' in z.files:
+        targets = np.asarray(z['targets']).astype(np.int64)
+        if targets.shape != (len(indptr) - 1,) or targets.max(initial=-1) >= n_train or targets.min(initial=-1) < -1:
+            raise ValueError('--user_sequences %s: targets must be [users] rows of the training set or -1' % F.user_sequences)
+    return indptr, items, targets
+
+
+def recommend_users_gru(F, model, enc, seqs):
+    """--user_sequences: train a GRU user encoder on the training embeddings, save it as user_gru.npz and the --top_k best unread
+    articles per user as user_gru_top_k_{index,score}.npy; with targets, the hit rate and recall of the GRU's and of the mean
+    profile's recommendations for the same reads are returned and printed."""
+    import scipy.sparse as sp
+    from dae_rnn_news_recommendation_b200 import helpers
+    from dae_rnn_news_recommendation_b200.user_model import UserGRU, history_matrix
+    indptr, items, targets = seqs
+    print('train a GRU user encoder on %d users (%d reads, %d epochs)' % (len(indptr) - 1, items.size, F.user_epochs))
+    gru = UserGRU(enc.shape[1], num_epochs=F.user_epochs, seed=max(F.seed, 0))
+    gru.fit((indptr, items), enc)
+    gru.save(model.data_dir + 'user_gru.npz')
+    idx, score = gru.recommend((indptr, items), enc, k=F.top_k)
+    np.save(model.data_dir + 'user_gru_top_k_index', idx)
+    np.save(model.data_dir + 'user_gru_top_k_score', score)
+    out = {'user_gru_train_loss': gru.train_loss[-1] if gru.train_loss else float('nan')}
+    if targets is not None:
+        n_u, n = len(indptr) - 1, enc.shape[0]
+        has = targets >= 0
+        tg = sp.csr_matrix((np.ones(int(has.sum()), np.float32), (np.flatnonzero(has), targets[has])), shape=(n_u, n))
+        hist = history_matrix(indptr, items, n)
+        r = helpers.recommendation_recall(idx, tg)
+        m = helpers.recommendation_recall(helpers.recommend(hist, enc, k=F.top_k)[0], tg)
+        out.update({'user_gru_hit_rate': r['hit_rate'], 'user_gru_recall': r['recall'], 'user_mean_hit_rate': m['hit_rate'],
+                    'user_mean_recall': m['recall']})
+        print('users (GRU): hit rate@%d %.4f recall@%d %.4f; mean profile: hit rate@%d %.4f recall@%d %.4f (%d users with targets)'
+              % (F.top_k, r['hit_rate'], F.top_k, r['recall'], F.top_k, m['hit_rate'], F.top_k, m['recall'], r['users']))
+    return out
+
+
 def main(argv=None):
     F = check_flags(apply_env_overrides(build_parser().parse_args(argv)))
     print(__file__ + ': Start')
@@ -423,6 +475,7 @@ def main(argv=None):
         (trX, vlX), (trL, vlL) = data[F.input_format], data['label_' + F.label]
         trX, vlX, trL, vlL = trX.astype(np.float32), vlX.astype(np.float32), np.asarray(trL), np.asarray(vlL)
     histories, targets = load_user_files(F, trX.shape[0]) if F.user_histories else (None, None)
+    seqs = load_user_sequences(F, trX.shape[0]) if F.user_sequences else None
     print('fit')
     model.fit(train_set=trX, validation_set=vlX if F.validation else None, train_set_label=trL,
               validation_set_label=vlL if F.validation else None, restore_previous_model=F.restore_previous_model)
@@ -443,6 +496,8 @@ def main(argv=None):
             model.evaluation.update(recommend_top_k_input(F, model, trX, vlX, trL, vlL, model.evaluation))
         if histories is not None:
             model.evaluation.update(recommend_users(F, model, enc, histories, targets))
+        if seqs is not None:
+            model.evaluation.update(recommend_users_gru(F, model, enc, seqs))
     if F.dedup_threshold > 0:
         model.evaluation.update(find_duplicates(F, model, enc, enc_v, trL, vlL, 'cosine', 'article_duplicates'))
         if F.dedup_input:
