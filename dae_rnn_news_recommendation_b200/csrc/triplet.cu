@@ -58,9 +58,16 @@ __device__ __forceinline__ void triplet_pair_tile(f2 U, const f2 (&V)[kTK], f2& 
 // One 4 x 4 register tile of triplets: sg[a][b] = sigmoid(x_ab) = e/(1+e) with e = exp(x_ab) = u_a v_b (computed as e * 1/(1+e),
 // which keeps full relative accuracy when sigmoid is tiny), lg += sum of log2(1 + e).
 //   TIER 0 (row range < 10): t = 1 + e <= 2.2e4, so products of four t's stay finite: ONE lg2 and ONE rcp per four
-//                            triplets (log of the product; Montgomery batch inversion) -> 0.5 MUFU per triplet.
+//                            triplets (log of the product; Montgomery batch inversion) -> 0.5 MUFU per triplet.  x >= -10 here,
+//                            so e >= 4.5e-5 and fp32's t = 1 + e keeps the term.
 //   TIER 1 (row range < 80): one lg2 + one rcp per triplet on the factorised exponentials.
 //   TIER 2                 : direct, overflow-safe evaluation (3 MUFU per triplet).
+// In tiers 1 and 2, log2(1 + e) for e < 2^-12 is the series (e - e^2 / 2) / ln 2, within e^2 / 3 <= 2^-25 of the term: fp32's
+// 1 + e is 1 for e < 2^-24 (x < -16.6), so lg2(t) would drop a well-separated triplet's loss term, and lg2.approx's 2^-22 absolute
+// error is already 2^-10.5 of log2(1 + e) at e = 2^-12.  Only the loss changes: sigma = e * rcp(t) keeps full relative accuracy.
+constexpr float kSeriesMax = 0x1p-12f;
+__device__ __forceinline__ float ln_1p_small(float e) { return fmaf(-0.5f * e, e, e); }   // e - e^2 / 2
+
 template <int TIER>
 __device__ __forceinline__ void triplet_tile(const float (&s_j)[kTJ], const float (&u_j)[kTJ], const float (&s_k)[kTK],
                                              const float (&v_k)[kTK], float (&sg)[kTJ][kTK], float& lg) {
@@ -79,13 +86,13 @@ __device__ __forceinline__ void triplet_tile(const float (&s_j)[kTJ], const floa
       for (int b = 0; b < kTK; ++b) {
         const float e = u_j[a] * v_k[b];
         const float t = e + 1.0f;
-        lg += fast_lg2(t);
+        if (e < kSeriesMax) lg = fmaf(ln_1p_small(e), kLog2e, lg); else lg += fast_lg2(t);
         sg[a][b] = e * fast_rcp(t);
       }
     } else if (TIER == 3) {   // pos_triplets_only (triplet_loss_utils.py:118-120): softplus and COUNTS over positive triplets only
 #pragma unroll
       for (int b = 0; b < kTK; ++b) {
-        const bool pos = (s_j[a] < 1.0e38f) && (s_k[b] > s_j[a]);   // s_j carries the +1e-16 of the positive test
+        const bool pos = (s_j[a] < 1.0e38f) && (s_k[b] > s_j[a]);   // s_j is the positive test's threshold (pos_threshold)
         const float x = s_k[b] - s_j[a];
         const float em = fast_ex2(-fabsf(x) * kLog2e);
         lg += pos ? (fmaxf(x, 0.0f) * kLog2e + fast_lg2(1.0f + em)) : 0.0f;
@@ -99,15 +106,32 @@ __device__ __forceinline__ void triplet_tile(const float (&s_j)[kTJ], const floa
         const float em = fast_ex2(-fabsf(x) * kLog2e);
         const float t = 1.0f + em;
         const float r = fast_rcp(t);
-        lg += valid ? (fmaxf(x, 0.0f) * kLog2e + fast_lg2(t)) : 0.0f;
+        const float l1p = (em < kSeriesMax) ? ln_1p_small(em) * kLog2e : fast_lg2(t);
+        lg += valid ? (fmaxf(x, 0.0f) * kLog2e + l1p) : 0.0f;
         sg[a][b] = valid ? (x >= 0.0f ? r : em * r) : 0.0f;
       }
     }
   }
 }
 
+// The reference counts a triplet as positive when fp32(S_ik - S_ij) > 1e-16f (triplet_loss_utils.py:114).  fp32(b - a) is monotone
+// in b, so that test is S_ik > t(S_ij) with t(a) = the largest fp32 b for which fp32(b - a) <= 1e-16f: one compare per triplet.
+// t(a) = a whenever |a| >= 2^-29 (one ulp of a exceeds 1e-16f).  Below, a bisection on the ordered-integer encoding of fp32 finds it
+// (stepping ulp by ulp would take ~2^23 steps near a = -1e-16); the staging loops run it once per positive, not per triplet.
+__device__ __forceinline__ int f32_ordered(float f) { const int b = __float_as_int(f); return b < 0 ? -(b & 0x7fffffff) : b; }
+__device__ __forceinline__ float f32_from_ordered(int o) { return __int_as_float(o < 0 ? ((-o) | (int)0x80000000) : o); }
+__device__ __noinline__ float pos_threshold_small(float a) {
+  int lo = f32_ordered(a), hi = f32_ordered(__fadd_rn(a, 1e-15f));   // fp32(a - a) = 0 passes, fp32(hi - a) ~ 1e-15 fails
+  while (hi - lo > 1) {
+    const int mid = lo + ((hi - lo) >> 1);
+    if (__fsub_rn(f32_from_ordered(mid), a) <= 1e-16f) lo = mid; else hi = mid;
+  }
+  return f32_from_ordered(lo);
+}
+__device__ __forceinline__ float pos_threshold(float a) { return fabsf(a) >= 0x1p-29f ? a : pos_threshold_small(a); }
+
 // smem layout (floats): sj[Pj] uj[Pj] gj[Pj] | sk[Pk] vk[Pk] | gk[kTY][Pk]      Pj, Pk = padded counts
-// sj holds S_ij + 1e-16 so that the reference's positive test (S_ik - S_ij) > 1e-16 is one compare per triplet.
+// sj holds pos_threshold(S_ij), so that the reference's positive test is one compare per triplet.
 template <int TIER>
 __device__ __forceinline__ void triplet_sweep(const float* sj, const float* uj, float* gj, const float* sk, const float* vk, float* gk,
                                               int Pj, int Pk, int Pk_max, int tx, int ty, float& lacc, int& npos) {
@@ -130,7 +154,7 @@ __device__ __forceinline__ void triplet_sweep(const float* sj, const float* uj, 
 #pragma unroll
         for (int a = 0; a < kTJ; ++a) {
 #pragma unroll
-          for (int b = 0; b < kTK; ++b)   // (S_ik - S_ij) > 1e-16 (triplet_loss_utils.py:114): one compare + one predicated add
+          for (int b = 0; b < kTK; ++b)   // fp32(S_ik - S_ij) > 1e-16 (triplet_loss_utils.py:114): one compare + one predicated add
             asm("{ .reg .pred p; setp.gt.f32 p, %1, %2; @p add.s32 %0, %0, 1; }" : "+r"(npos) : "f"(s_k[b]), "f"(s_j[a]));
         }
         float4* g = reinterpret_cast<float4*>(gk + ty * Pk_max + q0);
@@ -158,7 +182,7 @@ __device__ __forceinline__ void triplet_sweep(const float* sj, const float* uj, 
       for (int a = 0; a < kTJ; ++a) {
 #pragma unroll
         for (int b = 0; b < kTK; ++b) {
-          // (S_ik - S_ij) > 1e-16 (triplet_loss_utils.py:114): one compare + one predicated add
+          // fp32(S_ik - S_ij) > 1e-16 (triplet_loss_utils.py:114): one compare + one predicated add
           asm("{ .reg .pred p; setp.gt.f32 p, %1, %2; @p add.s32 %0, %0, 1; }" : "+r"(npos) : "f"(s_k[b]), "f"(s_j[a]));
           rs[a] += sg[a][b];
           cs[b] += sg[a][b];
@@ -230,7 +254,7 @@ __global__ void __launch_bounds__(kTripThreads) triplet_batch_all_kernel(const f
     const int c = lo + p;
     const bool ok = (p < nj) && (c != i);
     const float s = ok ? srow[c] : 3.0e38f;               // +huge: never "positive", contributes 0
-    sj[p] = ok ? s + 1e-16f : s;   // (S_ik - S_ij) > 1e-16 becomes one compare per triplet
+    sj[p] = ok ? pos_threshold(s) : s;   // fp32(S_ik - S_ij) > 1e-16 becomes one compare per triplet
     uj[p] = ok ? fast_ex2((mid - s) * kLog2e) : 0.0f;
     gj[p] = 0.0f;
   }
@@ -362,7 +386,7 @@ __global__ void __launch_bounds__(kTripThreads) triplet_batch_all_tiled_kernel(c
         const int c = lo + j0 + p;
         const bool ok = (p < cj) && (c != i);
         const float s = ok ? srow[c] : 3.0e38f;
-        sj[p] = ok ? s + 1e-16f : s;
+        sj[p] = ok ? pos_threshold(s) : s;
         uj[p] = ok ? fast_ex2((mid - s) * kLog2e) : 0.0f;
         gj[p] = 0.0f;
       }
