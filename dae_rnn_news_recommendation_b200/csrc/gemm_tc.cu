@@ -861,6 +861,8 @@ struct TopkParams {
   // topk_kernel<KMAX, true>: per-row exclusion lists (CSR structure, rows sorted, no duplicates, indices in [0, N)).  Last, so the
   // fields above keep their parameter offsets in the plain instantiations.
   const int64_t* ex_indptr; const int32_t* ex_indices;
+  // topk_kernel<KMAX, true, true>: groups[c] >= 0 is corpus row c's group label; only one row per group enters a list
+  const int32_t* groups;
 };
 
 // (row block, column-tile range) work items, items blockIdx.x, blockIdx.x + gridDim.x, ...; next() returns one column tile at a time,
@@ -918,11 +920,48 @@ __device__ __forceinline__ void topk_offer(float (&sv)[KMAX], int (&si)[KMAX], f
   thr = t;
 }
 
+// GROUPS: offer (v, col) of group g to a list whose first k entries hold distinct groups, each its best so far.  If entry gp < k
+// holds g, v replaces it only if it beats it, moving up over the entries in between (entries after gp stay); otherwise (v, col)
+// goes through the ordinary insert.  Slots k..KMAX-1 hold shifted-out entries and never block a group: a group whose best left the
+// first k can only come back above thr, and then that value is its best so far.  The entries' groups live in registers (sg, REG)
+// or are reloaded from `groups` on this rare path (!REG: KMAX = 32, whose 64-register list leaves no room for 32 more).
+template <int KMAX, bool REG>
+__device__ __forceinline__ void topk_offer_group(float (&sv)[KMAX], int (&si)[KMAX], int (&sg)[REG ? KMAX : 1], float& thr, int k,
+                                                 float v, int col, int g, int n_lim, int excl, const int32_t* __restrict__ groups) {
+  if (!(v > thr) || col >= n_lim || col == excl) return;
+  int gp = KMAX - 1;                      // the last entry that may move
+  bool drop = false;
+#pragma unroll
+  for (int j = 0; j < KMAX; ++j) {
+    if (j < k) {
+      const int gj = REG ? sg[REG ? j : 0] : (si[j] >= 0 ? __ldg(groups + si[j]) : -1);
+      if (gj == g) { gp = j; drop = !(v > sv[j]); }
+    }
+  }
+  if (drop) return;
+#pragma unroll
+  for (int j = KMAX - 1; j >= 0; --j) {   // topk_offer's update, on entries 0..gp only
+    const bool up = (j > 0) && j <= gp && (v > sv[j > 0 ? j - 1 : 0]);
+    const bool here = j <= gp && v > sv[j];
+    si[j] = up ? si[j > 0 ? j - 1 : 0] : (here ? col : si[j]);
+    if constexpr (REG) sg[REG ? j : 0] = up ? sg[REG && j > 0 ? j - 1 : 0] : (here ? g : sg[REG ? j : 0]);
+    sv[j] = up ? sv[j > 0 ? j - 1 : 0] : (here ? v : sv[j]);
+  }
+  float t = sv[0];
+#pragma unroll
+  for (int j = 1; j < KMAX; ++j)
+    asm("{\n.reg .pred q;\nsetp.eq.s32 q, %1, %2;\nselp.f32 %0, %3, %0, q;\n}\n" : "+f"(t) : "r"(j), "r"(k - 1), "f"(sv[j]));
+  thr = t;
+}
+
 // EXCL: the columns in row m's exclusion list are never candidates.  Before scanning a tile, the epilogue thread writes -inf over
 // the listed columns of its own (row, 64-column half) staging run -- its alone until it arrives on `drained` -- and -inf never beats
 // thr.  A cursor into the sorted list, placed by binary search at the item's first column, only moves forward during the item; the
 // next listed column waits in a register, so a tile without a listed column costs one compare.
-template <int KMAX, bool EXCL = false>
+// GROUPS (with EXCL; ex_indptr may be null: no lists): the list holds the k best group representatives of the columns seen
+// (topk_offer_group), the groups of its entries in registers.  Each epilogue warp copies the labels of its 64 columns of the tile
+// to shared memory, as pair_hist_kernel does; they are read only on the rare path behind the unchanged `max > thr` filter.
+template <int KMAX, bool EXCL = false, bool GROUPS = false>
 __global__ void __launch_bounds__(kDecodeThreads, 1) topk_kernel(const __grid_constant__ CUtensorMap tm_a_hi,
                                                                  const __grid_constant__ CUtensorMap tm_a_lo,
                                                                  const __grid_constant__ CUtensorMap tm_b_hi,
@@ -993,6 +1032,10 @@ __global__ void __launch_bounds__(kDecodeThreads, 1) topk_kernel(const __grid_co
     const float* srow = stg + row_in_tile * SROW + half * HALF_N;
     float sv[KMAX];
     int si[KMAX];
+    constexpr bool REG_GROUPS = GROUPS && KMAX <= 16;
+    [[maybe_unused]] int sg[REG_GROUPS ? KMAX : 1];                   // GROUPS, KMAX = 16: the group of each entry
+    [[maybe_unused]] __shared__ __align__(16) int32_t s_grp[8][HALF_N];   // GROUPS: per epilogue warp, its 64 columns' labels
+    [[maybe_unused]] const int ew = warp - 12;                        // epilogue warp 0..7
     float thr = neg_inf();
     int m = 0, excl = -1;
     [[maybe_unused]] int64_t ex_cur = 0, ex_end = 0;   // EXCL: cursor into row m's list and its end
@@ -1003,13 +1046,17 @@ __global__ void __launch_bounds__(kDecodeThreads, 1) topk_kernel(const __grid_co
       if (sched.first) {
 #pragma unroll
         for (int j = 0; j < KMAX; ++j) { sv[j] = neg_inf(); si[j] = -1; }
+        if constexpr (REG_GROUPS) {
+#pragma unroll
+          for (int j = 0; j < KMAX; ++j) sg[j] = -1;
+        }
         thr = neg_inf();
         m = mb * BLOCK_M + row_in_tile;
         const int64_t e = (int64_t)m + tp.diag_offset;
         excl = (tp.exclude && e >= 0 && e < p.N) ? (int)e : -1;
         if constexpr (EXCL) {
           ex_next = INT_MAX;
-          if (m < p.M) {
+          if (m < p.M && (!GROUPS || tp.ex_indptr)) {
             const int c_first = nb * BLOCK_N + half * HALF_N;   // the first column this thread sees in the item
             int64_t lo = tp.ex_indptr[m], hi = tp.ex_indptr[m + 1];
             ex_end = hi;
@@ -1023,6 +1070,12 @@ __global__ void __launch_bounds__(kDecodeThreads, 1) topk_kernel(const __grid_co
         }
       }
       const int n0 = nb * BLOCK_N + half * HALF_N;
+      if constexpr (GROUPS) {   // the previous tile's reads ended at the __syncwarp before `drained`
+        const int j0 = n0 + lane, j1 = n0 + 32 + lane;
+        s_grp[ew][lane] = j0 < p.N ? tp.groups[j0] : -1;
+        s_grp[ew][lane + 32] = j1 < p.N ? tp.groups[j1] : -1;
+        __syncwarp();
+      }
       mbar_wait(&staged_bar[h], tphase);
       if (m < p.M) {
         if constexpr (EXCL) {
@@ -1036,10 +1089,18 @@ __global__ void __launch_bounds__(kDecodeThreads, 1) topk_kernel(const __grid_co
         for (int c = 0; c < HALF_N; c += 4) {
           const float4 v = *reinterpret_cast<const float4*>(srow + c);
           if (fmaxf(fmaxf(v.x, v.y), fmaxf(v.z, v.w)) > thr) {   // rare once the list has filled
-            topk_offer<KMAX>(sv, si, thr, k, v.x, n0 + c, p.N, excl);
-            topk_offer<KMAX>(sv, si, thr, k, v.y, n0 + c + 1, p.N, excl);
-            topk_offer<KMAX>(sv, si, thr, k, v.z, n0 + c + 2, p.N, excl);
-            topk_offer<KMAX>(sv, si, thr, k, v.w, n0 + c + 3, p.N, excl);
+            if constexpr (GROUPS) {
+              const int4 g = *reinterpret_cast<const int4*>(&s_grp[ew][c]);
+              topk_offer_group<KMAX, REG_GROUPS>(sv, si, sg, thr, k, v.x, n0 + c, g.x, p.N, excl, tp.groups);
+              topk_offer_group<KMAX, REG_GROUPS>(sv, si, sg, thr, k, v.y, n0 + c + 1, g.y, p.N, excl, tp.groups);
+              topk_offer_group<KMAX, REG_GROUPS>(sv, si, sg, thr, k, v.z, n0 + c + 2, g.z, p.N, excl, tp.groups);
+              topk_offer_group<KMAX, REG_GROUPS>(sv, si, sg, thr, k, v.w, n0 + c + 3, g.w, p.N, excl, tp.groups);
+            } else {
+              topk_offer<KMAX>(sv, si, thr, k, v.x, n0 + c, p.N, excl);
+              topk_offer<KMAX>(sv, si, thr, k, v.y, n0 + c + 1, p.N, excl);
+              topk_offer<KMAX>(sv, si, thr, k, v.z, n0 + c + 2, p.N, excl);
+              topk_offer<KMAX>(sv, si, thr, k, v.w, n0 + c + 3, p.N, excl);
+            }
           }
         }
       }
@@ -1617,7 +1678,7 @@ static int launch_decode(const Operand& A, const Operand& B, const GemmParams& p
 }
 
 // fused similarity + k-best: Q [M x K] and C [N x K], both K-major; one persistent CTA per SM over the (row block, split) work items
-template <int KMAX, bool EXCL>
+template <int KMAX, bool EXCL, bool GROUPS = false>
 static int launch_topk(const Operand& A, const Operand& B, const TopkParams& tp, cudaStream_t st) {
   CUtensorMap ta_hi, ta_lo, tb_hi, tb_lo;
   int rc;
@@ -1628,7 +1689,7 @@ static int launch_topk(const Operand& A, const Operand& B, const TopkParams& tp,
   if ((rc = make_map(&tb_lo, B.lo, p.K, p.N, B.ld, kDecodeN, kTopkBK))) return rc;
   // operand ring + accumulator staging tile + alignment slack
   constexpr int smem = kTopkStages * (2 * BLOCK_M * kTopkBK * 2 + 2 * kDecodeN * kTopkBK * 2) + BLOCK_M * (kDecodeN + 4) * 4 + 1024;
-  auto kern = topk_kernel<KMAX, EXCL>;
+  auto kern = topk_kernel<KMAX, EXCL, GROUPS>;
   static bool attr_done[64] = {false};
   if ((rc = ensure_smem_attr(kern, smem, attr_done))) return rc;
   const int items = ((p.M + BLOCK_M - 1) / BLOCK_M) * tp.splits;
@@ -2032,6 +2093,43 @@ extern "C" int dae_similarity_topk_excl_bf16x3(int32_t n_query, int32_t n_corpus
   DAE_CHECK_LAUNCH("dae_similarity_topk_excl_bf16x3");
   topk_merge_kernel<<<(n_query + 7) / 8, 256, 0, st>>>(tp.ws_val, tp.ws_idx, n_query, 2 * s, k, idx_out, val_out);
   DAE_CHECK_LAUNCH("dae_similarity_topk_excl_bf16x3 (merge)");
+  return DAE_OK;
+}
+
+extern "C" int dae_similarity_topk_groups_bf16x3(int32_t n_query, int32_t n_corpus, int32_t dim, const void* q_hi, const void* q_lo,
+                                                 int64_t ldq, const void* c_hi, const void* c_lo, int64_t ldc, int32_t k,
+                                                 int64_t diag_offset, int32_t exclude, int32_t splits, void* workspace,
+                                                 int64_t workspace_bytes, int32_t* idx_out, float* val_out, const int64_t* ex_indptr,
+                                                 const int32_t* ex_indices, int64_t ex_nnz, const int32_t* groups, void* stream) {
+  DAE_REQUIRE(q_hi && q_lo && c_hi && c_lo && workspace && idx_out && val_out && groups && (ex_nnz == 0 || (ex_indptr && ex_indices)),
+              "dae_similarity_topk_groups_bf16x3: null pointer");
+  DAE_REQUIRE(n_query > 0 && n_corpus > 0 && dim > 0 && ex_nnz >= 0, "dae_similarity_topk_groups_bf16x3: bad sizes");
+  DAE_REQUIRE(k >= 1 && k <= kTopkMaxK, "dae_similarity_topk_groups_bf16x3: k = %d is outside the supported range 1 <= k <= %d", k,
+              kTopkMaxK);
+  DAE_REQUIRE(ldq >= dim && ldc >= dim && ldq % 8 == 0 && ldc % 8 == 0,
+              "dae_similarity_topk_groups_bf16x3: leading dimensions must cover dim and be multiples of 8 (TMA 16-byte strides)");
+  DAE_REQUIRE(((uintptr_t)q_hi | (uintptr_t)q_lo | (uintptr_t)c_hi | (uintptr_t)c_lo | (uintptr_t)workspace) % 16 == 0 &&
+                  (uintptr_t)ex_indptr % 8 == 0 && ((uintptr_t)ex_indices | (uintptr_t)groups) % 4 == 0,
+              "dae_similarity_topk_groups_bf16x3: operands and workspace must be 16-byte, ex_indptr 8-byte, ex_indices and groups "
+              "4-byte aligned");
+  const int s = topk_splits(n_query, n_corpus, splits);
+  const int64_t need = topk_workspace_bytes(n_query, k, s);
+  DAE_REQUIRE(workspace_bytes >= need,
+              "dae_similarity_topk_groups_bf16x3: workspace of %lld bytes, %lld needed (dae_similarity_topk_workspace)",
+              (long long)workspace_bytes, (long long)need);
+  cudaStream_t st = (cudaStream_t)stream;
+  TopkParams tp{};
+  tp.g.M = n_query; tp.g.N = n_corpus; tp.g.K = dim; tp.g.k_splits = 1; tp.g.alpha = 1.0f; tp.g.special_col = -1;
+  tp.k = k; tp.splits = s; tp.exclude = exclude ? 1 : 0; tp.diag_offset = diag_offset;
+  tp.ws_val = reinterpret_cast<float*>(workspace);
+  tp.ws_idx = reinterpret_cast<int32_t*>(reinterpret_cast<float*>(workspace) + (int64_t)n_query * 2 * s * k);
+  tp.ex_indptr = ex_indptr; tp.ex_indices = ex_indices; tp.groups = groups;
+  Operand A{q_hi, q_lo, ldq, 0}, B{c_hi, c_lo, ldc, 0};
+  int rc = (k <= 16) ? launch_topk<16, true, true>(A, B, tp, st) : launch_topk<32, true, true>(A, B, tp, st);
+  if (rc) return rc;
+  DAE_CHECK_LAUNCH("dae_similarity_topk_groups_bf16x3");
+  topk_merge_groups_kernel<<<(n_query + 7) / 8, 256, 0, st>>>(tp.ws_val, tp.ws_idx, groups, n_query, 2 * s, k, idx_out, val_out);
+  DAE_CHECK_LAUNCH("dae_similarity_topk_groups_bf16x3 (merge)");
   return DAE_OK;
 }
 

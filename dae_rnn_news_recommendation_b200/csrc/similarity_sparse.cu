@@ -165,9 +165,11 @@ struct SpParams {
   // kSpTopkExcl: per-query exclusion lists (CSR structure, rows sorted, no duplicates, indices in [0, n_corpus)).  Last, so the
   // fields above keep their parameter offsets in the other modes.
   const int64_t* ex_indptr; const int32_t* ex_indices;
+  // kSpTopkGroups: groups[c] >= 0 is corpus row c's group label; only one row per group enters a list
+  const int32_t* groups;
 };
 
-enum SpMode { kSpTopk, kSpHist, kSpPairs, kSpTopkExcl };
+enum SpMode { kSpTopk, kSpHist, kSpPairs, kSpTopkExcl, kSpTopkGroups };
 
 // offer (v, col) to the warp's list (lane j < k holds entry j); warp-uniform arguments
 __device__ __forceinline__ void sp_offer(float v, int col, int n_corpus, int excl, int k, int lane, float& lv, int& li, float& thr) {
@@ -180,6 +182,28 @@ __device__ __forceinline__ void sp_offer(float v, int col, int n_corpus, int exc
   thr = __shfl_sync(kFull, lv, k - 1);
 }
 
+// sp_offer for a list of group representatives (lane j < k also holds entry j's group lg; the groups are distinct).  If entry
+// `last` holds g, v replaces it only if it beats it, and the entries from v's position to `last` move down one lane; otherwise
+// (v, col) goes through the ordinary insert.
+__device__ __forceinline__ void sp_offer_group(float v, int col, const int32_t* __restrict__ groups, int n_corpus, int excl, int k,
+                                               int lane, float& lv, int& li, int& lg, float& thr) {
+  if (!(v > thr) || col >= n_corpus || col == excl) return;
+  const int g = __ldg(groups + col);
+  const unsigned same = __ballot_sync(kFull, lane < k && lg == g);
+  int last = k - 1;                       // the last entry that may move
+  if (same) {
+    last = __ffs(same) - 1;
+    if (!(v > __shfl_sync(kFull, lv, last))) return;
+  }
+  const int pos = __popc(__ballot_sync(kFull, lane < k && lv >= v));   // <= last: the list is sorted and lv[last] < v
+  const float uv = __shfl_up_sync(kFull, lv, 1);
+  const int ui = __shfl_up_sync(kFull, li, 1);
+  const int ug = __shfl_up_sync(kFull, lg, 1);
+  if (lane == pos) { lv = v; li = col; lg = g; }
+  else if (lane > pos && lane <= last) { lv = uv; li = ui; lg = ug; }
+  thr = __shfl_sync(kFull, lv, k - 1);
+}
+
 // kSpTopk: k-best lists (dae_csr_similarity_topk).  kSpHist: the related / unrelated pair histogram of Q against itself
 // (dae_csr_similarity_pair_hist): the same postings, accumulation and scores, but only the ranges that start below q are
 // accumulated and only slots c < q are counted -- the strict lower triangle.  The scan bins every non-zero slot (runs of equal
@@ -189,9 +213,12 @@ __device__ __forceinline__ void sp_offer(float v, int col, int n_corpus, int exc
 // kSpTopkExcl: kSpTopk, but the corpus rows in q's exclusion list are never candidates.  Before each slab scan the warp writes -inf
 // into the listed slots of the range, 32 list entries per load from a cursor that only moves forward (placed by binary search at
 // the split's first row); -inf never beats thr, and the scan zeroes those slots as it does the others.
+// kSpTopkGroups: kSpTopkExcl (ex_indptr may be null: no lists) whose list holds the k best group representatives of the slots
+// scanned (sp_offer_group); the duplicate test is one ballot over the lanes' groups.
 template <SpMode MODE>
 __global__ void __launch_bounds__(kSpWarps * 32, 3) sp_topk_kernel(const SpParams p) {
   constexpr bool HIST = MODE == kSpHist;
+  constexpr bool EXCL = MODE == kSpTopkExcl || MODE == kSpTopkGroups;
   extern __shared__ float4 sp_smem4[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int64_t item = (int64_t)blockIdx.x * kSpWarps + warp;
@@ -219,8 +246,9 @@ __global__ void __launch_bounds__(kSpWarps * 32, 3) sp_topk_kernel(const SpParam
   for (int j = lane; j < kSpW / 4; j += 32) slab4[j] = make_float4(0.f, 0.f, 0.f, 0.f);
   float lv = neg_inf(), thr = neg_inf();
   int li = -1;
-  [[maybe_unused]] int64_t ex_cur = 0, ex_end = 0;   // kSpTopkExcl: cursor into q's list and its end (warp-uniform)
-  if constexpr (MODE == kSpTopkExcl) {
+  [[maybe_unused]] int lg = -1;                      // kSpTopkGroups: the group of entry `lane`
+  [[maybe_unused]] int64_t ex_cur = 0, ex_end = 0;   // EXCL: cursor into q's list and its end (warp-uniform)
+  if constexpr (EXCL) if (MODE == kSpTopkExcl || p.ex_indptr) {
     int64_t lo = p.ex_indptr[q], hi = p.ex_indptr[q + 1];
     ex_end = hi;
     const int c_first = r0 * kSpW;
@@ -296,7 +324,7 @@ __global__ void __launch_bounds__(kSpWarps * 32, 3) sp_topk_kernel(const SpParam
         }
       }
     } else {
-      if constexpr (MODE == kSpTopkExcl) {
+      if constexpr (EXCL) {
         // -inf into the listed slots of this range; the list is sorted, so the lanes below the range's end form a prefix
         while (ex_cur < ex_end) {
           const int c = (ex_cur + lane < ex_end) ? p.ex_indices[ex_cur + lane] : INT_MAX;
@@ -319,10 +347,17 @@ __global__ void __launch_bounds__(kSpWarps * 32, 3) sp_topk_kernel(const SpParam
           const float y0 = __shfl_sync(kFull, x.x, l), y1 = __shfl_sync(kFull, x.y, l);
           const float y2 = __shfl_sync(kFull, x.z, l), y3 = __shfl_sync(kFull, x.w, l);
           const int c = base + j0 + 4 * l;
-          sp_offer(y0, c, p.n_corpus, excl, k, lane, lv, li, thr);
-          sp_offer(y1, c + 1, p.n_corpus, excl, k, lane, lv, li, thr);
-          sp_offer(y2, c + 2, p.n_corpus, excl, k, lane, lv, li, thr);
-          sp_offer(y3, c + 3, p.n_corpus, excl, k, lane, lv, li, thr);
+          if constexpr (MODE == kSpTopkGroups) {
+            sp_offer_group(y0, c, p.groups, p.n_corpus, excl, k, lane, lv, li, lg, thr);
+            sp_offer_group(y1, c + 1, p.groups, p.n_corpus, excl, k, lane, lv, li, lg, thr);
+            sp_offer_group(y2, c + 2, p.groups, p.n_corpus, excl, k, lane, lv, li, lg, thr);
+            sp_offer_group(y3, c + 3, p.groups, p.n_corpus, excl, k, lane, lv, li, lg, thr);
+          } else {
+            sp_offer(y0, c, p.n_corpus, excl, k, lane, lv, li, thr);
+            sp_offer(y1, c + 1, p.n_corpus, excl, k, lane, lv, li, thr);
+            sp_offer(y2, c + 2, p.n_corpus, excl, k, lane, lv, li, thr);
+            sp_offer(y3, c + 3, p.n_corpus, excl, k, lane, lv, li, thr);
+          }
         }
       }
     }
@@ -407,14 +442,18 @@ extern "C" int dae_csr_similarity_topk_workspace(int32_t n_query, int32_t n_corp
   return DAE_OK;
 }
 
-// dae_csr_similarity_topk (excl false) and dae_csr_similarity_topk_excl (excl true, the lists ex_indptr / ex_indices)
+// dae_csr_similarity_topk (excl false), dae_csr_similarity_topk_excl (excl true, the lists ex_indptr / ex_indices) and
+// dae_csr_similarity_topk_groups (excl true, groups non-null; ex_indptr may be null when ex_nnz = 0: no lists)
 static int csr_topk(const char* fn, const int64_t* q_indptr, const int32_t* q_indices, const float* q_values, int32_t n_query,
                     int64_t q_nnz, int32_t q_features, const int64_t* c_indptr, const int32_t* c_indices, const float* c_values,
                     int32_t n_corpus, int64_t c_nnz, int32_t c_features, int32_t k, int64_t diag_offset, int32_t exclude,
                     int32_t splits, void* workspace, int64_t workspace_bytes, int32_t* idx_out, float* val_out, bool excl,
-                    const int64_t* ex_indptr, const int32_t* ex_indices, int64_t ex_nnz, void* stream) {
+                    const int64_t* ex_indptr, const int32_t* ex_indices, int64_t ex_nnz, const int32_t* groups, bool grouped,
+                    void* stream) {
   DAE_REQUIRE(q_indptr && c_indptr && workspace && idx_out && val_out && (q_nnz == 0 || (q_indices && q_values)) &&
-              (c_nnz == 0 || (c_indices && c_values)) && (!excl || (ex_indptr && (ex_nnz == 0 || ex_indices))), "%s: null pointer", fn);
+              (c_nnz == 0 || (c_indices && c_values)) &&
+              (!excl || (grouped ? (groups && (ex_nnz == 0 || (ex_indptr && ex_indices))) : (ex_indptr && (ex_nnz == 0 || ex_indices)))),
+              "%s: null pointer", fn);
   DAE_REQUIRE(n_query > 0 && n_corpus > 0 && q_features > 0 && c_features > 0 && q_nnz >= 0 && c_nnz >= 0 && c_nnz < INT32_MAX &&
               (!excl || ex_nnz >= 0), "%s: bad sizes", fn);
   DAE_REQUIRE(k >= 1 && k <= kSpMaxK, "%s: k = %d is outside the supported range 1 <= k <= %d", fn, k, kSpMaxK);
@@ -422,6 +461,7 @@ static int csr_topk(const char* fn, const int64_t* q_indptr, const int32_t* q_in
   DAE_REQUIRE((uintptr_t)workspace % 16 == 0, "%s: workspace must be 16-byte aligned", fn);
   DAE_REQUIRE(!excl || ((uintptr_t)ex_indptr % 8 == 0 && (uintptr_t)ex_indices % 4 == 0),
               "%s: ex_indptr must be 8-byte, ex_indices 4-byte aligned", fn);
+  DAE_REQUIRE((uintptr_t)groups % 4 == 0, "%s: groups must be 4-byte aligned", fn);
   const SpLayout L = sp_layout(n_query, n_corpus, c_nnz, c_features, k, splits);
   DAE_REQUIRE(workspace_bytes >= L.total, "%s: workspace of %lld bytes, %lld needed (dae_csr_similarity_topk_workspace)", fn,
               (long long)workspace_bytes, (long long)L.total);
@@ -440,11 +480,14 @@ static int csr_topk(const char* fn, const int64_t* q_indptr, const int32_t* q_in
   sp.idx_out = idx_out; sp.val_out = val_out;
   sp.ws_val = reinterpret_cast<float*>(ws + L.off_val);
   sp.ws_idx = reinterpret_cast<int32_t*>(ws + L.off_idx);
-  sp.ex_indptr = ex_indptr; sp.ex_indices = ex_indices;
-  if ((rc = excl ? sp_launch<kSpTopkExcl>(sp, st) : sp_launch<kSpTopk>(sp, st))) return rc;
+  sp.ex_indptr = ex_indptr; sp.ex_indices = ex_indices; sp.groups = groups;
+  if ((rc = grouped ? sp_launch<kSpTopkGroups>(sp, st) : excl ? sp_launch<kSpTopkExcl>(sp, st) : sp_launch<kSpTopk>(sp, st))) return rc;
   DAE_CHECK_LAUNCH(fn);
   if (L.splits > 1) {
-    topk_merge_kernel<<<(n_query + 7) / 8, 256, 0, st>>>(sp.ws_val, sp.ws_idx, n_query, L.splits, k, idx_out, val_out);
+    if (grouped)
+      topk_merge_groups_kernel<<<(n_query + 7) / 8, 256, 0, st>>>(sp.ws_val, sp.ws_idx, groups, n_query, L.splits, k, idx_out, val_out);
+    else
+      topk_merge_kernel<<<(n_query + 7) / 8, 256, 0, st>>>(sp.ws_val, sp.ws_idx, n_query, L.splits, k, idx_out, val_out);
     DAE_CHECK_LAUNCH("sparse similarity top-k (merge)");
   }
   return DAE_OK;
@@ -457,7 +500,7 @@ extern "C" int dae_csr_similarity_topk(const int64_t* q_indptr, const int32_t* q
                                        int32_t* idx_out, float* val_out, void* stream) {
   return csr_topk("dae_csr_similarity_topk", q_indptr, q_indices, q_values, n_query, q_nnz, q_features, c_indptr, c_indices, c_values,
                   n_corpus, c_nnz, c_features, k, diag_offset, exclude, splits, workspace, workspace_bytes, idx_out, val_out, false,
-                  nullptr, nullptr, 0, stream);
+                  nullptr, nullptr, 0, nullptr, false, stream);
 }
 
 extern "C" int dae_csr_similarity_topk_excl(const int64_t* q_indptr, const int32_t* q_indices, const float* q_values, int32_t n_query,
@@ -468,7 +511,18 @@ extern "C" int dae_csr_similarity_topk_excl(const int64_t* q_indptr, const int32
                                             const int32_t* ex_indices, int64_t ex_nnz, void* stream) {
   return csr_topk("dae_csr_similarity_topk_excl", q_indptr, q_indices, q_values, n_query, q_nnz, q_features, c_indptr, c_indices,
                   c_values, n_corpus, c_nnz, c_features, k, diag_offset, exclude, splits, workspace, workspace_bytes, idx_out, val_out,
-                  true, ex_indptr, ex_indices, ex_nnz, stream);
+                  true, ex_indptr, ex_indices, ex_nnz, nullptr, false, stream);
+}
+
+extern "C" int dae_csr_similarity_topk_groups(const int64_t* q_indptr, const int32_t* q_indices, const float* q_values, int32_t n_query,
+                                              int64_t q_nnz, int32_t q_features, const int64_t* c_indptr, const int32_t* c_indices,
+                                              const float* c_values, int32_t n_corpus, int64_t c_nnz, int32_t c_features, int32_t k,
+                                              int64_t diag_offset, int32_t exclude, int32_t splits, void* workspace,
+                                              int64_t workspace_bytes, int32_t* idx_out, float* val_out, const int64_t* ex_indptr,
+                                              const int32_t* ex_indices, int64_t ex_nnz, const int32_t* groups, void* stream) {
+  return csr_topk("dae_csr_similarity_topk_groups", q_indptr, q_indices, q_values, n_query, q_nnz, q_features, c_indptr, c_indices,
+                  c_values, n_corpus, c_nnz, c_features, k, diag_offset, exclude, splits, workspace, workspace_bytes, idx_out, val_out,
+                  true, ex_indptr, ex_indices, ex_nnz, groups, true, stream);
 }
 
 extern "C" int dae_csr_similarity_pair_hist_workspace(int32_t n, int64_t nnz, int32_t n_features, int64_t* bytes) {

@@ -3,15 +3,18 @@ nearest-article lookup of main_autoencoder.py:307-318,352-359) -- SURVEY section
 
     pairwise_similarity(in_df, norm='', metric='cosine', set_diagonal_zero=True) -> ndarray [N, N]     (reference signature)
     nearest_neighbors(embeddings, metric='cosine', chunk=8192) -> (index[N], score[N])                (no N x N matrix on the host)
-    top_k_similar(embeddings, k=10, corpus=None, metric='cosine', exclude=None) -> (index[Nq, k], score[Nq, k])
+    top_k_similar(embeddings, k=10, corpus=None, metric='cosine', exclude=None, groups=None) -> (index[Nq, k], score[Nq, k])
                                                                                                       (no similarity matrix at all;
                                                                                                         dense or scipy sparse inputs;
-                                                                                                        per-query exclusion lists)
+                                                                                                        per-query exclusion lists;
+                                                                                                        at most one row per group)
     label_precision_at_k(index, query_labels, corpus_labels) -> float                                 (share of same-label neighbours)
     user_profiles(histories, embeddings) -> [U, H]                                                    (weighted mean of the read articles)
-    recommend(histories, embeddings, k=10, candidates=None, exclude_read=True, profiles=None) -> (index[U, k], score[U, k])
+    recommend(histories, embeddings, k=10, candidates=None, exclude_read=True, profiles=None, groups=None)
+                                                                                   -> (index[U, k], score[U, k])
                                                                                                       (k best unread articles per user;
-                                                                                                        mean or given profiles)
+                                                                                                        mean or given profiles;
+                                                                                                        one article per story)
     sequences_from_csr(m) -> (indptr[U + 1], items)                                                   (reads ordered by stored time)
     recommendation_recall(index, targets) -> dict                                                     (hit rate / recall of held-out reads)
     similar_pairs(data, threshold, corpus=None, metric='cosine') -> (i[P], j[P], score[P])            (every pair with score >= threshold,
@@ -139,10 +142,11 @@ def nearest_neighbors(embeddings, metric='cosine', chunk=8192, device='cuda:0'):
     return idx.cpu().numpy(), val.cpu().numpy()
 
 
-def _similarity_topk(q, c, n_q, n_c, h, k, diag_offset=0, exclude=False, splits=0, lists=None):
+def _similarity_topk(q, c, n_q, n_c, h, k, diag_offset=0, exclude=False, splits=0, lists=None, groups=None):
     """k best corpus rows per query row of the bf16 hi / lo operand pairs q and c (dae_similarity_topk_bf16x3): device tensors
     (index int32 [n_q, k], score float32 [n_q, k]); with `exclude`, column i + diag_offset is not a candidate of row i.  lists:
-    per-row exclusion lists (_DeviceLists) through dae_similarity_topk_excl_bf16x3."""
+    per-row exclusion lists (_DeviceLists) through dae_similarity_topk_excl_bf16x3.  groups: device int32 [n_c] labels, at most
+    one row per group (dae_similarity_topk_groups_bf16x3, with or without lists)."""
     dev = q[0].device
     need = (ctypes.c_int64 * 1)()
     call('dae_similarity_topk_workspace', n_q, n_c, k, splits, ctypes.addressof(need))
@@ -151,11 +155,20 @@ def _similarity_topk(q, c, n_q, n_c, h, k, diag_offset=0, exclude=False, splits=
     val = torch.empty(n_q, k, dtype=torch.float32, device=dev)
     args = (n_q, n_c, h, q[0].data_ptr(), q[1].data_ptr(), q[0].stride(0), c[0].data_ptr(), c[1].data_ptr(), c[0].stride(0), k, diag_offset,
             1 if exclude else 0, splits, ws.data_ptr(), ws.numel(), idx.data_ptr(), val.data_ptr())
-    if lists is None:
+    if groups is not None:
+        call('dae_similarity_topk_groups_bf16x3', *args, *_list_args(lists), groups.data_ptr(), _stream())
+    elif lists is None:
         call('dae_similarity_topk_bf16x3', *args, _stream())
     else:
         call('dae_similarity_topk_excl_bf16x3', *args, lists.indptr.data_ptr(), lists.indices.data_ptr(), lists.nnz, _stream())
     return idx, val
+
+
+def _list_args(lists):
+    """(ex_indptr, ex_indices, ex_nnz) of the *_groups exports: NULL pointers for no lists."""
+    if lists is None:
+        return None, None, 0
+    return lists.indptr.data_ptr(), (lists.indices.data_ptr() if lists.nnz else None), lists.nnz
 
 
 class _DeviceLists:
@@ -211,10 +224,11 @@ def _csr_operand(x, metric):
     return m
 
 
-def _csr_similarity_topk(q, c, k, diag_offset=0, exclude=False, splits=0, lists=None):
+def _csr_similarity_topk(q, c, k, diag_offset=0, exclude=False, splits=0, lists=None, groups=None):
     """k best corpus rows per query row of the DeviceCSR matrices q and c by S = Q.C^T (dae_csr_similarity_topk): device tensors
     (index int32 [n_q, k], score float32 [n_q, k]); with `exclude`, column i + diag_offset is not a candidate of row i.  lists:
-    per-row exclusion lists (_DeviceLists) through dae_csr_similarity_topk_excl."""
+    per-row exclusion lists (_DeviceLists) through dae_csr_similarity_topk_excl.  groups: device int32 [n_c] labels, at most one
+    row per group (dae_csr_similarity_topk_groups)."""
     dev = q.indptr.device
     n_q, n_c = q.shape[0], c.shape[0]
     need = (ctypes.c_int64 * 1)()
@@ -225,22 +239,60 @@ def _csr_similarity_topk(q, c, k, diag_offset=0, exclude=False, splits=0, lists=
     args = (q.indptr.data_ptr(), q.indices.data_ptr(), q.values.data_ptr(), n_q, q.nnz, q.shape[1], c.indptr.data_ptr(),
             c.indices.data_ptr(), c.values.data_ptr(), n_c, c.nnz, c.shape[1], k, diag_offset, 1 if exclude else 0, splits, ws.data_ptr(),
             ws.numel(), idx.data_ptr(), val.data_ptr())
-    if lists is None:
+    if groups is not None:
+        call('dae_csr_similarity_topk_groups', *args, *_list_args(lists), groups.data_ptr(), _stream())
+    elif lists is None:
         call('dae_csr_similarity_topk', *args, _stream())
     else:
         call('dae_csr_similarity_topk_excl', *args, lists.indptr.data_ptr(), lists.indices.data_ptr(), lists.nnz, _stream())
     return idx, val
 
 
-def _top_k_similar_sparse(embeddings, k, corpus, metric, device, splits, lists=None):
+def _top_k_similar_sparse(embeddings, k, corpus, metric, device, splits, lists=None, groups=None):
     if corpus is not None and corpus.shape[1] != embeddings.shape[1]:
         raise ValueError('top_k_similar: corpus rows have %d columns, queries %d' % (corpus.shape[1], embeddings.shape[1]))
     q = DeviceCSR(_csr_operand(embeddings, metric), device)
     c = q if corpus is None else DeviceCSR(_csr_operand(corpus, metric), device)
-    return _csr_similarity_topk(q, c, k, exclude=corpus is None, splits=splits, lists=lists)
+    return _csr_similarity_topk(q, c, k, exclude=corpus is None, splits=splits, lists=lists, groups=groups)
 
 
-def top_k_similar(embeddings, k=10, corpus=None, metric='cosine', device='cuda:0', to_host=True, splits=0, exclude=None):
+def _group_labels(groups, n, fn):
+    """groups as int32 [n] on the host: ValueError unless it is a 1-D integer array of n labels in [0, 2^31)."""
+    g = np.asarray(groups.cpu() if isinstance(groups, torch.Tensor) else groups)
+    if g.ndim != 1 or g.shape[0] != n:
+        raise ValueError('%s: groups has shape %s, [%d] (one label per corpus row) expected' % (fn, g.shape, n))
+    if not np.issubdtype(g.dtype, np.integer):
+        raise ValueError('%s: groups must hold integers, not %s' % (fn, g.dtype))
+    if g.size and (g.min() < 0 or g.max() > np.iinfo(np.int32).max):
+        raise ValueError('%s: groups hold a label outside [0, 2^31)' % fn)
+    return g.astype(np.int32)
+
+
+def _read_group_lists(indptr, indices, groups, corpus_groups):
+    """recommend's exclusion lists with groups: user u's list holds every corpus position whose group holds an article u read.
+    indptr int64 [U + 1] / indices int32: the canonical history CSR over article rows; groups: int32 labels of the article rows;
+    corpus_groups: int32 labels of the corpus positions (groups[candidates], or groups).  Torch tensors on one device; vectorised,
+    no per-user loop.  Returns (indptr int64 [U + 1], indices int32), rows sorted and without duplicates."""
+    dev = indices.device
+    n_u, n_c = indptr.numel() - 1, corpus_groups.numel()
+    users = torch.repeat_interleave(torch.arange(n_u, device=dev), indptr[1:] - indptr[:-1])
+    n_g = max(int(groups.max()), int(corpus_groups.max())) + 1
+    pairs = torch.unique(users * n_g + groups[indices.long()].long())              # the (user, group) pairs read, sorted
+    p_user, p_group = pairs // n_g, pairs % n_g
+    cg = corpus_groups.long()
+    order = torch.argsort(cg, stable=True)                                         # corpus positions by group
+    cg_sorted = cg[order]
+    start = torch.searchsorted(cg_sorted, p_group)
+    count = torch.searchsorted(cg_sorted, p_group, right=True) - start
+    pair = torch.repeat_interleave(torch.arange(pairs.numel(), device=dev), count)
+    offset = torch.arange(pair.numel(), device=dev) - (torch.cumsum(count, 0) - count)[pair]
+    keys = torch.sort(p_user[pair] * n_c + order[start[pair] + offset]).values     # groups are disjoint: no duplicates
+    out_ptr = torch.zeros(n_u + 1, dtype=torch.int64, device=dev)
+    out_ptr[1:] = torch.cumsum(torch.bincount(keys // n_c, minlength=n_u), 0)
+    return out_ptr, (keys % n_c).to(torch.int32)
+
+
+def top_k_similar(embeddings, k=10, corpus=None, metric='cosine', device='cuda:0', to_host=True, splits=0, exclude=None, groups=None):
     """For every row of `embeddings` the k most similar rows of `corpus` and their scores, best first (among equal scores the
     lower index first), without forming the similarity matrix.  corpus=None ranks the set against itself and leaves each row's
     self match out.  Rows with fewer than k candidates are padded with index -1 and score -inf.  metric: 'cosine' or
@@ -251,6 +303,13 @@ def top_k_similar(embeddings, k=10, corpus=None, metric='cosine', device='cuda:0
     exclude: a scipy sparse matrix [Nq, Nc] whose stored positions (i, j) are never returned for query i (values ignored,
     explicit zeros count), e.g. the articles a user has read; the kernels skip them in their epilogues (dae_*_topk_excl*), and
     the self match stays out with corpus=None.  A wrong shape or an index outside it raises ValueError before any device work.
+    groups: an integer array [Nc] of labels >= 0 of the corpus rows (the rows themselves with corpus=None), e.g. duplicate_groups'
+    output: rows with equal labels are one story, and at most one row per group is returned -- the group's best candidate by
+    (score desc, index asc), with scores bit-identical to the call without groups.  The selection happens in the kernels
+    (dae_*_topk_groups*), so a story with many rewrites cannot leave the list short.  It composes with `exclude`: an excluded row
+    hands its group to the group's next best candidate.  With corpus=None only the self match is left out; the other members of
+    the query's own group remain candidates (pass them in `exclude` to leave them out too).  A wrong length, a non-integer dtype
+    or a label outside [0, 2^31) raises ValueError before any device work.
     Returns (index int32 [Nq, k], score float32 [Nq, k]) as ndarrays, or device tensors with to_host=False.  `splits`
     (> 0) fixes the number of corpus parts the work is cut into; it does not change the result."""
     assert metric in ['cosine', 'linear kernel']
@@ -258,14 +317,16 @@ def top_k_similar(embeddings, k=10, corpus=None, metric='cosine', device='cuda:0
         raise _cabi.DaeError('top_k_similar: k = %d is outside the supported range 1 <= k <= 32' % k)
     if corpus is not None and sp.issparse(embeddings) != sp.issparse(corpus):
         raise ValueError('top_k_similar: queries and corpus must be both sparse or both dense')
-    lists = None
+    lists = g_dev = None
+    n_c = embeddings.shape[0] if corpus is None else corpus.shape[0]
     if exclude is not None:
-        n_q = embeddings.shape[0]
-        n_c = n_q if corpus is None else corpus.shape[0]
-        indptr, indices, _ = _stored_positions(exclude, (n_q, n_c), 'exclude', 'top_k_similar')
+        indptr, indices, _ = _stored_positions(exclude, (embeddings.shape[0], n_c), 'exclude', 'top_k_similar')
+    if groups is not None:
+        g_dev = torch.from_numpy(_group_labels(groups, n_c, 'top_k_similar')).to(device)
+    if exclude is not None:
         lists = _DeviceLists.from_host(indptr, indices, device)
     if sp.issparse(embeddings):
-        idx, val = _top_k_similar_sparse(embeddings, k, corpus, metric, device, splits, lists)
+        idx, val = _top_k_similar_sparse(embeddings, k, corpus, metric, device, splits, lists, g_dev)
         if to_host:
             return idx.cpu().numpy(), val.cpu().numpy()
         return idx, val
@@ -281,7 +342,7 @@ def top_k_similar(embeddings, k=10, corpus=None, metric='cosine', device='cuda:0
             raise ValueError('top_k_similar: corpus rows have %d columns, queries %d' % (xc.shape[1], h))
         n_c = xc.shape[0]
         c = _normalised_operands(xc, norm_kind)[:2]
-    idx, val = _similarity_topk(q, c, n_q, n_c, h, k, exclude=corpus is None, splits=splits, lists=lists)
+    idx, val = _similarity_topk(q, c, n_q, n_c, h, k, exclude=corpus is None, splits=splits, lists=lists, groups=g_dev)
     if to_host:
         return idx.cpu().numpy(), val.cpu().numpy()
     return idx, val
@@ -377,7 +438,7 @@ def sequences_from_csr(m):
 
 
 def recommend(histories, embeddings, k=10, candidates=None, metric='cosine', exclude_read=True, device='cuda:0', to_host=True,
-              splits=0, profiles=None):
+              splits=0, profiles=None, groups=None):
     """For every user the k best articles by `metric` between the user's profile (user_profiles: the weighted mean of the read
     articles' embeddings) and the articles: 'cosine', or 'linear kernel' (the plain inner product).  Order, ties and padding as in
     top_k_similar.  exclude_read: no article of the user's history is returned -- the history goes to the top-k kernel as the
@@ -386,6 +447,10 @@ def recommend(histories, embeddings, k=10, candidates=None, metric='cosine', exc
     A user without reads, or whose weights sum to 0, gets a padding row (-1 / -inf).  Embeddings only: dense [N, H].
     profiles: an optional [U, H] array or tensor ranked in place of the mean profiles (e.g. UserGRU.transform's user vectors); the
     histories still give the exclusion lists and the padding rows.
+    groups: an integer array [N] of labels >= 0 of the article rows (e.g. duplicate_groups' output): at most one article per group
+    is recommended, as in top_k_similar(groups=...).  With exclude_read, every article of a group the user has read is excluded
+    too, so a user is not shown a rewrite of a story they read; those lists are built on the device from the histories and the
+    labels (over the candidates' positions when candidates are given).
     Returns (index int32 [U, k], score float32 [U, k]) as ndarrays (device tensors with to_host=False)."""
     if metric not in ('cosine', 'linear kernel'):
         raise ValueError("recommend: metric = %r: 'cosine' or 'linear kernel'" % (metric,))
@@ -396,8 +461,9 @@ def recommend(histories, embeddings, k=10, candidates=None, metric='cosine', exc
         _dense_embeddings(embeddings, device, 'recommend')
     w, empty = _history_weights(histories, n_art, 'recommend')
     cand = None if candidates is None else _candidate_rows(candidates, n_art, 'recommend')
+    g = None if groups is None else _group_labels(groups, n_art, 'recommend')
     lists_host = None
-    if exclude_read and cand is not None:
+    if exclude_read and cand is not None and g is None:
         lists_host = _remap_lists(w.indptr, w.indices, cand)
     if profiles is not None:
         if sp.issparse(profiles) or tuple(profiles.shape) != (w.shape[0], embeddings.shape[1]):
@@ -406,12 +472,19 @@ def recommend(histories, embeddings, k=10, candidates=None, metric='cosine', exc
     emb = _dense_embeddings(embeddings, device, 'recommend')
     hist = DeviceCSR(w, device)
     prof = _profiles(hist, emb) if profiles is None else _as_device_dense(profiles, emb.device)
-    lists = None
-    if exclude_read:
-        lists = _DeviceLists(hist.indptr, hist.indices, hist.nnz) if cand is None else _DeviceLists.from_host(*lists_host, device)
     cand_dev = None if cand is None else torch.from_numpy(cand).to(device)
+    g_dev = cg_dev = None
+    if g is not None:
+        g_dev = torch.from_numpy(g).to(device)
+        cg_dev = g_dev if cand_dev is None else g_dev.index_select(0, cand_dev)
+    lists = None
+    if exclude_read and g is not None:
+        ptr, ind = _read_group_lists(hist.indptr, hist.indices, g_dev, cg_dev)
+        lists = _DeviceLists(ptr, ind, ind.numel())
+    elif exclude_read:
+        lists = _DeviceLists(hist.indptr, hist.indices, hist.nnz) if cand is None else _DeviceLists.from_host(*lists_host, device)
     corpus = emb if cand is None else emb.index_select(0, cand_dev)
-    idx, val = _recommend_topk(prof, corpus, k, metric, lists, splits)
+    idx, val = _recommend_topk(prof, corpus, k, metric, lists, splits, cg_dev)
     if empty.any():
         e = torch.from_numpy(empty).to(device)
         idx[e] = -1
@@ -423,12 +496,13 @@ def recommend(histories, embeddings, k=10, candidates=None, metric='cosine', exc
     return idx, val
 
 
-def _recommend_topk(prof, corpus, k, metric, lists, splits=0):
-    """The ranking half of recommend: profiles [U, H] against corpus [Nc, H] on the tensor cores, with the exclusion lists."""
+def _recommend_topk(prof, corpus, k, metric, lists, splits=0, groups=None):
+    """The ranking half of recommend: profiles [U, H] against corpus [Nc, H] on the tensor cores, with the exclusion lists and
+    the corpus rows' group labels."""
     norm_kind = 2 if metric == 'cosine' else 0
     q = _normalised_operands(prof, norm_kind)[:2]
     c = _normalised_operands(corpus, norm_kind)[:2]
-    return _similarity_topk(q, c, prof.shape[0], corpus.shape[0], prof.shape[1], k, splits=splits, lists=lists)
+    return _similarity_topk(q, c, prof.shape[0], corpus.shape[0], prof.shape[1], k, splits=splits, lists=lists, groups=groups)
 
 
 def recommendation_recall(index, targets):

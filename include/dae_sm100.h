@@ -382,6 +382,28 @@ int dae_csr_similarity_topk_excl(const int64_t* q_indptr, const int32_t* q_indic
                                  int32_t* idx_out, float* val_out, const int64_t* ex_indptr, const int32_t* ex_indices,
                                  int64_t ex_nnz, void* stream);
 
+/* ---- at most one article per story: top-k over near-duplicate groups ------------------------------------------------
+ * dae_similarity_topk_groups_bf16x3 / dae_csr_similarity_topk_groups: the *_excl exports with the same arguments, workspace (the
+ *   plain *_workspace queries) and exclusion lists, plus groups int32 [n_corpus]: one label >= 0 per corpus row, rows with equal
+ *   labels forming one group (helpers.duplicate_groups' output fits as is).  For each query row the candidates are those of the
+ *   *_excl call; each group is represented by its candidate that comes first by (score desc, index asc), and the k best
+ *   representatives are returned in that order, padded with -1 / -inf.  Scores are the plain calls' bits; the result does not
+ *   depend on `splits`.  ex_indptr may be NULL (no lists; ex_nnz must then be 0).  groups 4-byte aligned.  The kernels do not
+ *   check the label values: the caller guarantees 0 <= groups[c].  With groups[c] = c the output equals the *_excl call's bit for
+ *   bit (the plain call's without lists).
+ */
+int dae_similarity_topk_groups_bf16x3(int32_t n_query, int32_t n_corpus, int32_t dim, const void* q_hi, const void* q_lo,
+                                      int64_t ldq, const void* c_hi, const void* c_lo, int64_t ldc, int32_t k,
+                                      int64_t diag_offset, int32_t exclude, int32_t splits, void* workspace,
+                                      int64_t workspace_bytes, int32_t* idx_out, float* val_out, const int64_t* ex_indptr,
+                                      const int32_t* ex_indices, int64_t ex_nnz, const int32_t* groups, void* stream);
+int dae_csr_similarity_topk_groups(const int64_t* q_indptr, const int32_t* q_indices, const float* q_values, int32_t n_query,
+                                   int64_t q_nnz, int32_t q_features, const int64_t* c_indptr, const int32_t* c_indices,
+                                   const float* c_values, int32_t n_corpus, int64_t c_nnz, int32_t c_features, int32_t k,
+                                   int64_t diag_offset, int32_t exclude, int32_t splits, void* workspace, int64_t workspace_bytes,
+                                   int32_t* idx_out, float* val_out, const int64_t* ex_indptr, const int32_t* ex_indices,
+                                   int64_t ex_nnz, const int32_t* groups, void* stream);
+
 /* ---- "next" row (SURVEY 8f rank 2): related-vs-unrelated AUROC of a pairwise similarity matrix ---------------------
  * Replaces the numeric part of helpers.visualize_pairwise_similarity (helpers.py:88-100).
  * dae_pair_partition: for every pair i > j of the strict lower triangle with labels[i] >= 0 and labels[j] >= 0

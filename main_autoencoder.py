@@ -69,6 +69,12 @@ def build_parser():
     ap.add_argument('--top_k_input', action='store_true', default=False,
                     help='with --top_k K: also rank by the input vectors (cosine for binary, linear kernel for tf-idf), save '
                          'article_top_k_input_{index,score}[_validate].npy and report their label precision next to the embedding\'s')
+    ap.add_argument('--top_k_dedup', type=float, default=0.0,
+                    help='with --top_k K: T > 0 groups the training articles whose embedding cosine similarity is >= T (near-duplicates, '
+                         'helpers.similar_pairs + duplicate_groups) and saves K-best lists with at most one article per group as '
+                         'article_top_k_dedup_{index,score}[_validate].npy (and user_top_k_dedup_{index,score}.npy with '
+                         '--user_histories, read groups excluded); their label precision (and hit rate / recall) is reported next to '
+                         'the plain lists\'; 0 = off')
     ap.add_argument('--dedup_threshold', type=float, default=0.0,
                     help='T > 0: after transform, list every pair of training articles whose embedding cosine similarity is >= T '
                          '(near-duplicates) and every (validation, training) pair, save them with their duplicate groups as '
@@ -146,6 +152,8 @@ def check_flags(F):
     assert F.label in ['category_publish_name', 'story']
     assert 0 <= F.top_k <= 32
     assert not F.top_k_input or F.top_k > 0, '--top_k_input needs --top_k K > 0'
+    assert F.top_k_dedup >= 0.0
+    assert not F.top_k_dedup or F.top_k > 0, '--top_k_dedup needs --top_k K > 0'
     assert F.dedup_threshold >= 0.0
     assert not F.dedup_input or F.dedup_threshold > 0, '--dedup_input needs --dedup_threshold T > 0'
     assert not F.user_histories or F.top_k > 0, '--user_histories needs --top_k K > 0'
@@ -347,6 +355,42 @@ def recommend_top_k_input(F, model, trX, vlX, trL, vlL, emb_out):
     return out
 
 
+def recommend_top_k_dedup(F, model, enc, enc_v, trL, vlL, histories, targets, emb_out):
+    """--top_k_dedup T: the --top_k lists with at most one article per story.  The training articles are grouped by
+    helpers.similar_pairs(enc, T) + duplicate_groups; top_k_similar / recommend then take each group's best article only (and
+    recommend leaves out every group a user has read).  Saved as article_top_k_dedup_{index,score}[_validate].npy and
+    user_top_k_dedup_{index,score}.npy; the label precision (hit rate / recall with --user_targets) is printed next to the plain
+    lists' (emb_out)."""
+    from dae_rnn_news_recommendation_b200 import helpers
+    out = {}
+    i, j, _ = helpers.similar_pairs(enc, F.top_k_dedup, metric='cosine')
+    groups = helpers.duplicate_groups(i, j, enc.shape[0])
+    n_groups = int(np.unique(groups).size)
+    print('calculate top %d similar articles, one per duplicate group (cosine >= %g: %d groups of %d articles)'
+          % (F.top_k, F.top_k_dedup, n_groups, enc.shape[0]))
+    for split, E, lab in (('', enc, trL), ('_validate', enc_v, vlL)):
+        if E is None or E.shape[0] == 0:
+            continue
+        idx, score = helpers.top_k_similar(E, k=F.top_k, corpus=None if split == '' else enc, metric='cosine', groups=groups)
+        np.save(model.data_dir + 'article_top_k_dedup_index' + split, idx)
+        np.save(model.data_dir + 'article_top_k_dedup_score' + split, score)
+        out['top_k_dedup' + split] = (idx, score)
+        out['top_k_dedup_precision' + split] = helpers.label_precision_at_k(idx, lab, trL)
+        print('top %d%s label precision: one per group %.4f  plain %.4f' % (
+            F.top_k, split, out['top_k_dedup_precision' + split], emb_out.get('top_k_precision' + split, float('nan'))))
+    if histories is not None:
+        idx, score = helpers.recommend(histories, enc, k=F.top_k, groups=groups)
+        np.save(model.data_dir + 'user_top_k_dedup_index', idx)
+        np.save(model.data_dir + 'user_top_k_dedup_score', score)
+        if targets is not None:
+            r = helpers.recommendation_recall(idx, targets)
+            out.update({'user_dedup_hit_rate': r['hit_rate'], 'user_dedup_recall': r['recall']})
+            print('users, one per group: hit rate@%d %.4f recall@%d %.4f  plain: hit rate %.4f recall %.4f (%d users with targets)' % (
+                F.top_k, r['hit_rate'], F.top_k, r['recall'], emb_out.get('user_hit_rate', float('nan')),
+                emb_out.get('user_recall', float('nan')), r['users']))
+    return out
+
+
 def find_duplicates(F, model, X, X_v, trL, vlL, metric, name, emb_out=None):
     """--dedup_threshold T: every pair of training rows of X with similarity >= T (self) and every (validation, training) pair
     (corpus), through helpers.similar_pairs, without the similarity matrix.  Saved under data_dir as <name>[_validate].npz with
@@ -498,6 +542,8 @@ def main(argv=None):
             model.evaluation.update(recommend_users(F, model, enc, histories, targets))
         if seqs is not None:
             model.evaluation.update(recommend_users_gru(F, model, enc, seqs))
+        if F.top_k_dedup > 0:
+            model.evaluation.update(recommend_top_k_dedup(F, model, enc, enc_v, trL, vlL, histories, targets, model.evaluation))
     if F.dedup_threshold > 0:
         model.evaluation.update(find_duplicates(F, model, enc, enc_v, trL, vlL, 'cosine', 'article_duplicates'))
         if F.dedup_input:
