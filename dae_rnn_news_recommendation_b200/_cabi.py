@@ -88,6 +88,8 @@ _SIGNATURES = {
     'dae_pairs_sort_workspace': (C.c_int, [i64, i32, p]),
     'dae_allreduce_multimem': (C.c_int, [p, p, p, i32, i32, i64, i32, p]),
     'dae_mask_values': (C.c_int, [p, p, i64, f32, u64, u64, p, p]),
+    'dae_salt_pepper_csr': (C.c_int, [p, p, p, i64, i64, i32, i64, f32, f32, p, u64, u64, p, p, p, i64, p, p, sz, p]),
+    'dae_salt_pepper_workspace': (C.c_int, [i64, p]),
     # GRU user encoder
     'dae_gather_split_bf16': (C.c_int, [p, i64, p, i32, i32, p, p, i64, i32, p]),
     'dae_gru_cell_fwd': (C.c_int, [i32, i32, p, i64, p, i64, p, i64, p, i64, i32, p, p, i64, p, i64, p]),

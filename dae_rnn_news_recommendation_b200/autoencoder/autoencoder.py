@@ -161,18 +161,25 @@ class DenoisingAutoencoder(object):
 
     def _host_rng_prefetch(self, train_csr_host, n):
         """rng_mode='numpy': the reference's per-epoch draws from the global NumPy stream -- rand(nnz) for the masking noise
-        (utils.py:111), then the shuffle of the row order (utils.py:50-51) -- produced IN THAT ORDER by a worker thread that runs
-        one epoch ahead of the GPU.  Returns a function handing out (keep mask or None, permutation) epoch by epoch."""
+        (utils.py:111) or the salt-and-pepper draws (utils.py:137-139), then the shuffle of the row order (utils.py:50-51) -- produced IN
+        THAT ORDER by a worker thread that runs one epoch ahead of the GPU.  Returns a function handing out (keep mask / packed draws or
+        None, permutation) epoch by epoch.  The salt-and-pepper draws take N * v * 4 bytes per epoch (1.2 GB at 100 000 rows of 10 000
+        features, corr_frac 0.3): at most one epoch waits in the queue, so the host holds at most three (queued, being drawn, in use)."""
         import queue
         import threading
-        if self.rng_mode != 'numpy' or self.corr_type not in ('masking', 'none', 'decay'):
+        if self.rng_mode != 'numpy' or self.corr_type not in ('masking', 'none', 'decay', 'salt_and_pepper'):
             return None
-        q = queue.Queue(maxsize=2)
+        sp_v = self._salt_pepper_v(train_csr_host) if self.corr_type == 'salt_and_pepper' else None
+        q = queue.Queue(maxsize=1 if sp_v is not None else 2)
 
         def work():
             try:
                 for _ in range(self.num_epochs):
-                    keep = utils.masking_keep_mask(train_csr_host, self.corr_frac) if self.corr_type == 'masking' else None
+                    keep = None
+                    if self.corr_type == 'masking':
+                        keep = utils.masking_keep_mask(train_csr_host, self.corr_frac)
+                    elif sp_v is not None:
+                        keep = utils.salt_and_pepper_draws(train_csr_host, sp_v)
                     order = list(range(n))
                     np.random.shuffle(order)
                     q.put((keep, np.asarray(order, dtype=np.int32)))
@@ -189,8 +196,20 @@ class DenoisingAutoencoder(object):
         take.thread = t
         return take
 
+    def _salt_pepper_v(self, train_csr_host):
+        return int(np.round(self.corr_frac * train_csr_host.shape[1]))  # autoencoder.py:187
+
+    def _salt_pepper_range(self, train_csr_host):
+        """(lo, hi) of salt-and-pepper noise: X.min() / X.max() over the whole matrix, implicit zeros included (utils.py:129), computed
+        once per host matrix."""
+        c = getattr(self, '_sp_range', None)
+        if c is None or c[0] is not train_csr_host:
+            c = self._sp_range = (train_csr_host, float(train_csr_host.min()), float(train_csr_host.max()))
+        return c[1], c[2]
+
     def _corrupt_on_device(self, train_csr_host, epoch, keep=None):
-        """Per-epoch corruption of the WHOLE training set (autoencoder.py:218,248-270)."""
+        """Per-epoch corruption of the WHOLE training set (autoencoder.py:218,248-270).  keep: rng_mode='numpy' draws of the epoch (the
+        masking keep mask, or the packed salt-and-pepper draws), or None to draw them here."""
         eng = self.engine
         eng.in_scale = 1.0
         if self.corr_type == 'masking':
@@ -204,9 +223,14 @@ class DenoisingAutoencoder(object):
             eng.set_data(eng.csr, None, eng.labels)
             eng.in_scale = 1.0 - self.corr_frac
         elif self.corr_type == 'salt_and_pepper':
-            v = np.round(self.corr_frac * train_csr_host.shape[1]).astype(int)  # autoencoder.py:187
-            xc = utils.salt_and_pepper_noise(train_csr_host, v)
-            eng.set_data(eng.csr, None, eng.labels, csr_corrupt=DeviceCSR(xc, eng.device))
+            v = self._salt_pepper_v(train_csr_host)
+            lo, hi = self._salt_pepper_range(train_csr_host)
+            if self.rng_mode == 'numpy':
+                if keep is None:
+                    keep = utils.salt_and_pepper_draws(train_csr_host, v)
+                eng.corrupt_salt_pepper(v, lo, hi, draws_host=keep)
+            else:
+                eng.corrupt_salt_pepper(v, lo, hi, seed=max(self.seed, 0), epoch=epoch)
         elif self.corr_type == 'none':
             eng.set_data(eng.csr, None, eng.labels)
         else:
@@ -233,10 +257,11 @@ class DenoisingAutoencoder(object):
         if self.rng_mode == 'device' and self.seed >= 0:
             torch.manual_seed(self.seed)
         # Full-size batches are replayed from ONE captured CUDA graph (their offsets are start0 + g * stride, advanced on the
-        # device); a short last batch runs eagerly.  Salt-and-pepper rebuilds the corrupted CSR every epoch -> eager.
+        # device); a short last batch runs eagerly.  Every corruption writes into buffers allocated once, so the graph reads each
+        # epoch's corrupted copy at the same addresses.
         full = [s0 for s0 in starts if s0 + bs <= n]
         tail = [s0 for s0 in starts if s0 + bs > n]
-        use_graph = (os.environ.get('DAE_CUDA_GRAPH', '1') == '1' and self.corr_type != 'salt_and_pepper' and len(full) >= 2)
+        use_graph = (os.environ.get('DAE_CUDA_GRAPH', '1') == '1' and len(full) >= 2)
         perm_buf = torch.zeros(n, dtype=torch.int32, device=eng.device)
         R = self.mining_block_rows
         nv = 0 if validation_set is None else validation_set.shape[0]
@@ -291,6 +316,8 @@ class DenoisingAutoencoder(object):
                     eng.step(perm_buf, s0, min(bs, n - s0), log[k])
             torch.cuda.synchronize(eng.device)
             self.train_time = time.time() - t0
+            if self.corr_type == 'salt_and_pepper':
+                eng.check_corruption()
             vals = log[:len(starts)].cpu().numpy()
             self.history.append(vals.copy())
             self.train_cost_batch = (list(vals[:, STAT['cost']].astype(np.float32)),

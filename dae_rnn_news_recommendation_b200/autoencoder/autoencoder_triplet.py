@@ -69,11 +69,13 @@ class DenoisingAutoencoderTriplet(DenoisingAutoencoder):
             vhost = [canonical_csr(validation_set[k]) for k in keys]
             vcsr = (DeviceCSR(sp.vstack(vhost).tocsr(), eng.device), vhost[0].shape[0])
             eng._ensure_ws(3 * max(bs, vcsr[1]))   # size the workspaces once: a larger validation batch must not force a re-capture
-        # Full-size batches are replayed from ONE captured CUDA graph (device-side row ids and cursors); a short last batch and the
-        # salt-and-pepper corruption (its CSR is rebuilt every epoch) run eagerly.
+        # Full-size batches are replayed from ONE captured CUDA graph (device-side row ids and cursors); a short last batch runs eagerly.
         full = [s0 for s0 in starts if s0 + bs <= n]
         tail = [s0 for s0 in starts if s0 + bs > n]
-        use_graph = (os.environ.get('DAE_CUDA_GRAPH', '1') == '1' and self.corr_type != 'salt_and_pepper' and len(full) >= 2)
+        use_graph = (os.environ.get('DAE_CUDA_GRAPH', '1') == '1' and len(full) >= 2)
+        if self.corr_type == 'salt_and_pepper':   # the reference calls salt_and_pepper_noise once per stream: lo / hi per stream
+            sp_v = int(np.round(self.corr_frac * n_features_of(host[0])))
+            sp_segments = [(k * n, n, float(h.min()), float(h.max())) for k, h in enumerate(host)]
         perm_buf = torch.zeros(n, dtype=torch.int32, device=eng.device)
         # DenoisingAutoencoder's condition (rng_mode 'numpy' draws from np.random, seeded in __init__), here only in the deterministic
         # mode: the default mode's explicit-triplet runs keep the device permutations they always drew
@@ -94,9 +96,12 @@ class DenoisingAutoencoderTriplet(DenoisingAutoencoder):
             elif self.corr_type == 'decay':
                 eng.in_scale = 1.0 - self.corr_frac
             elif self.corr_type == 'salt_and_pepper':
-                v = np.round(self.corr_frac * n_features_of(host[0])).astype(int)
-                xc = sp.vstack([utils.salt_and_pepper_noise(h, v) for h in host]).tocsr()
-                eng.set_data(csr, None, None, csr_corrupt=DeviceCSR(xc, eng.device))
+                # three appended calls over the stacked rows; rng_mode 'numpy' draws org, pos, neg in that order
+                if self.rng_mode == 'numpy':
+                    draws = np.concatenate([utils.salt_and_pepper_draws(h, sp_v).reshape(-1) for h in host])
+                    eng.corrupt_salt_pepper(sp_v, None, None, draws_host=draws, segments=sp_segments)
+                else:
+                    eng.corrupt_salt_pepper(sp_v, None, None, seed=max(self.seed, 0), epoch=i, segments=sp_segments)
             perm_buf.copy_(self._epoch_permutation(n))
             if world > 1:
                 torch.distributed.broadcast(perm_buf, src=0, group=eng.pg)
@@ -113,6 +118,8 @@ class DenoisingAutoencoderTriplet(DenoisingAutoencoder):
                     eng.step_explicit(perm_buf, s0, min(bs, n - s0), n, log[k])
             torch.cuda.synchronize(eng.device)
             self.train_time = time.time() - t0
+            if self.corr_type == 'salt_and_pepper':
+                eng.check_corruption()
             vals = log[:len(starts)].cpu().numpy()
             self.train_cost_batch = (list(vals[:, STAT['cost']].astype(np.float32)),
                                      list(vals[:, STAT['ae_loss']].astype(np.float32)),

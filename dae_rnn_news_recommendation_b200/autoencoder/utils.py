@@ -107,6 +107,21 @@ def salt_and_pepper_noise(X, v):
     return out.tocsr() if not isinstance(X, np.ndarray) else out
 
 
+def salt_and_pepper_draws(X, v):
+    """The draws salt_and_pepper_noise(X, v) takes from the global NumPy stream, in its order -- per row randint(0, F, v), then v
+    random() calls (as one random_sample(v): the same numbers) -- packed as uint32[rows x v] = column | (u >= 0.5) << 31, bit 31 set
+    where the draw writes the maximum.  dae_salt_pepper_csr applied to them reproduces salt_and_pepper_noise(X, v) bit for bit."""
+    n, F = X.shape
+    assert F < (1 << 30) and v >= 0
+    v = int(v)
+    out = np.empty((n, v), dtype=np.uint32)
+    for i in range(n):
+        m = np.random.randint(0, F, v)
+        u = np.random.random_sample(v)
+        out[i] = m.astype(np.uint32) | ((u >= 0.5).astype(np.uint32) << np.uint32(31))
+    return out
+
+
 def decay_noise(X, v):
     """X * (1 - v) (reference utils.py:147-159)."""
     return X.copy() * (1. - v)

@@ -526,6 +526,61 @@ class TrainEngine:
         self._k('dae_mask_values', ptr(self.csr.values), ptr(keep), self.csr.nnz, float(corr_frac), int(seed), int(epoch),
                 ptr(self.values_c), _stream())
 
+    def salt_pepper_buffers(self, v):
+        """The corrupted-CSR buffers of salt-and-pepper noise with v draws per row over the current clean set, allocated once per data set
+        (and v): a captured step graph reads every epoch's corruption at the same addresses.  Capacity sum_r min(F, nnz_r + v) entries
+        (8 B each); max_row_nnz is the bound min(F, max_r nnz_r + v), so the step's scratch sized from it never grows between epochs."""
+        c, F, v = self.csr, self.F, int(v)
+        sp_ = getattr(self, '_sp', None)
+        if sp_ is not None and sp_['csr'] is c and sp_['v'] == v:
+            return sp_
+        self._sp = None
+        N = c.shape[0]
+        cap = int(torch.clamp(c.indptr[1:] - c.indptr[:-1] + v, max=F).sum().item()) if N else 0
+        ws_bytes = _cabi.query('dae_salt_pepper_workspace', N, ctype=ctypes.c_size_t)
+        dev = self.device
+        out = _CSRView(torch.zeros(N + 1, dtype=torch.int64, device=dev), torch.empty(max(cap, 1), dtype=torch.int32, device=dev),
+                       torch.empty(max(cap, 1), dtype=torch.float32, device=dev), c.shape)
+        out.max_row_nnz = min(F, int(c.max_row_nnz or 0) + v)
+        self._sp = {'csr': c, 'v': v, 'cap': cap, 'out': out, 'ws': torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=dev),
+                    'overflow': torch.zeros(1, dtype=torch.int32, device=dev), 'draws': None}
+        return self._sp
+
+    def corrupt_salt_pepper(self, v, lo, hi, seed=0, epoch=0, draws_host=None, segments=None):
+        """Salt-and-pepper noise of the WHOLE clean set on the device (utils.salt_and_pepper_noise, autoencoder/utils.py:118-144): the
+        corrupted copy, with its own structure, lands in the buffers of `salt_pepper_buffers(v)` and becomes the encode input csr_c.
+        segments: [(row0, n, lo, hi), ...] consecutive row ranges with their own lo / hi, appended into one CSR (the stacked [org; pos;
+        neg] set); None = one range over all rows with (lo, hi).  draws_host: uint32[rows * v] host draws in segment order
+        (utils.salt_and_pepper_draws: the reference's NumPy stream), else Philox keyed by (seed, epoch, global row)."""
+        b = self.salt_pepper_buffers(v)
+        v = b['v']
+        N = self.csr.shape[0]
+        segs = [(0, N, lo, hi)] if segments is None else [(int(r0), int(n), l, h) for r0, n, l, h in segments]
+        assert segs[0][0] == 0 and all(s[0] + s[1] == t[0] for s, t in zip(segs, segs[1:])) and segs[-1][0] + segs[-1][1] == N, \
+            'segments must tile the rows in order'
+        draws = None
+        if draws_host is not None:
+            dh = np.ascontiguousarray(draws_host, dtype=np.uint32).reshape(-1)
+            assert dh.size == N * v, 'draws_host: %d draws for %d rows x v = %d' % (dh.size, N, v)
+            if b['draws'] is None:   # one device buffer for the data set (N * v * 4 B)
+                b['draws'] = torch.empty(max(dh.size, 1), dtype=torch.int32, device=self.device)
+            b['draws'][:dh.size].copy_(torch.from_numpy(dh.view(np.int32)))
+            draws = b['draws']
+        out, ws = b['out'], b['ws']
+        for r0, n, l, h in segs:
+            self._k('dae_salt_pepper_csr', ptr(self.csr.indptr), ptr(self.csr.indices), ptr(self.csr.values), r0, n, self.F, v, float(l),
+                    float(h), None if draws is None else ptr(draws) + 4 * r0 * v, int(seed), int(epoch), ptr(out.indptr), ptr(out.indices),
+                    ptr(out.values), b['cap'], ptr(b['overflow']), ptr(ws), ws.numel(), _stream(), n_launch=3)
+        self.csr_c = out
+        self.values_c = out.values
+
+    def check_corruption(self):
+        """Raise if a salt-and-pepper call found its output beyond the buffers' capacity (it then leaves its rows empty; with the
+        capacity of salt_pepper_buffers this cannot happen).  One 4-byte read: call it once per epoch."""
+        b = getattr(self, '_sp', None)
+        if b is not None and int(b['overflow'].item()) != 0:
+            raise _cabi.DaeError('dae_salt_pepper_csr: corrupted CSR beyond its capacity of %d entries' % b['cap'])
+
     # ---- the GEMM used for the dense contractions (v1: fp32 CUDA-core kernel) ---------------------------------------
     def _gemm(self, M, N, K, alpha, A, sam, sak, Bm, sbn, sbk, beta, Cm, ldc, tag='gemm'):
         self._k('dae_sgemm', M, N, K, float(alpha), ptr(A), sam, sak, ptr(Bm), sbn, sbk, float(beta), ptr(Cm), ldc, _stream(),

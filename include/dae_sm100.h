@@ -309,6 +309,24 @@ int dae_optimizer_step(float* theta, const float* grad, float* slot1, float* slo
 int dae_mask_values(const float* values, const uint8_t* keep, int64_t nnz, float corr_frac, uint64_t seed,
                     uint64_t epoch, float* values_out, void* stream);
 
+/* Salt-and-pepper noise (utils.salt_and_pepper_noise, utils.py:118-144) of the clean CSR rows [row0, row0 + n), appended to an
+ * output CSR.  Row r draws v columns with replacement; draw j sets its column to hi (coin 1) or lo (coin 0), the last draw of a
+ * column decides, a column that ends at 0 is not stored, and untouched entries keep their clean value (explicit zeros too).  The
+ * input must be canonical (sorted, unique columns per row); so is the output.
+ *   draws == NULL: Philox4x32-10, key (seed lo, seed hi), counter (j / 2, r, epoch lo, epoch hi) with r the GLOBAL row; an even j
+ *     takes the output words (c0, c1), an odd j (c2, c3): column = floor(c_a * F / 2^32), coin = (c_b >= 2^31).
+ *   draws != NULL: n * v host draws (row-major), column | coin << 31 (utils.salt_and_pepper_draws: the reference's stream).
+ * The call writes indptr_out[row0 + 1 .. row0 + n], starting from indptr_out[row0] as the device holds it when the call runs (0 for
+ * the first call, or what the previous call on the stream wrote), so calls over consecutive row ranges form one stacked CSR.  If the
+ * total would exceed cap, no entry is written, rows row0 .. row0 + n - 1 are left empty and *overflow is set to 1 (never cleared).
+ * Sizes: F in [1, 2^30), v in [0, 2^30).  ws: dae_salt_pepper_workspace(n) bytes, reused by every call on the stream.
+ */
+int dae_salt_pepper_csr(const int64_t* indptr, const int32_t* indices, const float* values, int64_t row0, int64_t n, int32_t F,
+                        int64_t v, float lo, float hi, const uint32_t* draws, uint64_t seed, uint64_t epoch, int64_t* indptr_out,
+                        int32_t* indices_out, float* values_out, int64_t cap, int32_t* overflow, void* ws, size_t ws_bytes,
+                        void* stream);
+int dae_salt_pepper_workspace(int64_t n, size_t* bytes);
+
 /* ---- "next" row (SURVEY 8f rank 1): pairwise similarity of embeddings + nearest-article lookup -----------------
  * Replaces helpers.pairwise_similarity (helpers.py:11-50: sklearn cosine_similarity / linear_kernel, optional normalize,
  * zeroed diagonal) and the nanargmax lookup of main_autoencoder.py:352-353.  sim = normalize(E).normalize(E)^T runs on
