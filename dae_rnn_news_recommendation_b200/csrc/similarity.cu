@@ -11,7 +11,10 @@
 
 namespace dae {
 
-// one warp per row: out_hi/lo[r, :] = split( x[r, :] * s ), s = 1/max(||x||_2, 1e-12) (norm_kind 2), 1/||x||_1 (1), 1/max|x| (3), 1 (0)
+// one warp per row: out_hi/lo[r, :] = split( x[r, :] * s ), s = 1/sqrt(sum x^2) (norm_kind 2), 1/||x||_1 (1), 1/max|x| (3), 1 (0);
+// a row whose fp32 norm is 0 is left untouched (s = 1), as sklearn.preprocessing.normalize does -- including a row whose squared
+// norm underflows fp32.  A row whose squared norm overflows fp32 (max |x| above ~1.8e19) gets s = 0 and comes out as zeros.
+// Columns [cols, ld_dst) of hi / lo are written 0.
 __global__ void __launch_bounds__(256) rownorm_split_kernel(const float* __restrict__ X, int rows, int cols, int64_t ld, int norm_kind,
                                                             __nv_bfloat16* __restrict__ hi, __nv_bfloat16* __restrict__ lo, int64_t ld_dst,
                                                             float* __restrict__ x_out, int64_t ld_out) {
@@ -44,8 +47,11 @@ __global__ void __launch_bounds__(256) rownorm_split_kernel(const float* __restr
   }
 }
 
-// one warp per row: arg-max / max of S[r, :] skipping column (r + diag_offset) (np.fill_diagonal(., 0) + nanargmax semantics are
-// applied by the caller: the diagonal never wins); also optionally zeroes the diagonal entry in place.
+// one warp per row: arg-max / max of S[r, :] over the non-NaN entries, skipping column (r + diag_offset): the diagonal is never a
+// candidate, so a row whose other scores are all negative returns the best of them (the reference's nanargmax over the
+// zero-diagonal matrix would return the row itself with score 0 there).  The first maximum wins (np.argmax); -inf entries are
+// candidates.  A row without any candidate (cols = 1 with the diagonal, or all NaN) gets index -1 and value -inf, the top-k
+// kernels' padding.  Optionally zeroes the diagonal entry in place.
 __global__ void __launch_bounds__(256) row_argmax_kernel(float* __restrict__ S, int rows, int cols, int64_t ld, int64_t diag_offset,
                                                          int zero_diag, int32_t* __restrict__ idx_out, float* __restrict__ val_out) {
   const int lane = threadIdx.x & 31;
@@ -53,18 +59,18 @@ __global__ void __launch_bounds__(256) row_argmax_kernel(float* __restrict__ S, 
   if (r >= rows) return;
   float* s = S + (int64_t)r * ld;
   const int64_t dcol = (int64_t)r + diag_offset;
-  float best = -3.0e38f;
+  float best = -INFINITY;
   int bi = -1;
   for (int c = lane; c < cols; c += 32) {
     if (c == dcol) { if (zero_diag) s[c] = 0.0f; continue; }
     const float v = s[c];
-    if (v > best) { best = v; bi = c; }
+    if (v == v && (bi < 0 || v > best)) { best = v; bi = c; }   // NaN never; the first candidate always, then only a larger one
   }
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) {
     const float ob = __shfl_xor_sync(0xffffffffu, best, o);
     const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-    if (ob > best || (ob == best && oi >= 0 && (bi < 0 || oi < bi))) { best = ob; bi = oi; }   // first maximum wins (np.argmax)
+    if (oi >= 0 && (bi < 0 || ob > best || (ob == best && oi < bi))) { best = ob; bi = oi; }   // first maximum wins (np.argmax)
   }
   if (lane == 0) {
     if (idx_out) idx_out[r] = bi;

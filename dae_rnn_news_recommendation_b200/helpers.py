@@ -125,9 +125,11 @@ def _pairwise_sparse(m, norm, metric, set_diagonal_zero, device):
 
 
 def nearest_neighbors(embeddings, metric='cosine', chunk=8192, device='cuda:0'):
-    """For every row the most similar OTHER row and its score (np.nanargmax over the zero-diagonal similarity matrix,
-    main_autoencoder.py:352-353) without materialising N x N: row chunks of the similarity are produced by the GEMM and
-    reduced by dae_row_argmax on the device."""
+    """For every row the most similar OTHER row and its score (the lookup of main_autoencoder.py:352-353) without materialising
+    N x N: row chunks of the similarity are produced by the GEMM and reduced by dae_row_argmax on the device.  The first maximum
+    wins and NaN scores are skipped, as np.nanargmax does, but the row itself is never a candidate: where every other score is
+    negative the best of them is returned (the reference's nanargmax over the zero-diagonal matrix returns the row itself, with
+    score 0), and top_k_similar(k=1) follows the same rule.  A single row gets index -1 and score -inf."""
     x = _to_device_dense(embeddings, device)
     n, h = x.shape
     hi, lo, _ = _normalised_operands(x, 2 if metric == 'cosine' else 0)

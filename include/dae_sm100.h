@@ -331,9 +331,13 @@ int dae_salt_pepper_workspace(int64_t n, size_t* bytes);
  * Replaces helpers.pairwise_similarity (helpers.py:11-50: sklearn cosine_similarity / linear_kernel, optional normalize,
  * zeroed diagonal) and the nanargmax lookup of main_autoencoder.py:352-353.  sim = normalize(E).normalize(E)^T runs on
  * dae_gemm_bf16x3; these are the two kernels around it.
- * dae_rownorm_split_bf16: rows scaled by 1/||x||_2 (norm_kind 2; all-zero rows untouched, like sklearn), 1/||x||_1 (1),
- *   1/max|x| (3) or 1 (0), written as bf16 hi/lo [rows x ld_dst] (zero padded) and/or as fp32 x_out.
- * dae_row_argmax: per row arg-max / max of S skipping column row+diag_offset (optionally zeroing it in place).
+ * dae_rownorm_split_bf16: rows scaled by 1/||x||_2 (norm_kind 2), 1/||x||_1 (1), 1/max|x| (3) or 1 (0), written as bf16 hi/lo
+ *   [rows x ld_dst] (columns [cols, ld_dst) = 0) and/or as fp32 x_out.  A row whose fp32 norm is 0 (all zeros, or a squared norm
+ *   that underflows) is left untouched, like sklearn; a row whose norm overflows fp32 (for l2: max |x| above ~1.8e19) comes out
+ *   as zeros.
+ * dae_row_argmax: per row the arg-max / max of S over the non-NaN entries, skipping column row + diag_offset (optionally zeroing
+ *   it in place).  The first maximum wins (np.argmax); the skipped diagonal never wins, even when every other entry is negative.
+ *   A row without a candidate (cols = 1 with the diagonal, or every other entry NaN) gets index -1 and value -inf.
  */
 int dae_rownorm_split_bf16(const float* X, int32_t rows, int32_t cols, int64_t ld, int32_t norm_kind, void* hi, void* lo,
                            int64_t ld_dst, float* x_out, int64_t ld_out, void* stream);
@@ -576,7 +580,7 @@ int dae_triplet_loss_sum(const double* loss_slots, int32_t n, double* stats, voi
  *   dHP = [dr^, dz^, r dn^] as bf16 hi / lo rows (ld_g >= 3H) and carry <- dh z, onto which the caller accumulates dHP . W_hh.
  * dae_seq_negatives: neg[p] = (pos[p] + 1 + floor(u (n_items - 1))) mod n_items, u = c / 2^32 where c is the first word of
  *   Philox4x32-10 with key seed and counter (p, batch, epoch lo, epoch hi): uniform over the other articles, never pos[p].
- *   pos[p] < 0: neg[p] = -1.
+ *   pos[p] < 0: neg[p] = -1.  The counter's first word is p mod 2^32, so draws repeat beyond 2^32 positions in one call.
  * dae_seq_rank_loss: one warp per position p with pos[p] >= 0: x = h_p . e(neg[p]) - h_p . e(pos[p]); *loss_sum += softplus(x)
  *   (fp64 atomics); dh_p = scale s(x) (e(neg) - e(pos)).  Positions with pos[p] < 0 get dh_p = 0.
  */

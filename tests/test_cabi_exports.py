@@ -22,6 +22,15 @@ def test_header_symbols_are_exported_and_bound():
     assert lib.dae_version() >= 100
 
 
+def test_every_export_is_called_by_name_from_a_test():
+    """Each declared export appears as a quoted name ('dae_x' or "dae_x") in some tests/test_*.py other than this one, so no kernel
+    is reached only through the Python layer or not at all."""
+    here = Path(__file__).resolve()
+    texts = [p.read_text() for p in sorted((ROOT / 'tests').glob('test_*.py')) if p.resolve() != here]
+    missing = [n for n in _declared() if not any(("'%s'" % n) in t or ('"%s"' % n) in t for t in texts)]
+    assert not missing, 'exports no test calls by name: %s' % missing
+
+
 def test_bad_arguments_fail_loudly_without_gpu():
     import pytest
     from dae_rnn_news_recommendation_b200 import _cabi

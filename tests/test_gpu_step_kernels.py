@@ -68,7 +68,7 @@ def _encode_fwd(x_dev, rows, n_rows, F, H, in_scale, W, bh, act, ldE, ld_split=0
     hi = lo = None
     if ld_split:
         hi, lo = _bf16_sentinel(n_rows, ld_split), _bf16_sentinel(n_rows, ld_split)
-    rc = _cabi().lib().dae_encode_csr_fwd(ip.data_ptr(), ix.data_ptr(), vv.data_ptr(), None if rows is None else rows.data_ptr(),
+    rc = getattr(_cabi().lib(), 'dae_encode_csr_fwd')(ip.data_ptr(), ix.data_ptr(), vv.data_ptr(), None if rows is None else rows.data_ptr(),
                                           n_rows, F, H, in_scale, W.data_ptr(), bh.data_ptr(), _cabi().ACT[act], E.data_ptr(), ldE,
                                           None if col_count is None else col_count.data_ptr(), None if hi is None else hi.data_ptr(),
                                           None if lo is None else lo.data_ptr(), ld_split, _st())
@@ -215,7 +215,7 @@ def _encode_bwd_all(x, rows, n, F, H, in_scale, act, E, dE0, dE_add, bh, dW0, db
     cs, cur = torch.empty(F + 1, dtype=torch.int32, device=DEV), torch.empty(F, dtype=torch.int32, device=DEV)
     ec, er, ev = (torch.empty(cap, dtype=torch.int32, device=DEV), torch.empty(cap, dtype=torch.int32, device=DEV),
                   torch.empty(cap, device=DEV))
-    rc = c.lib().dae_encode_csr_bwd_gather(ip.data_ptr(), ix.data_ptr(), vv.data_ptr(), rows_p, n, F, H, in_scale, E.data_ptr(),
+    rc = getattr(c.lib(), 'dae_encode_csr_bwd_gather')(ip.data_ptr(), ix.data_ptr(), vv.data_ptr(), rows_p, n, F, H, in_scale, E.data_ptr(),
                                            bh.data_ptr(), c.ACT[act], dE.data_ptr(), add_p, H, dW.data_ptr(), dbh.data_ptr(),
                                            int(dbh_zeroed), cc.data_ptr(), cs.data_ptr(), cur.data_ptr(), ec.data_ptr(), er.data_ptr(),
                                            ev.data_ptr(), _st())

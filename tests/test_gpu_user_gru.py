@@ -12,24 +12,11 @@ pytestmark = pytest.mark.gpu
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+from gru_kernel_oracle import philox_first_word as _philox_first_word  # noqa: E402
 from helpers import rel_err  # noqa: E402
 from user_gru_oracle import NAMES, adam_tf, gru_states, loss_and_grads  # noqa: E402
 
 from dae_rnn_news_recommendation_b200.user_model import Packed, UserGRU, history_matrix, negatives_from_draws  # noqa: E402
-
-M32 = np.uint64(0xFFFFFFFF)
-
-
-def _philox_first_word(p, batch, epoch, seed):
-    """Philox4x32-10's first output word at counter (p, batch, epoch lo, epoch hi), key seed (NumPy, uint64 lanes)."""
-    c = [np.asarray(p, np.uint64) & M32, np.full(np.shape(p), batch, np.uint64), np.full(np.shape(p), epoch & 0xFFFFFFFF, np.uint64),
-         np.full(np.shape(p), epoch >> 32, np.uint64)]
-    k = [np.uint64(seed & 0xFFFFFFFF), np.uint64(seed >> 32)]
-    for _ in range(10):
-        p0, p1 = np.uint64(0xD2511F53) * c[0], np.uint64(0xCD9E8D57) * c[2]
-        c = [(p1 >> np.uint64(32)) ^ c[1] ^ k[0], p1 & M32, (p0 >> np.uint64(32)) ^ c[3] ^ k[1], p0 & M32]
-        k = [(k[0] + np.uint64(0x9E3779B9)) & M32, (k[1] + np.uint64(0xBB67AE85)) & M32]
-    return c[0]
 
 
 def _data(U, H, N, max_len, seed):
