@@ -1,0 +1,261 @@
+// Impression logs (DESIGN 4.13): the pairwise impression loss of the GRU user encoder and the per-impression ranking metrics.
+//
+// An impression is a list of shown articles items[indptr[i] .. indptr[i + 1]) with a click flag per article.  Both kernels give
+// one warp to one row of work and score the candidates with warp dot products (lane j takes the columns j, j + 32, ...), so a
+// candidate list of any length is walked in chunks of kImpChunk scores held in shared memory per warp.
+#include "common.cuh"
+
+namespace dae {
+
+constexpr int kImpWarps = 4;
+constexpr int kImpChunk = 256;
+
+// sigma(x) with the approximate divide (2 ulp, no slow-path subroutine: the pair loop keeps its state in registers)
+__device__ __forceinline__ float imp_sigmoid(float x) { return __fdividef(1.0f, 1.0f + expf(-x)); }
+
+// 1 / x for an integer-valued x in [1, 2^62]: the fp32 approximation refined by two Newton steps to fp64 accuracy, inline
+__device__ __forceinline__ double imp_recip(double x) {
+  double r = (double)__fdividef(1.0f, (float)x);
+  r = r * (2.0 - x * r);
+  return r * (2.0 - x * r);
+}
+
+__device__ __forceinline__ float warp_dot(const float* __restrict__ a, const float* __restrict__ b, int H, int lane) {
+  float s = 0.0f;
+#pragma unroll 1   // unrolled, the loss kernel's nested loops spill to local memory
+  for (int j = lane; j < H; j += 32) s = fmaf(a[j], b[j], s);
+  return warp_sum(s);
+}
+
+__device__ __forceinline__ int warp_sum_int(int v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+
+__device__ __forceinline__ long long warp_sum_ll(long long v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+
+// Clicked count of one impression's flags [0, m).
+__device__ __forceinline__ int count_clicked(const uint8_t* __restrict__ c, int64_t m, int lane) {
+  int n = 0;
+  for (int64_t k = lane; k < m; k += 32) n += c[k] != 0;
+  return warp_sum_int(n);
+}
+
+// Scores h . e(items[k]) of candidates [k0, k0 + n) into s[0, n) and their click flags into f[0, n) (shared, one warp).
+__device__ __forceinline__ void score_chunk(const float* __restrict__ h, const float* __restrict__ emb, int64_t ld_emb, int H,
+                                            const int32_t* __restrict__ items, const uint8_t* __restrict__ clicked, int64_t k0, int n,
+                                            float* s, uint8_t* f, int lane) {
+  for (int t = 0; t < n; ++t) {
+    const float v = warp_dot(h, emb + (int64_t)items[k0 + t] * ld_emb, H, lane);
+    if (lane == 0) s[t] = v;
+  }
+  for (int t = lane; t < n; t += 32) f[t] = clicked[k0 + t] != 0;
+  __syncwarp();
+}
+
+// One warp per packed position p: dh_p = sum over the impressions q in [pos_indptr[p], pos_indptr[p + 1]) (in that order) of
+// scale / (|C_q| |N_q|) sum_j w_j e_j with w_n = sum_c s(s_n - s_c), w_c = -sum_n s(s_n - s_c); *loss_sum += the impressions'
+// 1 / (|C| |N|) sum_{c, n} softplus(s_n - s_c).  Impressions without a click or without a non-click add nothing; a position
+// without impressions gets dh_p = 0.  The warp owns row p of dh: no atomics, the result does not depend on the schedule.
+// Candidates are taken kImpChunk at a time (chunk A, whose weights are summed in shared memory) against every chunk B of the
+// same impression, whose scores are recomputed when the impression has more than one chunk.
+__global__ void __launch_bounds__(kImpWarps * 32) impression_rank_loss_kernel(
+    const float* __restrict__ h, int64_t ld_h, const float* __restrict__ emb, int64_t ld_emb, int H, const int64_t* __restrict__ pos_indptr,
+    int64_t n_pos, const int64_t* __restrict__ imp_indptr, const int32_t* __restrict__ items, const uint8_t* __restrict__ clicked,
+    float scale, float* __restrict__ dh, int64_t ld_dh, double* __restrict__ loss_sum) {
+  __shared__ float s_a[kImpWarps][kImpChunk], s_b[kImpWarps][kImpChunk], s_w[kImpWarps][kImpChunk];
+  __shared__ uint8_t f_a[kImpWarps][kImpChunk], f_b[kImpWarps][kImpChunk];
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  double acc = 0.0;
+  for (int64_t p = (int64_t)blockIdx.x * kImpWarps + w; p < n_pos; p += (int64_t)gridDim.x * kImpWarps) {
+    float* d = dh + p * ld_dh;
+    for (int j = lane; j < H; j += 32) d[j] = 0.0f;
+    const float* hp = h + p * ld_h;
+    for (int64_t q = pos_indptr[p]; q < pos_indptr[p + 1]; ++q) {
+      const int64_t b0 = imp_indptr[q], m = imp_indptr[q + 1] - b0;
+      const int nc = count_clicked(clicked + b0, m, lane);
+      const int64_t nn = m - nc;
+      if (nc == 0 || nn == 0) continue;
+      const double inv = imp_recip((double)nc * (double)nn);
+      const float coef = (float)((double)scale * inv);
+      double l_imp = 0.0;
+      for (int64_t a0 = 0; a0 < m; a0 += kImpChunk) {
+        const int na = (int)min((int64_t)kImpChunk, m - a0);
+        score_chunk(hp, emb, ld_emb, H, items + b0, clicked + b0, a0, na, s_a[w], f_a[w], lane);
+        for (int t = lane; t < na; t += 32) s_w[w][t] = 0.0f;
+        for (int64_t c0 = 0; c0 < m; c0 += kImpChunk) {
+          const int nb = (int)min((int64_t)kImpChunk, m - c0);
+          const float* sb = s_a[w];
+          const uint8_t* fb = f_a[w];
+          if (c0 != a0) {
+            score_chunk(hp, emb, ld_emb, H, items + b0, clicked + b0, c0, nb, s_b[w], f_b[w], lane);
+            sb = s_b[w];
+            fb = f_b[w];
+          }
+          for (int t = lane; t < na; t += 32) {
+            const float sj = s_a[w][t];
+            const uint8_t cj = f_a[w][t];
+            float wj = s_w[w][t], lj = 0.0f;
+            for (int k = 0; k < nb; ++k) {
+              if (fb[k] == cj) continue;
+              if (cj) {   // j clicked, k not: x = s_k - s_j
+                const float x = sb[k] - sj;
+                wj -= imp_sigmoid(x);
+                lj += fmaxf(x, 0.0f) + log1pf(expf(-fabsf(x)));
+              } else {    // j not clicked, k clicked: x = s_j - s_k
+                wj += imp_sigmoid(sj - sb[k]);
+              }
+            }
+            s_w[w][t] = wj;
+            l_imp += (double)lj;
+          }
+          __syncwarp();
+        }
+        for (int t = 0; t < na; ++t) {
+          const float g = coef * s_w[w][t];
+          const float* e = emb + (int64_t)items[b0 + a0 + t] * ld_emb;
+#pragma unroll 1
+          for (int j = lane; j < H; j += 32) d[j] = fmaf(g, e[j], d[j]);
+        }
+        __syncwarp();
+      }
+      acc += l_imp * inv;
+    }
+  }
+  acc = warp_sum(acc);
+  if (lane == 0 && acc != 0.0) atomicAdd(loss_sum, acc);
+}
+
+// One warp per impression i: scores[k] = q_i . e(items[k]) (cosine: divided by |q_i| |e|, 0 when either is zero) for every k in
+// [indptr[i], indptr[i + 1]), then metrics[i] = (AUC, MRR, nDCG@5, nDCG@10) from those fp32 scores.  rank_j = #{k: s_k > s_j}
+// + #{k < j: s_k = s_j}.  The clicked candidates are taken 32 at a time, one per lane, against the whole list staged kImpChunk
+// scores at a time in shared memory: O(|C| m) comparisons, the AUC counted in integers.  No click or no non-click: NaN x 4.
+__global__ void __launch_bounds__(kImpWarps * 32) impression_metrics_kernel(
+    const float* __restrict__ qv, int64_t ld_q, const float* __restrict__ emb, int64_t ld_emb, int H, int cosine,
+    const int64_t* __restrict__ indptr, const int32_t* __restrict__ items, const uint8_t* __restrict__ clicked, int64_t n_imp,
+    float* scores, double* __restrict__ metrics) {
+  __shared__ float s_s[kImpWarps][kImpChunk];
+  __shared__ uint8_t s_f[kImpWarps][kImpChunk];
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  for (int64_t i = (int64_t)blockIdx.x * kImpWarps + w; i < n_imp; i += (int64_t)gridDim.x * kImpWarps) {
+    const int64_t b0 = indptr[i], m = indptr[i + 1] - b0;
+    const float* q = qv + i * ld_q;
+    float qn = 0.0f;
+    if (cosine) qn = sqrtf(warp_dot(q, q, H, lane));
+    for (int64_t k = 0; k < m; ++k) {
+      const float* e = emb + (int64_t)items[b0 + k] * ld_emb;
+      float dot = 0.0f, ee = 0.0f;
+      for (int j = lane; j < H; j += 32) {
+        const float x = e[j];
+        dot = fmaf(q[j], x, dot);
+        ee = fmaf(x, x, ee);
+      }
+      dot = warp_sum(dot);
+      float s = dot;
+      if (cosine) {
+        ee = warp_sum(ee);
+        s = (qn > 0.0f && ee > 0.0f) ? dot / (qn * sqrtf(ee)) : 0.0f;
+      }
+      if (lane == 0) scores[b0 + k] = s;
+    }
+    __syncwarp();   // the scores written by lane 0 are read by every lane below
+    const int nc = count_clicked(clicked + b0, m, lane);
+    const int64_t nn = m - nc;
+    double* out = metrics + i * 4;
+    if (nc == 0 || nn == 0) {
+      if (lane < 4) out[lane] = __longlong_as_double(0x7ff8000000000000LL);
+      continue;
+    }
+    long long auc2 = 0;
+    double rr = 0.0, g5 = 0.0, g10 = 0.0;
+    for (int64_t j0 = 0; j0 < m; j0 += 32) {
+      const int64_t j = j0 + lane;
+      const bool mine = j < m && clicked[b0 + j] != 0;
+      if (!__any_sync(0xffffffffu, mine)) continue;
+      const float sj = mine ? scores[b0 + j] : 0.0f;
+      long long gt = 0, tie_before = 0, below_n = 0, tie_n = 0;
+      for (int64_t k0 = 0; k0 < m; k0 += kImpChunk) {
+        const int nk = (int)min((int64_t)kImpChunk, m - k0);
+        __syncwarp();
+        for (int t = lane; t < nk; t += 32) {
+          s_s[w][t] = scores[b0 + k0 + t];
+          s_f[w][t] = clicked[b0 + k0 + t] != 0;
+        }
+        __syncwarp();
+        if (mine) {
+          for (int t = 0; t < nk; ++t) {
+            const float sk = s_s[w][t];
+            gt += sk > sj;
+            tie_before += (sk == sj) && (k0 + t < j);
+            if (!s_f[w][t]) {
+              below_n += sk < sj;
+              tie_n += sk == sj;
+            }
+          }
+        }
+      }
+      if (mine) {
+        const long long rank = gt + tie_before;
+        auc2 += 2 * below_n + tie_n;
+        rr += 1.0 / (double)(rank + 1);
+        if (rank < 10) {
+          const double g = 1.0 / log2((double)(rank + 2));
+          g10 += g;
+          if (rank < 5) g5 += g;
+        }
+      }
+    }
+    auc2 = warp_sum_ll(auc2);
+    rr = warp_sum(rr);
+    g5 = warp_sum(g5);
+    g10 = warp_sum(g10);
+    if (lane == 0) {
+      double i5 = 0.0, i10 = 0.0;
+      for (int r = 0; r < 10 && r < nc; ++r) {
+        const double g = 1.0 / log2((double)(r + 2));
+        i10 += g;
+        if (r < 5) i5 += g;
+      }
+      out[0] = (double)auc2 / (2.0 * (double)nc * (double)nn);
+      out[1] = rr / (double)nc;
+      out[2] = g5 / i5;
+      out[3] = g10 / i10;
+    }
+  }
+}
+
+static int imp_grid(int64_t rows) {
+  const int64_t b = (rows + kImpWarps - 1) / kImpWarps, cap = (int64_t)sm_count() * 16;
+  return (int)(b < 1 ? 1 : (b < cap ? b : cap));
+}
+
+}  // namespace dae
+
+using namespace dae;
+
+extern "C" int dae_impression_rank_loss(const float* h, int64_t ld_h, const float* emb, int64_t ld_emb, int32_t H, const int64_t* pos_indptr,
+                                        int64_t n_pos, const int64_t* imp_indptr, const int32_t* items, const uint8_t* clicked, float scale,
+                                        float* dh, int64_t ld_dh, double* loss_sum, void* stream) {
+  DAE_REQUIRE(h && emb && pos_indptr && imp_indptr && items && clicked && dh && loss_sum && H > 0 && n_pos > 0 && ld_h >= H &&
+              ld_emb >= H && ld_dh >= H, "dae_impression_rank_loss: bad arguments");
+  impression_rank_loss_kernel<<<imp_grid(n_pos), kImpWarps * 32, 0, (cudaStream_t)stream>>>(
+      h, ld_h, emb, ld_emb, H, pos_indptr, n_pos, imp_indptr, items, clicked, scale, dh, ld_dh, loss_sum);
+  DAE_CHECK_LAUNCH("dae_impression_rank_loss");
+  return DAE_OK;
+}
+
+extern "C" int dae_impression_metrics(const float* q, int64_t ld_q, const float* emb, int64_t ld_emb, int32_t H, int32_t cosine,
+                                      const int64_t* indptr, const int32_t* items, const uint8_t* clicked, int64_t n_imp, float* scores,
+                                      double* metrics, void* stream) {
+  DAE_REQUIRE(q && emb && indptr && items && clicked && scores && metrics && H > 0 && n_imp > 0 && ld_q >= H && ld_emb >= H &&
+              (cosine == 0 || cosine == 1), "dae_impression_metrics: bad arguments");
+  impression_metrics_kernel<<<imp_grid(n_imp), kImpWarps * 32, 0, (cudaStream_t)stream>>>(
+      q, ld_q, emb, ld_emb, H, cosine, indptr, items, clicked, n_imp, scores, metrics);
+  DAE_CHECK_LAUNCH("dae_impression_metrics");
+  return DAE_OK;
+}

@@ -17,6 +17,8 @@ nearest-article lookup of main_autoencoder.py:307-318,352-359) -- SURVEY section
                                                                                                         one article per story)
     sequences_from_csr(m) -> (indptr[U + 1], items)                                                   (reads ordered by stored time)
     recommendation_recall(index, targets) -> dict                                                     (hit rate / recall of held-out reads)
+    impression_metrics(vectors, embeddings, impressions, metric='linear kernel') -> dict              (AUC / MRR / nDCG@5, @10 per
+                                                                                                        impression, averaged)
     similar_pairs(data, threshold, corpus=None, metric='cosine') -> (i[P], j[P], score[P])            (every pair with score >= threshold,
                                                                                                         near-duplicates; no matrix)
     duplicate_groups(i, j, n) -> group[n]                                                             (connected components of the pairs)
@@ -529,6 +531,53 @@ def recommendation_recall(index, targets):
     pos = np.minimum(np.searchsorted(t_keys, keys), t_keys.size - 1)
     hits = ((index >= 0) & (t_keys[pos] == keys)).sum(1)
     return {'users': users, 'hit_rate': float((hits[use] > 0).mean()), 'recall': float((hits[use] / n_t[use]).mean())}
+
+
+def _impression_scores(q, emb, imp, metric):
+    """dae_impression_metrics on device tensors: (scores fp32 [nnz], metrics fp64 [I, 4] = AUC, MRR, nDCG@5, nDCG@10) as device
+    tensors.  imp: check_impressions' host arrays."""
+    n_imp, d = q.shape[0], emb.device
+    scores = torch.empty(imp['items'].size, dtype=torch.float32, device=d)
+    metrics = torch.full((n_imp, 4), float('nan'), dtype=torch.float64, device=d)
+    if n_imp == 0 or imp['items'].size == 0:
+        return scores, metrics
+    indptr = torch.from_numpy(imp['indptr']).to(d)
+    items = torch.from_numpy(imp['items']).to(d)
+    clicked = torch.from_numpy(imp['clicked']).to(d)
+    call('dae_impression_metrics', q.data_ptr(), q.stride(0), emb.data_ptr(), emb.stride(0), emb.shape[1], int(metric == 'cosine'),
+         indptr.data_ptr(), items.data_ptr(), clicked.data_ptr(), n_imp, scores.data_ptr(), metrics.data_ptr(), _stream())
+    return scores, metrics
+
+
+def impression_metrics(vectors, embeddings, impressions, metric='linear kernel', device='cuda:0'):
+    """Ranking quality on impression logs: for impression i the shown articles are scored against vectors[i] ('linear kernel':
+    the inner product, 'cosine': with a zero vector scoring 0) and ranked by score, descending, ties to the earlier position in
+    the impression's list.  Per impression: AUC of the clicks against the non-clicks (ties count one half; sklearn's
+    roc_auc_score), MRR (the mean of 1 / (rank + 1) over the clicks, as MIND's mrr_score) and nDCG@5 / nDCG@10 with binary gains
+    (MIND's ndcg_score).  MIND's scripts leave the order of tied scores to argsort; the tie rule above is the only place where
+    the ranks may differ from theirs.  The scores and the metrics come from dae_impression_metrics, one warp per impression.
+    vectors: [I, H] query vectors (UserGRU.impression_states, or user_profiles of user_model.prefix_histories); embeddings:
+    [N, H]; impressions: a mapping with 'indptr', 'items', 'clicked' (user_model.check_impressions).
+    Returns {'impressions': impressions scored, 'skipped': impressions without a click or without a non-click (left out of the
+    means), 'auc', 'mrr', 'ndcg@5', 'ndcg@10': means over the scored ones (NaN when none)}."""
+    from .user_model import check_impressions
+    if metric not in ('cosine', 'linear kernel'):
+        raise ValueError("impression_metrics: metric = %r: 'cosine' or 'linear kernel'" % (metric,))
+    emb = _dense_embeddings(embeddings, device, 'impression_metrics')
+    imp = check_impressions(impressions, emb.shape[0], 'impression_metrics')
+    n_imp = imp['indptr'].size - 1
+    if sp.issparse(vectors) or tuple(vectors.shape) != (n_imp, emb.shape[1]):
+        raise ValueError('impression_metrics: vectors have shape %s, [%d, %d] (impressions x embedding width) expected'
+                         % (tuple(vectors.shape), n_imp, emb.shape[1]))
+    q = _as_device_dense(vectors, emb.device)
+    if not bool(torch.isfinite(emb).all()) or not bool(torch.isfinite(q).all()):
+        raise ValueError('impression_metrics: embeddings and vectors must be finite')
+    _, m = _impression_scores(q, emb, imp, metric)
+    m = m.cpu().numpy()
+    ok = ~np.isnan(m[:, 0])
+    mean = m[ok].mean(0) if ok.any() else np.full(4, np.nan)
+    return {'impressions': int(ok.sum()), 'skipped': int(n_imp - ok.sum()), 'auc': float(mean[0]), 'mrr': float(mean[1]),
+            'ndcg@5': float(mean[2]), 'ndcg@10': float(mean[3])}
 
 
 def label_precision_at_k(index, query_labels, corpus_labels):

@@ -150,6 +150,87 @@ def make_sequences(n_users, labels, mean_len=20, session_len=5, seed=0, max_len=
     return indptr, items, targets
 
 
+def make_impressions(indptr, items, labels, targets=None, shown=20, seed=0, tries=20):
+    """Synthetic impression logs for make_sequences' users (user_model.check_impressions' keys).  Returns (train, test):
+    train has one impression per user and time t = 1 .. len - 1 that clicks read t + 1; test (with targets) has one per user
+    with a target, at time = len, that clicks the target.  Each shows the click and shown - 1 distinct other articles in a
+    random order: (shown - 1) // 2 from the classes of the user's reads before the impression other than the click's class (a
+    class drawn through a random earlier read; from the whole catalogue when there is none within `tries` draws) and the rest
+    from the whole catalogue.  Every distractor is a random read of all users' reads in its class, so articles are shown as
+    often as they are read (make_sequences' Zipf popularity) and popularity does not give the click away.  A distractor that
+    repeats the click or another distractor is redrawn up to `tries` times and dropped after that."""
+    rng = np.random.default_rng(seed)
+    indptr, items = np.asarray(indptr, np.int64), np.asarray(items, np.int64)
+    labels = np.asarray(labels).reshape(-1)
+    cls_of = labels[items].astype(np.int64)
+    pool = items[np.argsort(cls_of, kind='stable')]
+    classes = np.sort(cls_of)
+    ids = np.arange(int(classes.max(initial=0)) + 1)
+    c_lo, c_hi = np.searchsorted(classes, ids, 'left'), np.searchsorted(classes, ids, 'right')   # class c's reads: pool[c_lo:c_hi]
+    lens = np.diff(indptr)
+    k_user = (shown - 1) // 2
+
+    def impressions(user, time, click):
+        n = user.size
+        # the class of each user-side distractor: a random earlier read's class other than the click's
+        src_cls = np.full((n, k_user), -1, np.int64)
+        todo = np.ones((n, k_user), bool)
+        for _ in range(tries):
+            r, c = np.nonzero(todo)
+            if r.size == 0:
+                break
+            pick = indptr[user[r]] + (rng.random(r.size) * time[r]).astype(np.int64)
+            cl = cls_of[pick]
+            ok = cl != labels[click[r]]
+            src_cls[r[ok], c[ok]] = cl[ok]
+            todo[r[ok], c[ok]] = False
+
+        def draw(cl):   # a random read of class cl (a random read of all when cl < 0)
+            glob = cl < 0
+            lo = np.where(glob, 0, c_lo[np.maximum(cl, 0)])
+            hi = np.where(glob, pool.size, c_hi[np.maximum(cl, 0)])
+            return pool[lo + (rng.random(cl.size) * (hi - lo)).astype(np.int64)]
+
+        cls = np.concatenate([src_cls, np.full((n, shown - 1 - k_user), -1, np.int64)], 1).reshape(-1)
+        dis = draw(cls).reshape(n, shown - 1)
+        for _ in range(tries + 1):
+            full = np.concatenate([click[:, None], dis], 1)
+            o = np.argsort(full, axis=1, kind='stable')
+            srt = np.take_along_axis(full, o, 1)
+            dup = np.zeros_like(full, dtype=bool)
+            rep = np.zeros_like(srt, dtype=bool)
+            rep[:, 1:] = srt[:, 1:] == srt[:, :-1]
+            np.put_along_axis(dup, o, rep, 1)   # the stable sort keeps the click (column 0) first among equal articles
+            bad = dup[:, 1:]
+            if not bad.any():
+                break
+            r, c = np.nonzero(bad)
+            if _ < tries:
+                dis[r, c] = draw(cls.reshape(n, -1)[r, c])
+        keep = ~bad
+        m = 1 + keep.sum(1)
+        ind = np.concatenate([[0], np.cumsum(m)]).astype(np.int64)
+        rows = np.concatenate([click[:, None], dis], 1)[np.concatenate([np.ones((n, 1), bool), keep], 1)]
+        clicked = np.zeros(rows.size, np.uint8)
+        clicked[ind[:-1]] = 1
+        # a random order within each impression
+        key = np.repeat(np.arange(n), m) + rng.random(rows.size)
+        o = np.argsort(key, kind='stable')
+        return {'user': user.astype(np.int64), 'time': time.astype(np.int64), 'indptr': ind, 'items': rows[o].astype(np.int32),
+                'clicked': clicked[o]}
+
+    n_u = lens.size
+    t_user = np.repeat(np.arange(n_u), np.maximum(lens - 1, 0))
+    t_time = np.arange(t_user.size) - np.repeat(np.cumsum(np.maximum(lens - 1, 0)) - np.maximum(lens - 1, 0), np.maximum(lens - 1, 0)) + 1
+    train = impressions(t_user, t_time, items[indptr[t_user] + t_time])
+    test = None
+    if targets is not None:
+        targets = np.asarray(targets, np.int64)
+        u = np.flatnonzero((targets >= 0) & (lens > 0))
+        test = impressions(u, lens[u], targets[u])
+    return train, test
+
+
 def make_labels(n_rows, n_classes=4, seed=0):
     return np.random.default_rng(seed + 7919).integers(0, n_classes, n_rows).astype(np.float32)
 

@@ -20,6 +20,10 @@ Device path per training batch (users ordered by length, descending, so the user
   per step in reverse dae_gru_cell_bwd and the carry GEMM dh_{t-1} += dHP_t . W_hh;
   [dW_hh | db_hh] = dHP^T.[h_prev | 1] and [dW_ih | db_ih] = dXP^T.[X | 1] over all positions; dae_optimizer_step.
 Parameters: one flat fp32 buffer theta = [W~_hh (3H x (H+1)) | W~_ih (3H x (H+1))] with W~ = [W | b].
+
+Impression logs (DESIGN 4.13): fit(..., impressions=...) trains on the shown-but-not-clicked articles of each impression
+(dae_impression_rank_loss in place of the two random-negative kernels), impression_states gives the query vector before each
+impression and prefix_histories the reads before it for the mean-profile baseline.
 """
 import numpy as np
 import torch
@@ -61,6 +65,105 @@ def check_sequences(sequences, n_items, fn):
     if items.size and (items.min() < 0 or items.max() >= n_items):
         raise ValueError('%s: items hold an article outside [0, %d)' % (fn, n_items))
     return indptr.astype(np.int64), items.astype(np.int32)
+
+
+IMPRESSION_KEYS = ('user', 'time', 'indptr', 'items', 'clicked')
+
+
+def check_impressions(impressions, n_items, fn, seq_indptr=None):
+    """An impression set as a dict of fresh arrays {'user' int64 [I], 'time' int64 [I], 'indptr' int64 [I + 1], 'items' int32,
+    'clicked' uint8}, or ValueError before any device work.  impressions: a mapping with those keys (a dict, or np.load of the CLI's
+    .npz).  indptr must start at 0, never decrease and end at len(items); items lie in [0, n_items) and are distinct within one
+    impression; clicked has one 0 / 1 flag per shown article.  With seq_indptr (the sequences' offsets) user must be a row of the
+    sequences and 0 <= time <= that user's read count; without it user and time are not read.  The caller's arrays are not
+    modified."""
+    try:
+        got = {k: np.asarray(impressions[k]) for k in IMPRESSION_KEYS if seq_indptr is not None or k in ('indptr', 'items', 'clicked')}
+    except (KeyError, TypeError, IndexError, ValueError):
+        raise ValueError('%s: impressions must map %s to arrays' % (fn, ', '.join(IMPRESSION_KEYS)))
+    indptr, items, clicked = got['indptr'], got['items'], got['clicked']
+    if indptr.ndim != 1 or indptr.size < 1 or not np.issubdtype(indptr.dtype, np.integer):
+        raise ValueError('%s: impressions indptr must be a 1-D integer array of I + 1 offsets' % fn)
+    if items.ndim != 1 or not (np.issubdtype(items.dtype, np.integer) or items.size == 0):
+        raise ValueError('%s: impressions items must be a 1-D integer array' % fn)
+    if indptr[0] != 0 or indptr[-1] != items.size or (np.diff(indptr) < 0).any():
+        raise ValueError('%s: impressions indptr must start at 0, never decrease and end at len(items) = %d' % (fn, items.size))
+    if clicked.shape != items.shape or not (clicked.dtype == np.bool_ or np.issubdtype(clicked.dtype, np.integer)) or \
+            (clicked.size and not np.isin(clicked, (0, 1)).all()):
+        raise ValueError('%s: clicked must hold one 0 / 1 flag per shown article (%d)' % (fn, items.size))
+    if items.size and (items.min() < 0 or items.max() >= n_items):
+        raise ValueError('%s: impressions show an article outside [0, %d)' % (fn, n_items))
+    n_imp = indptr.size - 1
+    row = np.repeat(np.arange(n_imp, dtype=np.int64), np.diff(indptr))
+    key = row * max(int(n_items), 1) + items.astype(np.int64)
+    if key.size > 1 and (np.diff(np.sort(key)) == 0).any():
+        raise ValueError('%s: an impression shows the same article twice' % fn)
+    out = {'indptr': indptr.astype(np.int64), 'items': items.astype(np.int32), 'clicked': clicked.astype(np.uint8)}
+    if seq_indptr is not None:
+        user, time = got['user'], got['time']
+        for k, v in (('user', user), ('time', time)):
+            if v.shape != (n_imp,) or not (np.issubdtype(v.dtype, np.integer) or v.size == 0):
+                raise ValueError('%s: impressions %s must be an integer array of one entry per impression (%d)' % (fn, k, n_imp))
+        n_u = len(seq_indptr) - 1
+        if user.size and (user.min() < 0 or user.max() >= n_u):
+            raise ValueError('%s: impressions user outside [0, %d)' % (fn, n_u))
+        lens = np.diff(seq_indptr)
+        if time.size and ((time < 0).any() or (time > lens[user]).any()):
+            raise ValueError("%s: impressions time must lie in [0, the user's read count]" % fn)
+        out['user'], out['time'] = user.astype(np.int64), time.astype(np.int64)
+    return out
+
+
+def usable_impressions(imp, seq_indptr, max_len):
+    """Boolean [I]: the impressions the impression loss uses -- at least one click and one non-click, and a state inside the
+    user's trained window of the last max_len reads (time > len - min(len, max_len), so never time = 0)."""
+    lens = np.diff(seq_indptr)[imp['user']]
+    L = np.minimum(lens, max_len)
+    n = np.diff(imp['indptr'])
+    cs = np.concatenate([[0], np.cumsum(imp['clicked'], dtype=np.int64)])
+    nc = cs[imp['indptr'][1:]] - cs[imp['indptr'][:-1]]
+    return (nc > 0) & (nc < n) & (imp['time'] > lens - L) & (imp['time'] >= 1)
+
+
+class ImpressionBatch:
+    """The impressions of one packed training batch (pk: Packed), grouped by packed position.  An impression of user order[i] at
+    time t has its state at position off[t'] + i with t' = t - 1 - (len - L).  pos_indptr [P + 1]: position p's impressions are
+    [pos_indptr[p], pos_indptr[p + 1]) of this batch's own (indptr, items, clicked), in increasing impression id.  ids: the
+    impression ids in that order.  `buffer` packs the four arrays into one byte buffer for a single upload; `views` cuts the
+    uploaded copy back into typed device tensors."""
+
+    def __init__(self, pk, imp, use, seq_indptr):
+        slot = np.full(int(seq_indptr.size - 1), -1, np.int64)
+        slot[pk.order] = np.arange(pk.B)
+        ids = np.flatnonzero(use & (slot[imp['user']] >= 0))
+        u = imp['user'][ids]
+        i = slot[u]
+        lens = seq_indptr[u + 1] - seq_indptr[u]
+        t = imp['time'][ids] - 1 - (lens - pk.L[i])
+        p = pk.off[t] + i
+        o = np.argsort(p, kind='stable')
+        self.ids, self.p = ids[o], p[o]
+        self.n = int(self.ids.size)
+        self.pos_indptr = np.zeros(pk.P + 1, np.int64)
+        np.cumsum(np.bincount(self.p, minlength=pk.P), out=self.pos_indptr[1:])
+        lo, hi = imp['indptr'][self.ids], imp['indptr'][self.ids + 1]
+        m = hi - lo
+        self.indptr = np.concatenate([[0], np.cumsum(m)]).astype(np.int64)
+        src = np.repeat(lo - self.indptr[:-1], m) + np.arange(int(self.indptr[-1]))
+        self.items, self.clicked = imp['items'][src], imp['clicked'][src]
+
+    def buffer(self):
+        parts = [self.pos_indptr.view(np.uint8), self.indptr.view(np.uint8), self.items.view(np.uint8), self.clicked]
+        self._sizes = [a.size for a in parts]
+        pad = [(-s) % 8 for s in self._sizes]
+        return np.concatenate([np.concatenate([a, np.zeros(q, np.uint8)]) for a, q in zip(parts, pad)])
+
+    def views(self, dev):
+        out, o = [], 0
+        for s, dt in zip(self._sizes, (torch.int64, torch.int64, torch.int32, torch.uint8)):
+            out.append(dev[o:o + s].view(dt))
+            o += s + (-s) % 8
+        return out
 
 
 class Packed:
@@ -226,17 +329,23 @@ class UserGRU:
         return b
 
     # ---- training ---------------------------------------------------------------------------------------------------------
-    def _forward_backward(self, pk, emb, epoch, batch):
-        """Loss (added to self.stats) and the gradient (self.grad) of one packed batch with pk.terms > 0."""
+    def _forward_backward(self, pk, emb, epoch, batch, ib=None):
+        """Loss (added to self.stats) and the gradient (self.grad) of one packed batch with pk.terms > 0, or with ib (an
+        ImpressionBatch with ib.n > 0) the impression loss of its impressions in place of the random negatives."""
         H, P, T = self.dim, pk.P, len(pk.n)
         b = self._buffers(P, pk.B)
         st = _stream()
-        items, nxt = _upload(pk.items, self.device), _upload(pk.nxt, self.device)
+        items = _upload(pk.items, self.device)
+        if ib is None:
+            nxt = _upload(pk.nxt, self.device)
+        else:
+            pos_indptr, imp_indptr, imp_items, imp_clicked = ib.views(_upload(ib.buffer(), self.device))
         if not self._hh_valid:
             self._split('hh')
             self._hh_valid = True
         self._mark('start')
-        call('dae_seq_negatives', nxt.data_ptr(), P, emb.shape[0], self.seed, epoch, batch, b['neg'].data_ptr(), st)
+        if ib is None:
+            call('dae_seq_negatives', nxt.data_ptr(), P, emb.shape[0], self.seed, epoch, batch, b['neg'].data_ptr(), st)
         X_hi, X_lo = b['X_hl']
         call('dae_gather_split_bf16', emb.data_ptr(), emb.stride(0), items.data_ptr(), P, H, X_hi.data_ptr(), X_lo.data_ptr(), self.ldx,
              H, st)
@@ -258,8 +367,13 @@ class UserGRU:
                  Hp_hi[nx:].data_ptr() if n_next else None, Hp_lo[nx:].data_ptr() if n_next else None, self.ldx, G[o:].data_ptr(),
                  4 * H, st)
         self._mark('forward_recurrence')
-        call('dae_seq_rank_loss', Hs.data_ptr(), H, emb.data_ptr(), emb.stride(0), H, nxt.data_ptr(), b['neg'].data_ptr(), P,
-             1.0 / pk.terms, b['dH'].data_ptr(), H, self.stats.data_ptr(), st)
+        if ib is None:
+            call('dae_seq_rank_loss', Hs.data_ptr(), H, emb.data_ptr(), emb.stride(0), H, nxt.data_ptr(), b['neg'].data_ptr(), P,
+                 1.0 / pk.terms, b['dH'].data_ptr(), H, self.stats.data_ptr(), st)
+        else:
+            call('dae_impression_rank_loss', Hs.data_ptr(), H, emb.data_ptr(), emb.stride(0), H, pos_indptr.data_ptr(), P,
+                 imp_indptr.data_ptr(), imp_items.data_ptr(), imp_clicked.data_ptr(), 1.0 / ib.n, b['dH'].data_ptr(), H,
+                 self.stats.data_ptr(), st)
         self._mark('loss')
         carry, dH = b['carry'], b['dH']
         carry[:n0].zero_()
@@ -286,28 +400,49 @@ class UserGRU:
         self._hh_valid = True
         self._mark('optimizer')
 
-    def batches(self, indptr, epoch):
+    def batches(self, indptr, epoch, active=None):
         """The epoch's batches of user ids: a permutation (seeded by seed and epoch) of the users with at least 2 reads -- the
-        others have no loss term -- cut into batch_users."""
-        active = np.flatnonzero(np.diff(indptr) >= 2)
+        others have no loss term -- cut into batch_users.  active: the user ids to permute instead (sorted)."""
+        if active is None:
+            active = np.flatnonzero(np.diff(indptr) >= 2)
         perm = active[np.random.default_rng([self.seed, epoch]).permutation(active.size)]
         return [perm[i:i + self.batch_users] for i in range(0, perm.size, self.batch_users)]
 
-    def fit(self, sequences, embeddings):
-        """num_epochs epochs over the users; train_loss gets each epoch's mean loss term.  The article embeddings stay fixed."""
+    def fit(self, sequences, embeddings, impressions=None):
+        """num_epochs epochs over the users; train_loss gets each epoch's mean loss term.  The article embeddings stay fixed.
+
+        impressions (check_impressions' keys): train on them instead of random negatives.  Impression i of user u at time t
+        scores its shown articles with h, the packed training state after u's first t reads, and its loss is
+        1 / (|C| |N|) sum_{c clicked, n not} softplus(h.e_n - h.e_c); a batch's loss is the mean over its impressions.  An
+        impression counts when it has a click and a non-click and its state lies in the trained window of the user's last
+        max_len reads (time > len - min(len, max_len)); impression_counts gets {'used', 'skipped'}.  The batches permute the
+        users with a usable impression as batches() does; one impression with one click at time t on read t + 1 and one
+        non-click is exactly the random-negative term at position t."""
         emb = self._embeddings(embeddings, 'UserGRU.fit')
         indptr, items = check_sequences(sequences, emb.shape[0], 'UserGRU.fit')
+        imp = active = use = None
+        if impressions is not None:
+            imp = check_impressions(impressions, emb.shape[0], 'UserGRU.fit', indptr)
+            use = usable_impressions(imp, indptr, self.max_len)
+            active = np.unique(imp['user'][use])
+            self.impression_counts = {'used': int(use.sum()), 'skipped': int(use.size - use.sum())}
         for _ in range(self.num_epochs):
             epoch = self.epochs_done
             self.stats.zero_()
             terms = 0
-            for bi, users in enumerate(self.batches(indptr, epoch)):
+            for bi, users in enumerate(self.batches(indptr, epoch, active)):
                 pk = Packed(indptr, items, users, self.max_len)
-                if pk.terms == 0:   # max_len = 1
+                ib = None
+                if imp is not None:
+                    ib = ImpressionBatch(pk, imp, use, indptr)
+                    n = ib.n
+                else:
+                    n = pk.terms
+                if n == 0:   # max_len = 1
                     continue
-                self._forward_backward(pk, emb, epoch, bi)
+                self._forward_backward(pk, emb, epoch, bi, ib)
                 self._optimizer_step()
-                terms += pk.terms
+                terms += n
             self.train_loss.append(float(self.stats.item()) / max(terms, 1))
             self.epochs_done += 1
         return self
@@ -350,6 +485,79 @@ class UserGRU:
             out.index_copy_(0, torch.from_numpy(pk.order).to(d), h[:pk.B])
         return out.cpu().numpy() if to_host else out
 
+    def impression_states(self, sequences, embeddings, impressions, to_host=True):
+        """Query vectors [I, H] fp32 for impressions (check_impressions' keys): row i is the state after the last min(time, max_len)
+        reads of its user before the impression, a zero row at time = 0.  At time = len this is transform's row.
+
+        Training (fit(impressions=...)) takes the state from the packed window of the user's LAST max_len reads, which starts at
+        read len - max_len whatever the impression's time; here the window ENDS at the impression.  The two agree at time = len
+        and for users with at most max_len reads.  Each (user, window start) pair is one run of transform's step
+        loop, whose states are copied out at the steps that impressions ask for: a user whose impressions all lie within the first
+        max_len reads costs one run.  Device memory per batch is O(batch_users x 3H), as transform's."""
+        emb = self._embeddings(embeddings, 'UserGRU.impression_states')
+        indptr, items = check_sequences(sequences, emb.shape[0], 'UserGRU.impression_states')
+        imp = check_impressions(impressions, emb.shape[0], 'UserGRU.impression_states', indptr)
+        H, d, st = self.dim, self.device, _stream()
+        n_imp = imp['user'].size
+        out = torch.zeros(n_imp, H, dtype=torch.float32, device=d)
+        ids = np.flatnonzero(imp['time'] > 0)
+        if ids.size == 0:
+            return out.cpu().numpy() if to_host else out
+        u, t = imp['user'][ids], imp['time'][ids]
+        start = np.maximum(t - self.max_len, 0)
+        # runs: one per distinct (user, window start), each as long as its latest impression needs (<= max_len steps)
+        key = u * (int(indptr[-1]) + 1) + start
+        run_key, run_of = np.unique(key, return_inverse=True)
+        n_run = run_key.size
+        run_len = np.zeros(n_run, np.int64)
+        np.maximum.at(run_len, run_of, t - start)
+        first = np.zeros(n_run, np.int64)
+        first[run_of] = np.arange(ids.size)   # any impression of the run gives its user and start
+        r_src = indptr[u[first]] + start[first]
+        r_indptr = np.concatenate([[0], np.cumsum(run_len)]).astype(np.int64)
+        r_items = items[np.repeat(r_src - r_indptr[:-1], run_len) + np.arange(int(r_indptr[-1]))]
+        step = t - start - 1   # the step after which impression ids[j] reads its run's state
+        B = self.batch_users
+        if not self._hh_valid:
+            self._split('hh')
+            self._hh_valid = True
+        self._split('ih')
+        bf = dict(dtype=torch.bfloat16, device=d)
+        X_hi, X_lo = torch.zeros(B, self.ldx, **bf), torch.zeros(B, self.ldx, **bf)
+        h_hi, h_lo = torch.zeros(B, self.ldx, **bf), torch.zeros(B, self.ldx, **bf)
+        XP = torch.empty(B, 3 * H, dtype=torch.float32, device=d)
+        HP = torch.empty_like(XP)
+        h = torch.empty(B, H, dtype=torch.float32, device=d)
+        order = np.argsort(run_of, kind='stable')
+        for r0 in range(0, n_run, B):
+            pk = Packed(r_indptr, r_items, np.arange(r0, min(n_run, r0 + B)), self.max_len)
+            row = np.empty(n_run, np.int64)
+            row[pk.order] = np.arange(pk.B)
+            lo, hi = np.searchsorted(run_of[order], [r0, r0 + B])
+            sel = order[lo:hi]
+            cap_step, cap_row, cap_imp = step[sel], row[run_of[sel]], ids[sel]
+            o = np.argsort(cap_step, kind='stable')
+            cap_step, cap = cap_step[o], np.stack([cap_row[o], cap_imp[o]])
+            bounds = np.searchsorted(cap_step, np.arange(len(pk.n) + 1))
+            cap_d = _upload(np.ascontiguousarray(cap), d)
+            it = _upload(pk.items, d)
+            h_hi.zero_()
+            h_lo.zero_()
+            h_hi[:, H] = 1.0
+            h[:pk.B].zero_()
+            for tt in range(len(pk.n)):
+                o_, n = int(pk.off[tt]), int(pk.n[tt])
+                call('dae_gather_split_bf16', emb.data_ptr(), emb.stride(0), it[o_:].data_ptr(), n, H, X_hi.data_ptr(), X_lo.data_ptr(),
+                     self.ldx, H, st)
+                self._gemm(n, 3 * H, H + 1, (X_hi, X_lo), 0, self.W_hl['ih'], 0, XP, 3 * H)
+                self._gemm(n, 3 * H, H + 1, (h_hi, h_lo), 0, self.W_hl['hh'], 0, HP, 3 * H)
+                call('dae_gru_cell_fwd', n, H, XP.data_ptr(), 3 * H, HP.data_ptr(), 3 * H, h.data_ptr(), H, h.data_ptr(), H, n,
+                     h_hi.data_ptr(), h_lo.data_ptr(), self.ldx, None, 0, st)
+                a, b = int(bounds[tt]), int(bounds[tt + 1])
+                if b > a:
+                    out.index_copy_(0, cap_d[1, a:b], h.index_select(0, cap_d[0, a:b]))
+        return out.cpu().numpy() if to_host else out
+
     def recommend(self, sequences, embeddings, k=10, candidates=None, exclude_read=True, metric='linear kernel', to_host=True,
                   groups=None):
         """The k best articles per user for the GRU user vectors (helpers.recommend with profiles=transform(...)): every read
@@ -372,6 +580,18 @@ def history_matrix(indptr, items, n_items):
     m.sum_duplicates()
     m.data[:] = 1.0
     return m
+
+
+def prefix_histories(sequences, impressions, n_items):
+    """The reads before each impression as a scipy CSR [I, n_items] with 1 per article read (history_matrix of the prefixes
+    items[indptr[user] : indptr[user] + time], whole, not truncated to max_len): the histories of the mean-profile baseline,
+    helpers.user_profiles(prefix_histories(...), embeddings)."""
+    indptr, items = check_sequences(sequences, n_items, 'prefix_histories')
+    imp = check_impressions(impressions, n_items, 'prefix_histories', indptr)
+    t = imp['time']
+    p_indptr = np.concatenate([[0], np.cumsum(t)]).astype(np.int64)
+    src = np.repeat(indptr[imp['user']] - p_indptr[:-1], t) + np.arange(int(p_indptr[-1]))
+    return history_matrix(p_indptr, items[src], n_items)
 
 
 def negatives_from_draws(pos, c, n_items):

@@ -597,6 +597,28 @@ int dae_seq_negatives(const int32_t* pos, int64_t n_pos, int32_t n_items, uint64
 int dae_seq_rank_loss(const float* h, int64_t ld_h, const float* emb, int64_t ld_emb, int32_t H, const int32_t* pos, const int32_t* neg,
                       int64_t n_pos, float scale, float* dh, int64_t ld_dh, double* loss_sum, void* stream);
 
+/* ---- impression logs (DESIGN 4.13) ------------------------------------------------------------------------------------------
+ * An impression is a list of shown articles items[indptr[i] .. indptr[i + 1]) (rows of emb) with clicked[k] != 0 where the article
+ * was clicked; C and N are its clicked and not-clicked articles.  One warp per row of work; lists of any length are walked in
+ * chunks of per-warp shared memory.
+ * dae_impression_rank_loss: the impression loss of a packed GRU batch.  The impressions of packed position p are
+ *   [pos_indptr[p], pos_indptr[p + 1]) (ids into imp_indptr); with s_j = h_p . e(items[j]), impression q adds
+ *   l_q = 1 / (|C| |N|) sum_{c, n} softplus(s_n - s_c) to *loss_sum (fp64 atomics) and scale / (|C| |N|) sum_j w_j e(items[j])
+ *   to dh_p, where w_n = sum_c s(s_n - s_c) and w_c = -sum_n s(s_n - s_c).  Impressions with |C| = 0 or |N| = 0 add nothing.
+ *   EVERY row p < n_pos of dh is written (zero without impressions), in a fixed order per row: no atomics on dh.
+ * dae_impression_metrics: one query row q_i (ld_q) per impression.  scores[k] (fp32, every k < indptr[n_imp]) = q_i . e(items[k]),
+ *   or with cosine = 1 that over |q_i| |e(items[k])| (0 when either is zero).  metrics[i] (fp64 [n_imp x 4]) = AUC, MRR, nDCG@5,
+ *   nDCG@10 of those scores: rank_j = #{k: s_k > s_j} + #{k before j: s_k = s_j}; AUC = (#{s_c > s_n} + #{s_c = s_n} / 2) /
+ *   (|C| |N|); MRR = mean over C of 1 / (rank + 1); nDCG@K = sum_{c: rank < K} 1 / log2(rank + 2) over its value for the first
+ *   min(|C|, K) ranks.  |C| = 0 or |N| = 0: four NaNs.
+ */
+int dae_impression_rank_loss(const float* h, int64_t ld_h, const float* emb, int64_t ld_emb, int32_t H, const int64_t* pos_indptr,
+                             int64_t n_pos, const int64_t* imp_indptr, const int32_t* items, const uint8_t* clicked, float scale,
+                             float* dh, int64_t ld_dh, double* loss_sum, void* stream);
+int dae_impression_metrics(const float* q, int64_t ld_q, const float* emb, int64_t ld_emb, int32_t H, int32_t cosine,
+                           const int64_t* indptr, const int32_t* items, const uint8_t* clicked, int64_t n_imp, float* scores,
+                           double* metrics, void* stream);
+
 /* ---- data-parallel exchange step (SURVEY 8e): in-switch all-reduce of the flat gradient buffer -------------------
  * The reference is single-process; row-sharded training adds ONE sum over ranks of [dW | dbh | dbv] between the
  * gradient kernels and dae_optimizer_step.  Default transport: ncclAllReduce.  dae_allreduce_multimem is the

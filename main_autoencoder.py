@@ -103,6 +103,12 @@ def build_parser():
                          'the training embeddings, save user_gru.npz and user_gru_top_k_{index,score}.npy; with targets report '
                          'user_gru_hit_rate / user_gru_recall next to the mean profile\'s for the same reads')
     ap.add_argument('--user_epochs', type=int, default=5, help='with --user_sequences: training epochs of the GRU user encoder')
+    ap.add_argument('--user_impressions', default='',
+                    help='with --user_sequences: an .npz impression log (user, time, indptr, items, clicked; see '
+                         'user_model.check_impressions) to train the GRU on instead of random negatives')
+    ap.add_argument('--user_test_impressions', default='',
+                    help='with --user_sequences: an .npz impression log to score; report the AUC, MRR, nDCG@5 and nDCG@10 of the '
+                         'GRU states (user_gru_imp_*) and of the mean profile of the same reads (user_mean_imp_*)')
     ap.add_argument('--user_targets', default='',
                     help='with --user_histories: a save_npz matrix of the same shape holding held-out reads; report the hit rate '
                          'and recall of the recommendations against them (user_hit_rate, user_recall)')
@@ -161,6 +167,9 @@ def check_flags(F):
     assert not F.user_sequences or F.top_k > 0, '--user_sequences needs --top_k K > 0'
     assert not F.user_sequences or os.path.isfile(F.user_sequences), '--user_sequences %s: no such file' % F.user_sequences
     assert F.user_epochs >= 0, '--user_epochs must be >= 0'
+    for flag, path in (('--user_impressions', F.user_impressions), ('--user_test_impressions', F.user_test_impressions)):
+        assert not path or F.user_sequences, '%s needs --user_sequences' % flag
+        assert not path or os.path.isfile(path), '%s %s: no such file' % (flag, path)
     assert not F.user_targets or F.user_histories, '--user_targets needs --user_histories'
     assert not F.user_targets or os.path.isfile(F.user_targets), '--user_targets %s: no such file' % F.user_targets
     if F.input_format == 'tfidf':
@@ -470,17 +479,33 @@ def load_user_sequences(F, n_train):
     return indptr, items, targets
 
 
-def recommend_users_gru(F, model, enc, seqs):
+def load_user_impressions(F, n_train, seqs):
+    """--user_impressions / --user_test_impressions: (train, test) impression sets (None where the flag is not given), checked
+    against the training set's row count and the sequences before training."""
+    from dae_rnn_news_recommendation_b200.user_model import check_impressions
+    out = []
+    for flag, path in (('--user_impressions', F.user_impressions), ('--user_test_impressions', F.user_test_impressions)):
+        out.append(check_impressions(np.load(path), n_train, '%s %s' % (flag, path), seqs[0]) if path else None)
+    return tuple(out)
+
+
+def recommend_users_gru(F, model, enc, seqs, impressions=(None, None)):
     """--user_sequences: train a GRU user encoder on the training embeddings, save it as user_gru.npz and the --top_k best unread
     articles per user as user_gru_top_k_{index,score}.npy; with targets, the hit rate and recall of the GRU's and of the mean
-    profile's recommendations for the same reads are returned and printed."""
+    profile's recommendations for the same reads are returned and printed.  impressions: (train, test) from load_user_impressions;
+    the GRU trains on train's impressions when given, and test's are scored by the GRU states and by the mean profiles of the
+    same reads."""
     import scipy.sparse as sp
     from dae_rnn_news_recommendation_b200 import helpers
-    from dae_rnn_news_recommendation_b200.user_model import UserGRU, history_matrix
+    from dae_rnn_news_recommendation_b200.user_model import UserGRU, history_matrix, prefix_histories
     indptr, items, targets = seqs
-    print('train a GRU user encoder on %d users (%d reads, %d epochs)' % (len(indptr) - 1, items.size, F.user_epochs))
+    train_imp, test_imp = impressions
+    print('train a GRU user encoder on %d users (%d reads, %d epochs%s)' % (len(indptr) - 1, items.size, F.user_epochs,
+                                                                          ', impressions' if train_imp is not None else ''))
     gru = UserGRU(enc.shape[1], num_epochs=F.user_epochs, seed=max(F.seed, 0))
-    gru.fit((indptr, items), enc)
+    gru.fit((indptr, items), enc, impressions=train_imp)
+    if train_imp is not None:
+        print('impressions: %(used)d used, %(skipped)d skipped' % gru.impression_counts)
     gru.save(model.data_dir + 'user_gru.npz')
     idx, score = gru.recommend((indptr, items), enc, k=F.top_k)
     np.save(model.data_dir + 'user_gru_top_k_index', idx)
@@ -497,6 +522,15 @@ def recommend_users_gru(F, model, enc, seqs):
                     'user_mean_recall': m['recall']})
         print('users (GRU): hit rate@%d %.4f recall@%d %.4f; mean profile: hit rate@%d %.4f recall@%d %.4f (%d users with targets)'
               % (F.top_k, r['hit_rate'], F.top_k, r['recall'], F.top_k, m['hit_rate'], F.top_k, m['recall'], r['users']))
+    if test_imp is not None:
+        g = helpers.impression_metrics(gru.impression_states((indptr, items), enc, test_imp), enc, test_imp, metric='linear kernel')
+        prof = helpers.user_profiles(prefix_histories((indptr, items), test_imp, enc.shape[0]), enc)
+        m = helpers.impression_metrics(prof, enc, test_imp, metric='cosine')
+        for name, r in (('gru', g), ('mean', m)):
+            out.update({'user_%s_imp_%s' % (name, k.replace('@', '')): r[k] for k in ('auc', 'mrr', 'ndcg@5', 'ndcg@10')})
+        print('test impressions (GRU): AUC %.4f MRR %.4f nDCG@5 %.4f nDCG@10 %.4f; mean profile: AUC %.4f MRR %.4f nDCG@5 %.4f '
+              'nDCG@10 %.4f (%d scored, %d skipped)' % (g['auc'], g['mrr'], g['ndcg@5'], g['ndcg@10'], m['auc'], m['mrr'],
+                                                        m['ndcg@5'], m['ndcg@10'], g['impressions'], g['skipped']))
     return out
 
 
@@ -520,6 +554,7 @@ def main(argv=None):
         trX, vlX, trL, vlL = trX.astype(np.float32), vlX.astype(np.float32), np.asarray(trL), np.asarray(vlL)
     histories, targets = load_user_files(F, trX.shape[0]) if F.user_histories else (None, None)
     seqs = load_user_sequences(F, trX.shape[0]) if F.user_sequences else None
+    imps = load_user_impressions(F, trX.shape[0], seqs) if F.user_sequences else (None, None)
     print('fit')
     model.fit(train_set=trX, validation_set=vlX if F.validation else None, train_set_label=trL,
               validation_set_label=vlL if F.validation else None, restore_previous_model=F.restore_previous_model)
@@ -541,7 +576,7 @@ def main(argv=None):
         if histories is not None:
             model.evaluation.update(recommend_users(F, model, enc, histories, targets))
         if seqs is not None:
-            model.evaluation.update(recommend_users_gru(F, model, enc, seqs))
+            model.evaluation.update(recommend_users_gru(F, model, enc, seqs, imps))
         if F.top_k_dedup > 0:
             model.evaluation.update(recommend_top_k_dedup(F, model, enc, enc_v, trL, vlL, histories, targets, model.evaluation))
     if F.dedup_threshold > 0:
