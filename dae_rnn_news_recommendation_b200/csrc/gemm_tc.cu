@@ -1799,6 +1799,9 @@ extern "C" int dae_gemm_bf16x3(int32_t M, int32_t N, int32_t K, float alpha, con
   DAE_REQUIRE(((uintptr_t)a_hi | (uintptr_t)a_lo | (uintptr_t)b_hi | (uintptr_t)b_lo) % 16 == 0, "dae_gemm_bf16x3: operands must be 16-byte aligned");
   cudaStream_t st = (cudaStream_t)stream;
   if (n_store <= 0 || n_store > N) n_store = N;
+  DAE_REQUIRE(ldc >= n_store, "dae_gemm_bf16x3: ldc %lld below n_store %d", (long long)ldc, n_store);
+  DAE_REQUIRE(!special_out || (special_col >= n_store && special_col < N),
+              "dae_gemm_bf16x3: special_col %d outside [n_store, N) = [%d, %d)", special_col, n_store, N);
   const int kblocks = (K + BLOCK_K - 1) / BLOCK_K;
   const int tm = (M + 127) / 128, tn128 = (N + 127) / 128, tn64 = (N + 63) / 64;
   const int sms = sm_count();
@@ -1878,10 +1881,13 @@ extern "C" int dae_gemm_bf16x3_det(int32_t M, int32_t N, int32_t K, float alpha,
   DAE_REQUIRE(lda % 8 == 0 && ldb % 8 == 0, "dae_gemm_bf16x3_det: operand leading dimensions must be multiples of 8 (TMA 16-byte strides)");
   DAE_REQUIRE(((uintptr_t)a_hi | (uintptr_t)a_lo | (uintptr_t)b_hi | (uintptr_t)b_lo) % 16 == 0, "dae_gemm_bf16x3_det: operands must be 16-byte aligned");
   DAE_REQUIRE(k_splits == 1 || k_splits == -1, "dae_gemm_bf16x3_det: k_splits must be 1 or -1 (stream-K), got %d", k_splits);
+  if (n_store <= 0 || n_store > N) n_store = N;
+  DAE_REQUIRE(ldc >= n_store, "dae_gemm_bf16x3_det: ldc %lld below n_store %d", (long long)ldc, n_store);
+  DAE_REQUIRE(!special_out || (special_col >= n_store && special_col < N),
+              "dae_gemm_bf16x3_det: special_col %d outside [n_store, N) = [%d, %d)", special_col, n_store, N);
   DAE_REQUIRE(workspace && workspace_bytes >= sk_workspace_bytes(), "dae_gemm_bf16x3_det: workspace of %lld bytes, need %lld",
               (long long)workspace_bytes, (long long)sk_workspace_bytes());
   cudaStream_t st = (cudaStream_t)stream;
-  if (n_store <= 0 || n_store > N) n_store = N;
   const int tm = (M + 127) / 128, tn = (N + 127) / 128;
   const int stream_k = (k_splits < 0 && (tm * tn) % sm_count() != 0) ? 1 : 0;   // the choice of dae_gemm_bf16x3
   GemmParams p{};

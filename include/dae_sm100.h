@@ -186,7 +186,9 @@ int dae_sgemm(int32_t M, int32_t N, int32_t K, float alpha, const float* A, int6
  * dae_sym_split_bf16: hi/lo <- alpha * (G + G^T)   (dE_tri = alpha (G + G^T) E).
  * dae_gemm_bf16x3: C[m,n] (+)= alpha * sum_k A(m,k) B(n,k).
  *   a_mn_major = 0: A stored [M x lda] (K contiguous); 1: A stored [K x lda] (M contiguous).  Same for B/N.
- *   columns n < n_store go to C; column special_col (if special_out != NULL) goes to special_out[m].
+ *   columns n < n_store go to C; column special_col (if special_out != NULL) goes to special_out[m].  n_store <= 0 or > N means
+ *   N.  Rejected before any device work: ldc < n_store, and special_out != NULL unless n_store <= special_col < N (so the
+ *   special column never aliases a stored one).  The same rules hold for dae_gemm_bf16x3_det.
  *   k_splits > 1 (uniform split-K), k_splits < 0 (stream-K: the tile x k-block units are shared evenly by the SMs, chosen
  *   automatically when the 128x128 tiling does not fill whole waves) or accumulate != 0: fp32 atomics into C (C is zeroed
  *   first unless accumulate).

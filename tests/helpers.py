@@ -49,6 +49,41 @@ def xavier(F, H, seed=0):
     return np.random.default_rng(seed).uniform(-b, b, (F, H)).astype(np.float32)
 
 
+class _CAI:
+    def __init__(self, ptr, shape, typestr):
+        self.__cuda_array_interface__ = {'data': (int(ptr), False), 'shape': tuple(shape), 'typestr': typestr, 'version': 3}
+
+
+def device_copy(ptr, shape, typestr, device='cuda:0'):
+    """A torch copy (on the device) of the buffer of the given shape and NumPy typestr at the raw device pointer ptr."""
+    import torch
+    return torch.as_tensor(_CAI(ptr, shape, typestr), device=device).clone()
+
+
+def snap(ptr, rows, ld, kind='f4'):
+    """A copy of the device buffer [rows x ld] at ptr (fp32 'f4' or bf16 bits 'u2') as a NumPy array."""
+    import torch
+    if ptr is None or rows <= 0:
+        return None
+    t = device_copy(ptr, (rows, ld), '<f4' if kind == 'f4' else '<i2')
+    torch.cuda.synchronize()
+    a = t.cpu().numpy()
+    return a if kind == 'f4' else a.view(np.uint16)
+
+
+def snap_vec(ptr, n, typestr):
+    import torch
+    t = device_copy(ptr, (n,), typestr)
+    torch.cuda.synchronize()
+    return t.cpu().numpy()
+
+
+def pair_value(hi, lo):
+    """fp64 value hi + lo of two bf16 bit arrays (uint16)."""
+    f = lambda b: (np.asarray(b, np.uint16).astype(np.uint32) << 16).view(np.float32).astype(np.float64)
+    return f(hi) + f(lo)
+
+
 def load_uci_c1():
     """BASELINE.json configs[0] data (tests/golden/uci_c1.npz, written by tools/make_uci_fixture.py from the UCI corpus with the
     CLI's own preparation): binary CSR train 8000 x 10000 / validate 2000 x 10000, raw counts, category + story labels."""

@@ -7,6 +7,7 @@ import pytest
 import torch
 
 import gru_kernel_oracle as go
+from helpers import pair_value as _pair_value, snap as _snap, snap_vec as _snap_vec
 
 from dae_rnn_news_recommendation_b200 import user_model
 from dae_rnn_news_recommendation_b200.user_model import Packed, UserGRU
@@ -237,31 +238,6 @@ def test_seq_negatives(n_items):
 # ---------------------------------------------------------------------------------------------------------------------------
 # the composed batch: every kernel call of UserGRU._forward_backward / transform against its own inputs
 # ---------------------------------------------------------------------------------------------------------------------------
-class _CAI:
-    def __init__(self, ptr, shape, typestr):
-        self.__cuda_array_interface__ = {'data': (int(ptr), False), 'shape': tuple(shape), 'typestr': typestr, 'version': 3}
-
-
-def _snap(ptr, rows, ld, kind='f4'):
-    """A copy of the device buffer [rows x ld] at ptr (fp32 'f4' or bf16 bits 'u2') as a NumPy array."""
-    if ptr is None or rows <= 0:
-        return None
-    t = torch.as_tensor(_CAI(ptr, (rows, ld), '<f4' if kind == 'f4' else '<i2'), device=DEV).clone()
-    torch.cuda.synchronize()
-    a = t.cpu().numpy()
-    return a if kind == 'f4' else a.view(np.uint16)
-
-
-def _snap_vec(ptr, n, typestr):
-    t = torch.as_tensor(_CAI(ptr, (n,), typestr), device=DEV).clone()
-    torch.cuda.synchronize()
-    return t.cpu().numpy()
-
-
-def _pair_value(hi, lo):
-    return go.bf16_value(hi).astype(np.float64) + go.bf16_value(lo)
-
-
 class Recorder:
     """Stands in for user_model.call: snapshots each kernel's inputs, runs it, synchronizes and snapshots its outputs."""
 
