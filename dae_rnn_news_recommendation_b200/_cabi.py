@@ -76,6 +76,12 @@ _SIGNATURES = {
                                                     p]),
     'dae_csr_similarity_topk_groups': (C.c_int, [p, p, p, i32, i64, i32, p, p, p, i32, i64, i32, i32, i64, i32, i32, p, i64, p, p, p, p,
                                                  i64, p, p]),
+    'dae_similarity_topk_bound_bf16x3': (C.c_int, [i32, i32, i32, p, p, i64, p, p, i64, i32, i64, i32, i32, p, i64, p, p, i64, p, p,
+                                                   p]),
+    'dae_similarity_topk_bound_workspace': (C.c_int, [i32, i32, i32, i32, p]),
+    'dae_similarity_topk_collect_bf16x3': (C.c_int, [i32, i32, i32, p, p, i64, p, p, i64, i64, i32, p, p, p, i64, p, p, i64, p, p, p,
+                                                     p]),
+    'dae_similarity_topk_select': (C.c_int, [i32, i64, p, p, p, i32, p, p, p, p]),
     'dae_pair_partition': (C.c_int, [p, i64, i32, p, p, p, p, p]),
     'dae_auroc_count': (C.c_int, [p, i64, p, i64, i32, p, p]),
     'dae_similarity_pair_hist_bf16x3': (C.c_int, [i32, i32, p, p, i64, p, f32, i32, p, p, p]),

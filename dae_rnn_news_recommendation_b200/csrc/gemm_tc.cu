@@ -1295,6 +1295,14 @@ struct PairsParams {
   unsigned long long* count;         // caller-zeroed, accumulated: the number of qualifying pairs
   unsigned long long capacity;       // slots of i_out / j_out / s_out
   int32_t* i_out; int32_t* j_out; float* s_out;
+  // pairs_kernel<true> (long top-k lists, corpus-mode tiles): row i's threshold row_tau[i] (at least -FLT_MAX, so -inf and NaN
+  // never qualify), column i + diag_offset left out when `exclude`, per-row exclusion lists (may be null) and per-row counts
+  // row_count[i] (caller-zeroed, accumulated).  Last, so the fields above keep their parameter offsets in pairs_kernel<false>.
+  const float* row_tau;
+  int64_t diag_offset;
+  int exclude;
+  const int64_t* ex_indptr; const int32_t* ex_indices;
+  unsigned int* row_count;
 };
 
 // self: tiles t = mb (mb + 1) / 2 + nb, nb <= mb (PairHistSched's order); corpus: t = mb * tiles_n + nb.  Items blockIdx.x,
@@ -1329,6 +1337,10 @@ struct PairsSched {
   }
 };
 
+// ROWS: the collect stage of the long top-k lists -- a threshold per row; the self match and the listed columns are written as -inf
+// over the thread's own staging run before the scan (topk_kernel<KMAX, true>'s trick, with a binary search per tile since the
+// tiles of one row are not swept in one item), and -inf is below every threshold.
+template <bool ROWS = false>
 __global__ void __launch_bounds__(kDecodeThreads, 1) pairs_kernel(const __grid_constant__ CUtensorMap tm_a_hi,
                                                                   const __grid_constant__ CUtensorMap tm_a_lo,
                                                                   const __grid_constant__ CUtensorMap tm_b_hi,
@@ -1405,12 +1417,33 @@ __global__ void __launch_bounds__(kDecodeThreads, 1) pairs_kernel(const __grid_c
       const int lim = pp.self ? i : p.N;                          // columns j < lim (self: i < M = N)
       const int c_end = i < p.M ? max(0, min(HALF_N, lim - n0)) : 0;
       mbar_wait(&staged_bar[h], tphase);
+      [[maybe_unused]] float tau_i = tau;
+      if constexpr (ROWS) {
+        if (i < p.M) {
+          tau_i = fmaxf(pp.row_tau[i], -FLT_MAX);
+          float* wrow = stg + row_in_tile * SROW + half * HALF_N;
+          const int64_t e = (int64_t)i + pp.diag_offset;
+          if (pp.exclude && e >= n0 && e < n0 + HALF_N) wrow[e - n0] = neg_inf();
+          if (pp.ex_indptr) {
+            int64_t lo = pp.ex_indptr[i], hi = pp.ex_indptr[i + 1];
+            while (lo < hi) {
+              const int64_t mid = lo + ((hi - lo) >> 1);
+              if (pp.ex_indices[mid] < n0) lo = mid + 1; else hi = mid;
+            }
+            for (; lo < pp.ex_indptr[i + 1] && pp.ex_indices[lo] < n0 + HALF_N; ++lo) wrow[pp.ex_indices[lo] - n0] = neg_inf();
+          }
+        }
+      }
+      const float thr = ROWS ? tau_i : tau;
       int hits = 0;
 #pragma unroll 1
       for (int c = 0; c < c_end; c += 4) {   // NaN never qualifies: fmaxf drops it and every compare with it is false
         const float4 v = *reinterpret_cast<const float4*>(srow + c);
-        if (fmaxf(fmaxf(v.x, v.y), fmaxf(v.z, v.w)) >= tau)   // rare at a near-duplicate threshold
-          hits += (v.x >= tau) + (c + 1 < c_end && v.y >= tau) + (c + 2 < c_end && v.z >= tau) + (c + 3 < c_end && v.w >= tau);
+        if (fmaxf(fmaxf(v.x, v.y), fmaxf(v.z, v.w)) >= thr)   // rare at a near-duplicate threshold
+          hits += (v.x >= thr) + (c + 1 < c_end && v.y >= thr) + (c + 2 < c_end && v.z >= thr) + (c + 3 < c_end && v.w >= thr);
+      }
+      if constexpr (ROWS) {
+        if (hits) atomicAdd(pp.row_count + i, (unsigned int)hits);
       }
       if (__any_sync(0xffffffffu, hits != 0)) {
         unsigned long long slot = pair_slots(pp.count, hits);
@@ -1418,7 +1451,7 @@ __global__ void __launch_bounds__(kDecodeThreads, 1) pairs_kernel(const __grid_c
 #pragma unroll 1
           for (int c = 0; c < c_end; ++c) {
             const float s = srow[c];
-            if (s >= tau) pair_put(slot++, pp.capacity, i, n0 + c, s, pp.i_out, pp.j_out, pp.s_out);
+            if (s >= thr) pair_put(slot++, pp.capacity, i, n0 + c, s, pp.i_out, pp.j_out, pp.s_out);
           }
         }
       }
@@ -1717,6 +1750,7 @@ static int launch_pair_hist(const Operand& X, const PairHistParams& hp, cudaStre
 }
 
 // thresholded pairs: Q [M x K] and C [N x K], both K-major; one persistent CTA per SM over the tiles (self: the lower triangle)
+template <bool ROWS = false>
 static int launch_pairs(const Operand& A, const Operand& B, const PairsParams& pp, cudaStream_t st) {
   CUtensorMap ta_hi, ta_lo, tb_hi, tb_lo;
   int rc;
@@ -1727,11 +1761,11 @@ static int launch_pairs(const Operand& A, const Operand& B, const PairsParams& p
   if ((rc = make_map(&tb_lo, B.lo, p.K, p.N, B.ld, kDecodeN, kTopkBK))) return rc;
   constexpr int smem = kTopkStages * (2 * BLOCK_M * kTopkBK * 2 + 2 * kDecodeN * kTopkBK * 2) + BLOCK_M * (kDecodeN + 4) * 4 + 1024;
   static bool attr_done[64] = {false};
-  if ((rc = ensure_smem_attr(pairs_kernel, smem, attr_done))) return rc;
+  if ((rc = ensure_smem_attr(pairs_kernel<ROWS>, smem, attr_done))) return rc;
   const long long tm = (p.M + BLOCK_M - 1) / BLOCK_M, tn = (p.N + kDecodeN - 1) / kDecodeN;
   const long long tiles = pp.self ? tm * (tm + 1) / 2 : tm * tn;
   const int n = tiles < sm_count() ? (int)tiles : sm_count();
-  pairs_kernel<<<n, kDecodeThreads, smem, st>>>(ta_hi, ta_lo, tb_hi, tb_lo, pp);
+  pairs_kernel<ROWS><<<n, kDecodeThreads, smem, st>>>(ta_hi, ta_lo, tb_hi, tb_lo, pp);
   return DAE_OK;
 }
 
@@ -2187,5 +2221,130 @@ extern "C" int dae_similarity_pairs_bf16x3(int32_t n_query, int32_t n_corpus, in
   int rc = launch_pairs(A, B, pp, (cudaStream_t)stream);
   if (rc) return rc;
   DAE_CHECK_LAUNCH("dae_similarity_pairs_bf16x3");
+  return DAE_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// long top-k lists (k up to kTopkLongMaxK, DESIGN 4.14): bound, collect, select.  The bound runs topk_kernel<32> with enough splits
+// that the 2 * splits partial lists of 32 hold at least 2k entries; their k-th best is a lower bound tau_i on the row's k-th score.
+// The collect stage (pairs_kernel<true>) lists every candidate with s >= tau_i, so every answer; dae_pairs_sort makes each row's
+// candidates contiguous in increasing column order, and the select stage ranks them.  All scores come from the same tiles and
+// k16 order as topk_kernel's, so they are its bits.
+// ---------------------------------------------------------------------------------------------------------------------
+static int topk_bound_splits(int n_query, int n_corpus, int k, int requested) {
+  const int s = topk_splits(n_query, n_corpus, requested);
+  const int need = (k + 31) / 32;
+  return topk_splits(n_query, n_corpus, s > need ? s : need);
+}
+
+// rank chunk L of topk_bound_kernel / topk_select_kernel: a power of two >= k, and a multiple of the block size
+static int rank_chunk(int k) {
+  int L = kRankThreads;
+  while (L < k) L <<= 1;
+  return L;
+}
+
+extern "C" int dae_similarity_topk_bound_workspace(int32_t n_query, int32_t n_corpus, int32_t k, int32_t splits, int64_t* bytes) {
+  DAE_REQUIRE(bytes && n_query > 0 && n_corpus > 0, "dae_similarity_topk_bound_workspace: bad arguments");
+  DAE_REQUIRE(k >= 1 && k <= kTopkLongMaxK, "dae_similarity_topk_bound_workspace: k = %d is outside the supported range 1 <= k <= %d", k,
+              kTopkLongMaxK);
+  *bytes = topk_workspace_bytes(n_query, kTopkMaxK, topk_bound_splits(n_query, n_corpus, k, splits));
+  return DAE_OK;
+}
+
+extern "C" int dae_similarity_topk_bound_bf16x3(int32_t n_query, int32_t n_corpus, int32_t dim, const void* q_hi, const void* q_lo,
+                                                int64_t ldq, const void* c_hi, const void* c_lo, int64_t ldc, int32_t k,
+                                                int64_t diag_offset, int32_t exclude, int32_t splits, void* workspace,
+                                                int64_t workspace_bytes, const int64_t* ex_indptr, const int32_t* ex_indices,
+                                                int64_t ex_nnz, const int32_t* groups, float* tau, void* stream) {
+  DAE_REQUIRE(q_hi && q_lo && c_hi && c_lo && workspace && tau && (ex_nnz == 0 || (ex_indptr && ex_indices)),
+              "dae_similarity_topk_bound_bf16x3: null pointer");
+  DAE_REQUIRE(n_query > 0 && n_corpus > 0 && dim > 0 && ex_nnz >= 0, "dae_similarity_topk_bound_bf16x3: bad sizes");
+  DAE_REQUIRE(k >= 1 && k <= kTopkLongMaxK, "dae_similarity_topk_bound_bf16x3: k = %d is outside the supported range 1 <= k <= %d", k,
+              kTopkLongMaxK);
+  DAE_REQUIRE(ldq >= dim && ldc >= dim && ldq % 8 == 0 && ldc % 8 == 0,
+              "dae_similarity_topk_bound_bf16x3: leading dimensions must cover dim and be multiples of 8 (TMA 16-byte strides)");
+  DAE_REQUIRE(((uintptr_t)q_hi | (uintptr_t)q_lo | (uintptr_t)c_hi | (uintptr_t)c_lo | (uintptr_t)workspace) % 16 == 0 &&
+                  (uintptr_t)ex_indptr % 8 == 0 && ((uintptr_t)ex_indices | (uintptr_t)groups | (uintptr_t)tau) % 4 == 0,
+              "dae_similarity_topk_bound_bf16x3: operands and workspace must be 16-byte, ex_indptr 8-byte, ex_indices, groups and tau "
+              "4-byte aligned");
+  const int s = topk_bound_splits(n_query, n_corpus, k, splits);
+  const int64_t need = topk_workspace_bytes(n_query, kTopkMaxK, s);
+  DAE_REQUIRE(workspace_bytes >= need,
+              "dae_similarity_topk_bound_bf16x3: workspace of %lld bytes, %lld needed (dae_similarity_topk_bound_workspace)",
+              (long long)workspace_bytes, (long long)need);
+  cudaStream_t st = (cudaStream_t)stream;
+  TopkParams tp{};
+  tp.g.M = n_query; tp.g.N = n_corpus; tp.g.K = dim; tp.g.k_splits = 1; tp.g.alpha = 1.0f; tp.g.special_col = -1;
+  tp.k = kTopkMaxK; tp.splits = s; tp.exclude = exclude ? 1 : 0; tp.diag_offset = diag_offset;
+  tp.ws_val = reinterpret_cast<float*>(workspace);
+  tp.ws_idx = reinterpret_cast<int32_t*>(reinterpret_cast<float*>(workspace) + (int64_t)n_query * 2 * s * kTopkMaxK);
+  tp.ex_indptr = ex_nnz ? ex_indptr : nullptr; tp.ex_indices = ex_indices; tp.groups = groups;
+  Operand A{q_hi, q_lo, ldq, 0}, B{c_hi, c_lo, ldc, 0};
+  int rc = groups ? launch_topk<32, true, true>(A, B, tp, st)
+                  : (tp.ex_indptr ? launch_topk<32, true>(A, B, tp, st) : launch_topk<32, false>(A, B, tp, st));
+  if (rc) return rc;
+  DAE_CHECK_LAUNCH("dae_similarity_topk_bound_bf16x3");
+  const int L = rank_chunk(k);
+  if (groups)
+    topk_bound_kernel<true><<<n_query, kRankThreads, 4 * L * 8, st>>>(tp.ws_val, tp.ws_idx, 2 * s, kTopkMaxK, k, L, groups, tau);
+  else
+    topk_bound_kernel<false><<<n_query, kRankThreads, 2 * L * 8, st>>>(tp.ws_val, tp.ws_idx, 2 * s, kTopkMaxK, k, L, nullptr, tau);
+  DAE_CHECK_LAUNCH("dae_similarity_topk_bound_bf16x3 (bound)");
+  return DAE_OK;
+}
+
+extern "C" int dae_similarity_topk_collect_bf16x3(int32_t n_query, int32_t n_corpus, int32_t dim, const void* q_hi, const void* q_lo,
+                                                  int64_t ldq, const void* c_hi, const void* c_lo, int64_t ldc, int64_t diag_offset,
+                                                  int32_t exclude, const float* tau, const int64_t* ex_indptr, const int32_t* ex_indices,
+                                                  int64_t ex_nnz, uint64_t* count, uint32_t* row_count, int64_t capacity, int32_t* i_out,
+                                                  int32_t* j_out, float* s_out, void* stream) {
+  DAE_REQUIRE(q_hi && q_lo && c_hi && c_lo && tau && count && row_count && (ex_nnz == 0 || (ex_indptr && ex_indices)),
+              "dae_similarity_topk_collect_bf16x3: null pointer");
+  DAE_REQUIRE(capacity >= 0, "dae_similarity_topk_collect_bf16x3: capacity = %lld < 0", (long long)capacity);
+  DAE_REQUIRE(capacity == 0 || (i_out && j_out && s_out), "dae_similarity_topk_collect_bf16x3: null output with capacity %lld > 0",
+              (long long)capacity);
+  DAE_REQUIRE(n_query > 0 && n_corpus > 0 && dim > 0 && ex_nnz >= 0, "dae_similarity_topk_collect_bf16x3: bad sizes");
+  DAE_REQUIRE(ldq >= dim && ldc >= dim && ldq % 8 == 0 && ldc % 8 == 0,
+              "dae_similarity_topk_collect_bf16x3: leading dimensions must cover dim and be multiples of 8 (TMA 16-byte strides)");
+  DAE_REQUIRE(((uintptr_t)q_hi | (uintptr_t)q_lo | (uintptr_t)c_hi | (uintptr_t)c_lo) % 16 == 0 &&
+                  ((uintptr_t)count | (uintptr_t)ex_indptr) % 8 == 0 &&
+                  ((uintptr_t)tau | (uintptr_t)row_count | (uintptr_t)ex_indices | (uintptr_t)i_out | (uintptr_t)j_out |
+                   (uintptr_t)s_out) % 4 == 0,
+              "dae_similarity_topk_collect_bf16x3: operands must be 16-byte, the counter and ex_indptr 8-byte, the other arrays 4-byte "
+              "aligned");
+  PairsParams pp{};
+  pp.g.M = n_query; pp.g.N = n_corpus; pp.g.K = dim; pp.g.k_splits = 1; pp.g.alpha = 1.0f; pp.g.special_col = -1;
+  pp.self = 0; pp.tau = 0.0f;
+  pp.count = reinterpret_cast<unsigned long long*>(count); pp.capacity = (unsigned long long)capacity;
+  pp.i_out = i_out; pp.j_out = j_out; pp.s_out = s_out;
+  pp.row_tau = tau; pp.diag_offset = diag_offset; pp.exclude = exclude ? 1 : 0;
+  pp.ex_indptr = ex_nnz ? ex_indptr : nullptr; pp.ex_indices = ex_indices; pp.row_count = row_count;
+  Operand A{q_hi, q_lo, ldq, 0}, B{c_hi, c_lo, ldc, 0};
+  int rc = launch_pairs<true>(A, B, pp, (cudaStream_t)stream);
+  if (rc) return rc;
+  DAE_CHECK_LAUNCH("dae_similarity_topk_collect_bf16x3");
+  return DAE_OK;
+}
+
+extern "C" int dae_similarity_topk_select(int32_t n_query, int64_t n_pairs, const int32_t* i_sorted, const int32_t* j_sorted,
+                                          const float* s_sorted, int32_t k, const int32_t* groups, int32_t* idx_out, float* val_out,
+                                          void* stream) {
+  DAE_REQUIRE(idx_out && val_out && (n_pairs == 0 || (i_sorted && j_sorted && s_sorted)), "dae_similarity_topk_select: null pointer");
+  DAE_REQUIRE(n_query > 0 && n_pairs >= 0 && n_pairs <= INT32_MAX, "dae_similarity_topk_select: bad sizes");
+  DAE_REQUIRE(k >= 1 && k <= kTopkLongMaxK, "dae_similarity_topk_select: k = %d is outside the supported range 1 <= k <= %d", k,
+              kTopkLongMaxK);
+  DAE_REQUIRE(((uintptr_t)i_sorted | (uintptr_t)j_sorted | (uintptr_t)s_sorted | (uintptr_t)groups | (uintptr_t)idx_out |
+               (uintptr_t)val_out) % 4 == 0,
+              "dae_similarity_topk_select: arrays must be 4-byte aligned");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int L = rank_chunk(k);
+  if (groups)
+    topk_select_kernel<true><<<n_query, kRankThreads, 4 * L * 8, st>>>(i_sorted, j_sorted, s_sorted, n_pairs, k, L, groups, idx_out,
+                                                                        val_out);
+  else
+    topk_select_kernel<false><<<n_query, kRankThreads, 2 * L * 8, st>>>(i_sorted, j_sorted, s_sorted, n_pairs, k, L, nullptr, idx_out,
+                                                                         val_out);
+  DAE_CHECK_LAUNCH("dae_similarity_topk_select");
   return DAE_OK;
 }

@@ -168,6 +168,97 @@ def _similarity_topk(q, c, n_q, n_c, h, k, diag_offset=0, exclude=False, splits=
     return idx, val
 
 
+TOPK_MAX_K = 32                    # the register kernels (dae_similarity_topk_*)
+TOPK_LONG_MAX_K = 1024             # long_lists=True, dense inputs (dae_similarity_topk_bound / _collect / _select)
+TOPK_LONG_MAX_CANDIDATES = 1 << 24  # default candidate budget of the long lists: 12 B per candidate, 24 B more in the sort
+
+
+def _check_k(k, long_lists, sparse, fn):
+    """k validation of top_k_similar / recommend, before any device work."""
+    if long_lists:
+        if not 1 <= k <= TOPK_LONG_MAX_K:
+            raise _cabi.DaeError('%s: k = %d is outside the supported range 1 <= k <= %d' % (fn, k, TOPK_LONG_MAX_K))
+        if sparse and k > TOPK_MAX_K:
+            raise ValueError('%s: k = %d: sparse inputs rank at most %d results per query (long_lists needs dense inputs)'
+                             % (fn, k, TOPK_MAX_K))
+    elif not 1 <= k <= TOPK_MAX_K:
+        raise _cabi.DaeError('%s: k = %d is outside the supported range 1 <= k <= %d (long_lists=True ranks up to %d for dense '
+                             'inputs)' % (fn, k, TOPK_MAX_K, TOPK_LONG_MAX_K))
+
+
+def _check_budget(max_candidates, fn):
+    if isinstance(max_candidates, bool) or not isinstance(max_candidates, (int, np.integer)) or max_candidates < 1:
+        raise ValueError('%s: max_candidates = %r must be a positive integer' % (fn, max_candidates))
+    return int(max_candidates)
+
+
+def _similarity_topk_long(q, c, n_q, n_c, h, k, exclude=False, splits=0, lists=None, groups=None,
+                          max_candidates=TOPK_LONG_MAX_CANDIDATES):
+    """_similarity_topk for any 1 <= k <= 1024 in three stages per chunk of query rows (DESIGN 4.14): a lower bound tau_i on each
+    row's k-th score from the register kernels' partial lists (dae_similarity_topk_bound_bf16x3), every candidate with s >= tau_i
+    (dae_similarity_topk_collect_bf16x3), sorted by (i, j) (dae_pairs_sort), and each row's k best of them
+    (dae_similarity_topk_select).  The output equals the register kernels' for k <= 32, bit for bit.
+    Memory: at most max(max_candidates, n_c) candidates are held at once (12 B each, 24 B more during the sort), so a single row
+    always fits; the chunks hold max_candidates // (2k) rows.  When a chunk's candidates exceed that, its per-row counts cut it into
+    row ranges that fit, and each range is collected once more."""
+    dev = q[0].device
+    budget = max(int(max_candidates), n_c)
+    rows = max(1, min(n_q, budget // (2 * k)))
+    cap = min(budget, rows * n_c)
+    idx = torch.empty(n_q, k, dtype=torch.int32, device=dev)
+    val = torch.empty(n_q, k, dtype=torch.float32, device=dev)
+    need = (ctypes.c_int64 * 1)()
+    call('dae_similarity_topk_bound_workspace', rows, n_c, k, splits, ctypes.addressof(need))
+    ws = torch.empty(max(int(need[0]), 16), dtype=torch.uint8, device=dev)
+    tau = torch.empty(rows, dtype=torch.float32, device=dev)
+    row_count = torch.zeros(rows, dtype=torch.int32, device=dev)   # uint32 in the kernel
+    count = torch.zeros(1, dtype=torch.int64, device=dev)
+    i_buf = torch.empty(cap, dtype=torch.int32, device=dev)
+    j_buf = torch.empty(cap, dtype=torch.int32, device=dev)
+    s_buf = torch.empty(cap, dtype=torch.float32, device=dev)
+    ex_ptr, ex_ind, ex_nnz = _list_args(lists)
+    g_ptr = None if groups is None else groups.data_ptr()
+    row_bytes = lists.indptr.element_size() if lists is not None else 0
+
+    def operands(r0):   # (n_corpus, dim, q_hi, q_lo, ldq, c_hi, c_lo, ldc) of the query rows from r0 on
+        return (n_c, h, q[0][r0:].data_ptr(), q[1][r0:].data_ptr(), q[0].stride(0), c[0].data_ptr(), c[1].data_ptr(), c[0].stride(0))
+
+    def lists_from(r0):   # the exclusion lists of the query rows from r0 on (their indices stay absolute)
+        return (None if ex_ptr is None else ex_ptr + r0 * row_bytes), ex_ind, ex_nnz
+
+    def collect(r0, m, t0):   # rows [r0, r0 + m), tau[t0:]; the self match of query row r is column r
+        count.zero_()
+        row_count[:m].zero_()
+        call('dae_similarity_topk_collect_bf16x3', m, *operands(r0), r0, 1 if exclude else 0, tau[t0:].data_ptr(), *lists_from(r0),
+             count.data_ptr(), row_count.data_ptr(), cap, i_buf.data_ptr(), j_buf.data_ptr(), s_buf.data_ptr(), _stream())
+        return int(count.item())
+
+    def select(r0, m, n):
+        i, j, s = _sort_pairs([i_buf, j_buf, s_buf], n, m, n_c, dev)
+        call('dae_similarity_topk_select', m, n, i.data_ptr() if n else None, j.data_ptr() if n else None, s.data_ptr() if n else None,
+             k, g_ptr, idx[r0].data_ptr(), val[r0].data_ptr(), _stream())
+
+    for r0 in range(0, n_q, rows):
+        m = min(rows, n_q - r0)
+        call('dae_similarity_topk_bound_bf16x3', m, *operands(r0), k, r0, 1 if exclude else 0, splits, ws.data_ptr(), ws.numel(),
+             *lists_from(r0), g_ptr, tau.data_ptr(), _stream())
+        n = collect(r0, m, 0)
+        if n <= cap:
+            select(r0, m, n)
+            continue
+        per_row = row_count[:m].cpu().numpy().astype(np.int64)   # exact: the capacity only limits what is written
+        a = 0
+        while a < m:   # row ranges [a, b) of at most cap candidates; one row alone always fits (per_row <= n_c <= cap)
+            b = a + max(1, int(np.searchsorted(np.cumsum(per_row[a:]), cap, side='right')))
+            want = int(per_row[a:b].sum())
+            got = collect(r0 + a, b - a, a)
+            if got != want:
+                raise RuntimeError('top_k_similar: the second collect call counted %d candidates, the first %d' % (got, want))
+            select(r0 + a, b - a, got)
+            a = b
+    return idx, val
+
+
 def _list_args(lists):
     """(ex_indptr, ex_indices, ex_nnz) of the *_groups exports: NULL pointers for no lists."""
     if lists is None:
@@ -296,7 +387,8 @@ def _read_group_lists(indptr, indices, groups, corpus_groups):
     return out_ptr, (keys % n_c).to(torch.int32)
 
 
-def top_k_similar(embeddings, k=10, corpus=None, metric='cosine', device='cuda:0', to_host=True, splits=0, exclude=None, groups=None):
+def top_k_similar(embeddings, k=10, corpus=None, metric='cosine', device='cuda:0', to_host=True, splits=0, exclude=None, groups=None,
+                  long_lists=False, max_candidates=TOPK_LONG_MAX_CANDIDATES):
     """For every row of `embeddings` the k most similar rows of `corpus` and their scores, best first (among equal scores the
     lower index first), without forming the similarity matrix.  corpus=None ranks the set against itself and leaves each row's
     self match out.  Rows with fewer than k candidates are padded with index -1 and score -inf.  metric: 'cosine' or
@@ -315,10 +407,14 @@ def top_k_similar(embeddings, k=10, corpus=None, metric='cosine', device='cuda:0
     the query's own group remain candidates (pass them in `exclude` to leave them out too).  A wrong length, a non-integer dtype
     or a label outside [0, 2^31) raises ValueError before any device work.
     Returns (index int32 [Nq, k], score float32 [Nq, k]) as ndarrays, or device tensors with to_host=False.  `splits`
-    (> 0) fixes the number of corpus parts the work is cut into; it does not change the result."""
+    (> 0) fixes the number of corpus parts the work is cut into; it does not change the result.
+    1 <= k <= 32, or with long_lists=True 1 <= k <= 1024 for dense inputs (sparse inputs stay at 32: ValueError).  k <= 32 runs
+    the register kernels either way; a larger k runs the long-list stages (DESIGN 4.14) with the same contract -- order, ties,
+    padding, exclusion and groups -- and the same score bits.  They hold at most max(max_candidates, Nc) candidate pairs at once
+    (36 B each at the peak), cutting the queries into chunks of max_candidates // (2k) rows."""
     assert metric in ['cosine', 'linear kernel']
-    if not 1 <= k <= 32:
-        raise _cabi.DaeError('top_k_similar: k = %d is outside the supported range 1 <= k <= 32' % k)
+    _check_k(k, long_lists, sp.issparse(embeddings), 'top_k_similar')
+    max_candidates = _check_budget(max_candidates, 'top_k_similar')
     if corpus is not None and sp.issparse(embeddings) != sp.issparse(corpus):
         raise ValueError('top_k_similar: queries and corpus must be both sparse or both dense')
     lists = g_dev = None
@@ -346,7 +442,11 @@ def top_k_similar(embeddings, k=10, corpus=None, metric='cosine', device='cuda:0
             raise ValueError('top_k_similar: corpus rows have %d columns, queries %d' % (xc.shape[1], h))
         n_c = xc.shape[0]
         c = _normalised_operands(xc, norm_kind)[:2]
-    idx, val = _similarity_topk(q, c, n_q, n_c, h, k, exclude=corpus is None, splits=splits, lists=lists, groups=g_dev)
+    if k > TOPK_MAX_K:
+        idx, val = _similarity_topk_long(q, c, n_q, n_c, h, k, exclude=corpus is None, splits=splits, lists=lists, groups=g_dev,
+                                         max_candidates=max_candidates)
+    else:
+        idx, val = _similarity_topk(q, c, n_q, n_c, h, k, exclude=corpus is None, splits=splits, lists=lists, groups=g_dev)
     if to_host:
         return idx.cpu().numpy(), val.cpu().numpy()
     return idx, val
@@ -442,7 +542,7 @@ def sequences_from_csr(m):
 
 
 def recommend(histories, embeddings, k=10, candidates=None, metric='cosine', exclude_read=True, device='cuda:0', to_host=True,
-              splits=0, profiles=None, groups=None):
+              splits=0, profiles=None, groups=None, long_lists=False, max_candidates=TOPK_LONG_MAX_CANDIDATES):
     """For every user the k best articles by `metric` between the user's profile (user_profiles: the weighted mean of the read
     articles' embeddings) and the articles: 'cosine', or 'linear kernel' (the plain inner product).  Order, ties and padding as in
     top_k_similar.  exclude_read: no article of the user's history is returned -- the history goes to the top-k kernel as the
@@ -455,11 +555,12 @@ def recommend(histories, embeddings, k=10, candidates=None, metric='cosine', exc
     is recommended, as in top_k_similar(groups=...).  With exclude_read, every article of a group the user has read is excluded
     too, so a user is not shown a rewrite of a story they read; those lists are built on the device from the histories and the
     labels (over the candidates' positions when candidates are given).
+    long_lists / max_candidates: as in top_k_similar -- up to k = 1024 with long_lists=True.
     Returns (index int32 [U, k], score float32 [U, k]) as ndarrays (device tensors with to_host=False)."""
     if metric not in ('cosine', 'linear kernel'):
         raise ValueError("recommend: metric = %r: 'cosine' or 'linear kernel'" % (metric,))
-    if not 1 <= k <= 32:
-        raise _cabi.DaeError('recommend: k = %d is outside the supported range 1 <= k <= 32' % k)
+    _check_k(k, long_lists, False, 'recommend')
+    max_candidates = _check_budget(max_candidates, 'recommend')
     n_art = embeddings.shape[0]
     if sp.issparse(embeddings):
         _dense_embeddings(embeddings, device, 'recommend')
@@ -488,7 +589,7 @@ def recommend(histories, embeddings, k=10, candidates=None, metric='cosine', exc
     elif exclude_read:
         lists = _DeviceLists(hist.indptr, hist.indices, hist.nnz) if cand is None else _DeviceLists.from_host(*lists_host, device)
     corpus = emb if cand is None else emb.index_select(0, cand_dev)
-    idx, val = _recommend_topk(prof, corpus, k, metric, lists, splits, cg_dev)
+    idx, val = _recommend_topk(prof, corpus, k, metric, lists, splits, cg_dev, max_candidates)
     if empty.any():
         e = torch.from_numpy(empty).to(device)
         idx[e] = -1
@@ -500,12 +601,15 @@ def recommend(histories, embeddings, k=10, candidates=None, metric='cosine', exc
     return idx, val
 
 
-def _recommend_topk(prof, corpus, k, metric, lists, splits=0, groups=None):
+def _recommend_topk(prof, corpus, k, metric, lists, splits=0, groups=None, max_candidates=TOPK_LONG_MAX_CANDIDATES):
     """The ranking half of recommend: profiles [U, H] against corpus [Nc, H] on the tensor cores, with the exclusion lists and
-    the corpus rows' group labels."""
+    the corpus rows' group labels; k > 32 through the long-list stages."""
     norm_kind = 2 if metric == 'cosine' else 0
     q = _normalised_operands(prof, norm_kind)[:2]
     c = _normalised_operands(corpus, norm_kind)[:2]
+    if k > TOPK_MAX_K:
+        return _similarity_topk_long(q, c, prof.shape[0], corpus.shape[0], prof.shape[1], k, splits=splits, lists=lists, groups=groups,
+                                     max_candidates=max_candidates)
     return _similarity_topk(q, c, prof.shape[0], corpus.shape[0], prof.shape[1], k, splits=splits, lists=lists, groups=groups)
 
 
@@ -626,6 +730,16 @@ def _pairs_call(run, n_q, n_c, max_pairs, threshold, device):
         got = int(count.item())
         if got != n:
             raise RuntimeError('similar_pairs: the second call counted %d pairs, the first %d' % (got, n))
+    bufs = [i, j, s]
+    del i, j, s
+    return _sort_pairs(bufs, n, n_q, n_c, device)
+
+
+def _sort_pairs(bufs, n, n_q, n_c, device):
+    """The first n pairs of bufs = [i, j, s] (device int32, int32, float32; i < n_q, j < n_c) sorted by (i, j).  Takes the buffers:
+    the list is emptied, so that the caller keeps no reference to them."""
+    i, j, s = bufs
+    bufs.clear()
     # canonical order: the unique int64 keys i * Nc + j radix-sorted with the scores as payload (dae_pairs_sort), which writes the
     # decoded (i, j) into the key buffer it leaves free.  The first call's unused slots are released first, so from here on the
     # peak is 24 B per pair (two key and two score buffers) plus the sort's fixed scratch (DESIGN 4.8).

@@ -559,17 +559,18 @@ class UserGRU:
         return out.cpu().numpy() if to_host else out
 
     def recommend(self, sequences, embeddings, k=10, candidates=None, exclude_read=True, metric='linear kernel', to_host=True,
-                  groups=None):
+                  groups=None, long_lists=False):
         """The k best articles per user for the GRU user vectors (helpers.recommend with profiles=transform(...)): every read
         article (the whole history, not only the last max_len) is excluded with exclude_read, users without reads get padding.
-        groups: the articles' group labels, passed to helpers.recommend (at most one article per group, read groups excluded)."""
+        groups: the articles' group labels, passed to helpers.recommend (at most one article per group, read groups excluded).
+        long_lists: passed to helpers.recommend (k up to 1024)."""
         from .helpers import recommend
         emb = self._embeddings(embeddings, 'UserGRU.recommend')
         indptr, items = check_sequences(sequences, emb.shape[0], 'UserGRU.recommend')
         hist = history_matrix(indptr, items, emb.shape[0])
         prof = self.transform((indptr, items), emb, to_host=False)
         return recommend(hist, emb, k=k, candidates=candidates, metric=metric, exclude_read=exclude_read, device=self.device,
-                         to_host=to_host, profiles=prof, groups=groups)
+                         to_host=to_host, profiles=prof, groups=groups, long_lists=long_lists)
 
 
 def history_matrix(indptr, items, n_items):

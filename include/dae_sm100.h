@@ -428,6 +428,39 @@ int dae_csr_similarity_topk_groups(const int64_t* q_indptr, const int32_t* q_ind
                                    int32_t* idx_out, float* val_out, const int64_t* ex_indptr, const int32_t* ex_indices,
                                    int64_t ex_nnz, const int32_t* groups, void* stream);
 
+/* ---- long top-k lists: k up to 1024 on the tensor cores, in three stages (DESIGN 4.14) ------------------------------
+ * The stages give, per query row, exactly what dae_similarity_topk_groups_bf16x3 / _excl / the plain call would give for the same
+ * arguments if they accepted k: order (score desc, index asc), -0.0 equal to +0.0, padding -1 / -inf, no NaN, the same exclusion
+ * and group semantics, independent of `splits`, every score the bits those calls report for that (i, j).  1 <= k <= 1024.
+ * dae_similarity_topk_bound_bf16x3: the arguments of dae_similarity_topk_groups_bf16x3 (groups may be NULL: no groups;
+ *   ex_indptr may be NULL when ex_nnz = 0) with a bound workspace of at least dae_similarity_topk_bound_workspace bytes (16-byte
+ *   aligned, same n_query, n_corpus, k, splits).  Writes tau [n_query] (fp32, 4-byte aligned): a lower bound on row i's k-th best
+ *   answer score (-FLT_MAX when it has fewer than k answers).  `splits` sets the least number of corpus parts; the call uses at
+ *   least ceil(k / 32) of them.
+ * dae_similarity_topk_collect_bf16x3: every candidate (i, j) of the same rows (no self match with `exclude`, nothing listed in
+ *   ex_indptr / ex_indices) with S[i, j] >= max(tau[i], -FLT_MAX): so never -inf or NaN.  The count protocol of
+ *   dae_similarity_pairs_bf16x3 (*count caller-zeroed and accumulated, the first `capacity` written to i_out / j_out / s_out),
+ *   plus row_count [n_query] (uint32, caller-zeroed, accumulated): the candidates of each row.  Every tile of S is computed.
+ * dae_similarity_topk_select: n_pairs candidates sorted by (i, j) (dae_pairs_sort's output; i in [0, n_query)) -> idx_out /
+ *   val_out [n_query x k], the k best of each row by (score desc, j asc); with groups (int32 [n_corpus] labels >= 0, or NULL) each
+ *   group contributes its first candidate in that order only.  Any number of candidates per row.
+ * Every argument is checked before any CUDA call.
+ */
+int dae_similarity_topk_bound_bf16x3(int32_t n_query, int32_t n_corpus, int32_t dim, const void* q_hi, const void* q_lo,
+                                     int64_t ldq, const void* c_hi, const void* c_lo, int64_t ldc, int32_t k,
+                                     int64_t diag_offset, int32_t exclude, int32_t splits, void* workspace,
+                                     int64_t workspace_bytes, const int64_t* ex_indptr, const int32_t* ex_indices,
+                                     int64_t ex_nnz, const int32_t* groups, float* tau, void* stream);
+int dae_similarity_topk_bound_workspace(int32_t n_query, int32_t n_corpus, int32_t k, int32_t splits, int64_t* bytes);
+int dae_similarity_topk_collect_bf16x3(int32_t n_query, int32_t n_corpus, int32_t dim, const void* q_hi, const void* q_lo,
+                                       int64_t ldq, const void* c_hi, const void* c_lo, int64_t ldc, int64_t diag_offset,
+                                       int32_t exclude, const float* tau, const int64_t* ex_indptr, const int32_t* ex_indices,
+                                       int64_t ex_nnz, uint64_t* count, uint32_t* row_count, int64_t capacity, int32_t* i_out,
+                                       int32_t* j_out, float* s_out, void* stream);
+int dae_similarity_topk_select(int32_t n_query, int64_t n_pairs, const int32_t* i_sorted, const int32_t* j_sorted,
+                               const float* s_sorted, int32_t k, const int32_t* groups, int32_t* idx_out, float* val_out,
+                               void* stream);
+
 /* ---- "next" row (SURVEY 8f rank 2): related-vs-unrelated AUROC of a pairwise similarity matrix ---------------------
  * Replaces the numeric part of helpers.visualize_pairwise_similarity (helpers.py:88-100).
  * dae_pair_partition: for every pair i > j of the strict lower triangle with labels[i] >= 0 and labels[j] >= 0

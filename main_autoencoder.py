@@ -65,7 +65,10 @@ def build_parser():
                     help="'device': Philox masking + device permutation (default); 'numpy': the reference's host NumPy RNG stream")
     ap.add_argument('--top_k', type=int, default=0,
                     help='K > 0: after transform, save the K most similar training articles of every training and every validation '
-                         'article (K <= 32) and report the share that shares the label; 0 = off')
+                         'article (K <= 32, or K <= 1024 with --long_lists) and report the share that shares the label; 0 = off')
+    ap.add_argument('--long_lists', action='store_true', default=False,
+                    help='let --top_k K go up to 1024 (the long-list stages of helpers.top_k_similar / recommend) for the article '
+                         'lists, the user lists and --top_k_dedup; not with --top_k_input, whose sparse ranking stops at 32')
     ap.add_argument('--top_k_input', action='store_true', default=False,
                     help='with --top_k K: also rank by the input vectors (cosine for binary, linear kernel for tf-idf), save '
                          'article_top_k_input_{index,score}[_validate].npy and report their label precision next to the embedding\'s')
@@ -156,7 +159,10 @@ def check_flags(F):
     assert F.triplet_strategy in ['batch_all', 'batch_hard', 'none']
     assert F.input_format in ['binary', 'tfidf']
     assert F.label in ['category_publish_name', 'story']
-    assert 0 <= F.top_k <= 32
+    assert 0 <= F.top_k <= (1024 if F.long_lists else 32), '--top_k %d: K <= 32, or K <= 1024 with --long_lists' % F.top_k
+    if F.top_k_input and F.top_k > 32:
+        raise ValueError('--top_k_input ranks the sparse input vectors, at most 32 results per article: --top_k %d needs K <= 32'
+                         % F.top_k)
     assert not F.top_k_input or F.top_k > 0, '--top_k_input needs --top_k K > 0'
     assert F.top_k_dedup >= 0.0
     assert not F.top_k_dedup or F.top_k > 0, '--top_k_dedup needs --top_k K > 0'
@@ -332,7 +338,7 @@ def recommend_top_k(F, model, enc, enc_v, trL, vlL):
     for split, E, lab in (('', enc, trL), ('_validate', enc_v, vlL)):
         if E is None or E.shape[0] == 0:
             continue
-        idx, score = helpers.top_k_similar(E, k=F.top_k, corpus=None if split == '' else enc, metric='cosine')
+        idx, score = helpers.top_k_similar(E, k=F.top_k, corpus=None if split == '' else enc, metric='cosine', long_lists=F.long_lists)
         np.save(model.data_dir + 'article_top_k_index' + split, idx)
         np.save(model.data_dir + 'article_top_k_score' + split, score)
         out['top_k' + split] = (idx, score)
@@ -380,7 +386,8 @@ def recommend_top_k_dedup(F, model, enc, enc_v, trL, vlL, histories, targets, em
     for split, E, lab in (('', enc, trL), ('_validate', enc_v, vlL)):
         if E is None or E.shape[0] == 0:
             continue
-        idx, score = helpers.top_k_similar(E, k=F.top_k, corpus=None if split == '' else enc, metric='cosine', groups=groups)
+        idx, score = helpers.top_k_similar(E, k=F.top_k, corpus=None if split == '' else enc, metric='cosine', groups=groups,
+                                           long_lists=F.long_lists)
         np.save(model.data_dir + 'article_top_k_dedup_index' + split, idx)
         np.save(model.data_dir + 'article_top_k_dedup_score' + split, score)
         out['top_k_dedup' + split] = (idx, score)
@@ -388,7 +395,7 @@ def recommend_top_k_dedup(F, model, enc, enc_v, trL, vlL, histories, targets, em
         print('top %d%s label precision: one per group %.4f  plain %.4f' % (
             F.top_k, split, out['top_k_dedup_precision' + split], emb_out.get('top_k_precision' + split, float('nan'))))
     if histories is not None:
-        idx, score = helpers.recommend(histories, enc, k=F.top_k, groups=groups)
+        idx, score = helpers.recommend(histories, enc, k=F.top_k, groups=groups, long_lists=F.long_lists)
         np.save(model.data_dir + 'user_top_k_dedup_index', idx)
         np.save(model.data_dir + 'user_top_k_dedup_score', score)
         if targets is not None:
@@ -455,7 +462,7 @@ def recommend_users(F, model, enc, histories, targets):
     rate and recall of the held-out reads are returned and printed."""
     from dae_rnn_news_recommendation_b200 import helpers
     print('recommend %d unread articles to %d users' % (F.top_k, histories.shape[0]))
-    idx, score = helpers.recommend(histories, enc, k=F.top_k)
+    idx, score = helpers.recommend(histories, enc, k=F.top_k, long_lists=F.long_lists)
     np.save(model.data_dir + 'user_top_k_index', idx)
     np.save(model.data_dir + 'user_top_k_score', score)
     out = {}
@@ -507,7 +514,7 @@ def recommend_users_gru(F, model, enc, seqs, impressions=(None, None)):
     if train_imp is not None:
         print('impressions: %(used)d used, %(skipped)d skipped' % gru.impression_counts)
     gru.save(model.data_dir + 'user_gru.npz')
-    idx, score = gru.recommend((indptr, items), enc, k=F.top_k)
+    idx, score = gru.recommend((indptr, items), enc, k=F.top_k, long_lists=F.long_lists)
     np.save(model.data_dir + 'user_gru_top_k_index', idx)
     np.save(model.data_dir + 'user_gru_top_k_score', score)
     out = {'user_gru_train_loss': gru.train_loss[-1] if gru.train_loss else float('nan')}
@@ -517,7 +524,7 @@ def recommend_users_gru(F, model, enc, seqs, impressions=(None, None)):
         tg = sp.csr_matrix((np.ones(int(has.sum()), np.float32), (np.flatnonzero(has), targets[has])), shape=(n_u, n))
         hist = history_matrix(indptr, items, n)
         r = helpers.recommendation_recall(idx, tg)
-        m = helpers.recommendation_recall(helpers.recommend(hist, enc, k=F.top_k)[0], tg)
+        m = helpers.recommendation_recall(helpers.recommend(hist, enc, k=F.top_k, long_lists=F.long_lists)[0], tg)
         out.update({'user_gru_hit_rate': r['hit_rate'], 'user_gru_recall': r['recall'], 'user_mean_hit_rate': m['hit_rate'],
                     'user_mean_recall': m['recall']})
         print('users (GRU): hit rate@%d %.4f recall@%d %.4f; mean profile: hit rate@%d %.4f recall@%d %.4f (%d users with targets)'
