@@ -102,6 +102,9 @@ _SIGNATURES = {
     'dae_gru_cell_bwd': (C.c_int, [i32, i32, p, i64, p, i64, p, i64, p, i64, p, p, p, p, i64, p]),
     'dae_seq_negatives': (C.c_int, [p, i64, i32, u64, u64, u64, p, p]),
     'dae_seq_rank_loss': (C.c_int, [p, i64, p, i64, i32, p, p, i64, f32, p, i64, p, p]),
+    # LSTM user encoder
+    'dae_lstm_cell_fwd': (C.c_int, [i32, i32, p, i64, p, i64, p, i64, p, i64, p, i64, i32, p, p, i64, p, i64, p]),
+    'dae_lstm_cell_bwd': (C.c_int, [i32, i32, p, i64, p, i64, p, i64, p, i64, p, i64, p, i64, p, p, i64, p]),
     # impression logs
     'dae_impression_rank_loss': (C.c_int, [p, i64, p, i64, i32, p, i64, p, p, p, f32, p, i64, p, p]),
     'dae_impression_metrics': (C.c_int, [p, i64, p, i64, i32, i32, p, p, p, i64, p, p, p]),

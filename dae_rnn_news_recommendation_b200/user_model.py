@@ -24,6 +24,11 @@ Parameters: one flat fp32 buffer theta = [W~_hh (3H x (H+1)) | W~_ih (3H x (H+1)
 Impression logs (DESIGN 4.13): fit(..., impressions=...) trains on the shown-but-not-clicked articles of each impression
 (dae_impression_rank_loss in place of the two random-negative kernels), impression_states gives the query vector before each
 impression and prefix_histories the reads before it for the mean-profile baseline.
+
+UserLSTM (DESIGN 4.15) is the same encoder with torch.nn.LSTM's cell (gate order i, f, g, o; state_dict loads into a CPU
+torch.nn.LSTM(H, H)): the same constructor, losses, negatives, batches and methods, with 4H-wide projections and
+dae_lstm_cell_fwd / dae_lstm_cell_bwd in place of the GRU's cell kernels.  Both derive from _UserRNN, which holds everything
+that does not depend on the cell.
 """
 import numpy as np
 import torch
@@ -198,25 +203,34 @@ class Packed:
         return int(self.off[t] + i)
 
 
-class UserGRU:
-    """GRU user encoder over reading sequences; see the module docstring."""
+class _UserRNN:
+    """What the recurrent user encoders share (UserGRU, UserLSTM): the flat parameters theta = [W~_hh | W~_ih] of GATES H rows each,
+    the packed training batch, the fit loop, the step loop of transform and impression_states, recommend, save and load.  A cell
+    class supplies GATES, its extra buffers, the carries its backward zeroes, the packed gradient operands of the two weight GEMMs
+    and its two kernel calls (_cell_fwd / _cell_bwd for training, _step for inference)."""
+    GATES = 0
+    _STATES = ('h',)                 # [B x H] inference states, zero at a batch's first step
+    _CARRIES = ('carry',)            # [B x H] backward carries zeroed for the rows of step 0
+    _DGRAD = ('dHP_hl', 'dXP_hl')    # packed gradient operands of [dW_hh | db_hh] and [dW_ih | db_ih]
+    _CARRY_ACCUMULATE = 1            # the carry GEMM dh_{t-1} (+)= dHP_t . W_hh accumulates onto the cell's carry, or stores
 
     def __init__(self, dim, max_len=50, batch_users=1024, num_epochs=5, opt='adam', learning_rate=1e-3, seed=0, device='cuda:0',
                  momentum=0.5):
+        name = type(self).__name__
         if dim < 1 or max_len < 1 or batch_users < 1 or num_epochs < 0:
-            raise ValueError('UserGRU: dim, max_len and batch_users must be >= 1 and num_epochs >= 0')
+            raise ValueError('%s: dim, max_len and batch_users must be >= 1 and num_epochs >= 0' % name)
         if opt not in _cabi.OPT:
-            raise ValueError('UserGRU: opt = %r, one of %s' % (opt, sorted(_cabi.OPT)))
+            raise ValueError('%s: opt = %r, one of %s' % (name, opt, sorted(_cabi.OPT)))
         self.dim, self.max_len, self.batch_users, self.num_epochs = int(dim), int(max_len), int(batch_users), int(num_epochs)
         self.opt, self.learning_rate, self.momentum, self.seed = opt, float(learning_rate), float(momentum), int(seed)
         self.device = torch.device(device)
         self.train_loss = []
         self.steps = 0
         self.epochs_done = 0
-        H = self.dim
-        self.nW = 3 * H * (H + 1)
-        self.ldx, self.ldg = _ld8(H + 1), _ld8(3 * H)
-        # torch.nn.GRU's initialisation: every parameter uniform in [-1/sqrt(H), 1/sqrt(H)]
+        H, G = self.dim, self.GATES
+        self.nW = G * H * (H + 1)
+        self.ldx, self.ldg = _ld8(H + 1), _ld8(G * H)
+        # torch.nn.GRU's and torch.nn.LSTM's initialisation: every parameter uniform in [-1/sqrt(H), 1/sqrt(H)]
         rng = np.random.default_rng(self.seed)
         k = 1.0 / np.sqrt(H)
         self.theta = torch.from_numpy(rng.uniform(-k, k, 2 * self.nW).astype(np.float32)).to(self.device)
@@ -224,7 +238,7 @@ class UserGRU:
         self.slot1 = torch.full_like(self.theta, 0.1 if opt == 'ada_grad' else 0.0)
         self.slot2 = torch.zeros_like(self.theta)
         bf = dict(dtype=torch.bfloat16, device=self.device)
-        self.W_hl = {g: (torch.zeros(3 * H, self.ldx, **bf), torch.zeros(3 * H, self.ldx, **bf)) for g in ('hh', 'ih')}
+        self.W_hl = {g: (torch.zeros(G * H, self.ldx, **bf), torch.zeros(G * H, self.ldx, **bf)) for g in ('hh', 'ih')}
         self._hh_valid = False
         self._buf = {}
         self._cap = (0, 0)
@@ -233,30 +247,30 @@ class UserGRU:
 
     # ---- parameters -------------------------------------------------------------------------------------------------------
     def _theta(self, g):
-        """W~_g = [W_g | b_g] as a [3H, H+1] view of theta (g = 'hh' or 'ih')."""
+        """W~_g = [W_g | b_g] as a [GATES H, H+1] view of theta (g = 'hh' or 'ih')."""
         o = 0 if g == 'hh' else self.nW
-        return self.theta[o:o + self.nW].view(3 * self.dim, self.dim + 1)
+        return self.theta[o:o + self.nW].view(self.GATES * self.dim, self.dim + 1)
 
     def state_dict(self):
-        """torch.nn.GRU(H, H)'s parameter names and shapes (CPU fp32 tensors)."""
+        """torch.nn.GRU(H, H)'s / torch.nn.LSTM(H, H)'s parameter names and shapes (CPU fp32 tensors)."""
         ih, hh = self._theta('ih').cpu(), self._theta('hh').cpu()
         H = self.dim
         return {'weight_ih_l0': ih[:, :H].clone(), 'weight_hh_l0': hh[:, :H].clone(), 'bias_ih_l0': ih[:, H].clone(),
                 'bias_hh_l0': hh[:, H].clone()}
 
     def load_state_dict(self, sd):
-        H = self.dim
-        want = {'weight_ih_l0': (3 * H, H), 'weight_hh_l0': (3 * H, H), 'bias_ih_l0': (3 * H,), 'bias_hh_l0': (3 * H,)}
+        H, GH, name = self.dim, self.GATES * self.dim, type(self).__name__
+        want = {'weight_ih_l0': (GH, H), 'weight_hh_l0': (GH, H), 'bias_ih_l0': (GH,), 'bias_hh_l0': (GH,)}
         missing = set(want) - set(sd)
         if missing:
-            raise ValueError('UserGRU.load_state_dict: missing %s' % sorted(missing))
+            raise ValueError('%s.load_state_dict: missing %s' % (name, sorted(missing)))
         a = {}
-        for name, shape in want.items():
-            v = sd[name]
+        for k, shape in want.items():
+            v = sd[k]
             v = v.detach().cpu().numpy() if isinstance(v, torch.Tensor) else np.asarray(v)
             if tuple(v.shape) != shape:
-                raise ValueError('UserGRU.load_state_dict: %s has shape %s, %s expected (H = %d)' % (name, tuple(v.shape), shape, H))
-            a[name] = v.astype(np.float32)
+                raise ValueError('%s.load_state_dict: %s has shape %s, %s expected (H = %d)' % (name, k, tuple(v.shape), shape, H))
+            a[k] = v.astype(np.float32)
         for g in ('ih', 'hh'):
             t = np.concatenate([a['weight_%s_l0' % g], a['bias_%s_l0' % g][:, None]], 1)
             self._theta(g).copy_(torch.from_numpy(t))
@@ -271,7 +285,8 @@ class UserGRU:
 
     @classmethod
     def load(cls, path, **kw):
-        """A model from save()'s .npz; keyword arguments as the constructor's (dim and max_len come from the file)."""
+        """A model from save()'s .npz; keyword arguments as the constructor's (dim and max_len come from the file).  The parameter
+        shapes tell the cells apart: another cell's file fails load_state_dict's shape check."""
         z = np.load(path)
         kw.setdefault('max_len', int(z['max_len']))
         m = cls(int(z['weight_hh_l0'].shape[1]), **kw)
@@ -295,7 +310,7 @@ class UserGRU:
 
     def _split(self, g):
         hi, lo = self.W_hl[g]
-        call('dae_split_bf16', self._theta(g).data_ptr(), 3 * self.dim, self.dim + 1, self.dim + 1, hi.data_ptr(), lo.data_ptr(),
+        call('dae_split_bf16', self._theta(g).data_ptr(), self.GATES * self.dim, self.dim + 1, self.dim + 1, hi.data_ptr(), lo.data_ptr(),
              self.ldx, -1, 1.0, _stream())
 
     def _mark(self, name):
@@ -309,21 +324,20 @@ class UserGRU:
         if P <= self._cap[0] and B <= self._cap[1]:
             return self._buf
         P, B = max(P, self._cap[0]), max(B, self._cap[1])
-        H, d = self.dim, self.device
+        H, GH, d = self.dim, self.GATES * self.dim, self.device
         f32, bf, i32 = dict(dtype=torch.float32, device=d), dict(dtype=torch.bfloat16, device=d), dict(dtype=torch.int32, device=d)
         self._buf = None
         torch.cuda.empty_cache()
         b = {'neg': torch.empty(P, **i32),
              'X_hl': (torch.empty(P, self.ldx, **bf), torch.empty(P, self.ldx, **bf)),
-             'XP': torch.empty(P, 3 * H, **f32),
+             'XP': torch.empty(P, GH, **f32),
              'Hp_hl': (torch.zeros(P, self.ldx, **bf), torch.zeros(P, self.ldx, **bf)),   # [h_{t-1} | 1] of every position
-             'HP': torch.empty(B, 3 * H, **f32),
+             'HP': torch.empty(B, GH, **f32),
              'Hs': torch.empty(P, H, **f32),
              'gates': torch.empty(P, 4 * H, **f32),
              'dH': torch.empty(P, H, **f32),
-             'carry': torch.empty(B, H, **f32),
-             'dXP_hl': (torch.empty(P, self.ldg, **bf), torch.empty(P, self.ldg, **bf)),
-             'dHP_hl': (torch.empty(P, self.ldg, **bf), torch.empty(P, self.ldg, **bf))}
+             'carry': torch.empty(B, H, **f32)}
+        b.update(self._cell_buffers(P, B))
         b['Hp_hl'][0][:, H] = 1.0
         self._buf, self._cap = b, (P, B)
         return b
@@ -332,7 +346,7 @@ class UserGRU:
     def _forward_backward(self, pk, emb, epoch, batch, ib=None):
         """Loss (added to self.stats) and the gradient (self.grad) of one packed batch with pk.terms > 0, or with ib (an
         ImpressionBatch with ib.n > 0) the impression loss of its impressions in place of the random negatives."""
-        H, P, T = self.dim, pk.P, len(pk.n)
+        H, GH, P, T = self.dim, self.GATES * self.dim, pk.P, len(pk.n)
         b = self._buffers(P, pk.B)
         st = _stream()
         items = _upload(pk.items, self.device)
@@ -350,22 +364,18 @@ class UserGRU:
         call('dae_gather_split_bf16', emb.data_ptr(), emb.stride(0), items.data_ptr(), P, H, X_hi.data_ptr(), X_lo.data_ptr(), self.ldx,
              H, st)
         self._split('ih')
-        self._gemm(P, 3 * H, H + 1, b['X_hl'], 0, self.W_hl['ih'], 0, b['XP'], 3 * H)
+        self._gemm(P, GH, H + 1, b['X_hl'], 0, self.W_hl['ih'], 0, b['XP'], GH)
         self._mark('input_projection')
         Hp_hi, Hp_lo = b['Hp_hl']
         n0 = int(pk.n[0])
         Hp_hi[:n0, :H].zero_()
         Hp_lo[:n0].zero_()
-        Hs, XP, HP, G = b['Hs'], b['XP'], b['HP'], b['gates']
+        Hs, HP = b['Hs'], b['HP']
         for t in range(T):
             o, n = int(pk.off[t]), int(pk.n[t])
             n_next = int(pk.n[t + 1]) if t + 1 < T else 0
-            self._gemm(n, 3 * H, H + 1, (Hp_hi[o:], Hp_lo[o:]), 0, self.W_hl['hh'], 0, HP, 3 * H)
-            hprev = Hs[int(pk.off[t - 1]):].data_ptr() if t else None
-            nx = int(pk.off[t + 1])
-            call('dae_gru_cell_fwd', n, H, XP[o:].data_ptr(), 3 * H, HP.data_ptr(), 3 * H, hprev, H, Hs[o:].data_ptr(), H, n_next,
-                 Hp_hi[nx:].data_ptr() if n_next else None, Hp_lo[nx:].data_ptr() if n_next else None, self.ldx, G[o:].data_ptr(),
-                 4 * H, st)
+            self._gemm(n, GH, H + 1, (Hp_hi[o:], Hp_lo[o:]), 0, self.W_hl['hh'], 0, HP, GH)
+            self._cell_fwd(b, pk, t, n_next, st)
         self._mark('forward_recurrence')
         if ib is None:
             call('dae_seq_rank_loss', Hs.data_ptr(), H, emb.data_ptr(), emb.stride(0), H, nxt.data_ptr(), b['neg'].data_ptr(), P,
@@ -375,20 +385,21 @@ class UserGRU:
                  imp_indptr.data_ptr(), imp_items.data_ptr(), imp_clicked.data_ptr(), 1.0 / ib.n, b['dH'].data_ptr(), H,
                  self.stats.data_ptr(), st)
         self._mark('loss')
-        carry, dH = b['carry'], b['dH']
-        carry[:n0].zero_()
-        (dX_hi, dX_lo), (dP_hi, dP_lo) = b['dXP_hl'], b['dHP_hl']
+        # rows [n_t, n_{t-1}) of the carries belong to users whose last read is at t - 1: nothing flows into them from later steps,
+        # and no later step writes them (step t' > t - 1 writes rows [0, n_t') only), so zeroing rows [0, n_0) once keeps them zero
+        for k in self._CARRIES:
+            b[k][:n0].zero_()
+        carry = b['carry']
+        dP_hi, dP_lo = b[self._DGRAD[0]]
         for t in range(T - 1, -1, -1):
             o, n = int(pk.off[t]), int(pk.n[t])
-            hprev = Hs[int(pk.off[t - 1]):].data_ptr() if t else None
-            call('dae_gru_cell_bwd', n, H, dH[o:].data_ptr(), H, carry.data_ptr(), H, G[o:].data_ptr(), 4 * H, hprev, H,
-                 dX_hi[o:].data_ptr(), dX_lo[o:].data_ptr(), dP_hi[o:].data_ptr(), dP_lo[o:].data_ptr(), self.ldg, st)
+            self._cell_bwd(b, pk, t, st)
             if t:   # h_{-1} = 0 is a constant: no carry below step 0
-                self._gemm(n, H, 3 * H, (dP_hi[o:], dP_lo[o:]), 0, self.W_hl['hh'], 1, carry, H, accumulate=1)
+                self._gemm(n, H, GH, (dP_hi[o:], dP_lo[o:]), 0, self.W_hl['hh'], 1, carry, H, accumulate=self._CARRY_ACCUMULATE)
         self._mark('backward_recurrence')
         g_hh, g_ih = self.grad[:self.nW], self.grad[self.nW:]
-        self._gemm(3 * H, H + 1, P, b['dHP_hl'], 1, b['Hp_hl'], 1, g_hh, H + 1, k_splits=-1)
-        self._gemm(3 * H, H + 1, P, b['dXP_hl'], 1, b['X_hl'], 1, g_ih, H + 1, k_splits=-1)
+        self._gemm(GH, H + 1, P, b[self._DGRAD[0]], 1, b['Hp_hl'], 1, g_hh, H + 1, k_splits=-1)
+        self._gemm(GH, H + 1, P, b[self._DGRAD[1]], 1, b['X_hl'], 1, g_ih, H + 1, k_splits=-1)
         self._mark('weight_gradients')
 
     def _optimizer_step(self):
@@ -396,7 +407,7 @@ class UserGRU:
         hi, lo = self.W_hl['hh']
         call('dae_optimizer_step', self.theta.data_ptr(), self.grad.data_ptr(), self.slot1.data_ptr(), self.slot2.data_ptr(),
              2 * self.nW, _cabi.OPT[self.opt], self.learning_rate, self.momentum, 1.0, self.steps, None, hi.data_ptr(), lo.data_ptr(),
-             3 * self.dim, self.dim + 1, self.ldx, _stream())
+             self.GATES * self.dim, self.dim + 1, self.ldx, _stream())
         self._hh_valid = True
         self._mark('optimizer')
 
@@ -418,11 +429,12 @@ class UserGRU:
         max_len reads (time > len - min(len, max_len)); impression_counts gets {'used', 'skipped'}.  The batches permute the
         users with a usable impression as batches() does; one impression with one click at time t on read t + 1 and one
         non-click is exactly the random-negative term at position t."""
-        emb = self._embeddings(embeddings, 'UserGRU.fit')
-        indptr, items = check_sequences(sequences, emb.shape[0], 'UserGRU.fit')
+        fn = '%s.fit' % type(self).__name__
+        emb = self._embeddings(embeddings, fn)
+        indptr, items = check_sequences(sequences, emb.shape[0], fn)
         imp = active = use = None
         if impressions is not None:
-            imp = check_impressions(impressions, emb.shape[0], 'UserGRU.fit', indptr)
+            imp = check_impressions(impressions, emb.shape[0], fn, indptr)
             use = usable_impressions(imp, indptr, self.max_len)
             active = np.unique(imp['user'][use])
             self.impression_counts = {'used': int(use.sum()), 'skipped': int(use.size - use.sum())}
@@ -448,41 +460,60 @@ class UserGRU:
         return self
 
     # ---- inference --------------------------------------------------------------------------------------------------------
-    def transform(self, sequences, embeddings, to_host=True):
-        """User vectors [U, H] fp32: the state after each user's last (truncated) read; zero rows for users without reads.  Projects
-        step by step, so device memory per batch is O(batch_users x 3H), not O(positions x 3H)."""
-        emb = self._embeddings(embeddings, 'UserGRU.transform')
-        indptr, items = check_sequences(sequences, emb.shape[0], 'UserGRU.transform')
-        H, U, B, d, st = self.dim, len(indptr) - 1, self.batch_users, self.device, _stream()
-        out = torch.zeros(U, H, dtype=torch.float32, device=d)
+    def _step_buffers(self, B):
+        """transform / impression_states' buffers for batches of up to B users: O(B x GATES H) device memory.  Also refreshes the
+        bf16 hi / lo copies of W~_hh (when stale) and W~_ih that the steps read."""
+        H, GH, d = self.dim, self.GATES * self.dim, self.device
         if not self._hh_valid:
             self._split('hh')
             self._hh_valid = True
         self._split('ih')
         bf = dict(dtype=torch.bfloat16, device=d)
-        X_hi, X_lo = torch.zeros(B, self.ldx, **bf), torch.zeros(B, self.ldx, **bf)
-        h_hi, h_lo = torch.zeros(B, self.ldx, **bf), torch.zeros(B, self.ldx, **bf)
-        XP = torch.empty(B, 3 * H, dtype=torch.float32, device=d)
-        HP = torch.empty_like(XP)
-        h = torch.empty(B, H, dtype=torch.float32, device=d)
+        s = {'X_hl': (torch.zeros(B, self.ldx, **bf), torch.zeros(B, self.ldx, **bf)),
+             'h_hl': (torch.zeros(B, self.ldx, **bf), torch.zeros(B, self.ldx, **bf)),
+             'XP': torch.empty(B, GH, dtype=torch.float32, device=d),
+             'HP': torch.empty(B, GH, dtype=torch.float32, device=d),
+             'h': torch.empty(B, H, dtype=torch.float32, device=d)}
+        s.update(self._cell_step_buffers(B))
+        return s
+
+    def _steps(self, pk, emb, s, after=None):
+        """Run one packed batch from zero states, step by step: the input projection of the step's reads, the recurrent GEMM and the
+        cell, which updates s['h'] (and the cell's other states) in place.  after(t), if given, runs after step t."""
+        H, GH, st = self.dim, self.GATES * self.dim, _stream()
+        it = _upload(pk.items, self.device)
+        h_hi, h_lo = s['h_hl']
+        h_hi.zero_()
+        h_lo.zero_()
+        h_hi[:, H] = 1.0
+        for k in self._STATES:
+            s[k][:pk.B].zero_()
+        X_hi, X_lo = s['X_hl']
+        for t in range(len(pk.n)):
+            o, n = int(pk.off[t]), int(pk.n[t])
+            call('dae_gather_split_bf16', emb.data_ptr(), emb.stride(0), it[o:].data_ptr(), n, H, X_hi.data_ptr(), X_lo.data_ptr(),
+                 self.ldx, H, st)
+            self._gemm(n, GH, H + 1, (X_hi, X_lo), 0, self.W_hl['ih'], 0, s['XP'], GH)
+            self._gemm(n, GH, H + 1, (h_hi, h_lo), 0, self.W_hl['hh'], 0, s['HP'], GH)
+            self._step(s, n, st)
+            if after is not None:
+                after(t)
+
+    def transform(self, sequences, embeddings, to_host=True):
+        """User vectors [U, H] fp32: the state h after each user's last (truncated) read; zero rows for users without reads.
+        Projects step by step, so device memory per batch is O(batch_users x GATES H), not O(positions x GATES H)."""
+        fn = '%s.transform' % type(self).__name__
+        emb = self._embeddings(embeddings, fn)
+        indptr, items = check_sequences(sequences, emb.shape[0], fn)
+        H, U, B, d = self.dim, len(indptr) - 1, self.batch_users, self.device
+        out = torch.zeros(U, H, dtype=torch.float32, device=d)
+        s = self._step_buffers(B)
         for u0 in range(0, U, B):
             pk = Packed(indptr, items, np.arange(u0, min(U, u0 + B)), self.max_len)
             if pk.B == 0:
                 continue
-            it = _upload(pk.items, d)
-            h_hi.zero_()
-            h_lo.zero_()
-            h_hi[:, H] = 1.0
-            h[:pk.B].zero_()
-            for t in range(len(pk.n)):
-                o, n = int(pk.off[t]), int(pk.n[t])
-                call('dae_gather_split_bf16', emb.data_ptr(), emb.stride(0), it[o:].data_ptr(), n, H, X_hi.data_ptr(), X_lo.data_ptr(),
-                     self.ldx, H, st)
-                self._gemm(n, 3 * H, H + 1, (X_hi, X_lo), 0, self.W_hl['ih'], 0, XP, 3 * H)
-                self._gemm(n, 3 * H, H + 1, (h_hi, h_lo), 0, self.W_hl['hh'], 0, HP, 3 * H)
-                call('dae_gru_cell_fwd', n, H, XP.data_ptr(), 3 * H, HP.data_ptr(), 3 * H, h.data_ptr(), H, h.data_ptr(), H, n,
-                     h_hi.data_ptr(), h_lo.data_ptr(), self.ldx, None, 0, st)
-            out.index_copy_(0, torch.from_numpy(pk.order).to(d), h[:pk.B])
+            self._steps(pk, emb, s)
+            out.index_copy_(0, torch.from_numpy(pk.order).to(d), s['h'][:pk.B])
         return out.cpu().numpy() if to_host else out
 
     def impression_states(self, sequences, embeddings, impressions, to_host=True):
@@ -493,11 +524,12 @@ class UserGRU:
         read len - max_len whatever the impression's time; here the window ENDS at the impression.  The two agree at time = len
         and for users with at most max_len reads.  Each (user, window start) pair is one run of transform's step
         loop, whose states are copied out at the steps that impressions ask for: a user whose impressions all lie within the first
-        max_len reads costs one run.  Device memory per batch is O(batch_users x 3H), as transform's."""
-        emb = self._embeddings(embeddings, 'UserGRU.impression_states')
-        indptr, items = check_sequences(sequences, emb.shape[0], 'UserGRU.impression_states')
-        imp = check_impressions(impressions, emb.shape[0], 'UserGRU.impression_states', indptr)
-        H, d, st = self.dim, self.device, _stream()
+        max_len reads costs one run.  Device memory per batch is O(batch_users x GATES H), as transform's."""
+        fn = '%s.impression_states' % type(self).__name__
+        emb = self._embeddings(embeddings, fn)
+        indptr, items = check_sequences(sequences, emb.shape[0], fn)
+        imp = check_impressions(impressions, emb.shape[0], fn, indptr)
+        H, d = self.dim, self.device
         n_imp = imp['user'].size
         out = torch.zeros(n_imp, H, dtype=torch.float32, device=d)
         ids = np.flatnonzero(imp['time'] > 0)
@@ -518,16 +550,8 @@ class UserGRU:
         r_items = items[np.repeat(r_src - r_indptr[:-1], run_len) + np.arange(int(r_indptr[-1]))]
         step = t - start - 1   # the step after which impression ids[j] reads its run's state
         B = self.batch_users
-        if not self._hh_valid:
-            self._split('hh')
-            self._hh_valid = True
-        self._split('ih')
-        bf = dict(dtype=torch.bfloat16, device=d)
-        X_hi, X_lo = torch.zeros(B, self.ldx, **bf), torch.zeros(B, self.ldx, **bf)
-        h_hi, h_lo = torch.zeros(B, self.ldx, **bf), torch.zeros(B, self.ldx, **bf)
-        XP = torch.empty(B, 3 * H, dtype=torch.float32, device=d)
-        HP = torch.empty_like(XP)
-        h = torch.empty(B, H, dtype=torch.float32, device=d)
+        s = self._step_buffers(B)
+        h = s['h']
         order = np.argsort(run_of, kind='stable')
         for r0 in range(0, n_run, B):
             pk = Packed(r_indptr, r_items, np.arange(r0, min(n_run, r0 + B)), self.max_len)
@@ -540,37 +564,118 @@ class UserGRU:
             cap_step, cap = cap_step[o], np.stack([cap_row[o], cap_imp[o]])
             bounds = np.searchsorted(cap_step, np.arange(len(pk.n) + 1))
             cap_d = _upload(np.ascontiguousarray(cap), d)
-            it = _upload(pk.items, d)
-            h_hi.zero_()
-            h_lo.zero_()
-            h_hi[:, H] = 1.0
-            h[:pk.B].zero_()
-            for tt in range(len(pk.n)):
-                o_, n = int(pk.off[tt]), int(pk.n[tt])
-                call('dae_gather_split_bf16', emb.data_ptr(), emb.stride(0), it[o_:].data_ptr(), n, H, X_hi.data_ptr(), X_lo.data_ptr(),
-                     self.ldx, H, st)
-                self._gemm(n, 3 * H, H + 1, (X_hi, X_lo), 0, self.W_hl['ih'], 0, XP, 3 * H)
-                self._gemm(n, 3 * H, H + 1, (h_hi, h_lo), 0, self.W_hl['hh'], 0, HP, 3 * H)
-                call('dae_gru_cell_fwd', n, H, XP.data_ptr(), 3 * H, HP.data_ptr(), 3 * H, h.data_ptr(), H, h.data_ptr(), H, n,
-                     h_hi.data_ptr(), h_lo.data_ptr(), self.ldx, None, 0, st)
+
+            def capture(tt, bounds=bounds, cap_d=cap_d):
                 a, b = int(bounds[tt]), int(bounds[tt + 1])
                 if b > a:
                     out.index_copy_(0, cap_d[1, a:b], h.index_select(0, cap_d[0, a:b]))
+            self._steps(pk, emb, s, capture)
         return out.cpu().numpy() if to_host else out
 
     def recommend(self, sequences, embeddings, k=10, candidates=None, exclude_read=True, metric='linear kernel', to_host=True,
                   groups=None, long_lists=False):
-        """The k best articles per user for the GRU user vectors (helpers.recommend with profiles=transform(...)): every read
+        """The k best articles per user for the learned user vectors (helpers.recommend with profiles=transform(...)): every read
         article (the whole history, not only the last max_len) is excluded with exclude_read, users without reads get padding.
         groups: the articles' group labels, passed to helpers.recommend (at most one article per group, read groups excluded).
         long_lists: passed to helpers.recommend (k up to 1024)."""
         from .helpers import recommend
-        emb = self._embeddings(embeddings, 'UserGRU.recommend')
-        indptr, items = check_sequences(sequences, emb.shape[0], 'UserGRU.recommend')
+        fn = '%s.recommend' % type(self).__name__
+        emb = self._embeddings(embeddings, fn)
+        indptr, items = check_sequences(sequences, emb.shape[0], fn)
         hist = history_matrix(indptr, items, emb.shape[0])
         prof = self.transform((indptr, items), emb, to_host=False)
         return recommend(hist, emb, k=k, candidates=candidates, metric=metric, exclude_read=exclude_read, device=self.device,
                          to_host=to_host, profiles=prof, groups=groups, long_lists=long_lists)
+
+
+class UserGRU(_UserRNN):
+    """GRU user encoder over reading sequences (torch.nn.GRU's cell, gate order r, z, n); see the module docstring.  Its backward
+    writes dXP = [dr^, dz^, dn^] and dHP = [dr^, dz^, r dn^] separately (dHP's n-third differs), and carry <- dh z, onto which the
+    carry GEMM accumulates dHP . W_hh."""
+    GATES = 3
+
+    def _cell_buffers(self, P, B):
+        bf = dict(dtype=torch.bfloat16, device=self.device)
+        return {'dXP_hl': (torch.empty(P, self.ldg, **bf), torch.empty(P, self.ldg, **bf)),
+                'dHP_hl': (torch.empty(P, self.ldg, **bf), torch.empty(P, self.ldg, **bf))}
+
+    def _cell_fwd(self, b, pk, t, n_next, st):
+        H, o, n = self.dim, int(pk.off[t]), int(pk.n[t])
+        Hs, XP, HP, G = b['Hs'], b['XP'], b['HP'], b['gates']
+        Hp_hi, Hp_lo = b['Hp_hl']
+        hprev = Hs[int(pk.off[t - 1]):].data_ptr() if t else None
+        nx = int(pk.off[t + 1])
+        call('dae_gru_cell_fwd', n, H, XP[o:].data_ptr(), 3 * H, HP.data_ptr(), 3 * H, hprev, H, Hs[o:].data_ptr(), H, n_next,
+             Hp_hi[nx:].data_ptr() if n_next else None, Hp_lo[nx:].data_ptr() if n_next else None, self.ldx, G[o:].data_ptr(),
+             4 * H, st)
+
+    def _cell_bwd(self, b, pk, t, st):
+        H, o, n = self.dim, int(pk.off[t]), int(pk.n[t])
+        Hs, dH, G, carry = b['Hs'], b['dH'], b['gates'], b['carry']
+        (dX_hi, dX_lo), (dP_hi, dP_lo) = b['dXP_hl'], b['dHP_hl']
+        hprev = Hs[int(pk.off[t - 1]):].data_ptr() if t else None
+        call('dae_gru_cell_bwd', n, H, dH[o:].data_ptr(), H, carry.data_ptr(), H, G[o:].data_ptr(), 4 * H, hprev, H,
+             dX_hi[o:].data_ptr(), dX_lo[o:].data_ptr(), dP_hi[o:].data_ptr(), dP_lo[o:].data_ptr(), self.ldg, st)
+
+    def _cell_step_buffers(self, B):
+        return {}
+
+    def _step(self, s, n, st):
+        H, h = self.dim, s['h']
+        h_hi, h_lo = s['h_hl']
+        call('dae_gru_cell_fwd', n, H, s['XP'].data_ptr(), 3 * H, s['HP'].data_ptr(), 3 * H, h.data_ptr(), H, h.data_ptr(), H, n,
+             h_hi.data_ptr(), h_lo.data_ptr(), self.ldx, None, 0, st)
+
+
+class UserLSTM(_UserRNN):
+    """LSTM user encoder over reading sequences (DESIGN 4.15): torch.nn.LSTM(H, H)'s cell (one layer, bias, no projection, gate
+    order i, f, g, o), h_0 = c_0 = 0; the user vector is h after the last (truncated) read.  Everything else -- the constructor,
+    the losses and negatives, fit, transform, impression_states, recommend, save / load -- is UserGRU's; theta =
+    [W~_hh (4H x (H+1)) | W~_ih (4H x (H+1))].
+
+    Training keeps c_t of every position (Cs) next to h_t, and the gates [i | f | g | o].  The backward writes one packed gradient
+    dA = [di | df | dg | do]: the pre-activation is XP + HP, so dXP = dHP = dA feeds both weight GEMMs and the carry GEMM.  The cell
+    kernel reads the h carry and the carry GEMM then STORES dh_{t-1}[0, n_t) = dA_t . W_hh over it instead of accumulating: h_{t-1}
+    reaches step t only through HP_t (there is no direct h -> h term, unlike the GRU's z h_{t-1}), so once the cell has read the
+    carry nothing else contributes to it.  The c carry (carry_c <- dc f) is the cell kernel's own."""
+    GATES = 4
+    _STATES = ('h', 'c')
+    _CARRIES = ('carry', 'carry_c')
+    _DGRAD = ('dA_hl', 'dA_hl')
+    _CARRY_ACCUMULATE = 0
+
+    def _cell_buffers(self, P, B):
+        f32, bf = dict(dtype=torch.float32, device=self.device), dict(dtype=torch.bfloat16, device=self.device)
+        return {'Cs': torch.empty(P, self.dim, **f32),
+                'carry_c': torch.empty(B, self.dim, **f32),
+                'dA_hl': (torch.empty(P, self.ldg, **bf), torch.empty(P, self.ldg, **bf))}
+
+    def _cell_fwd(self, b, pk, t, n_next, st):
+        H, o, n = self.dim, int(pk.off[t]), int(pk.n[t])
+        Cs = b['Cs']
+        Hp_hi, Hp_lo = b['Hp_hl']
+        cprev = Cs[int(pk.off[t - 1]):].data_ptr() if t else None
+        nx = int(pk.off[t + 1])
+        call('dae_lstm_cell_fwd', n, H, b['XP'][o:].data_ptr(), 4 * H, b['HP'].data_ptr(), 4 * H, cprev, H, Cs[o:].data_ptr(), H,
+             b['Hs'][o:].data_ptr(), H, n_next, Hp_hi[nx:].data_ptr() if n_next else None, Hp_lo[nx:].data_ptr() if n_next else None,
+             self.ldx, b['gates'][o:].data_ptr(), 4 * H, st)
+
+    def _cell_bwd(self, b, pk, t, st):
+        H, o, n = self.dim, int(pk.off[t]), int(pk.n[t])
+        Cs = b['Cs']
+        dA_hi, dA_lo = b['dA_hl']
+        cprev = Cs[int(pk.off[t - 1]):].data_ptr() if t else None
+        call('dae_lstm_cell_bwd', n, H, b['dH'][o:].data_ptr(), H, b['carry'].data_ptr(), H, b['carry_c'].data_ptr(), H,
+             b['gates'][o:].data_ptr(), 4 * H, Cs[o:].data_ptr(), H, cprev, H, dA_hi[o:].data_ptr(), dA_lo[o:].data_ptr(), self.ldg, st)
+
+    def _cell_step_buffers(self, B):
+        return {'c': torch.empty(B, self.dim, dtype=torch.float32, device=self.device)}
+
+    def _step(self, s, n, st):
+        H, h, c = self.dim, s['h'], s['c']
+        h_hi, h_lo = s['h_hl']
+        call('dae_lstm_cell_fwd', n, H, s['XP'].data_ptr(), 4 * H, s['HP'].data_ptr(), 4 * H, c.data_ptr(), H, c.data_ptr(), H,
+             h.data_ptr(), H, n, h_hi.data_ptr(), h_lo.data_ptr(), self.ldx, None, 0, st)
 
 
 def history_matrix(indptr, items, n_items):

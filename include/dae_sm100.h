@@ -632,6 +632,27 @@ int dae_seq_negatives(const int32_t* pos, int64_t n_pos, int32_t n_items, uint64
 int dae_seq_rank_loss(const float* h, int64_t ld_h, const float* emb, int64_t ld_emb, int32_t H, const int32_t* pos, const int32_t* neg,
                       int64_t n_pos, float scale, float* dh, int64_t ld_dh, double* loss_sum, void* stream);
 
+/* ---- LSTM user encoder over reading sequences (DESIGN 4.15) ----------------------------------------------------------------
+ * The packed layout and the GEMMs are the GRU's above; the cell is torch.nn.LSTM's (gate order i, f, g, o) with XP and HP 4H wide:
+ * i = s(xi + hi), f = s(xf + hf), g = tanh(xg + hg), o = s(xo + ho), c_t = f c_{t-1} + i g, h_t = o tanh(c_t).
+ * dae_lstm_cell_fwd: one step for rows [0, n) from XP (ld_xp >= 4H), HP (ld_hp >= 4H) and c_prev (NULL: c_{t-1} = 0).  Writes c_out
+ *   and h_out (fp32); c_out may equal c_prev (then ld_c == ld_cprev).  h_{t-1} is not read (it enters through HP), so h_out may be
+ *   the buffer the step's GEMM operand came from.  Rows i < n_split of h also go to h_hi / h_lo [.. x ld_split] (the next step's
+ *   GEMM operand) when h_hi is non-NULL; gates (optional, ld_gates >= 4H) <- [i | f | g | o], what dae_lstm_cell_bwd needs with
+ *   c_t and c_{t-1}.
+ * dae_lstm_cell_bwd: one step backward for rows [0, n): dh = carry_h + dh_in (dh_in optional), dc = carry_c + dh o (1 - tanh^2 c_t)
+ *   with c = c_t and c_prev = c_{t-1} (NULL: 0).  Writes dA = [di, df, dg, do] (the pre-activation gradient, which is both dXP and
+ *   dHP) as bf16 hi / lo rows (ld_da >= 4H) and carry_c <- dc f.  carry_h is read only: the caller then STORES
+ *   dh_{t-1}[0, n) = dA . W_hh over it (there is no direct h -> h term).  Rows [n_t, n_{t-1}) of both carries must be zero when
+ *   step t - 1 starts: those users' last read is at t - 1.
+ */
+int dae_lstm_cell_fwd(int32_t n, int32_t H, const float* xp, int64_t ld_xp, const float* hp, int64_t ld_hp, const float* c_prev,
+                      int64_t ld_cprev, float* c_out, int64_t ld_c, float* h_out, int64_t ld_h, int32_t n_split, void* h_hi, void* h_lo,
+                      int64_t ld_split, float* gates, int64_t ld_gates, void* stream);
+int dae_lstm_cell_bwd(int32_t n, int32_t H, const float* dh_in, int64_t ld_dh_in, const float* carry_h, int64_t ld_carry_h,
+                      float* carry_c, int64_t ld_carry_c, const float* gates, int64_t ld_gates, const float* c, int64_t ld_c,
+                      const float* c_prev, int64_t ld_cprev, void* da_hi, void* da_lo, int64_t ld_da, void* stream);
+
 /* ---- impression logs (DESIGN 4.13) ------------------------------------------------------------------------------------------
  * An impression is a list of shown articles items[indptr[i] .. indptr[i + 1]) (rows of emb) with clicked[k] != 0 where the article
  * was clicked; C and N are its clicked and not-clicked articles.  One warp per row of work; lists of any length are walked in

@@ -106,6 +106,9 @@ def build_parser():
                          'the training embeddings, save user_gru.npz and user_gru_top_k_{index,score}.npy; with targets report '
                          'user_gru_hit_rate / user_gru_recall next to the mean profile\'s for the same reads')
     ap.add_argument('--user_epochs', type=int, default=5, help='with --user_sequences: training epochs of the GRU user encoder')
+    ap.add_argument('--user_cell', default='gru', choices=['gru', 'lstm'],
+                    help='with --user_sequences: the user encoder\'s recurrent cell, user_model.UserGRU (gru, the default) or '
+                         'user_model.UserLSTM (lstm); with lstm the files and keys say user_lstm in place of user_gru')
     ap.add_argument('--user_impressions', default='',
                     help='with --user_sequences: an .npz impression log (user, time, indptr, items, clicked; see '
                          'user_model.check_impressions) to train the GRU on instead of random negatives')
@@ -496,28 +499,31 @@ def load_user_impressions(F, n_train, seqs):
     return tuple(out)
 
 
-def recommend_users_gru(F, model, enc, seqs, impressions=(None, None)):
-    """--user_sequences: train a GRU user encoder on the training embeddings, save it as user_gru.npz and the --top_k best unread
-    articles per user as user_gru_top_k_{index,score}.npy; with targets, the hit rate and recall of the GRU's and of the mean
-    profile's recommendations for the same reads are returned and printed.  impressions: (train, test) from load_user_impressions;
-    the GRU trains on train's impressions when given, and test's are scored by the GRU states and by the mean profiles of the
-    same reads."""
+def recommend_users_sequences(F, model, enc, seqs, impressions=(None, None)):
+    """--user_sequences: train a recurrent user encoder (--user_cell: UserGRU or UserLSTM) on the training embeddings, save it as
+    user_<cell>.npz and the --top_k best unread articles per user as user_<cell>_top_k_{index,score}.npy; with targets, the hit
+    rate and recall of the encoder's and of the mean profile's recommendations for the same reads are returned and printed.
+    impressions: (train, test) from load_user_impressions; the encoder trains on train's impressions when given, and test's are
+    scored by the encoder's states and by the mean profiles of the same reads."""
     import scipy.sparse as sp
     from dae_rnn_news_recommendation_b200 import helpers
-    from dae_rnn_news_recommendation_b200.user_model import UserGRU, history_matrix, prefix_histories
+    from dae_rnn_news_recommendation_b200.user_model import UserGRU, UserLSTM, history_matrix, prefix_histories
     indptr, items, targets = seqs
     train_imp, test_imp = impressions
-    print('train a GRU user encoder on %d users (%d reads, %d epochs%s)' % (len(indptr) - 1, items.size, F.user_epochs,
-                                                                          ', impressions' if train_imp is not None else ''))
-    gru = UserGRU(enc.shape[1], num_epochs=F.user_epochs, seed=max(F.seed, 0))
-    gru.fit((indptr, items), enc, impressions=train_imp)
+    cell = F.user_cell
+    label = cell.upper()
+    print('train a %s user encoder on %d users (%d reads, %d epochs%s)' % (label, len(indptr) - 1, items.size, F.user_epochs,
+                                                                         ', impressions' if train_imp is not None else ''))
+    enc_cls = {'gru': UserGRU, 'lstm': UserLSTM}[cell]
+    rnn = enc_cls(enc.shape[1], num_epochs=F.user_epochs, seed=max(F.seed, 0))
+    rnn.fit((indptr, items), enc, impressions=train_imp)
     if train_imp is not None:
-        print('impressions: %(used)d used, %(skipped)d skipped' % gru.impression_counts)
-    gru.save(model.data_dir + 'user_gru.npz')
-    idx, score = gru.recommend((indptr, items), enc, k=F.top_k, long_lists=F.long_lists)
-    np.save(model.data_dir + 'user_gru_top_k_index', idx)
-    np.save(model.data_dir + 'user_gru_top_k_score', score)
-    out = {'user_gru_train_loss': gru.train_loss[-1] if gru.train_loss else float('nan')}
+        print('impressions: %(used)d used, %(skipped)d skipped' % rnn.impression_counts)
+    rnn.save(model.data_dir + 'user_%s.npz' % cell)
+    idx, score = rnn.recommend((indptr, items), enc, k=F.top_k, long_lists=F.long_lists)
+    np.save(model.data_dir + 'user_%s_top_k_index' % cell, idx)
+    np.save(model.data_dir + 'user_%s_top_k_score' % cell, score)
+    out = {'user_%s_train_loss' % cell: rnn.train_loss[-1] if rnn.train_loss else float('nan')}
     if targets is not None:
         n_u, n = len(indptr) - 1, enc.shape[0]
         has = targets >= 0
@@ -525,18 +531,18 @@ def recommend_users_gru(F, model, enc, seqs, impressions=(None, None)):
         hist = history_matrix(indptr, items, n)
         r = helpers.recommendation_recall(idx, tg)
         m = helpers.recommendation_recall(helpers.recommend(hist, enc, k=F.top_k, long_lists=F.long_lists)[0], tg)
-        out.update({'user_gru_hit_rate': r['hit_rate'], 'user_gru_recall': r['recall'], 'user_mean_hit_rate': m['hit_rate'],
+        out.update({'user_%s_hit_rate' % cell: r['hit_rate'], 'user_%s_recall' % cell: r['recall'], 'user_mean_hit_rate': m['hit_rate'],
                     'user_mean_recall': m['recall']})
-        print('users (GRU): hit rate@%d %.4f recall@%d %.4f; mean profile: hit rate@%d %.4f recall@%d %.4f (%d users with targets)'
-              % (F.top_k, r['hit_rate'], F.top_k, r['recall'], F.top_k, m['hit_rate'], F.top_k, m['recall'], r['users']))
+        print('users (%s): hit rate@%d %.4f recall@%d %.4f; mean profile: hit rate@%d %.4f recall@%d %.4f (%d users with targets)'
+              % (label, F.top_k, r['hit_rate'], F.top_k, r['recall'], F.top_k, m['hit_rate'], F.top_k, m['recall'], r['users']))
     if test_imp is not None:
-        g = helpers.impression_metrics(gru.impression_states((indptr, items), enc, test_imp), enc, test_imp, metric='linear kernel')
+        g = helpers.impression_metrics(rnn.impression_states((indptr, items), enc, test_imp), enc, test_imp, metric='linear kernel')
         prof = helpers.user_profiles(prefix_histories((indptr, items), test_imp, enc.shape[0]), enc)
         m = helpers.impression_metrics(prof, enc, test_imp, metric='cosine')
-        for name, r in (('gru', g), ('mean', m)):
+        for name, r in ((cell, g), ('mean', m)):
             out.update({'user_%s_imp_%s' % (name, k.replace('@', '')): r[k] for k in ('auc', 'mrr', 'ndcg@5', 'ndcg@10')})
-        print('test impressions (GRU): AUC %.4f MRR %.4f nDCG@5 %.4f nDCG@10 %.4f; mean profile: AUC %.4f MRR %.4f nDCG@5 %.4f '
-              'nDCG@10 %.4f (%d scored, %d skipped)' % (g['auc'], g['mrr'], g['ndcg@5'], g['ndcg@10'], m['auc'], m['mrr'],
+        print('test impressions (%s): AUC %.4f MRR %.4f nDCG@5 %.4f nDCG@10 %.4f; mean profile: AUC %.4f MRR %.4f nDCG@5 %.4f '
+              'nDCG@10 %.4f (%d scored, %d skipped)' % (label, g['auc'], g['mrr'], g['ndcg@5'], g['ndcg@10'], m['auc'], m['mrr'],
                                                         m['ndcg@5'], m['ndcg@10'], g['impressions'], g['skipped']))
     return out
 
@@ -583,7 +589,7 @@ def main(argv=None):
         if histories is not None:
             model.evaluation.update(recommend_users(F, model, enc, histories, targets))
         if seqs is not None:
-            model.evaluation.update(recommend_users_gru(F, model, enc, seqs, imps))
+            model.evaluation.update(recommend_users_sequences(F, model, enc, seqs, imps))
         if F.top_k_dedup > 0:
             model.evaluation.update(recommend_top_k_dedup(F, model, enc, enc_v, trL, vlL, histories, targets, model.evaluation))
     if F.dedup_threshold > 0:

@@ -1,6 +1,8 @@
-"""Training and inference speed of the GRU user encoder (user_model.UserGRU), with a torch.nn.GRU (cuDNN) arm.  One JSON line.
+"""Training and inference speed of the GRU or LSTM user encoder (user_model.UserGRU / UserLSTM), with a torch.nn.GRU / torch.nn.LSTM
+(cuDNN) arm.  One JSON line.
 
-    python tools/bench_user_model.py [--n 100000] [--h 500] [--users 32768] [--batch_users 1024,4096] [--transform_users 100000,1000000]
+    python tools/bench_user_model.py [--cell gru|lstm] [--n 100000] [--h 500] [--users 32768] [--batch_users 1024,4096]
+                                     [--transform_users 100000,1000000]
 
 Workload: --n clustered articles of width --h (device resident) and synth.make_sequences users (mean length 20, truncated to the
 last 50 reads: about 18 reads each).  Reported:
@@ -8,8 +10,9 @@ last 50 reads: about 18 reads each).  Reported:
             over the phases of a batch (gather + input GEMM, forward recurrence, loss, backward recurrence, weight GEMMs, optimizer)
             from CUDA events in a separate epoch;
   cudnn[B]: the same batches (the same packed layout as a torch PackedSequence, the same negatives and loss) through
-            torch.nn.GRU in fp32 (cuDNN, TF32 off) with autograd and torch.optim.Adam;
-  transform[U]: UserGRU.transform of U users (batch_users 16384) and its peak device memory above the inputs and the output.
+            torch.nn.GRU (--cell gru, the default) or torch.nn.LSTM (--cell lstm) in fp32 (cuDNN, TF32 off) with autograd and
+            torch.optim.Adam;
+  transform[U]: the encoder's transform of U users (batch_users 16384) and its peak device memory above the inputs and the output.
 Times are CUDA-event or synchronised wall-clock spans around whole epochs / calls.
 """
 import argparse
@@ -24,7 +27,9 @@ sys.path.insert(0, ROOT)
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
 from dae_rnn_news_recommendation_b200.synth import make_sequences  # noqa: E402
-from dae_rnn_news_recommendation_b200.user_model import Packed, UserGRU  # noqa: E402
+from dae_rnn_news_recommendation_b200.user_model import Packed, UserGRU, UserLSTM  # noqa: E402
+
+CELLS = {'gru': (UserGRU, torch.nn.GRU), 'lstm': (UserLSTM, torch.nn.LSTM)}
 
 
 def _gpu_info():
@@ -50,7 +55,7 @@ def _epoch(m, indptr, items, emb, epoch, packs=None):
 
 
 def train_arm(args, B, indptr, items, emb):
-    m = UserGRU(args.h, max_len=50, batch_users=B, seed=0)
+    m = CELLS[args.cell][0](args.h, max_len=50, batch_users=B, seed=0)
     _epoch(m, indptr, items, emb, 0)                      # warm-up (buffers, module loads)
     packs = [Packed(indptr, items, u, m.max_len) for u in m.batches(indptr, 1)]   # host packing outside the timed span
     sec, pos, users, _ = _epoch(m, indptr, items, emb, 1, packs)
@@ -71,7 +76,7 @@ def train_arm(args, B, indptr, items, emb):
 def cudnn_arm(args, packs, emb, m_ref):
     torch.backends.cudnn.allow_tf32 = False
     H = args.h
-    g = torch.nn.GRU(H, H).cuda()
+    g = CELLS[args.cell][1](H, H).cuda()
     g.load_state_dict({k: v.cuda() for k, v in m_ref.state_dict().items()})
     opt = torch.optim.Adam(g.parameters(), lr=1e-3)
     negs = []
@@ -121,6 +126,7 @@ def transform_arm(args, m, labels, emb, U):
 
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument('--cell', default='gru', choices=sorted(CELLS))
     ap.add_argument('--n', type=int, default=100000)
     ap.add_argument('--h', type=int, default=500)
     ap.add_argument('--users', type=int, default=32768)
@@ -135,6 +141,8 @@ def main():
     indptr, items, _ = make_sequences(args.users, labels, mean_len=20, seed=1, holdout=False)
     res = {'N': args.n, 'H': args.h, 'train_users': args.users, 'mean_len_truncated': float(np.minimum(np.diff(indptr), 50).mean()),
            'gpu': _gpu_info(), 'device_name': torch.cuda.get_device_name(0), 'train': [], 'cudnn': []}
+    if args.cell != 'gru':   # the default GRU line keeps its keys
+        res['cell'] = args.cell
     m = None
     for B in (int(b) for b in args.batch_users.split(',')):
         r, packs, m = train_arm(args, B, indptr, items, emb)
