@@ -661,7 +661,10 @@ def impression_metrics(vectors, embeddings, impressions, metric='linear kernel',
     (MIND's ndcg_score).  MIND's scripts leave the order of tied scores to argsort; the tie rule above is the only place where
     the ranks may differ from theirs.  The scores and the metrics come from dae_impression_metrics, one warp per impression.
     vectors: [I, H] query vectors (UserGRU.impression_states, or user_profiles of user_model.prefix_histories); embeddings:
-    [N, H]; impressions: a mapping with 'indptr', 'items', 'clicked' (user_model.check_impressions).
+    [N, H]; impressions: a mapping with 'indptr', 'items', 'clicked' (user_model.check_impressions).  Both must be finite with
+    every |x| <= 2^63 / sqrt(H), so that no fp32 sum of the kernel overflows (ValueError otherwise).  Under 'cosine' a non-zero
+    vector whose fp32 squared norm underflows to 0 (every |x| <= 2^-75, about 2.6e-23) scores 0, as a zero vector does, and one
+    whose squared norm is subnormal (below 2^-126) scores without fp32's relative accuracy.
     Returns {'impressions': impressions scored, 'skipped': impressions without a click or without a non-click (left out of the
     means), 'auc', 'mrr', 'ndcg@5', 'ndcg@10': means over the scored ones (NaN when none)}."""
     from .user_model import check_impressions
@@ -676,6 +679,10 @@ def impression_metrics(vectors, embeddings, impressions, metric='linear kernel',
     q = _as_device_dense(vectors, emb.device)
     if not bool(torch.isfinite(emb).all()) or not bool(torch.isfinite(q).all()):
         raise ValueError('impression_metrics: embeddings and vectors must be finite')
+    # |x| <= 2^63 / sqrt(H) keeps every fp32 dot product and squared norm of the kernel below 2^126: no inf, so no NaN score
+    lim = 2.0 ** 63 / math.sqrt(emb.shape[1])
+    if float(emb.abs().max()) > lim or (q.numel() and float(q.abs().max()) > lim):
+        raise ValueError('impression_metrics: embeddings and vectors must lie within 2^63 / sqrt(H) = %.3g in magnitude' % lim)
     _, m = _impression_scores(q, emb, imp, metric)
     m = m.cpu().numpy()
     ok = ~np.isnan(m[:, 0])

@@ -663,7 +663,11 @@ int dae_lstm_cell_bwd(int32_t n, int32_t H, const float* dh_in, int64_t ld_dh_in
  *   to dh_p, where w_n = sum_c s(s_n - s_c) and w_c = -sum_n s(s_n - s_c).  Impressions with |C| = 0 or |N| = 0 add nothing.
  *   EVERY row p < n_pos of dh is written (zero without impressions), in a fixed order per row: no atomics on dh.
  * dae_impression_metrics: one query row q_i (ld_q) per impression.  scores[k] (fp32, every k < indptr[n_imp]) = q_i . e(items[k]),
- *   or with cosine = 1 that over |q_i| |e(items[k])| (0 when either is zero).  metrics[i] (fp64 [n_imp x 4]) = AUC, MRR, nDCG@5,
+ *   or with cosine = 1 that over |q_i| |e(items[k])| (0 when either is zero).  The dot products and squared norms are fp32 sums:
+ *   with every |x| <= 2^63 / sqrt(H) they stay below 2^126 and every score is finite (impression_metrics rejects larger
+ *   entries); beyond that a score may be inf or NaN.  A cosine operand whose fp32 squared norm underflows to 0 (every |x| <=
+ *   2^-75) counts as zero and scores 0; a subnormal squared norm gives a finite score without fp32's relative accuracy.
+ *   metrics[i] (fp64 [n_imp x 4]) = AUC, MRR, nDCG@5,
  *   nDCG@10 of those scores: rank_j = #{k: s_k > s_j} + #{k before j: s_k = s_j}; AUC = (#{s_c > s_n} + #{s_c = s_n} / 2) /
  *   (|C| |N|); MRR = mean over C of 1 / (rank + 1); nDCG@K = sum_{c: rank < K} 1 / log2(rank + 2) over its value for the first
  *   min(|C|, K) ranks.  |C| = 0 or |N| = 0: four NaNs.
