@@ -108,6 +108,7 @@ _SIGNATURES = {
     # impression logs
     'dae_impression_rank_loss': (C.c_int, [p, i64, p, i64, i32, p, i64, p, p, p, f32, p, i64, p, p]),
     'dae_impression_metrics': (C.c_int, [p, i64, p, i64, i32, i32, p, p, p, i64, p, p, p]),
+    'dae_impression_softmax_loss': (C.c_int, [p, i64, p, i64, i32, p, i64, p, p, p, p, i32, u64, u64, f32, p, i64, p, p, p]),
     # deterministic training step
     'dae_gemm_det_workspace': (C.c_int, [p]),
     'dae_gemm_bf16x3_det': (C.c_int, [i32, i32, i32, f32, p, p, i64, i32, p, p, i64, i32, p, i64, i32, i32, p, i32, i32, p, i64, p]),

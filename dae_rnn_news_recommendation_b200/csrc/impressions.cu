@@ -1,4 +1,5 @@
-// Impression logs (DESIGN 4.13): the pairwise impression loss of the GRU user encoder and the per-impression ranking metrics.
+// Impression logs (DESIGN 4.13, 4.16): the pairwise and the sampled-softmax impression losses of the user encoders and the
+// per-impression ranking metrics.
 //
 // An impression is a list of shown articles items[indptr[i] .. indptr[i + 1]) with a click flag per article.  Both kernels give
 // one warp to one row of work and score the candidates with warp dot products (lane j takes the columns j, j + 32, ...), so a
@@ -229,6 +230,140 @@ __global__ void __launch_bounds__(kImpWarps * 32) impression_metrics_kernel(
   }
 }
 
+constexpr int kImpMaxNegatives = 32;   // K <= 32: one draw per lane
+
+__device__ __forceinline__ float warp_max(float v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
+  return v;
+}
+
+// Draw d of click r (its ordinal among the impression's clicks) of global impression id: word d & 3 of Philox4x32-10 with key
+// (seed lo, seed hi) and counter (id, r, epoch lo, d >> 2).  It depends on nothing else: not on the batch, the position or the grid.
+__device__ __forceinline__ uint32_t softmax_draw(uint64_t seed, uint64_t epoch, uint32_t id, uint32_t r, int d) {
+  uint32_t c[4] = {id, r, (uint32_t)epoch, (uint32_t)(d >> 2)};
+  uint32_t k[2] = {(uint32_t)seed, (uint32_t)(seed >> 32)};
+#pragma unroll
+  for (int i = 0; i < 10; ++i) philox_round(c, k);
+  const uint32_t lo = (d & 1) ? c[1] : c[0], hi = (d & 1) ? c[3] : c[2];
+  return (d & 2) ? hi : lo;
+}
+
+// One warp per packed position p, its impressions q in [pos_indptr[p], pos_indptr[p + 1]) in that order.  For each click c of a
+// usable impression (|C|, |N| >= 1), with r its ordinal in C: S_c = N if K = 0 or K >= |N|, else K distinct non-clicks by
+// Floyd's algorithm (d = 0 .. K - 1: j = |N| - K + d, t = floor(u_d (j + 1) / 2^32), take j if t is taken, else t; ordinals into N
+// in item order).  *loss_sum += l_c = log(e^{s_c} + sum_{S_c} e^{s_n}) - s_c (max subtracted; fp64 atomics, one per warp) and
+// dh_p += scale sum_c sum_{j in {c} + S_c} (p_cj - [j = c]) e_j.  The weights are summed per candidate first (ws: two 4-byte words
+// per shown article, word 0 the weight, word 1 the non-click list), then each candidate's row is read once, in item order; rows
+// of zero weight are skipped.  With S_c = N the impression is scored once: every click shares T = sum_N e^{s_n - M_N}, so the
+// work is O(m H + |C|).  Otherwise only the click and its K draws are scored, one draw per lane; Floyd's membership test is a
+// warp vote.  The warp owns row p of dh: no atomics on dh, the result does not depend on the schedule.  Launch bounds of 8 CTAs
+// per SM let ptxas use 64 registers; at its default of 48 it spilled the draw loop's state to the stack.
+__global__ void __launch_bounds__(kImpWarps * 32, 8) impression_softmax_loss_kernel(
+    const float* __restrict__ h, int64_t ld_h, const float* __restrict__ emb, int64_t ld_emb, int H, const int64_t* __restrict__ pos_indptr,
+    int64_t n_pos, const int64_t* __restrict__ imp_indptr, const int32_t* __restrict__ items, const uint8_t* __restrict__ clicked,
+    const int64_t* __restrict__ imp_ids, int K, uint64_t seed, uint64_t epoch, float scale, float* __restrict__ dh, int64_t ld_dh,
+    double* __restrict__ loss_sum, float* ws) {
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  const float neg_inf = __int_as_float(0xff800000);
+  double acc = 0.0;
+  for (int64_t p = (int64_t)blockIdx.x * kImpWarps + w; p < n_pos; p += (int64_t)gridDim.x * kImpWarps) {
+    float* d = dh + p * ld_dh;
+    for (int j = lane; j < H; j += 32) d[j] = 0.0f;
+    const float* hp = h + p * ld_h;
+    for (int64_t q = pos_indptr[p]; q < pos_indptr[p + 1]; ++q) {
+      const int64_t b0 = imp_indptr[q];
+      const int m = (int)(imp_indptr[q + 1] - b0);   // < 2^31: an impression's articles are distinct int32 rows
+      const int32_t* it = items + b0;
+      const uint8_t* cl = clicked + b0;
+      const int nc = count_clicked(cl, m, lane), nn = m - nc;
+      if (nc == 0 || nn == 0) continue;
+      float* wq = ws + 2 * b0;                           // wq[2 k]: candidate k's weight
+      int32_t* nq = reinterpret_cast<int32_t*>(ws) + 2 * b0 + 1;   // nq[2 o]: the position of the o-th non-click
+      if (K == 0 || K >= nn) {
+        for (int k = 0; k < m; ++k) {
+          const float v = warp_dot(hp, emb + (int64_t)it[k] * ld_emb, H, lane);
+          if (lane == 0) wq[2 * k] = v;
+        }
+        __syncwarp();
+        float mx = neg_inf;
+        for (int k = lane; k < m; k += 32)
+          if (!cl[k]) mx = fmaxf(mx, wq[2 * k]);
+        const float mn = warp_max(mx);
+        float t = 0.0f;
+        for (int k = lane; k < m; k += 32)
+          if (!cl[k]) t += expf(wq[2 * k] - mn);
+        const float tn = warp_sum(t);
+        float r = 0.0f;
+        for (int k = lane; k < m; k += 32) {
+          if (!cl[k]) continue;
+          const float sc = wq[2 * k], mc = fmaxf(sc, mn), xc = sc - mc, ec = expf(xc), en = expf(mn - mc);
+          const float z = fmaf(en, tn, ec), rz = __fdividef(1.0f, z);
+          acc += (double)(logf(z) - xc);
+          r = fmaf(en, rz, r);
+          wq[2 * k] = fmaf(ec, rz, -1.0f);
+        }
+        const float rn = warp_sum(r);
+        for (int k = lane; k < m; k += 32)
+          if (!cl[k]) wq[2 * k] = expf(wq[2 * k] - mn) * rn;
+      } else {
+        int base = 0;
+        for (int k0 = 0; k0 < m; k0 += 32) {
+          const int k = k0 + lane;
+          const bool nonc = k < m && !cl[k];
+          const unsigned b = __ballot_sync(0xffffffffu, nonc);
+          if (nonc) nq[2 * (base + __popc(b & ((1u << lane) - 1u)))] = k;
+          if (k < m) wq[2 * k] = 0.0f;
+          base += __popc(b);
+        }
+        __syncwarp();
+        const uint32_t id = (uint32_t)imp_ids[q];
+        uint32_t r = 0;
+        for (int k0 = 0; k0 < m; k0 += 32) {
+          for (unsigned bits = __ballot_sync(0xffffffffu, k0 + lane < m && cl[k0 + lane]); bits; bits &= bits - 1u, ++r) {
+            const int c = k0 + __ffs(bits) - 1;
+            const uint32_t u = lane < K ? softmax_draw(seed, epoch, id, r, lane) : 0u;
+            int sel = -1;
+            for (int dd = 0; dd < K; ++dd) {
+              const int j = nn - K + dd;
+              const int t = (int)(((uint64_t)__shfl_sync(0xffffffffu, u, dd) * (uint64_t)(j + 1)) >> 32);
+              const bool taken = __any_sync(0xffffffffu, lane < dd && sel == t);
+              if (lane == dd) sel = taken ? j : t;
+            }
+            const int pos = lane < K ? nq[2 * sel] : 0;
+            float s = 0.0f;
+            for (int dd = 0; dd < K; ++dd) {
+              const float v = warp_dot(hp, emb + (int64_t)it[__shfl_sync(0xffffffffu, pos, dd)] * ld_emb, H, lane);
+              if (lane == dd) s = v;
+            }
+            const float sc = warp_dot(hp, emb + (int64_t)it[c] * ld_emb, H, lane);
+            const float mc = fmaxf(sc, warp_max(lane < K ? s : neg_inf)), xc = sc - mc, ec = expf(xc);
+            const float e = lane < K ? expf(s - mc) : 0.0f;
+            const float z = warp_sum(e) + ec, rz = __fdividef(1.0f, z);
+            if (lane < K) wq[2 * pos] += e * rz;
+            if (lane == 0) {
+              wq[2 * c] = fmaf(ec, rz, -1.0f);
+              acc += (double)(logf(z) - xc);
+            }
+            __syncwarp();
+          }
+        }
+      }
+      __syncwarp();
+      for (int k = 0; k < m; ++k) {
+        const float g = scale * wq[2 * k];
+        if (g == 0.0f) continue;
+        const float* e = emb + (int64_t)it[k] * ld_emb;
+#pragma unroll 1
+        for (int j = lane; j < H; j += 32) d[j] = fmaf(g, e[j], d[j]);
+      }
+      __syncwarp();   // the next impression of this warp may write ws entries that lanes read above
+    }
+  }
+  acc = warp_sum(acc);
+  if (lane == 0 && acc != 0.0) atomicAdd(loss_sum, acc);
+}
+
 static int imp_grid(int64_t rows) {
   const int64_t b = (rows + kImpWarps - 1) / kImpWarps, cap = (int64_t)sm_count() * 16;
   return (int)(b < 1 ? 1 : (b < cap ? b : cap));
@@ -246,6 +381,19 @@ extern "C" int dae_impression_rank_loss(const float* h, int64_t ld_h, const floa
   impression_rank_loss_kernel<<<imp_grid(n_pos), kImpWarps * 32, 0, (cudaStream_t)stream>>>(
       h, ld_h, emb, ld_emb, H, pos_indptr, n_pos, imp_indptr, items, clicked, scale, dh, ld_dh, loss_sum);
   DAE_CHECK_LAUNCH("dae_impression_rank_loss");
+  return DAE_OK;
+}
+
+extern "C" int dae_impression_softmax_loss(const float* h, int64_t ld_h, const float* emb, int64_t ld_emb, int32_t H,
+                                           const int64_t* pos_indptr, int64_t n_pos, const int64_t* imp_indptr, const int32_t* items,
+                                           const uint8_t* clicked, const int64_t* imp_ids, int32_t K, uint64_t seed, uint64_t epoch,
+                                           float scale, float* dh, int64_t ld_dh, double* loss_sum, void* workspace, void* stream) {
+  DAE_REQUIRE(h && emb && pos_indptr && imp_indptr && items && clicked && imp_ids && dh && loss_sum && workspace && H > 0 && n_pos > 0 &&
+              ld_h >= H && ld_emb >= H && ld_dh >= H && K >= 0 && K <= kImpMaxNegatives, "dae_impression_softmax_loss: bad arguments");
+  impression_softmax_loss_kernel<<<imp_grid(n_pos), kImpWarps * 32, 0, (cudaStream_t)stream>>>(
+      h, ld_h, emb, ld_emb, H, pos_indptr, n_pos, imp_indptr, items, clicked, imp_ids, K, seed, epoch, scale, dh, ld_dh, loss_sum,
+      (float*)workspace);
+  DAE_CHECK_LAUNCH("dae_impression_softmax_loss");
   return DAE_OK;
 }
 

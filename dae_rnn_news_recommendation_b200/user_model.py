@@ -25,6 +25,12 @@ Impression logs (DESIGN 4.13): fit(..., impressions=...) trains on the shown-but
 (dae_impression_rank_loss in place of the two random-negative kernels), impression_states gives the query vector before each
 impression and prefix_histories the reads before it for the mean-profile baseline.
 
+Sampled softmax (DESIGN 4.16): with impression_loss='softmax' each click of an impression is one sample, scored against
+impression_negatives = K non-clicks of the same impression drawn per click (all of them with K = 0 or K >= |N|) under a
+(K + 1)-way softmax cross-entropy, the objective of MIND's NRMS / NAML / LSTUR trainers (npratio = 4).  The draws depend only on
+(seed, epoch, impression id, the click's ordinal); dae_impression_softmax_loss replaces dae_impression_rank_loss.  Unlike MIND's
+code, an impression with fewer than K non-clicks is not padded: its clicks are scored against all of them.
+
 UserLSTM (DESIGN 4.15) is the same encoder with torch.nn.LSTM's cell (gate order i, f, g, o; state_dict loads into a CPU
 torch.nn.LSTM(H, H)): the same constructor, losses, negatives, batches and methods, with 4H-wide projections and
 dae_lstm_cell_fwd / dae_lstm_cell_bwd in place of the GRU's cell kernels.  Both derive from _UserRNN, which holds everything
@@ -73,6 +79,8 @@ def check_sequences(sequences, n_items, fn):
 
 
 IMPRESSION_KEYS = ('user', 'time', 'indptr', 'items', 'clicked')
+IMPRESSION_LOSSES = ('pairwise', 'softmax')
+MAX_IMPRESSION_NEGATIVES = 32   # dae_impression_softmax_loss draws one negative per lane
 
 
 def check_impressions(impressions, n_items, fn, seq_indptr=None):
@@ -130,12 +138,20 @@ def usable_impressions(imp, seq_indptr, max_len):
     return (nc > 0) & (nc < n) & (imp['time'] > lens - L) & (imp['time'] >= 1)
 
 
+def _count(impressions):
+    """The impression count len(indptr) - 1 without reading the arrays (0 when malformed: check_impressions reports that)."""
+    try:
+        return len(impressions['indptr']) - 1
+    except (KeyError, TypeError, IndexError, ValueError):
+        return 0
+
+
 class ImpressionBatch:
     """The impressions of one packed training batch (pk: Packed), grouped by packed position.  An impression of user order[i] at
     time t has its state at position off[t'] + i with t' = t - 1 - (len - L).  pos_indptr [P + 1]: position p's impressions are
     [pos_indptr[p], pos_indptr[p + 1]) of this batch's own (indptr, items, clicked), in increasing impression id.  ids: the
-    impression ids in that order.  `buffer` packs the four arrays into one byte buffer for a single upload; `views` cuts the
-    uploaded copy back into typed device tensors."""
+    impression ids in that order; clicks: their click count.  `buffer` packs the four arrays (and with ids=True the ids) into one
+    byte buffer for a single upload; `views` cuts the uploaded copy back into typed device tensors."""
 
     def __init__(self, pk, imp, use, seq_indptr):
         slot = np.full(int(seq_indptr.size - 1), -1, np.int64)
@@ -156,16 +172,19 @@ class ImpressionBatch:
         self.indptr = np.concatenate([[0], np.cumsum(m)]).astype(np.int64)
         src = np.repeat(lo - self.indptr[:-1], m) + np.arange(int(self.indptr[-1]))
         self.items, self.clicked = imp['items'][src], imp['clicked'][src]
+        self.clicks = int(np.count_nonzero(self.clicked))
 
-    def buffer(self):
+    def buffer(self, ids=False):
         parts = [self.pos_indptr.view(np.uint8), self.indptr.view(np.uint8), self.items.view(np.uint8), self.clicked]
+        if ids:
+            parts.append(self.ids.astype(np.int64).view(np.uint8))
         self._sizes = [a.size for a in parts]
         pad = [(-s) % 8 for s in self._sizes]
         return np.concatenate([np.concatenate([a, np.zeros(q, np.uint8)]) for a, q in zip(parts, pad)])
 
     def views(self, dev):
         out, o = [], 0
-        for s, dt in zip(self._sizes, (torch.int64, torch.int64, torch.int32, torch.uint8)):
+        for s, dt in zip(self._sizes, (torch.int64, torch.int64, torch.int32, torch.uint8, torch.int64)):
             out.append(dev[o:o + s].view(dt))
             o += s + (-s) % 8
         return out
@@ -215,12 +234,19 @@ class _UserRNN:
     _CARRY_ACCUMULATE = 1            # the carry GEMM dh_{t-1} (+)= dHP_t . W_hh accumulates onto the cell's carry, or stores
 
     def __init__(self, dim, max_len=50, batch_users=1024, num_epochs=5, opt='adam', learning_rate=1e-3, seed=0, device='cuda:0',
-                 momentum=0.5):
+                 momentum=0.5, impression_loss='pairwise', impression_negatives=4):
         name = type(self).__name__
         if dim < 1 or max_len < 1 or batch_users < 1 or num_epochs < 0:
             raise ValueError('%s: dim, max_len and batch_users must be >= 1 and num_epochs >= 0' % name)
         if opt not in _cabi.OPT:
             raise ValueError('%s: opt = %r, one of %s' % (name, opt, sorted(_cabi.OPT)))
+        if impression_loss not in IMPRESSION_LOSSES:
+            raise ValueError('%s: impression_loss = %r, one of %s' % (name, impression_loss, list(IMPRESSION_LOSSES)))
+        if isinstance(impression_negatives, bool) or not isinstance(impression_negatives, (int, np.integer)) or \
+                not 0 <= impression_negatives <= MAX_IMPRESSION_NEGATIVES:
+            raise ValueError('%s: impression_negatives = %r, an integer in [0, %d] (0: every non-click)'
+                             % (name, impression_negatives, MAX_IMPRESSION_NEGATIVES))
+        self.impression_loss, self.impression_negatives = impression_loss, int(impression_negatives)
         self.dim, self.max_len, self.batch_users, self.num_epochs = int(dim), int(max_len), int(batch_users), int(num_epochs)
         self.opt, self.learning_rate, self.momentum, self.seed = opt, float(learning_rate), float(momentum), int(seed)
         self.device = torch.device(device)
@@ -345,13 +371,16 @@ class _UserRNN:
     # ---- training ---------------------------------------------------------------------------------------------------------
     def _forward_backward(self, pk, emb, epoch, batch, ib=None):
         """Loss (added to self.stats) and the gradient (self.grad) of one packed batch with pk.terms > 0, or with ib (an
-        ImpressionBatch with ib.n > 0) the impression loss of its impressions in place of the random negatives."""
+        ImpressionBatch with ib.n > 0) the impression loss of its impressions in place of the random negatives: pairwise, or with
+        impression_loss='softmax' the sampled softmax over its ib.clicks samples."""
         H, GH, P, T = self.dim, self.GATES * self.dim, pk.P, len(pk.n)
         b = self._buffers(P, pk.B)
         st = _stream()
         items = _upload(pk.items, self.device)
         if ib is None:
             nxt = _upload(pk.nxt, self.device)
+        elif self.impression_loss == 'softmax':
+            pos_indptr, imp_indptr, imp_items, imp_clicked, imp_ids = ib.views(_upload(ib.buffer(ids=True), self.device))
         else:
             pos_indptr, imp_indptr, imp_items, imp_clicked = ib.views(_upload(ib.buffer(), self.device))
         if not self._hh_valid:
@@ -380,6 +409,11 @@ class _UserRNN:
         if ib is None:
             call('dae_seq_rank_loss', Hs.data_ptr(), H, emb.data_ptr(), emb.stride(0), H, nxt.data_ptr(), b['neg'].data_ptr(), P,
                  1.0 / pk.terms, b['dH'].data_ptr(), H, self.stats.data_ptr(), st)
+        elif self.impression_loss == 'softmax':
+            ws = torch.empty(2 * ib.items.size, dtype=torch.int32, device=self.device)   # 8 bytes per shown article
+            call('dae_impression_softmax_loss', Hs.data_ptr(), H, emb.data_ptr(), emb.stride(0), H, pos_indptr.data_ptr(), P,
+                 imp_indptr.data_ptr(), imp_items.data_ptr(), imp_clicked.data_ptr(), imp_ids.data_ptr(), self.impression_negatives,
+                 self.seed, epoch, 1.0 / ib.clicks, b['dH'].data_ptr(), H, self.stats.data_ptr(), ws.data_ptr(), st)
         else:
             call('dae_impression_rank_loss', Hs.data_ptr(), H, emb.data_ptr(), emb.stride(0), H, pos_indptr.data_ptr(), P,
                  imp_indptr.data_ptr(), imp_items.data_ptr(), imp_clicked.data_ptr(), 1.0 / ib.n, b['dH'].data_ptr(), H,
@@ -428,16 +462,30 @@ class _UserRNN:
         impression counts when it has a click and a non-click and its state lies in the trained window of the user's last
         max_len reads (time > len - min(len, max_len)); impression_counts gets {'used', 'skipped'}.  The batches permute the
         users with a usable impression as batches() does; one impression with one click at time t on read t + 1 and one
-        non-click is exactly the random-negative term at position t."""
+        non-click is exactly the random-negative term at position t.
+
+        With impression_loss='softmax' (DESIGN 4.16) each click c of a usable impression is one sample: its loss is
+        log(e^{s_c} + sum_{n in S_c} e^{s_n}) - s_c with S_c = impression_negatives non-clicks of the same impression drawn for
+        that click (every non-click when impression_negatives = 0 or the impression has no more), a batch's loss is the mean
+        over its clicks, train_loss the epoch mean over clicks, and impression_counts also gets 'clicks'.  The log must hold
+        fewer than 2^32 impressions (the draws are keyed by the impression id)."""
         fn = '%s.fit' % type(self).__name__
         emb = self._embeddings(embeddings, fn)
         indptr, items = check_sequences(sequences, emb.shape[0], fn)
         imp = active = use = None
         if impressions is not None:
+            softmax = self.impression_loss == 'softmax'
+            if softmax and _count(impressions) >= 2 ** 32:
+                raise ValueError('%s: impression_loss=\'softmax\' keys its draws by a 32-bit impression id: at most 2^32 - 1 '
+                                 'impressions' % fn)
             imp = check_impressions(impressions, emb.shape[0], fn, indptr)
             use = usable_impressions(imp, indptr, self.max_len)
             active = np.unique(imp['user'][use])
             self.impression_counts = {'used': int(use.sum()), 'skipped': int(use.size - use.sum())}
+            if softmax:
+                ends = imp['indptr']
+                cs = np.concatenate([[0], np.cumsum(imp['clicked'], dtype=np.int64)])
+                self.impression_counts['clicks'] = int((cs[ends[1:]] - cs[ends[:-1]])[use].sum())
         for _ in range(self.num_epochs):
             epoch = self.epochs_done
             self.stats.zero_()
@@ -447,7 +495,7 @@ class _UserRNN:
                 ib = None
                 if imp is not None:
                     ib = ImpressionBatch(pk, imp, use, indptr)
-                    n = ib.n
+                    n = ib.clicks if self.impression_loss == 'softmax' else ib.n
                 else:
                     n = pk.terms
                 if n == 0:   # max_len = 1

@@ -662,6 +662,15 @@ int dae_lstm_cell_bwd(int32_t n, int32_t H, const float* dh_in, int64_t ld_dh_in
  *   l_q = 1 / (|C| |N|) sum_{c, n} softplus(s_n - s_c) to *loss_sum (fp64 atomics) and scale / (|C| |N|) sum_j w_j e(items[j])
  *   to dh_p, where w_n = sum_c s(s_n - s_c) and w_c = -sum_n s(s_n - s_c).  Impressions with |C| = 0 or |N| = 0 add nothing.
  *   EVERY row p < n_pos of dh is written (zero without impressions), in a fixed order per row: no atomics on dh.
+ * dae_impression_softmax_loss (DESIGN 4.16): the sampled-softmax impression loss of a packed batch, arguments as
+ *   dae_impression_rank_loss's plus imp_ids (int64 [pos_indptr[n_pos]]: impression q's global id, < 2^32), K in [0, 32], seed,
+ *   epoch and workspace (8 bytes per shown article: imp_indptr[pos_indptr[n_pos]] x 8 bytes, any contents).  For each click c of
+ *   a usable impression, r its ordinal among the impression's clicks: S_c = N when K = 0 or K >= |N|, else K distinct non-clicks
+ *   by Floyd's algorithm over the ordinals into N in item order (d = 0 .. K - 1: j = |N| - K + d, t = floor(u_d (j + 1) / 2^32);
+ *   j if t is already chosen, else t), u_d = word d & 3 of Philox4x32-10, key (seed lo, seed hi), counter (imp_ids[q] lo,
+ *   r, epoch lo, d >> 2).  *loss_sum += l_c = log(e^{s_c} + sum_{n in S_c} e^{s_n}) - s_c (max subtracted, fp64 atomics) and
+ *   dh_p += scale sum_c sum_{j in {c} + S_c} (p_cj - [j = c]) e(items[j]), p_cj the softmax weight.  Every row p < n_pos of dh
+ *   is written (zero without impressions), in a fixed order per row: no atomics on dh.
  * dae_impression_metrics: one query row q_i (ld_q) per impression.  scores[k] (fp32, every k < indptr[n_imp]) = q_i . e(items[k]),
  *   or with cosine = 1 that over |q_i| |e(items[k])| (0 when either is zero).  The dot products and squared norms are fp32 sums:
  *   with every |x| <= 2^63 / sqrt(H) they stay below 2^126 and every score is finite (impression_metrics rejects larger
@@ -675,6 +684,10 @@ int dae_lstm_cell_bwd(int32_t n, int32_t H, const float* dh_in, int64_t ld_dh_in
 int dae_impression_rank_loss(const float* h, int64_t ld_h, const float* emb, int64_t ld_emb, int32_t H, const int64_t* pos_indptr,
                              int64_t n_pos, const int64_t* imp_indptr, const int32_t* items, const uint8_t* clicked, float scale,
                              float* dh, int64_t ld_dh, double* loss_sum, void* stream);
+int dae_impression_softmax_loss(const float* h, int64_t ld_h, const float* emb, int64_t ld_emb, int32_t H, const int64_t* pos_indptr,
+                                int64_t n_pos, const int64_t* imp_indptr, const int32_t* items, const uint8_t* clicked,
+                                const int64_t* imp_ids, int32_t K, uint64_t seed, uint64_t epoch, float scale, float* dh, int64_t ld_dh,
+                                double* loss_sum, void* workspace, void* stream);
 int dae_impression_metrics(const float* q, int64_t ld_q, const float* emb, int64_t ld_emb, int32_t H, int32_t cosine,
                            const int64_t* indptr, const int32_t* items, const uint8_t* clicked, int64_t n_imp, float* scores,
                            double* metrics, void* stream);

@@ -112,6 +112,13 @@ def build_parser():
     ap.add_argument('--user_impressions', default='',
                     help='with --user_sequences: an .npz impression log (user, time, indptr, items, clicked; see '
                          'user_model.check_impressions) to train the GRU on instead of random negatives')
+    ap.add_argument('--user_impression_loss', default=None, choices=['pairwise', 'softmax'],
+                    help='with --user_impressions: the impression loss, pairwise (every click against every non-click; the '
+                         'default) or softmax (each click against --user_negatives non-clicks of its impression under a softmax '
+                         'cross-entropy, as MIND\'s trainers do)')
+    ap.add_argument('--user_negatives', type=int, default=None,
+                    help='with --user_impressions: K, the non-clicks drawn per click by --user_impression_loss softmax, '
+                         '0 <= K <= 32 (default 4; 0 = every non-click)')
     ap.add_argument('--user_test_impressions', default='',
                     help='with --user_sequences: an .npz impression log to score; report the AUC, MRR, nDCG@5 and nDCG@10 of the '
                          'GRU states (user_gru_imp_*) and of the mean profile of the same reads (user_mean_imp_*)')
@@ -179,6 +186,11 @@ def check_flags(F):
     for flag, path in (('--user_impressions', F.user_impressions), ('--user_test_impressions', F.user_test_impressions)):
         assert not path or F.user_sequences, '%s needs --user_sequences' % flag
         assert not path or os.path.isfile(path), '%s %s: no such file' % (flag, path)
+    for flag, v in (('--user_impression_loss', F.user_impression_loss), ('--user_negatives', F.user_negatives)):
+        assert v is None or F.user_impressions, '%s needs --user_impressions' % flag
+    F.user_impression_loss = F.user_impression_loss or 'pairwise'
+    F.user_negatives = 4 if F.user_negatives is None else F.user_negatives
+    assert 0 <= F.user_negatives <= 32, '--user_negatives %d: 0 <= K <= 32' % F.user_negatives
     assert not F.user_targets or F.user_histories, '--user_targets needs --user_histories'
     assert not F.user_targets or os.path.isfile(F.user_targets), '--user_targets %s: no such file' % F.user_targets
     if F.input_format == 'tfidf':
@@ -515,10 +527,14 @@ def recommend_users_sequences(F, model, enc, seqs, impressions=(None, None)):
     print('train a %s user encoder on %d users (%d reads, %d epochs%s)' % (label, len(indptr) - 1, items.size, F.user_epochs,
                                                                          ', impressions' if train_imp is not None else ''))
     enc_cls = {'gru': UserGRU, 'lstm': UserLSTM}[cell]
-    rnn = enc_cls(enc.shape[1], num_epochs=F.user_epochs, seed=max(F.seed, 0))
+    rnn = enc_cls(enc.shape[1], num_epochs=F.user_epochs, seed=max(F.seed, 0), impression_loss=F.user_impression_loss,
+                  impression_negatives=F.user_negatives)
     rnn.fit((indptr, items), enc, impressions=train_imp)
     if train_imp is not None:
         print('impressions: %(used)d used, %(skipped)d skipped' % rnn.impression_counts)
+        if F.user_impression_loss == 'softmax':
+            print('impression loss: softmax over each click and %s of its non-clicks (%d clicks)' % (
+                'all' if F.user_negatives == 0 else 'at most %d' % F.user_negatives, rnn.impression_counts['clicks']))
     rnn.save(model.data_dir + 'user_%s.npz' % cell)
     idx, score = rnn.recommend((indptr, items), enc, k=F.top_k, long_lists=F.long_lists)
     np.save(model.data_dir + 'user_%s_top_k_index' % cell, idx)

@@ -1,14 +1,15 @@
-"""Impression logs: GRU training on impressions against random negatives, and the per-impression ranking metrics against a
-padded torch arm.  One JSON line.
+"""Impression logs: GRU training on impressions (the pairwise loss, and the sampled softmax at K = 4 and K = 0) against random
+negatives, and the per-impression ranking metrics against a padded torch arm.  One JSON line.
 
     python tools/bench_user_impressions.py [--n 100000] [--h 500] [--users 32768] [--batch_users 1024,4096] [--imps 1000000] [--reps 3]
 
 Workload: --n clustered articles of width --h (device resident), synth.make_sequences users (mean length 20, the last 50 reads
 trained) and synth.make_impressions (shown = 20: one impression per read after the first).  Reported:
-  train[B]: one epoch at batch_users B with impressions and one with random negatives (host packing and the impression batches
-            built outside the timed span, the arms in rotating order, medians of --reps epochs after a warm-up epoch of each):
-            positions/s, impressions/s, and the loss kernel's device time per epoch (dae_impression_rank_loss against
-            dae_seq_rank_loss, CUDA events around the kernel in a separate epoch);
+  train[B]: one epoch at batch_users B per arm -- impressions with the pairwise loss, with the softmax loss at K = 4 and at K = 0,
+            and random negatives -- (host packing and the impression batches built outside the timed span, the arms in rotating
+            order, medians of --reps epochs after a warm-up epoch of each): positions/s, impressions/s, clicks/s, and the loss
+            kernel's device time per epoch (dae_impression_rank_loss, dae_impression_softmax_loss or dae_seq_rank_loss, CUDA
+            events around the kernel in a separate epoch);
   metrics: --imps impressions of 20-54 shown articles (mean 37) with random queries: dae_impression_metrics alone (inputs on
            the device, CUDA events), helpers.impression_metrics as a whole (host checks, uploads, the means; synchronised
            wall clock), and a torch arm on the same device (padded gather + bmm, the ranks and the four metrics by padded torch
@@ -63,14 +64,19 @@ def _loss_ms(m, batches, emb, epoch):
     return ms
 
 
+ARMS = {'impressions': {}, 'softmax K=4': dict(impression_loss='softmax', impression_negatives=4),
+        'softmax K=0': dict(impression_loss='softmax', impression_negatives=0), 'random negatives': {}}
+
+
 def train_arm(args, B, indptr, items, emb, imp):
     res = {'batch_users': B}
     use = usable_impressions(imp, indptr, 50)
     active = np.unique(imp['user'][use])
     arms = {}
-    for name in ('impressions', 'random negatives'):
-        m = UserGRU(args.h, max_len=50, batch_users=B, seed=0)
-        if name == 'impressions':
+    names = list(ARMS)
+    for name in names:
+        m = UserGRU(args.h, max_len=50, batch_users=B, seed=0, **ARMS[name])
+        if name != 'random negatives':
             b = []
             for u in m.batches(indptr, 0, active):
                 pk = Packed(indptr, items, u, 50)
@@ -80,7 +86,7 @@ def train_arm(args, B, indptr, items, emb, imp):
         _epoch(m, b, emb, 0)                                        # warm-up
         arms[name] = (m, b, [])
     for r in range(args.reps):
-        for name in (('impressions', 'random negatives') if r % 2 == 0 else ('random negatives', 'impressions')):
+        for name in names[r % len(names):] + names[:r % len(names)]:
             m, b, t = arms[name]
             t.append(_epoch(m, b, emb, 1 + r))
     for name, (m, b, t) in arms.items():
@@ -88,9 +94,9 @@ def train_arm(args, B, indptr, items, emb, imp):
         pos = sum(pk.P for pk, _ in b)
         out = {'epoch_s': sec, 'epochs_s': t, 'positions_per_s': pos / sec, 'positions': pos, 'batches': len(b),
                'loss_kernel_ms_per_epoch': _loss_ms(m, b, emb, 99)}
-        if name == 'impressions':
-            n = sum(ib.n for _, ib in b)
-            out.update({'impressions': n, 'impressions_per_s': n / sec})
+        if name != 'random negatives':
+            n, c = sum(ib.n for _, ib in b), sum(ib.clicks for _, ib in b)
+            out.update({'impressions': n, 'impressions_per_s': n / sec, 'clicks': c, 'clicks_per_s': c / sec})
         res[name] = out
     return res
 
