@@ -105,6 +105,11 @@ _SIGNATURES = {
     # LSTM user encoder
     'dae_lstm_cell_fwd': (C.c_int, [i32, i32, p, i64, p, i64, p, i64, p, i64, p, i64, i32, p, p, i64, p, i64, p]),
     'dae_lstm_cell_bwd': (C.c_int, [i32, i32, p, i64, p, i64, p, i64, p, i64, p, i64, p, i64, p, p, i64, p]),
+    # attention user encoder
+    'dae_seq_attention_fwd': (C.c_int, [i32, i32, p, p, i32, i32, p, i64, p, i64, p, p, i64, p, i64, p]),
+    'dae_seq_attention_bwd': (C.c_int, [i32, i32, p, p, i32, i32, p, i64, p, i64, p, i64, p, i64, p, p, i64, p]),
+    'dae_seq_pool_fwd': (C.c_int, [i32, i32, p, p, i32, i32, p, i64, p, p, i64, p, i64, p, p, p]),
+    'dae_seq_pool_bwd': (C.c_int, [i32, i32, p, p, i32, i32, p, i64, p, i64, p, i64, p, i64, p, p, p, p, i64, p, p, i64, p, p, p]),
     # impression logs
     'dae_impression_rank_loss': (C.c_int, [p, i64, p, i64, i32, p, i64, p, p, p, f32, p, i64, p, p]),
     'dae_impression_metrics': (C.c_int, [p, i64, p, i64, i32, i32, p, p, p, i64, p, p, p]),

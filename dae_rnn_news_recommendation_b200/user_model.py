@@ -222,16 +222,15 @@ class Packed:
         return int(self.off[t] + i)
 
 
-class _UserRNN:
-    """What the recurrent user encoders share (UserGRU, UserLSTM): the flat parameters theta = [W~_hh | W~_ih] of GATES H rows each,
-    the packed training batch, the fit loop, the step loop of transform and impression_states, recommend, save and load.  A cell
-    class supplies GATES, its extra buffers, the carries its backward zeroes, the packed gradient operands of the two weight GEMMs
-    and its two kernel calls (_cell_fwd / _cell_bwd for training, _step for inference)."""
-    GATES = 0
-    _STATES = ('h',)                 # [B x H] inference states, zero at a batch's first step
-    _CARRIES = ('carry',)            # [B x H] backward carries zeroed for the rows of step 0
-    _DGRAD = ('dHP_hl', 'dXP_hl')    # packed gradient operands of [dW_hh | db_hh] and [dW_ih | db_ih]
-    _CARRY_ACCUMULATE = 1            # the carry GEMM dh_{t-1} (+)= dHP_t . W_hh accumulates onto the cell's carry, or stores
+class _UserEncoder:
+    """What every user encoder shares (UserGRU, UserLSTM, UserAttention): the constructor's checks, the flat fp32 parameters theta
+    and their optimizer slots, the loss dispatch of a packed training batch, the fit loop, batches, the optimizer step, the
+    impression runs of impression_states, transform's batch loop, recommend, save and load.  An encoder class supplies the
+    parameters and their files (state_dict, load_state_dict, _CONFIG / _PARAMS / _dim_of), its training buffers, _refresh (the
+    bf16 weight operands before a forward), _forward (the states Hs of every packed position) and _backward (theta's gradient from
+    dH), and for inference _infer_buffers, _last_states and _run_capture."""
+    _CONFIG = ()                     # constructor arguments save() stores next to max_len
+    _PARAMS = ()                     # state_dict names
 
     def __init__(self, dim, max_len=50, batch_users=1024, num_epochs=5, opt='adam', learning_rate=1e-3, seed=0, device='cuda:0',
                  momentum=0.5, impression_loss='pairwise', impression_negatives=4):
@@ -253,40 +252,26 @@ class _UserRNN:
         self.train_loss = []
         self.steps = 0
         self.epochs_done = 0
-        H, G = self.dim, self.GATES
-        self.nW = G * H * (H + 1)
-        self.ldx, self.ldg = _ld8(H + 1), _ld8(G * H)
-        # torch.nn.GRU's and torch.nn.LSTM's initialisation: every parameter uniform in [-1/sqrt(H), 1/sqrt(H)]
-        rng = np.random.default_rng(self.seed)
-        k = 1.0 / np.sqrt(H)
-        self.theta = torch.from_numpy(rng.uniform(-k, k, 2 * self.nW).astype(np.float32)).to(self.device)
-        self.grad = torch.zeros_like(self.theta)
-        self.slot1 = torch.full_like(self.theta, 0.1 if opt == 'ada_grad' else 0.0)
-        self.slot2 = torch.zeros_like(self.theta)
-        bf = dict(dtype=torch.bfloat16, device=self.device)
-        self.W_hl = {g: (torch.zeros(G * H, self.ldx, **bf), torch.zeros(G * H, self.ldx, **bf)) for g in ('hh', 'ih')}
-        self._hh_valid = False
         self._buf = {}
         self._cap = (0, 0)
         self.stats = torch.zeros(1, dtype=torch.float64, device=self.device)
         self.phase_events = None   # a list to record (phase name, CUDA event) pairs into (tools/bench_user_model.py)
 
-    # ---- parameters -------------------------------------------------------------------------------------------------------
-    def _theta(self, g):
-        """W~_g = [W_g | b_g] as a [GATES H, H+1] view of theta (g = 'hh' or 'ih')."""
-        o = 0 if g == 'hh' else self.nW
-        return self.theta[o:o + self.nW].view(self.GATES * self.dim, self.dim + 1)
+    def _set_theta(self, theta):
+        """theta (fp32 NumPy) on the device, its gradient and the optimizer slots."""
+        self.theta = torch.from_numpy(theta).to(self.device)
+        self.grad = torch.zeros_like(self.theta)
+        self.slot1 = torch.full_like(self.theta, 0.1 if self.opt == 'ada_grad' else 0.0)
+        self.slot2 = torch.zeros_like(self.theta)
 
-    def state_dict(self):
-        """torch.nn.GRU(H, H)'s / torch.nn.LSTM(H, H)'s parameter names and shapes (CPU fp32 tensors)."""
-        ih, hh = self._theta('ih').cpu(), self._theta('hh').cpu()
-        H = self.dim
-        return {'weight_ih_l0': ih[:, :H].clone(), 'weight_hh_l0': hh[:, :H].clone(), 'bias_ih_l0': ih[:, H].clone(),
-                'bias_hh_l0': hh[:, H].clone()}
+    def _reset_slots(self):
+        self.slot1.fill_(0.1 if self.opt == 'ada_grad' else 0.0)
+        self.slot2.zero_()
+        self.steps = 0
 
-    def load_state_dict(self, sd):
-        H, GH, name = self.dim, self.GATES * self.dim, type(self).__name__
-        want = {'weight_ih_l0': (GH, H), 'weight_hh_l0': (GH, H), 'bias_ih_l0': (GH,), 'bias_hh_l0': (GH,)}
+    def _load_arrays(self, sd, want):
+        """{name: fp32 NumPy array} from a state dict, or ValueError naming the missing keys or a wrong shape."""
+        name = type(self).__name__
         missing = set(want) - set(sd)
         if missing:
             raise ValueError('%s.load_state_dict: missing %s' % (name, sorted(missing)))
@@ -295,28 +280,28 @@ class _UserRNN:
             v = sd[k]
             v = v.detach().cpu().numpy() if isinstance(v, torch.Tensor) else np.asarray(v)
             if tuple(v.shape) != shape:
-                raise ValueError('%s.load_state_dict: %s has shape %s, %s expected (H = %d)' % (name, k, tuple(v.shape), shape, H))
+                raise ValueError('%s.load_state_dict: %s has shape %s, %s expected (H = %d)' % (name, k, tuple(v.shape), shape,
+                                                                                              self.dim))
             a[k] = v.astype(np.float32)
-        for g in ('ih', 'hh'):
-            t = np.concatenate([a['weight_%s_l0' % g], a['bias_%s_l0' % g][:, None]], 1)
-            self._theta(g).copy_(torch.from_numpy(t))
-        self.slot1.fill_(0.1 if self.opt == 'ada_grad' else 0.0)
-        self.slot2.zero_()
-        self.steps = 0
-        self._hh_valid = False
+        return a
 
     def save(self, path):
         sd = self.state_dict()
-        np.savez(path, max_len=self.max_len, **{k: v.numpy() for k, v in sd.items()})
+        np.savez(path, max_len=self.max_len, **{k: getattr(self, k) for k in self._CONFIG}, **{k: v.numpy() for k, v in sd.items()})
 
     @classmethod
     def load(cls, path, **kw):
-        """A model from save()'s .npz; keyword arguments as the constructor's (dim and max_len come from the file).  The parameter
-        shapes tell the cells apart: another cell's file fails load_state_dict's shape check."""
+        """A model from save()'s .npz; keyword arguments as the constructor's (dim, max_len and the encoder's _CONFIG come from the
+        file).  A file without this encoder's keys -- another encoder's -- raises ValueError naming them; another recurrent cell's
+        file fails load_state_dict's shape check."""
         z = np.load(path)
-        kw.setdefault('max_len', int(z['max_len']))
-        m = cls(int(z['weight_hh_l0'].shape[1]), **kw)
-        m.load_state_dict({k: z[k] for k in _NAMES})
+        missing = sorted(set(('max_len',) + cls._CONFIG + cls._PARAMS) - set(z.files))
+        if missing:
+            raise ValueError('%s.load: %s is not a %s file: it lacks %s' % (cls.__name__, path, cls.__name__, missing))
+        for k in ('max_len',) + cls._CONFIG:
+            kw.setdefault(k, int(z[k]))
+        m = cls(cls._dim_of(z), **kw)
+        m.load_state_dict({k: z[k] for k in cls._PARAMS})
         return m
 
     # ---- device helpers ---------------------------------------------------------------------------------------------------
@@ -334,46 +319,18 @@ class _UserRNN:
         call('dae_gemm_bf16x3', M, N, K, 1.0, a_hi.data_ptr(), a_lo.data_ptr(), a_hi.stride(0), a_mn, b_hi.data_ptr(), b_lo.data_ptr(),
              b_hi.stride(0), b_mn, C.data_ptr(), ldc, 0, -1, None, k_splits, accumulate, _stream())
 
-    def _split(self, g):
-        hi, lo = self.W_hl[g]
-        call('dae_split_bf16', self._theta(g).data_ptr(), self.GATES * self.dim, self.dim + 1, self.dim + 1, hi.data_ptr(), lo.data_ptr(),
-             self.ldx, -1, 1.0, _stream())
-
     def _mark(self, name):
         if self.phase_events is not None:
             e = torch.cuda.Event(enable_timing=True)
             e.record()
             self.phase_events.append((name, e))
 
-    def _buffers(self, P, B):
-        """Training buffers for P positions and B users (grown, never shrunk)."""
-        if P <= self._cap[0] and B <= self._cap[1]:
-            return self._buf
-        P, B = max(P, self._cap[0]), max(B, self._cap[1])
-        H, GH, d = self.dim, self.GATES * self.dim, self.device
-        f32, bf, i32 = dict(dtype=torch.float32, device=d), dict(dtype=torch.bfloat16, device=d), dict(dtype=torch.int32, device=d)
-        self._buf = None
-        torch.cuda.empty_cache()
-        b = {'neg': torch.empty(P, **i32),
-             'X_hl': (torch.empty(P, self.ldx, **bf), torch.empty(P, self.ldx, **bf)),
-             'XP': torch.empty(P, GH, **f32),
-             'Hp_hl': (torch.zeros(P, self.ldx, **bf), torch.zeros(P, self.ldx, **bf)),   # [h_{t-1} | 1] of every position
-             'HP': torch.empty(B, GH, **f32),
-             'Hs': torch.empty(P, H, **f32),
-             'gates': torch.empty(P, 4 * H, **f32),
-             'dH': torch.empty(P, H, **f32),
-             'carry': torch.empty(B, H, **f32)}
-        b.update(self._cell_buffers(P, B))
-        b['Hp_hl'][0][:, H] = 1.0
-        self._buf, self._cap = b, (P, B)
-        return b
-
     # ---- training ---------------------------------------------------------------------------------------------------------
     def _forward_backward(self, pk, emb, epoch, batch, ib=None):
         """Loss (added to self.stats) and the gradient (self.grad) of one packed batch with pk.terms > 0, or with ib (an
         ImpressionBatch with ib.n > 0) the impression loss of its impressions in place of the random negatives: pairwise, or with
         impression_loss='softmax' the sampled softmax over its ib.clicks samples."""
-        H, GH, P, T = self.dim, self.GATES * self.dim, pk.P, len(pk.n)
+        H, P = self.dim, pk.P
         b = self._buffers(P, pk.B)
         st = _stream()
         items = _upload(pk.items, self.device)
@@ -383,29 +340,12 @@ class _UserRNN:
             pos_indptr, imp_indptr, imp_items, imp_clicked, imp_ids = ib.views(_upload(ib.buffer(ids=True), self.device))
         else:
             pos_indptr, imp_indptr, imp_items, imp_clicked = ib.views(_upload(ib.buffer(), self.device))
-        if not self._hh_valid:
-            self._split('hh')
-            self._hh_valid = True
+        self._refresh()
         self._mark('start')
         if ib is None:
             call('dae_seq_negatives', nxt.data_ptr(), P, emb.shape[0], self.seed, epoch, batch, b['neg'].data_ptr(), st)
-        X_hi, X_lo = b['X_hl']
-        call('dae_gather_split_bf16', emb.data_ptr(), emb.stride(0), items.data_ptr(), P, H, X_hi.data_ptr(), X_lo.data_ptr(), self.ldx,
-             H, st)
-        self._split('ih')
-        self._gemm(P, GH, H + 1, b['X_hl'], 0, self.W_hl['ih'], 0, b['XP'], GH)
-        self._mark('input_projection')
-        Hp_hi, Hp_lo = b['Hp_hl']
-        n0 = int(pk.n[0])
-        Hp_hi[:n0, :H].zero_()
-        Hp_lo[:n0].zero_()
-        Hs, HP = b['Hs'], b['HP']
-        for t in range(T):
-            o, n = int(pk.off[t]), int(pk.n[t])
-            n_next = int(pk.n[t + 1]) if t + 1 < T else 0
-            self._gemm(n, GH, H + 1, (Hp_hi[o:], Hp_lo[o:]), 0, self.W_hl['hh'], 0, HP, GH)
-            self._cell_fwd(b, pk, t, n_next, st)
-        self._mark('forward_recurrence')
+        self._forward(b, pk, emb, items, st)
+        Hs = b['Hs']
         if ib is None:
             call('dae_seq_rank_loss', Hs.data_ptr(), H, emb.data_ptr(), emb.stride(0), H, nxt.data_ptr(), b['neg'].data_ptr(), P,
                  1.0 / pk.terms, b['dH'].data_ptr(), H, self.stats.data_ptr(), st)
@@ -419,30 +359,16 @@ class _UserRNN:
                  imp_indptr.data_ptr(), imp_items.data_ptr(), imp_clicked.data_ptr(), 1.0 / ib.n, b['dH'].data_ptr(), H,
                  self.stats.data_ptr(), st)
         self._mark('loss')
-        # rows [n_t, n_{t-1}) of the carries belong to users whose last read is at t - 1: nothing flows into them from later steps,
-        # and no later step writes them (step t' > t - 1 writes rows [0, n_t') only), so zeroing rows [0, n_0) once keeps them zero
-        for k in self._CARRIES:
-            b[k][:n0].zero_()
-        carry = b['carry']
-        dP_hi, dP_lo = b[self._DGRAD[0]]
-        for t in range(T - 1, -1, -1):
-            o, n = int(pk.off[t]), int(pk.n[t])
-            self._cell_bwd(b, pk, t, st)
-            if t:   # h_{-1} = 0 is a constant: no carry below step 0
-                self._gemm(n, H, GH, (dP_hi[o:], dP_lo[o:]), 0, self.W_hl['hh'], 1, carry, H, accumulate=self._CARRY_ACCUMULATE)
-        self._mark('backward_recurrence')
-        g_hh, g_ih = self.grad[:self.nW], self.grad[self.nW:]
-        self._gemm(GH, H + 1, P, b[self._DGRAD[0]], 1, b['Hp_hl'], 1, g_hh, H + 1, k_splits=-1)
-        self._gemm(GH, H + 1, P, b[self._DGRAD[1]], 1, b['X_hl'], 1, g_ih, H + 1, k_splits=-1)
-        self._mark('weight_gradients')
+        self._backward(b, pk, st)
 
     def _optimizer_step(self):
+        """One dae_optimizer_step over all of theta; _step_split() names the bf16 hi / lo copy of theta's leading block that the
+        step also writes (or None)."""
         self.steps += 1
-        hi, lo = self.W_hl['hh']
+        hi, lo, rows, cols, ld = self._step_split()
         call('dae_optimizer_step', self.theta.data_ptr(), self.grad.data_ptr(), self.slot1.data_ptr(), self.slot2.data_ptr(),
-             2 * self.nW, _cabi.OPT[self.opt], self.learning_rate, self.momentum, 1.0, self.steps, None, hi.data_ptr(), lo.data_ptr(),
-             self.GATES * self.dim, self.dim + 1, self.ldx, _stream())
-        self._hh_valid = True
+             self.theta.numel(), _cabi.OPT[self.opt], self.learning_rate, self.momentum, 1.0, self.steps, None, hi, lo, rows, cols,
+             ld, _stream())
         self._mark('optimizer')
 
     def batches(self, indptr, epoch, active=None):
@@ -508,60 +434,21 @@ class _UserRNN:
         return self
 
     # ---- inference --------------------------------------------------------------------------------------------------------
-    def _step_buffers(self, B):
-        """transform / impression_states' buffers for batches of up to B users: O(B x GATES H) device memory.  Also refreshes the
-        bf16 hi / lo copies of W~_hh (when stale) and W~_ih that the steps read."""
-        H, GH, d = self.dim, self.GATES * self.dim, self.device
-        if not self._hh_valid:
-            self._split('hh')
-            self._hh_valid = True
-        self._split('ih')
-        bf = dict(dtype=torch.bfloat16, device=d)
-        s = {'X_hl': (torch.zeros(B, self.ldx, **bf), torch.zeros(B, self.ldx, **bf)),
-             'h_hl': (torch.zeros(B, self.ldx, **bf), torch.zeros(B, self.ldx, **bf)),
-             'XP': torch.empty(B, GH, dtype=torch.float32, device=d),
-             'HP': torch.empty(B, GH, dtype=torch.float32, device=d),
-             'h': torch.empty(B, H, dtype=torch.float32, device=d)}
-        s.update(self._cell_step_buffers(B))
-        return s
-
-    def _steps(self, pk, emb, s, after=None):
-        """Run one packed batch from zero states, step by step: the input projection of the step's reads, the recurrent GEMM and the
-        cell, which updates s['h'] (and the cell's other states) in place.  after(t), if given, runs after step t."""
-        H, GH, st = self.dim, self.GATES * self.dim, _stream()
-        it = _upload(pk.items, self.device)
-        h_hi, h_lo = s['h_hl']
-        h_hi.zero_()
-        h_lo.zero_()
-        h_hi[:, H] = 1.0
-        for k in self._STATES:
-            s[k][:pk.B].zero_()
-        X_hi, X_lo = s['X_hl']
-        for t in range(len(pk.n)):
-            o, n = int(pk.off[t]), int(pk.n[t])
-            call('dae_gather_split_bf16', emb.data_ptr(), emb.stride(0), it[o:].data_ptr(), n, H, X_hi.data_ptr(), X_lo.data_ptr(),
-                 self.ldx, H, st)
-            self._gemm(n, GH, H + 1, (X_hi, X_lo), 0, self.W_hl['ih'], 0, s['XP'], GH)
-            self._gemm(n, GH, H + 1, (h_hi, h_lo), 0, self.W_hl['hh'], 0, s['HP'], GH)
-            self._step(s, n, st)
-            if after is not None:
-                after(t)
-
     def transform(self, sequences, embeddings, to_host=True):
-        """User vectors [U, H] fp32: the state h after each user's last (truncated) read; zero rows for users without reads.
-        Projects step by step, so device memory per batch is O(batch_users x GATES H), not O(positions x GATES H)."""
+        """User vectors [U, H] fp32: the state after each user's last (truncated) read; zero rows for users without reads.  Device
+        memory per batch: O(batch_users x GATES H) for the recurrent cells, which project step by step; O(batch positions x (3H + A))
+        for UserAttention, which runs each batch in one pass."""
         fn = '%s.transform' % type(self).__name__
         emb = self._embeddings(embeddings, fn)
         indptr, items = check_sequences(sequences, emb.shape[0], fn)
         H, U, B, d = self.dim, len(indptr) - 1, self.batch_users, self.device
         out = torch.zeros(U, H, dtype=torch.float32, device=d)
-        s = self._step_buffers(B)
+        s = self._infer_buffers(B)
         for u0 in range(0, U, B):
             pk = Packed(indptr, items, np.arange(u0, min(U, u0 + B)), self.max_len)
             if pk.B == 0:
                 continue
-            self._steps(pk, emb, s)
-            out.index_copy_(0, torch.from_numpy(pk.order).to(d), s['h'][:pk.B])
+            out.index_copy_(0, torch.from_numpy(pk.order).to(d), self._last_states(pk, emb, s))
         return out.cpu().numpy() if to_host else out
 
     def impression_states(self, sequences, embeddings, impressions, to_host=True):
@@ -570,9 +457,9 @@ class _UserRNN:
 
         Training (fit(impressions=...)) takes the state from the packed window of the user's LAST max_len reads, which starts at
         read len - max_len whatever the impression's time; here the window ENDS at the impression.  The two agree at time = len
-        and for users with at most max_len reads.  Each (user, window start) pair is one run of transform's step
-        loop, whose states are copied out at the steps that impressions ask for: a user whose impressions all lie within the first
-        max_len reads costs one run.  Device memory per batch is O(batch_users x GATES H), as transform's."""
+        and for users with at most max_len reads.  Each (user, window start) pair is one run of a packed batch, whose states are
+        copied out at the steps that impressions ask for: a user whose impressions all lie within the first max_len reads costs
+        one run.  Device memory per batch is transform's."""
         fn = '%s.impression_states' % type(self).__name__
         emb = self._embeddings(embeddings, fn)
         indptr, items = check_sequences(sequences, emb.shape[0], fn)
@@ -598,8 +485,7 @@ class _UserRNN:
         r_items = items[np.repeat(r_src - r_indptr[:-1], run_len) + np.arange(int(r_indptr[-1]))]
         step = t - start - 1   # the step after which impression ids[j] reads its run's state
         B = self.batch_users
-        s = self._step_buffers(B)
-        h = s['h']
+        s = self._infer_buffers(B)
         order = np.argsort(run_of, kind='stable')
         for r0 in range(0, n_run, B):
             pk = Packed(r_indptr, r_items, np.arange(r0, min(n_run, r0 + B)), self.max_len)
@@ -607,17 +493,7 @@ class _UserRNN:
             row[pk.order] = np.arange(pk.B)
             lo, hi = np.searchsorted(run_of[order], [r0, r0 + B])
             sel = order[lo:hi]
-            cap_step, cap_row, cap_imp = step[sel], row[run_of[sel]], ids[sel]
-            o = np.argsort(cap_step, kind='stable')
-            cap_step, cap = cap_step[o], np.stack([cap_row[o], cap_imp[o]])
-            bounds = np.searchsorted(cap_step, np.arange(len(pk.n) + 1))
-            cap_d = _upload(np.ascontiguousarray(cap), d)
-
-            def capture(tt, bounds=bounds, cap_d=cap_d):
-                a, b = int(bounds[tt]), int(bounds[tt + 1])
-                if b > a:
-                    out.index_copy_(0, cap_d[1, a:b], h.index_select(0, cap_d[0, a:b]))
-            self._steps(pk, emb, s, capture)
+            self._run_capture(pk, emb, s, step[sel], row[run_of[sel]], ids[sel], out)
         return out.cpu().numpy() if to_host else out
 
     def recommend(self, sequences, embeddings, k=10, candidates=None, exclude_read=True, metric='linear kernel', to_host=True,
@@ -634,6 +510,200 @@ class _UserRNN:
         prof = self.transform((indptr, items), emb, to_host=False)
         return recommend(hist, emb, k=k, candidates=candidates, metric=metric, exclude_read=exclude_read, device=self.device,
                          to_host=to_host, profiles=prof, groups=groups, long_lists=long_lists)
+
+
+class _UserRNN(_UserEncoder):
+    """What the recurrent user encoders share (UserGRU, UserLSTM): the flat parameters theta = [W~_hh | W~_ih] of GATES H rows each,
+    their torch.nn.GRU / torch.nn.LSTM names, the packed training batch's step loops and the step loop of transform and
+    impression_states.  A cell class supplies GATES, its extra buffers, the carries its backward zeroes, the packed gradient
+    operands of the two weight GEMMs and its two kernel calls (_cell_fwd / _cell_bwd for training, _step for inference)."""
+    GATES = 0
+    _STATES = ('h',)                 # [B x H] inference states, zero at a batch's first step
+    _CARRIES = ('carry',)            # [B x H] backward carries zeroed for the rows of step 0
+    _DGRAD = ('dHP_hl', 'dXP_hl')    # packed gradient operands of [dW_hh | db_hh] and [dW_ih | db_ih]
+    _CARRY_ACCUMULATE = 1            # the carry GEMM dh_{t-1} (+)= dHP_t . W_hh accumulates onto the cell's carry, or stores
+    _PARAMS = _NAMES
+
+    def __init__(self, dim, *args, **kw):
+        super().__init__(dim, *args, **kw)
+        H, G = self.dim, self.GATES
+        self.nW = G * H * (H + 1)
+        self.ldx, self.ldg = _ld8(H + 1), _ld8(G * H)
+        # torch.nn.GRU's and torch.nn.LSTM's initialisation: every parameter uniform in [-1/sqrt(H), 1/sqrt(H)]
+        rng = np.random.default_rng(self.seed)
+        k = 1.0 / np.sqrt(H)
+        self._set_theta(rng.uniform(-k, k, 2 * self.nW).astype(np.float32))
+        bf = dict(dtype=torch.bfloat16, device=self.device)
+        self.W_hl = {g: (torch.zeros(G * H, self.ldx, **bf), torch.zeros(G * H, self.ldx, **bf)) for g in ('hh', 'ih')}
+        self._hh_valid = False
+
+    # ---- parameters -------------------------------------------------------------------------------------------------------
+    def _theta(self, g):
+        """W~_g = [W_g | b_g] as a [GATES H, H+1] view of theta (g = 'hh' or 'ih')."""
+        o = 0 if g == 'hh' else self.nW
+        return self.theta[o:o + self.nW].view(self.GATES * self.dim, self.dim + 1)
+
+    def state_dict(self):
+        """torch.nn.GRU(H, H)'s / torch.nn.LSTM(H, H)'s parameter names and shapes (CPU fp32 tensors)."""
+        ih, hh = self._theta('ih').cpu(), self._theta('hh').cpu()
+        H = self.dim
+        return {'weight_ih_l0': ih[:, :H].clone(), 'weight_hh_l0': hh[:, :H].clone(), 'bias_ih_l0': ih[:, H].clone(),
+                'bias_hh_l0': hh[:, H].clone()}
+
+    def load_state_dict(self, sd):
+        H, GH = self.dim, self.GATES * self.dim
+        a = self._load_arrays(sd, {'weight_ih_l0': (GH, H), 'weight_hh_l0': (GH, H), 'bias_ih_l0': (GH,), 'bias_hh_l0': (GH,)})
+        for g in ('ih', 'hh'):
+            t = np.concatenate([a['weight_%s_l0' % g], a['bias_%s_l0' % g][:, None]], 1)
+            self._theta(g).copy_(torch.from_numpy(t))
+        self._reset_slots()
+        self._hh_valid = False
+
+    @staticmethod
+    def _dim_of(z):
+        return int(z['weight_hh_l0'].shape[1])
+
+    # ---- device helpers ---------------------------------------------------------------------------------------------------
+    def _split(self, g):
+        hi, lo = self.W_hl[g]
+        call('dae_split_bf16', self._theta(g).data_ptr(), self.GATES * self.dim, self.dim + 1, self.dim + 1, hi.data_ptr(), lo.data_ptr(),
+             self.ldx, -1, 1.0, _stream())
+
+    def _buffers(self, P, B):
+        """Training buffers for P positions and B users (grown, never shrunk)."""
+        if P <= self._cap[0] and B <= self._cap[1]:
+            return self._buf
+        P, B = max(P, self._cap[0]), max(B, self._cap[1])
+        H, GH, d = self.dim, self.GATES * self.dim, self.device
+        f32, bf, i32 = dict(dtype=torch.float32, device=d), dict(dtype=torch.bfloat16, device=d), dict(dtype=torch.int32, device=d)
+        self._buf = None
+        torch.cuda.empty_cache()
+        b = {'neg': torch.empty(P, **i32),
+             'X_hl': (torch.empty(P, self.ldx, **bf), torch.empty(P, self.ldx, **bf)),
+             'XP': torch.empty(P, GH, **f32),
+             'Hp_hl': (torch.zeros(P, self.ldx, **bf), torch.zeros(P, self.ldx, **bf)),   # [h_{t-1} | 1] of every position
+             'HP': torch.empty(B, GH, **f32),
+             'Hs': torch.empty(P, H, **f32),
+             'gates': torch.empty(P, 4 * H, **f32),
+             'dH': torch.empty(P, H, **f32),
+             'carry': torch.empty(B, H, **f32)}
+        b.update(self._cell_buffers(P, B))
+        b['Hp_hl'][0][:, H] = 1.0
+        self._buf, self._cap = b, (P, B)
+        return b
+
+    # ---- training ---------------------------------------------------------------------------------------------------------
+    def _refresh(self):
+        if not self._hh_valid:
+            self._split('hh')
+            self._hh_valid = True
+
+    def _forward(self, b, pk, emb, items, st):
+        """The input projection of every position, then per step the recurrent GEMM and the cell: b['Hs']."""
+        H, GH, P, T = self.dim, self.GATES * self.dim, pk.P, len(pk.n)
+        X_hi, X_lo = b['X_hl']
+        call('dae_gather_split_bf16', emb.data_ptr(), emb.stride(0), items.data_ptr(), P, H, X_hi.data_ptr(), X_lo.data_ptr(), self.ldx,
+             H, st)
+        self._split('ih')
+        self._gemm(P, GH, H + 1, b['X_hl'], 0, self.W_hl['ih'], 0, b['XP'], GH)
+        self._mark('input_projection')
+        Hp_hi, Hp_lo = b['Hp_hl']
+        n0 = int(pk.n[0])
+        Hp_hi[:n0, :H].zero_()
+        Hp_lo[:n0].zero_()
+        Hs, HP = b['Hs'], b['HP']
+        for t in range(T):
+            o, n = int(pk.off[t]), int(pk.n[t])
+            n_next = int(pk.n[t + 1]) if t + 1 < T else 0
+            self._gemm(n, GH, H + 1, (Hp_hi[o:], Hp_lo[o:]), 0, self.W_hl['hh'], 0, HP, GH)
+            self._cell_fwd(b, pk, t, n_next, st)
+        self._mark('forward_recurrence')
+
+    def _backward(self, b, pk, st):
+        """Backpropagation through time from b['dH'], then the two weight GEMMs into self.grad."""
+        H, GH, P, T = self.dim, self.GATES * self.dim, pk.P, len(pk.n)
+        n0 = int(pk.n[0])
+        # rows [n_t, n_{t-1}) of the carries belong to users whose last read is at t - 1: nothing flows into them from later steps,
+        # and no later step writes them (step t' > t - 1 writes rows [0, n_t') only), so zeroing rows [0, n_0) once keeps them zero
+        for k in self._CARRIES:
+            b[k][:n0].zero_()
+        carry = b['carry']
+        dP_hi, dP_lo = b[self._DGRAD[0]]
+        for t in range(T - 1, -1, -1):
+            o, n = int(pk.off[t]), int(pk.n[t])
+            self._cell_bwd(b, pk, t, st)
+            if t:   # h_{-1} = 0 is a constant: no carry below step 0
+                self._gemm(n, H, GH, (dP_hi[o:], dP_lo[o:]), 0, self.W_hl['hh'], 1, carry, H, accumulate=self._CARRY_ACCUMULATE)
+        self._mark('backward_recurrence')
+        g_hh, g_ih = self.grad[:self.nW], self.grad[self.nW:]
+        self._gemm(GH, H + 1, P, b[self._DGRAD[0]], 1, b['Hp_hl'], 1, g_hh, H + 1, k_splits=-1)
+        self._gemm(GH, H + 1, P, b[self._DGRAD[1]], 1, b['X_hl'], 1, g_ih, H + 1, k_splits=-1)
+        self._mark('weight_gradients')
+
+    def _step_split(self):
+        hi, lo = self.W_hl['hh']
+        self._hh_valid = True
+        return hi.data_ptr(), lo.data_ptr(), self.GATES * self.dim, self.dim + 1, self.ldx
+
+    # ---- inference --------------------------------------------------------------------------------------------------------
+    def _step_buffers(self, B):
+        """transform / impression_states' buffers for batches of up to B users: O(B x GATES H) device memory.  Also refreshes the
+        bf16 hi / lo copies of W~_hh (when stale) and W~_ih that the steps read."""
+        H, GH, d = self.dim, self.GATES * self.dim, self.device
+        if not self._hh_valid:
+            self._split('hh')
+            self._hh_valid = True
+        self._split('ih')
+        bf = dict(dtype=torch.bfloat16, device=d)
+        s = {'X_hl': (torch.zeros(B, self.ldx, **bf), torch.zeros(B, self.ldx, **bf)),
+             'h_hl': (torch.zeros(B, self.ldx, **bf), torch.zeros(B, self.ldx, **bf)),
+             'XP': torch.empty(B, GH, dtype=torch.float32, device=d),
+             'HP': torch.empty(B, GH, dtype=torch.float32, device=d),
+             'h': torch.empty(B, H, dtype=torch.float32, device=d)}
+        s.update(self._cell_step_buffers(B))
+        return s
+
+    _infer_buffers = _step_buffers
+
+    def _last_states(self, pk, emb, s):
+        self._steps(pk, emb, s)
+        return s['h'][:pk.B]
+
+    def _run_capture(self, pk, emb, s, cap_step, cap_row, cap_imp, out):
+        """Run pk step by step; after step cap_step[j], row cap_row[j] of the states is impression cap_imp[j]'s row of out."""
+        o = np.argsort(cap_step, kind='stable')
+        cap_step, cap = cap_step[o], np.stack([cap_row[o], cap_imp[o]])
+        bounds = np.searchsorted(cap_step, np.arange(len(pk.n) + 1))
+        cap_d = _upload(np.ascontiguousarray(cap), self.device)
+        h = s['h']
+
+        def capture(tt):
+            a, b = int(bounds[tt]), int(bounds[tt + 1])
+            if b > a:
+                out.index_copy_(0, cap_d[1, a:b], h.index_select(0, cap_d[0, a:b]))
+        self._steps(pk, emb, s, capture)
+
+    def _steps(self, pk, emb, s, after=None):
+        """Run one packed batch from zero states, step by step: the input projection of the step's reads, the recurrent GEMM and the
+        cell, which updates s['h'] (and the cell's other states) in place.  after(t), if given, runs after step t."""
+        H, GH, st = self.dim, self.GATES * self.dim, _stream()
+        it = _upload(pk.items, self.device)
+        h_hi, h_lo = s['h_hl']
+        h_hi.zero_()
+        h_lo.zero_()
+        h_hi[:, H] = 1.0
+        for k in self._STATES:
+            s[k][:pk.B].zero_()
+        X_hi, X_lo = s['X_hl']
+        for t in range(len(pk.n)):
+            o, n = int(pk.off[t]), int(pk.n[t])
+            call('dae_gather_split_bf16', emb.data_ptr(), emb.stride(0), it[o:].data_ptr(), n, H, X_hi.data_ptr(), X_lo.data_ptr(),
+                 self.ldx, H, st)
+            self._gemm(n, GH, H + 1, (X_hi, X_lo), 0, self.W_hl['ih'], 0, s['XP'], GH)
+            self._gemm(n, GH, H + 1, (h_hi, h_lo), 0, self.W_hl['hh'], 0, s['HP'], GH)
+            self._step(s, n, st)
+            if after is not None:
+                after(t)
 
 
 class UserGRU(_UserRNN):
@@ -724,6 +794,197 @@ class UserLSTM(_UserRNN):
         h_hi, h_lo = s['h_hl']
         call('dae_lstm_cell_fwd', n, H, s['XP'].data_ptr(), 4 * H, s['HP'].data_ptr(), 4 * H, c.data_ptr(), H, c.data_ptr(), H,
              h.data_ptr(), H, n, h_hi.data_ptr(), h_lo.data_ptr(), self.ldx, None, 0, st)
+
+
+MAX_ATTENTION_LEN = 1024     # dae_seq_attention_* / dae_seq_pool_*: reads per window
+MAX_HEAD_DIM = 128           # dae_seq_attention_*: H / heads
+ATTENTION_NAMES = ('self_attn.in_proj_weight', 'self_attn.in_proj_bias', 'self_attn.out_proj.weight', 'self_attn.out_proj.bias',
+                   'pool.weight', 'pool.bias', 'pool.query')
+
+
+def default_heads(dim):
+    """The largest divisor of dim that is at most 20 (NRMS's head count): 20 at H = 500, 1 at H = 37."""
+    return max(k for k in range(1, min(int(dim), 20) + 1) if dim % k == 0)
+
+
+class UserAttention(_UserEncoder):
+    """NRMS's user encoder over reading sequences, made causal (DESIGN 4.17): for a window of reads with article vectors x_1..x_L,
+    m = torch.nn.MultiheadAttention(H, heads, batch_first=True)(x, x, x) with a causal mask (read t attends to reads s <= t), then
+    additive pooling a_s = q . tanh(W_a m_s + b_a) and u_t = sum_{s <= t} softmax_{s <= t}(a)_s m_s.  u_t depends only on the
+    reads up to t, like an RNN's h_t, so the losses, fit, transform (u_L), impression_states and recommend are the recurrent
+    encoders'.  NRMS concatenates the heads without an output projection; this encoder keeps torch's out_proj so that a CPU
+    torch.nn.MultiheadAttention loads the self_attn.* parameters.
+
+    heads: None for default_heads(dim); H / heads <= 128.  attention_dim: A >= 1, the pooling width.  max_len <= 1024.
+    theta = [W~_in (3H x (H+1)) | W~_out (H x (H+1)) | W~_a (A x (H+1)) | q (A)] with W~ = [W | b], updated by one optimizer step.
+
+    Device path per batch (one pass over every packed position, no step loop): [X | 1] and QKV = [X | 1].W~_in^T;
+    dae_seq_attention_fwd (O, its bf16 split and the row log-sum-exps); M = [O | 1].W~_out^T; Z = [M | 1].W~_a^T; dae_seq_pool_fwd
+    (Hs).  Backward: dae_seq_pool_bwd (dM's value path, dZ, dq); dM += dZ.W_a; dO = dM.W_out; dae_seq_attention_bwd (dQKV); the
+    three weight GEMMs.  Device memory per batch is O(batch positions x (3H + A)), in training and in inference."""
+    _CONFIG = ('heads', 'attention_dim')
+    _PARAMS = ATTENTION_NAMES
+
+    def __init__(self, dim, heads=None, attention_dim=200, **kw):
+        super().__init__(dim, **kw)
+        name = type(self).__name__
+        H = self.dim
+        if heads is None:
+            heads = default_heads(H)
+        if isinstance(heads, bool) or not isinstance(heads, (int, np.integer)) or heads < 1 or H % heads:
+            raise ValueError('%s: heads = %r must be a positive divisor of dim = %d' % (name, heads, H))
+        if H // heads > MAX_HEAD_DIM:
+            raise ValueError('%s: head dim H / heads = %d exceeds %d' % (name, H // heads, MAX_HEAD_DIM))
+        if isinstance(attention_dim, bool) or not isinstance(attention_dim, (int, np.integer)) or attention_dim < 1:
+            raise ValueError('%s: attention_dim = %r must be an integer >= 1' % (name, attention_dim))
+        if self.max_len > MAX_ATTENTION_LEN:
+            raise ValueError('%s: max_len = %d exceeds %d' % (name, self.max_len, MAX_ATTENTION_LEN))
+        self.heads, self.attention_dim = int(heads), int(attention_dim)
+        A = self.attention_dim
+        self.ldx, self.ld3, self.lda = _ld8(H + 1), _ld8(3 * H), _ld8(A)
+        self._rows = {'in': 3 * H, 'out': H, 'pool': A}
+        self._off = {'in': 0, 'out': 3 * H * (H + 1), 'pool': 4 * H * (H + 1), 'query': (4 * H + A) * (H + 1)}
+        # torch.nn.MultiheadAttention's initialisation (Xavier-uniform in_proj, out_proj uniform +-1/sqrt(H), zero biases) and NRMS's
+        # pooling layer's (Glorot-uniform W_a [A x H] and q [A x 1], zero b_a), drawn in that order
+        rng = np.random.default_rng(self.seed)
+        w_in = rng.uniform(-1.0, 1.0, (3 * H, H)) * np.sqrt(6.0 / (4 * H))
+        w_out = rng.uniform(-1.0, 1.0, (H, H)) / np.sqrt(H)
+        w_a = rng.uniform(-1.0, 1.0, (A, H)) * np.sqrt(6.0 / (A + H))
+        q = rng.uniform(-1.0, 1.0, A) * np.sqrt(6.0 / (A + 1))
+        pad = lambda w: np.concatenate([w, np.zeros((w.shape[0], 1))], 1).ravel()   # noqa: E731
+        self._set_theta(np.concatenate([pad(w_in), pad(w_out), pad(w_a), q]).astype(np.float32))
+        bf = dict(dtype=torch.bfloat16, device=self.device)
+        self.W_hl = {g: (torch.zeros(r, self.ldx, **bf), torch.zeros(r, self.ldx, **bf)) for g, r in self._rows.items()}
+
+    # ---- parameters -------------------------------------------------------------------------------------------------------
+    def _theta(self, g, t=None):
+        """W~_g = [W_g | b_g] as a [rows, H+1] view of theta (g = 'in', 'out' or 'pool'), or q [A] (g = 'query'); t: theta or grad."""
+        t = self.theta if t is None else t
+        o = self._off[g]
+        if g == 'query':
+            return t[o:o + self.attention_dim]
+        return t[o:o + self._rows[g] * (self.dim + 1)].view(self._rows[g], self.dim + 1)
+
+    def state_dict(self):
+        """torch.nn.MultiheadAttention's names under 'self_attn.' and the pooling layer's under 'pool.' (CPU fp32 tensors)."""
+        H = self.dim
+        w = {g: self._theta(g).cpu() for g in ('in', 'out', 'pool')}
+        return {'self_attn.in_proj_weight': w['in'][:, :H].clone(), 'self_attn.in_proj_bias': w['in'][:, H].clone(),
+                'self_attn.out_proj.weight': w['out'][:, :H].clone(), 'self_attn.out_proj.bias': w['out'][:, H].clone(),
+                'pool.weight': w['pool'][:, :H].clone(), 'pool.bias': w['pool'][:, H].clone(),
+                'pool.query': self._theta('query').cpu().clone()}
+
+    def load_state_dict(self, sd):
+        H, A = self.dim, self.attention_dim
+        a = self._load_arrays(sd, {'self_attn.in_proj_weight': (3 * H, H), 'self_attn.in_proj_bias': (3 * H,),
+                                   'self_attn.out_proj.weight': (H, H), 'self_attn.out_proj.bias': (H,), 'pool.weight': (A, H),
+                                   'pool.bias': (A,), 'pool.query': (A,)})
+        for g, (wk, bk) in (('in', ('self_attn.in_proj_weight', 'self_attn.in_proj_bias')),
+                            ('out', ('self_attn.out_proj.weight', 'self_attn.out_proj.bias')), ('pool', ('pool.weight', 'pool.bias'))):
+            self._theta(g).copy_(torch.from_numpy(np.concatenate([a[wk], a[bk][:, None]], 1)))
+        self._theta('query').copy_(torch.from_numpy(a['pool.query']))
+        self._reset_slots()
+
+    @staticmethod
+    def _dim_of(z):
+        return int(z['self_attn.out_proj.weight'].shape[0])
+
+    # ---- device helpers ---------------------------------------------------------------------------------------------------
+    def _buffers(self, P, B):
+        """Buffers for P positions and B users (grown, never shrunk): O(P x (3H + A))."""
+        if P <= self._cap[0] and B <= self._cap[1]:
+            return self._buf
+        P, B = max(P, self._cap[0]), max(B, self._cap[1])
+        H, A, d = self.dim, self.attention_dim, self.device
+        f32, bf, i32 = dict(dtype=torch.float32, device=d), dict(dtype=torch.bfloat16, device=d), dict(dtype=torch.int32, device=d)
+        pair = lambda ld: (torch.zeros(P, ld, **bf), torch.zeros(P, ld, **bf))   # noqa: E731
+        self._buf = None
+        torch.cuda.empty_cache()
+        b = {'neg': torch.empty(P, **i32), 'X_hl': pair(self.ldx), 'QKV': torch.empty(P, 3 * H, **f32), 'O': torch.empty(P, H, **f32),
+             'O_hl': pair(self.ldx), 'lse': torch.empty(P, self.heads, **f32), 'M': torch.empty(P, H, **f32), 'M_hl': pair(self.ldx),
+             'Z': torch.empty(P, A, **f32), 'score': torch.empty(P, **f32), 'plse': torch.empty(P, **f32),
+             'Hs': torch.empty(P, H, **f32), 'dH': torch.empty(P, H, **f32), 'dM': torch.empty(P, H, **f32), 'dM_hl': pair(self.ldx),
+             'dZ_hl': pair(self.lda), 'dO': torch.empty(P, H, **f32), 'dQKV_hl': pair(self.ld3), 'ws': torch.empty(B, A, **f32)}
+        b['O_hl'][0][:, H] = 1.0      # [O | 1]: the kernel writes columns [0, H)
+        self._buf, self._cap = b, (P, B)
+        return b
+
+    def _refresh(self):
+        """The bf16 hi / lo operands of W~_in, W~_out and W~_a from theta."""
+        for g, r in self._rows.items():
+            hi, lo = self.W_hl[g]
+            call('dae_split_bf16', self._theta(g).data_ptr(), r, self.dim + 1, self.dim + 1, hi.data_ptr(), lo.data_ptr(), self.ldx, -1,
+                 1.0, _stream())
+
+    def _layout(self, pk):
+        """off (int64 [T + 1]) and the users' window lengths (int32 [B]) on the device, and T."""
+        return (_upload(pk.off.astype(np.int64), self.device), _upload(pk.L.astype(np.int32), self.device), len(pk.n))
+
+    # ---- training ---------------------------------------------------------------------------------------------------------
+    def _forward(self, b, pk, emb, items, st):
+        H, A, P = self.dim, self.attention_dim, pk.P
+        self._dev_layout = off, lens, T = self._layout(pk)
+        X_hi, X_lo = b['X_hl']
+        call('dae_gather_split_bf16', emb.data_ptr(), emb.stride(0), items.data_ptr(), P, H, X_hi.data_ptr(), X_lo.data_ptr(), self.ldx,
+             H, st)
+        self._gemm(P, 3 * H, H + 1, b['X_hl'], 0, self.W_hl['in'], 0, b['QKV'], 3 * H)
+        self._mark('input_projection')
+        O_hi, O_lo = b['O_hl']
+        call('dae_seq_attention_fwd', pk.B, T, off.data_ptr(), lens.data_ptr(), H, self.heads, b['QKV'].data_ptr(), 3 * H,
+             b['O'].data_ptr(), H, O_hi.data_ptr(), O_lo.data_ptr(), self.ldx, b['lse'].data_ptr(), self.heads, st)
+        self._mark('attention')
+        self._gemm(P, H, H + 1, b['O_hl'], 0, self.W_hl['out'], 0, b['M'], H)
+        M_hi, M_lo = b['M_hl']
+        call('dae_split_bf16', b['M'].data_ptr(), P, H, H, M_hi.data_ptr(), M_lo.data_ptr(), self.ldx, H, 1.0, st)
+        self._gemm(P, A, H + 1, b['M_hl'], 0, self.W_hl['pool'], 0, b['Z'], A)
+        self._mark('output_projection')
+        call('dae_seq_pool_fwd', pk.B, T, off.data_ptr(), lens.data_ptr(), H, A, b['Z'].data_ptr(), A, self._theta('query').data_ptr(),
+             b['M'].data_ptr(), H, b['Hs'].data_ptr(), H, b['score'].data_ptr(), b['plse'].data_ptr(), st)
+        self._mark('pooling')
+
+    def _backward(self, b, pk, st):
+        H, A, P = self.dim, self.attention_dim, pk.P
+        off, lens, T = self._dev_layout
+        dZ_hi, dZ_lo = b['dZ_hl']
+        call('dae_seq_pool_bwd', pk.B, T, off.data_ptr(), lens.data_ptr(), H, A, b['dH'].data_ptr(), H, b['Hs'].data_ptr(), H,
+             b['M'].data_ptr(), H, b['Z'].data_ptr(), A, self._theta('query').data_ptr(), b['score'].data_ptr(), b['plse'].data_ptr(),
+             b['dM'].data_ptr(), H, dZ_hi.data_ptr(), dZ_lo.data_ptr(), self.lda, self._theta('query', self.grad).data_ptr(),
+             b['ws'].data_ptr(), st)
+        self._gemm(P, H, A, b['dZ_hl'], 0, self.W_hl['pool'], 1, b['dM'], H, accumulate=1)
+        dM_hi, dM_lo = b['dM_hl']
+        call('dae_split_bf16', b['dM'].data_ptr(), P, H, H, dM_hi.data_ptr(), dM_lo.data_ptr(), self.ldx, -1, 1.0, st)
+        self._mark('pooling_backward')
+        self._gemm(P, H, H, b['dM_hl'], 0, self.W_hl['out'], 1, b['dO'], H)
+        dQ_hi, dQ_lo = b['dQKV_hl']
+        call('dae_seq_attention_bwd', pk.B, T, off.data_ptr(), lens.data_ptr(), H, self.heads, b['QKV'].data_ptr(), 3 * H,
+             b['O'].data_ptr(), H, b['lse'].data_ptr(), self.heads, b['dO'].data_ptr(), H, dQ_hi.data_ptr(), dQ_lo.data_ptr(), self.ld3,
+             st)
+        self._mark('attention_backward')
+        for g, dA, Bop in (('in', 'dQKV_hl', 'X_hl'), ('out', 'dM_hl', 'O_hl'), ('pool', 'dZ_hl', 'M_hl')):
+            self._gemm(self._rows[g], H + 1, P, b[dA], 1, b[Bop], 1, self._theta(g, self.grad), H + 1, k_splits=-1)
+        self._mark('weight_gradients')
+
+    def _step_split(self):
+        return None, None, 0, 0, 0
+
+    # ---- inference --------------------------------------------------------------------------------------------------------
+    def _infer_buffers(self, B):
+        self._refresh()
+        return None
+
+    def _states(self, pk, emb):
+        """Hs of every position of pk (one forward pass)."""
+        b = self._buffers(pk.P, pk.B)
+        self._forward(b, pk, emb, _upload(pk.items, self.device), _stream())
+        return b['Hs']
+
+    def _last_states(self, pk, emb, s):
+        last = pk.off[pk.L - 1] + np.arange(pk.B)
+        return self._states(pk, emb).index_select(0, _upload(last.astype(np.int64), self.device))
+
+    def _run_capture(self, pk, emb, s, cap_step, cap_row, cap_imp, out):
+        cap = _upload(np.stack([pk.off[cap_step] + cap_row, cap_imp]).astype(np.int64), self.device)
+        out.index_copy_(0, cap[1], self._states(pk, emb).index_select(0, cap[0]))
 
 
 def history_matrix(indptr, items, n_items):

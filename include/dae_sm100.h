@@ -653,6 +653,37 @@ int dae_lstm_cell_bwd(int32_t n, int32_t H, const float* dh_in, int64_t ld_dh_in
                       float* carry_c, int64_t ld_carry_c, const float* gates, int64_t ld_gates, const float* c, int64_t ld_c,
                       const float* c_prev, int64_t ld_cprev, void* da_hi, void* da_lo, int64_t ld_da, void* stream);
 
+/* ---- attention user encoder over reading sequences (DESIGN 4.17) -----------------------------------------------------------
+ * NRMS's user encoder made causal, in the packed layout above: batch user i (of B) has lens[i] reads (int32, device), read t at
+ * position off[t] + i (off: int64 [T + 1], device; lens[i] <= T <= 1024 must hold, the kernels trust it).  H = heads x d with head
+ * dim d <= 128.  The projections QKV = [X | 1].[W_in | b_in]^T, M = [O | 1].[W_out | b_out]^T and Z = [M | 1].[W_a | b_a]^T are
+ * dae_gemm_bf16x3 calls.  Every output element is written by one thread in a fixed order: the same bits on every run.
+ * dae_seq_attention_fwd: per (user, head), with q, k, v the head's columns [h d, (h + 1) d) of QKV's thirds (ld_qkv >= 3H),
+ *   O_t = sum_{s <= t} softmax_s(q_t . k_s / sqrt(d)) v_s.  Writes O (fp32, columns [0, H)), its bf16 hi / lo split (columns
+ *   [0, H) of o_hi / o_lo [.. x ld_split]; the caller keeps column H at 1 for the bias) and lse[p * ld_lse + h], the log-sum-exp
+ *   of row p's scaled scores.
+ * dae_seq_attention_bwd: from QKV, O, lse and dO (ld_do >= H) writes dQKV = [dQ | dK | dV] as bf16 hi / lo rows (columns [0, 3H),
+ *   ld_dqkv >= 3H), the operand of [dW_in | db_in] = dQKV^T.[X | 1].  The probabilities are recomputed from lse.
+ * dae_seq_pool_fwd: a_s = q . tanh(Z_s) (Z: ld_z >= A, q: [A]) -> score[p], the prefix log-sum-exp lse_t = log sum_{s <= t} e^{a_s}
+ *   -> plse[p], and u_t = sum_{s <= t} e^{a_s - lse_t} M_s -> u (ld_u >= H).
+ * dae_seq_pool_bwd: from dU (du), u, M, Z, q, score and plse writes dM (fp32, ld_dm >= H; the value path sum_{t >= s} w_ts dU_t),
+ *   dZ = da q (1 - tanh^2 Z) as bf16 hi / lo (columns [0, A), ld_dz >= A) with da_s = sum_{t >= s} w_ts dU_t . (M_s - u_t), and
+ *   dq[k] = sum_s da_s tanh Z_s[k] (fp32 [A], stored; a fixed-order sum over users).  workspace: B x A floats.  The scorer path
+ *   of dM is the caller's GEMM dM += dZ.W_a.
+ */
+int dae_seq_attention_fwd(int32_t B, int32_t T, const int64_t* off, const int32_t* lens, int32_t H, int32_t heads, const float* qkv,
+                          int64_t ld_qkv, float* o, int64_t ld_o, void* o_hi, void* o_lo, int64_t ld_split, float* lse, int64_t ld_lse,
+                          void* stream);
+int dae_seq_attention_bwd(int32_t B, int32_t T, const int64_t* off, const int32_t* lens, int32_t H, int32_t heads, const float* qkv,
+                          int64_t ld_qkv, const float* o, int64_t ld_o, const float* lse, int64_t ld_lse, const float* dout, int64_t ld_do,
+                          void* dqkv_hi, void* dqkv_lo, int64_t ld_dqkv, void* stream);
+int dae_seq_pool_fwd(int32_t B, int32_t T, const int64_t* off, const int32_t* lens, int32_t H, int32_t A, const float* z, int64_t ld_z,
+                     const float* q, const float* m, int64_t ld_m, float* u, int64_t ld_u, float* score, float* plse, void* stream);
+int dae_seq_pool_bwd(int32_t B, int32_t T, const int64_t* off, const int32_t* lens, int32_t H, int32_t A, const float* du, int64_t ld_du,
+                     const float* u, int64_t ld_u, const float* m, int64_t ld_m, const float* z, int64_t ld_z, const float* q,
+                     const float* score, const float* plse, float* dm, int64_t ld_dm, void* dz_hi, void* dz_lo, int64_t ld_dz, float* dq,
+                     void* workspace, void* stream);
+
 /* ---- impression logs (DESIGN 4.13) ------------------------------------------------------------------------------------------
  * An impression is a list of shown articles items[indptr[i] .. indptr[i + 1]) (rows of emb) with clicked[k] != 0 where the article
  * was clicked; C and N are its clicked and not-clicked articles.  One warp per row of work; lists of any length are walked in

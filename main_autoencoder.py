@@ -106,9 +106,15 @@ def build_parser():
                          'the training embeddings, save user_gru.npz and user_gru_top_k_{index,score}.npy; with targets report '
                          'user_gru_hit_rate / user_gru_recall next to the mean profile\'s for the same reads')
     ap.add_argument('--user_epochs', type=int, default=5, help='with --user_sequences: training epochs of the GRU user encoder')
-    ap.add_argument('--user_cell', default='gru', choices=['gru', 'lstm'],
-                    help='with --user_sequences: the user encoder\'s recurrent cell, user_model.UserGRU (gru, the default) or '
-                         'user_model.UserLSTM (lstm); with lstm the files and keys say user_lstm in place of user_gru')
+    ap.add_argument('--user_cell', default='gru', choices=['gru', 'lstm', 'attention'],
+                    help='with --user_sequences: the user encoder, user_model.UserGRU (gru, the default), user_model.UserLSTM (lstm) '
+                         'or user_model.UserAttention (attention: NRMS\'s causal self-attention and additive pooling); the files '
+                         'and keys say user_<cell> in place of user_gru')
+    ap.add_argument('--user_heads', type=int, default=None,
+                    help='with --user_cell attention: attention heads, a divisor of the embedding width with at most 128 '
+                         'columns per head (default: its largest divisor <= 20)')
+    ap.add_argument('--user_attention_dim', type=int, default=None,
+                    help='with --user_cell attention: width of the additive pooling layer (default 200)')
     ap.add_argument('--user_impressions', default='',
                     help='with --user_sequences: an .npz impression log (user, time, indptr, items, clicked; see '
                          'user_model.check_impressions) to train the GRU on instead of random negatives')
@@ -189,6 +195,11 @@ def check_flags(F):
     for flag, v in (('--user_impression_loss', F.user_impression_loss), ('--user_negatives', F.user_negatives)):
         assert v is None or F.user_impressions, '%s needs --user_impressions' % flag
     F.user_impression_loss = F.user_impression_loss or 'pairwise'
+    for flag, v in (('--user_heads', F.user_heads), ('--user_attention_dim', F.user_attention_dim)):
+        assert v is None or F.user_cell == 'attention', '%s needs --user_cell attention' % flag
+    assert F.user_heads is None or F.user_heads >= 1, '--user_heads must be >= 1'
+    F.user_attention_dim = 200 if F.user_attention_dim is None else F.user_attention_dim
+    assert F.user_attention_dim >= 1, '--user_attention_dim must be >= 1'
     F.user_negatives = 4 if F.user_negatives is None else F.user_negatives
     assert 0 <= F.user_negatives <= 32, '--user_negatives %d: 0 <= K <= 32' % F.user_negatives
     assert not F.user_targets or F.user_histories, '--user_targets needs --user_histories'
@@ -512,23 +523,24 @@ def load_user_impressions(F, n_train, seqs):
 
 
 def recommend_users_sequences(F, model, enc, seqs, impressions=(None, None)):
-    """--user_sequences: train a recurrent user encoder (--user_cell: UserGRU or UserLSTM) on the training embeddings, save it as
+    """--user_sequences: train a user encoder (--user_cell: UserGRU, UserLSTM or UserAttention) on the training embeddings, save it as
     user_<cell>.npz and the --top_k best unread articles per user as user_<cell>_top_k_{index,score}.npy; with targets, the hit
     rate and recall of the encoder's and of the mean profile's recommendations for the same reads are returned and printed.
     impressions: (train, test) from load_user_impressions; the encoder trains on train's impressions when given, and test's are
     scored by the encoder's states and by the mean profiles of the same reads."""
     import scipy.sparse as sp
     from dae_rnn_news_recommendation_b200 import helpers
-    from dae_rnn_news_recommendation_b200.user_model import UserGRU, UserLSTM, history_matrix, prefix_histories
+    from dae_rnn_news_recommendation_b200.user_model import UserAttention, UserGRU, UserLSTM, history_matrix, prefix_histories
     indptr, items, targets = seqs
     train_imp, test_imp = impressions
     cell = F.user_cell
     label = cell.upper()
     print('train a %s user encoder on %d users (%d reads, %d epochs%s)' % (label, len(indptr) - 1, items.size, F.user_epochs,
                                                                          ', impressions' if train_imp is not None else ''))
-    enc_cls = {'gru': UserGRU, 'lstm': UserLSTM}[cell]
+    kw = dict(heads=F.user_heads, attention_dim=F.user_attention_dim) if cell == 'attention' else {}
+    enc_cls = {'gru': UserGRU, 'lstm': UserLSTM, 'attention': UserAttention}[cell]
     rnn = enc_cls(enc.shape[1], num_epochs=F.user_epochs, seed=max(F.seed, 0), impression_loss=F.user_impression_loss,
-                  impression_negatives=F.user_negatives)
+                  impression_negatives=F.user_negatives, **kw)
     rnn.fit((indptr, items), enc, impressions=train_imp)
     if train_imp is not None:
         print('impressions: %(used)d used, %(skipped)d skipped' % rnn.impression_counts)
