@@ -487,6 +487,7 @@ int dae_auroc_count(const float* queries, int64_t n_queries, const float* sorted
  *   independent of atomic order and launch shape) and sums fp64 [2] (the fp32 scores of each group summed in fp64, for the mean).
  *   The AUROC on the grid, twice_u = sum_b n_r[b] (2 sum_{b' < b} n_u[b'] + n_u[b]), differs from the exact AUROC of the same
  *   fp32 scores by at most sum_b n_r[b] n_u[b] / (2 R U); helpers.auroc_from_histograms computes both on the host.
+ * NaN scores (a row holding NaN or inf): a NaN score is counted in bin 0 of its group, and that group's sums entry becomes NaN.
  * Every argument is checked before any CUDA call; n >= 2.
  * dae_similarity_pair_hist_bf16x3: S = X.X^T of dense rows (bf16 hi / lo pair [n x ldx], ldx >= dim and a multiple of 8, 16-byte
  *   aligned, e.g. from dae_rownorm_split_bf16) on the tensor cores, bf16x3 as dae_similarity_topk_bf16x3; only the tiles on and
