@@ -366,10 +366,14 @@ int dae_similarity_topk_workspace(int32_t n_query, int32_t n_corpus, int32_t k, 
 
 /* ---- k most similar articles of sparse (bag-of-words) vectors ------------------------------------------------------
  * dae_csr_similarity_topk: the same selection as dae_similarity_topk_bf16x3 for S[q, c] = sum_f Q[q, f] C[c, f] of two CSR
- *   matrices (indptr int64, indices int32 sorted inside a row, values fp32; q_features == c_features), on the CUDA cores and
- *   without forming S.  Every corpus row is a candidate, a row sharing no column with q included (score 0), except column
- *   q + diag_offset when `exclude` is set; order (score desc, index asc); padding -1 / -inf.  Each score accumulates in fp32 from
- *   0, one term per shared column in increasing column order, each term the product rounded to fp32 and then added (no FMA), so
+ *   matrices (indptr int64, indices int32 strictly increasing inside a row, values fp32; q_features == c_features), on the CUDA
+ *   cores and without forming S.  A column may appear only once in a row, in Q and in C: the kernels bucket the corpus entries by
+ *   (2048-row range, column) and add a bucket's entries into distinct accumulators at once, so a repeated column would race
+ *   (scipy's sum_duplicates() / sort_indices() give the required form; helpers canonicalise every matrix they upload).  Every
+ *   corpus row is a candidate, a row sharing no column with q included (score 0), except column q + diag_offset when `exclude`
+ *   is set; order (score desc, index asc); padding -1 / -inf.  A NaN or -inf score is never a candidate, so a row whose every
+ *   candidate scores NaN or -inf (a stored 0 times inf gives NaN) is all padding; +inf is listed.  Each score accumulates in fp32
+ *   from 0, one term per shared column in increasing column order, each term the product rounded to fp32 and then added (no FMA), so
  *   the output does not depend on `splits` (> 0: the number of corpus parts, 0: automatic) and a float32 host loop over the
  *   columns reproduces it exactly.  1 <= k <= 32; corpus nnz < 2^31; workspace 16-byte aligned, at least
  *   dae_csr_similarity_topk_workspace bytes for the same n_query, n_corpus, c_nnz, features, k and splits.
