@@ -23,6 +23,31 @@ extern "C" int dae_last_error(char* buf, size_t len) {
 
 namespace dae {
 
+// Label classes are those of the reference's tf.equal: -0.0 and +0.0 are one class, and a NaN label equals nothing, itself included,
+// so every NaN row is a class of one.  The sorts compare one total-order key per label: the float's bits mapped to an unsigned
+// integer that orders like the value, -0.0 folded into +0.0 and every NaN mapped to the largest key, after +inf.  Ties (one class,
+// or the NaN rows) are broken by row id, so the order is ascending (label, row id) with the NaN rows last in row-id order.
+constexpr uint32_t kNanKey = 0xffffffffu;
+__device__ __forceinline__ uint32_t label_key(float x) {
+  if (x != x) return kNanKey;
+  const uint32_t u = __float_as_uint(x) == 0x80000000u ? 0u : __float_as_uint(x);
+  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+__device__ __forceinline__ bool pair_greater(uint32_t ka, int va, uint32_t kb, int vb) { return (ka > kb) || (ka == kb && va > vb); }
+
+// class segment of sorted position i: [first index with key k, one past the last) by binary searches in keys[0, B); a NaN row is
+// the class [i, i + 1)
+__device__ __forceinline__ void class_segment(const uint32_t* keys, int B, int i, int32_t* lo, int32_t* hi) {
+  const uint32_t k = keys[i];
+  if (k == kNanKey) { lo[i] = i; hi[i] = i + 1; return; }
+  int a = 0, b = i;               // lower bound in [0, i]
+  while (a < b) { const int m = (a + b) >> 1; if (keys[m] < k) a = m + 1; else b = m; }
+  lo[i] = a;
+  a = i + 1; b = B;               // upper bound in (i, B]
+  while (a < b) { const int m = (a + b) >> 1; if (keys[m] <= k) a = m + 1; else b = m; }
+  hi[i] = a;
+}
+
 // One CTA. Orders the batch rows by label (bitonic sort in smem), derives class segments and the
 // closed-form batch_all data weights:
 //   w_i = 2(n-1)(B-n) + sum_{c != c_i} n_c(n_c-1),   N_valid = sum_c n_c(n_c-1)(B-n_c)
@@ -35,11 +60,12 @@ __global__ void __launch_bounds__(1024) batch_prepare_kernel(
     int32_t* seg_hi, float* __restrict__ weight_out, double* __restrict__ stats, int64_t n_perm) {
   if (ctl) offset += ctl[0];  // device-resident batch cursor (CUDA-graph replay)
   if (n_perm > 0 && offset + B > n_perm) return;  // staging the batch AFTER the epoch's last one: nothing to prepare
-  __shared__ float keys[kMaxB];
+  __shared__ uint32_t keys[kMaxB];
   __shared__ int vals[kMaxB];
   __shared__ double red[32];
   int32_t* lo = seg_lo;
   int32_t* hi = seg_hi;
+  const bool labelled = strategy != DAE_TRIPLET_NONE && labels_all;
   const int tid = threadIdx.x, nt = blockDim.x;
   int P = 1;
   while (P < B) P <<= 1;
@@ -47,21 +73,22 @@ __global__ void __launch_bounds__(1024) batch_prepare_kernel(
     if (i < B) {
       const int r = perm ? perm[offset + i] : (int)(offset + i);
       vals[i] = r;
-      keys[i] = (strategy != DAE_TRIPLET_NONE && labels_all) ? labels_all[r] : 0.0f;
+      keys[i] = labelled ? label_key(labels_all[r]) : label_key(0.0f);
     } else {
       vals[i] = 0x7fffffff;
-      keys[i] = __int_as_float(0x7f800000);  // +inf sorts last
+      keys[i] = kNanKey;  // (largest key, largest row id): the padding sorts last
     }
   }
   __syncthreads();
   if (strategy != DAE_TRIPLET_NONE && P <= 1024) {
     // bitonic sort with one element per thread held in registers: partner exchange by warp shuffle for strides < 32
-    // (40 of the 55 stages at P = 1024), through shared memory otherwise
-    float key = keys[tid < P ? tid : 0];
+    // (40 of the 55 stages at P = 1024), through shared memory otherwise.  Both partners evaluate the one predicate
+    // pair_greater(lower, upper), so every compare-exchange swaps the pair or keeps it: the network permutes its inputs.
+    uint32_t key = keys[tid < P ? tid : 0];
     int val = vals[tid < P ? tid : 0];
     for (int k = 2; k <= P; k <<= 1) {
       for (int j = k >> 1; j > 0; j >>= 1) {
-        float okey; int oval;
+        uint32_t okey; int oval;
         if (j < 32) {
           okey = __shfl_xor_sync(0xffffffffu, key, j);
           oval = __shfl_xor_sync(0xffffffffu, val, j);
@@ -73,9 +100,8 @@ __global__ void __launch_bounds__(1024) batch_prepare_kernel(
           oval = vals[(tid ^ j) & (P - 1)];
         }
         const bool up = ((tid & k) == 0), is_lower = ((tid & j) == 0);
-        const bool other_less = (okey < key) || (okey == key && oval < val);
-        const bool take_other = (up == is_lower) ? other_less : !other_less && !(okey == key && oval == val);
-        if (take_other) { key = okey; val = oval; }
+        const bool gt = is_lower ? pair_greater(key, val, okey, oval) : pair_greater(okey, oval, key, val);
+        if (gt == up) { key = okey; val = oval; }
       }
     }
     __syncthreads();
@@ -87,11 +113,10 @@ __global__ void __launch_bounds__(1024) batch_prepare_kernel(
         for (int i = tid; i < P; i += nt) {
           const int ixj = i ^ j;
           if (ixj > i) {
-            const float ka = keys[i], kb = keys[ixj];
+            const uint32_t ka = keys[i], kb = keys[ixj];
             const int va = vals[i], vb = vals[ixj];
-            const bool gt = (ka > kb) || (ka == kb && va > vb);
             const bool up = ((i & k) == 0);
-            if (gt == up) {
+            if (pair_greater(ka, va, kb, vb) == up) {
               keys[i] = kb; keys[ixj] = ka;
               vals[i] = vb; vals[ixj] = va;
             }
@@ -101,16 +126,7 @@ __global__ void __launch_bounds__(1024) batch_prepare_kernel(
       }
     }
   }
-  // class segment of every row: [first index with this label, one past the last) -- binary searches in the sorted keys
-  for (int i = tid; i < B; i += nt) {
-    const float k = keys[i];
-    int a = 0, b = i;               // lower bound in [0, i]
-    while (a < b) { const int m = (a + b) >> 1; if (keys[m] < k) a = m + 1; else b = m; }
-    lo[i] = a;
-    a = i + 1; b = B;               // upper bound in (i, B]
-    while (a < b) { const int m = (a + b) >> 1; if (keys[m] <= k) a = m + 1; else b = m; }
-    hi[i] = a;
-  }
+  for (int i = tid; i < B; i += nt) class_segment(keys, B, i, lo, hi);
   __syncthreads();
   double t_part = 0.0, nv_part = 0.0;
   for (int i = tid; i < B; i += nt) {
@@ -123,7 +139,7 @@ __global__ void __launch_bounds__(1024) batch_prepare_kernel(
   for (int i = tid; i < B; i += nt) {
     const double n = (double)(hi[i] - lo[i]);
     rows_out[i] = vals[i];
-    if (labels_out) labels_out[i] = keys[i];
+    if (labels_out) labels_out[i] = labelled ? labels_all[vals[i]] : 0.0f;  // the label's own bits (-0.0, NaN payloads)
     if (weight_out) {
       float w = 1.0f;
       if (strategy == DAE_TRIPLET_BATCH_ALL) w = (float)(2.0 * (n - 1.0) * ((double)B - n) + T - n * (n - 1.0));
@@ -139,21 +155,20 @@ __global__ void __launch_bounds__(1024) batch_prepare_kernel(
   }
 }
 
-// B > kMaxB (up to DAE_MAX_TRIPLET_BATCH): the same outputs from one CTA that sorts inside the caller's buffers -- labels_out holds
-// the keys, rows_out the row ids.  The network is the bitonic sort whose every compare-exchange puts the smaller (label, row) pair at
-// the lower index (the first step of each merge compares mirrored positions), so the power-of-two padding needs no storage: a
-// virtual +inf at an index >= B never moves.  Partner distances below kMaxB run on aligned kMaxB-element blocks staged in shared
-// memory; only the longer ones (6 stages at B = 32768) go through global memory.  Rows end in ascending (label, row id) order, the
-// order batch_prepare_kernel produces.
-__device__ __forceinline__ bool pair_greater(float ka, int va, float kb, int vb) { return (ka > kb) || (ka == kb && va > vb); }
+// B > kMaxB (up to DAE_MAX_BLOCKED_BATCH): the same outputs from one CTA that sorts inside the caller's buffers -- labels_out holds
+// the keys (label_key bits) until the segments are known, rows_out the row ids.  The network is the bitonic sort whose every
+// compare-exchange puts the smaller (key, row) pair at the lower index (the first step of each merge compares mirrored positions),
+// so the power-of-two padding needs no storage: a virtual (largest key, largest row) at an index >= B never moves.  Partner
+// distances below kMaxB run on aligned kMaxB-element blocks staged in shared memory; only the longer ones (6 stages at B = 32768)
+// go through global memory.  Rows end in the order batch_prepare_kernel produces.
 
 // one global compare-exchange stage: pair t's lower index a (bit log2(j) clear), partner a + j, or its mirror a ^ (2j - 1) (flip)
-__device__ void prepare_global_stage(float* keys, int32_t* vals, int B, int P, int j, bool flip) {
+__device__ void prepare_global_stage(uint32_t* keys, int32_t* vals, int B, int P, int j, bool flip) {
   for (int t = threadIdx.x; t < P / 2; t += blockDim.x) {
     const int a = 2 * t - (t & (j - 1));
     const int b = flip ? (a ^ (2 * j - 1)) : a + j;
     if (b < B) {
-      const float ka = keys[a], kb = keys[b];
+      const uint32_t ka = keys[a], kb = keys[b];
       const int va = vals[a], vb = vals[b];
       if (pair_greater(ka, va, kb, vb)) { keys[a] = kb; keys[b] = ka; vals[a] = vb; vals[b] = va; }
     }
@@ -163,11 +178,11 @@ __device__ void prepare_global_stage(float* keys, int32_t* vals, int B, int P, i
 
 // the stages of merge size k with partner distances j < kMaxB, on each aligned kMaxB block in shared memory (k <= kMaxB: the whole
 // merge, flip step included)
-__device__ void prepare_local_stages(float* keys, int32_t* vals, int B, int k, float* sk, int* sv) {
+__device__ void prepare_local_stages(uint32_t* keys, int32_t* vals, int B, int k, uint32_t* sk, int* sv) {
   for (int b0 = 0; b0 < B; b0 += kMaxB) {
     for (int t = threadIdx.x; t < kMaxB; t += blockDim.x) {
       const bool ok = b0 + t < B;
-      sk[t] = ok ? keys[b0 + t] : __int_as_float(0x7f800000);
+      sk[t] = ok ? keys[b0 + t] : kNanKey;
       sv[t] = ok ? vals[b0 + t] : 0x7fffffff;
     }
     __syncthreads();
@@ -178,7 +193,7 @@ __device__ void prepare_local_stages(float* keys, int32_t* vals, int B, int k, f
         for (int t = threadIdx.x; t < kMaxB / 2; t += blockDim.x) {
           const int a = 2 * t - (t & (j - 1));
           const int b = flip ? (a ^ (2 * j - 1)) : a + j;
-          const float ka = sk[a], kb = sk[b];
+          const uint32_t ka = sk[a], kb = sk[b];
           const int va = sv[a], vb = sv[b];
           if (pair_greater(ka, va, kb, vb)) { sk[a] = kb; sk[b] = ka; sv[a] = vb; sv[b] = va; }
         }
@@ -196,16 +211,16 @@ __global__ void __launch_bounds__(1024) batch_prepare_large_kernel(
     double* __restrict__ stats, int64_t n_perm) {
   if (ctl) offset += ctl[0];
   if (n_perm > 0 && offset + B > n_perm) return;
-  __shared__ float sk[kMaxB];
+  __shared__ uint32_t sk[kMaxB];
   __shared__ int sv[kMaxB];
   __shared__ double red[32];
   const int tid = threadIdx.x, nt = blockDim.x;
-  float* keys = labels_out;
+  uint32_t* keys = reinterpret_cast<uint32_t*>(labels_out);
   int32_t* vals = rows_out;
   for (int i = tid; i < B; i += nt) {
     const int r = perm ? perm[offset + i] : (int)(offset + i);
     vals[i] = r;
-    keys[i] = labels_all[r];
+    keys[i] = label_key(labels_all[r]);
   }
   __syncthreads();
   int P = 1;
@@ -216,17 +231,9 @@ __global__ void __launch_bounds__(1024) batch_prepare_large_kernel(
     for (int j = k >> 2; j >= kMaxB; j >>= 1) prepare_global_stage(keys, vals, B, P, j, false);
     prepare_local_stages(keys, vals, B, k, sk, sv);
   }
-  // class segments: binary searches in the sorted labels (as batch_prepare_kernel)
-  for (int i = tid; i < B; i += nt) {
-    const float k = keys[i];
-    int a = 0, b = i;
-    while (a < b) { const int m = (a + b) >> 1; if (keys[m] < k) a = m + 1; else b = m; }
-    seg_lo[i] = a;
-    a = i + 1; b = B;
-    while (a < b) { const int m = (a + b) >> 1; if (keys[m] <= k) a = m + 1; else b = m; }
-    seg_hi[i] = a;
-  }
+  for (int i = tid; i < B; i += nt) class_segment(keys, B, i, seg_lo, seg_hi);
   __syncthreads();
+  for (int i = tid; i < B; i += nt) labels_out[i] = labels_all[vals[i]];  // keys -> the labels' own bits (-0.0, NaN payloads)
   double t_part = 0.0, nv_part = 0.0;
   for (int i = tid; i < B; i += nt) {
     const double n = (double)(seg_hi[i] - seg_lo[i]);
@@ -399,6 +406,9 @@ extern "C" int dae_batch_commit(int32_t B, const int32_t* rows_s, const float* l
 extern "C" int dae_batch_prepare_explicit(const int32_t* perm, int64_t offset, const int64_t* ctl, int32_t B, int64_t n_each,
                                           int32_t* rows_out, double* stats, void* stream) {
   DAE_REQUIRE(B >= 1 && n_each >= 1 && rows_out && stats, "dae_batch_prepare_explicit: bad arguments");
+  // the neg block's row ids r + 2 n_each (r < n_each) must fit in int32
+  DAE_REQUIRE(n_each <= INT32_MAX / 3, "dae_batch_prepare_explicit: n_each = %lld rows per block: the row ids of [org; pos; neg] "
+              "overflow int32 above %d", (long long)n_each, INT32_MAX / 3);
   dae::batch_rows_explicit_kernel<<<(B + 255) / 256, 256, 0, (cudaStream_t)stream>>>(perm, offset, ctl, B, n_each, rows_out, stats);
   DAE_CHECK_LAUNCH("dae_batch_prepare_explicit");
   return DAE_OK;

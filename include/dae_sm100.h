@@ -83,6 +83,9 @@ int dae_last_error(char* buf, size_t len);
  * for batch_all - the closed-form data weight w_i and N_valid.  strategy none: order kept, w = 1.
  * One CTA.  Triplet strategies: B <= DAE_MAX_TRIPLET_BATCH; up to 4096 rows the batch is sorted in shared memory, above that
  * inside labels_out / rows_out (labels_out must then be non-NULL).  The order is ascending (label, row id) either way.
+ * Classes are those of the reference's tf.equal: -0.0 and +0.0 are one class (ordered as one key, by row id); a NaN label equals
+ * nothing, so each NaN row is a class of one, [seg_lo, seg_hi) = [i, i + 1), and the NaN rows come last in row-id order.
+ * labels_out holds labels_all[rows_out] with their own bits.
  * stats: float64[DAE_STAT_SLOTS], zeroed here, SUM_W / N_VALID filled.
  * ctl (optional, device int64[4]): per-step cursors kept in device memory so that a captured CUDA graph of the
  * step can be replayed without host-side argument changes -- ctl[0] is added to `offset`, ctl[1] is the row of the
@@ -110,7 +113,8 @@ int dae_batch_commit(int32_t B, const int32_t* rows_s, const float* labels_s, co
                      const int32_t* seg_hi_s, const float* weight_s, const double* stats_s, int32_t* rows,
                      float* labels_b, int32_t* seg_lo, int32_t* seg_hi, float* weight, double* stats, void* stream);
 /* explicit (org, pos, neg) triplets (autoencoder/utils.py:73-91, autoencoder_triplet.py:106-147): rows_out[3B] = the batch's
- * rows in the three blocks of the stacked [org; pos; neg] matrix (n_each rows per block); stats zeroed, SUM_W = B. */
+ * rows in the three blocks of the stacked [org; pos; neg] matrix (n_each rows per block, n_each <= (2^31 - 1) / 3 so that every
+ * row id fits in int32); stats zeroed, SUM_W = B. */
 int dae_batch_prepare_explicit(const int32_t* perm, int64_t offset, const int64_t* ctl, int32_t B, int64_t n_each,
                                int32_t* rows_out, double* stats, void* stream);
 

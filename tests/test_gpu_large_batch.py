@@ -9,6 +9,7 @@ import numpy as np
 import pytest
 import torch
 
+import batch_prepare_oracle as bo
 from helpers import REL_TOL, rel_err, elem_err, xavier
 
 pytestmark = pytest.mark.gpu
@@ -36,17 +37,8 @@ def _t(a):
 
 
 def _expected_prepare(perm, offset, B, labels_all, strategy):
-    rows = perm[offset:offset + B]
-    lab = labels_all[rows]
-    o = np.lexsort((rows, lab))
-    rows, lab = rows[o], lab[o]
-    lo = np.searchsorted(lab, lab, side='left')
-    hi = np.searchsorted(lab, lab, side='right')
-    n = (hi - lo).astype(np.float64)
-    T = float(np.sum(n - 1.0))
-    NV = float(np.sum((n - 1.0) * (B - n)))
-    w = (2.0 * (n - 1.0) * (B - n) + T - n * (n - 1.0)).astype(np.float32) if strategy == 1 else np.zeros(B, np.float32)
-    return rows, lab, lo, hi, w, NV
+    rows, lab, lo, hi, w, stats = bo.prepare(perm, offset, B, labels_all, strategy)
+    return rows, lab, lo, hi, w, stats[bo.STAT_N_VALID]
 
 
 @pytest.mark.parametrize('B', [4097, 9800, 32768])
