@@ -7,7 +7,8 @@ import pytest
 import torch
 
 import gru_kernel_oracle as go
-from helpers import pair_value as _pair_value, snap as _snap, snap_vec as _snap_vec
+from encoder_stages import Recorder, check_log
+from helpers import pair_value as _pair_value
 
 from dae_rnn_news_recommendation_b200 import user_model
 from dae_rnn_news_recommendation_b200.user_model import Packed, UserGRU
@@ -238,109 +239,6 @@ def test_seq_negatives(n_items):
 # ---------------------------------------------------------------------------------------------------------------------------
 # the composed batch: every kernel call of UserGRU._forward_backward / transform against its own inputs
 # ---------------------------------------------------------------------------------------------------------------------------
-class Recorder:
-    """Stands in for user_model.call: snapshots each kernel's inputs, runs it, synchronizes and snapshots its outputs."""
-
-    def __init__(self, real):
-        self.real, self.log = real, []
-
-    def __call__(self, name, *a):
-        pre, post = {}, {}
-        if name == 'dae_gru_cell_fwd':
-            n, H = a[0], a[1]
-            pre = {'xp': _snap(a[2], n, a[3]), 'hp': _snap(a[4], n, a[5]), 'h_prev': _snap(a[6], n, a[7])}
-        elif name == 'dae_gru_cell_bwd':
-            n, H = a[0], a[1]
-            pre = {'dh_in': _snap(a[2], n, a[3]), 'carry': _snap(a[4], a[0], a[5]), 'gates': _snap(a[6], n, a[7]),
-                   'h_prev': _snap(a[8], n, a[9])}
-        elif name == 'dae_gemm_bf16x3':
-            M, N, K = a[0], a[1], a[2]
-            ra, rb = (K if a[7] else M), (K if a[11] else N)
-            pre = {'a': _pair_value(_snap(a[4], ra, a[6], 'u2'), _snap(a[5], ra, a[6], 'u2')),
-                   'b': _pair_value(_snap(a[8], rb, a[10], 'u2'), _snap(a[9], rb, a[10], 'u2')),
-                   'c': _snap(a[12], M, a[13]) if a[18] else None}
-        elif name == 'dae_seq_rank_loss':
-            pre = {'h': _snap(a[0], a[7], a[1]), 'pos': _snap_vec(a[5], a[7], '<i4'), 'neg': _snap_vec(a[6], a[7], '<i4'),
-                   'loss': _snap_vec(a[11], 1, '<f8')}
-        elif name == 'dae_seq_negatives':
-            pre = {'pos': _snap_vec(a[0], a[1], '<i4')}
-        elif name == 'dae_gather_split_bf16':
-            pre = {'rows': _snap_vec(a[2], a[3], '<i4')}
-        self.real(name, *a)
-        torch.cuda.synchronize()
-        if name == 'dae_gru_cell_fwd':
-            n, H = a[0], a[1]
-            post = {'h': _snap(a[8], n, a[9]), 'h_hi': _snap(a[11], a[10], a[13], 'u2') if a[11] else None,
-                    'h_lo': _snap(a[12], a[10], a[13], 'u2') if a[11] else None, 'gates': _snap(a[14], n, a[15]) if a[14] else None}
-        elif name == 'dae_gru_cell_bwd':
-            n = a[0]
-            post = {'carry': _snap(a[4], n, a[5])}
-            post.update({k: _snap(a[10 + i], n, a[14], 'u2') for i, k in enumerate(('dxp_hi', 'dxp_lo', 'dhp_hi', 'dhp_lo'))})
-        elif name == 'dae_gemm_bf16x3':
-            post = {'c': _snap(a[12], a[0], a[13])}
-        elif name == 'dae_seq_rank_loss':
-            post = {'dh': _snap(a[9], a[7], a[10]), 'loss': _snap_vec(a[11], 1, '<f8')}
-        elif name == 'dae_seq_negatives':
-            post = {'neg': _snap_vec(a[6], a[1], '<i4')}
-        elif name == 'dae_gather_split_bf16':
-            post = {'hi': _snap(a[5], a[3], a[7], 'u2'), 'lo': _snap(a[6], a[3], a[7], 'u2')}
-        self.log.append((name, a, pre, post))
-
-
-def _check_log(log, emb, H, tag):
-    """Every recorded kernel call against the fp64 reference of its own inputs; returns the calls by name."""
-    by = {}
-    prev_bwd_n = None
-    for name, a, pre, post in log:
-        by.setdefault(name, []).append((a, pre, post))
-        if name == 'dae_gru_cell_fwd':
-            n = a[0]
-            want = go.cell_fwd(pre['xp'], pre['hp'], pre['h_prev'], H)
-            go.check('%s fwd h' % tag, post['h'][:, :H], *want['h'], go.C_FP32)
-            if post['gates'] is not None:
-                for k, g in enumerate(('r', 'z', 'n')):
-                    go.check('%s fwd %s' % (tag, g), post['gates'][:, k * H:(k + 1) * H], *want[g], go.C_FP32)
-                assert np.array_equal(post['gates'][:, 3 * H:4 * H], pre['hp'][:, 2 * H:3 * H])
-            if post['h_hi'] is not None:
-                w_hi, w_lo = go.bf16_split(post['h'][:a[10], :H])
-                assert np.array_equal(post['h_hi'][:, :H], w_hi) and np.array_equal(post['h_lo'][:, :H], w_lo)
-        elif name == 'dae_gru_cell_bwd':
-            n = a[0]
-            c0 = pre['carry'][:, :H]
-            # rows of users whose last read is at this step carry nothing from later steps
-            lo_row = 0 if prev_bwd_n is None else prev_bwd_n
-            assert (c0[lo_row:] == 0).all(), '%s: carry rows [%d, %d) not zero' % (tag, lo_row, n)
-            prev_bwd_n = n
-            want = go.cell_bwd(pre['dh_in'], c0, pre['gates'], pre['h_prev'], H)
-            go.check('%s bwd carry' % tag, post['carry'][:, :H], *want['carry'], go.C_FP32)
-            for k, g in enumerate(('dr', 'dz', 'dn')):
-                sl = slice(k * H, (k + 1) * H)
-                go.check_pair('%s bwd %s' % (tag, g), post['dxp_hi'][:, sl], post['dxp_lo'][:, sl], *want[g], go.C_FP32)
-            assert np.array_equal(post['dhp_hi'][:, :2 * H], post['dxp_hi'][:, :2 * H])
-            assert np.array_equal(post['dhp_lo'][:, :2 * H], post['dxp_lo'][:, :2 * H])
-            go.check_pair('%s bwd r dn' % tag, post['dhp_hi'][:, 2 * H:3 * H], post['dhp_lo'][:, 2 * H:3 * H], *want['rdn'], go.C_FP32)
-        elif name == 'dae_gemm_bf16x3':
-            M, N, K = a[0], a[1], a[2]
-            A = pre['a'].T[:M, :K] if a[7] else pre['a'][:M, :K]
-            B = pre['b'].T[:N, :K] if a[11] else pre['b'][:N, :K]
-            want, s = go.gemm_nt(A, B)
-            want, s = a[3] * want, abs(a[3]) * s
-            if a[18]:
-                want, s = want + pre['c'][:, :N], s + np.abs(pre['c'][:, :N])
-            go.check('%s gemm %dx%dx%d' % (tag, M, N, K), post['c'][:, :N], want, s, go.C_BF16X3)
-        elif name == 'dae_seq_rank_loss':
-            w_dh, s_dh, lt, s_lt = go.seq_rank_loss(pre['h'], emb, pre['pos'], pre['neg'], a[8], H)
-            go.check('%s loss dh' % tag, post['dh'][:, :H], w_dh, s_dh, go.C_FP32)
-            assert (post['dh'][pre['pos'] < 0, :H] == 0).all()
-            go.check('%s loss sum' % tag, post['loss'][0] - pre['loss'][0], lt.sum(), s_lt.sum(), go.C_FP32, tiny=1e-15)
-        elif name == 'dae_seq_negatives':
-            assert np.array_equal(post['neg'], go.seq_negatives(pre['pos'], a[2], a[3], a[4], a[5]))
-        elif name == 'dae_gather_split_bf16':
-            w_hi, w_lo = go.gather_split(emb, pre['rows'], a[4], a[7], a[8])
-            assert np.array_equal(post['hi'], w_hi) and np.array_equal(post['lo'], w_lo)
-    return by
-
-
 def _data(U, H, N, max_len, seed):
     rng = np.random.default_rng(seed)
     lens = rng.integers(1, max_len + 4, U)
@@ -376,7 +274,7 @@ def test_training_batch_every_stage(H, U, max_len, monkeypatch):
     m._optimizer_step()
     torch.cuda.synchronize()
     tag = 'train H=%d U=%d' % (H, U)
-    by = _check_log(rec.log, emb, H, tag)
+    by = check_log(rec.log, emb, H, tag)
     T = len(pk.n)
     assert len(by['dae_gru_cell_fwd']) == T and len(by['dae_gru_cell_bwd']) == T
     # the recurrent GEMM of step t reads [h_{t-1} | 1 | 0 ...]: the forward cell's fp32 states of step t-1, bit for bit
@@ -412,7 +310,7 @@ def test_transform_every_stage(monkeypatch):
     rec = Recorder(user_model.call)
     monkeypatch.setattr(user_model, 'call', rec)
     out = m.transform((indptr, items), emb)
-    by = _check_log(rec.log, emb, H, 'transform')
+    by = check_log(rec.log, emb, H, 'transform')
     for a, pre, post in by['dae_gru_cell_fwd']:
         assert a[6] == a[8] and a[10] == a[0] and a[14] is None       # h_out == h_prev, n_split = n, no gates
     assert out.shape == (U, H) and np.isfinite(out).all()

@@ -1,5 +1,5 @@
 """The impression kernels (csrc/impressions.cu) through the C ABI against the fp64 references of tests/impression_kernel_oracle.py,
-element by element, and every dae_impression_rank_loss call of real UserGRU / UserLSTM impression batches against its own
+element by element, and every dae_impression_rank_loss call of real UserGRU / UserLSTM / UserAttention impression batches against its own
 inputs.  Outputs start as sentinels, every operand has its own leading dimension with NaN in the padding, and the row counts run
 the grid-stride loops past three passes, so a wrong stride, a skipped row or a write past the end fails."""
 import numpy as np
@@ -11,7 +11,8 @@ import impression_oracle as io
 from helpers import snap, snap_vec
 
 from dae_rnn_news_recommendation_b200 import _cabi, helpers, user_model
-from dae_rnn_news_recommendation_b200.user_model import ImpressionBatch, Packed, UserGRU, UserLSTM, check_impressions, usable_impressions
+from dae_rnn_news_recommendation_b200.user_model import (ImpressionBatch, Packed, UserAttention, UserGRU, UserLSTM, check_impressions,
+                                                         usable_impressions)
 
 pytestmark = pytest.mark.gpu
 DEV = 'cuda:0'
@@ -205,7 +206,10 @@ class LossRecorder:
 
 
 SENTINEL_BUFFERS = {UserGRU: (('XP', 'HP', 'Hs', 'gates', 'dH', 'carry'), ('X_hl', 'dXP_hl', 'dHP_hl')),
-                    UserLSTM: (('XP', 'HP', 'Hs', 'Cs', 'gates', 'dH', 'carry', 'carry_c'), ('X_hl', 'dA_hl'))}
+                    UserLSTM: (('XP', 'HP', 'Hs', 'Cs', 'gates', 'dH', 'carry', 'carry_c'), ('X_hl', 'dA_hl')),
+                    # O_hl keeps the ones column _buffers gave it: no kernel writes column H
+                    UserAttention: (('QKV', 'O', 'lse', 'M', 'Z', 'score', 'plse', 'Hs', 'dH', 'dM', 'dO', 'ws'),
+                                    ('X_hl', 'M_hl', 'dM_hl', 'dZ_hl', 'dQKV_hl'))}
 
 
 def _data(U, H, N, max_len, seed):
@@ -233,7 +237,7 @@ def _impressions(rng, indptr, N, per_user=3):
             'items': np.concatenate(lists).astype(np.int32), 'clicked': np.concatenate(clicks).astype(np.uint8)}
 
 
-@pytest.mark.parametrize('cell', [UserGRU, UserLSTM])
+@pytest.mark.parametrize('cell', [UserGRU, UserLSTM, UserAttention])
 def test_training_batch_loss_calls(cell, monkeypatch):
     H, N, max_len = 37, 900, 10
     U = 4 * _pass_rows() // 6                                        # about 6.5 positions per user: P past three passes

@@ -1,6 +1,7 @@
 """The sampled-softmax impression loss on the GPU: dae_impression_softmax_loss through the C ABI against the fp64 reference of
 tests/impression_softmax_oracle.py element by element, the drawn sets themselves bit for bit against the host draws, whole
-UserGRU / UserLSTM batches against fp64 autograd, the K = 1 reduction to the pairwise fit, the learning check and the CLI."""
+UserGRU / UserLSTM / UserAttention batches against fp64 autograd, the K = 1 reduction to the pairwise fit, the learning check and
+the CLI."""
 import os
 import sys
 
@@ -10,12 +11,14 @@ import torch
 
 import impression_kernel_oracle as ko
 import impression_softmax_oracle as so
+import user_attention_oracle as ao
 from helpers import rel_err
 from user_gru_oracle import NAMES, gru_states
 from user_lstm_oracle import lstm_states
 
 from dae_rnn_news_recommendation_b200 import _cabi, helpers
-from dae_rnn_news_recommendation_b200.user_model import ImpressionBatch, Packed, UserGRU, UserLSTM, check_impressions, usable_impressions
+from dae_rnn_news_recommendation_b200.user_model import (ATTENTION_NAMES, ImpressionBatch, Packed, UserAttention, UserGRU, UserLSTM,
+                                                         check_impressions, usable_impressions)
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -177,12 +180,15 @@ def _impressions(rng, indptr, N, per_user=3, shown=(2, 16)):
 
 
 SENTINELS = {UserGRU: (('XP', 'HP', 'Hs', 'gates', 'dH', 'carry'), ('X_hl', 'dXP_hl', 'dHP_hl')),
-             UserLSTM: (('XP', 'HP', 'Hs', 'Cs', 'gates', 'dH', 'carry', 'carry_c'), ('X_hl', 'dA_hl'))}
+             UserLSTM: (('XP', 'HP', 'Hs', 'Cs', 'gates', 'dH', 'carry', 'carry_c'), ('X_hl', 'dA_hl')),
+             # O_hl keeps the ones column _buffers gave it: no kernel writes column H
+             UserAttention: (('QKV', 'O', 'lse', 'M', 'Z', 'score', 'plse', 'Hs', 'dH', 'dM', 'dO', 'ws'),
+                             ('X_hl', 'M_hl', 'dM_hl', 'dZ_hl', 'dQKV_hl'))}
 
 
 @pytest.mark.parametrize('K', [4, 0])
 @pytest.mark.parametrize('H,U,max_len', [(37, 200, 10), (500, 100, 8)])
-@pytest.mark.parametrize('cell', [UserGRU, UserLSTM])
+@pytest.mark.parametrize('cell', [UserGRU, UserLSTM, UserAttention])
 def test_batch_gradients_against_autograd(cell, H, U, max_len, K):
     N, seed, epoch = 900, 4, 2
     indptr, items, emb = _data(U, H, N, max_len, seed=H + 1)
@@ -206,20 +212,35 @@ def test_batch_gradients_against_autograd(cell, H, U, max_len, K):
     loss = float(m.stats.item()) / ib.clicks
     seqs = [pk.items[[pk.position(i, t) for t in range(int(pk.L[i]))]] for i in range(pk.B)]
     row = {int(u): i for i, u in enumerate(pk.order)}
-    params = {k: torch.tensor(v.double().numpy(), requires_grad=True) for k, v in m.state_dict().items()}
-    hs = (gru_states if cell is UserGRU else lstm_states)(params, seqs, emb)
-    E = torch.as_tensor(emb.astype(np.float64))
-    terms, sampled = [], 0                                        # sampled: clicks whose impression has more than K non-clicks
+    samples, sampled = [], 0                                      # sampled: clicks whose impression has more than K non-clicks
     for q, iid in enumerate(ib.ids):
         u = int(imp['user'][iid])
         i = row[u]
         t = int(imp['time'][iid]) - 1 - (int(indptr[u + 1] - indptr[u]) - int(pk.L[i]))
         a, z = ib.indptr[q], ib.indptr[q + 1]
-        s = E[torch.from_numpy(ib.items[a:z].astype(np.int64))] @ hs[i][t]
         for c, S in so.negative_sets(ib.clicked[a:z], int(iid), K, seed, epoch):
             sampled += int(0 < K < (ib.clicked[a:z] == 0).sum())
-            terms.append(torch.logsumexp(torch.cat([s[c:c + 1], s[torch.from_numpy(np.asarray(S, np.int64))]]), 0) - s[c])
-    assert len(terms) == ib.clicks and (sampled > 20 or K == 0)
+            samples.append((i, t, a + c, a + np.asarray(S, np.int64)))
+    assert len(samples) == ib.clicks and (sampled > 20 or K == 0)
+    if cell is UserAttention:
+        o_loss, o_g = ao.softmax_loss_and_grads({k: v.double().numpy() for k, v in m.state_dict().items()}, seqs, emb,
+                                                [(i, t, ib.items[c], ib.items[S]) for i, t, c, S in samples], m.heads)
+        assert rel_err(loss, o_loss) < 1e-4, (loss, o_loss)
+        A = m.attention_dim
+        g = {x: m._theta(x, m.grad).cpu().double().numpy() for x in ('in', 'out', 'pool', 'query')}
+        got = {'self_attn.in_proj_weight': g['in'][:, :H], 'self_attn.in_proj_bias': g['in'][:, H],
+               'self_attn.out_proj.weight': g['out'][:, :H], 'self_attn.out_proj.bias': g['out'][:, H],
+               'pool.weight': g['pool'][:, :H], 'pool.bias': g['pool'][:, H], 'pool.query': g['query'][:A]}
+        for k in ATTENTION_NAMES:
+            assert rel_err(got[k], o_g[k]) < 1e-4, (k, rel_err(got[k], o_g[k]))
+        return
+    params = {k: torch.tensor(v.double().numpy(), requires_grad=True) for k, v in m.state_dict().items()}
+    hs = (gru_states if cell is UserGRU else lstm_states)(params, seqs, emb)
+    E = torch.as_tensor(emb.astype(np.float64))
+    terms = []
+    for i, t, c, S in samples:
+        s = E[torch.from_numpy(ib.items[np.concatenate([[c], S])].astype(np.int64))] @ hs[i][t]
+        terms.append(torch.logsumexp(s, 0) - s[0])
     o_loss = torch.stack(terms).mean()
     o_loss.backward()
     o_loss = float(o_loss.detach())
