@@ -1690,83 +1690,51 @@ __global__ void __launch_bounds__(256) sk_fixup_kernel(const GemmParams p, int t
 
 static int64_t sk_workspace_bytes() { return (int64_t)2 * sm_count() * BLOCK_M * 128 * (int64_t)sizeof(float); }
 
-// the fused decode: E [M x K] and W [N x K], both K-major; one persistent CTA per SM over the 128 x 128 output tiles
-template <int ACT, int LOSS>
-static int launch_decode(const Operand& A, const Operand& B, const GemmParams& p, cudaStream_t st) {
+// the fused decode, top-k, pair-histogram and pairs kernels: A [M x K] and B [N x K] (M, N and K from g), both K-major, in 128-row
+// and kDecodeN-row boxes; one persistent CTA per SM over the kernel's work items.  Templated on the kernel itself, not its type, so
+// that every kernel has its own attr_done (topk_kernel<16, false> and <32, false> share a type).
+template <auto Kern, int BK, int STAGES, class Params>
+static int launch_persistent(const Operand& A, const Operand& B, const GemmParams& g, const Params& kp, long long items,
+                             cudaStream_t st) {
   CUtensorMap ta_hi, ta_lo, tb_hi, tb_lo;
   int rc;
-  if ((rc = make_map(&ta_hi, A.hi, p.K, p.M, A.ld, BLOCK_M, kDecodeBK))) return rc;
-  if ((rc = make_map(&ta_lo, A.lo, p.K, p.M, A.ld, BLOCK_M, kDecodeBK))) return rc;
-  if ((rc = make_map(&tb_hi, B.hi, p.K, p.N, B.ld, kDecodeN, kDecodeBK))) return rc;
-  if ((rc = make_map(&tb_lo, B.lo, p.K, p.N, B.ld, kDecodeN, kDecodeBK))) return rc;
-  // operand ring + accumulator staging tile + alignment slack (the dZ transpose blocks are static)
-  constexpr int smem = kDecodeStages * (2 * BLOCK_M * kDecodeBK * 2 + 2 * kDecodeN * kDecodeBK * 2) + BLOCK_M * (kDecodeN + 4) * 4 + 1024;
-  auto kern = decode_fused_kernel<ACT, LOSS>;
+  if ((rc = make_map(&ta_hi, A.hi, g.K, g.M, A.ld, BLOCK_M, BK))) return rc;
+  if ((rc = make_map(&ta_lo, A.lo, g.K, g.M, A.ld, BLOCK_M, BK))) return rc;
+  if ((rc = make_map(&tb_hi, B.hi, g.K, g.N, B.ld, kDecodeN, BK))) return rc;
+  if ((rc = make_map(&tb_lo, B.lo, g.K, g.N, B.ld, kDecodeN, BK))) return rc;
+  // operand ring + accumulator staging tile + alignment slack (the decode's dZ transpose blocks are static)
+  constexpr int smem = STAGES * (2 * BLOCK_M * BK * 2 + 2 * kDecodeN * BK * 2) + BLOCK_M * (kDecodeN + 4) * 4 + 1024;
   static bool attr_done[64] = {false};
-  if ((rc = ensure_smem_attr(kern, smem, attr_done))) return rc;
-  const int tiles = ((p.M + BLOCK_M - 1) / BLOCK_M) * ((p.N + kDecodeN - 1) / kDecodeN);
-  const int n = tiles < sm_count() ? tiles : sm_count();
-  kern<<<n, kDecodeThreads, smem, st>>>(ta_hi, ta_lo, tb_hi, tb_lo, p);
+  if ((rc = ensure_smem_attr(Kern, smem, attr_done))) return rc;
+  const int n = items < sm_count() ? (int)items : sm_count();
+  Kern<<<n, kDecodeThreads, smem, st>>>(ta_hi, ta_lo, tb_hi, tb_lo, kp);
   return DAE_OK;
 }
 
-// fused similarity + k-best: Q [M x K] and C [N x K], both K-major; one persistent CTA per SM over the (row block, split) work items
-template <int KMAX, bool EXCL, bool GROUPS = false>
+// the fused decode: E [M x K] and W [N x K]; work items: the 128 x kDecodeN output tiles
+template <int LOSS>
+static int launch_decode(int dec_act, const Operand& A, const Operand& B, const GemmParams& p, cudaStream_t st) {
+  const long long tiles = (long long)((p.M + BLOCK_M - 1) / BLOCK_M) * ((p.N + kDecodeN - 1) / kDecodeN);
+  if (dec_act == DAE_ACT_SIGMOID)
+    return launch_persistent<decode_fused_kernel<DAE_ACT_SIGMOID, LOSS>, kDecodeBK, kDecodeStages>(A, B, p, p, tiles, st);
+  if (dec_act == DAE_ACT_TANH)
+    return launch_persistent<decode_fused_kernel<DAE_ACT_TANH, LOSS>, kDecodeBK, kDecodeStages>(A, B, p, p, tiles, st);
+  return launch_persistent<decode_fused_kernel<DAE_ACT_NONE, LOSS>, kDecodeBK, kDecodeStages>(A, B, p, p, tiles, st);
+}
+
+// fused similarity + k-best: Q [M x K] and C [N x K]; work items: (row block, split); the kernel keeps lists of 16 or 32 >= tp.k
+template <bool EXCL, bool GROUPS>
 static int launch_topk(const Operand& A, const Operand& B, const TopkParams& tp, cudaStream_t st) {
-  CUtensorMap ta_hi, ta_lo, tb_hi, tb_lo;
-  int rc;
-  const GemmParams& p = tp.g;
-  if ((rc = make_map(&ta_hi, A.hi, p.K, p.M, A.ld, BLOCK_M, kTopkBK))) return rc;
-  if ((rc = make_map(&ta_lo, A.lo, p.K, p.M, A.ld, BLOCK_M, kTopkBK))) return rc;
-  if ((rc = make_map(&tb_hi, B.hi, p.K, p.N, B.ld, kDecodeN, kTopkBK))) return rc;
-  if ((rc = make_map(&tb_lo, B.lo, p.K, p.N, B.ld, kDecodeN, kTopkBK))) return rc;
-  // operand ring + accumulator staging tile + alignment slack
-  constexpr int smem = kTopkStages * (2 * BLOCK_M * kTopkBK * 2 + 2 * kDecodeN * kTopkBK * 2) + BLOCK_M * (kDecodeN + 4) * 4 + 1024;
-  auto kern = topk_kernel<KMAX, EXCL, GROUPS>;
-  static bool attr_done[64] = {false};
-  if ((rc = ensure_smem_attr(kern, smem, attr_done))) return rc;
-  const int items = ((p.M + BLOCK_M - 1) / BLOCK_M) * tp.splits;
-  const int n = items < sm_count() ? items : sm_count();
-  kern<<<n, kDecodeThreads, smem, st>>>(ta_hi, ta_lo, tb_hi, tb_lo, tp);
-  return DAE_OK;
+  const long long items = (long long)((tp.g.M + BLOCK_M - 1) / BLOCK_M) * tp.splits;
+  if (tp.k <= 16) return launch_persistent<topk_kernel<16, EXCL, GROUPS>, kTopkBK, kTopkStages>(A, B, tp.g, tp, items, st);
+  return launch_persistent<topk_kernel<32, EXCL, GROUPS>, kTopkBK, kTopkStages>(A, B, tp.g, tp, items, st);
 }
 
-// related / unrelated pair histogram: X [N x K] K-major as both operands; one persistent CTA per SM over the lower-triangle tiles
-static int launch_pair_hist(const Operand& X, const PairHistParams& hp, cudaStream_t st) {
-  CUtensorMap ta_hi, ta_lo, tb_hi, tb_lo;
-  int rc;
-  const GemmParams& p = hp.g;
-  if ((rc = make_map(&ta_hi, X.hi, p.K, p.M, X.ld, BLOCK_M, kTopkBK))) return rc;
-  if ((rc = make_map(&ta_lo, X.lo, p.K, p.M, X.ld, BLOCK_M, kTopkBK))) return rc;
-  if ((rc = make_map(&tb_hi, X.hi, p.K, p.N, X.ld, kDecodeN, kTopkBK))) return rc;
-  if ((rc = make_map(&tb_lo, X.lo, p.K, p.N, X.ld, kDecodeN, kTopkBK))) return rc;
-  constexpr int smem = kTopkStages * (2 * BLOCK_M * kTopkBK * 2 + 2 * kDecodeN * kTopkBK * 2) + BLOCK_M * (kDecodeN + 4) * 4 + 1024;
-  static bool attr_done[64] = {false};
-  if ((rc = ensure_smem_attr(pair_hist_kernel, smem, attr_done))) return rc;
-  const long long tm = (p.M + BLOCK_M - 1) / BLOCK_M, tiles = tm * (tm + 1) / 2;
-  const int n = tiles < sm_count() ? (int)tiles : sm_count();
-  pair_hist_kernel<<<n, kDecodeThreads, smem, st>>>(ta_hi, ta_lo, tb_hi, tb_lo, hp);
-  return DAE_OK;
-}
-
-// thresholded pairs: Q [M x K] and C [N x K], both K-major; one persistent CTA per SM over the tiles (self: the lower triangle)
-template <bool ROWS = false>
+// thresholded pairs: Q [M x K] and C [N x K]; work items: the tiles (self: the lower triangle)
+template <bool ROWS>
 static int launch_pairs(const Operand& A, const Operand& B, const PairsParams& pp, cudaStream_t st) {
-  CUtensorMap ta_hi, ta_lo, tb_hi, tb_lo;
-  int rc;
-  const GemmParams& p = pp.g;
-  if ((rc = make_map(&ta_hi, A.hi, p.K, p.M, A.ld, BLOCK_M, kTopkBK))) return rc;
-  if ((rc = make_map(&ta_lo, A.lo, p.K, p.M, A.ld, BLOCK_M, kTopkBK))) return rc;
-  if ((rc = make_map(&tb_hi, B.hi, p.K, p.N, B.ld, kDecodeN, kTopkBK))) return rc;
-  if ((rc = make_map(&tb_lo, B.lo, p.K, p.N, B.ld, kDecodeN, kTopkBK))) return rc;
-  constexpr int smem = kTopkStages * (2 * BLOCK_M * kTopkBK * 2 + 2 * kDecodeN * kTopkBK * 2) + BLOCK_M * (kDecodeN + 4) * 4 + 1024;
-  static bool attr_done[64] = {false};
-  if ((rc = ensure_smem_attr(pairs_kernel<ROWS>, smem, attr_done))) return rc;
-  const long long tm = (p.M + BLOCK_M - 1) / BLOCK_M, tn = (p.N + kDecodeN - 1) / kDecodeN;
-  const long long tiles = pp.self ? tm * (tm + 1) / 2 : tm * tn;
-  const int n = tiles < sm_count() ? (int)tiles : sm_count();
-  pairs_kernel<ROWS><<<n, kDecodeThreads, smem, st>>>(ta_hi, ta_lo, tb_hi, tb_lo, pp);
-  return DAE_OK;
+  const long long tm = (pp.g.M + BLOCK_M - 1) / BLOCK_M, tn = (pp.g.N + kDecodeN - 1) / kDecodeN;
+  return launch_persistent<pairs_kernel<ROWS>, kTopkBK, kTopkStages>(A, B, pp.g, pp, pp.self ? tm * (tm + 1) / 2 : tm * tn, st);
 }
 
 // column splits of dae_similarity_topk_bf16x3: `requested` (> 0), or the fewest that give every SM a work item while each split
@@ -1824,18 +1792,24 @@ extern "C" int dae_gemm_config(int32_t pair_mode, int32_t lean) {
   return DAE_OK;
 }
 
-extern "C" int dae_gemm_bf16x3(int32_t M, int32_t N, int32_t K, float alpha, const void* a_hi, const void* a_lo, int64_t lda,
-                               int32_t a_mn_major, const void* b_hi, const void* b_lo, int64_t ldb, int32_t b_mn_major, float* C,
-                               int64_t ldc, int32_t n_store, int32_t special_col, float* special_out, int32_t k_splits,
-                               int32_t accumulate, void* stream) {
-  DAE_REQUIRE(a_hi && a_lo && b_hi && b_lo && C && M > 0 && N > 0 && K > 0, "dae_gemm_bf16x3: bad arguments");
-  DAE_REQUIRE(lda % 8 == 0 && ldb % 8 == 0, "dae_gemm_bf16x3: operand leading dimensions must be multiples of 8 (TMA 16-byte strides)");
-  DAE_REQUIRE(((uintptr_t)a_hi | (uintptr_t)a_lo | (uintptr_t)b_hi | (uintptr_t)b_lo) % 16 == 0, "dae_gemm_bf16x3: operands must be 16-byte aligned");
+// dae_gemm_bf16x3 and, with det, dae_gemm_bf16x3_det: the same schedules and main loops without the CTA-pair and lean engines;
+// partial stream-K tiles go through the workspace and sk_fixup_kernel instead of atomic adds into a zeroed C
+static int gemm_bf16x3(const char* fn, bool det, int32_t M, int32_t N, int32_t K, float alpha, const void* a_hi, const void* a_lo,
+                       int64_t lda, int32_t a_mn_major, const void* b_hi, const void* b_lo, int64_t ldb, int32_t b_mn_major, float* C,
+                       int64_t ldc, int32_t n_store, int32_t special_col, float* special_out, int32_t k_splits, int32_t accumulate,
+                       void* workspace, int64_t workspace_bytes, void* stream) {
+  DAE_REQUIRE(a_hi && a_lo && b_hi && b_lo && C && M > 0 && N > 0 && K > 0, "%s: bad arguments", fn);
+  DAE_REQUIRE(lda % 8 == 0 && ldb % 8 == 0, "%s: operand leading dimensions must be multiples of 8 (TMA 16-byte strides)", fn);
+  DAE_REQUIRE(((uintptr_t)a_hi | (uintptr_t)a_lo | (uintptr_t)b_hi | (uintptr_t)b_lo) % 16 == 0, "%s: operands must be 16-byte aligned",
+              fn);
+  DAE_REQUIRE(!det || k_splits == 1 || k_splits == -1, "%s: k_splits must be 1 or -1 (stream-K), got %d", fn, k_splits);
   cudaStream_t st = (cudaStream_t)stream;
   if (n_store <= 0 || n_store > N) n_store = N;
-  DAE_REQUIRE(ldc >= n_store, "dae_gemm_bf16x3: ldc %lld below n_store %d", (long long)ldc, n_store);
-  DAE_REQUIRE(!special_out || (special_col >= n_store && special_col < N),
-              "dae_gemm_bf16x3: special_col %d outside [n_store, N) = [%d, %d)", special_col, n_store, N);
+  DAE_REQUIRE(ldc >= n_store, "%s: ldc %lld below n_store %d", fn, (long long)ldc, n_store);
+  DAE_REQUIRE(!special_out || (special_col >= n_store && special_col < N), "%s: special_col %d outside [n_store, N) = [%d, %d)", fn,
+              special_col, n_store, N);
+  DAE_REQUIRE(!det || (workspace && workspace_bytes >= sk_workspace_bytes()), "%s: workspace of %lld bytes, need %lld", fn,
+              (long long)workspace_bytes, (long long)sk_workspace_bytes());
   const int kblocks = (K + BLOCK_K - 1) / BLOCK_K;
   const int tm = (M + 127) / 128, tn128 = (N + 127) / 128, tn64 = (N + 63) / 64;
   const int sms = sm_count();
@@ -1852,12 +1826,13 @@ extern "C" int dae_gemm_bf16x3(int32_t M, int32_t N, int32_t K, float alpha, con
     k_splits = (kblocks + per - 1) / per;
   }
   const bool partial = (k_splits > 1) || stream_k;
-  if (partial && !accumulate) {
+  if (!det && partial && !accumulate) {
     DAE_CUDA(cudaMemset2DAsync(C, ldc * sizeof(float), 0, (size_t)n_store * sizeof(float), M, st));
     if (special_col >= 0 && special_out) DAE_CUDA(cudaMemsetAsync(special_out, 0, sizeof(float) * M, st));
   }
   GemmParams p{};
-  p.M = M; p.N = N; p.K = K; p.k_splits = k_splits; p.stream_k = stream_k; p.atomic = (partial || accumulate) ? 1 : 0; p.alpha = alpha;
+  p.M = M; p.N = N; p.K = K; p.k_splits = k_splits; p.stream_k = stream_k; p.alpha = alpha;
+  p.atomic = ((partial && !det) || accumulate) ? 1 : 0;   // det: every element has one writer, the GEMM or the fixup
   p.C = C; p.ldc = ldc; p.n_store = n_store;
   p.special_col = (special_out ? special_col : -1); p.special_out = special_out;
   Operand A{a_hi, a_lo, lda, a_mn_major}, B{b_hi, b_lo, ldb, b_mn_major};
@@ -1866,108 +1841,91 @@ extern "C" int dae_gemm_bf16x3(int32_t M, int32_t N, int32_t K, float alpha, con
   // 4 stages of 32-wide k-blocks: the same 128 KB as 2 x 64, but three stages (96 KB) in flight behind the one being multiplied
   // instead of one (64 KB), which the L2 -> shared-memory latency of dE / dW needs (see DESIGN 4.1).  The lean and pair test
   // configurations keep the 2 x 64 rings.
-  int rc;
+  int rc, n = 0;
   const int tiles128 = tm * tn128 * k_splits, tiles64 = tm * tn64 * k_splits;
   const float cost128 = 2.0f * (float)((tiles128 + sms - 1) / sms), cost64 = 1.1f * (float)((tiles64 + sms - 1) / sms);
-  if (g_lean) rc = launch_gemm<64, 2, 0>(A, B, p, st);
-  else if (use_pair()) rc = launch_gemm<128, 2, 1>(A, B, p, st);
-  else if (stream_k) rc = launch_gemm<128, 4, 0, 32>(A, B, p, st);
-  else if (!stream_k && cost64 < cost128) rc = launch_gemm<64, 3, 0>(A, B, p, st);
+  if (det && stream_k) p.sk_ws = (float*)workspace;
+  if (!det && g_lean) rc = launch_gemm<64, 2, 0>(A, B, p, st);
+  else if (!det && use_pair()) rc = launch_gemm<128, 2, 1>(A, B, p, st);
+  else if (stream_k) rc = launch_gemm<128, 4, 0, 32>(A, B, p, st, &n);
+  else if (cost64 < cost128) rc = launch_gemm<64, 3, 0>(A, B, p, st);
   else rc = launch_gemm<128, 2, 0>(A, B, p, st);
   if (rc) return rc;
-  DAE_CHECK_LAUNCH("dae_gemm_bf16x3");
+  if (det && stream_k) {
+    DAE_REQUIRE(n <= kMaxFixupCtas, "%s: %d stream-K CTAs exceed the fixup's %d", fn, n, kMaxFixupCtas);
+    sk_fixup_kernel<128><<<dim3(tm * tn128, kFixupSlices), 256, 0, st>>>(p, tm, tm * tn128, (K + 31) / 32, n);
+  }
+  DAE_CHECK_LAUNCH(fn);
   return DAE_OK;
 }
 
-// C[m, n] (+)= alpha * sum_k (G[m, k] + G[k, m]) * B[k, n] for a square G [M x M] (bf16 hi / lo, row-major, ld = ldg) and B stored
-// [M x ldb] row-major (n contiguous).  ONE launch: the k loop runs over G's columns and then over G's rows (the same array through
-// an M-contiguous tensor map), so G + G^T is never formed.  dE2 = alpha (G + G^T) E of the batch_all / batch_hard backward.
-extern "C" int dae_gemm_sym_bf16x3(int32_t M, int32_t N, float alpha, const void* g_hi, const void* g_lo, int64_t ldg, const void* b_hi,
-                                   const void* b_lo, int64_t ldb, float* C, int64_t ldc, int32_t accumulate, void* stream) {
-  DAE_REQUIRE(g_hi && g_lo && b_hi && b_lo && C && M > 0 && N > 0, "dae_gemm_sym_bf16x3: bad arguments");
-  DAE_REQUIRE(ldg % 8 == 0 && ldb % 8 == 0 && ldg >= M && ldb >= N, "dae_gemm_sym_bf16x3: leading dimensions must be multiples of 8 and cover the matrices");
-  DAE_REQUIRE(((uintptr_t)g_hi | (uintptr_t)g_lo | (uintptr_t)b_hi | (uintptr_t)b_lo) % 16 == 0, "dae_gemm_sym_bf16x3: operands must be 16-byte aligned");
-  GemmParams p{};
-  const int kb_half = (M + BLOCK_K - 1) / BLOCK_K;
-  // stream-K: 28 tiles of 128 x 128 at B = 800 would leave 104 SMs idle for a 26-k-block main loop; ~6 k-blocks per CTA instead
-  p.M = M; p.N = N; p.K = 2 * kb_half * BLOCK_K; p.k_splits = 1; p.stream_k = 1; p.atomic = 1; p.alpha = alpha;
-  p.C = C; p.ldc = ldc; p.n_store = N; p.special_col = -1; p.special_out = nullptr; p.a_sym_kb = kb_half;
-  if (!accumulate) DAE_CUDA(cudaMemset2DAsync(C, ldc * sizeof(float), 0, (size_t)N * sizeof(float), M, (cudaStream_t)stream));
-  Operand A{g_hi, g_lo, ldg, 0}, B{b_hi, b_lo, ldb, 1};
-  int rc = launch_gemm_maj<128, 2, 0, 6>(A, B, p, (cudaStream_t)stream);
-  if (rc) return rc;
-  DAE_CHECK_LAUNCH("dae_gemm_sym_bf16x3");
-  return DAE_OK;
-}
-
-// ---- deterministic variants: the same schedules and main loops; partial stream-K tiles go through the workspace and sk_fixup_kernel
-extern "C" int dae_gemm_det_workspace(int64_t* bytes) {
-  DAE_REQUIRE(bytes, "dae_gemm_det_workspace: null pointer");
-  *bytes = sk_workspace_bytes();
-  return DAE_OK;
+extern "C" int dae_gemm_bf16x3(int32_t M, int32_t N, int32_t K, float alpha, const void* a_hi, const void* a_lo, int64_t lda,
+                               int32_t a_mn_major, const void* b_hi, const void* b_lo, int64_t ldb, int32_t b_mn_major, float* C,
+                               int64_t ldc, int32_t n_store, int32_t special_col, float* special_out, int32_t k_splits,
+                               int32_t accumulate, void* stream) {
+  return gemm_bf16x3("dae_gemm_bf16x3", false, M, N, K, alpha, a_hi, a_lo, lda, a_mn_major, b_hi, b_lo, ldb, b_mn_major, C, ldc, n_store,
+                     special_col, special_out, k_splits, accumulate, nullptr, 0, stream);
 }
 
 extern "C" int dae_gemm_bf16x3_det(int32_t M, int32_t N, int32_t K, float alpha, const void* a_hi, const void* a_lo, int64_t lda,
                                    int32_t a_mn_major, const void* b_hi, const void* b_lo, int64_t ldb, int32_t b_mn_major, float* C,
                                    int64_t ldc, int32_t n_store, int32_t special_col, float* special_out, int32_t k_splits,
                                    int32_t accumulate, void* workspace, int64_t workspace_bytes, void* stream) {
-  DAE_REQUIRE(a_hi && a_lo && b_hi && b_lo && C && M > 0 && N > 0 && K > 0, "dae_gemm_bf16x3_det: bad arguments");
-  DAE_REQUIRE(lda % 8 == 0 && ldb % 8 == 0, "dae_gemm_bf16x3_det: operand leading dimensions must be multiples of 8 (TMA 16-byte strides)");
-  DAE_REQUIRE(((uintptr_t)a_hi | (uintptr_t)a_lo | (uintptr_t)b_hi | (uintptr_t)b_lo) % 16 == 0, "dae_gemm_bf16x3_det: operands must be 16-byte aligned");
-  DAE_REQUIRE(k_splits == 1 || k_splits == -1, "dae_gemm_bf16x3_det: k_splits must be 1 or -1 (stream-K), got %d", k_splits);
-  if (n_store <= 0 || n_store > N) n_store = N;
-  DAE_REQUIRE(ldc >= n_store, "dae_gemm_bf16x3_det: ldc %lld below n_store %d", (long long)ldc, n_store);
-  DAE_REQUIRE(!special_out || (special_col >= n_store && special_col < N),
-              "dae_gemm_bf16x3_det: special_col %d outside [n_store, N) = [%d, %d)", special_col, n_store, N);
-  DAE_REQUIRE(workspace && workspace_bytes >= sk_workspace_bytes(), "dae_gemm_bf16x3_det: workspace of %lld bytes, need %lld",
+  return gemm_bf16x3("dae_gemm_bf16x3_det", true, M, N, K, alpha, a_hi, a_lo, lda, a_mn_major, b_hi, b_lo, ldb, b_mn_major, C, ldc,
+                     n_store, special_col, special_out, k_splits, accumulate, workspace, workspace_bytes, stream);
+}
+
+// C[m, n] (+)= alpha * sum_k (G[m, k] + G[k, m]) * B[k, n] for a square G [M x M] (bf16 hi / lo, row-major, ld = ldg) and B stored
+// [M x ldb] row-major (n contiguous).  ONE launch: the k loop runs over G's columns and then over G's rows (the same array through
+// an M-contiguous tensor map), so G + G^T is never formed.  dE2 = alpha (G + G^T) E of the batch_all / batch_hard backward.
+// det (dae_gemm_sym_bf16x3_det): partial stream-K tiles go through the workspace and sk_fixup_kernel instead of atomics.
+static int gemm_sym_bf16x3(const char* fn, bool det, int32_t M, int32_t N, float alpha, const void* g_hi, const void* g_lo, int64_t ldg,
+                           const void* b_hi, const void* b_lo, int64_t ldb, float* C, int64_t ldc, int32_t accumulate, void* workspace,
+                           int64_t workspace_bytes, void* stream) {
+  DAE_REQUIRE(g_hi && g_lo && b_hi && b_lo && C && M > 0 && N > 0, "%s: bad arguments", fn);
+  DAE_REQUIRE(ldg % 8 == 0 && ldb % 8 == 0 && ldg >= M && ldb >= N, "%s: leading dimensions must be multiples of 8 and cover the matrices",
+              fn);
+  DAE_REQUIRE(((uintptr_t)g_hi | (uintptr_t)g_lo | (uintptr_t)b_hi | (uintptr_t)b_lo) % 16 == 0, "%s: operands must be 16-byte aligned",
+              fn);
+  DAE_REQUIRE(!det || (workspace && workspace_bytes >= sk_workspace_bytes()), "%s: workspace of %lld bytes, need %lld", fn,
               (long long)workspace_bytes, (long long)sk_workspace_bytes());
   cudaStream_t st = (cudaStream_t)stream;
-  const int tm = (M + 127) / 128, tn = (N + 127) / 128;
-  const int stream_k = (k_splits < 0 && (tm * tn) % sm_count() != 0) ? 1 : 0;   // the choice of dae_gemm_bf16x3
   GemmParams p{};
-  p.M = M; p.N = N; p.K = K; p.k_splits = 1; p.stream_k = stream_k; p.atomic = accumulate ? 1 : 0; p.alpha = alpha;
-  p.C = C; p.ldc = ldc; p.n_store = n_store;
-  p.special_col = (special_out ? special_col : -1); p.special_out = special_out;
-  Operand A{a_hi, a_lo, lda, a_mn_major}, B{b_hi, b_lo, ldb, b_mn_major};
-  int rc;
-  if (stream_k) {
-    p.sk_ws = (float*)workspace;
-    int n = 0;
-    if ((rc = launch_gemm<128, 4, 0, 32>(A, B, p, st, &n))) return rc;
-    DAE_REQUIRE(n <= kMaxFixupCtas, "dae_gemm_bf16x3_det: %d stream-K CTAs exceed the fixup's %d", n, kMaxFixupCtas);
-    sk_fixup_kernel<128><<<dim3(tm * tn, kFixupSlices), 256, 0, st>>>(p, tm, tm * tn, (K + 31) / 32, n);
-  } else {   // whole tiles: every element has one writer
-    const int sms = sm_count(), tn64 = (N + 63) / 64;
-    const float cost128 = 2.0f * (float)((tm * tn + sms - 1) / sms), cost64 = 1.1f * (float)((tm * tn64 + sms - 1) / sms);
-    rc = (cost64 < cost128) ? launch_gemm<64, 3, 0>(A, B, p, st) : launch_gemm<128, 2, 0>(A, B, p, st);
-    if (rc) return rc;
+  const int kb_half = (M + BLOCK_K - 1) / BLOCK_K;
+  // stream-K: 28 tiles of 128 x 128 at B = 800 would leave 104 SMs idle for a 26-k-block main loop; ~6 k-blocks per CTA instead
+  p.M = M; p.N = N; p.K = 2 * kb_half * BLOCK_K; p.k_splits = 1; p.stream_k = 1; p.atomic = (!det || accumulate) ? 1 : 0; p.alpha = alpha;
+  p.C = C; p.ldc = ldc; p.n_store = N; p.special_col = -1; p.special_out = nullptr; p.a_sym_kb = kb_half;
+  if (det) p.sk_ws = (float*)workspace;
+  else if (!accumulate) DAE_CUDA(cudaMemset2DAsync(C, ldc * sizeof(float), 0, (size_t)N * sizeof(float), M, st));
+  Operand A{g_hi, g_lo, ldg, 0}, B{b_hi, b_lo, ldb, 1};
+  int n = 0;
+  int rc = launch_gemm_maj<128, 2, 0, 6>(A, B, p, st, &n);
+  if (rc) return rc;
+  if (det) {
+    DAE_REQUIRE(n <= kMaxFixupCtas, "%s: %d stream-K CTAs exceed the fixup's %d", fn, n, kMaxFixupCtas);
+    const int tm = (M + 127) / 128, tn = (N + 127) / 128;
+    sk_fixup_kernel<128><<<dim3(tm * tn, kFixupSlices), 256, 0, st>>>(p, tm, tm * tn, 2 * kb_half, n);
   }
-  DAE_CHECK_LAUNCH("dae_gemm_bf16x3_det");
+  DAE_CHECK_LAUNCH(fn);
   return DAE_OK;
+}
+
+extern "C" int dae_gemm_sym_bf16x3(int32_t M, int32_t N, float alpha, const void* g_hi, const void* g_lo, int64_t ldg, const void* b_hi,
+                                   const void* b_lo, int64_t ldb, float* C, int64_t ldc, int32_t accumulate, void* stream) {
+  return gemm_sym_bf16x3("dae_gemm_sym_bf16x3", false, M, N, alpha, g_hi, g_lo, ldg, b_hi, b_lo, ldb, C, ldc, accumulate, nullptr, 0,
+                         stream);
 }
 
 extern "C" int dae_gemm_sym_bf16x3_det(int32_t M, int32_t N, float alpha, const void* g_hi, const void* g_lo, int64_t ldg, const void* b_hi,
                                        const void* b_lo, int64_t ldb, float* C, int64_t ldc, int32_t accumulate, void* workspace,
                                        int64_t workspace_bytes, void* stream) {
-  DAE_REQUIRE(g_hi && g_lo && b_hi && b_lo && C && M > 0 && N > 0, "dae_gemm_sym_bf16x3_det: bad arguments");
-  DAE_REQUIRE(ldg % 8 == 0 && ldb % 8 == 0 && ldg >= M && ldb >= N, "dae_gemm_sym_bf16x3_det: leading dimensions must be multiples of 8 and cover the matrices");
-  DAE_REQUIRE(((uintptr_t)g_hi | (uintptr_t)g_lo | (uintptr_t)b_hi | (uintptr_t)b_lo) % 16 == 0, "dae_gemm_sym_bf16x3_det: operands must be 16-byte aligned");
-  DAE_REQUIRE(workspace && workspace_bytes >= sk_workspace_bytes(), "dae_gemm_sym_bf16x3_det: workspace of %lld bytes, need %lld",
-              (long long)workspace_bytes, (long long)sk_workspace_bytes());
-  cudaStream_t st = (cudaStream_t)stream;
-  GemmParams p{};
-  const int kb_half = (M + BLOCK_K - 1) / BLOCK_K;
-  p.M = M; p.N = N; p.K = 2 * kb_half * BLOCK_K; p.k_splits = 1; p.stream_k = 1; p.atomic = accumulate ? 1 : 0; p.alpha = alpha;
-  p.C = C; p.ldc = ldc; p.n_store = N; p.special_col = -1; p.special_out = nullptr; p.a_sym_kb = kb_half;
-  p.sk_ws = (float*)workspace;
-  Operand A{g_hi, g_lo, ldg, 0}, B{b_hi, b_lo, ldb, 1};
-  int n = 0;
-  int rc = launch_gemm_maj<128, 2, 0, 6>(A, B, p, st, &n);
-  if (rc) return rc;
-  DAE_REQUIRE(n <= kMaxFixupCtas, "dae_gemm_sym_bf16x3_det: %d stream-K CTAs exceed the fixup's %d", n, kMaxFixupCtas);
-  const int tm = (M + 127) / 128, tn = (N + 127) / 128;
-  sk_fixup_kernel<128><<<dim3(tm * tn, kFixupSlices), 256, 0, st>>>(p, tm, tm * tn, 2 * kb_half, n);
-  DAE_CHECK_LAUNCH("dae_gemm_sym_bf16x3_det");
+  return gemm_sym_bf16x3("dae_gemm_sym_bf16x3_det", true, M, N, alpha, g_hi, g_lo, ldg, b_hi, b_lo, ldb, C, ldc, accumulate, workspace,
+                         workspace_bytes, stream);
+}
+
+extern "C" int dae_gemm_det_workspace(int64_t* bytes) {
+  DAE_REQUIRE(bytes, "dae_gemm_det_workspace: null pointer");
+  *bytes = sk_workspace_bytes();
   return DAE_OK;
 }
 
@@ -1983,47 +1941,44 @@ extern "C" int dae_decode_prepare(int32_t Brows, int32_t F, const int64_t* indpt
   return DAE_OK;
 }
 
-extern "C" int dae_decode_fused_bf16x3(int32_t Brows, int32_t F, int32_t K, const void* e_hi, const void* e_lo, int64_t lde,
-                                       const void* w_hi, const void* w_lo, int64_t ldw, const int64_t* indptr, const int32_t* indices,
-                                       const float* values, const int32_t* rows, const float* bv, int32_t dec_act, int32_t loss_func,
-                                       const float* weight, const double* stats, void* dz_hi, void* dz_lo, int64_t ld_dz,
-                                       float* row_loss_part, int32_t* tile_ptr, int32_t prepared, void* stream) {
+// dae_decode_fused_bf16x3 and, with det, dae_decode_fused_bf16x3_det: row_loss_part is then [dae_decode_loss_parts][Brows], one store
+// per (half tile, row) instead of an atomic add per row
+static int decode_fused(const char* fn, bool det, int32_t Brows, int32_t F, int32_t K, const void* e_hi, const void* e_lo, int64_t lde,
+                        const void* w_hi, const void* w_lo, int64_t ldw, const int64_t* indptr, const int32_t* indices,
+                        const float* values, const int32_t* rows, const float* bv, int32_t dec_act, int32_t loss_func,
+                        const float* weight, const double* stats, void* dz_hi, void* dz_lo, int64_t ld_dz, float* row_loss_part,
+                        int32_t* tile_ptr, int32_t prepared, void* stream) {
   DAE_REQUIRE(e_hi && e_lo && w_hi && w_lo && indptr && indices && values && bv && stats && dz_hi && dz_lo && row_loss_part && tile_ptr,
-              "dae_decode_fused_bf16x3: null pointer");
-  DAE_REQUIRE(loss_func == DAE_LOSS_CE || loss_func == DAE_LOSS_MSE, "dae_decode_fused_bf16x3: cosine loss uses the unfused path");
-  DAE_REQUIRE(lde % 8 == 0 && ldw % 8 == 0 && ld_dz % 32 == 0 && ld_dz >= F, "dae_decode_fused_bf16x3: bad leading dimensions");
+              "%s: null pointer", fn);
+  DAE_REQUIRE(loss_func == DAE_LOSS_CE || loss_func == DAE_LOSS_MSE, "%s: cosine loss uses the unfused path", fn);
+  DAE_REQUIRE(lde % 8 == 0 && ldw % 8 == 0 && ld_dz % 32 == 0 && ld_dz >= F, "%s: bad leading dimensions", fn);
   cudaStream_t st = (cudaStream_t)stream;
   GemmParams p{};
   p.M = Brows; p.N = F; p.K = K; p.k_splits = 1; p.alpha = 1.0f; p.special_col = -1;
   p.indptr = indptr; p.indices = indices; p.values = values; p.rows = rows; p.bv = bv; p.weight = weight; p.stats = stats;
   p.dz_hi = (__nv_bfloat16*)dz_hi; p.dz_lo = (__nv_bfloat16*)dz_lo; p.ld_dz = ld_dz; p.row_loss_part = row_loss_part;
-  p.tile_ptr = tile_ptr;
-  if (!prepared) {   // dae_decode_prepare not issued by the caller (e.g. on a parallel graph branch): do it in line
+  p.tile_ptr = tile_ptr; p.loss_parts = det ? 1 : 0;
+  // dae_decode_prepare not issued by the caller (e.g. on a parallel graph branch): do it in line.  (det: its zeroing of the first
+  // Brows floats is harmless, every part is stored)
+  if (!prepared) {
     int rc0 = dae_decode_prepare(Brows, F, indptr, indices, rows, row_loss_part, tile_ptr, stream);
     if (rc0) return rc0;
   }
   Operand A{e_hi, e_lo, lde, 0}, B{w_hi, w_lo, ldw, 0};
-  int rc = 0;
-#define DAE_DEC(ACT, LOSS) rc = launch_decode<ACT, LOSS>(A, B, p, st)
-  if (loss_func == DAE_LOSS_CE) {
-    if (dec_act == DAE_ACT_SIGMOID) DAE_DEC(DAE_ACT_SIGMOID, DAE_LOSS_CE);
-    else if (dec_act == DAE_ACT_TANH) DAE_DEC(DAE_ACT_TANH, DAE_LOSS_CE);
-    else DAE_DEC(DAE_ACT_NONE, DAE_LOSS_CE);
-  } else {
-    if (dec_act == DAE_ACT_SIGMOID) DAE_DEC(DAE_ACT_SIGMOID, DAE_LOSS_MSE);
-    else if (dec_act == DAE_ACT_TANH) DAE_DEC(DAE_ACT_TANH, DAE_LOSS_MSE);
-    else DAE_DEC(DAE_ACT_NONE, DAE_LOSS_MSE);
-  }
-#undef DAE_DEC
+  int rc = (loss_func == DAE_LOSS_CE) ? launch_decode<DAE_LOSS_CE>(dec_act, A, B, p, st)
+                                      : launch_decode<DAE_LOSS_MSE>(dec_act, A, B, p, st);
   if (rc) return rc;
-  DAE_CHECK_LAUNCH("dae_decode_fused_bf16x3");
+  DAE_CHECK_LAUNCH(fn);
   return DAE_OK;
 }
 
-extern "C" int dae_decode_loss_parts(int32_t F, int32_t* n_parts) {
-  DAE_REQUIRE(F > 0 && n_parts, "dae_decode_loss_parts: bad arguments");
-  *n_parts = 2 * ((F + kDecodeN - 1) / kDecodeN);
-  return DAE_OK;
+extern "C" int dae_decode_fused_bf16x3(int32_t Brows, int32_t F, int32_t K, const void* e_hi, const void* e_lo, int64_t lde,
+                                       const void* w_hi, const void* w_lo, int64_t ldw, const int64_t* indptr, const int32_t* indices,
+                                       const float* values, const int32_t* rows, const float* bv, int32_t dec_act, int32_t loss_func,
+                                       const float* weight, const double* stats, void* dz_hi, void* dz_lo, int64_t ld_dz,
+                                       float* row_loss_part, int32_t* tile_ptr, int32_t prepared, void* stream) {
+  return decode_fused("dae_decode_fused_bf16x3", false, Brows, F, K, e_hi, e_lo, lde, w_hi, w_lo, ldw, indptr, indices, values, rows, bv,
+                      dec_act, loss_func, weight, stats, dz_hi, dz_lo, ld_dz, row_loss_part, tile_ptr, prepared, stream);
 }
 
 extern "C" int dae_decode_fused_bf16x3_det(int32_t Brows, int32_t F, int32_t K, const void* e_hi, const void* e_lo, int64_t lde,
@@ -2031,35 +1986,13 @@ extern "C" int dae_decode_fused_bf16x3_det(int32_t Brows, int32_t F, int32_t K, 
                                            const float* values, const int32_t* rows, const float* bv, int32_t dec_act, int32_t loss_func,
                                            const float* weight, const double* stats, void* dz_hi, void* dz_lo, int64_t ld_dz,
                                            float* row_loss_parts, int32_t* tile_ptr, int32_t prepared, void* stream) {
-  DAE_REQUIRE(e_hi && e_lo && w_hi && w_lo && indptr && indices && values && bv && stats && dz_hi && dz_lo && row_loss_parts && tile_ptr,
-              "dae_decode_fused_bf16x3_det: null pointer");
-  DAE_REQUIRE(loss_func == DAE_LOSS_CE || loss_func == DAE_LOSS_MSE, "dae_decode_fused_bf16x3_det: cosine loss uses the unfused path");
-  DAE_REQUIRE(lde % 8 == 0 && ldw % 8 == 0 && ld_dz % 32 == 0 && ld_dz >= F, "dae_decode_fused_bf16x3_det: bad leading dimensions");
-  cudaStream_t st = (cudaStream_t)stream;
-  GemmParams p{};
-  p.M = Brows; p.N = F; p.K = K; p.k_splits = 1; p.alpha = 1.0f; p.special_col = -1;
-  p.indptr = indptr; p.indices = indices; p.values = values; p.rows = rows; p.bv = bv; p.weight = weight; p.stats = stats;
-  p.dz_hi = (__nv_bfloat16*)dz_hi; p.dz_lo = (__nv_bfloat16*)dz_lo; p.ld_dz = ld_dz; p.row_loss_part = row_loss_parts;
-  p.tile_ptr = tile_ptr; p.loss_parts = 1;
-  if (!prepared) {   // (its zeroing of the first Brows floats is harmless: every part is stored)
-    int rc0 = dae_decode_prepare(Brows, F, indptr, indices, rows, row_loss_parts, tile_ptr, stream);
-    if (rc0) return rc0;
-  }
-  Operand A{e_hi, e_lo, lde, 0}, B{w_hi, w_lo, ldw, 0};
-  int rc = 0;
-#define DAE_DEC(ACT, LOSS) rc = launch_decode<ACT, LOSS>(A, B, p, st)
-  if (loss_func == DAE_LOSS_CE) {
-    if (dec_act == DAE_ACT_SIGMOID) DAE_DEC(DAE_ACT_SIGMOID, DAE_LOSS_CE);
-    else if (dec_act == DAE_ACT_TANH) DAE_DEC(DAE_ACT_TANH, DAE_LOSS_CE);
-    else DAE_DEC(DAE_ACT_NONE, DAE_LOSS_CE);
-  } else {
-    if (dec_act == DAE_ACT_SIGMOID) DAE_DEC(DAE_ACT_SIGMOID, DAE_LOSS_MSE);
-    else if (dec_act == DAE_ACT_TANH) DAE_DEC(DAE_ACT_TANH, DAE_LOSS_MSE);
-    else DAE_DEC(DAE_ACT_NONE, DAE_LOSS_MSE);
-  }
-#undef DAE_DEC
-  if (rc) return rc;
-  DAE_CHECK_LAUNCH("dae_decode_fused_bf16x3_det");
+  return decode_fused("dae_decode_fused_bf16x3_det", true, Brows, F, K, e_hi, e_lo, lde, w_hi, w_lo, ldw, indptr, indices, values, rows,
+                      bv, dec_act, loss_func, weight, stats, dz_hi, dz_lo, ld_dz, row_loss_parts, tile_ptr, prepared, stream);
+}
+
+extern "C" int dae_decode_loss_parts(int32_t F, int32_t* n_parts) {
+  DAE_REQUIRE(F > 0 && n_parts, "dae_decode_loss_parts: bad arguments");
+  *n_parts = 2 * ((F + kDecodeN - 1) / kDecodeN);
   return DAE_OK;
 }
 
@@ -2070,34 +2003,75 @@ extern "C" int dae_similarity_topk_workspace(int32_t n_query, int32_t n_corpus, 
   return DAE_OK;
 }
 
-extern "C" int dae_similarity_topk_bf16x3(int32_t n_query, int32_t n_corpus, int32_t dim, const void* q_hi, const void* q_lo, int64_t ldq,
-                                          const void* c_hi, const void* c_lo, int64_t ldc, int32_t k, int64_t diag_offset, int32_t exclude,
-                                          int32_t splits, void* workspace, int64_t workspace_bytes, int32_t* idx_out, float* val_out,
-                                          void* stream) {
-  DAE_REQUIRE(q_hi && q_lo && c_hi && c_lo && workspace && idx_out && val_out, "dae_similarity_topk_bf16x3: null pointer");
-  DAE_REQUIRE(n_query > 0 && n_corpus > 0 && dim > 0, "dae_similarity_topk_bf16x3: bad sizes");
-  DAE_REQUIRE(k >= 1 && k <= kTopkMaxK, "dae_similarity_topk_bf16x3: k = %d is outside the supported range 1 <= k <= %d", k, kTopkMaxK);
+// the leading-dimension and alignment checks of the similarity exports over Q [n_query x dim] and C [n_corpus x dim] (bf16 hi / lo,
+// K-major, read by TMA); a16 / a8 / a4: the export's other pointers that must be 16- / 8- / 4-byte aligned, or-ed together
+static int check_operands(const char* fn, int32_t dim, const void* q_hi, const void* q_lo, int64_t ldq, const void* c_hi, const void* c_lo,
+                          int64_t ldc, uintptr_t a16, uintptr_t a8, uintptr_t a4, const char* alignment) {
   DAE_REQUIRE(ldq >= dim && ldc >= dim && ldq % 8 == 0 && ldc % 8 == 0,
-              "dae_similarity_topk_bf16x3: leading dimensions must cover dim and be multiples of 8 (TMA 16-byte strides)");
-  DAE_REQUIRE(((uintptr_t)q_hi | (uintptr_t)q_lo | (uintptr_t)c_hi | (uintptr_t)c_lo | (uintptr_t)workspace) % 16 == 0,
-              "dae_similarity_topk_bf16x3: operands and workspace must be 16-byte aligned");
-  const int s = topk_splits(n_query, n_corpus, splits);
-  const int64_t need = topk_workspace_bytes(n_query, k, s);
-  DAE_REQUIRE(workspace_bytes >= need, "dae_similarity_topk_bf16x3: workspace of %lld bytes, %lld needed (dae_similarity_topk_workspace)",
-              (long long)workspace_bytes, (long long)need);
-  cudaStream_t st = (cudaStream_t)stream;
+              "%s: leading dimensions must cover dim and be multiples of 8 (TMA 16-byte strides)", fn);
+  DAE_REQUIRE(((uintptr_t)q_hi | (uintptr_t)q_lo | (uintptr_t)c_hi | (uintptr_t)c_lo | a16) % 16 == 0 && a8 % 8 == 0 && a4 % 4 == 0,
+              "%s: %s", fn, alignment);
+  return DAE_OK;
+}
+
+// the partial lists of k in `workspace`: 2 s per query row
+static TopkParams topk_params(int32_t n_query, int32_t n_corpus, int32_t dim, int k, int s, int64_t diag_offset, int32_t exclude,
+                              void* workspace) {
   TopkParams tp{};
   tp.g.M = n_query; tp.g.N = n_corpus; tp.g.K = dim; tp.g.k_splits = 1; tp.g.alpha = 1.0f; tp.g.special_col = -1;
   tp.k = k; tp.splits = s; tp.exclude = exclude ? 1 : 0; tp.diag_offset = diag_offset;
   tp.ws_val = reinterpret_cast<float*>(workspace);
   tp.ws_idx = reinterpret_cast<int32_t*>(reinterpret_cast<float*>(workspace) + (int64_t)n_query * 2 * s * k);
-  Operand A{q_hi, q_lo, ldq, 0}, B{c_hi, c_lo, ldc, 0};
-  int rc = (k <= 16) ? launch_topk<16, false>(A, B, tp, st) : launch_topk<32, false>(A, B, tp, st);
+  return tp;
+}
+
+// dae_similarity_topk_bf16x3 (excl false), dae_similarity_topk_excl_bf16x3 (excl true, the lists ex_indptr / ex_indices) and
+// dae_similarity_topk_groups_bf16x3 (excl true, groups non-null; ex_indptr may be null when ex_nnz = 0: no lists)
+static int dense_topk(const char* fn, int32_t n_query, int32_t n_corpus, int32_t dim, const void* q_hi, const void* q_lo, int64_t ldq,
+                      const void* c_hi, const void* c_lo, int64_t ldc, int32_t k, int64_t diag_offset, int32_t exclude, int32_t splits,
+                      void* workspace, int64_t workspace_bytes, int32_t* idx_out, float* val_out, bool excl, const int64_t* ex_indptr,
+                      const int32_t* ex_indices, int64_t ex_nnz, const int32_t* groups, bool grouped, void* stream) {
+  DAE_REQUIRE(q_hi && q_lo && c_hi && c_lo && workspace && idx_out && val_out &&
+              (!excl || (grouped ? (groups && (ex_nnz == 0 || (ex_indptr && ex_indices))) : (ex_indptr && (ex_nnz == 0 || ex_indices)))),
+              "%s: null pointer", fn);
+  DAE_REQUIRE(n_query > 0 && n_corpus > 0 && dim > 0 && (!excl || ex_nnz >= 0), "%s: bad sizes", fn);
+  DAE_REQUIRE(k >= 1 && k <= kTopkMaxK, "%s: k = %d is outside the supported range 1 <= k <= %d", fn, k, kTopkMaxK);
+  int rc = check_operands(fn, dim, q_hi, q_lo, ldq, c_hi, c_lo, ldc, (uintptr_t)workspace, (uintptr_t)ex_indptr,
+                          (uintptr_t)ex_indices | (uintptr_t)groups,
+                          !excl     ? "operands and workspace must be 16-byte aligned"
+                          : grouped ? "operands and workspace must be 16-byte, ex_indptr 8-byte, ex_indices and groups 4-byte aligned"
+                                    : "operands and workspace must be 16-byte, ex_indptr 8-byte, ex_indices 4-byte aligned");
   if (rc) return rc;
-  DAE_CHECK_LAUNCH("dae_similarity_topk_bf16x3");
-  topk_merge_kernel<<<(n_query + 7) / 8, 256, 0, st>>>(tp.ws_val, tp.ws_idx, n_query, 2 * s, k, idx_out, val_out);
-  DAE_CHECK_LAUNCH("dae_similarity_topk_bf16x3 (merge)");
+  const int s = topk_splits(n_query, n_corpus, splits);
+  const int64_t need = topk_workspace_bytes(n_query, k, s);
+  DAE_REQUIRE(workspace_bytes >= need, "%s: workspace of %lld bytes, %lld needed (dae_similarity_topk_workspace)", fn,
+              (long long)workspace_bytes, (long long)need);
+  cudaStream_t st = (cudaStream_t)stream;
+  TopkParams tp = topk_params(n_query, n_corpus, dim, k, s, diag_offset, exclude, workspace);
+  tp.ex_indptr = ex_indptr; tp.ex_indices = ex_indices; tp.groups = groups;
+  Operand A{q_hi, q_lo, ldq, 0}, B{c_hi, c_lo, ldc, 0};
+  rc = !excl ? launch_topk<false, false>(A, B, tp, st) : !grouped ? launch_topk<true, false>(A, B, tp, st)
+                                                         : launch_topk<true, true>(A, B, tp, st);
+  if (rc) return rc;
+  DAE_CHECK_LAUNCH(fn);
+  if (grouped)
+    topk_merge_groups_kernel<<<(n_query + 7) / 8, 256, 0, st>>>(tp.ws_val, tp.ws_idx, groups, n_query, 2 * s, k, idx_out, val_out);
+  else
+    topk_merge_kernel<<<(n_query + 7) / 8, 256, 0, st>>>(tp.ws_val, tp.ws_idx, n_query, 2 * s, k, idx_out, val_out);
+  const cudaError_t e = cudaGetLastError();   // DAE_CHECK_LAUNCH with the name "<fn> (merge)"
+  if (e != cudaSuccess) {
+    set_error("%s (merge): %s", fn, cudaGetErrorString(e));
+    return DAE_ERR_CUDA;
+  }
   return DAE_OK;
+}
+
+extern "C" int dae_similarity_topk_bf16x3(int32_t n_query, int32_t n_corpus, int32_t dim, const void* q_hi, const void* q_lo, int64_t ldq,
+                                          const void* c_hi, const void* c_lo, int64_t ldc, int32_t k, int64_t diag_offset, int32_t exclude,
+                                          int32_t splits, void* workspace, int64_t workspace_bytes, int32_t* idx_out, float* val_out,
+                                          void* stream) {
+  return dense_topk("dae_similarity_topk_bf16x3", n_query, n_corpus, dim, q_hi, q_lo, ldq, c_hi, c_lo, ldc, k, diag_offset, exclude,
+                    splits, workspace, workspace_bytes, idx_out, val_out, false, nullptr, nullptr, 0, nullptr, false, stream);
 }
 
 extern "C" int dae_similarity_topk_excl_bf16x3(int32_t n_query, int32_t n_corpus, int32_t dim, const void* q_hi, const void* q_lo,
@@ -2105,35 +2079,8 @@ extern "C" int dae_similarity_topk_excl_bf16x3(int32_t n_query, int32_t n_corpus
                                                int64_t diag_offset, int32_t exclude, int32_t splits, void* workspace,
                                                int64_t workspace_bytes, int32_t* idx_out, float* val_out, const int64_t* ex_indptr,
                                                const int32_t* ex_indices, int64_t ex_nnz, void* stream) {
-  DAE_REQUIRE(q_hi && q_lo && c_hi && c_lo && workspace && idx_out && val_out && ex_indptr && (ex_nnz == 0 || ex_indices),
-              "dae_similarity_topk_excl_bf16x3: null pointer");
-  DAE_REQUIRE(n_query > 0 && n_corpus > 0 && dim > 0 && ex_nnz >= 0, "dae_similarity_topk_excl_bf16x3: bad sizes");
-  DAE_REQUIRE(k >= 1 && k <= kTopkMaxK, "dae_similarity_topk_excl_bf16x3: k = %d is outside the supported range 1 <= k <= %d", k,
-              kTopkMaxK);
-  DAE_REQUIRE(ldq >= dim && ldc >= dim && ldq % 8 == 0 && ldc % 8 == 0,
-              "dae_similarity_topk_excl_bf16x3: leading dimensions must cover dim and be multiples of 8 (TMA 16-byte strides)");
-  DAE_REQUIRE(((uintptr_t)q_hi | (uintptr_t)q_lo | (uintptr_t)c_hi | (uintptr_t)c_lo | (uintptr_t)workspace) % 16 == 0 &&
-                  (uintptr_t)ex_indptr % 8 == 0 && (uintptr_t)ex_indices % 4 == 0,
-              "dae_similarity_topk_excl_bf16x3: operands and workspace must be 16-byte, ex_indptr 8-byte, ex_indices 4-byte aligned");
-  const int s = topk_splits(n_query, n_corpus, splits);
-  const int64_t need = topk_workspace_bytes(n_query, k, s);
-  DAE_REQUIRE(workspace_bytes >= need,
-              "dae_similarity_topk_excl_bf16x3: workspace of %lld bytes, %lld needed (dae_similarity_topk_workspace)",
-              (long long)workspace_bytes, (long long)need);
-  cudaStream_t st = (cudaStream_t)stream;
-  TopkParams tp{};
-  tp.g.M = n_query; tp.g.N = n_corpus; tp.g.K = dim; tp.g.k_splits = 1; tp.g.alpha = 1.0f; tp.g.special_col = -1;
-  tp.k = k; tp.splits = s; tp.exclude = exclude ? 1 : 0; tp.diag_offset = diag_offset;
-  tp.ws_val = reinterpret_cast<float*>(workspace);
-  tp.ws_idx = reinterpret_cast<int32_t*>(reinterpret_cast<float*>(workspace) + (int64_t)n_query * 2 * s * k);
-  tp.ex_indptr = ex_indptr; tp.ex_indices = ex_indices;
-  Operand A{q_hi, q_lo, ldq, 0}, B{c_hi, c_lo, ldc, 0};
-  int rc = (k <= 16) ? launch_topk<16, true>(A, B, tp, st) : launch_topk<32, true>(A, B, tp, st);
-  if (rc) return rc;
-  DAE_CHECK_LAUNCH("dae_similarity_topk_excl_bf16x3");
-  topk_merge_kernel<<<(n_query + 7) / 8, 256, 0, st>>>(tp.ws_val, tp.ws_idx, n_query, 2 * s, k, idx_out, val_out);
-  DAE_CHECK_LAUNCH("dae_similarity_topk_excl_bf16x3 (merge)");
-  return DAE_OK;
+  return dense_topk("dae_similarity_topk_excl_bf16x3", n_query, n_corpus, dim, q_hi, q_lo, ldq, c_hi, c_lo, ldc, k, diag_offset, exclude,
+                    splits, workspace, workspace_bytes, idx_out, val_out, true, ex_indptr, ex_indices, ex_nnz, nullptr, false, stream);
 }
 
 extern "C" int dae_similarity_topk_groups_bf16x3(int32_t n_query, int32_t n_corpus, int32_t dim, const void* q_hi, const void* q_lo,
@@ -2141,36 +2088,9 @@ extern "C" int dae_similarity_topk_groups_bf16x3(int32_t n_query, int32_t n_corp
                                                  int64_t diag_offset, int32_t exclude, int32_t splits, void* workspace,
                                                  int64_t workspace_bytes, int32_t* idx_out, float* val_out, const int64_t* ex_indptr,
                                                  const int32_t* ex_indices, int64_t ex_nnz, const int32_t* groups, void* stream) {
-  DAE_REQUIRE(q_hi && q_lo && c_hi && c_lo && workspace && idx_out && val_out && groups && (ex_nnz == 0 || (ex_indptr && ex_indices)),
-              "dae_similarity_topk_groups_bf16x3: null pointer");
-  DAE_REQUIRE(n_query > 0 && n_corpus > 0 && dim > 0 && ex_nnz >= 0, "dae_similarity_topk_groups_bf16x3: bad sizes");
-  DAE_REQUIRE(k >= 1 && k <= kTopkMaxK, "dae_similarity_topk_groups_bf16x3: k = %d is outside the supported range 1 <= k <= %d", k,
-              kTopkMaxK);
-  DAE_REQUIRE(ldq >= dim && ldc >= dim && ldq % 8 == 0 && ldc % 8 == 0,
-              "dae_similarity_topk_groups_bf16x3: leading dimensions must cover dim and be multiples of 8 (TMA 16-byte strides)");
-  DAE_REQUIRE(((uintptr_t)q_hi | (uintptr_t)q_lo | (uintptr_t)c_hi | (uintptr_t)c_lo | (uintptr_t)workspace) % 16 == 0 &&
-                  (uintptr_t)ex_indptr % 8 == 0 && ((uintptr_t)ex_indices | (uintptr_t)groups) % 4 == 0,
-              "dae_similarity_topk_groups_bf16x3: operands and workspace must be 16-byte, ex_indptr 8-byte, ex_indices and groups "
-              "4-byte aligned");
-  const int s = topk_splits(n_query, n_corpus, splits);
-  const int64_t need = topk_workspace_bytes(n_query, k, s);
-  DAE_REQUIRE(workspace_bytes >= need,
-              "dae_similarity_topk_groups_bf16x3: workspace of %lld bytes, %lld needed (dae_similarity_topk_workspace)",
-              (long long)workspace_bytes, (long long)need);
-  cudaStream_t st = (cudaStream_t)stream;
-  TopkParams tp{};
-  tp.g.M = n_query; tp.g.N = n_corpus; tp.g.K = dim; tp.g.k_splits = 1; tp.g.alpha = 1.0f; tp.g.special_col = -1;
-  tp.k = k; tp.splits = s; tp.exclude = exclude ? 1 : 0; tp.diag_offset = diag_offset;
-  tp.ws_val = reinterpret_cast<float*>(workspace);
-  tp.ws_idx = reinterpret_cast<int32_t*>(reinterpret_cast<float*>(workspace) + (int64_t)n_query * 2 * s * k);
-  tp.ex_indptr = ex_indptr; tp.ex_indices = ex_indices; tp.groups = groups;
-  Operand A{q_hi, q_lo, ldq, 0}, B{c_hi, c_lo, ldc, 0};
-  int rc = (k <= 16) ? launch_topk<16, true, true>(A, B, tp, st) : launch_topk<32, true, true>(A, B, tp, st);
-  if (rc) return rc;
-  DAE_CHECK_LAUNCH("dae_similarity_topk_groups_bf16x3");
-  topk_merge_groups_kernel<<<(n_query + 7) / 8, 256, 0, st>>>(tp.ws_val, tp.ws_idx, groups, n_query, 2 * s, k, idx_out, val_out);
-  DAE_CHECK_LAUNCH("dae_similarity_topk_groups_bf16x3 (merge)");
-  return DAE_OK;
+  return dense_topk("dae_similarity_topk_groups_bf16x3", n_query, n_corpus, dim, q_hi, q_lo, ldq, c_hi, c_lo, ldc, k, diag_offset,
+                    exclude, splits, workspace, workspace_bytes, idx_out, val_out, true, ex_indptr, ex_indices, ex_nnz, groups, true,
+                    stream);
 }
 
 extern "C" int dae_similarity_pair_hist_bf16x3(int32_t n, int32_t dim, const void* x_hi, const void* x_lo, int64_t ldx,
@@ -2190,10 +2110,21 @@ extern "C" int dae_similarity_pair_hist_bf16x3(int32_t n, int32_t dim, const voi
   hp.labels = labels; hp.range = range; hp.scale = (float)bins / (2.0f * range); hp.bins = (uint32_t)bins;
   hp.hist = reinterpret_cast<unsigned long long*>(hist); hp.sums = sums;
   Operand X{x_hi, x_lo, ldx, 0};
-  int rc = launch_pair_hist(X, hp, (cudaStream_t)stream);
+  const long long tm = (n + BLOCK_M - 1) / BLOCK_M;   // work items: the lower-triangle tiles
+  int rc = launch_persistent<pair_hist_kernel, kTopkBK, kTopkStages>(X, X, hp.g, hp, tm * (tm + 1) / 2, (cudaStream_t)stream);
   if (rc) return rc;
   DAE_CHECK_LAUNCH("dae_similarity_pair_hist_bf16x3");
   return DAE_OK;
+}
+
+// the PairsParams common to dae_similarity_pairs_bf16x3 and the collect stage of long top-k lists
+static PairsParams pairs_params(int32_t n_query, int32_t n_corpus, int32_t dim, uint64_t* count, int64_t capacity, int32_t* i_out,
+                                int32_t* j_out, float* s_out) {
+  PairsParams pp{};
+  pp.g.M = n_query; pp.g.N = n_corpus; pp.g.K = dim; pp.g.k_splits = 1; pp.g.alpha = 1.0f; pp.g.special_col = -1;
+  pp.count = reinterpret_cast<unsigned long long*>(count); pp.capacity = (unsigned long long)capacity;
+  pp.i_out = i_out; pp.j_out = j_out; pp.s_out = s_out;
+  return pp;
 }
 
 extern "C" int dae_similarity_pairs_bf16x3(int32_t n_query, int32_t n_corpus, int32_t dim, const void* q_hi, const void* q_lo, int64_t ldq,
@@ -2207,18 +2138,14 @@ extern "C" int dae_similarity_pairs_bf16x3(int32_t n_query, int32_t n_corpus, in
   DAE_REQUIRE(!self || (n_query == n_corpus && q_hi == c_hi && q_lo == c_lo && ldq == ldc),
               "dae_similarity_pairs_bf16x3: self mode needs the corpus operands to be the query operands");
   DAE_REQUIRE(pair_threshold_ok(threshold), "dae_similarity_pairs_bf16x3: threshold %g is not finite", (double)threshold);
-  DAE_REQUIRE(ldq >= dim && ldc >= dim && ldq % 8 == 0 && ldc % 8 == 0,
-              "dae_similarity_pairs_bf16x3: leading dimensions must cover dim and be multiples of 8 (TMA 16-byte strides)");
-  DAE_REQUIRE(((uintptr_t)q_hi | (uintptr_t)q_lo | (uintptr_t)c_hi | (uintptr_t)c_lo) % 16 == 0 && (uintptr_t)count % 8 == 0 &&
-                  ((uintptr_t)i_out | (uintptr_t)j_out | (uintptr_t)s_out) % 4 == 0,
-              "dae_similarity_pairs_bf16x3: operands must be 16-byte, the counter 8-byte and the outputs 4-byte aligned");
-  PairsParams pp{};
-  pp.g.M = n_query; pp.g.N = n_corpus; pp.g.K = dim; pp.g.k_splits = 1; pp.g.alpha = 1.0f; pp.g.special_col = -1;
+  int rc = check_operands("dae_similarity_pairs_bf16x3", dim, q_hi, q_lo, ldq, c_hi, c_lo, ldc, 0, (uintptr_t)count,
+                          (uintptr_t)i_out | (uintptr_t)j_out | (uintptr_t)s_out,
+                          "operands must be 16-byte, the counter 8-byte and the outputs 4-byte aligned");
+  if (rc) return rc;
+  PairsParams pp = pairs_params(n_query, n_corpus, dim, count, capacity, i_out, j_out, s_out);
   pp.self = self ? 1 : 0; pp.tau = threshold;
-  pp.count = reinterpret_cast<unsigned long long*>(count); pp.capacity = (unsigned long long)capacity;
-  pp.i_out = i_out; pp.j_out = j_out; pp.s_out = s_out;
   Operand A{q_hi, q_lo, ldq, 0}, B{c_hi, c_lo, ldc, 0};
-  int rc = launch_pairs(A, B, pp, (cudaStream_t)stream);
+  rc = launch_pairs<false>(A, B, pp, (cudaStream_t)stream);
   if (rc) return rc;
   DAE_CHECK_LAUNCH("dae_similarity_pairs_bf16x3");
   return DAE_OK;
@@ -2262,27 +2189,21 @@ extern "C" int dae_similarity_topk_bound_bf16x3(int32_t n_query, int32_t n_corpu
   DAE_REQUIRE(n_query > 0 && n_corpus > 0 && dim > 0 && ex_nnz >= 0, "dae_similarity_topk_bound_bf16x3: bad sizes");
   DAE_REQUIRE(k >= 1 && k <= kTopkLongMaxK, "dae_similarity_topk_bound_bf16x3: k = %d is outside the supported range 1 <= k <= %d", k,
               kTopkLongMaxK);
-  DAE_REQUIRE(ldq >= dim && ldc >= dim && ldq % 8 == 0 && ldc % 8 == 0,
-              "dae_similarity_topk_bound_bf16x3: leading dimensions must cover dim and be multiples of 8 (TMA 16-byte strides)");
-  DAE_REQUIRE(((uintptr_t)q_hi | (uintptr_t)q_lo | (uintptr_t)c_hi | (uintptr_t)c_lo | (uintptr_t)workspace) % 16 == 0 &&
-                  (uintptr_t)ex_indptr % 8 == 0 && ((uintptr_t)ex_indices | (uintptr_t)groups | (uintptr_t)tau) % 4 == 0,
-              "dae_similarity_topk_bound_bf16x3: operands and workspace must be 16-byte, ex_indptr 8-byte, ex_indices, groups and tau "
-              "4-byte aligned");
+  int rc = check_operands("dae_similarity_topk_bound_bf16x3", dim, q_hi, q_lo, ldq, c_hi, c_lo, ldc, (uintptr_t)workspace,
+                          (uintptr_t)ex_indptr, (uintptr_t)ex_indices | (uintptr_t)groups | (uintptr_t)tau,
+                          "operands and workspace must be 16-byte, ex_indptr 8-byte, ex_indices, groups and tau 4-byte aligned");
+  if (rc) return rc;
   const int s = topk_bound_splits(n_query, n_corpus, k, splits);
   const int64_t need = topk_workspace_bytes(n_query, kTopkMaxK, s);
   DAE_REQUIRE(workspace_bytes >= need,
               "dae_similarity_topk_bound_bf16x3: workspace of %lld bytes, %lld needed (dae_similarity_topk_bound_workspace)",
               (long long)workspace_bytes, (long long)need);
   cudaStream_t st = (cudaStream_t)stream;
-  TopkParams tp{};
-  tp.g.M = n_query; tp.g.N = n_corpus; tp.g.K = dim; tp.g.k_splits = 1; tp.g.alpha = 1.0f; tp.g.special_col = -1;
-  tp.k = kTopkMaxK; tp.splits = s; tp.exclude = exclude ? 1 : 0; tp.diag_offset = diag_offset;
-  tp.ws_val = reinterpret_cast<float*>(workspace);
-  tp.ws_idx = reinterpret_cast<int32_t*>(reinterpret_cast<float*>(workspace) + (int64_t)n_query * 2 * s * kTopkMaxK);
+  TopkParams tp = topk_params(n_query, n_corpus, dim, kTopkMaxK, s, diag_offset, exclude, workspace);
   tp.ex_indptr = ex_nnz ? ex_indptr : nullptr; tp.ex_indices = ex_indices; tp.groups = groups;
   Operand A{q_hi, q_lo, ldq, 0}, B{c_hi, c_lo, ldc, 0};
-  int rc = groups ? launch_topk<32, true, true>(A, B, tp, st)
-                  : (tp.ex_indptr ? launch_topk<32, true>(A, B, tp, st) : launch_topk<32, false>(A, B, tp, st));
+  rc = groups ? launch_topk<true, true>(A, B, tp, st)
+              : (tp.ex_indptr ? launch_topk<true, false>(A, B, tp, st) : launch_topk<false, false>(A, B, tp, st));
   if (rc) return rc;
   DAE_CHECK_LAUNCH("dae_similarity_topk_bound_bf16x3");
   const int L = rank_chunk(k);
@@ -2305,23 +2226,17 @@ extern "C" int dae_similarity_topk_collect_bf16x3(int32_t n_query, int32_t n_cor
   DAE_REQUIRE(capacity == 0 || (i_out && j_out && s_out), "dae_similarity_topk_collect_bf16x3: null output with capacity %lld > 0",
               (long long)capacity);
   DAE_REQUIRE(n_query > 0 && n_corpus > 0 && dim > 0 && ex_nnz >= 0, "dae_similarity_topk_collect_bf16x3: bad sizes");
-  DAE_REQUIRE(ldq >= dim && ldc >= dim && ldq % 8 == 0 && ldc % 8 == 0,
-              "dae_similarity_topk_collect_bf16x3: leading dimensions must cover dim and be multiples of 8 (TMA 16-byte strides)");
-  DAE_REQUIRE(((uintptr_t)q_hi | (uintptr_t)q_lo | (uintptr_t)c_hi | (uintptr_t)c_lo) % 16 == 0 &&
-                  ((uintptr_t)count | (uintptr_t)ex_indptr) % 8 == 0 &&
-                  ((uintptr_t)tau | (uintptr_t)row_count | (uintptr_t)ex_indices | (uintptr_t)i_out | (uintptr_t)j_out |
-                   (uintptr_t)s_out) % 4 == 0,
-              "dae_similarity_topk_collect_bf16x3: operands must be 16-byte, the counter and ex_indptr 8-byte, the other arrays 4-byte "
-              "aligned");
-  PairsParams pp{};
-  pp.g.M = n_query; pp.g.N = n_corpus; pp.g.K = dim; pp.g.k_splits = 1; pp.g.alpha = 1.0f; pp.g.special_col = -1;
-  pp.self = 0; pp.tau = 0.0f;
-  pp.count = reinterpret_cast<unsigned long long*>(count); pp.capacity = (unsigned long long)capacity;
-  pp.i_out = i_out; pp.j_out = j_out; pp.s_out = s_out;
+  int rc = check_operands("dae_similarity_topk_collect_bf16x3", dim, q_hi, q_lo, ldq, c_hi, c_lo, ldc, 0,
+                          (uintptr_t)count | (uintptr_t)ex_indptr,
+                          (uintptr_t)tau | (uintptr_t)row_count | (uintptr_t)ex_indices | (uintptr_t)i_out | (uintptr_t)j_out |
+                              (uintptr_t)s_out,
+                          "operands must be 16-byte, the counter and ex_indptr 8-byte, the other arrays 4-byte aligned");
+  if (rc) return rc;
+  PairsParams pp = pairs_params(n_query, n_corpus, dim, count, capacity, i_out, j_out, s_out);
   pp.row_tau = tau; pp.diag_offset = diag_offset; pp.exclude = exclude ? 1 : 0;
   pp.ex_indptr = ex_nnz ? ex_indptr : nullptr; pp.ex_indices = ex_indices; pp.row_count = row_count;
   Operand A{q_hi, q_lo, ldq, 0}, B{c_hi, c_lo, ldc, 0};
-  int rc = launch_pairs<true>(A, B, pp, (cudaStream_t)stream);
+  rc = launch_pairs<true>(A, B, pp, (cudaStream_t)stream);
   if (rc) return rc;
   DAE_CHECK_LAUNCH("dae_similarity_topk_collect_bf16x3");
   return DAE_OK;

@@ -155,3 +155,74 @@ def test_gemm_output_contract_rejected_before_device_work(args, what, det):
     a = a + ((112, 1 << 30, None) if det else (None,))
     with pytest.raises(_cabi.DaeError, match='%s: .*%s' % (name, what)):
         _cabi.call(name, *a)
+
+
+# the argument checks of dae_decode_fused_bf16x3 / _det and dae_gemm_sym_bf16x3 / _det, each under the export's own name; the
+# pointers are never dereferenced, since every case is rejected before any device work
+def _decode_args(**bad):
+    a = dict(Brows=100, F=500, K=64, e_hi=16, e_lo=32, lde=64, w_hi=48, w_lo=64, ldw=64, indptr=80, indices=96, values=112, rows=None,
+             bv=128, dec_act=1, loss_func=0, weight=None, stats=144, dz_hi=160, dz_lo=176, ld_dz=512, row_loss_part=192, tile_ptr=208,
+             prepared=1, stream=None)
+    a.update(bad)
+    return tuple(a.values())
+
+
+BAD_DECODE = [
+    (dict(e_hi=None), 'null pointer'),
+    (dict(w_lo=None), 'null pointer'),
+    (dict(indices=None), 'null pointer'),
+    (dict(stats=None), 'null pointer'),
+    (dict(dz_lo=None), 'null pointer'),
+    (dict(row_loss_part=None), 'null pointer'),
+    (dict(tile_ptr=None), 'null pointer'),
+    (dict(loss_func=2), 'cosine loss uses the unfused path'),     # DAE_LOSS_COSINE
+    (dict(loss_func=7), 'cosine loss uses the unfused path'),
+    (dict(ld_dz=520), 'bad leading dimensions'),                   # covers F, not a multiple of 32
+    (dict(ld_dz=480), 'bad leading dimensions'),                   # a multiple of 32 below F
+    (dict(lde=60), 'bad leading dimensions'),
+    (dict(ldw=68), 'bad leading dimensions'),
+]
+
+
+@pytest.mark.parametrize('bad,what', BAD_DECODE)
+@pytest.mark.parametrize('det', [False, True])
+def test_decode_fused_arguments_rejected_before_device_work(bad, what, det):
+    from dae_rnn_news_recommendation_b200 import _cabi
+    name = 'dae_decode_fused_bf16x3_det' if det else 'dae_decode_fused_bf16x3'
+    with pytest.raises(_cabi.DaeError, match=r'%s failed \(-1\): %s: .*%s' % (name, name, what)):
+        _cabi.call(name, *_decode_args(**bad))
+
+
+def _sym_args(det, **bad):
+    a = dict(M=100, N=500, alpha=1.0, g_hi=16, g_lo=32, ldg=104, b_hi=48, b_lo=64, ldb=504, C=80, ldc=500, accumulate=0)
+    if det:
+        a.update(workspace=96, workspace_bytes=1 << 40)
+    a['stream'] = None
+    a.update(bad)
+    return tuple(a.values())
+
+
+BAD_SYM = [
+    (dict(g_hi=None), 'bad arguments'),
+    (dict(b_lo=None), 'bad arguments'),
+    (dict(C=None), 'bad arguments'),
+    (dict(M=0), 'bad arguments'),
+    (dict(ldg=100), 'multiples of 8 and cover'),       # covers M, not a multiple of 8
+    (dict(ldg=96), 'multiples of 8 and cover'),        # below M
+    (dict(ldb=502), 'multiples of 8 and cover'),
+    (dict(ldb=496), 'multiples of 8 and cover'),       # below N
+    (dict(g_lo=40), '16-byte aligned'),
+    (dict(b_hi=56), '16-byte aligned'),
+]
+BAD_SYM_DET = [
+    (dict(workspace_bytes=1), 'workspace of 1 bytes, need'),
+    (dict(workspace=None), 'workspace of .* bytes, need'),
+]
+
+
+@pytest.mark.parametrize('bad,what,det', [(b, w, d) for b, w in BAD_SYM for d in (False, True)] + [(b, w, True) for b, w in BAD_SYM_DET])
+def test_gemm_sym_arguments_rejected_before_device_work(bad, what, det):
+    from dae_rnn_news_recommendation_b200 import _cabi
+    name = 'dae_gemm_sym_bf16x3_det' if det else 'dae_gemm_sym_bf16x3'
+    with pytest.raises(_cabi.DaeError, match=r'%s failed \(-1\): %s: .*%s' % (name, name, what)):
+        _cabi.call(name, *_sym_args(det, **bad))
