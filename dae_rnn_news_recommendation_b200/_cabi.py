@@ -105,6 +105,8 @@ _SIGNATURES = {
     # LSTM user encoder
     'dae_lstm_cell_fwd': (C.c_int, [i32, i32, p, i64, p, i64, p, i64, p, i64, p, i64, i32, p, p, i64, p, i64, p]),
     'dae_lstm_cell_bwd': (C.c_int, [i32, i32, p, i64, p, i64, p, i64, p, i64, p, i64, p, i64, p, p, i64, p]),
+    # long-term user vectors
+    'dae_rows_optimizer_step': (C.c_int, [p, i64, i32, p, i32, p, i64, p, p, p, i32, f32, f32, p]),
     # attention user encoder
     'dae_seq_attention_fwd': (C.c_int, [i32, i32, p, p, i32, i32, p, i64, p, i64, p, p, i64, p, i64, p]),
     'dae_seq_attention_bwd': (C.c_int, [i32, i32, p, p, i32, i32, p, i64, p, i64, p, i64, p, i64, p, p, i64, p]),

@@ -231,6 +231,50 @@ def make_impressions(indptr, items, labels, targets=None, shown=20, seed=0, trie
     return train, test
 
 
+def make_long_term_impressions(n_users, labels, window=5, history=(20, 40), shown=5, home_share=0.7, seed=0):
+    """Reading sequences whose signal lies before the last `window` reads, and one training and one test impression per user
+    (user_model.check_impressions' keys): the learning check of the long-term user vectors (DESIGN 4.18).  labels: class ids of
+    the articles (at least 3 classes).  Each user has a home class.  The first h reads (h uniform in `history`) come in sessions
+    of 2 to 5 reads, each from the home class with probability home_share and from another class otherwise; the last `window`
+    reads are one session of a noise class, never home.  Both impressions are at time = len, so an encoder that sees only the
+    last `window` reads has seen only the noise session: each clicks one home-class article and shows shown - 1 non-clicks,
+    (shown - 1) // 2 from the noise class and the rest from the classes that are neither.  Returns (indptr, items, train, test)."""
+    rng = np.random.default_rng(seed)
+    labels = np.asarray(labels).astype(np.int64)
+    C = int(labels.max()) + 1
+    pools = [np.flatnonzero(labels == c) for c in range(C)]
+    seqs = []
+    imps = ([], [])
+    n_noise = (shown - 1) // 2
+    for u in range(n_users):
+        home = int(rng.integers(C))
+        others = [c for c in range(C) if c != home]
+        h = int(rng.integers(history[0], history[1] + 1))
+        s = []
+        while len(s) < h:
+            c = home if rng.random() < home_share else others[int(rng.integers(len(others)))]
+            s.extend(rng.choice(pools[c], int(rng.integers(2, 6))))
+        noise = others[int(rng.integers(len(others)))]
+        s = np.concatenate([np.asarray(s[:h]), rng.choice(pools[noise], window)])
+        seqs.append(s)
+        rest = np.concatenate([pools[c] for c in others if c != noise])
+        for imp in imps:
+            shown_items = np.concatenate([rng.choice(pools[home], 1), rng.choice(pools[noise], n_noise, replace=False),
+                                          rng.choice(rest, shown - 1 - n_noise, replace=False)])
+            clicked = np.zeros(shown, np.uint8)
+            clicked[0] = 1
+            o = rng.permutation(shown)
+            imp.append((u, s.size, shown_items[o], clicked[o]))
+    indptr = np.concatenate([[0], np.cumsum([s.size for s in seqs])]).astype(np.int64)
+    items = np.concatenate(seqs).astype(np.int32)
+
+    def pack(imp):
+        return {'user': np.array([x[0] for x in imp], np.int64), 'time': np.array([x[1] for x in imp], np.int64),
+                'indptr': np.arange(len(imp) + 1, dtype=np.int64) * shown, 'items': np.concatenate([x[2] for x in imp]).astype(np.int32),
+                'clicked': np.concatenate([x[3] for x in imp])}
+    return indptr, items, pack(imps[0]), pack(imps[1])
+
+
 def make_labels(n_rows, n_classes=4, seed=0):
     return np.random.default_rng(seed + 7919).integers(0, n_classes, n_rows).astype(np.float32)
 

@@ -35,14 +35,22 @@ UserLSTM (DESIGN 4.15) is the same encoder with torch.nn.LSTM's cell (gate order
 torch.nn.LSTM(H, H)): the same constructor, losses, negatives, batches and methods, with 4H-wide projections and
 dae_lstm_cell_fwd / dae_lstm_cell_bwd in place of the GRU's cell kernels.  Both derive from _UserRNN, which holds everything
 that does not depend on the cell.
+
+Long-term user vectors (DESIGN 4.18, LSTUR-ini): UserGRU / UserLSTM(..., long_term_users=U) learn a vector P[u] per user (the
+long_term attribute, [U, H] fp32, zero at first) and start u's window from h_0 = P[u] instead of 0, so that what a user read
+before the last max_len reads still shapes the state.  Training masks each batch user with probability long_term_mask (LSTUR's
+training: a masked user starts from 0) and updates only the rows of the unmasked batch users, by dae_rows_optimizer_step
+(long_term_learning_rate).  transform, impression_states and recommend start every user from its row, with no mask; users at or
+beyond row U (cold-start users) start from 0.  save() / load() keep the table; state_dict() keeps torch's four keys.
 """
 import numpy as np
 import torch
 
-from . import _cabi
+from . import _cabi, sparse_optim
 from ._cabi import call
 
 _NAMES = ('weight_ih_l0', 'weight_hh_l0', 'bias_ih_l0', 'bias_hh_l0')
+LONG_TERM_LEARNING_RATE = 0.1    # the long-term table's default learning rate: the best of 0.01, 0.03 and 0.1 (DESIGN 4.18)
 
 
 def _stream():
@@ -193,7 +201,8 @@ class ImpressionBatch:
 class Packed:
     """One batch in the PackedSequence layout.  order: the batch's users (ids) by truncated length L, descending (stable), users with
     L = 0 left out; n[t] = users with L > t; off[t] = first position of step t; position off[t] + i is user order[i]'s read t.
-    items[p]: the article read at position p; nxt[p]: the article read next (-1 at a user's last position)."""
+    items[p]: the article read at position p; nxt[p]: the article read next (-1 at a user's last position).  users: the user each
+    row belongs to, order itself unless the rows are impression_states' runs (which set it)."""
 
     def __init__(self, indptr, items, users, max_len):
         users = np.asarray(users, dtype=np.int64)
@@ -202,6 +211,7 @@ class Packed:
         users, L = users[keep], L[keep]
         s = np.argsort(-L, kind='stable')
         self.order, self.L = users[s], L[s]
+        self.users = self.order
         self.B = int(self.order.size)
         T = int(self.L[0]) if self.B else 0
         self.n = np.searchsorted(-self.L, -np.arange(T), side='left').astype(np.int64)   # #{i: L_i > t}
@@ -285,9 +295,13 @@ class _UserEncoder:
             a[k] = v.astype(np.float32)
         return a
 
-    def save(self, path):
+    def _files(self):
+        """save()'s arrays: max_len, the encoder's _CONFIG and the state dict."""
         sd = self.state_dict()
-        np.savez(path, max_len=self.max_len, **{k: getattr(self, k) for k in self._CONFIG}, **{k: v.numpy() for k, v in sd.items()})
+        return dict(max_len=self.max_len, **{k: getattr(self, k) for k in self._CONFIG}, **{k: v.numpy() for k, v in sd.items()})
+
+    def save(self, path):
+        np.savez(path, **self._files())
 
     @classmethod
     def load(cls, path, **kw):
@@ -435,7 +449,9 @@ class _UserEncoder:
 
     # ---- inference --------------------------------------------------------------------------------------------------------
     def transform(self, sequences, embeddings, to_host=True):
-        """User vectors [U, H] fp32: the state after each user's last (truncated) read; zero rows for users without reads.  Device
+        """User vectors [U, H] fp32: the state after each user's last (truncated) read; zero rows for users without reads.  With a
+        long-term table (UserGRU / UserLSTM) user u's window starts from P[u], and users at or beyond long_term_users (cold-start
+        users, whom training never saw) from 0, as without the table.  Device
         memory per batch: O(batch_users x GATES H) for the recurrent cells, which project step by step; O(batch positions x (3H + A))
         for UserAttention, which runs each batch in one pass."""
         fn = '%s.transform' % type(self).__name__
@@ -459,7 +475,8 @@ class _UserEncoder:
         read len - max_len whatever the impression's time; here the window ENDS at the impression.  The two agree at time = len
         and for users with at most max_len reads.  Each (user, window start) pair is one run of a packed batch, whose states are
         copied out at the steps that impressions ask for: a user whose impressions all lie within the first max_len reads costs
-        one run.  Device memory per batch is transform's."""
+        one run.  With a long-term table every run starts from P[its user] (a cold-start user at or beyond long_term_users from 0),
+        whatever the window's start.  Device memory per batch is transform's."""
         fn = '%s.impression_states' % type(self).__name__
         emb = self._embeddings(embeddings, fn)
         indptr, items = check_sequences(sequences, emb.shape[0], fn)
@@ -487,8 +504,10 @@ class _UserEncoder:
         B = self.batch_users
         s = self._infer_buffers(B)
         order = np.argsort(run_of, kind='stable')
+        run_user = u[first]
         for r0 in range(0, n_run, B):
             pk = Packed(r_indptr, r_items, np.arange(r0, min(n_run, r0 + B)), self.max_len)
+            pk.users = run_user[pk.order]
             row = np.empty(n_run, np.int64)
             row[pk.order] = np.arange(pk.B)
             lo, hi = np.searchsorted(run_of[order], [r0, r0 + B])
@@ -516,16 +535,35 @@ class _UserRNN(_UserEncoder):
     """What the recurrent user encoders share (UserGRU, UserLSTM): the flat parameters theta = [W~_hh | W~_ih] of GATES H rows each,
     their torch.nn.GRU / torch.nn.LSTM names, the packed training batch's step loops and the step loop of transform and
     impression_states.  A cell class supplies GATES, its extra buffers, the carries its backward zeroes, the packed gradient
-    operands of the two weight GEMMs and its two kernel calls (_cell_fwd / _cell_bwd for training, _step for inference)."""
+    operands of the two weight GEMMs and its two kernel calls (_cell_fwd / _cell_bwd for training, _step for inference).
+
+    Long-term user vectors (LSTUR-ini, DESIGN 4.18): with long_term_users = U the encoder keeps a table P [U, H] fp32 (the
+    long_term attribute), zero at first, and user u's window starts from h_0 = P[u] (the LSTM's c_0 stays 0) in fit, transform,
+    impression_states and recommend; users at or beyond row U (cold-start users) start from 0.  In training each batch user is
+    masked with probability long_term_mask, drawn per (seed, epoch, user id): a masked user starts from 0 and its row is not
+    updated.  dL/dh_0 of the unmasked users updates their rows after theta's step by dae_rows_optimizer_step (the encoder's opt
+    and momentum, learning rate long_term_learning_rate, Adam's bias correction counted per row); other rows and their slots are
+    not touched.  The table holds one more row, index U, that stays zero: masked and cold-start users gather it."""
     GATES = 0
-    _STATES = ('h',)                 # [B x H] inference states, zero at a batch's first step
+    _STATES = ('h',)                 # [B x H] inference states, zero at a batch's first step (h: P[u] with the long-term table)
     _CARRIES = ('carry',)            # [B x H] backward carries zeroed for the rows of step 0
     _DGRAD = ('dHP_hl', 'dXP_hl')    # packed gradient operands of [dW_hh | db_hh] and [dW_ih | db_ih]
     _CARRY_ACCUMULATE = 1            # the carry GEMM dh_{t-1} (+)= dHP_t . W_hh accumulates onto the cell's carry, or stores
     _PARAMS = _NAMES
 
-    def __init__(self, dim, *args, **kw):
+    def __init__(self, dim, *args, long_term_users=None, long_term_mask=0.5, long_term_learning_rate=None, **kw):
         super().__init__(dim, *args, **kw)
+        name = type(self).__name__
+        if long_term_users is not None and (isinstance(long_term_users, bool) or not isinstance(long_term_users, (int, np.integer))
+                                            or long_term_users < 1):
+            raise ValueError('%s: long_term_users = %r, None or an integer >= 1' % (name, long_term_users))
+        if not 0.0 <= long_term_mask <= 1.0:
+            raise ValueError('%s: long_term_mask = %r must lie in [0, 1]' % (name, long_term_mask))
+        lr = LONG_TERM_LEARNING_RATE if long_term_learning_rate is None else float(long_term_learning_rate)
+        if not lr > 0.0:
+            raise ValueError('%s: long_term_learning_rate = %r must be > 0' % (name, long_term_learning_rate))
+        self.long_term_users = None if long_term_users is None else int(long_term_users)
+        self.long_term_mask, self.long_term_learning_rate = float(long_term_mask), lr
         H, G = self.dim, self.GATES
         self.nW = G * H * (H + 1)
         self.ldx, self.ldg = _ld8(H + 1), _ld8(G * H)
@@ -536,6 +574,43 @@ class _UserRNN(_UserEncoder):
         bf = dict(dtype=torch.bfloat16, device=self.device)
         self.W_hl = {g: (torch.zeros(G * H, self.ldx, **bf), torch.zeros(G * H, self.ldx, **bf)) for g in ('hh', 'ih')}
         self._hh_valid = False
+        self._lt = self._lt_slot1 = self._lt_slot2 = self._lt_count = self._lt_batch = self._lt_kept = None
+        if self.long_term_users is not None:
+            shape, f32 = (self.long_term_users + 1, H), dict(dtype=torch.float32, device=self.device)
+            self._lt = torch.zeros(shape, **f32)
+            if self.opt != 'gradient_descent':
+                self._lt_slot1 = torch.full(shape, 0.1 if self.opt == 'ada_grad' else 0.0, **f32)
+            if self.opt == 'adam':
+                self._lt_slot2 = torch.zeros(shape, **f32)
+            self._lt_count = torch.zeros(shape[0], dtype=torch.int32, device=self.device)
+
+    @property
+    def long_term(self):
+        """The long-term user vectors P [long_term_users, H] fp32 on the device (a view: writing it changes the model), or None."""
+        return None if self._lt is None else self._lt[:self.long_term_users]
+
+    def long_term_kept(self, epoch):
+        """Boolean [long_term_users]: the users that start from their row of P in the training batches of this epoch, each kept
+        with probability 1 - long_term_mask by a draw keyed by (seed, epoch, user id), so the set does not depend on batch_users or
+        on the batch order."""
+        if self._lt_kept is None or self._lt_kept[0] != epoch:
+            u = np.random.default_rng([self.seed, epoch, 1]).random(self.long_term_users)
+            self._lt_kept = (epoch, u >= self.long_term_mask)
+        return self._lt_kept[1]
+
+    def _table_rows(self, users):
+        """The row of P each user starts from: its own below long_term_users, else the zero row."""
+        return np.where(users < self.long_term_users, users, self.long_term_users).astype(np.int32)
+
+    def _initial_states(self, rows, n, hi, lo, h, st):
+        """h_0 of rows [0, n): [P[rows] | 1] as the recurrent GEMM's bf16 hi / lo operand, and P[rows] in fp32 into h."""
+        H = self.dim
+        call('dae_gather_split_bf16', self._lt.data_ptr(), H, rows.data_ptr(), n, H, hi.data_ptr(), lo.data_ptr(), self.ldx, H, st)
+        torch.index_select(self._lt, 0, rows[:n], out=h[:n])
+
+    def _h0(self, b):
+        """The training cell's h_prev at step 0: the gathered P rows with the long-term table, else NULL (h_{-1} = 0)."""
+        return None if self._lt is None else b['h0'].data_ptr()
 
     # ---- parameters -------------------------------------------------------------------------------------------------------
     def _theta(self, g):
@@ -563,6 +638,40 @@ class _UserRNN(_UserEncoder):
     def _dim_of(z):
         return int(z['weight_hh_l0'].shape[1])
 
+    def _files(self):
+        f = super()._files()
+        if self._lt is not None:
+            f.update(long_term_users=self.long_term_users, long_term=self.long_term.cpu().numpy())
+        return f
+
+    @classmethod
+    def load(cls, path, **kw):
+        """As _UserEncoder.load; a file with a long-term table (long_term_users and long_term) restores it."""
+        z = np.load(path)
+        if 'long_term_users' in z.files:
+            kw.setdefault('long_term_users', int(z['long_term_users']))
+        m = super().load(path, **kw)
+        if m._lt is not None and 'long_term' in z.files:
+            P = z['long_term']
+            if P.shape != tuple(m.long_term.shape):
+                raise ValueError('%s.load: %s holds a long-term table of shape %s, the model has %s' % (
+                    cls.__name__, path, P.shape, tuple(m.long_term.shape)))
+            m.long_term.copy_(torch.from_numpy(P.astype(np.float32)))
+        return m
+
+    def fit(self, sequences, embeddings, impressions=None):
+        """_UserEncoder.fit; with the long-term table the sequences may hold at most long_term_users rows (ValueError before any
+        device work otherwise)."""
+        if self._lt is not None:
+            try:
+                n_u = len(sequences[0]) - 1
+            except (TypeError, IndexError, KeyError):
+                n_u = 0      # malformed: check_sequences reports it
+            if n_u > self.long_term_users:
+                raise ValueError('%s.fit: the sequences hold %d users, the long-term table %d rows (long_term_users)' % (
+                    type(self).__name__, n_u, self.long_term_users))
+        return super().fit(sequences, embeddings, impressions)
+
     # ---- device helpers ---------------------------------------------------------------------------------------------------
     def _split(self, g):
         hi, lo = self.W_hl[g]
@@ -588,6 +697,8 @@ class _UserRNN(_UserEncoder):
              'dH': torch.empty(P, H, **f32),
              'carry': torch.empty(B, H, **f32)}
         b.update(self._cell_buffers(P, B))
+        if self._lt is not None:
+            b['h0'] = torch.empty(B, H, **f32)     # fp32 h_0 of the batch's users
         b['Hp_hl'][0][:, H] = 1.0
         self._buf, self._cap = b, (P, B)
         return b
@@ -597,6 +708,22 @@ class _UserRNN(_UserEncoder):
         if not self._hh_valid:
             self._split('hh')
             self._hh_valid = True
+
+    def _forward_backward(self, pk, emb, epoch, batch, ib=None):
+        if self._lt is not None:   # per user of the batch: the row h_0 comes from (masked: the zero row) and the row to update (-1)
+            keep = self.long_term_kept(epoch)[pk.order]
+            rows = np.stack([np.where(keep, pk.order, self.long_term_users), np.where(keep, pk.order, -1)]).astype(np.int32)
+            self._lt_batch = (_upload(rows, self.device), pk.B)
+        super()._forward_backward(pk, emb, epoch, batch, ib)
+
+    def _optimizer_step(self):
+        """theta's step, then with the long-term table the row step of the batch's unmasked users from dL/dh_0 (the carry)."""
+        super()._optimizer_step()
+        if self._lt is not None:
+            rows, n = self._lt_batch
+            sparse_optim.rows_step(self._lt, self._lt_slot1, self._lt_slot2, self._lt_count, rows[1], n, self._buf['carry'], self.opt,
+                                   self.long_term_learning_rate, self.momentum, _stream())
+            self._mark('long_term')
 
     def _forward(self, b, pk, emb, items, st):
         """The input projection of every position, then per step the recurrent GEMM and the cell: b['Hs']."""
@@ -609,8 +736,11 @@ class _UserRNN(_UserEncoder):
         self._mark('input_projection')
         Hp_hi, Hp_lo = b['Hp_hl']
         n0 = int(pk.n[0])
-        Hp_hi[:n0, :H].zero_()
-        Hp_lo[:n0].zero_()
+        if self._lt is None:
+            Hp_hi[:n0, :H].zero_()
+            Hp_lo[:n0].zero_()
+        else:
+            self._initial_states(self._lt_batch[0][0], n0, Hp_hi, Hp_lo, b['h0'], st)
         Hs, HP = b['Hs'], b['HP']
         for t in range(T):
             o, n = int(pk.off[t]), int(pk.n[t])
@@ -632,7 +762,8 @@ class _UserRNN(_UserEncoder):
         for t in range(T - 1, -1, -1):
             o, n = int(pk.off[t]), int(pk.n[t])
             self._cell_bwd(b, pk, t, st)
-            if t:   # h_{-1} = 0 is a constant: no carry below step 0
+            # without the long-term table h_{-1} = 0 is a constant: no carry below step 0; with it the carry leaves dL/dh_0 in carry[:n0]
+            if t or self._lt is not None:
                 self._gemm(n, H, GH, (dP_hi[o:], dP_lo[o:]), 0, self.W_hl['hh'], 1, carry, H, accumulate=self._CARRY_ACCUMULATE)
         self._mark('backward_recurrence')
         g_hh, g_ih = self.grad[:self.nW], self.grad[self.nW:]
@@ -684,16 +815,20 @@ class _UserRNN(_UserEncoder):
         self._steps(pk, emb, s, capture)
 
     def _steps(self, pk, emb, s, after=None):
-        """Run one packed batch from zero states, step by step: the input projection of the step's reads, the recurrent GEMM and the
-        cell, which updates s['h'] (and the cell's other states) in place.  after(t), if given, runs after step t."""
+        """Run one packed batch from zero states (h_0 = P[pk.users] with the long-term table), step by step: the input projection of
+        the step's reads, the recurrent GEMM and the cell, which updates s['h'] (and the cell's other states) in place.  after(t), if
+        given, runs after step t."""
         H, GH, st = self.dim, self.GATES * self.dim, _stream()
         it = _upload(pk.items, self.device)
         h_hi, h_lo = s['h_hl']
-        h_hi.zero_()
-        h_lo.zero_()
-        h_hi[:, H] = 1.0
+        if self._lt is None:
+            h_hi.zero_()
+            h_lo.zero_()
+            h_hi[:, H] = 1.0
         for k in self._STATES:
             s[k][:pk.B].zero_()
+        if self._lt is not None:
+            self._initial_states(_upload(self._table_rows(pk.users), self.device), pk.B, h_hi, h_lo, s['h'], st)
         X_hi, X_lo = s['X_hl']
         for t in range(len(pk.n)):
             o, n = int(pk.off[t]), int(pk.n[t])
@@ -721,7 +856,7 @@ class UserGRU(_UserRNN):
         H, o, n = self.dim, int(pk.off[t]), int(pk.n[t])
         Hs, XP, HP, G = b['Hs'], b['XP'], b['HP'], b['gates']
         Hp_hi, Hp_lo = b['Hp_hl']
-        hprev = Hs[int(pk.off[t - 1]):].data_ptr() if t else None
+        hprev = Hs[int(pk.off[t - 1]):].data_ptr() if t else self._h0(b)
         nx = int(pk.off[t + 1])
         call('dae_gru_cell_fwd', n, H, XP[o:].data_ptr(), 3 * H, HP.data_ptr(), 3 * H, hprev, H, Hs[o:].data_ptr(), H, n_next,
              Hp_hi[nx:].data_ptr() if n_next else None, Hp_lo[nx:].data_ptr() if n_next else None, self.ldx, G[o:].data_ptr(),
@@ -731,7 +866,7 @@ class UserGRU(_UserRNN):
         H, o, n = self.dim, int(pk.off[t]), int(pk.n[t])
         Hs, dH, G, carry = b['Hs'], b['dH'], b['gates'], b['carry']
         (dX_hi, dX_lo), (dP_hi, dP_lo) = b['dXP_hl'], b['dHP_hl']
-        hprev = Hs[int(pk.off[t - 1]):].data_ptr() if t else None
+        hprev = Hs[int(pk.off[t - 1]):].data_ptr() if t else self._h0(b)
         call('dae_gru_cell_bwd', n, H, dH[o:].data_ptr(), H, carry.data_ptr(), H, G[o:].data_ptr(), 4 * H, hprev, H,
              dX_hi[o:].data_ptr(), dX_lo[o:].data_ptr(), dP_hi[o:].data_ptr(), dP_lo[o:].data_ptr(), self.ldg, st)
 
@@ -747,7 +882,7 @@ class UserGRU(_UserRNN):
 
 class UserLSTM(_UserRNN):
     """LSTM user encoder over reading sequences (DESIGN 4.15): torch.nn.LSTM(H, H)'s cell (one layer, bias, no projection, gate
-    order i, f, g, o), h_0 = c_0 = 0; the user vector is h after the last (truncated) read.  Everything else -- the constructor,
+    order i, f, g, o), h_0 = c_0 = 0 (h_0 = P[u] with the long-term table); the user vector is h after the last (truncated) read.  Everything else -- the constructor,
     the losses and negatives, fit, transform, impression_states, recommend, save / load -- is UserGRU's; theta =
     [W~_hh (4H x (H+1)) | W~_ih (4H x (H+1))].
 

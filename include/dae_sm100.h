@@ -662,6 +662,16 @@ int dae_lstm_cell_bwd(int32_t n, int32_t H, const float* dh_in, int64_t ld_dh_in
                       float* carry_c, int64_t ld_carry_c, const float* gates, int64_t ld_gates, const float* c, int64_t ld_c,
                       const float* c_prev, int64_t ld_cprev, void* da_hi, void* da_lo, int64_t ld_da, void* stream);
 
+/* ---- long-term user vectors (LSTUR-ini, DESIGN 4.18) -------------------------------------------------------------------------
+ * dae_rows_optimizer_step: the row-sparse (lazy) optimizer step of a table [rows x ld] (columns [0, cols) used).  For each i < n
+ *   with rows[i] >= 0, row rows[i] of table, slot1 and slot2 (laid out as the table) is updated from grad row i ([n x ld_grad]) by
+ *   dae_optimizer_step's rules (grad_scale 1); rows not listed and their slots are not touched.  counts (int32, one per table row;
+ *   required for adam, optional otherwise) is incremented for each updated row, and Adam's bias correction uses the incremented
+ *   count as its step.  The listed rows must be distinct (no atomics; the result is deterministic).
+ */
+int dae_rows_optimizer_step(float* table, int64_t ld, int32_t cols, const int32_t* rows, int32_t n, const float* grad, int64_t ld_grad,
+                            float* slot1, float* slot2, int32_t* counts, int32_t opt, float lr, float momentum, void* stream);
+
 /* ---- attention user encoder over reading sequences (DESIGN 4.17) -----------------------------------------------------------
  * NRMS's user encoder made causal, in the packed layout above: batch user i (of B) has lens[i] reads (int32, device), read t at
  * position off[t] + i (off: int64 [T + 1], device; lens[i] <= T <= 1024 must hold, the kernels trust it).  H = heads x d with head

@@ -115,6 +115,14 @@ def build_parser():
                          'columns per head (default: its largest divisor <= 20)')
     ap.add_argument('--user_attention_dim', type=int, default=None,
                     help='with --user_cell attention: width of the additive pooling layer (default 200)')
+    ap.add_argument('--user_long_term', action='store_true', default=False,
+                    help='with --user_sequences and --user_cell gru or lstm: learn a long-term vector per user (one row per sequence '
+                         'row) and start each user\'s window of recent reads from it (LSTUR-ini, DESIGN 4.18)')
+    ap.add_argument('--user_long_term_mask', type=float, default=None,
+                    help='with --user_long_term: the probability that a training batch user starts from 0 instead (default 0.5)')
+    ap.add_argument('--user_long_term_lr', type=float, default=None,
+                    help='with --user_long_term: the learning rate of the long-term vectors (default '
+                         'user_model.LONG_TERM_LEARNING_RATE)')
     ap.add_argument('--user_impressions', default='',
                     help='with --user_sequences: an .npz impression log (user, time, indptr, items, clicked; see '
                          'user_model.check_impressions) to train the GRU on instead of random negatives')
@@ -198,6 +206,13 @@ def check_flags(F):
     for flag, v in (('--user_heads', F.user_heads), ('--user_attention_dim', F.user_attention_dim)):
         assert v is None or F.user_cell == 'attention', '%s needs --user_cell attention' % flag
     assert F.user_heads is None or F.user_heads >= 1, '--user_heads must be >= 1'
+    assert not F.user_long_term or F.user_sequences, '--user_long_term needs --user_sequences'
+    assert not F.user_long_term or F.user_cell in ('gru', 'lstm'), '--user_long_term needs --user_cell gru or lstm'
+    for flag, v in (('--user_long_term_mask', F.user_long_term_mask), ('--user_long_term_lr', F.user_long_term_lr)):
+        assert v is None or F.user_long_term, '%s needs --user_long_term' % flag
+    F.user_long_term_mask = 0.5 if F.user_long_term_mask is None else F.user_long_term_mask
+    assert 0.0 <= F.user_long_term_mask <= 1.0, '--user_long_term_mask must lie in [0, 1]'
+    assert F.user_long_term_lr is None or F.user_long_term_lr > 0, '--user_long_term_lr must be > 0'
     F.user_attention_dim = 200 if F.user_attention_dim is None else F.user_attention_dim
     assert F.user_attention_dim >= 1, '--user_attention_dim must be >= 1'
     F.user_negatives = 4 if F.user_negatives is None else F.user_negatives
@@ -538,6 +553,8 @@ def recommend_users_sequences(F, model, enc, seqs, impressions=(None, None)):
     print('train a %s user encoder on %d users (%d reads, %d epochs%s)' % (label, len(indptr) - 1, items.size, F.user_epochs,
                                                                          ', impressions' if train_imp is not None else ''))
     kw = dict(heads=F.user_heads, attention_dim=F.user_attention_dim) if cell == 'attention' else {}
+    if F.user_long_term:
+        kw.update(long_term_users=len(indptr) - 1, long_term_mask=F.user_long_term_mask, long_term_learning_rate=F.user_long_term_lr)
     enc_cls = {'gru': UserGRU, 'lstm': UserLSTM, 'attention': UserAttention}[cell]
     rnn = enc_cls(enc.shape[1], num_epochs=F.user_epochs, seed=max(F.seed, 0), impression_loss=F.user_impression_loss,
                   impression_negatives=F.user_negatives, **kw)
