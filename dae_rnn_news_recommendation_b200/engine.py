@@ -34,6 +34,23 @@ def canonical_csr(x):
     return m
 
 
+def canonical_values(x, values, m):
+    """values: one value per stored entry of x, in x's own entry order (the storage order of a CSR / CSC / COO matrix, the row-major
+    nonzeros of an ndarray) -> those values in the entry order of m = canonical_csr(x), summed where x holds duplicate entries as m's
+    values are: the corrupted copy of a batch lands on the columns of the clean entries it was drawn from."""
+    v = np.asarray(values, dtype=np.float32).reshape(-1)
+    if sp.issparse(x) and x.format == 'csr' and x.has_canonical_format:
+        if v.size != m.nnz:
+            raise ValueError('x_corr_values: %d values for %d stored entries' % (v.size, m.nnz))
+        return v
+    c = sp.coo_matrix(x)
+    if v.size != c.nnz:
+        raise ValueError('x_corr_values: %d values for %d stored entries' % (v.size, c.nnz))
+    mc = canonical_csr(sp.coo_matrix((v, (c.row, c.col)), shape=c.shape))
+    assert np.array_equal(mc.indptr, m.indptr) and np.array_equal(mc.indices, m.indices)
+    return mc.data
+
+
 class DeviceCSR:
     """CSR matrix resident in HBM: indptr int64[N+1], indices int32[nnz], values fp32[nnz]."""
 
@@ -62,7 +79,8 @@ class HostFeed:
     autoencoder/autoencoder.py:228): [indptr int64 | indices int32 | values f32 | corrupted values f32 | labels f32]."""
 
     def __init__(self, x_batch, x_corr_values, labels, cap_nnz=None):
-        """cap_nnz: lay the buffer out for up to cap_nnz stored entries, so that every feed of a run has the SAME device
+        """x_corr_values: the corrupted values, one per stored entry of x_batch in its own entry order (canonical_values), or None (the
+        clean values).  cap_nnz: lay the buffer out for up to cap_nnz stored entries, so that every feed of a run has the SAME device
         layout and the step can be replayed from one captured CUDA graph."""
         m = canonical_csr(x_batch)
         B, real_nnz = m.shape[0], int(m.nnz)
@@ -84,7 +102,7 @@ class HostFeed:
         hb[self.off_indptr:self.off_indptr + 8 * (B + 1)] = m.indptr.astype(np.int64).view(np.uint8)
         hb[self.off_indices:self.off_indices + 4 * real_nnz] = m.indices.astype(np.int32).view(np.uint8)
         hb[self.off_values:self.off_values + 4 * real_nnz] = m.data.astype(np.float32).view(np.uint8)
-        xc = m.data if x_corr_values is None else x_corr_values
+        xc = m.data if x_corr_values is None else canonical_values(x_batch, x_corr_values, m)
         hb[self.off_values_c:self.off_values_c + 4 * real_nnz] = np.asarray(xc, dtype=np.float32).view(np.uint8)
         lab = np.zeros(B, np.float32) if labels is None else np.asarray(labels, dtype=np.float32).reshape(-1)
         hb[self.off_labels:self.off_labels + 4 * B] = lab.view(np.uint8)
@@ -252,6 +270,7 @@ class TrainEngine:
     def run_feed(self, feed, stats_log_row=None):
         """H2D copy of one packed pinned HostFeed, one training step on it, D2H read of the step's scalars.
         Feeds built with a common `cap_nnz` share one device layout: the step is then captured once and replayed."""
+        self._check_feed(feed)
         if self._feed_dev is None or self._feed_dev.numel() < feed.nbytes:
             self._feed_dev = torch.empty(max(feed.nbytes, 1 << 20), dtype=torch.uint8, device=self.device)
             self._feed_graph = None
@@ -285,6 +304,14 @@ class TrainEngine:
         s = self._stats_host.numpy()
         return {k: float(s[i]) for k, i in STAT.items()}
 
+    def _check_feed(self, feed):
+        """Refuse a feed this engine's step cannot train on, before any device work."""
+        if self.strategy in (1, 2) and not feed.has_labels:
+            raise ValueError('triplet strategy %s mines the batch by its labels: this feed has none'
+                             % next(k for k, v in _cabi.STRATEGY.items() if v == self.strategy))
+        if self.strategy == 3 and feed.B % 3 != 0:
+            raise ValueError('explicit triplets: the feed holds stacked [org; pos; neg] rows, a multiple of 3 (got %d rows)' % feed.B)
+
     def _feed_bind(self, feed, buf=None):
         """Point the engine's batch views (CSR, corrupted values, labels) at the feed layout inside `buf` (default: run_feed's buffer)."""
         d, B, nnz = (self._feed_dev if buf is None else buf), feed.B, feed.nnz
@@ -306,6 +333,7 @@ class TrainEngine:
         f0 = feeds[0]
         assert all(f.cap_nnz is not None and (f.B, f.nnz, f.has_labels, f.F, f.nbytes) == (f0.B, f0.nnz, f0.has_labels, f0.F, f0.nbytes)
                    for f in feeds), 'run_feeds needs feeds of one common layout (HostFeed(..., cap_nnz=...))'
+        self._check_feed(f0)
         key = (f0.B, f0.nnz, f0.has_labels, f0.F)
         out = []
         if not (self._feed_graph is not None and self._feed_graph[0] == key and self._feed_dev.numel() >= f0.nbytes):
@@ -1053,6 +1081,8 @@ class TrainEngine:
                 self._allreduce_grad()
             gscale = 1.0 / self.world
         self.step_count += 1
+        if getattr(self, '_ctl', None) is None:   # an eager step: the device step counter ctl[2] stays behind step_count, so the next
+            self._ctl_owner = None                 # run_feed replay re-synchronises it (Adam's bias correction reads it)
         tc = self.gemm_mode == 'tc'
         self._k('dae_optimizer_step', ptr(self.theta), ptr(self.grad), ptr(self.slot1), ptr(self.slot2), self.n_params,
                 self.opt, self.lr, self.momentum, gscale, self.step_count, ptr(getattr(self, '_ctl', None)),
