@@ -15,6 +15,9 @@ import torch
 from . import _cabi
 from ._cabi import call, ptr, STAT, STAT_SLOTS
 
+_BATCH_ALL, _BATCH_HARD, _EXPLICIT = (_cabi.STRATEGY[k] for k in ('batch_all', 'batch_hard', 'explicit'))
+_COSINE = _cabi.LOSS['cosine_proximity']
+
 
 def _stream():
     return torch.cuda.current_stream().cuda_stream
@@ -190,16 +193,14 @@ class TrainEngine:
         self.stats = torch.zeros(STAT_SLOTS, dtype=torch.float64, device=self.device)
         self._ws_B = 0
         self._w_split_valid = False
-        self._graph = None
-        # dense contractions: 'tc' = wgmma bf16x3 kernels (production), 'ffma' = fp32 CUDA-core validation kernels
+        # dense contractions: 'tc' = wgmma bf16x3 kernels (production), 'ffma' = fp32 CUDA-core validation kernels.  The two small
+        # contractions of the mining branch (S = E.E^T, dE2 = alpha (G + G^T) E; 0.64 GFLOP each) follow it: on the tensor cores the
+        # fp32 CUDA-core kernel would co-reside with the persistent tensor-core CTAs (17 KB of shared memory) but is several times
+        # slower on these shapes
         self.gemm_mode = gemm or os.environ.get('DAE_GEMM', 'tc')
         assert self.gemm_mode in ('tc', 'ffma')
-        # the two SMALL contractions of the mining branch (S = E.E^T, dE2 = alpha (G + G^T) E; 0.64 GFLOP each) also run on the tensor
-        # cores: the fp32 CUDA-core kernel would co-reside with the persistent tensor-core CTAs (17 KB of shared memory) but is several
-        # times slower on these shapes
-        self.small_gemm = self.gemm_mode
         if self.block_rows is not None:
-            assert self.gemm_mode == self.small_gemm == 'tc', 'mining_block_rows needs the tensor-core path (gemm="tc")'
+            assert self.gemm_mode == 'tc', 'mining_block_rows needs the tensor-core path (gemm="tc")'
         # the batch preparation exports of this engine: the block-mined one accepts batches above MAX_TRIPLET_BATCH
         self._prepare = 'dae_batch_prepare' if self.block_rows is None else 'dae_batch_prepare_blocked'
         self._prepare_next = 'dae_batch_prepare_next' if self.block_rows is None else 'dae_batch_prepare_next_blocked'
@@ -217,12 +218,32 @@ class TrainEngine:
         self.in_scale = 1.0  # decay noise folds into the encode kernels (utils.decay_noise, autoencoder/utils.py:147-159)
         self.launches = 0  # kernels launched by this engine (bench.py reports it)
         self.timed = None  # {kernel name: [(start_event, end_event), ...]} when per-kernel timing is on
+        # the data binding (set_data, corrupt_*, _feed_bind)
+        self.csr = self.csr_c = self.values_c = self.labels = None
+        # per-batch workspaces, sized by _ensure_ws for _ws_B rows (S, G and the GG pair: mining strategies; the bf16 operands and
+        # tile_ptr: tensor-core path; gemm_ws, loss_parts, loss_slots: deterministic mode)
+        self.E = self.dE = self.dE2 = self.row_loss = self.weight = self.rows = self.labels_b = self.seg_lo = self.seg_hi = None
+        if self.loss == _COSINE or self.gemm_mode != 'tc':   # the other engines never hold Z = E.W^T (F floats per batch row)
+            self.Z = None
+        self._stage = self.S = self.G = self.GG_hi = self.GG_lo = None
+        self.E_hi = self.E_lo = self.dZ_hi = self.dZ_lo = self.tile_ptr = self.W_hi = self.W_lo = None
+        self.Bp = self.n_loss_parts = 0
+        self.gemm_ws = self.loss_parts = self.loss_slots = None
+        # scratch of the encode backward (_ensure_bucket_scratch), the salt-and-pepper buffers, the SM count
+        self.col_count = self.col_start = self.col_cursor = self.ent_col = self.ent_row = self.ent_val = self.enc_det_ws = None
+        self._sp = self._sms = None
+        # graph replay: the fit's step graph (+ the optimizer graph of the 'nccl' exchange) and what it was captured on, the device
+        # cursors ctl and the step's view of them (_ctl: ctl when the running step is captured, else None), the host feeds' graphs
+        self._graph = self._graph2 = self._graph_meta = None
+        self.graph_launches = None
+        self.ctl = self._ctl = None
+        self._ctl_owner = None
+        self._ctl_host, self._ctl_host_i = None, 0
         self._feed_dev = None
         self._feed_graph = None
         self._feed_stream = None
         self._labels_next = None
-        self._graph2 = None
-        self._ctl_owner = None
+        self._mm = None   # the multimem exchange's symmetric-memory handles
         self._stats_host = torch.empty(STAT_SLOTS, dtype=torch.float64).pin_memory()
         # gradient exchange of the data-parallel step: 'multimem' = in-switch reduction by dae_allreduce_multimem (a plain kernel,
         # captured inside the step's graph; needs NVSwitch multicast); 'nccl_graph' = the NCCL all-reduce captured inside the step's
@@ -239,11 +260,16 @@ class TrainEngine:
             flag = torch.tensor([ok], dtype=torch.int32, device=self.device)
             torch.distributed.all_reduce(flag, op=torch.distributed.ReduceOp.MIN, group=self.pg)   # all ranks take the same path
             self.allreduce_mode = 'multimem' if int(flag.item()) == 1 else 'nccl_graph'
-            if self.allreduce_mode != 'multimem' and hasattr(self, '_mm'):
-                del self._mm
+            if self.allreduce_mode != 'multimem' and self._mm is not None:
+                self._mm = None
                 self.grad = torch.zeros(n, **f32)
         elif self.allreduce_mode == 'multimem':
             self._setup_multimem()
+
+    @property
+    def _mines(self):
+        """batch_all / batch_hard: the step mines its triplets from the batch's labels."""
+        return self.strategy in (_BATCH_ALL, _BATCH_HARD)
 
     # ---- kernel launch plumbing --------------------------------------------------------------------------------------
     def time_kernels(self, names):
@@ -276,29 +302,21 @@ class TrainEngine:
             self._feed_graph = None
         d = self._feed_dev
         d[:feed.nbytes].copy_(feed.host, non_blocking=True)
-        B, nnz = feed.B, feed.nnz
-        key = (B, nnz, feed.has_labels, feed.F)
+        key = (feed.B, feed.nnz, feed.has_labels, feed.F)
+        B, explicit_n = self._feed_batch(feed.B)
         fixed = feed.cap_nnz is not None and os.environ.get('DAE_CUDA_GRAPH', '1') == '1'
         if not (fixed and self._feed_graph is not None and self._feed_graph[0] == key):
             self._feed_bind(feed)
             if fixed:   # capture the step on this layout (restores the parameters after its warm-up steps)
-                saved = (self._graph, self._graph2, getattr(self, '_graph_meta', None))
-                if self.strategy == 3:   # explicit triplets: the feed holds the stacked [org; pos; neg] rows of the batch
-                    g = self.capture_step_graph(None, B // 3, None, row_stride=0, staged=False, explicit_n=B // 3)
-                else:
-                    g = self.capture_step_graph(None, B, None, row_stride=0, staged=False)
-                self._feed_graph = (key, g, self._graph2)
-                self._graph, self._graph2, self._graph_meta = saved
+                self._feed_graph = (key, *self._capture(None, B, None, 0, None, explicit_n))
                 self._ctl_owner = None
         if fixed:
             if self._ctl_owner != 'feed':   # cursors: offset 0 / log row 0 never move (stride 0); the optimizer step advances on the device
                 self.ctl.copy_(torch.tensor([0, 0, self.step_count + 1, 0], dtype=torch.int64))
                 self._ctl_owner = 'feed'
             self._replay(self._feed_graph[1], self._feed_graph[2])
-        elif self.strategy == 3:
-            self.step_explicit(None, 0, B // 3, B // 3, stats_log_row)
         else:
-            self.step(None, 0, B, stats_log_row)
+            self._step(None, 0, B, stats_log_row, explicit_n=explicit_n)
         self._stats_host.copy_(self.stats, non_blocking=True)
         torch.cuda.current_stream().synchronize()
         s = self._stats_host.numpy()
@@ -306,11 +324,15 @@ class TrainEngine:
 
     def _check_feed(self, feed):
         """Refuse a feed this engine's step cannot train on, before any device work."""
-        if self.strategy in (1, 2) and not feed.has_labels:
+        if self._mines and not feed.has_labels:
             raise ValueError('triplet strategy %s mines the batch by its labels: this feed has none'
                              % next(k for k, v in _cabi.STRATEGY.items() if v == self.strategy))
-        if self.strategy == 3 and feed.B % 3 != 0:
+        if self.strategy == _EXPLICIT and feed.B % 3 != 0:
             raise ValueError('explicit triplets: the feed holds stacked [org; pos; neg] rows, a multiple of 3 (got %d rows)' % feed.B)
+
+    def _feed_batch(self, rows):
+        """(B, explicit_n) of the step on a feed of `rows` rows: explicit triplets stack [org; pos; neg], rows / 3 of each."""
+        return (rows // 3, rows // 3) if self.strategy == _EXPLICIT else (rows, None)
 
     def _feed_bind(self, feed, buf=None):
         """Point the engine's batch views (CSR, corrupted values, labels) at the feed layout inside `buf` (default: run_feed's buffer)."""
@@ -356,28 +378,24 @@ class TrainEngine:
         # ~20 us) on a side branch from the labels inside buffer (k+1) % 3, and starts with the copy-out dae_batch_commit.
         NS = 3
         B, nb = f0.B, f0.nbytes
-        staged = self.strategy in (1, 2) and f0.has_labels
+        staged = self._mines          # (mined feeds carry labels: _check_feed)
         st = self._feed_stream
         if st is None or st['owner'] is not self._feed_graph:
             bufs = [torch.empty(self._feed_dev.numel(), dtype=torch.uint8, device=self.device) for _ in range(NS)]
             for bk in bufs:
                 bk[:nb].copy_(self._feed_dev[:nb])       # a valid batch of this layout for the captures' warm-up steps
             log = torch.zeros(LOG_ROWS, STAT_SLOTS, dtype=torch.float64, device=self.device)
-            saved = (self._graph, self._graph2, getattr(self, '_graph_meta', None))
             graphs = []
+            step_B, explicit_n = self._feed_batch(B)
             try:
                 for k in range(NS):
                     self._feed_bind(f0, bufs[k])
                     if staged:
                         self._labels_next = bufs[(k + 1) % NS][f0.off_labels:f0.off_labels + 4 * B].view(torch.float32)
-                    if self.strategy == 3:
-                        g = self.capture_step_graph(None, B // 3, log, row_stride=0, staged=False, explicit_n=B // 3)
-                    else:
-                        g = self.capture_step_graph(None, B, log, row_stride=0, staged='feed' if staged else False)
-                    graphs.append((g, self._graph2))
+                    # staged: the next batch comes from rows 0..B-1 (stride 0) of the next feed, its labels from self._labels_next
+                    graphs.append(self._capture(None, step_B, log, 0, (B, 0) if staged else None, explicit_n))
             finally:
                 self._labels_next = None
-                self._graph, self._graph2, self._graph_meta = saved
                 self._feed_bind(f0)
             st = self._feed_stream = {'owner': self._feed_graph, 'bufs': bufs, 'log': log, 'graphs': graphs,
                                       'copy_stream': torch.cuda.Stream(device=self.device),
@@ -457,17 +475,21 @@ class TrainEngine:
                 'dec_b': self.bv.cpu().numpy().copy()}
 
     # ---- workspaces ----------------------------------------------------------------------------------------------
+    def _drop_graphs(self):
+        """Buffers move: the captured step graphs (if any) are stale and must be re-captured."""
+        self._graph = self._graph2 = None
+        self._feed_graph = None
+
     def _ensure_ws(self, B):
         if B <= self._ws_B:
             return
-        self._graph = None  # buffers move: a captured step graph (if any) is stale and must be re-captured
-        self._feed_graph = None
+        self._drop_graphs()
         f32 = dict(dtype=torch.float32, device=self.device)
         i32 = dict(dtype=torch.int32, device=self.device)
         self.E = torch.empty(B, self.H, **f32)
         self.dE = torch.empty(B, self.H, **f32)
         self.dE2 = torch.empty(B, self.H, **f32)   # triplet part of dL/dE, alpha (G + G^T) E (written on the mining branch)
-        if self.loss == 2 or self.gemm_mode != 'tc':   # Z = E.W^T is only materialised by the cosine loss and the CUDA-core path
+        if self.loss == _COSINE or self.gemm_mode != 'tc':   # Z = E.W^T is only materialised by the cosine loss and the CUDA-core path
             self.Z = torch.empty(B, self.F, **f32)
         self.row_loss = torch.empty(B, **f32)
         self.weight = torch.empty(B, **f32)
@@ -480,7 +502,7 @@ class TrainEngine:
                        torch.zeros(STAT_SLOTS, dtype=torch.float64, device=self.device))
         # the mining's S / G (and their bf16 hi / lo pair below): B x B, or R anchor rows x B when mined in blocks
         mine_rows = B if self.block_rows is None else min(self.block_rows, B)
-        if self.strategy in (1, 2):
+        if self._mines:
             self.S = torch.empty(mine_rows, B, **f32)
             self.G = torch.empty(mine_rows, B, **f32)
         if self.gemm_mode == 'tc':
@@ -492,10 +514,10 @@ class TrainEngine:
             self.dZ_hi = torch.empty(B, self.Fp, **bf)
             self.dZ_lo = torch.empty(B, self.Fp, **bf)
             self.tile_ptr = torch.empty(B, 4 * ((self.F + 255) // 256) + 1, **i32)
-            if not hasattr(self, 'W_hi'):
+            if self.W_hi is None:
                 self.W_hi = torch.empty(self.F, self.Hp, **bf)
                 self.W_lo = torch.empty(self.F, self.Hp, **bf)
-            if self.strategy in (1, 2):
+            if self._mines:
                 self.GG_hi = torch.empty(mine_rows, self.Bp, **bf)
                 self.GG_lo = torch.empty(mine_rows, self.Bp, **bf)
         if self.deterministic:
@@ -512,24 +534,22 @@ class TrainEngine:
         """Scratch of dae_encode_csr_bwd_gather: per-column counts / offsets and the bucketed (row, value) entries."""
         c = self.csr_c
         cap = int(c.nnz) if c.max_row_nnz is None else int(min(c.nnz, B * max(c.max_row_nnz, 1)))
-        if not hasattr(self, 'col_count'):
+        if self.col_count is None:
             i32 = dict(dtype=torch.int32, device=self.device)
             self.col_count = torch.zeros(self.F, **i32)
             self.col_start = torch.zeros(self.F + 1, **i32)
             self.col_cursor = torch.zeros(self.F, **i32)
         if cap > self._ent_cap:
             cap = int(cap * 1.5) if c.max_row_nnz is None else cap   # per-step host feeds vary in size: grow geometrically
-            self._graph = None
-            self._feed_graph = None
+            self._drop_graphs()
             self.ent_col = torch.empty(cap, dtype=torch.int32, device=self.device)
             self.ent_row = torch.empty(cap, dtype=torch.int32, device=self.device)
             self.ent_val = torch.empty(cap, dtype=torch.float32, device=self.device)
             self._ent_cap = cap
         if self.enc_bwd_mode == 'det':
             need = _cabi.query('dae_encode_csr_bwd_det_workspace', B, self.F, self.H, self._ent_cap)
-            if getattr(self, 'enc_det_ws', None) is None or self.enc_det_ws.numel() < need:   # (laid out per call from B and the cap)
-                self._graph = None
-                self._feed_graph = None
+            if self.enc_det_ws is None or self.enc_det_ws.numel() < need:   # (laid out per call from B and the cap)
+                self._drop_graphs()
                 self.enc_det_ws = torch.empty(need, dtype=torch.uint8, device=self.device)
 
     # ---- data ----------------------------------------------------------------------------------------------------
@@ -559,9 +579,8 @@ class TrainEngine:
         (and v): a captured step graph reads every epoch's corruption at the same addresses.  Capacity sum_r min(F, nnz_r + v) entries
         (8 B each); max_row_nnz is the bound min(F, max_r nnz_r + v), so the step's scratch sized from it never grows between epochs."""
         c, F, v = self.csr, self.F, int(v)
-        sp_ = getattr(self, '_sp', None)
-        if sp_ is not None and sp_['csr'] is c and sp_['v'] == v:
-            return sp_
+        if self._sp is not None and self._sp['csr'] is c and self._sp['v'] == v:
+            return self._sp
         self._sp = None
         N = c.shape[0]
         cap = int(torch.clamp(c.indptr[1:] - c.indptr[:-1] + v, max=F).sum().item()) if N else 0
@@ -605,7 +624,7 @@ class TrainEngine:
     def check_corruption(self):
         """Raise if a salt-and-pepper call found its output beyond the buffers' capacity (it then leaves its rows empty; with the
         capacity of salt_pepper_buffers this cannot happen).  One 4-byte read: call it once per epoch."""
-        b = getattr(self, '_sp', None)
+        b = self._sp
         if b is not None and int(b['overflow'].item()) != 0:
             raise _cabi.DaeError('dae_salt_pepper_csr: corrupted CSR beyond its capacity of %d entries' % b['cap'])
 
@@ -633,7 +652,7 @@ class TrainEngine:
                 tag=tag)
 
     def _sm_count(self):
-        if getattr(self, '_sms', None) is None:
+        if self._sms is None:
             self._sms = torch.cuda.get_device_properties(self.device).multi_processor_count
         return self._sms
 
@@ -654,34 +673,48 @@ class TrainEngine:
         return self._sides[i]
 
     @staticmethod
+    def _record(stream):
+        ev = torch.cuda.Event()
+        ev.record(stream)
+        return ev
+
+    @staticmethod
     def _fork(src, dst):
         """dst waits for everything issued on src so far (an edge of the step's graph once captured)."""
-        ev = torch.cuda.Event()
-        ev.record(src)
-        dst.wait_event(ev)
+        dst.wait_event(TrainEngine._record(src))
 
     def step(self, perm, offset, B, stats_log_row=None, train=True, ctl=None, staged=None):
         """perm: int32 device tensor (epoch permutation) or None (identity); rows perm[offset:offset+B] form the batch.
         stats_log_row: optional float64[STAT_SLOTS] device view receiving this step's scalars.
         staged = (n_perm, stride): graph-replayed steps of the triplet strategies take their batch from the staging buffers
         (dae_batch_commit) and stage the batch at cursor + stride for the next replay on a side branch."""
-        F, H = self.F, self.H
-        self._ensure_ws(B)
-        strat = self.strategy
+        self._step(perm, offset, B, stats_log_row, train, ctl, staged)
+
+    def step_explicit(self, perm, offset, B, n_rows_each, stats_log_row=None, ctl=None):
+        """self.csr holds [org; pos; neg] stacked (3*n_rows_each rows). autoencoder_triplet.py:256-258,286-288,303-314."""
+        self._step(perm, offset, B, stats_log_row, ctl=ctl, explicit_n=n_rows_each)
+
+    def _step(self, perm, offset, B, stats_log_row, train=True, ctl=None, staged=None, explicit_n=None, defer_update=False):
+        """One step (train=False: its forward and scalars only) on the batch at `offset`.  explicit_n: the rows per block of the
+        stacked [org; pos; neg] set -- the step then runs on 3 B rows, B of each block.  defer_update: stop before the optimizer
+        (the 'nccl' exchange captures it into a graph of its own)."""
+        rows = B if explicit_n is None else 3 * B
+        self._ensure_ws(rows)
         self._ctl = ctl  # device int64[4] cursors (offset, log row, optimizer step) when the step is graph-captured
-        main = torch.cuda.current_stream()
-        st = main.cuda_stream
-        use_stage = staged is not None and strat in (1, 2) and train
-        if use_stage:
+        st = _stream()
+        stage_next = None
+        if explicit_n is not None:
+            self._k('dae_batch_prepare_explicit', ptr(perm), int(offset), ptr(ctl), B, int(explicit_n), ptr(self.rows), ptr(self.stats), st)
+        elif staged is not None and self._mines and train:
             self._k('dae_batch_commit', B, *[ptr(t) for t in self._stage], ptr(self.rows), ptr(self.labels_b), ptr(self.seg_lo),
                     ptr(self.seg_hi), ptr(self.weight), ptr(self.stats), st)
+            stage_next = (perm, staged)
         else:
-            self._k(self._prepare, ptr(perm), int(offset), ptr(ctl), B, ptr(self.labels), strat, ptr(self.rows), ptr(self.labels_b),
-                    ptr(self.seg_lo), ptr(self.seg_hi), ptr(self.weight), ptr(self.stats), st)
-        self._branch_b_prologue(B, train)
-        self._encode_forward(B, train)
-        self._train_tail(B, strat, self.weight if strat != 0 else None, stats_log_row, train,
-                         stage_next=(perm, staged) if use_stage else None)
+            self._k(self._prepare, ptr(perm), int(offset), ptr(ctl), B, ptr(self.labels), self.strategy, ptr(self.rows),
+                    ptr(self.labels_b), ptr(self.seg_lo), ptr(self.seg_hi), ptr(self.weight), ptr(self.stats), st)
+        prologue_b = self._branch_b_prologue(rows, train)
+        self._encode_forward(rows, train)
+        self._train_tail(rows, prologue_b, stats_log_row, train, stage_next, B if explicit_n is not None else 0, defer_update)
 
     def _stage_next_batch(self, perm, staged, B, stream):
         n_perm, stride = staged
@@ -699,24 +732,22 @@ class TrainEngine:
     def _branch_b_prologue(self, B, train):
         """Start of branch B, forked BEFORE K1: everything the later kernels need that depends on nothing but the batch's row ids --
         zero the gradient buffer (dense dW, sparse dW and dbh accumulate into it) and dE (its stream-K GEMM accumulates), and the
-        row-id part of the fused decode (row-loss zeroing, per-tile CSR offsets)."""
-        self._branch_b = (0, None)
+        row-id part of the fused decode (row-loss zeroing, per-tile CSR offsets).  Returns (decode prepared, the branch's event), or
+        None when the step has no branch B (CUDA-core path, forward only, or fork_branches off)."""
         if not (self.gemm_mode == 'tc' and train and self.fork_branches):
-            return
+            return None
         main, sideB = torch.cuda.current_stream(), self._side_stream(1)
         self._fork(main, sideB)
         prepared = 0
         with torch.cuda.stream(sideB):
-            if self.loss != 2:   # first on the branch: it becomes runnable together with K1 (whose 800 CTAs then fill the machine)
+            if self.loss != _COSINE:   # first on the branch: it becomes runnable together with K1 (whose 800 CTAs then fill the machine)
                 c = self.csr
                 self._k('dae_decode_prepare', B, self.F, ptr(c.indptr), ptr(c.indices), ptr(self.rows), ptr(self.row_loss),
                         ptr(self.tile_ptr), sideB.cuda_stream)
                 prepared = 1
             self.grad.zero_()
             self.dE.zero_()
-            ev = torch.cuda.Event()
-            ev.record(sideB)
-        self._branch_b = (prepared, ev)
+            return prepared, self._record(sideB)
 
     def _encode_forward(self, B, train):
         """K1 on the batch rows; also emits E as the bf16 hi/lo pair (plus the all-ones column kept in E_hi) the tensor-core GEMMs
@@ -732,7 +763,7 @@ class TrainEngine:
         if tc:
             self._ensure_w_split()
 
-    def _train_tail(self, B, strat, weight, stats_log_row, train, stage_next=None, explicit_B=0):
+    def _train_tail(self, B, prologue_b, stats_log_row, train, stage_next=None, explicit_B=0, defer_update=False):
         """Everything after the encode forward.  Dependencies of the step (tensor-core path):
 
             batch -+-> K1 -+-> decode(+loss, dZ) -> dE = dZ.W ----------+-> encode backward (dA, dbh, sparse dW) -+-> exchange, optimizer
@@ -745,152 +776,153 @@ class TrainEngine:
         batch_all's mining needs only E (its data weights are closed-form) and runs as branch A next to the decode chain; the
         dense dW GEMM only meets the sparse dW of the encode backward in the (zeroed) gradient buffer, where both accumulate, so it
         runs as branch B next to the latency-bound encode-backward kernels.  batch_hard's weights come out of the mining kernel,
-        so there the mining stays in line.  Eagerly these are streams + events; captured, parallel branches of ONE graph."""
+        so there the mining stays in line.  Eagerly these are streams + events; captured, parallel branches of ONE graph.
+        prologue_b: what _branch_b_prologue returned.  stage_next: (perm, staged) of the batch the step stages for the next replay."""
         F, H = self.F, self.H
         main = torch.cuda.current_stream()
         tc = self.gemm_mode == 'tc'
+        mines = self._mines
+        weight = self.weight if mines else None
         gather = train and self.enc_bwd_mode == 'gather'
-        par = tc and train and self.fork_branches                   # branch B exists
-        fork = par and strat == 1                                   # branch A exists
-        rows = self.rows
-        sideA = self._side_stream(0) if (par or stage_next) else None
-        sideB = self._side_stream(1) if par else None
-        ev_mined, used_a = None, False
-        if fork:
-            used_a = True
+        branch_b = prologue_b is not None                  # branch B exists (tensor-core training with fork_branches)
+        branch_a = branch_b and self.strategy == _BATCH_ALL  # branch A exists: the mining runs on it
+        # dE2 = alpha (G + G^T) E has a GEMM of its own unless the block loop of _mining_blocked accumulated it; without branch A it
+        # goes on the side stream when branch B exists (batch_hard), in line otherwise
+        dE2_gemm = mines and tc and train and self.block_rows is None
+        dE2_side = dE2_gemm and branch_b and not branch_a
+        # the next batch is staged at the tail of branch A, else on a side branch of its own, forked before the decode
+        stage_fork = stage_next is not None and not branch_a
+        used_a = branch_a or dE2_side or stage_fork
+        # side stream A is created by the first step that forks, used or not: torch hands out its pooled CUDA streams in creation order
+        sideA = self._side_stream(0) if (branch_b or stage_next is not None) else None
+        sideB = self._side_stream(1) if branch_b else None
+        ev_mined = None
+        if branch_a:
             self._fork(main, sideA)
             with torch.cuda.stream(sideA):
-                self._mining(B, strat, tc, train)
-                self._dE_triplet(B, sideA)
-                ev_mined = torch.cuda.Event()
-                ev_mined.record(sideA)
-        elif strat in (1, 2):
-            self._mining(B, strat, tc, train)     # in line: batch_hard's data weights come out of the mining kernel
-            if self.block_rows is not None:       # (mined in blocks: each block's dE contribution is already in dE2)
-                pass
-            elif tc and train and par:            # ... but its dE contribution can still run next to the decode chain
-                used_a = True
+                self._mining(B, train)
+                if dE2_gemm:
+                    self._dE_triplet(B, sideA)
+                ev_mined = self._record(sideA)
+        elif mines:
+            self._mining(B, train)                # in line: batch_hard's data weights come out of the mining kernel
+            if dE2_side:                          # ... but its dE contribution can still run next to the decode chain
                 self._fork(main, sideA)
                 self._dE_triplet(B, sideA)
-                ev_mined = torch.cuda.Event()
-                ev_mined.record(sideA)
-            elif tc and train:
+                ev_mined = self._record(sideA)
+            elif dE2_gemm:
                 self._dE_triplet(B, main)
-        dec_prepared, ev_zero = 0, None
-        if par:
-            dec_prepared, ev_zero = self._branch_b
+        dec_prepared = 0
+        if branch_b:
+            dec_prepared, ev_zero = prologue_b
             main.wait_event(ev_zero)              # zeroed gradient / dE buffers (issued before K1)
             if gather:   # the column-bucket offsets of the backward gather only need K1's counts: branch B, far from any critical path
                 self._fork(main, sideB)
                 with torch.cuda.stream(sideB):
                     self._k('dae_col_scan', ptr(self.col_count), F, ptr(self.col_start), ptr(self.col_cursor), sideB.cuda_stream)
-                    self._scan_done = True
-                    ev_scan = torch.cuda.Event()
-                    ev_scan.record(sideB)
-        if stage_next is not None and not fork:   # (batch_hard) the staging buffers were consumed by dae_batch_commit: refill them now
-            used_a = True
+                    ev_scan = self._record(sideB)
+        if stage_fork:                            # the staging buffers were consumed by dae_batch_commit: refill them now
             self._fork(main, sideA)
             with torch.cuda.stream(sideA):
-                self._stage_next_batch(stage_next[0], stage_next[1], B, sideA)
-        if not tc:
-            self._decode_and_backward(B, rows, weight, train)
+                self._stage_next_batch(*stage_next, B, sideA)
+        if tc:
+            self._decode_tc(B, weight, train, prepared=dec_prepared)
         else:
-            self._decode_tc(B, rows, weight, train, prepared=dec_prepared)
+            self._decode_and_backward(B, weight, train)
         if not train:
             if explicit_B:   # forward only: the kernel's loss statistics are what is wanted, its dE contribution lands in scratch
                 self._triplet_explicit(explicit_B, main)
-            self._finalize(B, strat, weight, stats_log_row, main)
+            self._finalize(B, weight, stats_log_row, main)
             return
-        if fork:
+        if branch_a:
             # the step's scalars only need the decode row losses (main branch) and the mining statistics (branch A): reduce them on
             # branch A while the main one continues with the backward GEMMs / encode backward / optimizer
             self._fork(main, sideA)
             with torch.cuda.stream(sideA):
-                self._finalize(B, strat, weight, stats_log_row, sideA)
+                self._finalize(B, weight, stats_log_row, sideA)
         if tc:
             Whl, dZhl = (self.W_hi, self.W_lo), (self.dZ_hi, self.dZ_lo)
-            if not par:   # in line: the dense dW is stored first, the encode backward then adds its sparse part
+            if not branch_b:   # in line: the dense dW is stored first, the encode backward then adds its sparse part
                 self._dW_gemm(B, accumulate=0)
             # k_splits = -1: stream-K (the 28 tiles of dE / 316 tiles of dW do not fill the 132 SMs in whole waves); with branch B
             # the output was zeroed there, so the GEMM accumulates and needs no memset node of its own
             det = self.deterministic   # (deterministic: stored, the zeroing on branch B notwithstanding)
-            self._tc_gemm(B, H, F, 1.0, dZhl, 0, Whl, 1, self.dE, H, k_splits=-1, accumulate=1 if (par and not det) else 0,
+            self._tc_gemm(B, H, F, 1.0, dZhl, 0, Whl, 1, self.dE, H, k_splits=-1, accumulate=1 if (branch_b and not det) else 0,
                           tag='gemm_decode_dE', ws=self.gemm_ws[0] if det else None)
         if explicit_B:   # explicit (org, pos, neg) triplets: row-wise softplus(e.e- - e.e+), adds its dE (autoencoder_triplet.py:303-314)
             self._triplet_explicit(explicit_B, main)
-        if par:
+        if branch_b:
             self._fork(main, sideB)           # branch B: after the zeroing (already on sideB) and once dE owns the SMs; it needs
             with torch.cuda.stream(sideB):    # nothing from the mining branch, so it does not wait for it
                 self._dW_gemm(B, accumulate=1)
-        if strat in (1, 2):  # dE += alpha (G + G^T) E: on the tensor-core path the product already sits in dE2 (mining branch)
-            if ev_mined is not None:
-                main.wait_event(ev_mined)
-            if not tc:
-                self._gemm(B, H, B, self.alpha, self.G, B, 1, self.E, 1, H, 1.0, self.dE, H, tag='gemm_dE_tri')
-                self._gemm(B, H, B, self.alpha, self.G, 1, B, self.E, 1, H, 1.0, self.dE, H, tag='gemm_dE_tri')
-        if par and gather:
+        if ev_mined is not None:              # dE += alpha (G + G^T) E: on the tensor-core path the product already sits in dE2
+            main.wait_event(ev_mined)
+        if mines and not tc:
+            self._gemm(B, H, B, self.alpha, self.G, B, 1, self.E, 1, H, 1.0, self.dE, H, tag='gemm_dE_tri')
+            self._gemm(B, H, B, self.alpha, self.G, 1, B, self.E, 1, H, 1.0, self.dE, H, tag='gemm_dE_tri')
+        if branch_b and gather:
             main.wait_event(ev_scan)
-        self._encode_backward(B, rows, dE_add=self.dE2 if (tc and strat in (1, 2)) else None, dbh_zeroed=1 if par else 0)
-        if not fork:
-            self._finalize(B, strat, weight, stats_log_row, main)
+        self._encode_backward(B, dE_add=self.dE2 if (tc and mines) else None, dbh_zeroed=1 if branch_b else 0,
+                              scan_done=branch_b and gather)
+        if not branch_a:
+            self._finalize(B, weight, stats_log_row, main)
         elif stage_next is not None:          # tail of branch A, after the step's scalars
             with torch.cuda.stream(sideA):
-                self._stage_next_batch(stage_next[0], stage_next[1], B, sideA)
-        if par:
+                self._stage_next_batch(*stage_next, B, sideA)
+        if branch_b:
             self._fork(sideB, main)           # the dense dW / dbv are in the gradient buffer
         if self.enc_bwd_mode == 'det':        # deterministic: the sparse dW joins the stored dense dW in one fixed-order add
             self._k('dae_encode_sparse_dw_add', B, F, H, self._ent_cap, ptr(self.enc_det_ws), self.enc_det_ws.numel(), ptr(self._gW()),
                     main.cuda_stream)
-        if getattr(self, '_defer_update', False):
-            if used_a:
-                self._fork(sideA, main)
-            return
         # branch A's tail (the step's scalars, the NEXT batch's staging: a 1-CTA sort that only gets an SM once a GEMM CTA retires)
         # does not feed the update: it joins after the optimizer, before the cursors advance / the next step reuses `stats`
-        self._apply_update()
+        if not defer_update:
+            self._apply_update()
         if used_a:
             self._fork(sideA, main)
 
+    def _triplet(self, name, *args, stream, anchors=0, n_launch=1):
+        """The triplet-loss export `name`.  Deterministic: its `_det` twin, which leaves one fp64 loss per anchor in loss_slots, then
+        (anchors > 0) dae_triplet_loss_sum adds the first `anchors` slots to the statistics in anchor order."""
+        if not self.deterministic:
+            self._k(name, *args, stream, n_launch=n_launch)
+            return
+        self._k(name + '_det', *args, ptr(self.loss_slots), stream, n_launch=n_launch)
+        self._sum_loss_slots(anchors, stream)
+
+    def _sum_loss_slots(self, anchors, stream):
+        if self.deterministic and anchors:
+            self._k('dae_triplet_loss_sum', ptr(self.loss_slots), anchors, ptr(self.stats), stream)
+
     def _triplet_explicit(self, Bx, stream):
         E, d, H = self.E, self.dE, self.H
-        args = (ptr(E[0:Bx]), ptr(E[Bx:2 * Bx]), ptr(E[2 * Bx:3 * Bx]), Bx, H, H, self.alpha, ptr(d[0:Bx]), ptr(d[Bx:2 * Bx]),
-                ptr(d[2 * Bx:3 * Bx]), ptr(self.stats))
-        if self.deterministic:
-            self._k('dae_triplet_explicit_det', *args, ptr(self.loss_slots), stream.cuda_stream)
-            self._k('dae_triplet_loss_sum', ptr(self.loss_slots), Bx, ptr(self.stats), stream.cuda_stream)
-        else:
-            self._k('dae_triplet_explicit', *args, stream.cuda_stream)
+        self._triplet('dae_triplet_explicit', ptr(E[0:Bx]), ptr(E[Bx:2 * Bx]), ptr(E[2 * Bx:3 * Bx]), Bx, H, H, self.alpha, ptr(d[0:Bx]),
+                      ptr(d[Bx:2 * Bx]), ptr(d[2 * Bx:3 * Bx]), ptr(self.stats), stream=stream.cuda_stream, anchors=Bx)
 
     def _dE_triplet(self, B, stream):
         """dE2 = alpha (G + G^T) E, the triplet part of dL/dE; the encode backward adds it to the decode part (dE_add)."""
-        if self.block_rows is not None:    # the block loop of _mining_blocked accumulated it block by block
-            return
+        st = stream.cuda_stream
         with torch.cuda.stream(stream):
-            if self.small_gemm == 'tc' and self.strategy == 1 and self.deterministic:
-                ws = self.gemm_ws[2]
-                self._k('dae_gemm_sym_bf16x3_det', B, self.H, float(self.alpha), ptr(self.GG_hi), ptr(self.GG_lo), self.GG_hi.stride(0),
-                        ptr(self.E_hi), ptr(self.E_lo), self.E_hi.stride(0), ptr(self.dE2), self.H, 0, ptr(ws), ws.numel(),
-                        stream.cuda_stream, n_launch=2, tag='gemm_dE_tri')
-            elif self.small_gemm == 'tc' and self.strategy == 1:
+            if self.strategy == _BATCH_ALL:
                 # batch_all: the sweep wrote G as bf16 hi / lo; ONE GEMM walks G's columns and then its rows: alpha (G + G^T) E
-                self._k('dae_gemm_sym_bf16x3', B, self.H, float(self.alpha), ptr(self.GG_hi), ptr(self.GG_lo), self.GG_hi.stride(0),
-                        ptr(self.E_hi), ptr(self.E_lo), self.E_hi.stride(0), ptr(self.dE2), self.H, 0, stream.cuda_stream, tag='gemm_dE_tri')
-            elif self.small_gemm == 'tc':
-                self._k('dae_sym_split_bf16', ptr(self.G), B, B, self.alpha, ptr(self.GG_hi), ptr(self.GG_lo), self.GG_hi.stride(0),
-                        stream.cuda_stream)
+                args = (B, self.H, float(self.alpha), ptr(self.GG_hi), ptr(self.GG_lo), self.GG_hi.stride(0), ptr(self.E_hi),
+                        ptr(self.E_lo), self.E_hi.stride(0), ptr(self.dE2), self.H, 0)
+                if self.deterministic:
+                    ws = self.gemm_ws[2]
+                    self._k('dae_gemm_sym_bf16x3_det', *args, ptr(ws), ws.numel(), st, n_launch=2, tag='gemm_dE_tri')
+                else:
+                    self._k('dae_gemm_sym_bf16x3', *args, st, tag='gemm_dE_tri')
+            else:
+                self._k('dae_sym_split_bf16', ptr(self.G), B, B, self.alpha, ptr(self.GG_hi), ptr(self.GG_lo), self.GG_hi.stride(0), st)
                 self._tc_gemm(B, self.H, B, 1.0, (self.GG_hi, self.GG_lo), 0, (self.E_hi, self.E_lo), 1, self.dE2, self.H, tag='gemm_dE_tri')
-            else:   # G.E, then G^T.E on top (the transpose is a stride swap)
-                H = self.H
-                self._gemm(B, H, B, self.alpha, self.G, B, 1, self.E, 1, H, 0.0, self.dE2, H, tag='gemm_dE_tri')
-                self._gemm(B, H, B, self.alpha, self.G, 1, B, self.E, 1, H, 1.0, self.dE2, H, tag='gemm_dE_tri')
 
-    def _finalize(self, B, strat, weight, stats_log_row, stream):
-        if self.deterministic and self.loss != 2:
+    def _finalize(self, B, weight, stats_log_row, stream):
+        if self.deterministic and self.loss != _COSINE:
             # the fused decode's per-(half tile, row) partials, summed in part order by one thread per row (the finalize's parts path does
             # the same sums on ONE CTA: 4-5x slower at B = 800)
             self._k('dae_reduce_parts', ptr(self.loss_parts), self.n_loss_parts, B, ptr(self.row_loss), stream.cuda_stream)
-        self._k('dae_step_finalize', ptr(self.row_loss), None, 0, ptr(weight), B, strat, self.alpha, ptr(self.stats),
-                ptr(stats_log_row), ptr(getattr(self, '_ctl', None)), stream.cuda_stream)
+        self._k('dae_step_finalize', ptr(self.row_loss), None, 0, ptr(weight), B, self.strategy, self.alpha, ptr(self.stats),
+                ptr(stats_log_row), ptr(self._ctl), stream.cuda_stream)
 
     def _dW_gemm(self, B, accumulate):
         """[dW_dec | dbv] = dZ^T . [E | 1]  (F x (H+1): the all-ones column of E_hl delivers dbv)."""
@@ -899,31 +931,28 @@ class TrainEngine:
                       n_store=self.H, special_col=self.H, special_out=self._gbv(), k_splits=-1, accumulate=0 if det else accumulate,
                       tag='gemm_decode_dW', ws=self.gemm_ws[1] if det else None)
 
-    def _mining(self, B, strat, tc, train=True):
+    def _mining(self, B, train=True):
         """S = E.E^T and the triplet kernel (loss, statistics, G = dL/dS; batch_hard: also the data weights)."""
         if self.block_rows is not None:
-            self._mining_blocked(B, strat, train)
+            self._mining_blocked(B, train)
             return
         H, st = self.H, _stream()
-        if tc and self.small_gemm == 'tc':
+        tc = self.gemm_mode == 'tc'
+        if tc:
             Ehl = (self.E_hi, self.E_lo)
             self._tc_gemm(B, B, H, 1.0, Ehl, 0, Ehl, 0, self.S, B, tag='gemm_gram')
         else:
             self._gemm(B, B, H, 1.0, self.E, H, 1, self.E, H, 1, 0.0, self.S, B, tag='gemm_gram')  # S = E.E^T
-        det = self.deterministic
-        slots = (ptr(self.loss_slots),) if det else ()   # deterministic: one loss slot per anchor, summed in anchor order below
-        if strat == 1:
+        if self.strategy == _BATCH_ALL:
             # G also leaves as the bf16 hi / lo pair the (G + G^T).E GEMM reads
-            self._k('dae_triplet_batch_all_det' if det else 'dae_triplet_batch_all', ptr(self.S), B, B, ptr(self.seg_lo), ptr(self.seg_hi),
-                    ptr(self.G), B, ptr(self.stats), 0, ptr(self.GG_hi) if tc else None, ptr(self.GG_lo) if tc else None,
-                    self.GG_hi.stride(0) if tc else 0, *slots, st)
+            self._triplet('dae_triplet_batch_all', ptr(self.S), B, B, ptr(self.seg_lo), ptr(self.seg_hi), ptr(self.G), B, ptr(self.stats),
+                          0, ptr(self.GG_hi) if tc else None, ptr(self.GG_lo) if tc else None, self.GG_hi.stride(0) if tc else 0,
+                          stream=st, anchors=B)
         else:
-            self._k('dae_triplet_batch_hard_det' if det else 'dae_triplet_batch_hard', ptr(self.S), B, B, ptr(self.labels_b), ptr(self.G),
-                    B, ptr(self.weight), ptr(self.stats), *slots, st, n_launch=2)
-        if det:
-            self._k('dae_triplet_loss_sum', ptr(self.loss_slots), B, ptr(self.stats), st)
+            self._triplet('dae_triplet_batch_hard', ptr(self.S), B, B, ptr(self.labels_b), ptr(self.G), B, ptr(self.weight),
+                          ptr(self.stats), stream=st, anchors=B, n_launch=2)
 
-    def _mining_blocked(self, B, strat, train):
+    def _mining_blocked(self, B, train):
         """The mining one block of R anchor rows at a time, for r0 = 0, R, 2R, ... (the last block is short):
             S_blk = E[r0:r0+n].E^T;  the strategy's rows kernel -> G_blk (batch_all: scaled, with its bf16 hi / lo pair; batch_hard:
             unscaled, split to hi / lo times alpha here);  training: dE2[r0:r0+n] += a G_blk.E  and  dE2 += a G_blk^T.E[r0:r0+n].
@@ -934,68 +963,56 @@ class TrainEngine:
         Ehl = (self.E_hi, self.E_lo)
         Ghl = (self.GG_hi, self.GG_lo)
         lds, ldg, ldgg = self.S.stride(0), self.G.stride(0), self.GG_hi.stride(0)
-        if strat == 2:
+        batch_all = self.strategy == _BATCH_ALL
+        if not batch_all:
             self.weight.zero_()          # the rows kernels accumulate the data weights
         if train:
             self.dE2.zero_()
-        a = self.alpha if strat == 1 else 1.0   # batch_hard's hi / lo already carry alpha
+        a = self.alpha if batch_all else 1.0   # batch_hard's hi / lo already carry alpha
         for r0 in range(0, B, R):
             n = min(R, B - r0)
             Eblk = (self.E_hi[r0:], self.E_lo[r0:])
             self._tc_gemm(n, B, H, 1.0, Eblk, 0, Ehl, 0, self.S, lds, tag='gemm_gram')
-            det = self.deterministic
-            slots = (ptr(self.loss_slots),) if det else ()
-            if strat == 1:
-                self._k('dae_triplet_batch_all_rows_det' if det else 'dae_triplet_batch_all_rows', ptr(self.S), lds, r0, n, B,
-                        ptr(self.seg_lo), ptr(self.seg_hi), ptr(self.G), ldg, ptr(self.stats), 0, ptr(self.GG_hi) if train else None,
-                        ptr(self.GG_lo) if train else None, ldgg if train else 0, *slots, st)
+            if batch_all:
+                self._triplet('dae_triplet_batch_all_rows', ptr(self.S), lds, r0, n, B, ptr(self.seg_lo), ptr(self.seg_hi), ptr(self.G),
+                              ldg, ptr(self.stats), 0, ptr(self.GG_hi) if train else None, ptr(self.GG_lo) if train else None,
+                              ldgg if train else 0, stream=st)
             else:
-                self._k('dae_triplet_batch_hard_rows_det' if det else 'dae_triplet_batch_hard_rows', ptr(self.S), lds, r0, n, B,
-                        ptr(self.labels_b), ptr(self.G), ldg, ptr(self.weight), ptr(self.stats), *slots, st)
+                self._triplet('dae_triplet_batch_hard_rows', ptr(self.S), lds, r0, n, B, ptr(self.labels_b), ptr(self.G), ldg,
+                              ptr(self.weight), ptr(self.stats), stream=st)
                 if train:
                     self._tc_split(self.G, n, B, ldg, self.GG_hi, self.GG_lo, scale=self.alpha)
             if train:
                 self._tc_gemm(n, H, B, a, Ghl, 0, Ehl, 1, self.dE2[r0:], H, accumulate=1, tag='gemm_dE_tri')
                 self._tc_gemm(B, H, n, a, Ghl, 1, Eblk, 1, self.dE2, H, accumulate=1, tag='gemm_dE_tri')
-        if self.deterministic:
-            self._k('dae_triplet_loss_sum', ptr(self.loss_slots), B, ptr(self.stats), st)
-        if strat == 2:
+        self._sum_loss_slots(B, st)
+        if not batch_all:
             self._k('dae_triplet_batch_hard_finish', ptr(self.weight), B, ptr(self.stats), ptr(self.dE2) if train else None, H, H, st)
 
     def evaluate(self, csr, labels, B=None):
         """Forward-only cost of the whole set fed as ONE batch with x_corr = x, like the reference's validation pass
         (autoencoder/autoencoder.py:300-309).  Returns the stats dict."""
-        saved = (self.csr, self.csr_c, self.values_c, self.labels, self.in_scale)
-        try:
-            self.set_data(csr, None, labels)
-            self.in_scale = 1.0
-            self.step(None, 0, csr.shape[0] if B is None else B, None, train=False)
-            return self.read_stats()
-        finally:
-            self.csr, self.csr_c, self.values_c, self.labels, self.in_scale = saved
+        return self._evaluate(csr, labels, csr.shape[0] if B is None else B)
 
     def evaluate_explicit(self, csr_stacked, n_each):
         """Forward-only cost of a stacked [org; pos; neg] set fed as ONE batch with x_corr = x: the validation pass of
         DenoisingAutoencoderTriplet (reference autoencoder/autoencoder_triplet.py:166-199).  Returns the stats dict."""
+        return self._evaluate(csr_stacked, None, int(n_each), explicit_n=int(n_each))
+
+    def _evaluate(self, csr, labels, B, explicit_n=None):
         saved = (self.csr, self.csr_c, self.values_c, self.labels, self.in_scale)
         try:
-            self.set_data(csr_stacked, None, None)
+            self.set_data(csr, None, labels)
             self.in_scale = 1.0
-            B = int(n_each)
-            self._ctl = None
-            self._ensure_ws(3 * B)
-            self._k('dae_batch_prepare_explicit', None, 0, None, B, B, ptr(self.rows), ptr(self.stats), _stream())
-            self._branch_b_prologue(3 * B, False)
-            self._encode_forward(3 * B, False)
-            self._train_tail(3 * B, 3, None, None, False, explicit_B=B)
+            self._step(None, 0, B, None, train=False, explicit_n=explicit_n)
             return self.read_stats()
         finally:
             self.csr, self.csr_c, self.values_c, self.labels, self.in_scale = saved
 
-    def _decode_and_backward(self, B, rows, weight, train=True):
+    def _decode_and_backward(self, B, weight, train=True):
         """fp32 CUDA-core validation path of the decode chain (gemm_mode 'ffma')."""
         F, H, st = self.F, self.H, _stream()
-        c = self.csr
+        c, rows = self.csr, self.rows
         self._gemm(B, F, H, 1.0, self.E, H, 1, self.W, H, 1, 0.0, self.Z, F, tag='gemm_decode_fwd')  # Z = E.W^T
         self._k('dae_decode_loss_bwd', ptr(c.indptr), ptr(c.indices), ptr(c.values), ptr(rows), B, F, ptr(self.bv),
                 self.dec_act, self.loss, ptr(weight), ptr(self.stats), ptr(self.Z), F, ptr(self.row_loss), st)
@@ -1005,13 +1022,13 @@ class TrainEngine:
         self._gemm(F, H, B, 1.0, self.Z, 1, F, self.E, 1, H, 0.0, self._gW(), H, tag='gemm_decode_dW')  # dW_dec = dZ^T.E
         self._gemm(B, H, F, 1.0, self.Z, F, 1, self.W, 1, H, 0.0, self.dE, H, tag='gemm_decode_dE')    # dE = dZ.W
 
-    def _decode_tc(self, B, rows, weight, train=True, prepared=0):
+    def _decode_tc(self, B, weight, train=True, prepared=0):
         """Decode forward + loss on the tensor cores (bf16x3):  Z = E.W^T with the loss epilogue fused (no Z / D / dense X in
         HBM); dZ leaves as the bf16 hi/lo pair the two backward GEMMs consume."""
         F, H, st = self.F, self.H, _stream()
-        c = self.csr
+        c, rows = self.csr, self.rows
         Ehl, Whl = (self.E_hi, self.E_lo), (self.W_hi, self.W_lo)
-        if self.loss != 2:
+        if self.loss != _COSINE:
             det = self.deterministic   # deterministic: the row-loss partials are stored to [n_parts x B], not added
             self._k('dae_decode_fused_bf16x3_det' if det else 'dae_decode_fused_bf16x3', B, F, H, ptr(self.E_hi), ptr(self.E_lo), self.Hp, ptr(self.W_hi), ptr(self.W_lo),
                     self.Hp, ptr(c.indptr), ptr(c.indices), ptr(c.values), ptr(rows), ptr(self.bv), self.dec_act, self.loss,
@@ -1024,26 +1041,23 @@ class TrainEngine:
             if train:
                 self._tc_split(self.Z, B, F, F, self.dZ_hi, self.dZ_lo)
 
-    def _encode_backward(self, B, rows, dE_add=None, dbh_zeroed=0):
-        """K5: dA = dE * f'(A), dbh, and the sparse part of dW (X_c^T . dA) accumulated into the gradient buffer."""
+    def _encode_backward(self, B, dE_add=None, dbh_zeroed=0, scan_done=False):
+        """K5: dA = dE * f'(A), dbh, and the sparse part of dW (X_c^T . dA) accumulated into the gradient buffer.  scan_done: the
+        gather's column scan already ran (dae_col_scan on branch B)."""
         F, H, st = self.F, self.H, _stream()
         c = self.csr_c
+        head = (ptr(c.indptr), ptr(c.indices), ptr(self.values_c), ptr(self.rows), B, F, H, self.in_scale, ptr(self.E), ptr(self.bh),
+                self.enc_act, ptr(self.dE), ptr(dE_add), H)
         if self.enc_bwd_mode == 'det':   # dA, dbh stored; the sparse dW waits in the workspace for dae_encode_sparse_dw_add
-            self._k('dae_encode_csr_bwd_det', ptr(c.indptr), ptr(c.indices), ptr(self.values_c), ptr(rows), B, F, H, self.in_scale,
-                    ptr(self.E), ptr(self.bh), self.enc_act, ptr(self.dE), ptr(dE_add), H, ptr(self._gbh()), ptr(self.col_count),
-                    self._ent_cap, ptr(self.enc_det_ws), self.enc_det_ws.numel(), st, tag='dae_encode_csr_bwd',
+            self._k('dae_encode_csr_bwd_det', *head, ptr(self._gbh()), ptr(self.col_count), self._ent_cap, ptr(self.enc_det_ws),
+                    self.enc_det_ws.numel(), st, tag='dae_encode_csr_bwd',
                     n_launch=8)   # column scan, tile count, tile scan, placement, rows (dA), two dbh levels, gather
         elif self.enc_bwd_mode == 'gather':
-            scan_done = getattr(self, '_scan_done', False)
-            self._scan_done = False
-            self._k('dae_encode_csr_bwd_gather', ptr(c.indptr), ptr(c.indices), ptr(self.values_c), ptr(rows), B, F, H, self.in_scale,
-                    ptr(self.E), ptr(self.bh), self.enc_act, ptr(self.dE), ptr(dE_add), H, ptr(self._gW()), ptr(self._gbh()), int(dbh_zeroed),
-                    None if scan_done else ptr(self.col_count),
+            self._k('dae_encode_csr_bwd_gather', *head, ptr(self._gW()), ptr(self._gbh()), int(dbh_zeroed), None if scan_done else ptr(self.col_count),
                     ptr(self.col_start), ptr(self.col_cursor), ptr(self.ent_col), ptr(self.ent_row), ptr(self.ent_val), st, n_launch=3,
                     tag='dae_encode_csr_bwd')
         else:
-            self._k('dae_encode_csr_bwd', ptr(c.indptr), ptr(c.indices), ptr(self.values_c), ptr(rows), B, F, H, self.in_scale,
-                    ptr(self.E), ptr(self.bh), self.enc_act, ptr(self.dE), ptr(dE_add), H, ptr(self._gW()), ptr(self._gbh()), int(dbh_zeroed), st)
+            self._k('dae_encode_csr_bwd', *head, ptr(self._gW()), ptr(self._gbh()), int(dbh_zeroed), st)
 
     def _setup_multimem(self, n_blocks=132):
         """Move the gradient buffer into symmetric memory bound to a multicast address and create the peer-mapped flag words
@@ -1081,23 +1095,12 @@ class TrainEngine:
                 self._allreduce_grad()
             gscale = 1.0 / self.world
         self.step_count += 1
-        if getattr(self, '_ctl', None) is None:   # an eager step: the device step counter ctl[2] stays behind step_count, so the next
-            self._ctl_owner = None                 # run_feed replay re-synchronises it (Adam's bias correction reads it)
+        if self._ctl is None:       # an eager step: the device step counter ctl[2] stays behind step_count, so the next
+            self._ctl_owner = None  # run_feed replay re-synchronises it (Adam's bias correction reads it)
         tc = self.gemm_mode == 'tc'
         self._k('dae_optimizer_step', ptr(self.theta), ptr(self.grad), ptr(self.slot1), ptr(self.slot2), self.n_params,
-                self.opt, self.lr, self.momentum, gscale, self.step_count, ptr(getattr(self, '_ctl', None)),
+                self.opt, self.lr, self.momentum, gscale, self.step_count, ptr(self._ctl),
                 ptr(self.W_hi) if tc else None, ptr(self.W_lo) if tc else None, F, H, self.Hp, st)
-
-    # ---- explicit (anchor, pos, neg) triplets: DenoisingAutoencoderTriplet ---------------------------------------------
-    def step_explicit(self, perm, offset, B, n_rows_each, stats_log_row=None, ctl=None):
-        """self.csr holds [org; pos; neg] stacked (3*n_rows_each rows). autoencoder_triplet.py:256-258,286-288,303-314."""
-        B3 = 3 * B
-        self._ctl = ctl
-        self._ensure_ws(B3)
-        self._k('dae_batch_prepare_explicit', ptr(perm), int(offset), ptr(ctl), B, int(n_rows_each), ptr(self.rows), ptr(self.stats), _stream())
-        self._branch_b_prologue(B3, True)
-        self._encode_forward(B3, True)
-        self._train_tail(B3, 3, None, stats_log_row, True, explicit_B=B)
 
     # ---- transform ------------------------------------------------------------------------------------------------------
     # dae_encode_csr_fwd_hot (hot rows of W staged in shared memory by bulk TMA) is OFF by default: it cuts the L2 -> L1 gather traffic
@@ -1149,26 +1152,29 @@ class TrainEngine:
         `self.values_c`.  staged: the triplet strategies take their (label-sorted) batch from staging buffers filled by the
         previous replay (set_step_cursor stages the first one).  explicit_n: rows per block of the stacked [org; pos; neg] set
         (DenoisingAutoencoderTriplet).  Returns the graph; replay with `replay_step()` after `set_step_cursor()`."""
-        if not hasattr(self, 'ctl'):
-            self.ctl = torch.zeros(4, dtype=torch.int64, device=self.device)
         stride = int(B if row_stride is None else row_stride)
+        use_stage = bool(staged) and explicit_n is None and self._mines and perm_buf is not None
+        self._graph, self._graph2 = self._capture(perm_buf, B, log_buf, stride, (int(perm_buf.numel()), stride) if use_stage else None,
+                                                  explicit_n)
+        self._graph_meta = {'perm': perm_buf, 'B': B, 'staged': use_stage}
+        return self._graph
+
+    def _capture(self, perm_buf, B, log_buf, stride, staged, explicit_n):
+        """Capture the step of `_step(perm_buf, 0, B, log_buf, ctl=self.ctl, staged=staged, explicit_n=explicit_n)` followed by
+        dae_step_advance(stride), after two warm-up steps whose parameter updates are undone.  Returns (g, g2): g2 is the optimizer
+        graph of the 'nccl' exchange, else None."""
+        if self.ctl is None:
+            self.ctl = torch.zeros(4, dtype=torch.int64, device=self.device)
         saved = (self.step_count, self.timed)
         self.timed = None
-        feed = staged == 'feed'       # run_feeds: rows 0..B-1 of the feed buffer, the next batch's labels in self._labels_next
-        n_perm = int(perm_buf.numel()) if perm_buf is not None else (B if feed else 0)
-        use_stage = bool(staged) and explicit_n is None and self.strategy in (1, 2) and (perm_buf is not None or feed)
-        self._graph_meta = {'perm': perm_buf, 'B': B, 'staged': use_stage}
 
-        def one_step():
-            if explicit_n is not None:
-                self.step_explicit(perm_buf, 0, B, explicit_n, log_buf, ctl=self.ctl)
-            else:
-                self.step(perm_buf, 0, B, log_buf, ctl=self.ctl, staged=(n_perm, stride) if use_stage else None)
+        def one_step(defer_update=False):
+            self._step(perm_buf, 0, B, log_buf, ctl=self.ctl, staged=staged, explicit_n=explicit_n, defer_update=defer_update)
         # warm-up outside capture (workspace allocation, function attributes, NCCL channels)
         snap = (self.theta.clone(), None if self.slot1 is None else self.slot1.clone(), None if self.slot2 is None else self.slot2.clone(),
                 self.ctl.clone())
         self.ctl.copy_(torch.tensor([0, 0, 1, 0], dtype=torch.int64))  # warm-up / capture run on the first rows of perm_buf
-        if use_stage:
+        if staged is not None:
             self.stage_batch(perm_buf, 0, B)
         for _ in range(2):
             one_step()
@@ -1193,12 +1199,8 @@ class TrainEngine:
                 one_step()
                 call('dae_step_advance', ptr(self.ctl), stride, _stream())
         else:
-            self._defer_update = True
-            try:
-                with torch.cuda.graph(g, capture_error_mode='thread_local'):
-                    one_step()
-            finally:
-                self._defer_update = False
+            with torch.cuda.graph(g, capture_error_mode='thread_local'):
+                one_step(defer_update=True)
             g2 = torch.cuda.CUDAGraph()
             with torch.cuda.graph(g2, capture_error_mode='thread_local'):
                 self._apply_update(reduce=False)
@@ -1207,22 +1209,19 @@ class TrainEngine:
         self.launches = launches0
         self.step_count = saved[0]
         self.timed = saved[1]
-        self._graph = g
-        self._graph2 = g2
-        return g
+        return g, g2
 
     def set_step_cursor(self, offset, log_row=0):
         """Host-side (re)positioning of the device cursors, e.g. at an epoch start."""
         self._ctl_owner = 'fit'
         self._set_ctl(offset, log_row)
-        m = getattr(self, '_graph_meta', None)
+        m = self._graph_meta
         if m is not None and m['staged']:      # the replayed step takes its batch from the staging buffers
             self.stage_batch(m['perm'], int(offset), m['B'])
 
     def _set_ctl(self, offset, log_row):
-        if getattr(self, '_ctl_host', None) is None:
+        if self._ctl_host is None:
             self._ctl_host = [torch.zeros(4, dtype=torch.int64).pin_memory() for _ in range(8)]   # ring: the copies are asynchronous
-            self._ctl_host_i = 0
         h = self._ctl_host[self._ctl_host_i % len(self._ctl_host)]
         self._ctl_host_i += 1
         h[0], h[1], h[2], h[3] = int(offset), int(log_row), self.step_count + 1, 0
