@@ -116,6 +116,15 @@ _SIGNATURES = {
     'dae_impression_rank_loss': (C.c_int, [p, i64, p, i64, i32, p, i64, p, p, p, f32, p, i64, p, p]),
     'dae_impression_metrics': (C.c_int, [p, i64, p, i64, i32, i32, p, p, p, i64, p, p, p]),
     'dae_impression_softmax_loss': (C.c_int, [p, i64, p, i64, i32, p, i64, p, p, p, p, i32, u64, u64, f32, p, i64, p, p, p]),
+    # article encoder fine-tuned through the user encoders' losses
+    'dae_encode_csr_fwd_groups': (C.c_int, [p, p, p, p, i32, i32, i32, f32, p, p, i32, p, i64, p, p, p, i64, i32, p]),
+    'dae_seq_rank_loss_grad': (C.c_int, [p, i64, p, i64, i32, p, p, i64, f32, p, i64, p, p, i64, p]),
+    'dae_impression_rank_loss_grad': (C.c_int, [p, i64, p, i64, i32, p, i64, p, p, p, f32, p, i64, p, p, i64, p]),
+    'dae_impression_softmax_loss_grad': (C.c_int, [p, i64, p, i64, i32, p, i64, p, p, p, p, i32, u64, u64, f32, p, i64, p, p, p, i64,
+                                                   p]),
+    'dae_touch_compact_workspace': (C.c_int, [i64, p]),
+    'dae_touch_compact': (C.c_int, [p, i64, C.c_uint32, p, p, p, p, p, p]),
+    'dae_rows_scatter_add': (C.c_int, [p, i64, p, i64, i32, p, i64, p]),
     # deterministic training step
     'dae_gemm_det_workspace': (C.c_int, [p]),
     'dae_gemm_bf16x3_det': (C.c_int, [i32, i32, i32, f32, p, p, i64, i32, p, p, i64, i32, p, i64, i32, i32, p, i32, i32, p, i64, p]),

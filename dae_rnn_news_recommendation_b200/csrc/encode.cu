@@ -713,31 +713,55 @@ static inline int pick_nc(int H, int vw) {
 
 }  // namespace dae
 
-extern "C" int dae_encode_csr_fwd(const int64_t* indptr, const int32_t* indices, const float* values, const int32_t* rows,
-                                  int32_t n_rows, int32_t F, int32_t H, float in_scale, const float* W, const float* bh,
-                                  int32_t enc_act, float* E, int64_t ldE, int32_t* col_count, void* e_hi, void* e_lo,
-                                  int64_t ld_split, void* stream) {
-  using namespace dae;
-  DAE_REQUIRE(indptr && indices && values && W && bh && E, "dae_encode_csr_fwd: null pointer");
-  DAE_REQUIRE(n_rows >= 0 && F > 0 && H > 0 && ldE >= H, "dae_encode_csr_fwd: bad shape n_rows=%d F=%d H=%d ldE=%lld", n_rows, F, H, (long long)ldE);
-  DAE_REQUIRE(!e_hi || (e_lo && ld_split >= H), "dae_encode_csr_fwd: bad split outputs");
+namespace dae {
+
+// dae_encode_csr_fwd and dae_encode_csr_fwd_groups: `groups` thread groups of 128 per row (1 or 4); messages under `name`.
+static int encode_fwd(const char* name, const int64_t* indptr, const int32_t* indices, const float* values, const int32_t* rows,
+                      int32_t n_rows, int32_t F, int32_t H, float in_scale, const float* W, const float* bh, int32_t enc_act, float* E,
+                      int64_t ldE, int32_t* col_count, void* e_hi, void* e_lo, int64_t ld_split, int groups, void* stream) {
+  DAE_REQUIRE(indptr && indices && values && W && bh && E, "%s: null pointer", name);
+  DAE_REQUIRE(n_rows >= 0 && F > 0 && H > 0 && ldE >= H, "%s: bad shape n_rows=%d F=%d H=%d ldE=%lld", name, n_rows, F, H, (long long)ldE);
+  DAE_REQUIRE(!e_hi || (e_lo && ld_split >= H), "%s: bad split outputs", name);
   if (n_rows == 0) return DAE_OK;
   const int vw = pick_vw(H, H, W);
   const int nc = pick_nc(H, vw);
-  if (nc < 0) { set_error("dae_encode_csr_fwd: H=%d too large for vector width %d", H, vw); return DAE_ERR_UNSUPPORTED; }
+  if (nc < 0) { set_error("%s: H=%d too large for vector width %d", name, H, vw); return DAE_ERR_UNSUPPORTED; }
   cudaStream_t st = (cudaStream_t)stream;
   if (col_count) DAE_CUDA(cudaMemsetAsync(col_count, 0, sizeof(int32_t) * F, st));
   dim3 grid(n_rows);
-  // Few rows (a training batch): every row is resident at once and the launch lasts as long as its longest row -> split rows over
-  // 4 thread groups.  Many rows (transform): throughput-bound, one group per row keeps more rows in flight.
-  const int groups = (n_rows <= sm_count() * 32) ? 4 : 1;
   DAE_DISPATCH_ACT(enc_act, ACT, {
     if (vw == 4) launch_fwd_nc<ACT, 4>(nc, groups, grid, st, indptr, indices, values, rows, H, in_scale, W, bh, E, ldE, col_count, e_hi, e_lo, ld_split);
     else if (vw == 2) launch_fwd_nc<ACT, 2>(nc, groups, grid, st, indptr, indices, values, rows, H, in_scale, W, bh, E, ldE, col_count, e_hi, e_lo, ld_split);
     else launch_fwd_nc<ACT, 1>(nc, groups, grid, st, indptr, indices, values, rows, H, in_scale, W, bh, E, ldE, col_count, e_hi, e_lo, ld_split);
   });
-  DAE_CHECK_LAUNCH("dae_encode_csr_fwd");
+  DAE_CHECK_LAUNCH(name);
   return DAE_OK;
+}
+
+}  // namespace dae
+
+extern "C" int dae_encode_csr_fwd(const int64_t* indptr, const int32_t* indices, const float* values, const int32_t* rows,
+                                  int32_t n_rows, int32_t F, int32_t H, float in_scale, const float* W, const float* bh,
+                                  int32_t enc_act, float* E, int64_t ldE, int32_t* col_count, void* e_hi, void* e_lo,
+                                  int64_t ld_split, void* stream) {
+  using namespace dae;
+  // Few rows (a training batch): every row is resident at once and the launch lasts as long as its longest row -> split rows over
+  // 4 thread groups.  Many rows (transform): throughput-bound, one group per row keeps more rows in flight.
+  const int groups = (n_rows <= sm_count() * 32) ? 4 : 1;
+  return encode_fwd("dae_encode_csr_fwd", indptr, indices, values, rows, n_rows, F, H, in_scale, W, bh, enc_act, E, ldE, col_count, e_hi,
+                    e_lo, ld_split, groups, stream);
+}
+
+// The same with the group count given (1 or 4) instead of chosen from n_rows: a row's output bits depend on the group count only,
+// so a caller that pins it gets the same row whether it encodes the row alone, in a subset or in the whole set (DESIGN 4.19).
+extern "C" int dae_encode_csr_fwd_groups(const int64_t* indptr, const int32_t* indices, const float* values, const int32_t* rows,
+                                         int32_t n_rows, int32_t F, int32_t H, float in_scale, const float* W, const float* bh,
+                                         int32_t enc_act, float* E, int64_t ldE, int32_t* col_count, void* e_hi, void* e_lo,
+                                         int64_t ld_split, int32_t groups, void* stream) {
+  using namespace dae;
+  DAE_REQUIRE(groups == 1 || groups == 4, "dae_encode_csr_fwd_groups: groups = %d, 1 or 4", groups);
+  return encode_fwd("dae_encode_csr_fwd_groups", indptr, indices, values, rows, n_rows, F, H, in_scale, W, bh, enc_act, E, ldE, col_count,
+                    e_hi, e_lo, ld_split, groups, stream);
 }
 
 extern "C" int dae_encode_csr_bwd(const int64_t* indptr, const int32_t* indices, const float* values, const int32_t* rows,

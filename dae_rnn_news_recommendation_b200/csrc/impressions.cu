@@ -65,10 +65,13 @@ __device__ __forceinline__ void score_chunk(const float* __restrict__ h, const f
 // without impressions gets dh_p = 0.  The warp owns row p of dh: no atomics, the result does not depend on the schedule.
 // Candidates are taken kImpChunk at a time (chunk A, whose weights are summed in shared memory) against every chunk B of the
 // same impression, whose scores are recomputed when the impression has more than one chunk.
+// DEMB (dae_impression_rank_loss_grad, DESIGN 4.19): each candidate's coefficient g also adds g h_p into demb[items[j]] by fp32
+// atomics; the DEMB = false instance is dae_impression_rank_loss's kernel, its code unchanged by the flag.
+template <bool DEMB>
 __global__ void __launch_bounds__(kImpWarps * 32) impression_rank_loss_kernel(
     const float* __restrict__ h, int64_t ld_h, const float* __restrict__ emb, int64_t ld_emb, int H, const int64_t* __restrict__ pos_indptr,
     int64_t n_pos, const int64_t* __restrict__ imp_indptr, const int32_t* __restrict__ items, const uint8_t* __restrict__ clicked,
-    float scale, float* __restrict__ dh, int64_t ld_dh, double* __restrict__ loss_sum) {
+    float scale, float* __restrict__ dh, int64_t ld_dh, double* __restrict__ loss_sum, float* __restrict__ demb, int64_t ld_demb) {
   __shared__ float s_a[kImpWarps][kImpChunk], s_b[kImpWarps][kImpChunk], s_w[kImpWarps][kImpChunk];
   __shared__ uint8_t f_a[kImpWarps][kImpChunk], f_b[kImpWarps][kImpChunk];
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
@@ -122,6 +125,11 @@ __global__ void __launch_bounds__(kImpWarps * 32) impression_rank_loss_kernel(
           const float* e = emb + (int64_t)items[b0 + a0 + t] * ld_emb;
 #pragma unroll 1
           for (int j = lane; j < H; j += 32) d[j] = fmaf(g, e[j], d[j]);
+          if constexpr (DEMB) {
+            float* de = demb + (int64_t)items[b0 + a0 + t] * ld_demb;
+#pragma unroll 1
+            for (int j = lane; j < H; j += 32) atomicAdd(de + j, g * hp[j]);
+          }
         }
         __syncwarp();
       }
@@ -259,11 +267,14 @@ __device__ __forceinline__ uint32_t softmax_draw(uint64_t seed, uint64_t epoch, 
 // work is O(m H + |C|).  Otherwise only the click and its K draws are scored, one draw per lane; Floyd's membership test is a
 // warp vote.  The warp owns row p of dh: no atomics on dh, the result does not depend on the schedule.  Launch bounds of 8 CTAs
 // per SM let ptxas use 64 registers; at its default of 48 it spilled the draw loop's state to the stack.
+// DEMB (dae_impression_softmax_loss_grad, DESIGN 4.19): each candidate's weight g also adds g h_p into demb[it[k]] by fp32 atomics;
+// the DEMB = false instance is dae_impression_softmax_loss's kernel, its code unchanged by the flag.
+template <bool DEMB>
 __global__ void __launch_bounds__(kImpWarps * 32, 8) impression_softmax_loss_kernel(
     const float* __restrict__ h, int64_t ld_h, const float* __restrict__ emb, int64_t ld_emb, int H, const int64_t* __restrict__ pos_indptr,
     int64_t n_pos, const int64_t* __restrict__ imp_indptr, const int32_t* __restrict__ items, const uint8_t* __restrict__ clicked,
     const int64_t* __restrict__ imp_ids, int K, uint64_t seed, uint64_t epoch, float scale, float* __restrict__ dh, int64_t ld_dh,
-    double* __restrict__ loss_sum, float* ws) {
+    double* __restrict__ loss_sum, float* ws, float* __restrict__ demb, int64_t ld_demb) {
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
   const float neg_inf = __int_as_float(0xff800000);
   double acc = 0.0;
@@ -356,6 +367,11 @@ __global__ void __launch_bounds__(kImpWarps * 32, 8) impression_softmax_loss_ker
         const float* e = emb + (int64_t)it[k] * ld_emb;
 #pragma unroll 1
         for (int j = lane; j < H; j += 32) d[j] = fmaf(g, e[j], d[j]);
+        if constexpr (DEMB) {
+          float* de = demb + (int64_t)it[k] * ld_demb;
+#pragma unroll 1
+          for (int j = lane; j < H; j += 32) atomicAdd(de + j, g * hp[j]);
+        }
       }
       __syncwarp();   // the next impression of this warp may write ws entries that lanes read above
     }
@@ -378,9 +394,21 @@ extern "C" int dae_impression_rank_loss(const float* h, int64_t ld_h, const floa
                                         float* dh, int64_t ld_dh, double* loss_sum, void* stream) {
   DAE_REQUIRE(h && emb && pos_indptr && imp_indptr && items && clicked && dh && loss_sum && H > 0 && n_pos > 0 && ld_h >= H &&
               ld_emb >= H && ld_dh >= H, "dae_impression_rank_loss: bad arguments");
-  impression_rank_loss_kernel<<<imp_grid(n_pos), kImpWarps * 32, 0, (cudaStream_t)stream>>>(
-      h, ld_h, emb, ld_emb, H, pos_indptr, n_pos, imp_indptr, items, clicked, scale, dh, ld_dh, loss_sum);
+  impression_rank_loss_kernel<false><<<imp_grid(n_pos), kImpWarps * 32, 0, (cudaStream_t)stream>>>(
+      h, ld_h, emb, ld_emb, H, pos_indptr, n_pos, imp_indptr, items, clicked, scale, dh, ld_dh, loss_sum, nullptr, 0);
   DAE_CHECK_LAUNCH("dae_impression_rank_loss");
+  return DAE_OK;
+}
+
+extern "C" int dae_impression_rank_loss_grad(const float* h, int64_t ld_h, const float* emb, int64_t ld_emb, int32_t H,
+                                             const int64_t* pos_indptr, int64_t n_pos, const int64_t* imp_indptr, const int32_t* items,
+                                             const uint8_t* clicked, float scale, float* dh, int64_t ld_dh, double* loss_sum, float* demb,
+                                             int64_t ld_demb, void* stream) {
+  DAE_REQUIRE(h && emb && pos_indptr && imp_indptr && items && clicked && dh && loss_sum && demb && H > 0 && n_pos > 0 && ld_h >= H &&
+              ld_emb >= H && ld_dh >= H && ld_demb >= H, "dae_impression_rank_loss_grad: bad arguments");
+  impression_rank_loss_kernel<true><<<imp_grid(n_pos), kImpWarps * 32, 0, (cudaStream_t)stream>>>(
+      h, ld_h, emb, ld_emb, H, pos_indptr, n_pos, imp_indptr, items, clicked, scale, dh, ld_dh, loss_sum, demb, ld_demb);
+  DAE_CHECK_LAUNCH("dae_impression_rank_loss_grad");
   return DAE_OK;
 }
 
@@ -390,10 +418,25 @@ extern "C" int dae_impression_softmax_loss(const float* h, int64_t ld_h, const f
                                            float scale, float* dh, int64_t ld_dh, double* loss_sum, void* workspace, void* stream) {
   DAE_REQUIRE(h && emb && pos_indptr && imp_indptr && items && clicked && imp_ids && dh && loss_sum && workspace && H > 0 && n_pos > 0 &&
               ld_h >= H && ld_emb >= H && ld_dh >= H && K >= 0 && K <= kImpMaxNegatives, "dae_impression_softmax_loss: bad arguments");
-  impression_softmax_loss_kernel<<<imp_grid(n_pos), kImpWarps * 32, 0, (cudaStream_t)stream>>>(
+  impression_softmax_loss_kernel<false><<<imp_grid(n_pos), kImpWarps * 32, 0, (cudaStream_t)stream>>>(
       h, ld_h, emb, ld_emb, H, pos_indptr, n_pos, imp_indptr, items, clicked, imp_ids, K, seed, epoch, scale, dh, ld_dh, loss_sum,
-      (float*)workspace);
+      (float*)workspace, nullptr, 0);
   DAE_CHECK_LAUNCH("dae_impression_softmax_loss");
+  return DAE_OK;
+}
+
+extern "C" int dae_impression_softmax_loss_grad(const float* h, int64_t ld_h, const float* emb, int64_t ld_emb, int32_t H,
+                                                const int64_t* pos_indptr, int64_t n_pos, const int64_t* imp_indptr, const int32_t* items,
+                                                const uint8_t* clicked, const int64_t* imp_ids, int32_t K, uint64_t seed, uint64_t epoch,
+                                                float scale, float* dh, int64_t ld_dh, double* loss_sum, void* workspace, float* demb,
+                                                int64_t ld_demb, void* stream) {
+  DAE_REQUIRE(h && emb && pos_indptr && imp_indptr && items && clicked && imp_ids && dh && loss_sum && workspace && demb && H > 0 &&
+              n_pos > 0 && ld_h >= H && ld_emb >= H && ld_dh >= H && ld_demb >= H && K >= 0 && K <= kImpMaxNegatives,
+              "dae_impression_softmax_loss_grad: bad arguments");
+  impression_softmax_loss_kernel<true><<<imp_grid(n_pos), kImpWarps * 32, 0, (cudaStream_t)stream>>>(
+      h, ld_h, emb, ld_emb, H, pos_indptr, n_pos, imp_indptr, items, clicked, imp_ids, K, seed, epoch, scale, dh, ld_dh, loss_sum,
+      (float*)workspace, demb, ld_demb);
+  DAE_CHECK_LAUNCH("dae_impression_softmax_loss_grad");
   return DAE_OK;
 }
 

@@ -106,12 +106,16 @@ __global__ void __launch_bounds__(256) seq_negatives_kernel(const int32_t* __res
 
 // One warp per position p: s+ = h_p . e(pos), s- = h_p . e(neg), loss softplus(s- - s+) (summed into *loss_sum in fp64),
 // dh_p = scale sigma(s- - s+) (e(neg) - e(pos)).  Positions without a next read (pos < 0) get dh_p = 0.
+// DEMB (dae_seq_rank_loss_grad, DESIGN 4.19): also demb[neg] += g h_p and demb[pos] -= g h_p with g = scale sigma(s- - s+), by fp32
+// atomics; the DEMB = false instance is dae_seq_rank_loss's kernel, its code unchanged by the flag.
 constexpr int kLossWarps = 8;
+template <bool DEMB>
 __global__ void __launch_bounds__(kLossWarps * 32) seq_rank_loss_kernel(const float* __restrict__ h, int64_t ld_h,
                                                                         const float* __restrict__ emb, int64_t ld_emb, int H,
                                                                         const int32_t* __restrict__ pos, const int32_t* __restrict__ neg,
                                                                         int64_t n_pos, float scale, float* __restrict__ dh,
-                                                                        int64_t ld_dh, double* __restrict__ loss_sum) {
+                                                                        int64_t ld_dh, double* __restrict__ loss_sum,
+                                                                        float* __restrict__ demb, int64_t ld_demb) {
   __shared__ double s_loss[kLossWarps];
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
   double acc = 0.0;
@@ -132,6 +136,15 @@ __global__ void __launch_bounds__(kLossWarps * 32) seq_rank_loss_kernel(const fl
     const float x = sn - sp;
     const float g = scale * sigmoidf_(x);
     for (int j = lane; j < H; j += 32) d[j] = g * (en[j] - ep[j]);
+    if constexpr (DEMB) {
+      float* dp = demb + (int64_t)a * ld_demb;
+      float* dn = demb + (int64_t)neg[p] * ld_demb;
+      for (int j = lane; j < H; j += 32) {
+        const float x = g * hp[j];
+        atomicAdd(dn + j, x);
+        atomicAdd(dp + j, -x);
+      }
+    }
     if (lane == 0) acc += (double)(fmaxf(x, 0.0f) + log1pf(expf(-fabsf(x))));
   }
   if (lane == 0) s_loss[w] = acc;
@@ -201,8 +214,19 @@ extern "C" int dae_seq_rank_loss(const float* h, int64_t ld_h, const float* emb,
                                  const int32_t* neg, int64_t n_pos, float scale, float* dh, int64_t ld_dh, double* loss_sum, void* stream) {
   DAE_REQUIRE(h && emb && pos && neg && dh && loss_sum && H > 0 && n_pos > 0 && ld_h >= H && ld_emb >= H && ld_dh >= H,
               "dae_seq_rank_loss: bad arguments");
-  seq_rank_loss_kernel<<<grid_for(n_pos, kLossWarps, 16), kLossWarps * 32, 0, (cudaStream_t)stream>>>(
-      h, ld_h, emb, ld_emb, H, pos, neg, n_pos, scale, dh, ld_dh, loss_sum);
+  seq_rank_loss_kernel<false><<<grid_for(n_pos, kLossWarps, 16), kLossWarps * 32, 0, (cudaStream_t)stream>>>(
+      h, ld_h, emb, ld_emb, H, pos, neg, n_pos, scale, dh, ld_dh, loss_sum, nullptr, 0);
   DAE_CHECK_LAUNCH("dae_seq_rank_loss");
+  return DAE_OK;
+}
+
+extern "C" int dae_seq_rank_loss_grad(const float* h, int64_t ld_h, const float* emb, int64_t ld_emb, int32_t H, const int32_t* pos,
+                                      const int32_t* neg, int64_t n_pos, float scale, float* dh, int64_t ld_dh, double* loss_sum,
+                                      float* demb, int64_t ld_demb, void* stream) {
+  DAE_REQUIRE(h && emb && pos && neg && dh && loss_sum && demb && H > 0 && n_pos > 0 && ld_h >= H && ld_emb >= H && ld_dh >= H &&
+              ld_demb >= H, "dae_seq_rank_loss_grad: bad arguments");
+  seq_rank_loss_kernel<true><<<grid_for(n_pos, kLossWarps, 16), kLossWarps * 32, 0, (cudaStream_t)stream>>>(
+      h, ld_h, emb, ld_emb, H, pos, neg, n_pos, scale, dh, ld_dh, loss_sum, demb, ld_demb);
+  DAE_CHECK_LAUNCH("dae_seq_rank_loss_grad");
   return DAE_OK;
 }

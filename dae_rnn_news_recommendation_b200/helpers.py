@@ -469,6 +469,9 @@ def _history_weights(histories, n_articles, fn):
 
 
 def _dense_embeddings(embeddings, device, fn):
+    from .user_model import ArticleEncoder
+    if isinstance(embeddings, ArticleEncoder):   # a fine-tuned article encoder stands for its vectors (DESIGN 4.19)
+        return embeddings.vectors(to_host=False)
     if sp.issparse(embeddings):
         raise ValueError('%s: embeddings must be dense (an array or a tensor [N, H]); sparse bag-of-words profiles are not supported' % fn)
     x = _as_device_dense(embeddings, device)

@@ -2,7 +2,8 @@
 article (DESIGN 4.10).
 
     m = UserGRU(dim=H, max_len=50, batch_users=1024, num_epochs=5)
-    m.fit((indptr, items), embeddings)        # embeddings: [N, H] article vectors (transform()'s output), kept frozen
+    m.fit((indptr, items), embeddings)        # embeddings: [N, H] article vectors (transform()'s output), kept frozen, or an
+                                              # ArticleEncoder, trained with the model (DESIGN 4.19)
     U = m.transform((indptr, items), embeddings)            # [U, H] user vectors, score articles by inner product
     idx, score = m.recommend((indptr, items), embeddings, k=10)
 
@@ -42,12 +43,20 @@ before the last max_len reads still shapes the state.  Training masks each batch
 training: a masked user starts from 0) and updates only the rows of the unmasked batch users, by dae_rows_optimizer_step
 (long_term_learning_rate).  transform, impression_states and recommend start every user from its row, with no mask; users at or
 beyond row U (cold-start users) start from 0.  save() / load() keep the table; state_dict() keeps torch's four keys.
+
+Fine-tuned article encoder (DESIGN 4.19): fit(sequences, art) with an ArticleEncoder art in place of the embeddings trains the user
+encoder and the DAE encoder e(x) = f(s x W + bh) - f(bh) of art on the same loss, with e(a) in place of the frozen row a.  Each
+batch encodes only the T articles it touches (dae_touch_compact, dae_encode_csr_fwd_groups), runs every user-encoder kernel on that
+compact table with slot ids, takes the article gradient from the loss (the *_loss_grad exports) and from the input projection
+(dX = dXP . W_in, dae_rows_scatter_add), backpropagates it into [W | bh] (dae_encode_csr_bwd_gather) and steps [W | bh] after
+theta.  art.vectors(X) encodes any bag of words with the learned W and bh, articles never seen in training included.
 """
 import numpy as np
 import torch
 
 from . import _cabi, sparse_optim
 from ._cabi import call
+from .article_encoder import ARTICLE_ENCODE_GROUPS, ARTICLE_LEARNING_RATE, ArticleEncoder  # noqa: F401
 
 _NAMES = ('weight_ih_l0', 'weight_hh_l0', 'bias_ih_l0', 'bias_hh_l0')
 LONG_TERM_LEARNING_RATE = 0.1    # the long-term table's default learning rate: the best of 0.01, 0.03 and 0.1 (DESIGN 4.18)
@@ -319,8 +328,15 @@ class _UserEncoder:
         return m
 
     # ---- device helpers ---------------------------------------------------------------------------------------------------
+    def _check_articles(self, art, fn):
+        if art.dim != self.dim:
+            raise ValueError('%s: the article encoder has H = %d, the model %d' % (fn, art.dim, self.dim))
+
     def _embeddings(self, embeddings, fn):
         from .helpers import _dense_embeddings
+        if isinstance(embeddings, ArticleEncoder):
+            self._check_articles(embeddings, fn)
+            return embeddings.vectors(to_host=False)
         emb = _dense_embeddings(embeddings, self.device, fn)
         if emb.shape[1] != self.dim:
             raise ValueError('%s: embeddings are %d wide, the model has H = %d' % (fn, emb.shape[1], self.dim))
@@ -340,40 +356,74 @@ class _UserEncoder:
             self.phase_events.append((name, e))
 
     # ---- training ---------------------------------------------------------------------------------------------------------
-    def _forward_backward(self, pk, emb, epoch, batch, ib=None):
+    def _forward_backward(self, pk, emb, epoch, batch, ib=None, art=None):
         """Loss (added to self.stats) and the gradient (self.grad) of one packed batch with pk.terms > 0, or with ib (an
         ImpressionBatch with ib.n > 0) the impression loss of its impressions in place of the random negatives: pairwise, or with
-        impression_loss='softmax' the sampled softmax over its ib.clicks samples."""
+        impression_loss='softmax' the sampled softmax over its ib.clicks samples.  With art (an ArticleEncoder; emb is then None)
+        the batch runs on the compact table of the articles it touches and art.grad gets [dW | dbh] (DESIGN 4.19)."""
         H, P = self.dim, pk.P
         b = self._buffers(P, pk.B)
         st = _stream()
-        items = _upload(pk.items, self.device)
+        neg = b['neg']
+        if art is None:
+            items = _upload(pk.items, self.device)
+        elif ib is None:   # one upload of every id the batch touches: [items | nxt | neg (drawn below)] or [items | shown items]
+            ids = _upload(np.concatenate([pk.items, pk.nxt, np.full(P, -1, np.int32)]), self.device)
+        else:
+            ids = _upload(np.concatenate([pk.items, ib.items]), self.device)
         if ib is None:
-            nxt = _upload(pk.nxt, self.device)
+            nxt = _upload(pk.nxt, self.device) if art is None else ids[P:2 * P]
         elif self.impression_loss == 'softmax':
             pos_indptr, imp_indptr, imp_items, imp_clicked, imp_ids = ib.views(_upload(ib.buffer(ids=True), self.device))
         else:
             pos_indptr, imp_indptr, imp_items, imp_clicked = ib.views(_upload(ib.buffer(), self.device))
         self._refresh()
         self._mark('start')
-        if ib is None:
-            call('dae_seq_negatives', nxt.data_ptr(), P, emb.shape[0], self.seed, epoch, batch, b['neg'].data_ptr(), st)
+        if ib is None:   # in article-id space: the same negatives as a run on frozen embeddings
+            if art is not None:
+                neg = ids[2 * P:]
+            call('dae_seq_negatives', nxt.data_ptr(), P, emb.shape[0] if art is None else art.n, self.seed, epoch, batch, neg.data_ptr(),
+                 st)
+        grad = ()
+        if art is not None:
+            rows, slots, T = art.touch(ids)
+            items = slots[:P]
+            if ib is None:
+                nxt, neg = slots[P:2 * P], slots[2 * P:]
+            else:
+                imp_items = slots[P:]
+            self._mark('compact')
+            emb, col_count = art.encode_rows(rows, T)
+            dE = torch.zeros_like(emb)
+            grad = (dE.data_ptr(), H)
+            self._mark('encode')
+        sfx = '' if art is None else '_grad'
         self._forward(b, pk, emb, items, st)
         Hs = b['Hs']
         if ib is None:
-            call('dae_seq_rank_loss', Hs.data_ptr(), H, emb.data_ptr(), emb.stride(0), H, nxt.data_ptr(), b['neg'].data_ptr(), P,
-                 1.0 / pk.terms, b['dH'].data_ptr(), H, self.stats.data_ptr(), st)
+            call('dae_seq_rank_loss' + sfx, Hs.data_ptr(), H, emb.data_ptr(), emb.stride(0), H, nxt.data_ptr(), neg.data_ptr(), P,
+                 1.0 / pk.terms, b['dH'].data_ptr(), H, self.stats.data_ptr(), *grad, st)
         elif self.impression_loss == 'softmax':
             ws = torch.empty(2 * ib.items.size, dtype=torch.int32, device=self.device)   # 8 bytes per shown article
-            call('dae_impression_softmax_loss', Hs.data_ptr(), H, emb.data_ptr(), emb.stride(0), H, pos_indptr.data_ptr(), P,
+            call('dae_impression_softmax_loss' + sfx, Hs.data_ptr(), H, emb.data_ptr(), emb.stride(0), H, pos_indptr.data_ptr(), P,
                  imp_indptr.data_ptr(), imp_items.data_ptr(), imp_clicked.data_ptr(), imp_ids.data_ptr(), self.impression_negatives,
-                 self.seed, epoch, 1.0 / ib.clicks, b['dH'].data_ptr(), H, self.stats.data_ptr(), ws.data_ptr(), st)
+                 self.seed, epoch, 1.0 / ib.clicks, b['dH'].data_ptr(), H, self.stats.data_ptr(), ws.data_ptr(), *grad, st)
         else:
-            call('dae_impression_rank_loss', Hs.data_ptr(), H, emb.data_ptr(), emb.stride(0), H, pos_indptr.data_ptr(), P,
+            call('dae_impression_rank_loss' + sfx, Hs.data_ptr(), H, emb.data_ptr(), emb.stride(0), H, pos_indptr.data_ptr(), P,
                  imp_indptr.data_ptr(), imp_items.data_ptr(), imp_clicked.data_ptr(), 1.0 / ib.n, b['dH'].data_ptr(), H,
-                 self.stats.data_ptr(), st)
+                 self.stats.data_ptr(), *grad, st)
         self._mark('loss')
         self._backward(b, pk, st)
+        if art is not None:
+            # dX = dXP . W_in[:, :H] with the forward's bf16 copy of W_in, added into the rows of the positions' articles
+            dgrad, W_in, K = self._input_grad(b)
+            dX = torch.empty(P, H, dtype=torch.float32, device=self.device)
+            self._gemm(P, H, K, dgrad, 0, W_in, 1, dX, H)
+            art.scatter_rows(dX, items, dE)
+            self._mark('input_gradient')
+            art.backward(rows, T, emb, dE, col_count)
+            self._mark('article_backward')
+            self.article_batch = {'rows': rows, 'slots': slots, 'E': emb, 'dE': dE, 'dX': dX}   # the last batch's tables, for inspection
 
     def _optimizer_step(self):
         """One dae_optimizer_step over all of theta; _step_split() names the bf16 hi / lo copy of theta's leading block that the
@@ -394,7 +444,9 @@ class _UserEncoder:
         return [perm[i:i + self.batch_users] for i in range(0, perm.size, self.batch_users)]
 
     def fit(self, sequences, embeddings, impressions=None):
-        """num_epochs epochs over the users; train_loss gets each epoch's mean loss term.  The article embeddings stay fixed.
+        """num_epochs epochs over the users; train_loss gets each epoch's mean loss term.  embeddings: the article vectors [N, H],
+        which stay fixed, or an ArticleEncoder, whose [W | bh] is trained on the same loss (DESIGN 4.19): after theta's step (and the
+        long-term rows') one optimizer step of [W | bh] with the encoder's own opt and learning rate.
 
         impressions (check_impressions' keys): train on them instead of random negatives.  Impression i of user u at time t
         scores its shown articles with h, the packed training state after u's first t reads, and its loss is
@@ -410,15 +462,21 @@ class _UserEncoder:
         over its clicks, train_loss the epoch mean over clicks, and impression_counts also gets 'clicks'.  The log must hold
         fewer than 2^32 impressions (the draws are keyed by the impression id)."""
         fn = '%s.fit' % type(self).__name__
-        emb = self._embeddings(embeddings, fn)
-        indptr, items = check_sequences(sequences, emb.shape[0], fn)
+        art = embeddings if isinstance(embeddings, ArticleEncoder) else None
+        if art is not None:
+            self._check_articles(art, fn)
+            emb, n_items = None, art.n
+        else:
+            emb = self._embeddings(embeddings, fn)
+            n_items = emb.shape[0]
+        indptr, items = check_sequences(sequences, n_items, fn)
         imp = active = use = None
         if impressions is not None:
             softmax = self.impression_loss == 'softmax'
             if softmax and _count(impressions) >= 2 ** 32:
                 raise ValueError('%s: impression_loss=\'softmax\' keys its draws by a 32-bit impression id: at most 2^32 - 1 '
                                  'impressions' % fn)
-            imp = check_impressions(impressions, emb.shape[0], fn, indptr)
+            imp = check_impressions(impressions, n_items, fn, indptr)
             use = usable_impressions(imp, indptr, self.max_len)
             active = np.unique(imp['user'][use])
             self.impression_counts = {'used': int(use.sum()), 'skipped': int(use.size - use.sum())}
@@ -440,8 +498,11 @@ class _UserEncoder:
                     n = pk.terms
                 if n == 0:   # max_len = 1
                     continue
-                self._forward_backward(pk, emb, epoch, bi, ib)
+                self._forward_backward(pk, emb, epoch, bi, ib, art)
                 self._optimizer_step()
+                if art is not None:
+                    art.step()
+                    self._mark('article_step')
                 terms += n
             self.train_loss.append(float(self.stats.item()) / max(terms, 1))
             self.epochs_done += 1
@@ -709,12 +770,12 @@ class _UserRNN(_UserEncoder):
             self._split('hh')
             self._hh_valid = True
 
-    def _forward_backward(self, pk, emb, epoch, batch, ib=None):
+    def _forward_backward(self, pk, emb, epoch, batch, ib=None, art=None):
         if self._lt is not None:   # per user of the batch: the row h_0 comes from (masked: the zero row) and the row to update (-1)
             keep = self.long_term_kept(epoch)[pk.order]
             rows = np.stack([np.where(keep, pk.order, self.long_term_users), np.where(keep, pk.order, -1)]).astype(np.int32)
             self._lt_batch = (_upload(rows, self.device), pk.B)
-        super()._forward_backward(pk, emb, epoch, batch, ib)
+        super()._forward_backward(pk, emb, epoch, batch, ib, art)
 
     def _optimizer_step(self):
         """theta's step, then with the long-term table the row step of the batch's unmasked users from dL/dh_0 (the carry)."""
@@ -770,6 +831,10 @@ class _UserRNN(_UserEncoder):
         self._gemm(GH, H + 1, P, b[self._DGRAD[0]], 1, b['Hp_hl'], 1, g_hh, H + 1, k_splits=-1)
         self._gemm(GH, H + 1, P, b[self._DGRAD[1]], 1, b['X_hl'], 1, g_ih, H + 1, k_splits=-1)
         self._mark('weight_gradients')
+
+    def _input_grad(self, b):
+        """The input projection's packed gradient, W~_ih's bf16 copy and their inner width: dX = dXP . W_ih."""
+        return b[self._DGRAD[1]], self.W_hl['ih'], self.GATES * self.dim
 
     def _step_split(self):
         hi, lo = self.W_hl['hh']
@@ -1098,6 +1163,9 @@ class UserAttention(_UserEncoder):
         for g, dA, Bop in (('in', 'dQKV_hl', 'X_hl'), ('out', 'dM_hl', 'O_hl'), ('pool', 'dZ_hl', 'M_hl')):
             self._gemm(self._rows[g], H + 1, P, b[dA], 1, b[Bop], 1, self._theta(g, self.grad), H + 1, k_splits=-1)
         self._mark('weight_gradients')
+
+    def _input_grad(self, b):
+        return b['dQKV_hl'], self.W_hl['in'], 3 * self.dim
 
     def _step_split(self):
         return None, None, 0, 0, 0

@@ -742,6 +742,41 @@ int dae_impression_metrics(const float* q, int64_t ld_q, const float* emb, int64
                            const int64_t* indptr, const int32_t* items, const uint8_t* clicked, int64_t n_imp, float* scores,
                            double* metrics, void* stream);
 
+/* ---- article encoder fine-tuned through the user encoders' losses (DESIGN 4.19) -----------------------------------------
+ * dae_encode_csr_fwd_groups: dae_encode_csr_fwd with the thread groups per row given (groups = 1 or 4) instead of chosen from
+ *   n_rows.  A row's output bits depend on the group count, the row and the parameters only, so with the count pinned a row is
+ *   bit-identical whether it is encoded alone, within a subset (rows) or within the whole set.
+ * dae_seq_rank_loss_grad, dae_impression_rank_loss_grad, dae_impression_softmax_loss_grad: the losses above with the same
+ *   arguments and the same dh, bit for bit, plus the gradient with respect to the scored rows of emb: each scored candidate j of
+ *   position p adds g_j h_p to demb row items[j] (fp32 atomics, so the sums' order depends on the schedule), where g_j is the
+ *   coefficient of e_j in dh_p.  demb [rows of emb x ld_demb] is accumulated onto, never cleared.
+ * dae_touch_compact: the compact table of the ids a batch touches.  ids [n] (n < 2^31) are row ids in [0, N) of a table of N rows,
+ *   < 0 for none.  tag (uint64 [N], zero before the first call) keeps per id the last call's stamp; stamp > 0 must grow from call to
+ *   call on the same tag, so tag is never cleared.  slot_of (int32 [N]) is scratch.  Out: T distinct ids in rows[0, T) in the order
+ *   of their first occurrence in ids, slots[i] = the slot of ids[i] in rows (-1 where ids[i] < 0) and ws[0] = T; ws holds
+ *   dae_touch_compact_workspace(n) int32 words.
+ * dae_rows_scatter_add: dst[idx[p], 0:cols] += src[p, 0:cols] for p < n with idx[p] >= 0 (fp32 atomics).
+ */
+int dae_encode_csr_fwd_groups(const int64_t* indptr, const int32_t* indices, const float* values, const int32_t* rows, int32_t n_rows,
+                              int32_t F, int32_t H, float in_scale, const float* W, const float* bh, int32_t enc_act, float* E, int64_t ldE,
+                              int32_t* col_count, void* e_hi, void* e_lo, int64_t ld_split, int32_t groups, void* stream);
+int dae_seq_rank_loss_grad(const float* h, int64_t ld_h, const float* emb, int64_t ld_emb, int32_t H, const int32_t* pos,
+                           const int32_t* neg, int64_t n_pos, float scale, float* dh, int64_t ld_dh, double* loss_sum, float* demb,
+                           int64_t ld_demb, void* stream);
+int dae_impression_rank_loss_grad(const float* h, int64_t ld_h, const float* emb, int64_t ld_emb, int32_t H, const int64_t* pos_indptr,
+                                  int64_t n_pos, const int64_t* imp_indptr, const int32_t* items, const uint8_t* clicked, float scale,
+                                  float* dh, int64_t ld_dh, double* loss_sum, float* demb, int64_t ld_demb, void* stream);
+int dae_impression_softmax_loss_grad(const float* h, int64_t ld_h, const float* emb, int64_t ld_emb, int32_t H,
+                                     const int64_t* pos_indptr, int64_t n_pos, const int64_t* imp_indptr, const int32_t* items,
+                                     const uint8_t* clicked, const int64_t* imp_ids, int32_t K, uint64_t seed, uint64_t epoch, float scale,
+                                     float* dh, int64_t ld_dh, double* loss_sum, void* workspace, float* demb, int64_t ld_demb,
+                                     void* stream);
+int dae_touch_compact_workspace(int64_t n, int64_t* count);
+int dae_touch_compact(const int32_t* ids, int64_t n, uint32_t stamp, void* tag, int32_t* slot_of, int32_t* rows, int32_t* slots,
+                      int32_t* ws, void* stream);
+int dae_rows_scatter_add(const float* src, int64_t ld_src, const int32_t* idx, int64_t n, int32_t cols, float* dst, int64_t ld_dst,
+                         void* stream);
+
 /* ---- data-parallel exchange step (SURVEY 8e): in-switch all-reduce of the flat gradient buffer -------------------
  * The reference is single-process; row-sharded training adds ONE sum over ranks of [dW | dbh | dbv] between the
  * gradient kernels and dae_optimizer_step.  Default transport: ncclAllReduce.  dae_allreduce_multimem is the

@@ -123,6 +123,14 @@ def build_parser():
     ap.add_argument('--user_long_term_lr', type=float, default=None,
                     help='with --user_long_term: the learning rate of the long-term vectors (default '
                          'user_model.LONG_TERM_LEARNING_RATE)')
+    ap.add_argument('--user_fine_tune_articles', action='store_true', default=False,
+                    help='with --user_sequences: train the DAE encoder (W, bh) together with the user encoder on its loss '
+                         '(user_model.ArticleEncoder, inputs scaled by 1 - corr_frac); save user_<cell>_article_encoder.npz and '
+                         'article_encoded_fine_tuned.npy, and score the user encoder with the fine-tuned vectors (the mean profile '
+                         'keeps the DAE\'s)')
+    ap.add_argument('--user_article_lr', type=float, default=None,
+                    help='with --user_fine_tune_articles: the article encoder\'s learning rate (default '
+                         'user_model.ARTICLE_LEARNING_RATE)')
     ap.add_argument('--user_impressions', default='',
                     help='with --user_sequences: an .npz impression log (user, time, indptr, items, clicked; see '
                          'user_model.check_impressions) to train the GRU on instead of random negatives')
@@ -213,6 +221,9 @@ def check_flags(F):
     F.user_long_term_mask = 0.5 if F.user_long_term_mask is None else F.user_long_term_mask
     assert 0.0 <= F.user_long_term_mask <= 1.0, '--user_long_term_mask must lie in [0, 1]'
     assert F.user_long_term_lr is None or F.user_long_term_lr > 0, '--user_long_term_lr must be > 0'
+    assert not F.user_fine_tune_articles or F.user_sequences, '--user_fine_tune_articles needs --user_sequences'
+    assert F.user_article_lr is None or F.user_fine_tune_articles, '--user_article_lr needs --user_fine_tune_articles'
+    assert F.user_article_lr is None or F.user_article_lr >= 0, '--user_article_lr must be >= 0'
     F.user_attention_dim = 200 if F.user_attention_dim is None else F.user_attention_dim
     assert F.user_attention_dim >= 1, '--user_attention_dim must be >= 1'
     F.user_negatives = 4 if F.user_negatives is None else F.user_negatives
@@ -537,15 +548,18 @@ def load_user_impressions(F, n_train, seqs):
     return tuple(out)
 
 
-def recommend_users_sequences(F, model, enc, seqs, impressions=(None, None)):
+def recommend_users_sequences(F, model, enc, seqs, impressions=(None, None), X=None):
     """--user_sequences: train a user encoder (--user_cell: UserGRU, UserLSTM or UserAttention) on the training embeddings, save it as
     user_<cell>.npz and the --top_k best unread articles per user as user_<cell>_top_k_{index,score}.npy; with targets, the hit
     rate and recall of the encoder's and of the mean profile's recommendations for the same reads are returned and printed.
     impressions: (train, test) from load_user_impressions; the encoder trains on train's impressions when given, and test's are
-    scored by the encoder's states and by the mean profiles of the same reads."""
+    scored by the encoder's states and by the mean profiles of the same reads.  With --user_fine_tune_articles the DAE encoder over
+    the training articles X is trained with the user encoder (user_model.ArticleEncoder), saved as user_<cell>_article_encoder.npz
+    with its vectors as article_encoded_fine_tuned.npy, and the user encoder's recommendations and impression scores use them."""
     import scipy.sparse as sp
     from dae_rnn_news_recommendation_b200 import helpers
-    from dae_rnn_news_recommendation_b200.user_model import UserAttention, UserGRU, UserLSTM, history_matrix, prefix_histories
+    from dae_rnn_news_recommendation_b200.user_model import (ArticleEncoder, UserAttention, UserGRU, UserLSTM, history_matrix,
+                                                             prefix_histories)
     indptr, items, targets = seqs
     train_imp, test_imp = impressions
     cell = F.user_cell
@@ -558,14 +572,22 @@ def recommend_users_sequences(F, model, enc, seqs, impressions=(None, None)):
     enc_cls = {'gru': UserGRU, 'lstm': UserLSTM, 'attention': UserAttention}[cell]
     rnn = enc_cls(enc.shape[1], num_epochs=F.user_epochs, seed=max(F.seed, 0), impression_loss=F.user_impression_loss,
                   impression_negatives=F.user_negatives, **kw)
-    rnn.fit((indptr, items), enc, impressions=train_imp)
+    art = enc
+    if F.user_fine_tune_articles:
+        art = ArticleEncoder(X, model.get_model_parameters(), enc_act_func=model.enc_act_func, in_scale=1.0 - F.corr_frac,
+                             learning_rate=F.user_article_lr)
+    rnn.fit((indptr, items), art, impressions=train_imp)
+    if F.user_fine_tune_articles:
+        art.save(model.data_dir + 'user_%s_article_encoder.npz' % cell)
+        art = art.vectors()
+        np.save(model.data_dir + 'article_encoded_fine_tuned', art)
     if train_imp is not None:
         print('impressions: %(used)d used, %(skipped)d skipped' % rnn.impression_counts)
         if F.user_impression_loss == 'softmax':
             print('impression loss: softmax over each click and %s of its non-clicks (%d clicks)' % (
                 'all' if F.user_negatives == 0 else 'at most %d' % F.user_negatives, rnn.impression_counts['clicks']))
     rnn.save(model.data_dir + 'user_%s.npz' % cell)
-    idx, score = rnn.recommend((indptr, items), enc, k=F.top_k, long_lists=F.long_lists)
+    idx, score = rnn.recommend((indptr, items), art, k=F.top_k, long_lists=F.long_lists)
     np.save(model.data_dir + 'user_%s_top_k_index' % cell, idx)
     np.save(model.data_dir + 'user_%s_top_k_score' % cell, score)
     out = {'user_%s_train_loss' % cell: rnn.train_loss[-1] if rnn.train_loss else float('nan')}
@@ -581,7 +603,7 @@ def recommend_users_sequences(F, model, enc, seqs, impressions=(None, None)):
         print('users (%s): hit rate@%d %.4f recall@%d %.4f; mean profile: hit rate@%d %.4f recall@%d %.4f (%d users with targets)'
               % (label, F.top_k, r['hit_rate'], F.top_k, r['recall'], F.top_k, m['hit_rate'], F.top_k, m['recall'], r['users']))
     if test_imp is not None:
-        g = helpers.impression_metrics(rnn.impression_states((indptr, items), enc, test_imp), enc, test_imp, metric='linear kernel')
+        g = helpers.impression_metrics(rnn.impression_states((indptr, items), art, test_imp), art, test_imp, metric='linear kernel')
         prof = helpers.user_profiles(prefix_histories((indptr, items), test_imp, enc.shape[0]), enc)
         m = helpers.impression_metrics(prof, enc, test_imp, metric='cosine')
         for name, r in ((cell, g), ('mean', m)):
@@ -634,7 +656,7 @@ def main(argv=None):
         if histories is not None:
             model.evaluation.update(recommend_users(F, model, enc, histories, targets))
         if seqs is not None:
-            model.evaluation.update(recommend_users_sequences(F, model, enc, seqs, imps))
+            model.evaluation.update(recommend_users_sequences(F, model, enc, seqs, imps, X=trX))
         if F.top_k_dedup > 0:
             model.evaluation.update(recommend_top_k_dedup(F, model, enc, enc_v, trL, vlL, histories, targets, model.evaluation))
     if F.dedup_threshold > 0:
