@@ -125,6 +125,10 @@ _SIGNATURES = {
     'dae_touch_compact_workspace': (C.c_int, [i64, p]),
     'dae_touch_compact': (C.c_int, [p, i64, C.c_uint32, p, p, p, p, p, p]),
     'dae_rows_scatter_add': (C.c_int, [p, i64, p, i64, i32, p, i64, p]),
+    # bag-of-words user profiles
+    'dae_csr_profiles_count': (C.c_int, [p, p, i32, i32, p, p, i32, p, p]),
+    'dae_csr_profiles': (C.c_int, [p, p, p, i32, i32, p, p, p, i32, p, i32, i32, i32, p, p, p]),
+    'dae_csr_impression_metrics': (C.c_int, [p, p, p, p, p, p, i32, i32, i32, p, p, p, i64, p, p, p]),
     # deterministic training step
     'dae_gemm_det_workspace': (C.c_int, [p]),
     'dae_gemm_bf16x3_det': (C.c_int, [i32, i32, i32, f32, p, p, i64, i32, p, p, i64, i32, p, i64, i32, i32, p, i32, i32, p, i64, p]),

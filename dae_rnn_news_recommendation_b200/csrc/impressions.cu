@@ -5,11 +5,11 @@
 // one warp to one row of work and score the candidates with warp dot products (lane j takes the columns j, j + 32, ...), so a
 // candidate list of any length is walked in chunks of kImpChunk scores held in shared memory per warp.
 #include "common.cuh"
+#include "impression_rank.cuh"
 
 namespace dae {
 
 constexpr int kImpWarps = 4;
-constexpr int kImpChunk = 256;
 
 // sigma(x) with the approximate divide (2 ulp, no slow-path subroutine: the pair loop keeps its state in registers)
 __device__ __forceinline__ float imp_sigmoid(float x) { return __fdividef(1.0f, 1.0f + expf(-x)); }
@@ -26,25 +26,6 @@ __device__ __forceinline__ float warp_dot(const float* __restrict__ a, const flo
 #pragma unroll 1   // unrolled, the loss kernel's nested loops spill to local memory
   for (int j = lane; j < H; j += 32) s = fmaf(a[j], b[j], s);
   return warp_sum(s);
-}
-
-__device__ __forceinline__ int warp_sum_int(int v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-
-__device__ __forceinline__ long long warp_sum_ll(long long v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-
-// Clicked count of one impression's flags [0, m).
-__device__ __forceinline__ int count_clicked(const uint8_t* __restrict__ c, int64_t m, int lane) {
-  int n = 0;
-  for (int64_t k = lane; k < m; k += 32) n += c[k] != 0;
-  return warp_sum_int(n);
 }
 
 // Scores h . e(items[k]) of candidates [k0, k0 + n) into s[0, n) and their click flags into f[0, n) (shared, one warp).
@@ -141,9 +122,7 @@ __global__ void __launch_bounds__(kImpWarps * 32) impression_rank_loss_kernel(
 }
 
 // One warp per impression i: scores[k] = q_i . e(items[k]) (cosine: divided by |q_i| |e|, 0 when either is zero) for every k in
-// [indptr[i], indptr[i + 1]), then metrics[i] = (AUC, MRR, nDCG@5, nDCG@10) from those fp32 scores.  rank_j = #{k: s_k > s_j}
-// + #{k < j: s_k = s_j}.  The clicked candidates are taken 32 at a time, one per lane, against the whole list staged kImpChunk
-// scores at a time in shared memory: O(|C| m) comparisons, the AUC counted in integers.  No click or no non-click: NaN x 4.
+// [indptr[i], indptr[i + 1]), then metrics[i] = (AUC, MRR, nDCG@5, nDCG@10) from those fp32 scores (impression_rank_metrics).
 __global__ void __launch_bounds__(kImpWarps * 32) impression_metrics_kernel(
     const float* __restrict__ qv, int64_t ld_q, const float* __restrict__ emb, int64_t ld_emb, int H, int cosine,
     const int64_t* __restrict__ indptr, const int32_t* __restrict__ items, const uint8_t* __restrict__ clicked, int64_t n_imp,
@@ -173,68 +152,7 @@ __global__ void __launch_bounds__(kImpWarps * 32) impression_metrics_kernel(
       if (lane == 0) scores[b0 + k] = s;
     }
     __syncwarp();   // the scores written by lane 0 are read by every lane below
-    const int nc = count_clicked(clicked + b0, m, lane);
-    const int64_t nn = m - nc;
-    double* out = metrics + i * 4;
-    if (nc == 0 || nn == 0) {
-      if (lane < 4) out[lane] = __longlong_as_double(0x7ff8000000000000LL);
-      continue;
-    }
-    long long auc2 = 0;
-    double rr = 0.0, g5 = 0.0, g10 = 0.0;
-    for (int64_t j0 = 0; j0 < m; j0 += 32) {
-      const int64_t j = j0 + lane;
-      const bool mine = j < m && clicked[b0 + j] != 0;
-      if (!__any_sync(0xffffffffu, mine)) continue;
-      const float sj = mine ? scores[b0 + j] : 0.0f;
-      long long gt = 0, tie_before = 0, below_n = 0, tie_n = 0;
-      for (int64_t k0 = 0; k0 < m; k0 += kImpChunk) {
-        const int nk = (int)min((int64_t)kImpChunk, m - k0);
-        __syncwarp();
-        for (int t = lane; t < nk; t += 32) {
-          s_s[w][t] = scores[b0 + k0 + t];
-          s_f[w][t] = clicked[b0 + k0 + t] != 0;
-        }
-        __syncwarp();
-        if (mine) {
-          for (int t = 0; t < nk; ++t) {
-            const float sk = s_s[w][t];
-            gt += sk > sj;
-            tie_before += (sk == sj) && (k0 + t < j);
-            if (!s_f[w][t]) {
-              below_n += sk < sj;
-              tie_n += sk == sj;
-            }
-          }
-        }
-      }
-      if (mine) {
-        const long long rank = gt + tie_before;
-        auc2 += 2 * below_n + tie_n;
-        rr += 1.0 / (double)(rank + 1);
-        if (rank < 10) {
-          const double g = 1.0 / log2((double)(rank + 2));
-          g10 += g;
-          if (rank < 5) g5 += g;
-        }
-      }
-    }
-    auc2 = warp_sum_ll(auc2);
-    rr = warp_sum(rr);
-    g5 = warp_sum(g5);
-    g10 = warp_sum(g10);
-    if (lane == 0) {
-      double i5 = 0.0, i10 = 0.0;
-      for (int r = 0; r < 10 && r < nc; ++r) {
-        const double g = 1.0 / log2((double)(r + 2));
-        i10 += g;
-        if (r < 5) i5 += g;
-      }
-      out[0] = (double)auc2 / (2.0 * (double)nc * (double)nn);
-      out[1] = rr / (double)nc;
-      out[2] = g5 / i5;
-      out[3] = g10 / i10;
-    }
+    impression_rank_metrics(scores, clicked, b0, m, s_s[w], s_f[w], metrics + i * 4, lane);
   }
 }
 

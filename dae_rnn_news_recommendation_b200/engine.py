@@ -73,6 +73,15 @@ class DeviceCSR:
         self.values = va.to(device, non_blocking=True)
 
     @staticmethod
+    def from_tensors(indptr, indices, values, shape):
+        """A DeviceCSR over device tensors that already hold a canonical CSR (int64 indptr, int32 indices, fp32 values)."""
+        m = DeviceCSR.__new__(DeviceCSR)
+        m.shape, m.nnz, m.h2d_bytes = tuple(shape), int(indices.numel()), 0
+        m.max_row_nnz = int((indptr[1:] - indptr[:-1]).max()) if shape[0] else 0
+        m.indptr, m.indices, m.values = indptr, indices, values
+        return m
+
+    @staticmethod
     def vstack(mats, device):
         return DeviceCSR(sp.vstack([canonical_csr(m) for m in mats]).tocsr(), device)
 

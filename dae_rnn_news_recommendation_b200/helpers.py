@@ -10,6 +10,9 @@ nearest-article lookup of main_autoencoder.py:307-318,352-359) -- SURVEY section
                                                                                                         at most one row per group)
     label_precision_at_k(index, query_labels, corpus_labels) -> float                                 (share of same-label neighbours)
     user_profiles(histories, embeddings) -> [U, H]                                                    (weighted mean of the read articles)
+    sparse_profiles(histories, X) -> scipy CSR [U, F]                                                 (the same of the bag of words)
+    recommend_sparse(histories, X, k=10, candidates=None, exclude_read=True, groups=None) -> (index[U, k], score[U, k])
+                                                                                                      (recommend from sparse_profiles)
     recommend(histories, embeddings, k=10, candidates=None, exclude_read=True, profiles=None, groups=None)
                                                                                    -> (index[U, k], score[U, k])
                                                                                                       (k best unread articles per user;
@@ -19,6 +22,7 @@ nearest-article lookup of main_autoencoder.py:307-318,352-359) -- SURVEY section
     recommendation_recall(index, targets) -> dict                                                     (hit rate / recall of held-out reads)
     impression_metrics(vectors, embeddings, impressions, metric='linear kernel') -> dict              (AUC / MRR / nDCG@5, @10 per
                                                                                                         impression, averaged)
+    impression_metrics_sparse(profiles, X, impressions, metric='linear kernel') -> dict               (the same for sparse query rows)
     similar_pairs(data, threshold, corpus=None, metric='cosine') -> (i[P], j[P], score[P])            (every pair with score >= threshold,
                                                                                                         near-duplicates; no matrix)
     duplicate_groups(i, j, n) -> group[n]                                                             (connected components of the pairs)
@@ -616,6 +620,151 @@ def _recommend_topk(prof, corpus, k, metric, lists, splits=0, groups=None, max_c
     return _similarity_topk(q, c, prof.shape[0], corpus.shape[0], prof.shape[1], k, splits=splits, lists=lists, groups=groups)
 
 
+SPARSE_PROFILE_CHUNK_NNZ = 1 << 27   # recommend_sparse: profile entries filled and ranked at once (8 B each: 1 GB)
+PROFILE_MAX_FEATURES = 1 << 24       # the profile kernels' column limit
+
+
+def _data_ptr(t):
+    """device pointer of a tensor, NULL when it holds nothing (the CSR exports accept NULL indices / values then)"""
+    return t.data_ptr() if t.numel() else None
+
+
+def _sparse_articles(X, fn):
+    """X as the canonical fp32 CSR the profile kernels read: ValueError unless X is a scipy sparse matrix [N, F] with N >= 1 and
+    1 <= F <= 2^24."""
+    if not sp.issparse(X):
+        raise ValueError('%s: X must be a scipy sparse matrix [N, F] (the articles\' bag of words), not %s' % (fn, type(X).__name__))
+    if len(X.shape) != 2 or X.shape[0] < 1 or not 1 <= X.shape[1] <= PROFILE_MAX_FEATURES:
+        raise ValueError('%s: X has shape %s, [N, F] with N >= 1 and 1 <= F <= 2^24 expected' % (fn, tuple(X.shape)))
+    return canonical_csr(X).astype(np.float32)
+
+
+def _profile_weights(histories, m, fn):
+    """_history_weights for the profile kernels, with at least one user."""
+    w, empty = _history_weights(histories, m.shape[0], fn)
+    if w.shape[0] < 1:
+        raise ValueError('%s: histories hold no user' % fn)
+    return w, empty
+
+
+def _profile_structure(hist, x):
+    """dae_csr_profiles_count: the row pointers int64 [U + 1] of the profiles hist.X, on the device (DeviceCSR operands)."""
+    n_u, n = hist.shape
+    p_indptr = torch.empty(n_u + 1, dtype=torch.int64, device=hist.indptr.device)
+    call('dae_csr_profiles_count', hist.indptr.data_ptr(), _data_ptr(hist.indices), n_u, n, x.indptr.data_ptr(), _data_ptr(x.indices),
+         x.shape[1], p_indptr.data_ptr(), _stream())
+    return p_indptr
+
+
+def _profile_rows(hist, x, p_indptr, p_host, u0, u1, normalise):
+    """dae_csr_profiles: the profile rows [u0, u1) (L2-normalised with `normalise`) as a DeviceCSR.  p_indptr: the row pointers on
+    the device, p_host: their host copy."""
+    dev = hist.indptr.device
+    base, nnz = int(p_host[u0]), int(p_host[u1] - p_host[u0])
+    indices = torch.empty(nnz, dtype=torch.int32, device=dev)
+    values = torch.empty(nnz, dtype=torch.float32, device=dev)
+    call('dae_csr_profiles', hist.indptr.data_ptr(), _data_ptr(hist.indices), _data_ptr(hist.values), hist.shape[0], hist.shape[1],
+         x.indptr.data_ptr(), _data_ptr(x.indices), _data_ptr(x.values), x.shape[1], p_indptr.data_ptr(), u0, u1 - u0,
+         1 if normalise else 0, _data_ptr(indices), _data_ptr(values), _stream())
+    return DeviceCSR.from_tensors(p_indptr[u0:u1 + 1] - base, indices, values, (u1 - u0, x.shape[1]))
+
+
+def _profile_chunks(p_indptr, budget):
+    """recommend_sparse's user chunks: consecutive ranges [u0, u1) covering every user, each as long as its profiles hold at most
+    `budget` entries together; a user over the budget gets a range of its own.  p_indptr: the host row pointers."""
+    n_u, out, u0 = len(p_indptr) - 1, [], 0
+    while u0 < n_u:
+        u1 = int(np.searchsorted(p_indptr, p_indptr[u0] + budget, side='right')) - 1
+        u1 = min(max(u1, u0 + 1), n_u)
+        out.append((u0, u1))
+        u0 = u1
+    return out
+
+
+def sparse_profiles(histories, X, device='cuda:0', to_host=True):
+    """Bag-of-words user profiles: row u is the weighted mean of the rows of X (the articles' binary / tf-idf vectors, scipy
+    sparse [N, F], F <= 2^24) that user u read, with the weights of user_profiles (histories: scipy sparse [U, N], normalised per
+    user; a user whose weights sum to 0 gets an empty row).  The sparse x sparse product runs on the GPU (dae_csr_profiles_count,
+    then dae_csr_profiles) without a dense [U, F] buffer: row u stores the union of the columns of the rows read, explicit zeros
+    included, in increasing order, and each value is the fp32 sum of the rounded products w.x in increasing article order.
+    Returns a canonical scipy CSR [U, F] fp32, or an engine.DeviceCSR with to_host=False (impression_metrics_sparse takes both)."""
+    m = _sparse_articles(X, 'sparse_profiles')
+    w, _ = _profile_weights(histories, m, 'sparse_profiles')
+    hist, x = DeviceCSR(w, device), DeviceCSR(m, device)
+    p_indptr = _profile_structure(hist, x)
+    p_host = p_indptr.cpu().numpy()
+    out = _profile_rows(hist, x, p_indptr, p_host, 0, w.shape[0], False)
+    if not to_host:
+        return out
+    return sp.csr_matrix((out.values.cpu().numpy(), out.indices.cpu().numpy(), p_host), shape=out.shape)
+
+
+def recommend_sparse(histories, X, k=10, candidates=None, metric='cosine', exclude_read=True, groups=None, device='cuda:0',
+                     to_host=True):
+    """recommend for bag-of-words profiles: for every user the k best articles by `metric` between the user's sparse_profiles row
+    and the rows of X (scipy sparse [N, F]), ranked by the sparse top-k kernel (dae_csr_similarity_topk*): the content-based
+    baseline of the learned user vectors.  'cosine' ranks the L2-normalised profiles (dae_csr_profiles' normalise) against
+    the L2-normalised rows of X (as top_k_similar does), 'linear kernel' the plain ones.  Order, ties, padding (-1 / -inf for a
+    user whose weights sum to 0), exclude_read, candidates and groups as in recommend.  1 <= k <= 32 (ValueError otherwise).
+    The profiles are counted once for all users, then filled and ranked in chunks of users holding at most SPARSE_PROFILE_CHUNK_NNZ
+    profile entries (a single larger user is a chunk of its own), so they are never all resident.  The result does not depend on
+    the chunks.  Returns (index int32 [U, k], score float32 [U, k]) as ndarrays (device tensors with to_host=False)."""
+    if metric not in ('cosine', 'linear kernel'):
+        raise ValueError("recommend_sparse: metric = %r: 'cosine' or 'linear kernel'" % (metric,))
+    if isinstance(k, bool) or not isinstance(k, (int, np.integer)) or not 1 <= k <= TOPK_MAX_K:
+        raise ValueError('recommend_sparse: k = %r is outside the supported range 1 <= k <= %d (sparse profiles rank at most %d)'
+                         % (k, TOPK_MAX_K, TOPK_MAX_K))
+    k = int(k)
+    m = _sparse_articles(X, 'recommend_sparse')
+    n_art = m.shape[0]
+    w, empty = _profile_weights(histories, m, 'recommend_sparse')
+    cand = None if candidates is None else _candidate_rows(candidates, n_art, 'recommend_sparse')
+    g = None if groups is None else _group_labels(groups, n_art, 'recommend_sparse')
+    lists_host = None
+    if exclude_read and cand is not None and g is None:
+        lists_host = _remap_lists(w.indptr, w.indices, cand)
+    corpus_host = _csr_operand(m, metric)
+    if cand is not None:
+        corpus_host = corpus_host[cand]
+    hist, x, corpus = DeviceCSR(w, device), DeviceCSR(m, device), DeviceCSR(corpus_host, device)
+    cand_dev = None if cand is None else torch.from_numpy(cand).to(device)
+    g_dev = cg_dev = None
+    if g is not None:
+        g_dev = torch.from_numpy(g).to(device)
+        cg_dev = g_dev if cand_dev is None else g_dev.index_select(0, cand_dev)
+    lists = None
+    if exclude_read and g is not None:
+        ptr, ind = _read_group_lists(hist.indptr, hist.indices, g_dev, cg_dev)
+        lists = _DeviceLists(ptr, ind, ind.numel())
+    elif exclude_read:
+        lists = _DeviceLists(hist.indptr, hist.indices, hist.nnz) if cand is None else _DeviceLists.from_host(*lists_host, device)
+    n_u = w.shape[0]
+    idx = torch.empty(n_u, k, dtype=torch.int32, device=device)
+    val = torch.empty(n_u, k, dtype=torch.float32, device=device)
+    p_indptr = _profile_structure(hist, x)
+    p_host = p_indptr.cpu().numpy()
+    l_host = None if lists is None else lists.indptr.cpu().numpy()
+    for u0, u1 in _profile_chunks(p_host, SPARSE_PROFILE_CHUNK_NNZ):
+        q = _profile_rows(hist, x, p_indptr, p_host, u0, u1, metric == 'cosine')
+        chunk_lists = None
+        if lists is not None:
+            a, b = int(l_host[u0]), int(l_host[u1])
+            chunk_lists = _DeviceLists(lists.indptr[u0:u1 + 1] - a, lists.indices[a:b], b - a)
+        i, v = _csr_similarity_topk(q, corpus, k, lists=chunk_lists, groups=cg_dev)
+        idx[u0:u1] = i
+        val[u0:u1] = v
+        del q
+    if empty.any():
+        e = torch.from_numpy(empty).to(device)
+        idx[e] = -1
+        val[e] = float('-inf')
+    if cand_dev is not None:
+        idx = torch.where(idx >= 0, cand_dev[idx.clamp(min=0).long()].int(), idx)
+    if to_host:
+        return idx.cpu().numpy(), val.cpu().numpy()
+    return idx, val
+
+
 def recommendation_recall(index, targets):
     """How many held-out reads (e.g. each user's last click) the recommendations find, on the host.  index [U, k] (recommend's
     output, -1 = padding, never a hit); targets: scipy sparse [U, N] whose stored positions are the held-out articles.  Users
@@ -687,11 +836,68 @@ def impression_metrics(vectors, embeddings, impressions, metric='linear kernel',
     if float(emb.abs().max()) > lim or (q.numel() and float(q.abs().max()) > lim):
         raise ValueError('impression_metrics: embeddings and vectors must lie within 2^63 / sqrt(H) = %.3g in magnitude' % lim)
     _, m = _impression_scores(q, emb, imp, metric)
-    m = m.cpu().numpy()
+    return _impression_means(m.cpu().numpy(), n_imp)
+
+
+def _impression_means(m, n_imp):
+    """impression_metrics' dict from the per-impression metrics m [I, 4] (NaN rows: impressions left out)."""
     ok = ~np.isnan(m[:, 0])
     mean = m[ok].mean(0) if ok.any() else np.full(4, np.nan)
     return {'impressions': int(ok.sum()), 'skipped': int(n_imp - ok.sum()), 'auc': float(mean[0]), 'mrr': float(mean[1]),
             'ndcg@5': float(mean[2]), 'ndcg@10': float(mean[3])}
+
+
+def _csr_impression_scores(q, x, imp, metric):
+    """dae_csr_impression_metrics on DeviceCSR operands: (scores fp32 [nnz], metrics fp64 [I, 4]) as device tensors."""
+    n_imp, d = q.shape[0], x.indptr.device
+    scores = torch.empty(imp['items'].size, dtype=torch.float32, device=d)
+    metrics = torch.full((n_imp, 4), float('nan'), dtype=torch.float64, device=d)
+    if n_imp == 0 or imp['items'].size == 0:
+        return scores, metrics
+    indptr = torch.from_numpy(imp['indptr']).to(d)
+    items = torch.from_numpy(imp['items']).to(d)
+    clicked = torch.from_numpy(imp['clicked']).to(d)
+    call('dae_csr_impression_metrics', q.indptr.data_ptr(), _data_ptr(q.indices), _data_ptr(q.values), x.indptr.data_ptr(),
+         _data_ptr(x.indices), _data_ptr(x.values), x.shape[0], x.shape[1], int(metric == 'cosine'), indptr.data_ptr(),
+         items.data_ptr(), clicked.data_ptr(), n_imp, scores.data_ptr(), metrics.data_ptr(), _stream())
+    return scores, metrics
+
+
+def impression_metrics_sparse(profiles, X, impressions, metric='linear kernel', device='cuda:0'):
+    """impression_metrics for bag-of-words query rows: impression i's shown articles (rows of X, scipy sparse [N, F]) are scored
+    against row i of `profiles` -- a scipy sparse [I, F] or sparse_profiles(..., to_host=False), e.g.
+    sparse_profiles(user_model.prefix_histories(sequences, impressions, N), X) -- and ranked as impression_metrics ranks them.
+    'linear kernel': the fp32 sum of the rounded products over the shared columns in increasing column order (the sparse top-k's
+    score of the pair, bit for bit); 'cosine': that over sqrt(qq) sqrt(ee), the squared norms summed the same way, 0 when either
+    is 0.  The metrics come from the same device code as impression_metrics' (dae_csr_impression_metrics).  Both matrices must be
+    finite with every |x| <= 2^63 / sqrt(F) (ValueError otherwise, before any device work).  Returns impression_metrics' dict."""
+    from .user_model import check_impressions
+    fn = 'impression_metrics_sparse'
+    if metric not in ('cosine', 'linear kernel'):
+        raise ValueError("%s: metric = %r: 'cosine' or 'linear kernel'" % (fn, metric))
+    m = _sparse_articles(X, fn)
+    imp = check_impressions(impressions, m.shape[0], fn)
+    n_imp, n_f = imp['indptr'].size - 1, m.shape[1]
+    if not (isinstance(profiles, DeviceCSR) or sp.issparse(profiles)):
+        raise ValueError('%s: profiles must be a scipy sparse matrix or sparse_profiles(..., to_host=False), not %s'
+                         % (fn, type(profiles).__name__))
+    if tuple(profiles.shape) != (n_imp, n_f):
+        raise ValueError('%s: profiles have shape %s, [%d, %d] (impressions x features) expected' % (fn, tuple(profiles.shape), n_imp, n_f))
+    q_host = None if isinstance(profiles, DeviceCSR) else canonical_csr(profiles).astype(np.float32)
+    # |x| <= 2^63 / sqrt(F) keeps every fp32 dot product and squared norm of the kernel below 2^126: no inf, so no NaN score
+    lim = 2.0 ** 63 / math.sqrt(n_f)
+    if q_host is not None:
+        q_ok = bool(np.isfinite(q_host.data).all()) and (q_host.nnz == 0 or float(np.abs(q_host.data).max()) <= lim)
+    else:
+        v = profiles.values
+        q_ok = bool(torch.isfinite(v).all()) and (v.numel() == 0 or float(v.abs().max()) <= lim)
+    x_ok = bool(np.isfinite(m.data).all()) and (m.nnz == 0 or float(np.abs(m.data).max()) <= lim)
+    if not (q_ok and x_ok):
+        raise ValueError('%s: X and profiles must be finite and lie within 2^63 / sqrt(F) = %.3g in magnitude' % (fn, lim))
+    x = DeviceCSR(m, device)
+    q = profiles if q_host is None else DeviceCSR(q_host, device)
+    _, mt = _csr_impression_scores(q, x, imp, metric)
+    return _impression_means(mt.cpu().numpy(), n_imp)
 
 
 def label_precision_at_k(index, query_labels, corpus_labels):

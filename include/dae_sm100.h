@@ -777,6 +777,38 @@ int dae_touch_compact(const int32_t* ids, int64_t n, uint32_t stamp, void* tag, 
 int dae_rows_scatter_add(const float* src, int64_t ld_src, const int32_t* idx, int64_t n, int32_t cols, float* dst, int64_t ld_dst,
                          void* stream);
 
+/* ---- bag-of-words user profiles and their impression metrics (DESIGN 4.20) --------------------------------------------------
+ * The history W [n_users x n_articles] and the articles X [n_articles x n_features] are CSR matrices: indptr int64, indices int32
+ * strictly increasing inside a row (sorted, no duplicates), values fp32; the kernels do not check the contents.  The profiles
+ * P = W.X are the CSR matrix whose row u holds the union of the stored columns of every row of X that row u of W stores (explicit
+ * zero weights and explicit zero entries included).  Memory is O(nnz(P)): never n_users x n_features.  1 <= n_features <= 2^24.
+ * dae_csr_profiles_count: p_indptr (int64 [n_users + 1]) = the complete row pointers of P: p_indptr[0] = 0 and p_indptr[u + 1] -
+ *   p_indptr[u] = the column count of row u.  One pass over every user; w_indices / x_indices may be NULL when W / X store nothing.
+ * dae_csr_profiles: rows [first_user, first_user + n_fill) of P (n_fill >= 1), with p_indptr from dae_csr_profiles_count.  Entry t
+ *   of row u goes to p_indices / p_values[p_indptr[u] - p_indptr[first_user] + t], the columns increasing within the row, so a
+ *   caller can fill and use P a range of users at a time.  P[u, f] accumulates in fp32 from +0, one term per entry of row u of W
+ *   in increasing article order, each term __fmul_rn(w, x) added with __fadd_rn (no FMA): the values do not depend on the launch
+ *   shape or the range, and a float32 host loop reproduces them bit for bit.  normalise = 1 then divides each row by its L2 norm:
+ *   n^2 = the fp32 sum of the rounded squares in increasing column order, v = __fdiv_rn(v, __fsqrt_rn(n^2)); a row with n^2 = 0 is
+ *   left as it is.  Any user may read any number of articles.
+ * dae_csr_impression_metrics: dae_impression_metrics for CSR query rows (q_indptr [n_imp + 1], row i the query of impression i)
+ *   against the articles' CSR X (x_indptr [n_articles + 1], items in [0, n_articles)), columns < n_features in both.  scores[k] =
+ *   q_i . x(items[k]): the fp32 sum from +0 of the rounded products over the shared columns in increasing column order, the score
+ *   dae_csr_similarity_topk gives the same pair, bit for bit.  cosine = 1: dot / (sqrt(qq) sqrt(ee)), qq and ee the fp32 sums of
+ *   the rounded squares of the rows in increasing column order, every operation IEEE-rounded; 0 when qq or ee is 0.  metrics as in
+ *   dae_impression_metrics (the same device code).  q / x indices and values may be NULL when the matrix stores nothing.
+ */
+int dae_csr_profiles_count(const int64_t* w_indptr, const int32_t* w_indices, int32_t n_users, int32_t n_articles,
+                           const int64_t* x_indptr, const int32_t* x_indices, int32_t n_features, int64_t* p_indptr, void* stream);
+int dae_csr_profiles(const int64_t* w_indptr, const int32_t* w_indices, const float* w_values, int32_t n_users, int32_t n_articles,
+                     const int64_t* x_indptr, const int32_t* x_indices, const float* x_values, int32_t n_features,
+                     const int64_t* p_indptr, int32_t first_user, int32_t n_fill, int32_t normalise, int32_t* p_indices,
+                     float* p_values, void* stream);
+int dae_csr_impression_metrics(const int64_t* q_indptr, const int32_t* q_indices, const float* q_values, const int64_t* x_indptr,
+                               const int32_t* x_indices, const float* x_values, int32_t n_articles, int32_t n_features, int32_t cosine,
+                               const int64_t* indptr, const int32_t* items, const uint8_t* clicked, int64_t n_imp, float* scores,
+                               double* metrics, void* stream);
+
 /* ---- data-parallel exchange step (SURVEY 8e): in-switch all-reduce of the flat gradient buffer -------------------
  * The reference is single-process; row-sharded training adds ONE sum over ranks of [dW | dbh | dbv] between the
  * gradient kernels and dae_optimizer_step.  Default transport: ncclAllReduce.  dae_allreduce_multimem is the

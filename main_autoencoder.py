@@ -144,6 +144,13 @@ def build_parser():
     ap.add_argument('--user_test_impressions', default='',
                     help='with --user_sequences: an .npz impression log to score; report the AUC, MRR, nDCG@5 and nDCG@10 of the '
                          'GRU states (user_gru_imp_*) and of the mean profile of the same reads (user_mean_imp_*)')
+    ap.add_argument('--user_top_k_input', action='store_true', default=False,
+                    help='with --top_k K (1..32) and --user_histories or --user_sequences: also recommend from the bag-of-words '
+                         'profiles of the same reads (helpers.recommend_sparse; cosine for binary, linear kernel for tf-idf, as '
+                         '--top_k_input); with --user_histories save user_top_k_input_{index,score}.npy and report '
+                         'user_input_hit_rate / user_input_recall, with --user_sequences report user_input_seq_hit_rate / '
+                         '_recall and, with --user_test_impressions, user_input_imp_* next to the user encoder\'s and the mean '
+                         'profile\'s')
     ap.add_argument('--user_targets', default='',
                     help='with --user_histories: a save_npz matrix of the same shape holding held-out reads; report the hit rate '
                          'and recall of the recommendations against them (user_hit_rate, user_recall)')
@@ -230,6 +237,9 @@ def check_flags(F):
     assert 0 <= F.user_negatives <= 32, '--user_negatives %d: 0 <= K <= 32' % F.user_negatives
     assert not F.user_targets or F.user_histories, '--user_targets needs --user_histories'
     assert not F.user_targets or os.path.isfile(F.user_targets), '--user_targets %s: no such file' % F.user_targets
+    assert not F.user_top_k_input or 1 <= F.top_k <= 32, '--user_top_k_input needs --top_k K in 1..32'
+    assert not F.user_top_k_input or F.user_histories or F.user_sequences, \
+        '--user_top_k_input needs --user_histories or --user_sequences'
     if F.input_format == 'tfidf':
         assert F.loss_func in ['mean_squared', 'cosine_proximity']
     if F.main_dir == '':
@@ -525,6 +535,65 @@ def recommend_users(F, model, enc, histories, targets):
     return out
 
 
+def recommend_users_input(F, model, trX, histories, targets, emb_out):
+    """--user_top_k_input with --user_histories: the --top_k best unread training articles of every user from the bag-of-words
+    profile of the articles read (helpers.recommend_sparse, with --top_k_input's metric), saved under data_dir as
+    user_top_k_input_{index,score}.npy; with --user_targets the hit rate and recall are returned and printed next to the
+    embedding profile's (emb_out)."""
+    from dae_rnn_news_recommendation_b200 import helpers
+    in_metric = 'cosine' if F.input_format == 'binary' else 'linear kernel'
+    print('recommend %d unread articles to %d users from their input vectors (%s)' % (F.top_k, histories.shape[0], in_metric))
+    idx, score = helpers.recommend_sparse(histories, trX, k=F.top_k, metric=in_metric)
+    np.save(model.data_dir + 'user_top_k_input_index', idx)
+    np.save(model.data_dir + 'user_top_k_input_score', score)
+    out = {}
+    if targets is not None:
+        r = helpers.recommendation_recall(idx, targets)
+        out = {'user_input_hit_rate': r['hit_rate'], 'user_input_recall': r['recall']}
+        print('users: hit rate@%d embedding %.4f input vectors %.4f; recall@%d embedding %.4f input vectors %.4f (%d users with '
+              'targets)' % (F.top_k, emb_out.get('user_hit_rate', float('nan')), r['hit_rate'], F.top_k,
+                            emb_out.get('user_recall', float('nan')), r['recall'], r['users']))
+    return out
+
+
+def recommend_users_sequences_input(F, trX, seqs, impressions, emb_out):
+    """--user_top_k_input with --user_sequences: the bag-of-words baseline of the sequence users.  With targets, the hit rate and
+    recall of helpers.recommend_sparse over each user's reads (user_input_seq_*); with --user_test_impressions, the impression
+    metrics of the bag-of-words profiles of the reads before each impression (helpers.impression_metrics_sparse, user_input_imp_*).
+    Printed next to the user encoder's and the mean profile's (emb_out)."""
+    import scipy.sparse as sp
+    from dae_rnn_news_recommendation_b200 import helpers
+    from dae_rnn_news_recommendation_b200.user_model import history_matrix, prefix_histories
+    indptr, items, targets = seqs
+    in_metric = 'cosine' if F.input_format == 'binary' else 'linear kernel'
+    cell = F.user_cell
+    out = {}
+    if targets is not None:
+        n_u, n = len(indptr) - 1, trX.shape[0]
+        has = targets >= 0
+        tg = sp.csr_matrix((np.ones(int(has.sum()), np.float32), (np.flatnonzero(has), targets[has])), shape=(n_u, n))
+        idx, _ = helpers.recommend_sparse(history_matrix(indptr, items, n), trX, k=F.top_k, metric=in_metric)
+        r = helpers.recommendation_recall(idx, tg)
+        out.update({'user_input_seq_hit_rate': r['hit_rate'], 'user_input_seq_recall': r['recall']})
+        print('users: hit rate@%d %s %.4f mean profile %.4f input vectors %.4f; recall@%d %s %.4f mean profile %.4f input vectors '
+              '%.4f (%d users with targets)' % (
+                  F.top_k, cell.upper(), emb_out.get('user_%s_hit_rate' % cell, float('nan')),
+                  emb_out.get('user_mean_hit_rate', float('nan')), r['hit_rate'], F.top_k, cell.upper(),
+                  emb_out.get('user_%s_recall' % cell, float('nan')), emb_out.get('user_mean_recall', float('nan')), r['recall'],
+                  r['users']))
+    test_imp = impressions[1]
+    if test_imp is not None:
+        prof = helpers.sparse_profiles(prefix_histories((indptr, items), test_imp, trX.shape[0]), trX, to_host=False)
+        m = helpers.impression_metrics_sparse(prof, trX, test_imp, metric=in_metric)
+        out.update({'user_input_imp_%s' % k.replace('@', ''): m[k] for k in ('auc', 'mrr', 'ndcg@5', 'ndcg@10')})
+        nan = float('nan')
+        print('test impressions: ' + '; '.join(
+            '%s %s %.4f mean profile %.4f input vectors %.4f' % (
+                name, cell.upper(), emb_out.get('user_%s_imp_%s' % (cell, key), nan), emb_out.get('user_mean_imp_%s' % key, nan),
+                out['user_input_imp_' + key]) for key, name in (('auc', 'AUC'), ('mrr', 'MRR'), ('ndcg5', 'nDCG@5'), ('ndcg10', 'nDCG@10'))))
+    return out
+
+
 def load_user_sequences(F, n_train):
     """--user_sequences: (indptr, items, targets or None), checked against the training set's row count before training."""
     from dae_rnn_news_recommendation_b200.user_model import check_sequences
@@ -655,8 +724,12 @@ def main(argv=None):
             model.evaluation.update(recommend_top_k_input(F, model, trX, vlX, trL, vlL, model.evaluation))
         if histories is not None:
             model.evaluation.update(recommend_users(F, model, enc, histories, targets))
+            if F.user_top_k_input:
+                model.evaluation.update(recommend_users_input(F, model, trX, histories, targets, model.evaluation))
         if seqs is not None:
             model.evaluation.update(recommend_users_sequences(F, model, enc, seqs, imps, X=trX))
+            if F.user_top_k_input:
+                model.evaluation.update(recommend_users_sequences_input(F, trX, seqs, imps, model.evaluation))
         if F.top_k_dedup > 0:
             model.evaluation.update(recommend_top_k_dedup(F, model, enc, enc_v, trL, vlL, histories, targets, model.evaluation))
     if F.dedup_threshold > 0:
