@@ -145,6 +145,17 @@ _SIGNATURES = {
     'dae_triplet_batch_hard_rows_det': (C.c_int, [p, i64, i32, i32, i32, p, p, i64, p, p, p, p]),
     'dae_triplet_explicit_det': (C.c_int, [p, p, p, i32, i32, i64, f32, p, p, p, p, p, p]),
     'dae_triplet_loss_sum': (C.c_int, [p, i32, p, p]),
+    # deterministic user-encoder training
+    'dae_seq_rank_loss_det': (C.c_int, [p, i64, p, i64, i32, p, p, i64, f32, p, i64, p, p]),
+    'dae_seq_rank_loss_grad_det': (C.c_int, [p, i64, p, i64, i32, p, p, i64, f32, p, i64, p, p, p, p, p]),
+    'dae_impression_rank_loss_det': (C.c_int, [p, i64, p, i64, i32, p, i64, p, p, p, f32, p, i64, p, p]),
+    'dae_impression_rank_loss_grad_det': (C.c_int, [p, i64, p, i64, i32, p, i64, p, p, p, f32, p, i64, p, p, p, p, p]),
+    'dae_impression_softmax_loss_det': (C.c_int, [p, i64, p, i64, i32, p, i64, p, p, p, p, i32, u64, u64, f32, p, i64, p, p, p]),
+    'dae_impression_softmax_loss_grad_det': (C.c_int, [p, i64, p, i64, i32, p, i64, p, p, p, p, i32, u64, u64, f32, p, i64, p, p, p, p,
+                                                       p, p]),
+    'dae_loss_slots_sum': (C.c_int, [p, i64, p, p]),
+    'dae_ordered_rows_workspace': (C.c_int, [i64, i64, i32, p]),
+    'dae_ordered_rows': (C.c_int, [p, p, p, i64, p, i64, p, i64, p, i64, i32, i32, p, i64, p, i64, p]),
 }
 
 

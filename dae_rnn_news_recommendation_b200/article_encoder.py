@@ -131,10 +131,22 @@ class ArticleEncoder:
         self._encode(self.csr, rows, T, E, col_count)
         return E, col_count
 
-    def backward(self, rows, T, E, dE, col_count):
-        """grad = [dW | dbh] of the listed articles' gradient dE [T, H] (overwritten with dA), by dae_encode_csr_bwd_gather."""
+    def backward(self, rows, T, E, dE, col_count, deterministic=False):
+        """grad = [dW | dbh] of the listed articles' gradient dE [T, H] (overwritten with dA), by dae_encode_csr_bwd_gather, or with
+        deterministic=True by dae_encode_csr_bwd_det and dae_encode_sparse_dw_add onto a zeroed dW (DESIGN 4.21); the latter's
+        workspace size is kept in det_workspace_bytes."""
         F, H, i32 = self.F, self.dim, dict(dtype=torch.int32, device=self.device)
         cap = max(1, min(self.csr.nnz, T * self.csr.max_row_nnz))
+        if deterministic:
+            nb = _cabi.query('dae_encode_csr_bwd_det_workspace', T, F, H, cap)
+            self.det_workspace_bytes = nb
+            ws = torch.empty(nb, dtype=torch.uint8, device=self.device)
+            call('dae_encode_csr_bwd_det', self.csr.indptr.data_ptr(), self.csr.indices.data_ptr(), self.csr.values.data_ptr(),
+                 rows.data_ptr(), T, F, H, self.in_scale, E.data_ptr(), self.bh.data_ptr(), _cabi.act_code(self.enc_act_func),
+                 dE.data_ptr(), None, H, self.grad[F * H:].data_ptr(), col_count.data_ptr(), cap, ws.data_ptr(), nb, _stream())
+            self.grad[:F * H].zero_()
+            call('dae_encode_sparse_dw_add', T, F, H, cap, ws.data_ptr(), nb, self.grad.data_ptr(), _stream())
+            return
         col_start, col_cursor = torch.empty(F + 1, **i32), torch.empty(F, **i32)
         ent_col, ent_row = torch.empty(cap, **i32), torch.empty(cap, **i32)
         ent_val = torch.empty(cap, dtype=torch.float32, device=self.device)
@@ -147,6 +159,16 @@ class ArticleEncoder:
     def scatter_rows(self, src, slots, dE):
         """dE[slots[p]] += src[p] for every row p of src (dae_rows_scatter_add)."""
         call('dae_rows_scatter_add', src.data_ptr(), src.stride(0), slots.data_ptr(), src.shape[0], self.dim, dE.data_ptr(), dE.stride(0),
+             _stream())
+
+    def ordered_rows(self, trip, src, dX, slots, T, dE):
+        """dE [T, H] (stored) = per slot, the loss kernels' triples trip = (slot, row, coefficient) over the rows of src in triple
+        order, then dX[p] for every p with slots[p] = the slot, in p order (dae_ordered_rows)."""
+        t_slot, t_row, t_coef = trip
+        n_a, n_b = t_slot.numel(), dX.shape[0]
+        ws = torch.empty(max(1, _cabi.query('dae_ordered_rows_workspace', n_a, n_b, T)), dtype=torch.uint8, device=self.device)
+        call('dae_ordered_rows', t_slot.data_ptr(), t_row.data_ptr(), t_coef.data_ptr(), n_a, src.data_ptr(), src.stride(0),
+             slots.data_ptr(), n_b, dX.data_ptr(), dX.stride(0), T, self.dim, dE.data_ptr(), dE.stride(0), ws.data_ptr(), ws.numel(),
              _stream())
 
     def step(self):

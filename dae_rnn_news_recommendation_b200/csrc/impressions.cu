@@ -48,11 +48,17 @@ __device__ __forceinline__ void score_chunk(const float* __restrict__ h, const f
 // same impression, whose scores are recomputed when the impression has more than one chunk.
 // DEMB (dae_impression_rank_loss_grad, DESIGN 4.19): each candidate's coefficient g also adds g h_p into demb[items[j]] by fp32
 // atomics; the DEMB = false instance is dae_impression_rank_loss's kernel, its code unchanged by the flag.
-template <bool DEMB>
-__global__ void __launch_bounds__(kImpWarps * 32) impression_rank_loss_kernel(
+// DET (the *_det exports, DESIGN 4.21): position p's loss (the warp sum of its lanes' terms) is stored to loss_slots[p] instead of
+// added, and with DEMB candidate k of the packed items gets the triple (items[k], p, g) at index k (slot -1 in an impression without
+// a click or without a non-click) for dae_ordered_rows.  dh's arithmetic is the same in every instance.
+// The DET instances hold the loss-slot and triple pointers too: 8 CTAs per SM give them 64 registers and no spill (0: no minimum,
+// the default instances' bounds).
+template <bool DEMB, bool DET = false>
+__global__ void __launch_bounds__(kImpWarps * 32, DET ? 8 : 0) impression_rank_loss_kernel(
     const float* __restrict__ h, int64_t ld_h, const float* __restrict__ emb, int64_t ld_emb, int H, const int64_t* __restrict__ pos_indptr,
     int64_t n_pos, const int64_t* __restrict__ imp_indptr, const int32_t* __restrict__ items, const uint8_t* __restrict__ clicked,
-    float scale, float* __restrict__ dh, int64_t ld_dh, double* __restrict__ loss_sum, float* __restrict__ demb, int64_t ld_demb) {
+    float scale, float* __restrict__ dh, int64_t ld_dh, double* __restrict__ loss_sum, float* __restrict__ demb, int64_t ld_demb,
+    double* __restrict__ loss_slots, int32_t* __restrict__ t_slot, int32_t* __restrict__ t_row, float* __restrict__ t_coef) {
   __shared__ float s_a[kImpWarps][kImpChunk], s_b[kImpWarps][kImpChunk], s_w[kImpWarps][kImpChunk];
   __shared__ uint8_t f_a[kImpWarps][kImpChunk], f_b[kImpWarps][kImpChunk];
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
@@ -65,7 +71,12 @@ __global__ void __launch_bounds__(kImpWarps * 32) impression_rank_loss_kernel(
       const int64_t b0 = imp_indptr[q], m = imp_indptr[q + 1] - b0;
       const int nc = count_clicked(clicked + b0, m, lane);
       const int64_t nn = m - nc;
-      if (nc == 0 || nn == 0) continue;
+      if (nc == 0 || nn == 0) {
+        if constexpr (DEMB && DET) {
+          for (int64_t k = lane; k < m; k += 32) t_slot[b0 + k] = -1;
+        }
+        continue;
+      }
       const double inv = imp_recip((double)nc * (double)nn);
       const float coef = (float)((double)scale * inv);
       double l_imp = 0.0;
@@ -106,7 +117,12 @@ __global__ void __launch_bounds__(kImpWarps * 32) impression_rank_loss_kernel(
           const float* e = emb + (int64_t)items[b0 + a0 + t] * ld_emb;
 #pragma unroll 1
           for (int j = lane; j < H; j += 32) d[j] = fmaf(g, e[j], d[j]);
-          if constexpr (DEMB) {
+          if constexpr (DEMB && DET) {
+            if (lane == 0) {
+              const int64_t k = b0 + a0 + t;
+              t_slot[k] = items[k]; t_row[k] = (int32_t)p; t_coef[k] = g;
+            }
+          } else if constexpr (DEMB) {
             float* de = demb + (int64_t)items[b0 + a0 + t] * ld_demb;
 #pragma unroll 1
             for (int j = lane; j < H; j += 32) atomicAdd(de + j, g * hp[j]);
@@ -116,7 +132,13 @@ __global__ void __launch_bounds__(kImpWarps * 32) impression_rank_loss_kernel(
       }
       acc += l_imp * inv;
     }
+    if constexpr (DET) {
+      const double l = warp_sum(acc);
+      if (lane == 0) loss_slots[p] = l;
+      acc = 0.0;
+    }
   }
+  if constexpr (DET) return;
   acc = warp_sum(acc);
   if (lane == 0 && acc != 0.0) atomicAdd(loss_sum, acc);
 }
@@ -187,12 +209,16 @@ __device__ __forceinline__ uint32_t softmax_draw(uint64_t seed, uint64_t epoch, 
 // per SM let ptxas use 64 registers; at its default of 48 it spilled the draw loop's state to the stack.
 // DEMB (dae_impression_softmax_loss_grad, DESIGN 4.19): each candidate's weight g also adds g h_p into demb[it[k]] by fp32 atomics;
 // the DEMB = false instance is dae_impression_softmax_loss's kernel, its code unchanged by the flag.
-template <bool DEMB>
+// DET (the *_det exports, DESIGN 4.21): position p's loss is stored to loss_slots[p], and with DEMB shown article k gets the triple
+// (it[k], p, g) at its index in the packed items, g being its weight summed over the impression's clicks in click order (slot -1
+// where g = 0 or in an impression without a click or without a non-click).  dh's arithmetic is the same in every instance.
+template <bool DEMB, bool DET = false>
 __global__ void __launch_bounds__(kImpWarps * 32, 8) impression_softmax_loss_kernel(
     const float* __restrict__ h, int64_t ld_h, const float* __restrict__ emb, int64_t ld_emb, int H, const int64_t* __restrict__ pos_indptr,
     int64_t n_pos, const int64_t* __restrict__ imp_indptr, const int32_t* __restrict__ items, const uint8_t* __restrict__ clicked,
     const int64_t* __restrict__ imp_ids, int K, uint64_t seed, uint64_t epoch, float scale, float* __restrict__ dh, int64_t ld_dh,
-    double* __restrict__ loss_sum, float* ws, float* __restrict__ demb, int64_t ld_demb) {
+    double* __restrict__ loss_sum, float* ws, float* __restrict__ demb, int64_t ld_demb, double* __restrict__ loss_slots,
+    int32_t* __restrict__ t_slot, int32_t* __restrict__ t_row, float* __restrict__ t_coef) {
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
   const float neg_inf = __int_as_float(0xff800000);
   double acc = 0.0;
@@ -206,7 +232,12 @@ __global__ void __launch_bounds__(kImpWarps * 32, 8) impression_softmax_loss_ker
       const int32_t* it = items + b0;
       const uint8_t* cl = clicked + b0;
       const int nc = count_clicked(cl, m, lane), nn = m - nc;
-      if (nc == 0 || nn == 0) continue;
+      if (nc == 0 || nn == 0) {
+        if constexpr (DEMB && DET) {
+          for (int k = lane; k < m; k += 32) t_slot[b0 + k] = -1;
+        }
+        continue;
+      }
       float* wq = ws + 2 * b0;                           // wq[2 k]: candidate k's weight
       int32_t* nq = reinterpret_cast<int32_t*>(ws) + 2 * b0 + 1;   // nq[2 o]: the position of the o-th non-click
       if (K == 0 || K >= nn) {
@@ -281,11 +312,14 @@ __global__ void __launch_bounds__(kImpWarps * 32, 8) impression_softmax_loss_ker
       __syncwarp();
       for (int k = 0; k < m; ++k) {
         const float g = scale * wq[2 * k];
+        if constexpr (DEMB && DET) {
+          if (lane == 0) { t_slot[b0 + k] = g == 0.0f ? -1 : it[k]; t_row[b0 + k] = (int32_t)p; t_coef[b0 + k] = g; }
+        }
         if (g == 0.0f) continue;
         const float* e = emb + (int64_t)it[k] * ld_emb;
 #pragma unroll 1
         for (int j = lane; j < H; j += 32) d[j] = fmaf(g, e[j], d[j]);
-        if constexpr (DEMB) {
+        if constexpr (DEMB && !DET) {
           float* de = demb + (int64_t)it[k] * ld_demb;
 #pragma unroll 1
           for (int j = lane; j < H; j += 32) atomicAdd(de + j, g * hp[j]);
@@ -293,7 +327,13 @@ __global__ void __launch_bounds__(kImpWarps * 32, 8) impression_softmax_loss_ker
       }
       __syncwarp();   // the next impression of this warp may write ws entries that lanes read above
     }
+    if constexpr (DET) {
+      const double l = warp_sum(acc);
+      if (lane == 0) loss_slots[p] = l;
+      acc = 0.0;
+    }
   }
+  if constexpr (DET) return;
   acc = warp_sum(acc);
   if (lane == 0 && acc != 0.0) atomicAdd(loss_sum, acc);
 }
@@ -313,7 +353,8 @@ extern "C" int dae_impression_rank_loss(const float* h, int64_t ld_h, const floa
   DAE_REQUIRE(h && emb && pos_indptr && imp_indptr && items && clicked && dh && loss_sum && H > 0 && n_pos > 0 && ld_h >= H &&
               ld_emb >= H && ld_dh >= H, "dae_impression_rank_loss: bad arguments");
   impression_rank_loss_kernel<false><<<imp_grid(n_pos), kImpWarps * 32, 0, (cudaStream_t)stream>>>(
-      h, ld_h, emb, ld_emb, H, pos_indptr, n_pos, imp_indptr, items, clicked, scale, dh, ld_dh, loss_sum, nullptr, 0);
+      h, ld_h, emb, ld_emb, H, pos_indptr, n_pos, imp_indptr, items, clicked, scale, dh, ld_dh, loss_sum, nullptr, 0, nullptr, nullptr, nullptr,
+      nullptr);
   DAE_CHECK_LAUNCH("dae_impression_rank_loss");
   return DAE_OK;
 }
@@ -325,7 +366,8 @@ extern "C" int dae_impression_rank_loss_grad(const float* h, int64_t ld_h, const
   DAE_REQUIRE(h && emb && pos_indptr && imp_indptr && items && clicked && dh && loss_sum && demb && H > 0 && n_pos > 0 && ld_h >= H &&
               ld_emb >= H && ld_dh >= H && ld_demb >= H, "dae_impression_rank_loss_grad: bad arguments");
   impression_rank_loss_kernel<true><<<imp_grid(n_pos), kImpWarps * 32, 0, (cudaStream_t)stream>>>(
-      h, ld_h, emb, ld_emb, H, pos_indptr, n_pos, imp_indptr, items, clicked, scale, dh, ld_dh, loss_sum, demb, ld_demb);
+      h, ld_h, emb, ld_emb, H, pos_indptr, n_pos, imp_indptr, items, clicked, scale, dh, ld_dh, loss_sum, demb, ld_demb, nullptr, nullptr, nullptr,
+      nullptr);
   DAE_CHECK_LAUNCH("dae_impression_rank_loss_grad");
   return DAE_OK;
 }
@@ -338,7 +380,7 @@ extern "C" int dae_impression_softmax_loss(const float* h, int64_t ld_h, const f
               ld_h >= H && ld_emb >= H && ld_dh >= H && K >= 0 && K <= kImpMaxNegatives, "dae_impression_softmax_loss: bad arguments");
   impression_softmax_loss_kernel<false><<<imp_grid(n_pos), kImpWarps * 32, 0, (cudaStream_t)stream>>>(
       h, ld_h, emb, ld_emb, H, pos_indptr, n_pos, imp_indptr, items, clicked, imp_ids, K, seed, epoch, scale, dh, ld_dh, loss_sum,
-      (float*)workspace, nullptr, 0);
+      (float*)workspace, nullptr, 0, nullptr, nullptr, nullptr, nullptr);
   DAE_CHECK_LAUNCH("dae_impression_softmax_loss");
   return DAE_OK;
 }
@@ -353,7 +395,7 @@ extern "C" int dae_impression_softmax_loss_grad(const float* h, int64_t ld_h, co
               "dae_impression_softmax_loss_grad: bad arguments");
   impression_softmax_loss_kernel<true><<<imp_grid(n_pos), kImpWarps * 32, 0, (cudaStream_t)stream>>>(
       h, ld_h, emb, ld_emb, H, pos_indptr, n_pos, imp_indptr, items, clicked, imp_ids, K, seed, epoch, scale, dh, ld_dh, loss_sum,
-      (float*)workspace, demb, ld_demb);
+      (float*)workspace, demb, ld_demb, nullptr, nullptr, nullptr, nullptr);
   DAE_CHECK_LAUNCH("dae_impression_softmax_loss_grad");
   return DAE_OK;
 }
@@ -366,5 +408,74 @@ extern "C" int dae_impression_metrics(const float* q, int64_t ld_q, const float*
   impression_metrics_kernel<<<imp_grid(n_imp), kImpWarps * 32, 0, (cudaStream_t)stream>>>(
       q, ld_q, emb, ld_emb, H, cosine, indptr, items, clicked, n_imp, scores, metrics);
   DAE_CHECK_LAUNCH("dae_impression_metrics");
+  return DAE_OK;
+}
+
+// ---- deterministic mode (DESIGN 4.21) ------------------------------------------------------------------------------------------
+static bool imp_det_aligned(const double* loss_slots, const int32_t* t_slot, const int32_t* t_row, const float* t_coef) {
+  return ((uintptr_t)loss_slots & 7) == 0 && (((uintptr_t)t_slot | (uintptr_t)t_row | (uintptr_t)t_coef) & 3) == 0;
+}
+
+extern "C" int dae_impression_rank_loss_det(const float* h, int64_t ld_h, const float* emb, int64_t ld_emb, int32_t H,
+                                            const int64_t* pos_indptr, int64_t n_pos, const int64_t* imp_indptr, const int32_t* items,
+                                            const uint8_t* clicked, float scale, float* dh, int64_t ld_dh, double* loss_slots,
+                                            void* stream) {
+  DAE_REQUIRE(h && emb && pos_indptr && imp_indptr && items && clicked && dh && loss_slots && H > 0 && n_pos > 0 && ld_h >= H &&
+              ld_emb >= H && ld_dh >= H, "dae_impression_rank_loss_det: bad arguments");
+  DAE_REQUIRE(imp_det_aligned(loss_slots, nullptr, nullptr, nullptr), "dae_impression_rank_loss_det: loss_slots must be 8-byte aligned");
+  impression_rank_loss_kernel<false, true><<<imp_grid(n_pos), kImpWarps * 32, 0, (cudaStream_t)stream>>>(
+      h, ld_h, emb, ld_emb, H, pos_indptr, n_pos, imp_indptr, items, clicked, scale, dh, ld_dh, nullptr, nullptr, 0, loss_slots,
+      nullptr, nullptr, nullptr);
+  DAE_CHECK_LAUNCH("dae_impression_rank_loss_det");
+  return DAE_OK;
+}
+
+extern "C" int dae_impression_rank_loss_grad_det(const float* h, int64_t ld_h, const float* emb, int64_t ld_emb, int32_t H,
+                                                 const int64_t* pos_indptr, int64_t n_pos, const int64_t* imp_indptr,
+                                                 const int32_t* items, const uint8_t* clicked, float scale, float* dh, int64_t ld_dh,
+                                                 double* loss_slots, int32_t* t_slot, int32_t* t_row, float* t_coef, void* stream) {
+  DAE_REQUIRE(h && emb && pos_indptr && imp_indptr && items && clicked && dh && loss_slots && t_slot && t_row && t_coef && H > 0 &&
+              n_pos > 0 && n_pos < (1LL << 31) && ld_h >= H && ld_emb >= H && ld_dh >= H,
+              "dae_impression_rank_loss_grad_det: bad arguments");
+  DAE_REQUIRE(imp_det_aligned(loss_slots, t_slot, t_row, t_coef), "dae_impression_rank_loss_grad_det: misaligned loss_slots or triples");
+  impression_rank_loss_kernel<true, true><<<imp_grid(n_pos), kImpWarps * 32, 0, (cudaStream_t)stream>>>(
+      h, ld_h, emb, ld_emb, H, pos_indptr, n_pos, imp_indptr, items, clicked, scale, dh, ld_dh, nullptr, nullptr, 0, loss_slots,
+      t_slot, t_row, t_coef);
+  DAE_CHECK_LAUNCH("dae_impression_rank_loss_grad_det");
+  return DAE_OK;
+}
+
+extern "C" int dae_impression_softmax_loss_det(const float* h, int64_t ld_h, const float* emb, int64_t ld_emb, int32_t H,
+                                               const int64_t* pos_indptr, int64_t n_pos, const int64_t* imp_indptr, const int32_t* items,
+                                               const uint8_t* clicked, const int64_t* imp_ids, int32_t K, uint64_t seed, uint64_t epoch,
+                                               float scale, float* dh, int64_t ld_dh, double* loss_slots, void* workspace,
+                                               void* stream) {
+  DAE_REQUIRE(h && emb && pos_indptr && imp_indptr && items && clicked && imp_ids && dh && loss_slots && workspace && H > 0 &&
+              n_pos > 0 && ld_h >= H && ld_emb >= H && ld_dh >= H && K >= 0 && K <= kImpMaxNegatives,
+              "dae_impression_softmax_loss_det: bad arguments");
+  DAE_REQUIRE(imp_det_aligned(loss_slots, nullptr, nullptr, nullptr) && ((uintptr_t)workspace & 3) == 0,
+              "dae_impression_softmax_loss_det: misaligned loss_slots or workspace");
+  impression_softmax_loss_kernel<false, true><<<imp_grid(n_pos), kImpWarps * 32, 0, (cudaStream_t)stream>>>(
+      h, ld_h, emb, ld_emb, H, pos_indptr, n_pos, imp_indptr, items, clicked, imp_ids, K, seed, epoch, scale, dh, ld_dh, nullptr,
+      (float*)workspace, nullptr, 0, loss_slots, nullptr, nullptr, nullptr);
+  DAE_CHECK_LAUNCH("dae_impression_softmax_loss_det");
+  return DAE_OK;
+}
+
+extern "C" int dae_impression_softmax_loss_grad_det(const float* h, int64_t ld_h, const float* emb, int64_t ld_emb, int32_t H,
+                                                    const int64_t* pos_indptr, int64_t n_pos, const int64_t* imp_indptr,
+                                                    const int32_t* items, const uint8_t* clicked, const int64_t* imp_ids, int32_t K,
+                                                    uint64_t seed, uint64_t epoch, float scale, float* dh, int64_t ld_dh,
+                                                    double* loss_slots, void* workspace, int32_t* t_slot, int32_t* t_row,
+                                                    float* t_coef, void* stream) {
+  DAE_REQUIRE(h && emb && pos_indptr && imp_indptr && items && clicked && imp_ids && dh && loss_slots && workspace && t_slot && t_row &&
+              t_coef && H > 0 && n_pos > 0 && n_pos < (1LL << 31) && ld_h >= H && ld_emb >= H && ld_dh >= H && K >= 0 &&
+              K <= kImpMaxNegatives, "dae_impression_softmax_loss_grad_det: bad arguments");
+  DAE_REQUIRE(imp_det_aligned(loss_slots, t_slot, t_row, t_coef) && ((uintptr_t)workspace & 3) == 0,
+              "dae_impression_softmax_loss_grad_det: misaligned loss_slots, workspace or triples");
+  impression_softmax_loss_kernel<true, true><<<imp_grid(n_pos), kImpWarps * 32, 0, (cudaStream_t)stream>>>(
+      h, ld_h, emb, ld_emb, H, pos_indptr, n_pos, imp_indptr, items, clicked, imp_ids, K, seed, epoch, scale, dh, ld_dh, nullptr,
+      (float*)workspace, nullptr, 0, loss_slots, t_slot, t_row, t_coef);
+  DAE_CHECK_LAUNCH("dae_impression_softmax_loss_grad_det");
   return DAE_OK;
 }

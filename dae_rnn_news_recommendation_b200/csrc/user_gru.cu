@@ -108,14 +108,19 @@ __global__ void __launch_bounds__(256) seq_negatives_kernel(const int32_t* __res
 // dh_p = scale sigma(s- - s+) (e(neg) - e(pos)).  Positions without a next read (pos < 0) get dh_p = 0.
 // DEMB (dae_seq_rank_loss_grad, DESIGN 4.19): also demb[neg] += g h_p and demb[pos] -= g h_p with g = scale sigma(s- - s+), by fp32
 // atomics; the DEMB = false instance is dae_seq_rank_loss's kernel, its code unchanged by the flag.
+// DET (the *_det exports, DESIGN 4.21): the loss term of position p is stored to loss_slots[p] (0 without a next read) instead of
+// added, and with DEMB the article gradient is emitted as triples (t_slot, t_row, t_coef) at 2p = (neg, p, +g) and
+// 2p + 1 = (pos, p, -g) (slot -1 without a next read) for dae_ordered_rows; dh's arithmetic is the same in every instance.
 constexpr int kLossWarps = 8;
-template <bool DEMB>
+template <bool DEMB, bool DET = false>
 __global__ void __launch_bounds__(kLossWarps * 32) seq_rank_loss_kernel(const float* __restrict__ h, int64_t ld_h,
                                                                         const float* __restrict__ emb, int64_t ld_emb, int H,
                                                                         const int32_t* __restrict__ pos, const int32_t* __restrict__ neg,
                                                                         int64_t n_pos, float scale, float* __restrict__ dh,
                                                                         int64_t ld_dh, double* __restrict__ loss_sum,
-                                                                        float* __restrict__ demb, int64_t ld_demb) {
+                                                                        float* __restrict__ demb, int64_t ld_demb,
+                                                                        double* __restrict__ loss_slots, int32_t* __restrict__ t_slot,
+                                                                        int32_t* __restrict__ t_row, float* __restrict__ t_coef) {
   __shared__ double s_loss[kLossWarps];
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
   double acc = 0.0;
@@ -124,6 +129,12 @@ __global__ void __launch_bounds__(kLossWarps * 32) seq_rank_loss_kernel(const fl
     float* d = dh + p * ld_dh;
     if (a < 0) {
       for (int j = lane; j < H; j += 32) d[j] = 0.0f;
+      if constexpr (DET) {
+        if (lane == 0) {
+          loss_slots[p] = 0.0;
+          if constexpr (DEMB) { t_slot[2 * p] = -1; t_slot[2 * p + 1] = -1; }
+        }
+      }
       continue;
     }
     const float* hp = h + p * ld_h;
@@ -136,7 +147,12 @@ __global__ void __launch_bounds__(kLossWarps * 32) seq_rank_loss_kernel(const fl
     const float x = sn - sp;
     const float g = scale * sigmoidf_(x);
     for (int j = lane; j < H; j += 32) d[j] = g * (en[j] - ep[j]);
-    if constexpr (DEMB) {
+    if constexpr (DEMB && DET) {
+      if (lane == 0) {
+        t_slot[2 * p] = neg[p]; t_row[2 * p] = (int32_t)p; t_coef[2 * p] = g;
+        t_slot[2 * p + 1] = a; t_row[2 * p + 1] = (int32_t)p; t_coef[2 * p + 1] = -g;
+      }
+    } else if constexpr (DEMB) {
       float* dp = demb + (int64_t)a * ld_demb;
       float* dn = demb + (int64_t)neg[p] * ld_demb;
       for (int j = lane; j < H; j += 32) {
@@ -145,14 +161,36 @@ __global__ void __launch_bounds__(kLossWarps * 32) seq_rank_loss_kernel(const fl
         atomicAdd(dp + j, -x);
       }
     }
-    if (lane == 0) acc += (double)(fmaxf(x, 0.0f) + log1pf(expf(-fabsf(x))));
+    if constexpr (DET) {
+      if (lane == 0) loss_slots[p] = (double)(fmaxf(x, 0.0f) + log1pf(expf(-fabsf(x))));
+    } else {
+      if (lane == 0) acc += (double)(fmaxf(x, 0.0f) + log1pf(expf(-fabsf(x))));
+    }
   }
+  if constexpr (DET) return;
   if (lane == 0) s_loss[w] = acc;
   __syncthreads();
   if (threadIdx.x == 0) {
     double t = 0.0;
     for (int k = 0; k < kLossWarps; ++k) t += s_loss[k];
     if (t != 0.0) atomicAdd(loss_sum, t);
+  }
+}
+
+// *out += the sum of slots[0, n) in a fixed order: thread t of kSlotSumThreads adds slots t, t + kSlotSumThreads, ... in index
+// order from +0, then thread 0 adds the kSlotSumThreads partials in thread order from +0, then adds that total to *out.
+constexpr int kSlotSumThreads = 256;
+__global__ void __launch_bounds__(kSlotSumThreads) loss_slots_sum_kernel(const double* __restrict__ slots, int64_t n,
+                                                                          double* __restrict__ out) {
+  __shared__ double part[kSlotSumThreads];
+  double s = 0.0;
+  for (int64_t i = threadIdx.x; i < n; i += kSlotSumThreads) s += slots[i];
+  part[threadIdx.x] = s;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double t = 0.0;
+    for (int k = 0; k < kSlotSumThreads; ++k) t += part[k];
+    *out += t;
   }
 }
 
@@ -215,7 +253,7 @@ extern "C" int dae_seq_rank_loss(const float* h, int64_t ld_h, const float* emb,
   DAE_REQUIRE(h && emb && pos && neg && dh && loss_sum && H > 0 && n_pos > 0 && ld_h >= H && ld_emb >= H && ld_dh >= H,
               "dae_seq_rank_loss: bad arguments");
   seq_rank_loss_kernel<false><<<grid_for(n_pos, kLossWarps, 16), kLossWarps * 32, 0, (cudaStream_t)stream>>>(
-      h, ld_h, emb, ld_emb, H, pos, neg, n_pos, scale, dh, ld_dh, loss_sum, nullptr, 0);
+      h, ld_h, emb, ld_emb, H, pos, neg, n_pos, scale, dh, ld_dh, loss_sum, nullptr, 0, nullptr, nullptr, nullptr, nullptr);
   DAE_CHECK_LAUNCH("dae_seq_rank_loss");
   return DAE_OK;
 }
@@ -226,7 +264,40 @@ extern "C" int dae_seq_rank_loss_grad(const float* h, int64_t ld_h, const float*
   DAE_REQUIRE(h && emb && pos && neg && dh && loss_sum && demb && H > 0 && n_pos > 0 && ld_h >= H && ld_emb >= H && ld_dh >= H &&
               ld_demb >= H, "dae_seq_rank_loss_grad: bad arguments");
   seq_rank_loss_kernel<true><<<grid_for(n_pos, kLossWarps, 16), kLossWarps * 32, 0, (cudaStream_t)stream>>>(
-      h, ld_h, emb, ld_emb, H, pos, neg, n_pos, scale, dh, ld_dh, loss_sum, demb, ld_demb);
+      h, ld_h, emb, ld_emb, H, pos, neg, n_pos, scale, dh, ld_dh, loss_sum, demb, ld_demb, nullptr, nullptr, nullptr, nullptr);
   DAE_CHECK_LAUNCH("dae_seq_rank_loss_grad");
+  return DAE_OK;
+}
+
+extern "C" int dae_seq_rank_loss_det(const float* h, int64_t ld_h, const float* emb, int64_t ld_emb, int32_t H, const int32_t* pos,
+                                     const int32_t* neg, int64_t n_pos, float scale, float* dh, int64_t ld_dh, double* loss_slots,
+                                     void* stream) {
+  DAE_REQUIRE(h && emb && pos && neg && dh && loss_slots && H > 0 && n_pos > 0 && ld_h >= H && ld_emb >= H && ld_dh >= H,
+              "dae_seq_rank_loss_det: bad arguments");
+  DAE_REQUIRE(((uintptr_t)loss_slots & 7) == 0, "dae_seq_rank_loss_det: loss_slots must be 8-byte aligned");
+  seq_rank_loss_kernel<false, true><<<grid_for(n_pos, kLossWarps, 16), kLossWarps * 32, 0, (cudaStream_t)stream>>>(
+      h, ld_h, emb, ld_emb, H, pos, neg, n_pos, scale, dh, ld_dh, nullptr, nullptr, 0, loss_slots, nullptr, nullptr, nullptr);
+  DAE_CHECK_LAUNCH("dae_seq_rank_loss_det");
+  return DAE_OK;
+}
+
+extern "C" int dae_seq_rank_loss_grad_det(const float* h, int64_t ld_h, const float* emb, int64_t ld_emb, int32_t H, const int32_t* pos,
+                                          const int32_t* neg, int64_t n_pos, float scale, float* dh, int64_t ld_dh, double* loss_slots,
+                                          int32_t* t_slot, int32_t* t_row, float* t_coef, void* stream) {
+  DAE_REQUIRE(h && emb && pos && neg && dh && loss_slots && t_slot && t_row && t_coef && H > 0 && n_pos > 0 && n_pos < (1LL << 30) &&
+              ld_h >= H && ld_emb >= H && ld_dh >= H, "dae_seq_rank_loss_grad_det: bad arguments");
+  DAE_REQUIRE(((uintptr_t)loss_slots & 7) == 0 && (((uintptr_t)t_slot | (uintptr_t)t_row | (uintptr_t)t_coef) & 3) == 0,
+              "dae_seq_rank_loss_grad_det: misaligned loss_slots or triples");
+  seq_rank_loss_kernel<true, true><<<grid_for(n_pos, kLossWarps, 16), kLossWarps * 32, 0, (cudaStream_t)stream>>>(
+      h, ld_h, emb, ld_emb, H, pos, neg, n_pos, scale, dh, ld_dh, nullptr, nullptr, 0, loss_slots, t_slot, t_row, t_coef);
+  DAE_CHECK_LAUNCH("dae_seq_rank_loss_grad_det");
+  return DAE_OK;
+}
+
+extern "C" int dae_loss_slots_sum(const double* loss_slots, int64_t n, double* out, void* stream) {
+  DAE_REQUIRE(loss_slots && out && n >= 0, "dae_loss_slots_sum: bad arguments");
+  DAE_REQUIRE((((uintptr_t)loss_slots | (uintptr_t)out) & 7) == 0, "dae_loss_slots_sum: pointers must be 8-byte aligned");
+  loss_slots_sum_kernel<<<1, kSlotSumThreads, 0, (cudaStream_t)stream>>>(loss_slots, n, out);
+  DAE_CHECK_LAUNCH("dae_loss_slots_sum");
   return DAE_OK;
 }

@@ -50,6 +50,13 @@ batch encodes only the T articles it touches (dae_touch_compact, dae_encode_csr_
 compact table with slot ids, takes the article gradient from the loss (the *_loss_grad exports) and from the input projection
 (dX = dXP . W_in, dae_rows_scatter_add), backpropagates it into [W | bh] (dae_encode_csr_bwd_gather) and steps [W | bh] after
 theta.  art.vectors(X) encodes any bag of words with the learned W and bh, articles never seen in training included.
+
+Deterministic training (DESIGN 4.21): with deterministic=True, two fits with the same seed, inputs, build and GPU model give the same
+bits: theta, its slots, steps, train_loss, the long-term table, an ArticleEncoder's [W | bh] and slots, and everything computed from
+them.  The stream-K weight GEMMs run as dae_gemm_bf16x3_det, the loss kernels store one fp64 term per position that
+dae_loss_slots_sum adds in a fixed order, and with an ArticleEncoder the loss kernels emit the article gradient as (slot, row,
+coefficient) triples that dae_ordered_rows sums per slot in a fixed order together with dX, before dae_encode_csr_bwd_det.  It is a
+run option: save() does not store it.
 """
 import numpy as np
 import torch
@@ -59,6 +66,7 @@ from ._cabi import call
 from .article_encoder import ARTICLE_ENCODE_GROUPS, ARTICLE_LEARNING_RATE, ArticleEncoder  # noqa: F401
 
 _NAMES = ('weight_ih_l0', 'weight_hh_l0', 'bias_ih_l0', 'bias_hh_l0')
+_LOSS_SLOTS_SUM = 'dae_loss_slots_sum'   # the deterministic mode's fixed-order loss sum (DESIGN 4.21)
 LONG_TERM_LEARNING_RATE = 0.1    # the long-term table's default learning rate: the best of 0.01, 0.03 and 0.1 (DESIGN 4.18)
 
 
@@ -252,8 +260,10 @@ class _UserEncoder:
     _PARAMS = ()                     # state_dict names
 
     def __init__(self, dim, max_len=50, batch_users=1024, num_epochs=5, opt='adam', learning_rate=1e-3, seed=0, device='cuda:0',
-                 momentum=0.5, impression_loss='pairwise', impression_negatives=4):
+                 momentum=0.5, impression_loss='pairwise', impression_negatives=4, deterministic=False):
         name = type(self).__name__
+        if type(deterministic) is not bool:
+            raise ValueError('%s: deterministic = %r, True or False' % (name, deterministic))
         if dim < 1 or max_len < 1 or batch_users < 1 or num_epochs < 0:
             raise ValueError('%s: dim, max_len and batch_users must be >= 1 and num_epochs >= 0' % name)
         if opt not in _cabi.OPT:
@@ -265,6 +275,8 @@ class _UserEncoder:
             raise ValueError('%s: impression_negatives = %r, an integer in [0, %d] (0: every non-click)'
                              % (name, impression_negatives, MAX_IMPRESSION_NEGATIVES))
         self.impression_loss, self.impression_negatives = impression_loss, int(impression_negatives)
+        self.deterministic = deterministic
+        self._gemm_ws = None      # dae_gemm_bf16x3_det's workspace (deterministic mode; the user path runs on one stream)
         self.dim, self.max_len, self.batch_users, self.num_epochs = int(dim), int(max_len), int(batch_users), int(num_epochs)
         self.opt, self.learning_rate, self.momentum, self.seed = opt, float(learning_rate), float(momentum), int(seed)
         self.device = torch.device(device)
@@ -345,9 +357,17 @@ class _UserEncoder:
         return emb
 
     def _gemm(self, M, N, K, A, a_mn, Bm, b_mn, C, ldc, accumulate=0, k_splits=1):
+        """C (+)= A . B^T on the bf16x3 tensor cores.  The stream-K calls (k_splits = -1) add split tiles by fp32 atomics; in the
+        deterministic mode they run as dae_gemm_bf16x3_det.  Calls with k_splits = 1 have one writer per element in both modes."""
         (a_hi, a_lo), (b_hi, b_lo) = A, Bm
-        call('dae_gemm_bf16x3', M, N, K, 1.0, a_hi.data_ptr(), a_lo.data_ptr(), a_hi.stride(0), a_mn, b_hi.data_ptr(), b_lo.data_ptr(),
-             b_hi.stride(0), b_mn, C.data_ptr(), ldc, 0, -1, None, k_splits, accumulate, _stream())
+        args = (M, N, K, 1.0, a_hi.data_ptr(), a_lo.data_ptr(), a_hi.stride(0), a_mn, b_hi.data_ptr(), b_lo.data_ptr(), b_hi.stride(0),
+                b_mn, C.data_ptr(), ldc, 0, -1, None, k_splits, accumulate)
+        name, ws = 'dae_gemm_bf16x3', ()
+        if self.deterministic and k_splits != 1:
+            if self._gemm_ws is None:
+                self._gemm_ws = torch.empty(_cabi.query('dae_gemm_det_workspace'), dtype=torch.uint8, device=self.device)
+            name, ws = name + '_det', (self._gemm_ws.data_ptr(), self._gemm_ws.numel())
+        call(name, *args, *ws, _stream())
 
     def _mark(self, name):
         if self.phase_events is not None:
@@ -394,24 +414,37 @@ class _UserEncoder:
                 imp_items = slots[P:]
             self._mark('compact')
             emb, col_count = art.encode_rows(rows, T)
-            dE = torch.zeros_like(emb)
-            grad = (dE.data_ptr(), H)
             self._mark('encode')
-        sfx = '' if art is None else '_grad'
+        det = self.deterministic
+        if det:   # one fp64 loss slot per position; with art the article gradient as triples (slot, row of Hs, coefficient)
+            loss = torch.empty(P, dtype=torch.float64, device=self.device)
+            if art is not None:
+                n_trip = 2 * P if ib is None else int(ib.items.size)
+                trip = (torch.empty(n_trip, dtype=torch.int32, device=self.device), torch.empty(n_trip, dtype=torch.int32, device=self.device),
+                        torch.empty(n_trip, dtype=torch.float32, device=self.device))
+                grad = tuple(t.data_ptr() for t in trip)
+        else:
+            loss = self.stats
+            if art is not None:
+                dE = torch.zeros_like(emb)
+                grad = (dE.data_ptr(), H)
+        sfx = ('' if art is None else '_grad') + ('_det' if det else '')
         self._forward(b, pk, emb, items, st)
         Hs = b['Hs']
         if ib is None:
             call('dae_seq_rank_loss' + sfx, Hs.data_ptr(), H, emb.data_ptr(), emb.stride(0), H, nxt.data_ptr(), neg.data_ptr(), P,
-                 1.0 / pk.terms, b['dH'].data_ptr(), H, self.stats.data_ptr(), *grad, st)
+                 1.0 / pk.terms, b['dH'].data_ptr(), H, loss.data_ptr(), *grad, st)
         elif self.impression_loss == 'softmax':
             ws = torch.empty(2 * ib.items.size, dtype=torch.int32, device=self.device)   # 8 bytes per shown article
             call('dae_impression_softmax_loss' + sfx, Hs.data_ptr(), H, emb.data_ptr(), emb.stride(0), H, pos_indptr.data_ptr(), P,
                  imp_indptr.data_ptr(), imp_items.data_ptr(), imp_clicked.data_ptr(), imp_ids.data_ptr(), self.impression_negatives,
-                 self.seed, epoch, 1.0 / ib.clicks, b['dH'].data_ptr(), H, self.stats.data_ptr(), ws.data_ptr(), *grad, st)
+                 self.seed, epoch, 1.0 / ib.clicks, b['dH'].data_ptr(), H, loss.data_ptr(), ws.data_ptr(), *grad, st)
         else:
             call('dae_impression_rank_loss' + sfx, Hs.data_ptr(), H, emb.data_ptr(), emb.stride(0), H, pos_indptr.data_ptr(), P,
                  imp_indptr.data_ptr(), imp_items.data_ptr(), imp_clicked.data_ptr(), 1.0 / ib.n, b['dH'].data_ptr(), H,
-                 self.stats.data_ptr(), *grad, st)
+                 loss.data_ptr(), *grad, st)
+        if det:   # stats[0] += the slots in dae_loss_slots_sum's fixed order
+            call(_LOSS_SLOTS_SUM, loss.data_ptr(), P, self.stats.data_ptr(), st)
         self._mark('loss')
         self._backward(b, pk, st)
         if art is not None:
@@ -419,9 +452,13 @@ class _UserEncoder:
             dgrad, W_in, K = self._input_grad(b)
             dX = torch.empty(P, H, dtype=torch.float32, device=self.device)
             self._gemm(P, H, K, dgrad, 0, W_in, 1, dX, H)
-            art.scatter_rows(dX, items, dE)
+            if det:   # dE = the loss triples over Hs, then the dX rows, per slot in that order
+                dE = torch.empty_like(emb)
+                art.ordered_rows(trip, Hs, dX, items, T, dE)
+            else:
+                art.scatter_rows(dX, items, dE)
             self._mark('input_gradient')
-            art.backward(rows, T, emb, dE, col_count)
+            art.backward(rows, T, emb, dE, col_count, deterministic=det)
             self._mark('article_backward')
             self.article_batch = {'rows': rows, 'slots': slots, 'E': emb, 'dE': dE, 'dX': dX}   # the last batch's tables, for inspection
 

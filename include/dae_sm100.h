@@ -777,6 +777,51 @@ int dae_touch_compact(const int32_t* ids, int64_t n, uint32_t stamp, void* tag, 
 int dae_rows_scatter_add(const float* src, int64_t ld_src, const int32_t* idx, int64_t n, int32_t cols, float* dst, int64_t ld_dst,
                          void* stream);
 
+/* ---- deterministic user-encoder training (DESIGN 4.21) -----------------------------------------------------------------------
+ * With the same inputs, build and GPU model these give the same bits on every run.
+ * dae_seq_rank_loss_det, dae_impression_rank_loss_det, dae_impression_softmax_loss_det: the losses above with the same arguments and
+ *   the same dh, bit for bit, but loss_slots (fp64 [n_pos], 8-byte aligned) in place of loss_sum: position p's loss term is STORED
+ *   to loss_slots[p] (0 for a position without a term); nothing is added anywhere.  For the impression losses the slot is the
+ *   warp's butterfly sum of its lanes' terms for that position.
+ * dae_*_loss_grad_det: the same, and in place of demb the article gradient as triples (t_slot, t_row, t_coef: int32, int32, fp32)
+ *   meaning "add t_coef * h[t_row] to row t_slot", each at an index fixed by the data layout: the rank loss writes 2 n_pos triples,
+ *   2p = (neg[p], p, +g) and 2p + 1 = (pos[p], p, -g); the impression losses write one triple per shown article k at index k of
+ *   items (imp_indptr[pos_indptr[n_pos]] triples), with g its coefficient in dh_p.  t_slot = -1 marks a triple that adds nothing.
+ * dae_loss_slots_sum: *out += sum of loss_slots[0, n) in a fixed order: 256 partials, partial t the sum of slots t, t + 256, ... in
+ *   index order from +0, then the partials in order from +0, then that total added to *out.
+ * dae_ordered_rows: dst[t, 0:cols] for every t < n_slots, STORED: the terms whose slot is t, taken in term order, as
+ *   acc = acc + c * src_row (fp32, +0 first, each product and sum rounded on its own).  Term i < n_a is the triple (a_slot[i],
+ *   a_row[i], a_coef[i]) over rows of src_a; term n_a + p is (b_slot[p], p, 1) over rows of src_b.  Slots must be < n_slots; a
+ *   slot < 0 adds nothing; a slot without terms gets a zero row.  workspace (256-byte aligned): dae_ordered_rows_workspace bytes,
+ *   16 bytes per term (the sort's keys and values, double-buffered) plus cub's radix-sort scratch.
+ */
+int dae_seq_rank_loss_det(const float* h, int64_t ld_h, const float* emb, int64_t ld_emb, int32_t H, const int32_t* pos,
+                          const int32_t* neg, int64_t n_pos, float scale, float* dh, int64_t ld_dh, double* loss_slots, void* stream);
+int dae_seq_rank_loss_grad_det(const float* h, int64_t ld_h, const float* emb, int64_t ld_emb, int32_t H, const int32_t* pos,
+                               const int32_t* neg, int64_t n_pos, float scale, float* dh, int64_t ld_dh, double* loss_slots,
+                               int32_t* t_slot, int32_t* t_row, float* t_coef, void* stream);
+int dae_impression_rank_loss_det(const float* h, int64_t ld_h, const float* emb, int64_t ld_emb, int32_t H, const int64_t* pos_indptr,
+                                 int64_t n_pos, const int64_t* imp_indptr, const int32_t* items, const uint8_t* clicked, float scale,
+                                 float* dh, int64_t ld_dh, double* loss_slots, void* stream);
+int dae_impression_rank_loss_grad_det(const float* h, int64_t ld_h, const float* emb, int64_t ld_emb, int32_t H,
+                                      const int64_t* pos_indptr, int64_t n_pos, const int64_t* imp_indptr, const int32_t* items,
+                                      const uint8_t* clicked, float scale, float* dh, int64_t ld_dh, double* loss_slots, int32_t* t_slot,
+                                      int32_t* t_row, float* t_coef, void* stream);
+int dae_impression_softmax_loss_det(const float* h, int64_t ld_h, const float* emb, int64_t ld_emb, int32_t H,
+                                    const int64_t* pos_indptr, int64_t n_pos, const int64_t* imp_indptr, const int32_t* items,
+                                    const uint8_t* clicked, const int64_t* imp_ids, int32_t K, uint64_t seed, uint64_t epoch, float scale,
+                                    float* dh, int64_t ld_dh, double* loss_slots, void* workspace, void* stream);
+int dae_impression_softmax_loss_grad_det(const float* h, int64_t ld_h, const float* emb, int64_t ld_emb, int32_t H,
+                                         const int64_t* pos_indptr, int64_t n_pos, const int64_t* imp_indptr, const int32_t* items,
+                                         const uint8_t* clicked, const int64_t* imp_ids, int32_t K, uint64_t seed, uint64_t epoch,
+                                         float scale, float* dh, int64_t ld_dh, double* loss_slots, void* workspace, int32_t* t_slot,
+                                         int32_t* t_row, float* t_coef, void* stream);
+int dae_loss_slots_sum(const double* loss_slots, int64_t n, double* out, void* stream);
+int dae_ordered_rows_workspace(int64_t n_a, int64_t n_b, int32_t n_slots, int64_t* bytes);
+int dae_ordered_rows(const int32_t* a_slot, const int32_t* a_row, const float* a_coef, int64_t n_a, const float* src_a, int64_t ld_a,
+                     const int32_t* b_slot, int64_t n_b, const float* src_b, int64_t ld_b, int32_t n_slots, int32_t cols, float* dst,
+                     int64_t ld_dst, void* workspace, int64_t workspace_bytes, void* stream);
+
 /* ---- bag-of-words user profiles and their impression metrics (DESIGN 4.20) --------------------------------------------------
  * The history W [n_users x n_articles] and the articles X [n_articles x n_features] are CSR matrices: indptr int64, indices int32
  * strictly increasing inside a row (sorted, no duplicates), values fp32; the kernels do not check the contents.  The profiles

@@ -95,7 +95,8 @@ def build_parser():
     ap.add_argument('--deterministic', action='store_true', default=False,
                     help='add every floating-point sum of the training step in a fixed order, so that a rerun with the same --seed (>= 0) '
                          'and data gives bit-identical parameters, losses and embeddings on the same GPU model (slower; default: off, '
-                         'or the environment variable DAE_DETERMINISTIC=1)')
+                         'or the environment variable DAE_DETERMINISTIC=1); this covers the DAE step only, see --user_deterministic for the '
+                         'user encoder')
     ap.add_argument('--user_histories', default='',
                     help='with --top_k K: a scipy.sparse.save_npz matrix [users x training articles] of reading histories (values: '
                          'weights); after transform, recommend the K best unread training articles to every user (helpers.recommend) '
@@ -128,6 +129,10 @@ def build_parser():
                          '(user_model.ArticleEncoder, inputs scaled by 1 - corr_frac); save user_<cell>_article_encoder.npz and '
                          'article_encoded_fine_tuned.npy, and score the user encoder with the fine-tuned vectors (the mean profile '
                          'keeps the DAE\'s)')
+    ap.add_argument('--user_deterministic', action='store_true', default=False,
+                    help='with --user_sequences: train the user encoder (and with --user_fine_tune_articles the article encoder) in '
+                         'its deterministic mode, so that a rerun on the same embeddings gives bit-identical parameters and losses on '
+                         'the same GPU model (DESIGN 4.21); for a whole run to repeat, also pass --deterministic and --seed >= 0')
     ap.add_argument('--user_article_lr', type=float, default=None,
                     help='with --user_fine_tune_articles: the article encoder\'s learning rate (default '
                          'user_model.ARTICLE_LEARNING_RATE)')
@@ -230,6 +235,7 @@ def check_flags(F):
     assert F.user_long_term_lr is None or F.user_long_term_lr > 0, '--user_long_term_lr must be > 0'
     assert not F.user_fine_tune_articles or F.user_sequences, '--user_fine_tune_articles needs --user_sequences'
     assert F.user_article_lr is None or F.user_fine_tune_articles, '--user_article_lr needs --user_fine_tune_articles'
+    assert not F.user_deterministic or F.user_sequences, '--user_deterministic needs --user_sequences'
     assert F.user_article_lr is None or F.user_article_lr >= 0, '--user_article_lr must be >= 0'
     F.user_attention_dim = 200 if F.user_attention_dim is None else F.user_attention_dim
     assert F.user_attention_dim >= 1, '--user_attention_dim must be >= 1'
@@ -640,7 +646,7 @@ def recommend_users_sequences(F, model, enc, seqs, impressions=(None, None), X=N
         kw.update(long_term_users=len(indptr) - 1, long_term_mask=F.user_long_term_mask, long_term_learning_rate=F.user_long_term_lr)
     enc_cls = {'gru': UserGRU, 'lstm': UserLSTM, 'attention': UserAttention}[cell]
     rnn = enc_cls(enc.shape[1], num_epochs=F.user_epochs, seed=max(F.seed, 0), impression_loss=F.user_impression_loss,
-                  impression_negatives=F.user_negatives, **kw)
+                  impression_negatives=F.user_negatives, deterministic=F.user_deterministic, **kw)
     art = enc
     if F.user_fine_tune_articles:
         art = ArticleEncoder(X, model.get_model_parameters(), enc_act_func=model.enc_act_func, in_scale=1.0 - F.corr_frac,

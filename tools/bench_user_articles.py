@@ -110,39 +110,55 @@ def speed(args):
         art = ArticleEncoder(X, _params(args.f, args.h, 0), enc_act_func='sigmoid', in_scale=0.7, device=d)
         emb = art.vectors(to_host=False)
         ms = {'frozen': UserGRU(args.h, batch_users=B, seed=0), 'joint': UserGRU(args.h, batch_users=B, seed=0)}
+        if args.deterministic:   # DESIGN 4.21: both paths in the deterministic mode too, timed in the same alternation
+            ms.update(frozen_det=UserGRU(args.h, batch_users=B, seed=0, deterministic=True),
+                      joint_det=UserGRU(args.h, batch_users=B, seed=0, deterministic=True))
         packs = [Packed(indptr, items, u, 50) for u in ms['frozen'].batches(indptr, 0)]
         P = sum(p.P for p in packs)
+        joint = lambda name: name.startswith('joint')   # noqa: E731
         for name, m in ms.items():   # warm-up
-            _epoch(m, indptr, items, emb if name == 'frozen' else None, art if name == 'joint' else None, 0, packs)
-        rates = {'frozen': [], 'joint': []}
+            _epoch(m, indptr, items, None if joint(name) else emb, art if joint(name) else None, 0, packs)
+        rates = {name: [] for name in ms}
         for _ in range(args.rounds):
             for name, m in ms.items():
-                s = _epoch(m, indptr, items, emb if name == 'frozen' else None, art if name == 'joint' else None, 0, packs)
+                s = _epoch(m, indptr, items, None if joint(name) else emb, art if joint(name) else None, 0, packs)
                 rates[name].append(P / s)
-        m = ms['joint']
-        torch.cuda.synchronize()
-        base = torch.cuda.memory_allocated()
-        torch.cuda.reset_peak_memory_stats()
-        m.phase_events, Ts = [], []
-        for bi, pk in enumerate(packs):
-            m._forward_backward(pk, None, 0, bi, None, art)
-            Ts.append(int(m.article_batch['rows'].numel()))
-            m._optimizer_step()
-            art.step()
-            m._mark('article_step')
-        torch.cuda.synchronize()
-        peak = torch.cuda.max_memory_allocated() - base
-        ph = {}
-        ev = m.phase_events
-        for (n0, e0), (n1, e1) in zip(ev[:-1], ev[1:]):
-            if n1 != 'start':
-                ph[n1] = ph.get(n1, 0.0) + e0.elapsed_time(e1)
-        m.phase_events = None
         out[str(B)] = {'positions': P, 'batches': len(packs), 'frozen_positions_per_s': rates['frozen'],
-                       'joint_positions_per_s': rates['joint'], 'T_mean': float(np.mean(Ts)), 'T_max': int(np.max(Ts)),
-                       'phase_ms_per_batch': {k: v / len(packs) for k, v in ph.items()}, 'peak_bytes_above_inputs': int(peak),
-                       'regimes_at_T_mean': regimes(art, int(np.mean(Ts)))}
+                       'joint_positions_per_s': rates['joint']}
+        if args.deterministic:
+            out[str(B)].update(frozen_det_positions_per_s=rates['frozen_det'], joint_det_positions_per_s=rates['joint_det'])
+        for name in ('joint', 'joint_det') if args.deterministic else ('joint',):
+            out[str(B)].update(_joint_phases(ms[name], art, packs, '' if name == 'joint' else '_det'))
     return out
+
+
+def _joint_phases(m, art, packs, sfx):
+    """One epoch of the joint model with phase events: the per-batch phase times, the touched-article counts and the peak memory."""
+    torch.cuda.synchronize()
+    base = torch.cuda.memory_allocated()
+    torch.cuda.reset_peak_memory_stats()
+    m.phase_events, Ts = [], []
+    for bi, pk in enumerate(packs):
+        m._forward_backward(pk, None, 0, bi, None, art)
+        Ts.append(int(m.article_batch['rows'].numel()))
+        m._optimizer_step()
+        art.step()
+        m._mark('article_step')
+    torch.cuda.synchronize()
+    peak = torch.cuda.max_memory_allocated() - base
+    ph = {}
+    ev = m.phase_events
+    for (n0, e0), (n1, e1) in zip(ev[:-1], ev[1:]):
+        if n1 != 'start':
+            ph[n1] = ph.get(n1, 0.0) + e0.elapsed_time(e1)
+    m.phase_events = None
+    r = {'T_mean': float(np.mean(Ts)), 'T_max': int(np.max(Ts)), 'phase_ms_per_batch': {k: v / len(packs) for k, v in ph.items()},
+         'peak_bytes_above_inputs': int(peak)}
+    if sfx:
+        r['article_backward_workspace_bytes'] = int(art.det_workspace_bytes)
+    else:
+        r['regimes_at_T_mean'] = regimes(art, int(np.mean(Ts)))
+    return {k + sfx: v for k, v in r.items()}
 
 
 # ---- the cold-start learning check ---------------------------------------------------------------------------------------
@@ -206,11 +222,17 @@ def main():
     ap.add_argument('--rounds', type=int, default=2)
     ap.add_argument('--learning_lrs', default='1e-4,1e-3,1e-2')
     ap.add_argument('--skip_speed', action='store_true')
+    ap.add_argument('--skip_learning', action='store_true')
+    ap.add_argument('--deterministic', action='store_true',
+                    help='also time the frozen and joint paths in the deterministic mode (DESIGN 4.21)')
     args = ap.parse_args()
     args.batch_users = [int(x) for x in args.batch_users.split(',')]
     out = {'gpu': _gpu_info()}
     if not args.skip_speed:
         out['train'] = speed(args)
+    if args.skip_learning:
+        print(json.dumps(out))
+        return
     data = learning_workload()
     out['learning'] = {'frozen': learning_auc(data)}
     for lr in [float(x) for x in args.learning_lrs.split(',') if x]:

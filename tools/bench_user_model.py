@@ -56,14 +56,18 @@ def _epoch(m, indptr, items, emb, epoch, packs=None):
     return time.perf_counter() - t0, sum(p.P for p in packs), sum(p.B for p in packs), packs
 
 
-def train_arm(args, B, indptr, items, emb):
-    m = CELLS[args.cell][0](args.h, max_len=50, batch_users=B, seed=0)
+def train_arm(args, B, indptr, items, emb, deterministic=False):
+    m = CELLS[args.cell][0](args.h, max_len=50, batch_users=B, seed=0, deterministic=deterministic)
     _epoch(m, indptr, items, emb, 0)                      # warm-up (buffers, module loads)
     packs = [Packed(indptr, items, u, m.max_len) for u in m.batches(indptr, 1)]   # host packing outside the timed span
     sec, pos, users, _ = _epoch(m, indptr, items, emb, 1, packs)
     m.phase_events = []
+    torch.cuda.synchronize()
+    base = torch.cuda.memory_allocated()
+    torch.cuda.reset_peak_memory_stats()
     _epoch(m, indptr, items, emb, 2, packs)
     torch.cuda.synchronize()
+    peak = torch.cuda.max_memory_allocated() - base
     split = {}
     ev = m.phase_events
     for (_, a), (name, b) in zip(ev[:-1], ev[1:]):
@@ -71,7 +75,7 @@ def train_arm(args, B, indptr, items, emb):
             split[name] = split.get(name, 0.0) + a.elapsed_time(b)
     m.phase_events = None
     res = {'batch_users': B, 'batches': len(packs), 'positions': pos, 'users': users, 'epoch_s': sec, 'positions_per_s': pos / sec,
-           'users_per_s': users / sec, 'phase_ms_per_epoch': split, 'loss_last_epochs': m.train_loss}
+           'users_per_s': users / sec, 'phase_ms_per_epoch': split, 'loss_last_epochs': m.train_loss, 'peak_bytes_above_inputs': int(peak)}
     return res, packs, m
 
 
@@ -180,6 +184,9 @@ def main():
     ap.add_argument('--users', type=int, default=32768)
     ap.add_argument('--batch_users', default='1024,4096')
     ap.add_argument('--transform_users', default='100000,1000000')
+    ap.add_argument('--deterministic', action='store_true',
+                    help='time the training arm in the deterministic mode against the default mode (DESIGN 4.21), alternating '
+                         'the two; the cuDNN / torch and transform arms are skipped')
     args = ap.parse_args()
     if not torch.cuda.is_available():
         sys.exit('bench_user_model: no CUDA device')
@@ -192,6 +199,16 @@ def main():
     res['torch' if args.cell == 'attention' else 'cudnn'] = []
     if args.cell != 'gru':   # the default GRU line keeps its keys
         res['cell'] = args.cell
+    if args.deterministic:
+        res['deterministic'] = []
+        for B in (int(b) for b in args.batch_users.split(',')):
+            for _ in range(2):   # alternating arms: default, deterministic, default, deterministic
+                for det in (False, True):
+                    r = train_arm(args, B, indptr, items, emb, deterministic=det)[0]
+                    r['deterministic'] = det
+                    res['deterministic'].append(r)
+        print(json.dumps(res))
+        return
     m = None
     for B in (int(b) for b in args.batch_users.split(',')):
         r, packs, m = train_arm(args, B, indptr, items, emb)
