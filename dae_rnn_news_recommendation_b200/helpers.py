@@ -32,9 +32,11 @@ nearest-article lookup of main_autoencoder.py:307-318,352-359) -- SURVEY section
                                                                                                         grid, without the matrix)
     auroc_from_histograms(hist, sums, M, bins) -> dict                                                 (its host half, pure NumPy)
 
-Dense inputs (embeddings) go through the wgmma bf16x3 GEMM on row-normalised operands; sparse inputs (count / tf-idf
-matrices) through the CSR encode kernel against the dense transpose, except in top_k_similar, where they go through the
-sparse CSR x CSR top-k kernel (dae_csr_similarity_topk).  No CPU path.
+Dense inputs (embeddings) go through the wgmma bf16x3 kernels on row-normalised operands.  Sparse inputs (count / tf-idf
+matrices) go through the CSR x CSR kernels (dae_csr_*), except in pairwise_similarity, which runs the CSR encode kernel against
+the dense transpose.  top_k_similar, similar_pairs and similarity_auroc build their operands of either kind in one place
+(_Operands); recommend and recommend_sparse share their request (_recommend_request) and their output (_recommend_result), and
+differ only in how they rank.  No CPU path.
 """
 import ctypes
 import math
@@ -53,6 +55,18 @@ _NORM = {'': 0, 'l1': 1, 'l2': 2, 'max': 3}
 
 def _stream():
     return torch.cuda.current_stream().cuda_stream
+
+
+def _check_metric(metric, fn):
+    if metric not in ('cosine', 'linear kernel'):
+        raise ValueError("%s: metric = %r: 'cosine' or 'linear kernel'" % (fn, metric))
+
+
+def _result(out, to_host):
+    """An entry point's return value: the device tensor out (or tuple of them) as ndarrays with to_host, as it is without."""
+    if not to_host:
+        return out
+    return tuple(t.cpu().numpy() for t in out) if isinstance(out, tuple) else out.cpu().numpy()
 
 
 def _normalised_operands(x_dev, norm_kind):
@@ -84,8 +98,7 @@ def pairwise_similarity(in_df, norm='', metric='cosine', set_diagonal_zero=True,
     assert metric in ['cosine', 'linear kernel']
     assert norm in _NORM
     if sp.issparse(in_df):
-        out = _pairwise_sparse(in_df, norm, metric, set_diagonal_zero, device)
-        return out.cpu().numpy() if to_host else out
+        return _result(_pairwise_sparse(in_df, norm, metric, set_diagonal_zero, device), to_host)
     x = _to_device_dense(in_df, device)
     n, h = x.shape
     if norm != '':   # sklearn.preprocessing.normalize first (helpers.py:42-43) ...
@@ -97,7 +110,7 @@ def pairwise_similarity(in_df, norm='', metric='cosine', set_diagonal_zero=True,
     _gemm_nt((hi, lo), (hi, lo), n, n, h, out)
     if set_diagonal_zero:
         out.diagonal().zero_()
-    return out.cpu().numpy() if to_host else out
+    return _result(out, to_host)
 
 
 def _pairwise_sparse(m, norm, metric, set_diagonal_zero, device):
@@ -347,12 +360,39 @@ def _csr_similarity_topk(q, c, k, diag_offset=0, exclude=False, splits=0, lists=
     return idx, val
 
 
-def _top_k_similar_sparse(embeddings, k, corpus, metric, device, splits, lists=None, groups=None):
-    if corpus is not None and corpus.shape[1] != embeddings.shape[1]:
-        raise ValueError('top_k_similar: corpus rows have %d columns, queries %d' % (corpus.shape[1], embeddings.shape[1]))
-    q = DeviceCSR(_csr_operand(embeddings, metric), device)
-    c = q if corpus is None else DeviceCSR(_csr_operand(corpus, metric), device)
-    return _csr_similarity_topk(q, c, k, exclude=corpus is None, splits=splits, lists=lists, groups=groups)
+class _Operands:
+    """Queries and corpus of top_k_similar, similar_pairs and similarity_auroc as their kernels read them.  The constructor only
+    checks on the host that both are dense or both sparse (ValueError), so that it runs among the entry point's other argument
+    checks; build(device) then makes the device operands.  corpus=None (self mode) ranks the queries against themselves, and the
+    corpus operand is the query one."""
+
+    def __init__(self, queries, corpus, metric, fn):
+        self.sparse, self.self_mode = sp.issparse(queries), corpus is None
+        if corpus is not None and sp.issparse(corpus) != self.sparse:
+            raise ValueError('%s: queries and corpus must be both sparse or both dense' % fn)
+        self._inputs = (queries,) if corpus is None else (queries, corpus)
+        self._metric, self._fn = metric, fn
+
+    def build(self, device):
+        """Sets q and c: the bf16 hi / lo pairs of _normalised_operands (rows L2-normalised for 'cosine') of dense rows (arrays or
+        tensors), the DeviceCSR of _csr_operand of sparse ones (scipy sparse matrices); n_q, n_c and dim; and rows, the query rows
+        before the kernels' normalisation (the device fp32 tensor, or _csr_operand's host CSR).  ValueError when the corpus
+        rows are not as wide as the queries.  Returns self."""
+        if self.sparse:
+            rows = [_csr_operand(x, self._metric) for x in self._inputs]
+        else:
+            rows = [_as_device_dense(x, device) for x in self._inputs]
+        self.rows = rows[0]
+        self.n_q, self.dim = rows[0].shape
+        self.n_c = rows[-1].shape[0]
+        if rows[-1].shape[1] != self.dim:
+            raise ValueError('%s: corpus rows have %d columns, queries %d' % (self._fn, rows[-1].shape[1], self.dim))
+        if self.sparse:
+            ops = [DeviceCSR(m, device) for m in rows]
+        else:
+            ops = [_normalised_operands(x, 2 if self._metric == 'cosine' else 0)[:2] for x in rows]
+        self.q, self.c = ops[0], ops[-1]
+        return self
 
 
 def _group_labels(groups, n, fn):
@@ -419,41 +459,23 @@ def top_k_similar(embeddings, k=10, corpus=None, metric='cosine', device='cuda:0
     assert metric in ['cosine', 'linear kernel']
     _check_k(k, long_lists, sp.issparse(embeddings), 'top_k_similar')
     max_candidates = _check_budget(max_candidates, 'top_k_similar')
-    if corpus is not None and sp.issparse(embeddings) != sp.issparse(corpus):
-        raise ValueError('top_k_similar: queries and corpus must be both sparse or both dense')
-    lists = g_dev = None
+    ops = _Operands(embeddings, corpus, metric, 'top_k_similar')
     n_c = embeddings.shape[0] if corpus is None else corpus.shape[0]
     if exclude is not None:
         indptr, indices, _ = _stored_positions(exclude, (embeddings.shape[0], n_c), 'exclude', 'top_k_similar')
-    if groups is not None:
-        g_dev = torch.from_numpy(_group_labels(groups, n_c, 'top_k_similar')).to(device)
-    if exclude is not None:
-        lists = _DeviceLists.from_host(indptr, indices, device)
-    if sp.issparse(embeddings):
-        idx, val = _top_k_similar_sparse(embeddings, k, corpus, metric, device, splits, lists, g_dev)
-        if to_host:
-            return idx.cpu().numpy(), val.cpu().numpy()
-        return idx, val
-    norm_kind = 2 if metric == 'cosine' else 0
-    x = _as_device_dense(embeddings, device)
-    n_q, h = x.shape
-    q = _normalised_operands(x, norm_kind)[:2]
-    if corpus is None:
-        c, n_c = q, n_q
+    g = None if groups is None else _group_labels(groups, n_c, 'top_k_similar')
+    ops.build(device)
+    lists = None if exclude is None else _DeviceLists.from_host(indptr, indices, device)
+    g_dev = None if g is None else torch.from_numpy(g).to(device)
+    if ops.sparse:
+        idx, val = _csr_similarity_topk(ops.q, ops.c, k, exclude=ops.self_mode, splits=splits, lists=lists, groups=g_dev)
+    elif k > TOPK_MAX_K:
+        idx, val = _similarity_topk_long(ops.q, ops.c, ops.n_q, ops.n_c, ops.dim, k, exclude=ops.self_mode, splits=splits, lists=lists,
+                                         groups=g_dev, max_candidates=max_candidates)
     else:
-        xc = _as_device_dense(corpus, device)
-        if xc.shape[1] != h:
-            raise ValueError('top_k_similar: corpus rows have %d columns, queries %d' % (xc.shape[1], h))
-        n_c = xc.shape[0]
-        c = _normalised_operands(xc, norm_kind)[:2]
-    if k > TOPK_MAX_K:
-        idx, val = _similarity_topk_long(q, c, n_q, n_c, h, k, exclude=corpus is None, splits=splits, lists=lists, groups=g_dev,
-                                         max_candidates=max_candidates)
-    else:
-        idx, val = _similarity_topk(q, c, n_q, n_c, h, k, exclude=corpus is None, splits=splits, lists=lists, groups=g_dev)
-    if to_host:
-        return idx.cpu().numpy(), val.cpu().numpy()
-    return idx, val
+        idx, val = _similarity_topk(ops.q, ops.c, ops.n_q, ops.n_c, ops.dim, k, exclude=ops.self_mode, splits=splits, lists=lists,
+                                    groups=g_dev)
+    return _result((idx, val), to_host)
 
 
 def _history_weights(histories, n_articles, fn):
@@ -506,8 +528,7 @@ def user_profiles(histories, embeddings, device='cuda:0', to_host=True):
         _dense_embeddings(embeddings, device, 'user_profiles')
     w, _ = _history_weights(histories, embeddings.shape[0], 'user_profiles')
     emb = _dense_embeddings(embeddings, device, 'user_profiles')
-    out = _profiles(DeviceCSR(w, device), emb)
-    return out.cpu().numpy() if to_host else out
+    return _result(_profiles(DeviceCSR(w, device), emb), to_host)
 
 
 def _candidate_rows(candidates, n, fn):
@@ -532,6 +553,43 @@ def _remap_lists(indptr, indices, cand):
     new_ptr = np.zeros(len(indptr), dtype=np.int64)
     np.cumsum(np.bincount(rows[keep], minlength=len(indptr) - 1), out=new_ptr[1:])
     return new_ptr, pos[keep].astype(np.int32)
+
+
+def _recommend_request(w, n_art, candidates, groups, exclude_read, device, fn):
+    """The request recommend and recommend_sparse share, for the normalised histories w (scipy CSR [U, N]): candidates and groups
+    checked on the host (ValueError before any device work), then on the device the history CSR, the candidate rows, the group
+    labels of the corpus positions and, with exclude_read, the exclusion lists: every position of a group the user read
+    (_read_group_lists), the reads remapped to candidate positions, or the history CSR itself.
+    Returns (hist DeviceCSR, cand host int64 or None, cand_dev, corpus group labels or None, lists _DeviceLists or None)."""
+    cand = None if candidates is None else _candidate_rows(candidates, n_art, fn)
+    g = None if groups is None else _group_labels(groups, n_art, fn)
+    hist = DeviceCSR(w, device)
+    cand_dev = None if cand is None else torch.from_numpy(cand).to(device)
+    g_dev = cg_dev = None
+    if g is not None:
+        g_dev = torch.from_numpy(g).to(device)
+        cg_dev = g_dev if cand_dev is None else g_dev.index_select(0, cand_dev)
+    lists = None
+    if exclude_read and g is not None:
+        ptr, ind = _read_group_lists(hist.indptr, hist.indices, g_dev, cg_dev)
+        lists = _DeviceLists(ptr, ind, ind.numel())
+    elif exclude_read and cand is not None:
+        lists = _DeviceLists.from_host(*_remap_lists(w.indptr, w.indices, cand), device)
+    elif exclude_read:
+        lists = _DeviceLists(hist.indptr, hist.indices, hist.nnz)
+    return hist, cand, cand_dev, cg_dev, lists
+
+
+def _recommend_result(idx, val, empty, cand_dev, device, to_host):
+    """recommend's output from the top-k over the corpus positions: padding rows (-1 / -inf) for the users in `empty`, the
+    candidate positions mapped back to article rows."""
+    if empty.any():
+        e = torch.from_numpy(empty).to(device)
+        idx[e] = -1
+        val[e] = float('-inf')
+    if cand_dev is not None:
+        idx = torch.where(idx >= 0, cand_dev[idx.clamp(min=0).long()].int(), idx)
+    return _result((idx, val), to_host)
 
 
 def sequences_from_csr(m):
@@ -564,48 +622,23 @@ def recommend(histories, embeddings, k=10, candidates=None, metric='cosine', exc
     labels (over the candidates' positions when candidates are given).
     long_lists / max_candidates: as in top_k_similar -- up to k = 1024 with long_lists=True.
     Returns (index int32 [U, k], score float32 [U, k]) as ndarrays (device tensors with to_host=False)."""
-    if metric not in ('cosine', 'linear kernel'):
-        raise ValueError("recommend: metric = %r: 'cosine' or 'linear kernel'" % (metric,))
+    _check_metric(metric, 'recommend')
     _check_k(k, long_lists, False, 'recommend')
     max_candidates = _check_budget(max_candidates, 'recommend')
     n_art = embeddings.shape[0]
     if sp.issparse(embeddings):
         _dense_embeddings(embeddings, device, 'recommend')
     w, empty = _history_weights(histories, n_art, 'recommend')
-    cand = None if candidates is None else _candidate_rows(candidates, n_art, 'recommend')
-    g = None if groups is None else _group_labels(groups, n_art, 'recommend')
-    lists_host = None
-    if exclude_read and cand is not None and g is None:
-        lists_host = _remap_lists(w.indptr, w.indices, cand)
     if profiles is not None:
         if sp.issparse(profiles) or tuple(profiles.shape) != (w.shape[0], embeddings.shape[1]):
             raise ValueError('recommend: profiles have shape %s, [%d, %d] (users x embedding width) expected'
                              % (tuple(profiles.shape), w.shape[0], embeddings.shape[1]))
+    hist, _, cand_dev, cg_dev, lists = _recommend_request(w, n_art, candidates, groups, exclude_read, device, 'recommend')
     emb = _dense_embeddings(embeddings, device, 'recommend')
-    hist = DeviceCSR(w, device)
     prof = _profiles(hist, emb) if profiles is None else _as_device_dense(profiles, emb.device)
-    cand_dev = None if cand is None else torch.from_numpy(cand).to(device)
-    g_dev = cg_dev = None
-    if g is not None:
-        g_dev = torch.from_numpy(g).to(device)
-        cg_dev = g_dev if cand_dev is None else g_dev.index_select(0, cand_dev)
-    lists = None
-    if exclude_read and g is not None:
-        ptr, ind = _read_group_lists(hist.indptr, hist.indices, g_dev, cg_dev)
-        lists = _DeviceLists(ptr, ind, ind.numel())
-    elif exclude_read:
-        lists = _DeviceLists(hist.indptr, hist.indices, hist.nnz) if cand is None else _DeviceLists.from_host(*lists_host, device)
-    corpus = emb if cand is None else emb.index_select(0, cand_dev)
+    corpus = emb if cand_dev is None else emb.index_select(0, cand_dev)
     idx, val = _recommend_topk(prof, corpus, k, metric, lists, splits, cg_dev, max_candidates)
-    if empty.any():
-        e = torch.from_numpy(empty).to(device)
-        idx[e] = -1
-        val[e] = float('-inf')
-    if cand_dev is not None:
-        idx = torch.where(idx >= 0, cand_dev[idx.clamp(min=0).long()].int(), idx)
-    if to_host:
-        return idx.cpu().numpy(), val.cpu().numpy()
-    return idx, val
+    return _recommend_result(idx, val, empty, cand_dev, device, to_host)
 
 
 def _recommend_topk(prof, corpus, k, metric, lists, splits=0, groups=None, max_candidates=TOPK_LONG_MAX_CANDIDATES):
@@ -709,35 +742,16 @@ def recommend_sparse(histories, X, k=10, candidates=None, metric='cosine', exclu
     The profiles are counted once for all users, then filled and ranked in chunks of users holding at most SPARSE_PROFILE_CHUNK_NNZ
     profile entries (a single larger user is a chunk of its own), so they are never all resident.  The result does not depend on
     the chunks.  Returns (index int32 [U, k], score float32 [U, k]) as ndarrays (device tensors with to_host=False)."""
-    if metric not in ('cosine', 'linear kernel'):
-        raise ValueError("recommend_sparse: metric = %r: 'cosine' or 'linear kernel'" % (metric,))
+    _check_metric(metric, 'recommend_sparse')
     if isinstance(k, bool) or not isinstance(k, (int, np.integer)) or not 1 <= k <= TOPK_MAX_K:
         raise ValueError('recommend_sparse: k = %r is outside the supported range 1 <= k <= %d (sparse profiles rank at most %d)'
                          % (k, TOPK_MAX_K, TOPK_MAX_K))
     k = int(k)
     m = _sparse_articles(X, 'recommend_sparse')
-    n_art = m.shape[0]
     w, empty = _profile_weights(histories, m, 'recommend_sparse')
-    cand = None if candidates is None else _candidate_rows(candidates, n_art, 'recommend_sparse')
-    g = None if groups is None else _group_labels(groups, n_art, 'recommend_sparse')
-    lists_host = None
-    if exclude_read and cand is not None and g is None:
-        lists_host = _remap_lists(w.indptr, w.indices, cand)
+    hist, cand, cand_dev, cg_dev, lists = _recommend_request(w, m.shape[0], candidates, groups, exclude_read, device, 'recommend_sparse')
     corpus_host = _csr_operand(m, metric)
-    if cand is not None:
-        corpus_host = corpus_host[cand]
-    hist, x, corpus = DeviceCSR(w, device), DeviceCSR(m, device), DeviceCSR(corpus_host, device)
-    cand_dev = None if cand is None else torch.from_numpy(cand).to(device)
-    g_dev = cg_dev = None
-    if g is not None:
-        g_dev = torch.from_numpy(g).to(device)
-        cg_dev = g_dev if cand_dev is None else g_dev.index_select(0, cand_dev)
-    lists = None
-    if exclude_read and g is not None:
-        ptr, ind = _read_group_lists(hist.indptr, hist.indices, g_dev, cg_dev)
-        lists = _DeviceLists(ptr, ind, ind.numel())
-    elif exclude_read:
-        lists = _DeviceLists(hist.indptr, hist.indices, hist.nnz) if cand is None else _DeviceLists.from_host(*lists_host, device)
+    x, corpus = DeviceCSR(m, device), DeviceCSR(corpus_host if cand is None else corpus_host[cand], device)
     n_u = w.shape[0]
     idx = torch.empty(n_u, k, dtype=torch.int32, device=device)
     val = torch.empty(n_u, k, dtype=torch.float32, device=device)
@@ -754,15 +768,7 @@ def recommend_sparse(histories, X, k=10, candidates=None, metric='cosine', exclu
         idx[u0:u1] = i
         val[u0:u1] = v
         del q
-    if empty.any():
-        e = torch.from_numpy(empty).to(device)
-        idx[e] = -1
-        val[e] = float('-inf')
-    if cand_dev is not None:
-        idx = torch.where(idx >= 0, cand_dev[idx.clamp(min=0).long()].int(), idx)
-    if to_host:
-        return idx.cpu().numpy(), val.cpu().numpy()
-    return idx, val
+    return _recommend_result(idx, val, empty, cand_dev, device, to_host)
 
 
 def recommendation_recall(index, targets):
@@ -789,20 +795,25 @@ def recommendation_recall(index, targets):
     return {'users': users, 'hit_rate': float((hits[use] > 0).mean()), 'recall': float((hits[use] / n_t[use]).mean())}
 
 
+def _impression_call(export, operands, n_imp, imp, device):
+    """What the impression-metric exports share: the score and metric buffers on `device`, the impression arrays uploaded, and
+    export(*operands, indptr, items, clicked, n_imp, scores, metrics, stream) -- unless there is nothing to score.  Returns
+    (scores fp32 [nnz], metrics fp64 [I, 4] = AUC, MRR, nDCG@5, nDCG@10, NaN where not scored) as device tensors."""
+    scores = torch.empty(imp['items'].size, dtype=torch.float32, device=device)
+    metrics = torch.full((n_imp, 4), float('nan'), dtype=torch.float64, device=device)
+    if n_imp == 0 or imp['items'].size == 0:
+        return scores, metrics
+    indptr, items, clicked = (torch.from_numpy(imp[key]).to(device) for key in ('indptr', 'items', 'clicked'))
+    call(export, *operands, indptr.data_ptr(), items.data_ptr(), clicked.data_ptr(), n_imp, scores.data_ptr(), metrics.data_ptr(),
+         _stream())
+    return scores, metrics
+
+
 def _impression_scores(q, emb, imp, metric):
     """dae_impression_metrics on device tensors: (scores fp32 [nnz], metrics fp64 [I, 4] = AUC, MRR, nDCG@5, nDCG@10) as device
     tensors.  imp: check_impressions' host arrays."""
-    n_imp, d = q.shape[0], emb.device
-    scores = torch.empty(imp['items'].size, dtype=torch.float32, device=d)
-    metrics = torch.full((n_imp, 4), float('nan'), dtype=torch.float64, device=d)
-    if n_imp == 0 or imp['items'].size == 0:
-        return scores, metrics
-    indptr = torch.from_numpy(imp['indptr']).to(d)
-    items = torch.from_numpy(imp['items']).to(d)
-    clicked = torch.from_numpy(imp['clicked']).to(d)
-    call('dae_impression_metrics', q.data_ptr(), q.stride(0), emb.data_ptr(), emb.stride(0), emb.shape[1], int(metric == 'cosine'),
-         indptr.data_ptr(), items.data_ptr(), clicked.data_ptr(), n_imp, scores.data_ptr(), metrics.data_ptr(), _stream())
-    return scores, metrics
+    operands = (q.data_ptr(), q.stride(0), emb.data_ptr(), emb.stride(0), emb.shape[1], int(metric == 'cosine'))
+    return _impression_call('dae_impression_metrics', operands, q.shape[0], imp, emb.device)
 
 
 def impression_metrics(vectors, embeddings, impressions, metric='linear kernel', device='cuda:0'):
@@ -820,8 +831,7 @@ def impression_metrics(vectors, embeddings, impressions, metric='linear kernel',
     Returns {'impressions': impressions scored, 'skipped': impressions without a click or without a non-click (left out of the
     means), 'auc', 'mrr', 'ndcg@5', 'ndcg@10': means over the scored ones (NaN when none)}."""
     from .user_model import check_impressions
-    if metric not in ('cosine', 'linear kernel'):
-        raise ValueError("impression_metrics: metric = %r: 'cosine' or 'linear kernel'" % (metric,))
+    _check_metric(metric, 'impression_metrics')
     emb = _dense_embeddings(embeddings, device, 'impression_metrics')
     imp = check_impressions(impressions, emb.shape[0], 'impression_metrics')
     n_imp = imp['indptr'].size - 1
@@ -849,18 +859,9 @@ def _impression_means(m, n_imp):
 
 def _csr_impression_scores(q, x, imp, metric):
     """dae_csr_impression_metrics on DeviceCSR operands: (scores fp32 [nnz], metrics fp64 [I, 4]) as device tensors."""
-    n_imp, d = q.shape[0], x.indptr.device
-    scores = torch.empty(imp['items'].size, dtype=torch.float32, device=d)
-    metrics = torch.full((n_imp, 4), float('nan'), dtype=torch.float64, device=d)
-    if n_imp == 0 or imp['items'].size == 0:
-        return scores, metrics
-    indptr = torch.from_numpy(imp['indptr']).to(d)
-    items = torch.from_numpy(imp['items']).to(d)
-    clicked = torch.from_numpy(imp['clicked']).to(d)
-    call('dae_csr_impression_metrics', q.indptr.data_ptr(), _data_ptr(q.indices), _data_ptr(q.values), x.indptr.data_ptr(),
-         _data_ptr(x.indices), _data_ptr(x.values), x.shape[0], x.shape[1], int(metric == 'cosine'), indptr.data_ptr(),
-         items.data_ptr(), clicked.data_ptr(), n_imp, scores.data_ptr(), metrics.data_ptr(), _stream())
-    return scores, metrics
+    operands = (q.indptr.data_ptr(), _data_ptr(q.indices), _data_ptr(q.values), x.indptr.data_ptr(), _data_ptr(x.indices),
+                _data_ptr(x.values), x.shape[0], x.shape[1], int(metric == 'cosine'))
+    return _impression_call('dae_csr_impression_metrics', operands, q.shape[0], imp, x.indptr.device)
 
 
 def impression_metrics_sparse(profiles, X, impressions, metric='linear kernel', device='cuda:0'):
@@ -873,8 +874,7 @@ def impression_metrics_sparse(profiles, X, impressions, metric='linear kernel', 
     finite with every |x| <= 2^63 / sqrt(F) (ValueError otherwise, before any device work).  Returns impression_metrics' dict."""
     from .user_model import check_impressions
     fn = 'impression_metrics_sparse'
-    if metric not in ('cosine', 'linear kernel'):
-        raise ValueError("%s: metric = %r: 'cosine' or 'linear kernel'" % (fn, metric))
+    _check_metric(metric, fn)
     m = _sparse_articles(X, fn)
     imp = check_impressions(impressions, m.shape[0], fn)
     n_imp, n_f = imp['indptr'].size - 1, m.shape[1]
@@ -997,6 +997,16 @@ def _csr_similarity_pairs(q, c, self_mode, tau, max_pairs, threshold):
     return _pairs_call(run, n_q, n_c, max_pairs, threshold, dev)
 
 
+def _similarity_pairs(q, c, n_q, n_c, h, self_mode, tau, max_pairs, threshold):
+    """similar_pairs of the bf16 hi / lo operand pairs q and c (c is q in self mode) through dae_similarity_pairs_bf16x3: device
+    tensors (i, j, s) sorted by (i, j).  tau: the float32 threshold as a Python float."""
+    def run(count, cap, i, j, s):
+        call('dae_similarity_pairs_bf16x3', n_q, n_c, h, q[0].data_ptr(), q[1].data_ptr(), q[0].stride(0), c[0].data_ptr(),
+             c[1].data_ptr(), c[0].stride(0), 1 if self_mode else 0, tau, count.data_ptr(), cap, i.data_ptr(), j.data_ptr(),
+             s.data_ptr(), _stream())
+    return _pairs_call(run, n_q, n_c, max_pairs, threshold, q[0].device)
+
+
 def similar_pairs(data, threshold, corpus=None, metric='cosine', device='cuda:0', to_host=True, max_pairs=1 << 28):
     """Every pair of rows whose similarity reaches `threshold` (near-duplicate articles), without forming the similarity matrix.
     corpus=None: the pairs (i, j) with i > j of `data` against itself, scored S[i, j] with row i as the query.  With a corpus: every
@@ -1008,10 +1018,8 @@ def similar_pairs(data, threshold, corpus=None, metric='cosine', device='cuda:0'
     kernel call counts the pairs into max(2^20, 16 Nq) slots (12 B each); more than `max_pairs` qualifying pairs then raise
     ValueError before the full output is allocated, and more than the first capacity take exactly one more call.
     Returns (i int32, j int32, score float32), sorted by (i, j), as ndarrays (device tensors with to_host=False)."""
-    if metric not in ('cosine', 'linear kernel'):
-        raise ValueError("similar_pairs: metric = %r: 'cosine' or 'linear kernel'" % (metric,))
-    if corpus is not None and sp.issparse(data) != sp.issparse(corpus):
-        raise ValueError('similar_pairs: queries and corpus must be both sparse or both dense')
+    _check_metric(metric, 'similar_pairs')
+    ops = _Operands(data, corpus, metric, 'similar_pairs')
     try:
         with np.errstate(over='ignore'):   # out of float32 range: inf, refused below
             tau = np.float32(threshold)
@@ -1019,42 +1027,19 @@ def similar_pairs(data, threshold, corpus=None, metric='cosine', device='cuda:0'
         raise ValueError('similar_pairs: threshold %r is not a number' % (threshold,))
     if not np.isfinite(tau):
         raise ValueError('similar_pairs: threshold %r is not finite (as float32)' % (threshold,))
-    sparse = sp.issparse(data)
-    if sparse and not tau > 0:
+    if ops.sparse and not tau > 0:
         raise ValueError('similar_pairs: threshold %r must be > 0 on sparse input: a pair that shares no column scores exactly 0, so '
                          'almost every pair would qualify' % (threshold,))
     if not isinstance(max_pairs, (int, np.integer)) or max_pairs < 0:
         raise ValueError('similar_pairs: max_pairs = %r must be a non-negative integer' % (max_pairs,))
     max_pairs = int(max_pairs)
     tau = float(tau)
-    if sparse:
-        if corpus is not None and corpus.shape[1] != data.shape[1]:
-            raise ValueError('similar_pairs: corpus rows have %d columns, queries %d' % (corpus.shape[1], data.shape[1]))
-        q = DeviceCSR(_csr_operand(data, metric), device)
-        c = q if corpus is None else DeviceCSR(_csr_operand(corpus, metric), device)
-        i, j, s = _csr_similarity_pairs(q, c, corpus is None, tau, max_pairs, threshold)
+    ops.build(device)
+    if ops.sparse:
+        i, j, s = _csr_similarity_pairs(ops.q, ops.c, ops.self_mode, tau, max_pairs, threshold)
     else:
-        norm_kind = 2 if metric == 'cosine' else 0
-        x = _as_device_dense(data, device)
-        n_q, h = x.shape
-        q = _normalised_operands(x, norm_kind)[:2]
-        if corpus is None:
-            c, n_c = q, n_q
-        else:
-            xc = _as_device_dense(corpus, device)
-            if xc.shape[1] != h:
-                raise ValueError('similar_pairs: corpus rows have %d columns, queries %d' % (xc.shape[1], h))
-            n_c = xc.shape[0]
-            c = _normalised_operands(xc, norm_kind)[:2]
-
-        def run(count, cap, i, j, s):
-            call('dae_similarity_pairs_bf16x3', n_q, n_c, h, q[0].data_ptr(), q[1].data_ptr(), q[0].stride(0), c[0].data_ptr(),
-                 c[1].data_ptr(), c[0].stride(0), 1 if corpus is None else 0, tau, count.data_ptr(), cap, i.data_ptr(), j.data_ptr(),
-                 s.data_ptr(), _stream())
-        i, j, s = _pairs_call(run, n_q, n_c, max_pairs, threshold, device)
-    if to_host:
-        return i.cpu().numpy(), j.cpu().numpy(), s.cpu().numpy()
-    return i, j, s
+        i, j, s = _similarity_pairs(ops.q, ops.c, ops.n_q, ops.n_c, ops.dim, ops.self_mode, tau, max_pairs, threshold)
+    return _result((i, j, s), to_host)
 
 
 def _host_ints(a):
@@ -1308,8 +1293,7 @@ def similarity_auroc(data, labels, metric='cosine', bins=1 << 21, title=None, sa
 
 def _pair_histograms(data, labels, metric, bins, device='cuda:0'):
     """Device half of similarity_auroc: (hist int64 [2, bins], sums float64 [2]) device tensors and the grid's M."""
-    if metric not in ('cosine', 'linear kernel'):
-        raise ValueError("metric = %r: 'cosine' or 'linear kernel'" % (metric,))
+    _check_metric(metric, 'similarity_auroc')
     _check_bins(bins)
     labels = np.asarray(labels.values if hasattr(labels, 'values') else labels).reshape(-1)
     n = data.shape[0]
@@ -1319,19 +1303,17 @@ def _pair_histograms(data, labels, metric, bins, device='cuda:0'):
     lab_dev = torch.from_numpy(lab_i).to(device)
     hist = torch.zeros(2, bins, dtype=torch.int64, device=device)      # uint64 counts in the kernels
     sums = torch.zeros(2, dtype=torch.float64, device=device)
-    if sp.issparse(data):
-        m = _csr_operand(data, metric)
-        M = grid_range(float(np.asarray(m.multiply(m).sum(1), dtype=np.float64).max()) if metric != 'cosine' else 1.0, metric)
-        d = DeviceCSR(m, device)
+    ops = _Operands(data, None, metric, 'similarity_auroc').build(device)
+    q, x = ops.q, ops.rows
+    if ops.sparse:
+        M = grid_range(float(np.asarray(x.multiply(x).sum(1), dtype=np.float64).max()) if metric != 'cosine' else 1.0, metric)
         need = (ctypes.c_int64 * 1)()
-        call('dae_csr_similarity_pair_hist_workspace', n, d.nnz, m.shape[1], ctypes.addressof(need))
+        call('dae_csr_similarity_pair_hist_workspace', n, q.nnz, ops.dim, ctypes.addressof(need))
         ws = torch.empty(max(int(need[0]), 16), dtype=torch.uint8, device=device)
-        call('dae_csr_similarity_pair_hist', d.indptr.data_ptr(), d.indices.data_ptr(), d.values.data_ptr(), n, d.nnz, m.shape[1],
+        call('dae_csr_similarity_pair_hist', q.indptr.data_ptr(), q.indices.data_ptr(), q.values.data_ptr(), n, q.nnz, ops.dim,
              lab_dev.data_ptr(), M, bins, ws.data_ptr(), ws.numel(), hist.data_ptr(), sums.data_ptr(), _stream())
     else:
-        x = _as_device_dense(data, device)
         M = grid_range(_max_sq_norm_dense(x) if metric != 'cosine' else 1.0, metric)
-        hi, lo, ld = _normalised_operands(x, 2 if metric == 'cosine' else 0)
-        call('dae_similarity_pair_hist_bf16x3', n, x.shape[1], hi.data_ptr(), lo.data_ptr(), ld, lab_dev.data_ptr(), M, bins,
-             hist.data_ptr(), sums.data_ptr(), _stream())
+        call('dae_similarity_pair_hist_bf16x3', n, ops.dim, q[0].data_ptr(), q[1].data_ptr(), q[0].stride(0), lab_dev.data_ptr(), M,
+             bins, hist.data_ptr(), sums.data_ptr(), _stream())
     return hist, sums, M
